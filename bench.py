@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the headline metric of BASELINE.json on B200:
+"""bench.py -- the headline metric of BASELINE.json on H100:
 
     log-mll + gradient (update_mll_and_dmll!, src/GPE.jl:332-335) for GPE SEIso, N=32768, d=8, FP64
     reported as algorithmic GFLOP/s (F_alg = N^3 + 2 N^2, SURVEY.md §8(d)) and ms per evaluation.
@@ -13,7 +13,7 @@ MeanConst(0) -- config C2 of SURVEY.md §8(d)).
                memory and alpha / mll / dmll read back inside the timed region
   roofline     the dominant kernel (FP64 DMMA NT GEMM): algorithmic flops / sum of its launch
                durations (CUDA events around every launch in one extra profiled step) vs the DMMA
-               issue rate measured in the same run (MEASURED_PEAKS.json has no FP64 figure)
+               issue rate measured in the same run
   cpu_baseline the reference's algorithm (oracle port: scalar loops in C + LAPACK via OpenBLAS, all
                host cores) on a bounded sample (N=8192) of the same workload
   --impl reference   times only that CPU path (Julia is not installed in this image).
@@ -75,7 +75,7 @@ class StdoutToStderr:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -142,13 +142,12 @@ def extrapolate_full(seconds, n, n_full=N_FULL):
     return t2 * r ** 2 + t3 * r ** 3
 
 
-def full_size_record():
-    """One full-size (N=32768) CPU evaluation measured on a pool box and committed (profiles/): validates the extrapolation."""
-    pth = os.path.join(ROOT, "profiles", "r02_cpu_full_size.json")
-    try:
-        return json.load(open(pth))
-    except Exception:
-        return None
+def dump_outputs(out_dir, last):
+    """The arrays the timed step hands its caller, as float64 .npy files: alpha (N), mll, the kernel-parameter
+    gradient and tr(K^-1) of the last timed step.  Inputs are seeded, so two builds can be compared file by file."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in last.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.atleast_1d(np.asarray(v, dtype=np.float64)))
 
 
 def cpu_baseline_run(n, steps=1):
@@ -174,7 +173,7 @@ def run_reference(args, rank, world):
     from oracle import cpu_baseline as cb
     cores = pin_blas_threads()
     per_step = CPU_BUDGET_S / (args.steps + 1)
-    # ~8.5 s per evaluation at N=8192 on the pool's 64 host cores (round-1 records); time ~ N^3
+    # sizing assumption: ~8.5 s per evaluation at N=8192 on 64 host cores; time ~ N^3
     n = int(8192 * (per_step / 8.5) ** (1.0 / 3.0)) // 1024 * 1024
     n = max(2048, min(N_FULL, n))
     if os.environ.get("GPB200_CPU_SAMPLE_N"):
@@ -192,7 +191,6 @@ def run_reference(args, rank, world):
     rate_sample = falg(n) / t_sample * 1e-9
     t_full = extrapolate_full(phases, n) if n != N_FULL else t_sample
     val = falg(N_FULL) / t_full * 1e-9
-    rec = full_size_record()
     sample = ("each step = one full update_mll_and_dmll! with the reference's algorithm (scalar cov!/dmll_kern! loops in C, "
               "1 thread, as the reference; dpotrf + dpotrs(-I) + dger via OpenBLAS on %d threads) at N_sample=%d of 32768, d=8: "
               "%.2f s/step = %.1f GFLOP/s at N_sample; value = F_alg(32768) / t(32768) with t extrapolated per phase "
@@ -206,8 +204,7 @@ def run_reference(args, rank, world):
         "config": {"workload": WORKLOAD % N_FULL,
                    "sample": "N_sample=%d per step (bounded CPU sample); value is the phase-extrapolated rate at N=32768" % n,
                    "value_kind": "extrapolated_to_full_config" if n != N_FULL else "measured_full_config",
-                   "rate_at_sample_gflops": rate_sample, "seconds_full_config_extrapolated": t_full,
-                   "full_size_measured_once": rec},
+                   "rate_at_sample_gflops": rate_sample, "seconds_full_config_extrapolated": t_full},
         "cpu_baseline": {"value": val, "unit": "GFLOP/s", "cores": cores, "kind": "port", "sample": sample},
         "e2e": {"value": val, "unit": "GFLOP/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
@@ -223,7 +220,10 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--n", type=int, default=N_FULL, help="override N (debug only; the metric is N=32768)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -267,11 +267,13 @@ def main():
     theta = np.array([LL, LSIG])
     r = yh - 0.0
 
+    last = {}
+
     def step_resident():
         eng.factorize(theta, LNOISE)
-        eng.mll(r)
+        last["alpha"], last["mll"] = eng.mll(r)
         eng.grad_prepare()
-        return eng.grad_kernel()
+        last["grad_kernel"], last["trace"] = eng.grad_kernel()
 
     def step_e2e():
         gp.reload_data(Xh.T, yh)            # H2D of x and (inside update_mll) y
@@ -304,6 +306,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms_total = float(t.item())
     ms_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # ---- e2e: host buffers in, host results out, through the public GPE API -------------------
     step_e2e()
@@ -337,21 +341,12 @@ def main():
     if tp["gemm_ms"] > 0:
         alg = float(N) ** 3 / world                             # N^3/3 Cholesky + 2N^3/3 inverse, all in this kernel (per rank)
         achieved = alg / (tp["gemm_ms"] * 1e-3) * 1e-12
-        traffic = None
-        tj = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-        if os.path.exists(tj):
-            try:
-                traffic = json.load(open(tj)).get("dram_bytes_per_launch")
-            except Exception:
-                traffic = None
-        roof = {"bound": "tensor", "kernel": "gpb200_dgemm_nt_tma (FP64 DMMA.8x8x4 fed by TMA)",
+        roof = {"bound": "tensor", "kernel": "gpb200_dgemm_nt_tma (FP64 DMMA.16x8x4 fed by TMA)",
                 "achieved": achieved, "peak": pk["dmma_tflops"], "unit": "TFLOP/s", "frac": achieved / pk["dmma_tflops"],
-                "traffic": traffic,
-                "traffic_source": "dram__bytes_read+write of the largest launch (W'W) in the committed ncu --set full capture "
-                                  "(profiles/gemm_traffic.json); not re-measured in this run",
-                "peak_source": "DMMA.8x8x4 issue rate measured in this run (gpb200_fp64_peak); MEASURED_PEAKS.json "
-                               "carries no FP64 figure -- its HBM/bf16 numbers do not bound this kernel; DFMA rate "
-                               "%.1f TFLOP/s, cuBLAS DGEMM on this pool 36.5 TFLOP/s (profiles/r01_cublas_dgemm.txt)" % pk["dfma_tflops"],
+                "traffic": None,
+                "traffic_source": "not measured",
+                "peak_source": "DMMA.16x8x4 issue rate measured in this run (gpb200_fp64_peak); DFMA rate %.1f TFLOP/s"
+                               % pk["dfma_tflops"],
                 "launches_per_step": int(tp["gemm_launches"]), "kernel_ms_per_step": tp["gemm_ms"],
                 "kernel_share_of_step": tp["gemm_ms"] / ms_step,
                 "algorithmic_flops_per_step": alg, "executed_flops_per_step": tp["gemm_flops"]}
@@ -366,11 +361,7 @@ def main():
     predict_ms = float(np.median(pms))
     check["predict_mu_l1"] = float(np.sum(np.abs(mu_p)))
     check["predict_var_sum"] = float(np.sum(var_p))
-    hbm_peak = None
-    try:
-        hbm_peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
-    except Exception:
-        hbm_peak = 6574.5                  # B200_PROFILING.md fallback == the pool's measured copy bandwidth
+    hbm_peak = 3350.0                      # GB/s, H100 SXM data sheet (HBM3)
     Npad = (N + 127) // 128 * 128
     T = Npad // 128
     tri_bytes = 8.0 * 128 * 128 * (T * (T + 1) // 2)            # lower tiles of the N x N matrix
@@ -402,15 +393,14 @@ def main():
                              "cov!/dmll_kern! loops (C, 1 thread, as the reference) + dpotrf + dpotrs(-I) (OpenBLAS, %d threads); "
                              "%.1f s; phases %s; value = F_alg(32768)/t(32768), t extrapolated per phase (O(N^2) loops, "
                              "O(N^3) LAPACK) = %.0f s"
-                             % (N_CPU_SAMPLE, cores, tcpu, {k: round(v, 2) for k, v in res["seconds"].items()}, t_full),
-                   "full_size_measured_once": full_size_record()}
+                             % (N_CPU_SAMPLE, cores, tcpu, {k: round(v, 2) for k, v in res["seconds"].items()}, t_full)}
         val = falg(N) / (ms_step * 1e-3) * 1e-9
         line = {
             "metric": METRIC, "value": val, "unit": "GFLOP/s", "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True,
             "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": WORKLOAD % N,
-                       "l2": "working set (two 8.6 GB N x N FP64 matrices) exceeds the 126 MB L2; no flush needed",
+                       "l2": "working set (two 8.6 GB N x N FP64 matrices) exceeds the 50 MB L2; no flush needed",
                        "parallelism": "1 GPU" if world == 1 else
                        "%d GPUs: 1-D block-cyclic block columns (NCCL panel broadcast over NVLink, look-ahead), "
                        "split level-parallel inverse + all-gather, tile-row-cyclic W'W/trace + all-reduce of P+1 sums; "

@@ -1,8 +1,10 @@
-// gemm_nt.cu -- FP64 tensor-core (DMMA) "NT" GEMM for sm_100a.
+// gemm_nt.cu -- FP64 tensor-core (DMMA) "NT" GEMM for sm_90a (H100).
 //
-// tcgen05 has no FP64 kind (ptxas: "Unknown modifier '.kind::f64'"); the FP64 tensor path on
-// B200 is warp-level mma.sync.m8n8k4.f64, SASS DMMA.8x8x4.  The kernel therefore keeps the
-// Blackwell/Hopper *data-movement* structure -- one producer warp driving TMA
+// wgmma has no FP64 form; the FP64 tensor path on Hopper is warp-level mma.sync.f64.  On H100
+// m8n8k4 (SASS DMMA.8x8x4) issues at half the FP64 rate of the m16n8k{4,8,16} shapes, so the
+// kernel uses mma.sync.m16n8k4.f64 (DMMA.16x8x4).  Its A fragment is rows g and g+8 of one k
+// column, so fragment loads and accumulator layout are those of two stacked 8x8x4 tiles.  The
+// kernel keeps the Hopper *data-movement* structure -- one producer warp driving TMA
 // (cp.async.bulk.tensor.2d, 128B-swizzled 16x128 boxes) into a 5-stage shared-memory ring guarded
 // by full/empty mbarriers -- and feeds eight consumer warps that hold a 128x128 FP64 accumulator
 // tile in registers (64x32 per warp = 32 DMMA fragments).
@@ -13,9 +15,9 @@
 // 8-byte bank pairs under the swizzle, so every fragment LDS.64 is conflict-free (any assignment
 // of k indices to the mma's k slots is valid as long as A and B agree).
 //
-// Per CTA tile and k-step of 16: 32 KB staged for 128*128*16 FMAs = 4096 clk of DMMA at
-// 64 FMA/clk/SM -> 8 B/clk/SM of L2 traffic: far below the L2/HBM limits; the kernel is bound by
-// the DMMA pipe.
+// Per CTA tile and k-step of 16: 32 KB staged for 128*128*16 FMAs = 2048 clk of DMMA at
+// 128 FMA/clk/SM -> 16 B/clk/SM of L2 traffic; HBM traffic is a fraction of that thanks to the
+// grouped rasterisation below.
 #include "gemm_nt.cuh"
 #include <stdio.h>
 #include <string.h>
@@ -65,7 +67,7 @@ __device__ __forceinline__ TileCtx decode_tile(const GemmKP& p) {
     const int Kz = min(p.K, p.k_lim - t.zoff);
     {
         // L2-friendly rasterisation: the tm x tn tile rectangle is walked in groups of GROUP_M tile rows,
-        // column by column inside a group, so the ~148 CTAs in flight cover ~16 rows x ~9 columns and every
+        // column by column inside a group, so the ~132 CTAs in flight cover ~16 rows x ~8 columns and every
         // k-slice of an operand row panel fetched from DRAM is reused out of L2 by its neighbours (the CTAs
         // march through k in near lock-step).  A plain row-major walk re-read the B panels once per tile.
         // Launches whose k range starts at the tile row (GEMM_KLO_M: triangular operand) have row-dependent
@@ -139,9 +141,10 @@ __device__ __forceinline__ TileCtx decode_tile(const GemmKP& p) {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-    asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-        : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+// D[16x8] += A[16x4] B[4x8]: a0 / a1 = rows g / g+8 of A, {c0,c1} / {c2,c3} = rows g / g+8 of D.
+__device__ __forceinline__ void dmma1684(double (&c_lo)[2], double (&c_hi)[2], double a_lo, double a_hi, double b) {
+    asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+        : "+d"(c_lo[0]), "+d"(c_lo[1]), "+d"(c_hi[0]), "+d"(c_hi[1]) : "d"(a_lo), "d"(a_hi), "d"(b));
 }
 
 __device__ __forceinline__ double lds_f64(uint32_t addr) {
@@ -166,9 +169,9 @@ __device__ __forceinline__ void compute_stage(uint32_t sA, uint32_t sB,
 #pragma unroll
         for (int j = 0; j < 4; ++j) b[j] = lds_f64(pb + j * 1024 + coff[s]);
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
+        for (int i = 0; i < 8; i += 2)                  // a[i], a[i+1]: rows g + 8i and g + 8i + 8 of the warp tile
 #pragma unroll
-            for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+            for (int j = 0; j < 4; ++j) dmma1684(acc[i][j], acc[i + 1][j], a[i], a[i + 1], b[j]);
     }
 }
 

@@ -15,7 +15,7 @@
 // (truncation 3.5e-17), T[j] = sigma^2 2^(j/64) rounded once on the host, the power of two applied by an integer add to the
 // exponent field and underflow detected in the integer pipe: 9 FP64 instructions including the argument, < 2 ulp of the
 // exponential of the rounded argument (the argument's own rounding, |x| eps relative, is what any exp(-r/2l^2) carries).
-// 25 FP64 instructions per output instead of ~46: 1.19 ms -> ... at C2 (profiles/).
+// 25 FP64 instructions per output instead of ~46.
 #include "gram_fast.cuh"
 #include <math.h>
 #include <stdint.h>

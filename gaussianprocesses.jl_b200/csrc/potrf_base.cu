@@ -170,11 +170,9 @@ potrf128_inv_kernel(const double* __restrict__ G, long long ldg, double* __restr
 //            register tiles per thread, 16 shared-memory loads per 64 FMAs.
 //   phase 2: the 16 x 16 diagonal blocks are inverted (one warp per block, one column per lane), then W = L^-1 is built block
 //            row by block row:  W[i, j] = -W_ii * sum_{j <= k < i} L[i, k] W[k, j]  (two small products per block row).
-// ~40 barriers per tile instead of 256 and N^3/6-class FMA counts instead of N^3/2.  MEASURED on B200 (round 2, ncu
-// gpu__time_duration, profiles/r02_leaf_durations*.csv): first version 128 us (no better than the 123 us column kernel: the
-// 16 x 16 block was kept in local memory by the compiler and phase 2 was a chain of dependent shared-memory dot products) ->
-// 95 us with the template-recursive register block -> 74.5 us with the register-tiled right-looking phase 2.  Cholesky phase
-// at C2: 366.7 ms vs 377.1 ms with the column kernel.  Default since then; option "leaf" = 0 / GPB200_LEAF=0 selects the
+// ~40 barriers per tile instead of 256 and N^3/6-class FMA counts instead of N^3/2.  Written with plain unrolled loops the
+// 16 x 16 block stays in local memory and phase 2 becomes a chain of dependent shared-memory dot products; the template
+// recursion and the register-tiled right-looking phase 2 avoid both.  Default; option "leaf" = 0 / GPB200_LEAF=0 selects the
 // column kernel (cross-check).
 constexpr int NTB = 256;
 constexpr int PB = 16;                                     // panel width
@@ -182,8 +180,8 @@ constexpr int PB = 16;                                     // panel width
 __device__ __forceinline__ double& WT(double* S, int m, int j) { return S[j * LDS + m + 1]; }      // W[m][j], m >= j, in the upper part
 
 // 16 x 16 Cholesky in registers, rows across lanes (lane i = lane & 15 holds a[0..15] of row i).  Template recursion keeps every
-// array index a compile-time constant: with plain unrolled loops the compiler kept a[] in local memory (LDL/STL) and the
-// serial block cost ~7 us (ncu source page, profiles/r02_leaf_*): 8 of them were 43 % of the tile.
+// array index a compile-time constant: with plain unrolled loops the compiler kept a[] in local memory (LDL/STL), which made
+// the serial 16 x 16 blocks a large share of the tile.
 template <int J, int K>
 struct Chol16Upd {
     static __device__ __forceinline__ void run(double (&a)[PB], double lij, int i) {

@@ -1,6 +1,6 @@
 // shard_impl.cuh -- ROW-SHARDED multi-GPU schedules (included by gpb200.cu inside its anonymous namespace).
 //
-// North-star: "for N beyond one GPU's HBM the Gram matrix is row-block sharded across the 8 B200s and a 1-D block
+// North-star: "for N beyond one GPU's HBM the Gram matrix is row-block sharded across the 8 GPUs and a 1-D block
 // Cholesky exchanges panels over NVLink with NCCL" (config C4: Mat32Iso N=131072 d=16, 137 GB per N x N matrix).
 // Reference memory contract being replaced: four N x N host matrices per GPE (test/memory.jl:14-19, src/GP.jl:14-20).
 //

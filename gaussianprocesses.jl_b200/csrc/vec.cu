@@ -121,22 +121,22 @@ __global__ void exp2x_kernel(const double* __restrict__ ln, long long n, double*
 }
 }  // namespace
 
-// ---- FP64 pipe calibration (roofline denominator): DMMA.8x8x4 / DFMA issue rates from registers ----
+// ---- FP64 pipe calibration (roofline denominator): DMMA.16x8x4 (the GEMM's shape) / DFMA issue rates from registers ----
 namespace {
 __global__ void dmma_peak_kernel(double* out, int iters) {
-    double c[16][2];
+    double c[8][4];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) { c[i][0] = 0.0; c[i][1] = 0.0; }
+    for (int i = 0; i < 8; ++i) { c[i][0] = 0.0; c[i][1] = 0.0; c[i][2] = 0.0; c[i][3] = 0.0; }
     const double a = threadIdx.x * 1e-3, b = 1.0 + threadIdx.x * 1e-4;
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                         : "+d"(c[i][0]), "+d"(c[i][1]) : "d"(a), "d"(b));
+        for (int i = 0; i < 8; ++i)
+            asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                         : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(a), "d"(b));
     }
     double s = 0;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) s += c[i][0] + c[i][1];
+    for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 __global__ void dfma_peak_kernel(double* out, int iters) {
@@ -176,7 +176,7 @@ cudaError_t fp64_peak_measure(cudaStream_t st, double* tflops) {
         cudaEventRecord(e1, st); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1); if (rep && ms < best[1]) best[1] = ms;
     }
-    tflops[0] = 2.0 * 256 * 16.0 * iters * warps * sms / best[0] * 1e-9;
+    tflops[0] = 2.0 * 512 * 8.0 * iters * warps * sms / best[0] * 1e-9;     // 8 x (16*8*4 FMA) per warp and iteration
     tflops[1] = 2.0 * 32 * 16.0 * iters * warps * sms / best[1] * 1e-9;
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     cudaFree(out);

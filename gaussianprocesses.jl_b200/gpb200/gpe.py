@@ -1,5 +1,5 @@
 """GPE -- host-side mirror of the reference's exact GP object (src/GPE.jl:3-567) driving the
-B200 engine through the C ABI.  Same field names (x, y, mean, kernel, logNoise, dim, nobs, alpha,
+H100 engine through the C ABI.  Same field names (x, y, mean, kernel, logNoise, dim, nobs, alpha,
 mll, target, dmll, dtarget), same method names minus Julia's `!`, same gradient order
 [noise; mean; kernel] (src/GPE.jl:298-324) and the same error behaviour (PosDefException /
 ValueError where the reference throws PosDefException / ArgumentError).

@@ -11,7 +11,7 @@ for p in (ROOT, os.path.join(ROOT, "gaussianprocesses.jl_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     config.addinivalue_line("markers", "slow: full-size property tests (minutes)")
 
 

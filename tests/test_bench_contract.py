@@ -1,5 +1,5 @@
 """CPU: bench.py's contract -- the reference arm runs on host cores and prints one JSON line with the agreed
-keys; the committed B200 bench lines carry every key the driver / judge read."""
+keys; the committed H100 bench line carries every key a consumer of the line reads."""
 import json
 import os
 import subprocess
@@ -57,7 +57,7 @@ def test_reference_arm_other_ranks_stay_silent():
     assert r.returncode == 0 and r.stdout.strip() == ""
 
 
-@pytest.mark.parametrize("name", ["r01_final_bench_1gpu.json", "r01_final_bench_2gpu.json", "r01_final_bench_8gpu.json"])
+@pytest.mark.parametrize("name", ["h100_bench_1gpu.json"])
 def test_committed_bench_lines_have_every_key(name):
     j = json.load(open(os.path.join(ROOT, "profiles", name)))
     for k in REQUIRED + ["clocks", "roofline"]:

@@ -124,7 +124,7 @@ def test_c5_fitc_properties_at_full_size():
     # The reference's Woodbury form (fitc.jl:33-36: alpha = L^-1 (r - K_fu S^-1 K_uf L^-1 r)) inherits
     # cond(Sigma_QR) ~ lambda_max(K_uf L^-1 K_fu) / lambda_min(K_uu) ~ (M N kbar^2 / sigma^2) / 0.86 ~ 1e10 at C5, so the
     # residual of ANY implementation of those formulas sits near cond * eps ~ 1e-6 |r| (the numpy oracle shows 3e-10 at
-    # N=2e4, M=512 and 5e-10 at N=6e4, M=1024, growing with M N; measured here on the B200: 1.5e-7).
+    # N=2e4, M=512 and 5e-10 at N=6e4, M=1024, growing with M N).
     scond = (M * N * 0.135 ** 2 / nv) / 0.86
     print("C5 residual (Sigma alpha - r) on 48 rows: %.2e |r|   (cond(Sigma_QR) ~ %.1e, cond*eps = %.1e)"
           % (err, scond, scond * np.finfo(float).eps))
