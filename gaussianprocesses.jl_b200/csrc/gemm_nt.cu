@@ -1,19 +1,23 @@
 // gemm_nt.cu -- FP64 tensor-core (DMMA) "NT" GEMM for sm_90a (H100).
 //
 // wgmma has no FP64 form; the FP64 tensor path on Hopper is warp-level mma.sync.f64.  On H100
-// m8n8k4 (SASS DMMA.8x8x4) issues at half the FP64 rate of the m16n8k{4,8,16} shapes, so the
-// kernel uses mma.sync.m16n8k4.f64 (DMMA.16x8x4).  Its A fragment is rows g and g+8 of one k
-// column, so fragment loads and accumulator layout are those of two stacked 8x8x4 tiles.  The
-// kernel keeps the Hopper *data-movement* structure -- one producer warp driving TMA
-// (cp.async.bulk.tensor.2d, 128B-swizzled 16x128 boxes) into a 5-stage shared-memory ring guarded
-// by full/empty mbarriers -- and feeds eight consumer warps that hold a 128x128 FP64 accumulator
-// tile in registers (64x32 per warp = 32 DMMA fragments).
+// m8n8k4 (SASS DMMA.8x8x4) issues at half the FP64 rate of the m16n8k{4,8,16} shapes.  The kernel
+// uses mma.sync.m16n8k16.f64 (DMMA.16x8x16): one instruction per 16-deep stage and fragment pair,
+// 64 FMA per lane for 20 doubles of operand and accumulator traffic (m16n8k4: 16 FMA for 11), which
+// matters because the GEMM runs at the card's power cap.  The A fragment holds rows g and g+8,
+// so the accumulator layout is that of two stacked 8x8 tiles.  The kernel keeps the Hopper
+// *data-movement* structure -- one producer warp driving TMA (cp.async.bulk.tensor.2d,
+// 128B-swizzled 16x128 boxes) into a 5-stage shared-memory ring guarded by full/empty mbarriers --
+// and feeds eight consumer warps that hold a 128x128 FP64 accumulator tile in registers (64x32
+// per warp = 32 DMMA fragments).  The consumers load the first fragments of stage s+1 beside the
+// last MMAs of stage s, so the tensor pipe does not idle at stage boundaries.
 //
 // Shared-memory layout per stage: A tile [128 rows][16 k] then B tile [128 rows][16 k], each row
-// 128 bytes, TMA SWIZZLE_128B (16-byte chunk index ^= row & 7).  A DMMA k-step consumes the four
-// k indices {2s, 2s+1, 8+2s, 9+2s}: with that choice the 16 lanes of a half-warp hit 16 distinct
-// 8-byte bank pairs under the swizzle, so every fragment LDS.64 is conflict-free (any assignment
-// of k indices to the mma's k slots is valid as long as A and B agree).
+// 128 bytes, TMA SWIZZLE_128B (16-byte chunk index ^= row & 7).  Lane (g, tq) feeds k slot q of
+// the mma (logical k tq + 4q) from physical k 8*(tq>>1) + 2q + (tq&1): for each q the 16 lanes
+// of a half-warp hit 16 distinct 8-byte bank pairs under the swizzle, so every fragment LDS.64 is
+// conflict-free (any bijection of k indices to the mma's k slots is valid as long as A and B
+// agree).
 //
 // Per CTA tile and k-step of 16: 32 KB staged for 128*128*16 FMAs = 2048 clk of DMMA at
 // 128 FMA/clk/SM -> 16 B/clk/SM of L2 traffic; HBM traffic is a fraction of that thanks to the
@@ -141,10 +145,15 @@ __device__ __forceinline__ TileCtx decode_tile(const GemmKP& p) {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// D[16x8] += A[16x4] B[4x8]: a0 / a1 = rows g / g+8 of A, {c0,c1} / {c2,c3} = rows g / g+8 of D.
-__device__ __forceinline__ void dmma1684(double (&c_lo)[2], double (&c_hi)[2], double a_lo, double a_hi, double b) {
-    asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-        : "+d"(c_lo[0]), "+d"(c_lo[1]), "+d"(c_hi[0]), "+d"(c_hi[1]) : "d"(a_lo), "d"(a_hi), "d"(b));
+// D[16x8] += A[16x16] B[16x8]: a_lo / a_hi = rows g / g+8 of A, {c0,c1} / {c2,c3} = rows g / g+8 of D.  k slot q
+// of lane (g, tq) is a_lo[q], a_hi[q] and b[q].
+__device__ __forceinline__ void dmma16816(double (&c_lo)[2], double (&c_hi)[2], const double (&a_lo)[4],
+                                          const double (&a_hi)[4], const double (&b)[4]) {
+    asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+        "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+        : "+d"(c_lo[0]), "+d"(c_lo[1]), "+d"(c_hi[0]), "+d"(c_hi[1])
+        : "d"(a_lo[0]), "d"(a_hi[0]), "d"(a_lo[1]), "d"(a_hi[1]), "d"(a_lo[2]), "d"(a_hi[2]), "d"(a_lo[3]), "d"(a_hi[3]),
+          "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
 __device__ __forceinline__ double lds_f64(uint32_t addr) {
@@ -152,27 +161,48 @@ __device__ __forceinline__ double lds_f64(uint32_t addr) {
     asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(addr));
     return v;
 }
-__device__ __forceinline__ void sts_v2f64(uint32_t addr, double2 v) {
-    asm volatile("st.shared.v2.f64 [%0], {%1, %2};" ::"r"(addr), "d"(v.x), "d"(v.y) : "memory");
+
+// Fragment loads of one stage.  pa / pb point at row g of the warp's A / B rows in the stage; k slot q is physical k
+// coff[q] (the same for A and B, so any bijection is valid; this one is bank-conflict free, see the header).
+// A rows g + 8i and g + 8i + 8 (row pair i = 0, 2, 4, 6):
+__device__ __forceinline__ void load_a(uint32_t pa, int i, const int (&coff)[4], double (&alo)[4], double (&ahi)[4]) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { alo[q] = lds_f64(pa + i * 1024 + coff[q]); ahi[q] = lds_f64(pa + (i + 1) * 1024 + coff[q]); }
+}
+// B rows g + 8j:
+__device__ __forceinline__ void load_b(uint32_t pb, int j, const int (&coff)[4], double (&b)[4]) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) b[q] = lds_f64(pb + j * 1024 + coff[q]);
 }
 
-// One 16-deep k-step of the 64x32 warp tile out of swizzled shared memory (32-bit shared addresses).
+// Row pairs 0, 2 and 4 of a stage whose B fragments and pair-0 A fragments are in registers; the A fragments of the
+// next pair load beside each pair's MMAs.  Leaves pair 6's A fragments in alo / ahi.
+__device__ __forceinline__ void mma_pairs_0_to_4(uint32_t pa, const int (&coff)[4], double (&acc)[8][4][2],
+                                                 const double (&b)[4][4], double (&alo)[4], double (&ahi)[4]) {
+#pragma unroll
+    for (int i = 0; i < 6; i += 2) {
+        double nlo[4], nhi[4];
+        load_a(pa, i + 2, coff, nlo, nhi);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) dmma16816(acc[i][j], acc[i + 1][j], alo, ahi, b[j]);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { alo[q] = nlo[q]; ahi[q] = nhi[q]; }
+    }
+}
+
+// One 16-deep k-step of the 64x32 warp tile out of swizzled shared memory (32-bit shared addresses): one
+// m16n8k16 per (row pair, column fragment).  The TMA consumer loop issues the same MMAs in the same order.
 __device__ __forceinline__ void compute_stage(uint32_t sA, uint32_t sB,
                                               double (&acc)[8][4][2], int wm, int wn, int g, const int (&coff)[4]) {
     const uint32_t pa = sA + (wm * 64 + g) * 128;
     const uint32_t pb = sB + (wn * 32 + g) * 128;
+    double b[4][4], alo[4], ahi[4];
 #pragma unroll
-    for (int s = 0; s < 4; ++s) {
-        double a[8], b[4];
+    for (int j = 0; j < 4; ++j) load_b(pb, j, coff, b[j]);
+    load_a(pa, 0, coff, alo, ahi);
+    mma_pairs_0_to_4(pa, coff, acc, b, alo, ahi);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) a[i] = lds_f64(pa + i * 1024 + coff[s]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) b[j] = lds_f64(pb + j * 1024 + coff[s]);
-#pragma unroll
-        for (int i = 0; i < 8; i += 2)                  // a[i], a[i+1]: rows g + 8i and g + 8i + 8 of the warp tile
-#pragma unroll
-            for (int j = 0; j < 4; ++j) dmma1684(acc[i][j], acc[i + 1][j], a[i], a[i + 1], b[j]);
-    }
+    for (int j = 0; j < 4; ++j) dmma16816(acc[6][j], acc[7][j], alo, ahi, b[j]);
 }
 
 __device__ __forceinline__ void epilogue(const GemmKP& p, const TileCtx& t, double (&acc)[8][4][2],
@@ -236,6 +266,11 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
                  ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
+__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
 // TMA / mbarrier warp-specialised kernel
@@ -302,22 +337,56 @@ gpb200_dgemm_nt_tma(const __grid_constant__ CUtensorMap mapA, const __grid_const
 #pragma unroll
         for (int j = 0; j < 4; ++j) { acc[i][j][0] = 0.0; acc[i][j][1] = 0.0; }
 
-    int stage = 0; uint32_t phase = 0;
-    for (int kt = t.kt_lo; kt < t.kt_hi; ++kt) {
-        mbar_wait(&full[stage], phase);
-        const uint32_t sA = smem_base + stage * STAGE_BYTES;
-        compute_stage(sA, sA + TILE_BYTES, acc, wm, wn, g, coff);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[stage]);
-        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+    // compute_stage's MMAs, pipelined across stages: the B and first A fragments of stage s+1 load beside the last
+    // three MMAs of stage s, so no warp waits for a barrier or a fragment load at the top of a stage.  The consumers
+    // wait on exactly the stages the producer fills, in its order (one per k-step).
+    const uint32_t pa0 = smem_base + (wm * 64 + g) * 128;
+    const uint32_t pb0 = smem_base + TILE_BYTES + (wn * 32 + g) * 128;
+    const int nk = t.kt_hi - t.kt_lo;
+    if (nk > 0) {
+        int stage = 0; uint32_t phase = 0;
+        double b[4][4], alo[4], ahi[4];
+        mbar_wait(&full[0], 0);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) load_b(pb0, j, coff, b[j]);
+        load_a(pa0, 0, coff, alo, ahi);
+        for (int it = 1;; ++it) {
+            mma_pairs_0_to_4(pa0 + stage * STAGE_BYTES, coff, acc, b, alo, ahi);
+            // This MMA consumes the last fragments loaded from the stage (B was consumed by pair 0).
+            dmma16816(acc[6][0], acc[7][0], alo, ahi, b[0]);
+            if (it == nk) {                              // the producer refills no slot after its last k-step
+#pragma unroll
+                for (int j = 1; j < 4; ++j) dmma16816(acc[6][j], acc[7][j], alo, ahi, b[j]);
+                break;
+            }
+            const int done = stage;
+            if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+            mbar_wait(&full[stage], phase);
+            // The slot goes back to the producer only here: an arrive does not wait for outstanding LDS, and the
+            // wait loop above keeps the compiler from hoisting the arrive above the MMA that consumed them.
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[done]);
+            const uint32_t pb = pb0 + stage * STAGE_BYTES;
+            double nlo[4], nhi[4];
+            load_b(pb, 0, coff, b[0]);
+            load_a(pa0 + stage * STAGE_BYTES, 0, coff, nlo, nhi);
+#pragma unroll
+            for (int j = 1; j < 4; ++j) {
+                dmma16816(acc[6][j], acc[7][j], alo, ahi, b[j]);
+                load_b(pb, j, coff, b[j]);
+            }
+#pragma unroll
+            for (int q = 0; q < 4; ++q) { alo[q] = nlo[q]; ahi[q] = nhi[q]; }
+        }
     }
     epilogue(p, t, acc, wm, wn, g, tq);
 }
 
 // ---------------------------------------------------------------------------------------------
-// Simple kernel: same tile math and the same swizzled smem layout, but filled by plain
-// global loads with a register double-buffer and __syncthreads.  Kept as the bring-up /
-// cross-check path (option "gemm"=1) -- two independent loaders, one consumer.
+// Simple kernel: same tile math and the same swizzled smem layout, but filled by cp.async
+// (16-byte global -> shared copies, no register staging next to the 128 accumulator registers)
+// into two stages with __syncthreads.  Kept as the bring-up / cross-check path (option
+// "gemm"=1) -- two independent loaders, one consumer.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SIMPLE_THREADS, 1) gpb200_dgemm_nt_simple(const GemmKP p) {
     const TileCtx t = decode_tile(p);
@@ -340,26 +409,13 @@ __global__ void __launch_bounds__(SIMPLE_THREADS, 1) gpb200_dgemm_nt_simple(cons
 
     const int ar = p.a_row0 + t.zoff + t.bm * BM;
     const int br = p.b_row0 + t.zoff + t.bn * BN;
-    double2 ra[4], rb[4];
 
-    auto gload = [&](int kt) {
+    // 16-byte global -> shared copies of one k-step into the swizzled layout, in flight while the other stage computes
+    auto gcopy = [&](int kt, int stage) {
         const int ac = p.a_col0 + t.zoff + kt * BK;
         const int bc = p.b_col0 + t.zoff + kt * BK;
         const bool asub = p.a_has_sub && (ac >> 7) == (ar >> 7);
         const bool bsub = p.b_has_sub && (bc >> 7) == (br >> 7);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int chunk = threadIdx.x + i * SIMPLE_THREADS;
-            const int row = chunk >> 3, c = chunk & 7;
-            const double* pa = asub ? p.Asub + (long long)(ar + row) * 128 + (ac & 127) + c * 2
-                                    : p.A + (long long)(ar + row) * p.lda + ac + c * 2;
-            const double* pb = bsub ? p.Bsub + (long long)(br + row) * 128 + (bc & 127) + c * 2
-                                    : p.B + (long long)(br + row) * p.ldb + bc + c * 2;
-            ra[i] = *reinterpret_cast<const double2*>(pa);
-            rb[i] = *reinterpret_cast<const double2*>(pb);
-        }
-    };
-    auto sstore = [&](int stage) {
         const uint32_t sA = smem_base + stage * STAGE_BYTES;
         const uint32_t sB = sA + TILE_BYTES;
 #pragma unroll
@@ -367,23 +423,28 @@ __global__ void __launch_bounds__(SIMPLE_THREADS, 1) gpb200_dgemm_nt_simple(cons
             const int chunk = threadIdx.x + i * SIMPLE_THREADS;
             const int row = chunk >> 3, c = chunk & 7;
             const int off = row * 128 + ((c ^ (row & 7)) << 4);
-            sts_v2f64(sA + off, ra[i]);
-            sts_v2f64(sB + off, rb[i]);
+            const double* pa = asub ? p.Asub + (long long)(ar + row) * 128 + (ac & 127) + c * 2
+                                    : p.A + (long long)(ar + row) * p.lda + ac + c * 2;
+            const double* pb = bsub ? p.Bsub + (long long)(br + row) * 128 + (bc & 127) + c * 2
+                                    : p.B + (long long)(br + row) * p.ldb + bc + c * 2;
+            cp_async16(sA + off, pa);
+            cp_async16(sB + off, pb);
         }
+        cp_async_commit();
     };
 
     if (t.kt_lo < t.kt_hi) {
         const bool down = (p.flags & GEMM_KLO_M) != 0 && p.k_down;
         auto kmap = [&](int it) { return down ? (t.kt_hi - 1 - (it - t.kt_lo)) : it; };
-        gload(kmap(t.kt_lo));
-        sstore(0);
+        gcopy(kmap(t.kt_lo), 0);
+        cp_async_wait_all();
         __syncthreads();
         int stage = 0;
         for (int kt = t.kt_lo; kt < t.kt_hi; ++kt) {
-            if (kt + 1 < t.kt_hi) gload(kmap(kt + 1));
+            if (kt + 1 < t.kt_hi) gcopy(kmap(kt + 1), stage ^ 1);
             const uint32_t sA = smem_base + stage * STAGE_BYTES;
             compute_stage(sA, sA + TILE_BYTES, acc, wm, wn, g, coff);
-            if (kt + 1 < t.kt_hi) sstore(stage ^ 1);
+            cp_async_wait_all();
             __syncthreads();
             stage ^= 1;
         }

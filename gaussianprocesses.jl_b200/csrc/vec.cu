@@ -121,7 +121,7 @@ __global__ void exp2x_kernel(const double* __restrict__ ln, long long n, double*
 }
 }  // namespace
 
-// ---- FP64 pipe calibration (roofline denominator): DMMA.16x8x4 (the GEMM's shape) / DFMA issue rates from registers ----
+// ---- FP64 pipe calibration (roofline denominator): DMMA.16x8x16 (the GEMM's shape) / DFMA issue rates from registers ----
 namespace {
 __global__ void dmma_peak_kernel(double* out, int iters) {
     double c[8][4];
@@ -131,8 +131,9 @@ __global__ void dmma_peak_kernel(double* out, int iters) {
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
         for (int i = 0; i < 8; ++i)
-            asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-                         : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(a), "d"(b));
+            asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%4,%4,%4,%4,%4,%4,%4}, "
+                         "{%5,%5,%5,%5}, {%0,%1,%2,%3};"
+                         : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(b));
     }
     double s = 0;
 #pragma unroll
@@ -159,7 +160,7 @@ cudaError_t fp64_peak_measure(cudaStream_t st, double* tflops) {
     int dev = 0, sms = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int warps = 8, iters = 40000;
+    const int warps = 8, iters = 10000;
     double* out = nullptr;
     cudaError_t e = cudaMalloc(&out, sizeof(double) * sms * warps * 32);
     if (e != cudaSuccess) return e;
@@ -176,7 +177,7 @@ cudaError_t fp64_peak_measure(cudaStream_t st, double* tflops) {
         cudaEventRecord(e1, st); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1); if (rep && ms < best[1]) best[1] = ms;
     }
-    tflops[0] = 2.0 * 512 * 8.0 * iters * warps * sms / best[0] * 1e-9;     // 8 x (16*8*4 FMA) per warp and iteration
+    tflops[0] = 2.0 * 2048 * 8.0 * iters * warps * sms / best[0] * 1e-9;    // 8 x (16*8*16 FMA) per warp and iteration
     tflops[1] = 2.0 * 32 * 16.0 * iters * warps * sms / best[1] * 1e-9;
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     cudaFree(out);

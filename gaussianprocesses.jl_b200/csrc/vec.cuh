@@ -16,7 +16,7 @@ cudaError_t rowdot_launch(const double* Kst, int64_t ldk, const double* alpha, i
 cudaError_t rowvar_launch(const double* Vt, int64_t ldk, const double* kdiag, int64_t M, int64_t N, double* var, cudaStream_t st);
 // v[i] = exp(2*ln[i])
 cudaError_t exp2x_launch(const double* ln, int64_t n, double* out, cudaStream_t st);
-// FP64 issue-rate microbenchmark: tflops[0] = DMMA.16x8x4, tflops[1] = DFMA (register operands)
+// FP64 issue-rate microbenchmark: tflops[0] = DMMA.16x8x16, tflops[1] = DFMA (register operands)
 cudaError_t fp64_peak_measure(cudaStream_t st, double* tflops);
 // elementwise: op 0 out=a+s | 1 out=a/b | 2 out+=a | 3 out=(a-b)/c | 4 out=log(a) | 5 out=1/a
 cudaError_t ew_launch(int op, int64_t n, double* out, const double* a, const double* b, const double* c, double s, cudaStream_t st);

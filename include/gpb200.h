@@ -186,8 +186,8 @@ int  gpb200_set_option(gpb200_handle* h, const char* key, int64_t value);
 /* run all work of this handle on the caller's CUDA stream (cudaStream_t; NULL = a private
  * stream again), so that the caller's events bracket it (bench.py: torch.cuda.Event).         */
 int  gpb200_set_stream(gpb200_handle* h, void* cuda_stream);
-/* FP64 roofline denominators measured on this device: DMMA.16x8x4 (mma.sync f64, the FP64 tensor
- * path on sm_90a) and DFMA issue rates, TFLOP/s.                                             */
+/* FP64 roofline denominators measured on this device: DMMA.16x8x16 (mma.sync f64, the FP64 tensor
+ * path on sm_90a, the shape the GEMM issues) and DFMA issue rates, TFLOP/s.                  */
 int  gpb200_fp64_peak(gpb200_handle* h, double* tflops_dmma, double* tflops_dfma);
 
 /* ---- raw kernels exposed for the parity tests and the roofline bench ----------------------
