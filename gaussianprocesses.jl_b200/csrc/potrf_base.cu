@@ -292,20 +292,23 @@ __device__ __forceinline__ void trailing_update(double* S, int c0, int ty, int t
         }
 }
 
-__global__ void __launch_bounds__(NTB, 1)
-potrf128_blk_kernel(const double* __restrict__ G, long long ldg, double* __restrict__ F, long long ldf,
-                    double* __restrict__ Dinv, double* __restrict__ DinvT, double* __restrict__ logd,
-                    int* __restrict__ info, int p0, int tile_stride, const PotrfPeers peers) {
+// One tile.  G / Dinv / DinvT / logd point at the tile's origin (Dinv and DinvT share the leading dimension ldd); `p` is the
+// tile's diagonal offset in the peers' buffers and info_base + j + 1 is recorded for a non-positive pivot j.  kWriteF = false
+// skips the L output (the batched block-diagonal factorisation of fsa.cu needs only the two inverse tiles).
+template <bool kWriteF>
+__device__ __forceinline__ void potrf128_blk_tile(const double* __restrict__ G, long long ldg, double* __restrict__ F, long long ldf,
+                                                  double* __restrict__ Dinv, double* __restrict__ DinvT, long long ldd,
+                                                  double* __restrict__ logd, int* __restrict__ info, int info_base, int p,
+                                                  const PotrfPeers& peers) {
     extern __shared__ double S[];                  // [128][129] tile | W16[8][16][17] | T[16][129] | invd[128]
     double* W16 = S + T * LDS;
     double* Tb = W16 + 8 * PB * 17;
     double* invd = Tb + PB * LDS;
-    const int p = p0 + blockIdx.x * tile_stride;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     for (int idx = tid; idx < T * T; idx += NTB) {
         const int m = idx >> 7, n = idx & 127;
-        S[m * LDS + n] = (n <= m) ? G[(long long)(p + m) * ldg + p + n] : 0.0;
+        S[m * LDS + n] = (n <= m) ? G[(long long)m * ldg + n] : 0.0;
     }
     if (tid < T) S[tid * LDS + T] = 0.0;                  // column 128 holds W[127][.]: the phase-2 accumulators start from zero
     __syncthreads();
@@ -320,7 +323,7 @@ potrf128_blk_kernel(const double* __restrict__ G, long long ldg, double* __restr
             double a[PB];
 #pragma unroll
             for (int k = 0; k < PB; ++k) a[k] = (k <= i) ? S[(c0 + i) * LDS + c0 + k] : 0.0;
-            Chol16Step<0>::run(a, i, lane, invd + c0, info, p + c0);
+            Chol16Step<0>::run(a, i, lane, invd + c0, info, info_base + c0);
             if (lane < PB) {
 #pragma unroll
                 for (int k = 0; k < PB; ++k) if (k <= i) S[(c0 + i) * LDS + c0 + k] = a[k];
@@ -366,15 +369,15 @@ potrf128_blk_kernel(const double* __restrict__ G, long long ldg, double* __restr
     // pivots: logd = log(d_j) = 2 log L_jj
     if (tid < T) {
         const double lg = 2.0 * log(S[tid * LDS + tid]);
-        logd[p + tid] = lg;
+        logd[tid] = lg;
         for (int q = 0; q < peers.n; ++q) peers.logd[q][p + tid] = lg;
     }
     // L (lower triangle) to global memory
-    for (int idx = tid; idx < T * T; idx += NTB) {
+    for (int idx = tid; kWriteF && idx < T * T; idx += NTB) {
         const int m = idx >> 7, j = idx & 127;
         if (j <= m) {
             const double v = S[m * LDS + j];
-            F[(long long)(p + m) * ldf + p + j] = v;
+            F[(long long)m * ldf + j] = v;
             for (int q = 0; q < peers.n; ++q) peers.F[q][(long long)(p + m) * ldf + p + j] = v;
         }
     }
@@ -439,8 +442,8 @@ potrf128_blk_kernel(const double* __restrict__ G, long long ldg, double* __restr
         const int r = idx >> 7, c = idx & 127;
         const double wl = (c <= r) ? S[c * LDS + r + 1] : 0.0;
         const double wu = (c >= r) ? S[r * LDS + c + 1] : 0.0;
-        Dinv[(long long)(p + r) * T + c] = wl;
-        DinvT[(long long)(p + r) * T + c] = wu;
+        Dinv[(long long)r * ldd + c] = wl;
+        DinvT[(long long)r * ldd + c] = wu;
         for (int q = 0; q < peers.n; ++q) {
             peers.Dinv[q][(long long)(p + r) * T + c] = wl;
             peers.DinvT[q][(long long)(p + r) * T + c] = wu;
@@ -448,7 +451,23 @@ potrf128_blk_kernel(const double* __restrict__ G, long long ldg, double* __restr
     }
 }
 
-bool g_attr_set = false, g_attr_set_blk = false;
+__global__ void __launch_bounds__(NTB, 1)
+potrf128_blk_kernel(const double* __restrict__ G, long long ldg, double* __restrict__ F, long long ldf,
+                    double* __restrict__ Dinv, double* __restrict__ DinvT, double* __restrict__ logd,
+                    int* __restrict__ info, int p0, int tile_stride, const PotrfPeers peers) {
+    const int p = p0 + blockIdx.x * tile_stride;
+    potrf128_blk_tile<true>(G + (long long)p * ldg + p, ldg, F + (long long)p * ldf + p, ldf, Dinv + (long long)p * T,
+                            DinvT + (long long)p * T, T, logd + p, info, p, p, peers);
+}
+
+// pointer-table entry point: CTA b factors the tile of items[b]
+__global__ void __launch_bounds__(NTB, 1) potrf128_ptr_kernel(const Potrf128Item* __restrict__ items, int* __restrict__ info) {
+    const Potrf128Item it = items[blockIdx.x];
+    const PotrfPeers none{};
+    potrf128_blk_tile<false>(it.G, it.ld, nullptr, 0, it.Dinv, it.DinvT, it.ld, it.logd, info, it.info_base, 0, none);
+}
+
+bool g_attr_set = false, g_attr_set_blk = false, g_attr_set_ptr = false;
 int g_leaf_variant = -1;
 
 }  // namespace
@@ -482,3 +501,15 @@ cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf
     return cudaGetLastError();
 }
 void potrf128_set_variant(int blocked) { g_leaf_variant = blocked ? 1 : 0; }
+
+cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    const size_t smb = (size_t)(T * LDS + 8 * PB * 17 + PB * LDS + T) * sizeof(double);
+    if (!g_attr_set_ptr) {
+        cudaError_t e = cudaFuncSetAttribute(potrf128_ptr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb);
+        if (e != cudaSuccess) return e;
+        g_attr_set_ptr = true;
+    }
+    potrf128_ptr_kernel<<<n, NTB, smb, st>>>(items, info);
+    return cudaGetLastError();
+}

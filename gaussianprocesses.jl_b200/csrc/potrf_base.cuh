@@ -16,3 +16,17 @@ cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf
                             const PotrfPeers* peers = nullptr);
 // 1 (default) = blocked 16-column-panel kernel (74.5 us per tile), 0 = one-barrier-per-column kernel (123 us; cross-check); process-wide
 void potrf128_set_variant(int blocked);
+// pointer-table entry point (batched block-diagonal factorisation, fsa.cu): tile b of the launch reads the lower triangle of
+// items[b].G and writes W = L^-1 (clean lower) to items[b].Dinv, W' (clean upper) to items[b].DinvT, all three with leading
+// dimension items[b].ld, and 2 log L_jj to items[b].logd[j]; a non-positive pivot j records info_base + j + 1 (atomicMin,
+// *info initialised to INT_MAX).  G may equal Dinv: the tile is read completely before anything is written.
+struct Potrf128Item {
+    const double* G;
+    double* Dinv;
+    double* DinvT;
+    double* logd;
+    long long ld;
+    int info_base;
+    int pad_;
+};
+cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st);

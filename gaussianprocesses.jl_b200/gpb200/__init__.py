@@ -6,5 +6,5 @@ from .kernels import (Kernel, SEIso, SEArd, SE, Mat12Iso, Mat32Iso, Mat52Iso, Ma
                       FixedKernel, fix, flatten)
 from .means import Mean, MeanZero, MeanConst, MeanLin
 from .gpe import GPE, GP, ElasticGPE
-from .sparse import FITC, DTC, SoR
+from .sparse import FITC, DTC, SoR, FSA
 from . import dist

@@ -21,6 +21,7 @@ MAX_OPS, MAX_THETA, MAX_DIMS, OP_STRIDE = 16, 96, 128, 6
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int32)
+_lp = C.POINTER(C.c_int64)
 _H = C.c_void_p
 
 _SIGNATURES = {
@@ -69,6 +70,8 @@ _SIGNATURES = {
     "gpb200_fitc_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
     "gpb200_fitc_predict_cov": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp]),
     "gpb200_fitc_set_mode": (C.c_int, [_H, C.c_int]),
+    "gpb200_fitc_set_blocks": (C.c_int, [_H, C.c_int64, _lp, _lp]),
+    "gpb200_fitc_predict_fsa": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _lp, _dp, _dp, _dp]),
     "gpb200_fitc_launch_count": (C.c_int64, [_H]),
     "gpb200_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
     "gpb200_group_create": (C.c_int, [C.POINTER(_H), C.c_int]),
@@ -445,8 +448,34 @@ class FitcEngine:
         return mu, cov
 
     def set_mode(self, mode):
-        """0 FITC, 1 DTC, 2 SoR."""
+        """0 FITC, 1 DTC, 2 SoR, 3 FSA."""
         self._check(self._lib.gpb200_fitc_set_mode(self._h, int(mode)), "fitc_set_mode")
+
+    def set_blocks(self, block_ptr, idx):
+        """FSA training blocks in CSR form (0-based): block b is idx[block_ptr[b]:block_ptr[b+1]]."""
+        block_ptr = np.ascontiguousarray(block_ptr, dtype=np.int64)
+        idx = np.ascontiguousarray(idx, dtype=np.int64)
+        if block_ptr.ndim != 1 or block_ptr.size < 2 or idx.shape != (self.N,):
+            raise ValueError("fitc_set_blocks: block_ptr must have nblocks + 1 >= 2 entries and idx N entries")
+        self._check(self._lib.gpb200_fitc_set_blocks(self._h, block_ptr.size - 1, block_ptr.ctypes.data_as(_lp),
+                                                     idx.ctypes.data_as(_lp)), "fitc_set_blocks")
+
+    def predict_fsa(self, xs_pm, block_of, want_var=True, full_cov=False):
+        """FSA predictions: block_of[i] = training block paired with test point i (-1: none).  Returns (mu, var or cov)."""
+        xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
+        Ms, d = xs_pm.shape
+        if d != self.d:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        block_of = np.ascontiguousarray(block_of, dtype=np.int64)
+        if block_of.shape != (Ms,):
+            raise ValueError("fitc_predict_fsa: block_of must have one entry per test point")
+        mu = np.empty(Ms)
+        var = np.empty(Ms) if (want_var and not full_cov) else None
+        cov = np.empty((Ms, Ms)) if full_cov else None
+        self._check(self._lib.gpb200_fitc_predict_fsa(self._h, Ms, _as_dp(xs_pm), d, block_of.ctypes.data_as(_lp), _as_dp(mu),
+                                                      _as_dp(var) if var is not None else None,
+                                                      _as_dp(cov) if cov is not None else None), "fitc_predict_fsa")
+        return mu, (cov if full_cov else var)
 
     def launch_count(self):
         return int(self._lib.gpb200_fitc_launch_count(self._h))

@@ -1,7 +1,7 @@
 """FITC -- host mirror of the reference's sparse strategy `FITC(x, Xu, y, mean, kern, logNoise)`
 (src/sparse/fully_indep_train_conditional.jl:335-338 == GPE(..., FullyIndepStrat(Xu))), over the
 gpb200_fitc_* entry points: update_cK!, alpha / mll / logdet, dmll_noise, dmll_mean!, dmll_kern!,
-predict_f / predict_y."""
+predict_f / predict_y.  DTC, SoR and FSA are modes of the same engine."""
 import math
 
 import numpy as np
@@ -107,3 +107,81 @@ class DTC(FITC):
 class SoR(FITC):
     """Subset of Regressors (src/sparse/subsetofregressors.jl)."""
     _mode = 2
+
+
+FSA_MAX_BLOCK = 2048
+
+
+def blocks_to_csr(blockindices, nobs):
+    """0-based index arrays -> (block_ptr, idx); ValueError unless the blocks partition 0..nobs-1 (empty blocks are allowed)
+    and every block holds at most FSA_MAX_BLOCK points."""
+    blocks = [np.asarray(b, dtype=np.int64).ravel() for b in blockindices]
+    if not blocks:
+        raise ValueError("FSA needs at least one block")
+    sizes = np.array([b.size for b in blocks], dtype=np.int64)
+    if sizes.max() > FSA_MAX_BLOCK:
+        raise ValueError("an FSA block holds %d points; at most %d are supported" % (sizes.max(), FSA_MAX_BLOCK))
+    idx = np.concatenate(blocks) if sizes.sum() else np.zeros(0, dtype=np.int64)
+    if idx.size != nobs or not np.array_equal(np.sort(idx), np.arange(nobs)):
+        raise ValueError("the FSA blocks must partition the training points 0..%d" % (nobs - 1))
+    block_ptr = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    return block_ptr, idx
+
+
+class FSA(FITC):
+    """Full Scale Approximation (src/sparse/full_scale_approximation.jl:480-484): `FSA(x, Xu, blockindices, y, mean, kernel,
+    logNoise)`, the reference's argument order; `blockindices` is a list of 0-based index arrays that partition the
+    training points.  Lambda is block-diagonal: exact covariance inside each block, the inducing-point approximation
+    between blocks.  mll, logdet, alpha and the [noise; mean; kernel] gradient (dmll_noise :328-363, dmll_kern! :274-326) run
+    on the GPU (single device)."""
+    _mode = 3
+
+    def __init__(self, x, Xu, blockindices, y, mean=None, kernel=None, logNoise=-2.0, device=0, distributed=False):
+        if distributed:
+            raise ValueError("FSA runs on a single GPU (distributed=True is not supported)")
+        x = _as_dxn(x)
+        self.blockindices = [np.asarray(b, dtype=np.int64).ravel() for b in blockindices]
+        self._block_ptr, self._idx = blocks_to_csr(self.blockindices, x.shape[1])
+        self._pending_blocks = True
+        super().__init__(x, Xu, y, mean=mean, kernel=kernel, logNoise=logNoise, device=device)
+
+    def update_mll(self):
+        """update_mll! with cK::FullScalePDMat (update_cK! :197-230, `\\` :105-108, logdet :142)."""
+        if self._pending_blocks:
+            self._eng.set_blocks(self._block_ptr, self._idx)
+            self._pending_blocks = False
+        return super().update_mll()
+
+    def predict_f(self, x, blockindpred, full_cov=False):
+        """predict_f(gp, x, blockindpred; full_cov) (:456-477): test block j (0-based index arrays over the columns of x) is
+        paired with training block j; test points in no block (or in a block j >= the number of training blocks) get no
+        Lambda_xf term.  Without full_cov every point is its own one-point block: the variance is the diagonal of the
+        full_cov formula, clamped at 0 (GP.jl:75)."""
+        x = _as_dxn(x)
+        if x.shape[0] != self.dim:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        block_of = test_block_of(blockindpred, x.shape[1])
+        xs = np.ascontiguousarray(x.T)
+        mu, s2 = self._eng.predict_fsa(xs, block_of, full_cov=full_cov)
+        mu = mu + self.mean.mean(xs)
+        return (mu, s2) if full_cov else (mu, np.maximum(s2, 0.0))
+
+    def predict_y(self, x, blockindpred, full_cov=False):
+        mu, s2 = self.predict_f(x, blockindpred, full_cov=full_cov)
+        if full_cov:
+            return mu, s2 + self.noise_variance() * np.eye(s2.shape[0])
+        return mu, s2 + self.noise_variance()
+
+
+def test_block_of(blockindpred, npred):
+    """0-based test blocks -> block_of[npred] (the training block each test point is paired with, -1 for none);
+    ValueError for an index out of range or a test point in two blocks."""
+    block_of = np.full(npred, -1, dtype=np.int64)
+    for j, ind in enumerate(blockindpred):
+        ind = np.asarray(ind, dtype=np.int64).ravel()
+        if ind.size and (ind.min() < 0 or ind.max() >= npred):
+            raise ValueError("prediction block %d indexes outside the %d test points" % (j, npred))
+        if np.any(block_of[ind] != -1) or np.unique(ind).size != ind.size:
+            raise ValueError("a test point lies in two prediction blocks")
+        block_of[ind] = j
+    return block_of

@@ -357,7 +357,18 @@ struct B200Sparse{M<:AbstractMatrix} <: SparseStrategy
     device::Int
 end
 B200Sparse(Xu::AbstractMatrix, mode::Symbol=:FITC) = B200Sparse(Xu, mode, 0)
-const SPARSE_MODE = Dict(:FITC => 0, :DTC => 1, :SoR => 2)
+const SPARSE_MODE = Dict(:FITC => 0, :DTC => 1, :SoR => 2, :FSA => 3)
+
+# FSA (src/sparse/full_scale_approximation.jl) is mode 3 of the same engine, with the training blocks (1-based index vectors
+# that partition 1:n, at most 2048 points each):
+#     gp = GPE(x, y, mean, kernel, logNoise, B200FSA(Xu, blockindices));  predict_f(gp, xtest, blockindpred; full_cov)
+struct B200FSA{M<:AbstractMatrix} <: SparseStrategy
+    inducing::M
+    blockindices::Vector{Vector{Int}}
+    device::Int
+end
+B200FSA(Xu::AbstractMatrix, blockindices) = B200FSA(Xu, [Vector{Int}(b) for b in blockindices], 0)
+const B200SparseStrategy = Union{B200Sparse, B200FSA}
 
 mutable struct B200SparsePDMat <: AbstractPDMat{Float64}
     handle::Ptr{Cvoid}
@@ -387,12 +398,12 @@ function checks(cK::B200SparsePDMat, rc::Integer, what)
     error("$what failed ($rc): $msg")
 end
 
-KernelData(k::Kernel, X1::AbstractMatrix, X2::AbstractMatrix, ::B200Sparse) = EmptyData()
+KernelData(k::Kernel, X1::AbstractMatrix, X2::AbstractMatrix, ::B200SparseStrategy) = EmptyData()
 alloc_cK(cs::B200Sparse, nobs) = B200SparsePDMat(cs, nobs)
+alloc_cK(cs::B200FSA, nobs) = B200SparsePDMat(B200Sparse(cs.inducing, :FSA, cs.device), nobs)
 
-# update_cK!(::FullyIndepPDMat) fitc.jl:134-156 / update_cK!(::SubsetOfRegsPDMat) sor.jl:96-106
-function update_cK!(cK::B200SparsePDMat, x::AbstractMatrix, kernel::Kernel, logNoise::Real, data::KernelData, cs::B200Sparse)
-    X = Matrix{Float64}(x); Xu = Matrix{Float64}(cs.inducing)
+# inputs, inducing points and kernel program of update_cK!; returns the device parameter vector
+function sparse_data!(cK::B200SparsePDMat, X::Matrix{Float64}, Xu::Matrix{Float64}, kernel::Kernel)
     d, n = size(X)
     checks(cK, ccall((:gpb200_fitc_set_data, LIB), Cint,
                      (Ptr{Cvoid}, Int64, Int32, Ptr{Float64}, Int64, Int64, Ptr{Float64}, Int64),
@@ -401,6 +412,24 @@ function update_cK!(cK::B200SparsePDMat, x::AbstractMatrix, kernel::Kernel, logN
     cK.exposed = exposed; cK.ntheta = length(theta)
     checks(cK, ccall((:gpb200_fitc_set_kernel, LIB), Cint, (Ptr{Cvoid}, Int32, Ptr{Int32}, Int32, Ptr{Int32}, Int32),
                      cK.handle, length(ops) ÷ 6, ops, length(dims), dims, length(theta)), "fitc_set_kernel")
+    return theta
+end
+
+# update_cK!(::FullyIndepPDMat) fitc.jl:134-156 / update_cK!(::SubsetOfRegsPDMat) sor.jl:96-106
+function update_cK!(cK::B200SparsePDMat, x::AbstractMatrix, kernel::Kernel, logNoise::Real, data::KernelData, cs::B200Sparse)
+    theta = sparse_data!(cK, Matrix{Float64}(x), Matrix{Float64}(cs.inducing), kernel)
+    checks(cK, ccall((:gpb200_fitc_factorize, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Float64),
+                     cK.handle, theta, Float64(logNoise)), "fitc_factorize")
+    return cK
+end
+
+# update_cK!(::FullScalePDMat) full_scale_approximation.jl:197-230: the blocks cross the ABI in 0-based CSR form
+function update_cK!(cK::B200SparsePDMat, x::AbstractMatrix, kernel::Kernel, logNoise::Real, data::KernelData, cs::B200FSA)
+    theta = sparse_data!(cK, Matrix{Float64}(x), Matrix{Float64}(cs.inducing), kernel)
+    ptr = Int64[0; cumsum(length.(cs.blockindices))]
+    idx = Int64[i - 1 for b in cs.blockindices for i in b]
+    checks(cK, ccall((:gpb200_fitc_set_blocks, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}),
+                     cK.handle, length(cs.blockindices), ptr, idx), "fitc_set_blocks")
     checks(cK, ccall((:gpb200_fitc_factorize, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Float64),
                      cK.handle, theta, Float64(logNoise)), "fitc_factorize")
     return cK
@@ -417,15 +446,15 @@ end
 logdet(cK::B200SparsePDMat) = cK.logdet
 
 struct B200SparsePrecompute <: AbstractGradientPrecompute end
-init_precompute(::B200Sparse, X, y, k) = B200SparsePrecompute()
+init_precompute(::B200SparseStrategy, X, y, k) = B200SparsePrecompute()
 precompute!(::B200SparsePrecompute, gp) = nothing
 
-function dmll_noise(gp::GPE, ::B200SparsePrecompute, ::B200Sparse)                 # fitc.jl:243-257, sor.jl:159-166
+function dmll_noise(gp::GPE, ::B200SparsePrecompute, ::B200SparseStrategy)         # fitc.jl:243-257, sor.jl:159-166, fsa :328-363
     g = Ref{Float64}(0.0)
     checks(gp.cK, ccall((:gpb200_fitc_grad_noise, LIB), Cint, (Ptr{Cvoid}, Ref{Float64}), gp.cK.handle, g), "fitc_grad_noise")
     return g[]
 end
-function dmll_kern!(dmll::AbstractVector, gp, ::B200SparsePrecompute, ::B200Sparse)    # fitc.jl:200-234, sor.jl:219-253
+function dmll_kern!(dmll::AbstractVector, gp, ::B200SparsePrecompute, ::B200SparseStrategy)   # fitc.jl:200-234, sor.jl:219-253, fsa :274-326
     g = Vector{Float64}(undef, max(gp.cK.ntheta, 1))
     checks(gp.cK, ccall((:gpb200_fitc_grad_kernel, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}), gp.cK.handle, g), "fitc_grad_kernel")
     dmll .= g[gp.cK.exposed]
@@ -446,6 +475,26 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=fa
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
 end
 
-export B200Covariance, B200Sparse, B200ElasticGPE
+# predict_f(gp, x, blockindpred; full_cov) full_scale_approximation.jl:456-477: test block j is paired with training block j
+function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::AbstractVector; full_cov::Bool=false) where {X,Y,M,K,CS<:B200FSA,D,P}
+    size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
+    Xs = Matrix{Float64}(x); Ms = size(Xs, 2)
+    block_of = fill(Int64(-1), Ms)                                                 # 0-based training block of each test point
+    for (j, b) in enumerate(blockindpred), i in b
+        block_of[i] == -1 || throw(ArgumentError("test point $i lies in two prediction blocks"))
+        block_of[i] = j - 1
+    end
+    mu = Vector{Float64}(undef, Ms)
+    var = full_cov ? Float64[] : Vector{Float64}(undef, Ms)
+    Σ = full_cov ? Matrix{Float64}(undef, Ms, Ms) : Matrix{Float64}(undef, 0, 0)
+    checks(gp.cK, ccall((:gpb200_fitc_predict_fsa, LIB), Cint,
+                        (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                        gp.cK.handle, Ms, Xs, size(Xs, 1), block_of, mu, full_cov ? C_NULL : var, full_cov ? Σ : C_NULL),
+           "fitc_predict_fsa")
+    full_cov && return mu .+ mean(gp.mean, Xs), Σ                                 # Σ is symmetric: row- = column-major
+    return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
+end
+
+export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE
 
 end # module

@@ -260,8 +260,32 @@ int  gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64
 /* 0 = FITC (default), 1 = DTC (src/sparse/determ_train_conditional.jl), 2 = SoR
  * (src/sparse/subsetofregressors.jl): the two share Lambda = sigma^2 I (sor.jl:96-106, `\` sor.jl:50,
  * logdet sor.jl:53, dmll_noise sor.jl:159-166, dmll_kern! sor.jl:219-253); SoR's predictive covariance is
- * K_xu S^-1 K_ux (sor.jl:302-321), DTC's adds K_xx - Q_xx (dtc.jl:41-59).                         */
+ * K_xu S^-1 K_ux (sor.jl:302-321), DTC's adds K_xx - Q_xx (dtc.jl:41-59).
+ * 3 = FSA (src/sparse/full_scale_approximation.jl): Lambda = blockdiag(K_ii - Q_ii + (sigma^2 + 1e-10) I) over the
+ * training blocks of gpb200_fitc_set_blocks (update_cK! :197-230).  gpb200_fitc_mll (`\` :105-108, logdet :142) and
+ * gpb200_fitc_grad_noise (dmll_noise :328-363) return the FSA results, alpha in the caller's order; factorize returns
+ * k > 0 when a block of Lambda is not positive definite (k = 1 + the row of the first bad pivot in the padded block
+ * layout).  gpb200_fitc_grad_kernel returns the FSA kernel-parameter gradient (dmll_kern! :274-326).
+ * gpb200_fitc_predict / _predict_cov return GPB200_EINVAL (FSA predictions need test blocks: gpb200_fitc_predict_fsa).
+ * Single GPU only: after gpb200_fitc_comm_init with more than one rank, factorize returns GPB200_EINVAL.          */
 int  gpb200_fitc_set_mode(gpb200_fitc* f, int mode);
+/* FSA training blocks in CSR form: block b is idx[block_ptr[b] .. block_ptr[b+1]) (0-based), nblocks >= 1.  Call after
+ * gpb200_fitc_set_data (which clears them) and before gpb200_fitc_factorize (mode 3 without blocks: GPB200_ESTATE).  The
+ * blocks must partition 0..N-1 (GPB200_EINVAL otherwise); empty blocks are allowed; a block holds at most 2048 points
+ * (GPB200_EINVAL otherwise), which bounds the tile steps of the batched block factorisation.  The rows are reordered once
+ * so that every block starts on a 128-row boundary; device memory grows by 2 * sum_i B_i^2 doubles (the factor and its
+ * inverse, B_i = the block size rounded up to 128), one staging chunk's G_i blocks for the kernel gradient (at most
+ * 32768 * 2048 doubles), O(N) vectors and the work lists, and the staging chunk is grown to its full size.            */
+int  gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block_ptr, const int64_t* idx);
+/* FSA predictMVN / predict_f with test blocks (full_scale_approximation.jl:413-478), mode 3 after gpb200_fitc_mll.
+ * block_of[Ms] is the training block each test point is paired with (test block j pairs with training block j, as the
+ * reference's `zip`); -1 or a block id >= nblocks contributes no Lambda_xf term.  mu_minus_mean[Ms] = K_xu alpha_u +
+ * Lambda_xf alpha;  var[Ms] (may be NULL; not clamped) = the diagonal of Sigma_FSA = K_xx - (Q_xf + Lambda_xf) Sigma^-1
+ * (Q_xf + Lambda_xf)' (each point's variance does not depend on the other test points);  cov[Ms x Ms] (may be NULL) =
+ * Sigma_FSA, row-major.  Test blocks have no size limit (test rows are streamed in chunks); cov needs the test points,
+ * grouped by block and each group padded to a multiple of 128, to fit one staging chunk (GPB200_EINVAL otherwise).      */
+int  gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
+                             double* mu_minus_mean, double* var, double* cov);
 int64_t gpb200_fitc_launch_count(gpb200_fitc* f);
 
 #ifdef __cplusplus
