@@ -26,7 +26,6 @@
 #include "dmma_tile.cuh"
 #include <stdio.h>
 #include <string.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -38,6 +37,8 @@ constexpr int TMA_THREADS = 12 * 32;              // 2 consumer warpgroups (8 wa
 constexpr int SIMPLE_THREADS = 8 * 32;
 constexpr int SMEM_TMA = NSTAGE * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 constexpr int SMEM_SIMPLE = 2 * STAGE_BYTES + 1024;
+// rasterisation of triangular (GEMM_KLO_M) launches: group height in tile rows, k walked downwards (passed in GemmKP)
+constexpr int GM_TRI = 4, K_DOWN = 1;
 
 struct GemmKP {
     const double* A; const double* Asub; const double* B; const double* Bsub;
@@ -447,12 +448,7 @@ cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream) {
     p.a_has_sub = d.A.sub.base != nullptr; p.b_has_sub = d.B.sub.base != nullptr;
     p.klo_off = d.klo_off; p.bm_mod = d.bm_mod; p.bm_rem = d.bm_rem; p.bn_mod = d.bn_mod; p.bn_rem = d.bn_rem;
     p.bm_div = d.bm_div > 0 ? d.bm_div : 1; p.bm_off = d.bm_off; p.bn_div = d.bn_div > 0 ? d.bn_div : 1; p.bn_off = d.bn_off;
-    {
-        static int gm = -1, kd = -1;                 // tuning hooks (read once): GPB200_GM_TRI, GPB200_K_DOWN
-        if (gm < 0) { const char* e = getenv("GPB200_GM_TRI"); gm = e ? atoi(e) : 4; if (gm < 1 || gm > 64) gm = 4;
-                      const char* f = getenv("GPB200_K_DOWN"); kd = f ? (atoi(f) != 0) : 1; }
-        p.gm_tri = gm; p.k_down = kd;
-    }
+    p.gm_tri = GM_TRI; p.k_down = K_DOWN;
     p.own_compact = 0; p.n_own = 0; p.own_first = 0;
     p.n_peer = d.n_peer;
     for (int q = 0; q < 7; ++q) p.Cpeer[q] = q < d.n_peer ? d.Cpeer[q] : nullptr;

@@ -148,7 +148,6 @@ struct gpb200_handle {
     int shard_rb_opt = 0;                      // option "shard_rb": ownership block in 128-row tiles (0 = auto)
     bool sharded = false;                      // current storage mode of F / G
     int rb = 4;                                // effective ownership block (tiles); panel width NBp = 128 * rb
-    int shard_la = 1;                          // option "shard_la": look-ahead schedules of the sharded Cholesky / inverse
     int row_lim = 0;                           // chol_panel: rows below this limit only (diagonal block of a sharded panel); 0 = Npad
     VmBuf vmF, vmG;
     double* P[4] = {nullptr, nullptr, nullptr, nullptr};   // panel buffers, Npad x NBp (global row order); P[1], P[3] double as NBp x Npad row panels
@@ -1044,16 +1043,6 @@ int gpb200_create(gpb200_handle** out, int device) {
         cudaEventCreateWithFlags(&h->ev_la2, cudaEventDisableTiming);
     }
     if ((e = gemm_nt_init()) != cudaSuccess) return bail("gemm_nt_init", e);
-    const char* env = getenv("GPB200_GEMM");
-    if (env) h->gemm_impl = atoi(env);
-    env = getenv("GPB200_DIST_NB");
-    if (env) { int v = atoi(env); if (v == 128 || v == 256 || v == 512 || v == 1024 || v == 2048 || v == 4096) h->dist_nb = v; }
-    env = getenv("GPB200_SHARD_LA");
-    if (env) h->shard_la = atoi(env) ? 1 : 0;
-    env = getenv("GPB200_SHARD_RB");
-    if (env) { int v = atoi(env); if (v == 1 || v == 2 || v == 4 || v == 8) h->shard_rb_opt = v; }
-    env = getenv("GPB200_NB");
-    if (env) { int v = atoi(env); if (v == 0 || v == 128 || v == 256 || v == 512 || v == 1024 || v == 2048 || v == 4096) h->nb = v; }
     *out = h;
     return GPB200_OK;
 }
@@ -1112,7 +1101,6 @@ int gpb200_set_option(gpb200_handle* h, const char* key, int64_t value) {
     }
     if (!strcmp(key, "lookahead")) { h->lookahead = value ? 1 : 0; return GPB200_OK; }
     if (!strcmp(key, "gram_fast")) { h->gram_fast = value ? 1 : 0; return GPB200_OK; }
-    if (!strcmp(key, "leaf")) { potrf128_set_variant(value != 0); h->factored = h->inv_ready = false; return GPB200_OK; }
     if (!strcmp(key, "capacity")) {             // rows reserved by the next gpb200_set_data (>= N): room for gpb200_append
         if (value < 0 || value > ((int64_t)1 << 30)) return fail(h, GPB200_EINVAL, "capacity out of range");
         h->capacity = value; return GPB200_OK;
@@ -1121,16 +1109,13 @@ int gpb200_set_option(gpb200_handle* h, const char* key, int64_t value) {
         if (value < -1 || value > 1) return fail(h, GPB200_EINVAL, "shard must be -1 (auto), 0 or 1");
         h->shard_opt = (int)value; h->factored = h->inv_ready = false; return GPB200_OK;
     }
-    if (!strcmp(key, "shard_la")) { h->shard_la = value ? 1 : 0; return GPB200_OK; }
     if (!strcmp(key, "shard_rb")) {             // ownership block of the row-sharded storage in 128-row tiles (panel = 128 * rb)
         if (value != 0 && value != 1 && value != 2 && value != 4 && value != 8) return fail(h, GPB200_EINVAL, "shard_rb must be 0 (auto), 1, 2, 4 or 8");
         h->shard_rb_opt = (int)value; h->factored = h->inv_ready = false; return GPB200_OK;
     }
-    if (!strcmp(key, "trsv_fused")) {            // 0: one launch per block step; 1: round-1 single-launch kernels; 2 (default): resident-tile kernels
-        if (value < 0 || value > 2) return fail(h, GPB200_EINVAL, "trsv_fused must be 0, 1 or 2");
-        h->trsv_fused = value ? 1 : 0;
-        if (value) trsv_set_variant((int)value);
-        return GPB200_OK;
+    if (!strcmp(key, "trsv_fused")) {            // 0: one launch per block step; 1 (default): single-launch kernels
+        if (value != 0 && value != 1) return fail(h, GPB200_EINVAL, "trsv_fused must be 0 or 1");
+        h->trsv_fused = (int)value; return GPB200_OK;
     }
     if (!strcmp(key, "p2p")) {                 // 0: NCCL panel broadcast even if peer memory is mapped
         if (value && h->n_peer == 0) return fail(h, GPB200_ESTATE, "p2p: ipc_import first");
@@ -1320,7 +1305,7 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
             SCK(q, launch_gram(q, q->G, q->ld, q->rb, q->nranks, q->rank, 1));
         }
         CK(cudaEventRecord(h->ev1, h->st));
-        { int rc = h->shard_la ? shard_cholesky_la(L) : shard_cholesky(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
+        { int rc = shard_cholesky_la(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
         CK(cudaEventRecord(h->ev2, h->st));
         int info_s = 0;
         CK(cudaMemcpyAsync(&info_s, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
@@ -1450,7 +1435,7 @@ int gpb200_grad_prepare(gpb200_handle* h) {
     if (h->sharded) {
         Locals L;
         { int rc = shard_entry(h, L); if (rc) return rc; }
-        { int rc = h->shard_la ? shard_inverse_la(L) : shard_inverse(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
+        { int rc = shard_inverse_la(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
         CK(cudaEventRecord(h->ev1, h->st));
         { int rc = sync_all(L); if (rc) return rc; }
         for (auto* q : L) { profile_collect(q); q->inv_ready = true; }

@@ -9,171 +9,23 @@
 //   logd[p + j]                      <- log(d_j) = 2 log L_jj      (logdet = sum, GPE.jl:210)
 //   info                             <- p + j + 1 of the first non-positive pivot (atomicMin)
 //
-// Design: the tile lives in REGISTERS (512 threads x 32 doubles: thread (warp w, lane l) owns rows
-// l+32a, columns w+16c).  Rows across lanes / columns across warps makes every per-step predicate
-// warp-uniform and lets a whole warp publish a column: step j publishes the unscaled column j to
-// shared memory (S[m][j], m >= j), one __syncthreads, then every thread applies the rank-1 update
-// to its registers (entries above the diagonal are never read and may hold garbage).  Phase 2
-// computes W = L^-1 from W L = I by backward column elimination in the same register layout,
-// publishing column j of W into the strict upper triangle (S[j][m+1]).  One barrier per step, 256
-// steps per tile, no divergent branches, no shared-memory bank conflicts (row stride 129 doubles).
-#include "potrf_base.cuh"
-#include <math.h>
-#include <stdlib.h>
-
-namespace {
-
-constexpr int T = 128;
-constexpr int LDS = 129;
-constexpr int NTH = 512;
-
-__global__ void __launch_bounds__(NTH, 1)
-potrf128_inv_kernel(const double* __restrict__ G, long long ldg, double* __restrict__ F, long long ldf,
-                    double* __restrict__ Dinv, double* __restrict__ DinvT, double* __restrict__ logd,
-                    int* __restrict__ info, int p0, int tile_stride, const PotrfPeers peers) {
-    extern __shared__ double S[];                 // [128][129] + rs[128]
-    double* rs = S + T * LDS;
-    const int p = p0 + blockIdx.x * tile_stride;
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-
-    // coalesced tile load through shared memory, then into the register layout
-    for (int idx = threadIdx.x; idx < T * T; idx += NTH) {
-        const int m = idx >> 7, n = idx & 127;
-        S[m * LDS + n] = (n <= m) ? G[(long long)(p + m) * ldg + p + n] : 0.0;
-    }
-    __syncthreads();
-    double a[4][8];
-#pragma unroll
-    for (int ia = 0; ia < 4; ++ia)
-#pragma unroll
-        for (int c = 0; c < 8; ++c) a[ia][c] = S[(l + 32 * ia) * LDS + w + 16 * c];
-    __syncthreads();
-
-    // ---- phase 1: right-looking Cholesky, unscaled columns published to S[m][j] (m >= j) ----
-#pragma unroll 1
-    for (int j = 0; j < T; ++j) {
-        if (w == (j & 15)) {                       // warp-uniform: this warp owns column j
-            const int cj = j >> 4;
-#pragma unroll
-            for (int ia = 0; ia < 4; ++ia) {
-                double v = a[ia][0];
-#pragma unroll
-                for (int c = 1; c < 8; ++c) if (c == cj) v = a[ia][c];
-                const int m = l + 32 * ia;
-                if (m >= j) S[m * LDS + j] = v;
-            }
-        }
-        __syncthreads();
-        double d = S[j * LDS + j];
-        if (!(d > 0.0)) {                         // not positive definite (or NaN): record, keep going
-            if (threadIdx.x == 0) atomicMin(info, p + j + 1);
-            d = 1.0;
-        }
-        const double invd = __drcp_rn(d);
-        if (threadIdx.x == 0) rs[j] = d;          // pivot; turned into 1/sqrt(d) after the loop
-        double lm[4];
-#pragma unroll
-        for (int ia = 0; ia < 4; ++ia) {
-            const int m = l + 32 * ia;
-            lm[ia] = (m > j) ? S[m * LDS + j] * invd : 0.0;
-        }
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-            const int n = w + 16 * c;
-            if (n > j) {                           // warp-uniform
-                const double cn = S[n * LDS + j];  // broadcast
-#pragma unroll
-                for (int ia = 0; ia < 4; ++ia) a[ia][c] = fma(-lm[ia], cn, a[ia][c]);
-            }
-        }
-    }
-    __syncthreads();   // pivots + all columns published
-    if (threadIdx.x < T) {
-        const double d = rs[threadIdx.x];
-        const double lg = log(d);
-        logd[p + threadIdx.x] = lg;
-        for (int q = 0; q < peers.n; ++q) peers.logd[q][p + threadIdx.x] = lg;
-        rs[threadIdx.x] = 1.0 / sqrt(d);
-    }
-    __syncthreads();
-    // scale the published columns in place: S[m][j] = L[m][j], and write L (lower triangle)
-    for (int idx = threadIdx.x; idx < T * T; idx += NTH) {
-        const int m = idx >> 7, j = idx & 127;
-        if (j <= m) {
-            const double v = S[m * LDS + j] * rs[j];
-            S[m * LDS + j] = v;
-            F[(long long)(p + m) * ldf + p + j] = v;
-            for (int q = 0; q < peers.n; ++q) peers.F[q][(long long)(p + m) * ldf + p + j] = v;
-        }
-    }
-    __syncthreads();
-
-    // ---- phase 2: W L = I, backward over columns; column j of W published to S[j][m+1] (m >= j) ----
-#pragma unroll
-    for (int ia = 0; ia < 4; ++ia)
-#pragma unroll
-        for (int c = 0; c < 8; ++c) a[ia][c] = (l + 32 * ia == w + 16 * c) ? 1.0 : 0.0;
-#pragma unroll 1
-    for (int j = T - 1; j >= 0; --j) {
-        if (w == (j & 15)) {
-            const int cj = j >> 4;
-            const double rsj = rs[j];
-#pragma unroll
-            for (int ia = 0; ia < 4; ++ia) {
-                double v = a[ia][0];
-#pragma unroll
-                for (int c = 1; c < 8; ++c) if (c == cj) v = a[ia][c];
-                const int m = l + 32 * ia;
-                if (m >= j) S[j * LDS + m + 1] = v * rsj;          // W[m][j]
-            }
-        }
-        __syncthreads();
-        double wm[4];
-#pragma unroll
-        for (int ia = 0; ia < 4; ++ia) {
-            const int m = l + 32 * ia;
-            wm[ia] = (m >= j) ? S[j * LDS + m + 1] : 0.0;
-        }
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-            const int kk = w + 16 * c;
-            if (kk < j) {                          // warp-uniform
-                const double ljk = S[j * LDS + kk];                // L[j][k], broadcast
-#pragma unroll
-                for (int ia = 0; ia < 4; ++ia) a[ia][c] = fma(-wm[ia], ljk, a[ia][c]);
-            }
-        }
-    }
-    __syncthreads();
-
-    // ---- write W (clean lower) and W' (clean upper) ----
-    for (int idx = threadIdx.x; idx < T * T; idx += NTH) {
-        const int r = idx >> 7, c = idx & 127;
-        // Dinv[r][c] = W[r][c] = S[c][r+1] for c <= r
-        const double wl = (c <= r) ? S[c * LDS + r + 1] : 0.0;
-        // DinvT[r][c] = W[c][r] = S[r][c+1] for c >= r
-        const double wu = (c >= r) ? S[r * LDS + c + 1] : 0.0;
-        Dinv[(long long)(p + r) * T + c] = wl;
-        DinvT[(long long)(p + r) * T + c] = wu;
-        for (int q = 0; q < peers.n; ++q) {
-            peers.Dinv[q][(long long)(p + r) * T + c] = wl;
-            peers.DinvT[q][(long long)(p + r) * T + c] = wu;
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Blocked variant (option "leaf" = 1, default): the same outputs with 16-wide panels instead of one barrier per column.
+// Design: the tile lives in shared memory (row stride 129 doubles), factored in 16-wide panels.
 //   phase 1, per 16-column panel:  (a) warp 0 factors the 16 x 16 diagonal block in registers (rows across lanes, pivots and
 //            columns exchanged by shuffles);  (b) every row below solves its 16 unknowns against that block (one thread per
 //            row, forward substitution with broadcast reads);  (c) rank-16 update of the trailing lower triangle, 8 x 8
 //            register tiles per thread, 16 shared-memory loads per 64 FMAs.
 //   phase 2: the 16 x 16 diagonal blocks are inverted (one warp per block, one column per lane), then W = L^-1 is built block
 //            row by block row:  W[i, j] = -W_ii * sum_{j <= k < i} L[i, k] W[k, j]  (two small products per block row).
-// ~40 barriers per tile instead of 256 and N^3/6-class FMA counts instead of N^3/2.  Written with plain unrolled loops the
-// 16 x 16 block stays in local memory and phase 2 becomes a chain of dependent shared-memory dot products; the template
-// recursion and the register-tiled right-looking phase 2 avoid both.  Default; option "leaf" = 0 / GPB200_LEAF=0 selects the
-// column kernel (cross-check).
+// ~40 barriers per tile and N^3/6-class FMA counts.  Written with plain unrolled loops the 16 x 16 block stays in local memory
+// and phase 2 becomes a chain of dependent shared-memory dot products; the template recursion and the register-tiled
+// right-looking phase 2 avoid both.
+#include "potrf_base.cuh"
+#include <math.h>
+
+namespace {
+
+constexpr int T = 128;
+constexpr int LDS = 129;
 constexpr int NTB = 256;
 constexpr int PB = 16;                                     // panel width
 
@@ -467,8 +319,9 @@ __global__ void __launch_bounds__(NTB, 1) potrf128_ptr_kernel(const Potrf128Item
     potrf128_blk_tile<false>(it.G, it.ld, nullptr, 0, it.Dinv, it.DinvT, it.ld, it.logd, info, it.info_base, 0, none);
 }
 
-bool g_attr_set = false, g_attr_set_blk = false, g_attr_set_ptr = false;
-int g_leaf_variant = -1;
+// dynamic shared memory of both entry points (layout: potrf128_blk_tile)
+constexpr size_t SMEM_BLK = (size_t)(T * LDS + 8 * PB * 17 + PB * LDS + T) * sizeof(double);
+bool g_attr_set_blk = false, g_attr_set_ptr = false;
 
 }  // namespace
 
@@ -477,39 +330,22 @@ cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf
                             const PotrfPeers* peers) {
     PotrfPeers pp{};
     if (peers) pp = *peers;
-    const size_t sm = (size_t)(T * LDS + T) * sizeof(double);
-    if (!g_attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(potrf128_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    if (!g_attr_set_blk) {
+        cudaError_t e = cudaFuncSetAttribute(potrf128_blk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BLK);
         if (e != cudaSuccess) return e;
-        g_attr_set = true;
+        g_attr_set_blk = true;
     }
-    if (g_leaf_variant < 0) {                              // GPB200_LEAF=0 selects the column-per-barrier kernel (default: blocked kernel)
-        const char* e = getenv("GPB200_LEAF");
-        g_leaf_variant = e ? (atoi(e) != 0) : 1;
-    }
-    if (g_leaf_variant) {
-        const size_t smb = (size_t)(T * LDS + 8 * PB * 17 + PB * LDS + T) * sizeof(double);
-        if (!g_attr_set_blk) {
-            cudaError_t e = cudaFuncSetAttribute(potrf128_blk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb);
-            if (e != cudaSuccess) return e;
-            g_attr_set_blk = true;
-        }
-        potrf128_blk_kernel<<<ntiles, NTB, smb, st>>>(G, ldg, F, ldf, Dinv, DinvT, logd, info, p0, tile_stride, pp);
-        return cudaGetLastError();
-    }
-    potrf128_inv_kernel<<<ntiles, NTH, sm, st>>>(G, ldg, F, ldf, Dinv, DinvT, logd, info, p0, tile_stride, pp);
+    potrf128_blk_kernel<<<ntiles, NTB, SMEM_BLK, st>>>(G, ldg, F, ldf, Dinv, DinvT, logd, info, p0, tile_stride, pp);
     return cudaGetLastError();
 }
-void potrf128_set_variant(int blocked) { g_leaf_variant = blocked ? 1 : 0; }
 
 cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
-    const size_t smb = (size_t)(T * LDS + 8 * PB * 17 + PB * LDS + T) * sizeof(double);
     if (!g_attr_set_ptr) {
-        cudaError_t e = cudaFuncSetAttribute(potrf128_ptr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb);
+        cudaError_t e = cudaFuncSetAttribute(potrf128_ptr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BLK);
         if (e != cudaSuccess) return e;
         g_attr_set_ptr = true;
     }
-    potrf128_ptr_kernel<<<n, NTB, smb, st>>>(items, info);
+    potrf128_ptr_kernel<<<n, NTB, SMEM_BLK, st>>>(items, info);
     return cudaGetLastError();
 }

@@ -14,8 +14,6 @@ struct PotrfPeers {
 cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf, double* Dinv, double* DinvT,
                             double* logd, int* info, int p0, int ntiles, int tile_stride, cudaStream_t st,
                             const PotrfPeers* peers = nullptr);
-// 1 (default) = blocked 16-column-panel kernel (74.5 us per tile), 0 = one-barrier-per-column kernel (123 us; cross-check); process-wide
-void potrf128_set_variant(int blocked);
 // pointer-table entry point (batched block-diagonal factorisation, fsa.cu): tile b of the launch reads the lower triangle of
 // items[b].G and writes W = L^-1 (clean lower) to items[b].Dinv, W' (clean upper) to items[b].DinvT, all three with leading
 // dimension items[b].ld, and 2 log L_jj to items[b].logd[j]; a non-positive pivot j records info_base + j + 1 (atomicMin,

@@ -408,8 +408,8 @@ void own_cols_filter(gpb200_handle* h, GemmDesc& g, int row0_of_B) {
 }
 
 // ---- Cholesky -------------------------------------------------------------------------------------------------
-// G[r1.., c0+off .. c0+off+n) <- (same) * L_kk[off.., off..]^-T  on this rank's rows >= r1 (L_kk sits in P[0] rows c0..)
-cudaError_t shard_trsm_rows(gpb200_handle* h, int c0, int r1, int off, int n, int pb = 0) {
+// G[r1.., c0+off .. c0+off+n) <- (same) * L_kk[off.., off..]^-T  on this rank's rows >= r1 (L_kk sits in P[pb] rows c0..)
+cudaError_t shard_trsm_rows(gpb200_handle* h, int c0, int r1, int off, int n, int pb) {
     const int rows = (int)h->Npad - r1;
     if (n == TILE) {
         GemmDesc g = gemm_desc_default();
@@ -438,70 +438,7 @@ cudaError_t shard_trsm_rows(gpb200_handle* h, int c0, int r1, int off, int n, in
     return shard_trsm_rows(h, c0, r1, off + n1, n2, pb);
 }
 
-int shard_cholesky(const Locals& L) {
-    gpb200_handle* h0 = L[0];
-    const int Np = (int)h0->Npad, R = h0->nranks, NBp = shard_panel_width(h0);
-    const int nblk = (Np + NBp - 1) / NBp;
-    const long long tiles = Np / TILE;
-    for (int k = 0; k < nblk; ++k) {
-        const int c0 = k * NBp, nb = std::min(NBp, Np - c0), o = k % R, r1 = c0 + nb;
-        const int t1 = r1 / TILE;
-        // (a) the owner factors its diagonal block in place (recursive panel Cholesky restricted to the block's rows)
-        for (auto* q : L) {
-            if (q->rank != o) continue;
-            q->row_lim = r1;
-            cudaError_t e = chol_panel(q, c0, nb, NBp);
-            q->row_lim = 0;
-            SCK(q, e);
-            ++q->launches;
-            SCK(q, shard_copy_lower(q->P[0] + (size_t)c0 * NBp, NBp, q->F + (size_t)c0 * q->ld + c0, q->ld, nb, q->st));
-        }
-        // (b) broadcast of the block: L_kk (into the panel buffer), its inverted tiles, log-pivots
-        SRC(coll_group_begin(L));
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->P[0] + (size_t)c0 * NBp); }, sizeof(double) * (size_t)nb * NBp));
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->Dinv + (size_t)c0 * TILE); }, sizeof(double) * (size_t)nb * TILE));
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->DinvT + (size_t)c0 * TILE); }, sizeof(double) * (size_t)nb * TILE));
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->logd + c0); }, sizeof(double) * (size_t)nb));
-        SRC(coll_group_end(L));
-        if (r1 >= Np) break;
-        // (c) every rank: TRSM of its own rows of the panel, kept as rows of L and staged for the all-gather
-        long long maxown = 0;
-        for (int q = 0; q < R; ++q)
-            maxown = std::max(maxown, shard_own_before(tiles, q, h0->rb, R) - shard_own_before(t1, q, h0->rb, R));
-        const size_t per = (size_t)maxown * TILE * NBp;                               // doubles per rank region
-        for (auto* q : L) {
-            SCK(q, shard_trsm_rows(q, c0, r1, 0, nb));
-            ++q->launches;
-            SCK(q, shard_scatter_rows(q->G, q->F, q->ld, Np, c0, nb, t1, q->Sbuf + (size_t)q->rank * per, NBp, own_of(q), q->st));
-        }
-        // (d) all-gather of the panel rows
-        SRC(coll_allgather(L, [&](gpb200_handle* q) { return (void*)q->Sbuf; }, sizeof(double) * per));
-        // (e) global row order; the block owner also keeps the transposed panel = its rows of U = L'
-        for (auto* q : L) {
-            ++q->launches;
-            SCK(q, shard_unpack_panel(q->P[0], NBp, Np, nb, t1, q->Sbuf, (int64_t)per, own_of(q), q->st));
-            if (q->rank == o) {
-                ++q->launches;
-                SCK(q, shard_transpose(q->F + (size_t)c0 * q->ld + r1, q->ld, q->P[0] + (size_t)r1 * NBp, NBp, Np - r1, nb, q->st));
-            }
-        }
-        // (f) trailing update of the own rows: G[i, j] -= P[i] P[j]',  r1 <= j <= i
-        for (auto* q : L) {
-            GemmDesc g = gemm_desc_default();
-            g.A = GemmOperand{bufP(q, 0), bufNone(), r1, 0};
-            g.B = GemmOperand{bufP(q, 0), bufNone(), r1, 0};
-            g.C = q->G; g.ldc = q->ld; g.c_row0 = r1; g.c_col0 = r1;
-            g.M = Np - r1; g.N = Np - r1; g.K = nb;
-            g.alpha = -1.0; g.beta = 1.0;
-            g.flags = GEMM_LOWER_ONLY;
-            own_rows_filter(q, g, r1);
-            SCK(q, launch_gemm(q, g));
-        }
-    }
-    return coll_allreduce_min_info(L);
-}
-
-// Same factorisation with LOOK-AHEAD: the latency-bound chain of a panel (diagonal-block factorisation, its broadcast, the
+// Per panel (see the file head) with LOOK-AHEAD: the latency-bound chain of a panel (diagonal-block factorisation, its broadcast, the
 // R-way split TRSM, the all-gather) runs on the high-priority side stream while the main stream applies the PREVIOUS panel
 // to the bulk of the trailing matrix.  Per panel the main stream first updates only the columns of the next block ("narrow"
 // update, K = NBp, a few hundred tiles), hands over to the chain, then does the rest.  Panel buffers alternate (P[k & 1]).
@@ -657,83 +594,10 @@ int shard_solve(const Locals& L, double* gpb200_handle::*rhs, double* gpb200_han
     return GPB200_OK;
 }
 
-// ---- inverse: backward sweep over row panels ------------------------------------------------------------------------
-int shard_inverse(const Locals& L) {
-    gpb200_handle* h0 = L[0];
-    const int Np = (int)h0->Npad, R = h0->nranks, NBp = shard_panel_width(h0);
-    const int nblk = (Np + NBp - 1) / NBp;
-    for (auto* q : L) {
-        for (auto& run : q->vmG.runs) SCK(q, cudaMemsetAsync((char*)q->G + run.first, 0, run.second, q->st));
-        // W_kk = L_kk^-1 of the own diagonal blocks, level by level (strictly-lower tiles -> G lower, transposed -> G upper;
-        // the diagonal tiles stay in Dinv / DinvT, substituted by the GEMM producer)
-        for (int k = q->rank; k < nblk; k += R) {
-            const int c0 = k * NBp, nb = std::min(NBp, Np - c0);
-            for (int s = TILE; s < nb; s *= 2) {
-                const int batch = (nb + 2 * s - 1) / (2 * s);
-                const int n2 = (nb - s < s) ? nb - s : s;
-                SCK(q, merge_inverse(q, c0, s, n2, batch));
-            }
-        }
-    }
-    for (int k = nblk - 1; k >= 0; --k) {
-        const int j0 = k * NBp, nb = std::min(NBp, Np - j0), o = k % R, r1 = j0 + nb;
-        const int ncols = Np - r1;
-        // 1. owner: finalise X_J.  Beyond the block: Xt[c, i] = -sum_k accT[c, k] Wt_JJ[i, k]  (accT = transposed accumulator),
-        //    written as the column panel (P[0]) and, through the transposed-copy epilogue, as rows of X in place (G upper).
-        for (auto* q : L) {
-            if (q->rank != o) continue;
-            if (ncols > 0) {
-                ++q->launches;
-                SCK(q, shard_transpose(q->Sbuf + (size_t)r1 * NBp, NBp, q->G + (size_t)j0 * q->ld + r1, q->ld, nb, ncols, q->st));
-                GemmDesc g = gemm_desc_default();
-                g.A = GemmOperand{bufS(q), bufNone(), r1, 0};
-                g.B = GemmOperand{bufG(q), bufDinvT(q), j0, j0};
-                g.C = q->P[0]; g.ldc = NBp; g.c_row0 = r1; g.c_col0 = 0;
-                g.Ct = q->G; g.ldct = q->ld; g.ct_row0 = j0; g.ct_col0 = r1;
-                g.M = ncols; g.N = nb; g.K = nb;
-                g.alpha = -1.0;
-                g.flags = GEMM_KLO_N;
-                SCK(q, launch_gemm(q, g));
-            }
-            ++q->launches;
-            SCK(q, shard_pack_wblock(q->P[0], NBp, q->G, q->ld, q->Dinv, j0, nb, q->st));      // inside the block: Xt = W_JJ
-        }
-        // 2. broadcast the column-panel form Xt_J (rows j0.. of P[0])
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->P[0] + (size_t)j0 * NBp); }, sizeof(double) * (size_t)(Np - j0) * NBp));
-        for (auto* q : L) {
-            // 3. row-panel form X_J[i, c] (NBp x Npad view of P[1])
-            ++q->launches;
-            SCK(q, shard_transpose(q->P[1] + j0, Np, q->P[0] + (size_t)j0 * NBp, NBp, Np - j0, nb, q->st));
-            // (1) TRTRI part: accumulators of the own rows i < j0:  G[i, c >= j0] += U[i, J] X_J
-            if (j0 > 0) {
-                GemmDesc g = gemm_desc_default();
-                g.A = GemmOperand{bufF(q), bufNone(), 0, j0};
-                g.B = GemmOperand{bufP(q, 0), bufNone(), j0, 0};
-                g.C = q->G; g.ldc = q->ld; g.c_row0 = 0; g.c_col0 = j0;
-                g.M = j0; g.N = Np - j0; g.K = nb;
-                g.alpha = 1.0; g.beta = 1.0;
-                own_rows_filter(q, g, 0);
-                SCK(q, launch_gemm(q, g));
-            }
-            // (2) LAUUM part: K^-1[i, J] = sum_{c >= i} X[i, c] X_J[j, c] for the own rows i >= j0 (lower part only)
-            {
-                GemmDesc g = gemm_desc_default();
-                g.A = GemmOperand{bufG(q), bufDinvT(q), j0, j0};
-                g.B = GemmOperand{bufXR(q), bufNone(), 0, j0};
-                g.C = q->G; g.ldc = q->ld; g.c_row0 = j0; g.c_col0 = j0;
-                g.M = Np - j0; g.N = nb; g.K = Np - j0;
-                g.flags = GEMM_LOWER_ONLY | GEMM_KLO_M;
-                own_rows_filter(q, g, j0);
-                SCK(q, launch_gemm(q, g));
-            }
-        }
-    }
-    return GPB200_OK;
-}
-
-// The same sweep with LOOK-AHEAD.  Chain of panel J (side stream): finalise X_J, broadcast, transpose, and the part of the
-// TRTRI update that the NEXT finalisation needs (rows of block J-1 only); main stream: the bulk TRTRI update (rows before
-// block J-1) and the LAUUM part of panel J.  Panel buffers alternate between two sets {P[2s], P[2s+1]}.  Dependencies:
+// ---- inverse: backward sweep over row panels (see the file head) with LOOK-AHEAD ---------------------------------------
+// Chain of panel J (side stream): finalise X_J, broadcast, transpose, and the part of the TRTRI update that the NEXT
+// finalisation needs (rows of block J-1 only); main stream: the bulk TRTRI update (rows before block J-1) and the LAUUM
+// part of panel J.  Panel buffers alternate between two sets {P[2s], P[2s+1]}.  Dependencies:
 //   chain(K) starts after main(K+2) finished (its accumulators received panel K+2's contribution; buffer set K&1 is free),
 //   its narrow update waits for main(K+1)'s TRTRI part (both add into the rows of block K-1), main(K) waits for chain(K).
 int shard_inverse_la(const Locals& L) {
@@ -744,6 +608,8 @@ int shard_inverse_la(const Locals& L) {
     for (auto* q : L) {
         if (!q->st_side) return fail(q, GPB200_ECUDA, "sharded look-ahead needs the side stream");
         for (auto& run : q->vmG.runs) SCK(q, cudaMemsetAsync((char*)q->G + run.first, 0, run.second, q->st));
+        // W_kk = L_kk^-1 of the own diagonal blocks, level by level (strictly-lower tiles -> G lower, transposed -> G upper;
+        // the diagonal tiles stay in Dinv / DinvT, substituted by the GEMM producer)
         for (int k = q->rank; k < nblk; k += R) {
             const int c0 = k * NBp, nb = std::min(NBp, Np - c0);
             for (int s = TILE; s < nb; s *= 2) {
@@ -778,6 +644,9 @@ int shard_inverse_la(const Locals& L) {
         }
         int rc = GPB200_OK;
         do {
+            // owner: finalise X_J.  Beyond the block: Xt[c, i] = -sum_k accT[c, k] Wt_JJ[i, k]  (accT = transposed accumulator),
+            // written as the column panel and, through the transposed-copy epilogue, as rows of X in place (G upper);
+            // inside the block: Xt = W_JJ
             for (auto* q : L) {
                 if (q->rank != o) continue;
                 cudaError_t e = cudaSuccess;

@@ -11,7 +11,6 @@
 //  * predictive mean / variance epilogues (/root/reference/src/GP.jl:26, 51-54, 75).
 #include "vec.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace {
 constexpr int T = 128;
@@ -306,11 +305,14 @@ cudaError_t scale_launch(int mode, double* A, int64_t ld, int64_t nrows, int64_t
 }
 
 // ---- single-launch ("sync-free") triangular solves -------------------------------------------------
-// One CTA per 128-row block, all co-resident; CTA b consumes the solution blocks y_i (i < b) as their
-// ready-flags appear, then publishes y_b.  Dependencies always point to lower blockIdx, which the
-// hardware scheduler starts first, and 2*Npad/128 CTAs of 256 threads fit on the chip at once.  The two
-// tiles on the critical chain (L[b,b-1] and the inverted diagonal tile) are prefetched into L2 before
-// the CTA starts waiting.  A watchdog turns a missing flag into an error code instead of a hang.
+// One CTA per 128-row block; CTA b consumes the solution blocks y_i (i < b) as their ready-flags appear, then publishes y_b.
+// The two tiles on the critical chain are RESIDENT before the CTA starts waiting: the inverted diagonal tile in registers
+// (each thread keeps exactly the 16 x 4 entries its part of the tile mat-vec uses) and the neighbour tile L[b, b-1]
+// (forward) / L[b+1, b] (backward) in shared memory.  Per block step the chain is then: flag -> 1 KB vector -> mat-vec out
+// of shared memory -> mat-vec out of registers -> flag, instead of two 128 KB tile reads from L2 (19 us per step with the
+// tiles only prefetched to L2).  128 KB of dynamic shared memory per CTA: one CTA per SM; later CTAs start as earlier ones
+// retire, dependencies only point to lower blockIdx (in-order dispatch).  A watchdog turns a missing flag into an error
+// code instead of a hang.
 namespace {
 __device__ __forceinline__ int ld_acquire(const int* p) {
     int v;
@@ -319,13 +321,6 @@ __device__ __forceinline__ int ld_acquire(const int* p) {
 }
 __device__ __forceinline__ void st_release(int* p, int v) {
     asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void prefetch_tile_l2(const double* M, long long ld) {
-    // 128 rows x 1 KB: 8 lines of 128 B per row
-    for (int idx = threadIdx.x; idx < T * 8; idx += blockDim.x) {
-        const double* p = M + (long long)(idx >> 3) * ld + (idx & 7) * 16;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-    }
 }
 __device__ __forceinline__ bool wait_flag(const int* flag, int* err) {
     long long spins = 0;
@@ -336,71 +331,6 @@ __device__ __forceinline__ bool wait_flag(const int* flag, int* err) {
     return true;
 }
 
-__global__ void __launch_bounds__(256) trsv_fwd_persistent(const double* __restrict__ F, long long ldf, const double* __restrict__ Dinv,
-                                                           const double* __restrict__ r, double* __restrict__ y,
-                                                           int* __restrict__ flags, int* __restrict__ err) {
-    __shared__ double sAcc[T], sY[T], sO[T];
-    __shared__ int ok;
-    const int b = blockIdx.x;
-    const long long q = (long long)b * T;
-    if (threadIdx.x < T) sAcc[threadIdx.x] = r[q + threadIdx.x];
-    prefetch_tile_l2(Dinv + q * T, T);
-    if (b > 0) prefetch_tile_l2(F + q * ldf + (q - T), ldf);
-    __syncthreads();
-    for (int i = 0; i < b; ++i) {
-        if (threadIdx.x == 0) ok = wait_flag(flags + i, err) ? 1 : 0;
-        __syncthreads();
-        if (!ok) return;
-        if (threadIdx.x < T) sY[threadIdx.x] = __ldcg(y + (long long)i * T + threadIdx.x);
-        __syncthreads();
-        tile_matvec(F + q * ldf + (long long)i * T, ldf, sY, sO);
-        __syncthreads();
-        if (threadIdx.x < T) sAcc[threadIdx.x] -= sO[threadIdx.x];
-        __syncthreads();
-    }
-    tile_matvec(Dinv + q * T, T, sAcc, sO);               // y_b = W_bb (r_b - sum_i L_bi y_i)
-    __syncthreads();
-    if (threadIdx.x < T) y[q + threadIdx.x] = sO[threadIdx.x];
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) st_release(flags + b, 1);
-}
-
-__global__ void __launch_bounds__(256) trsv_bwd_persistent(const double* __restrict__ F, long long ldf, const double* __restrict__ DinvT,
-                                                           const double* __restrict__ z, double* __restrict__ a,
-                                                           int* __restrict__ flags, int* __restrict__ err, int nb) {
-    __shared__ double sAcc[T], sA[T], sO[T], sC[T];
-    __shared__ int ok;
-    const int b = nb - 1 - blockIdx.x;                     // dependencies (blocks > b) have lower blockIdx
-    const long long q = (long long)b * T;
-    if (threadIdx.x < T) sAcc[threadIdx.x] = z[q + threadIdx.x];
-    prefetch_tile_l2(DinvT + q * T, T);
-    if (b + 1 < nb) prefetch_tile_l2(F + (q + T) * ldf + q, ldf);
-    __syncthreads();
-    for (int i = nb - 1; i > b; --i) {
-        if (threadIdx.x == 0) ok = wait_flag(flags + i, err) ? 1 : 0;
-        __syncthreads();
-        if (!ok) return;
-        if (threadIdx.x < T) sA[threadIdx.x] = __ldcg(a + (long long)i * T + threadIdx.x);
-        __syncthreads();
-        tile_matvec_t(F + (long long)i * T * ldf + q, ldf, sA, sO, sC);     // L[i-block, b-block]' a_i
-        __syncthreads();
-        if (threadIdx.x < T) sAcc[threadIdx.x] -= sO[threadIdx.x];
-        __syncthreads();
-    }
-    tile_matvec(DinvT + q * T, T, sAcc, sO);              // a_b = W_bb' (z_b - sum_i L_ib' a_i)
-    __syncthreads();
-    if (threadIdx.x < T) a[q + threadIdx.x] = sO[threadIdx.x];
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) st_release(flags + b, 1);
-}
-// ---- version 2 of the single-launch solves: the two tiles on the critical chain are RESIDENT before the CTA starts waiting --
-// the inverted diagonal tile in registers (each thread keeps exactly the 16 x 4 entries its part of the tile mat-vec uses) and
-// the neighbour tile L[b, b-1] (forward) / L[b+1, b] (backward) in shared memory.  Per block step the chain is then: flag ->
-// 1 KB vector -> mat-vec out of shared memory -> mat-vec out of registers -> flag, instead of two 128 KB tile reads from L2
-// (round 1: 19 us per step, 4.8 + 5.9 ms at C2, the same at every GPU count).  128 KB of dynamic shared memory per CTA: one
-// CTA per SM; later CTAs start as earlier ones retire, dependencies only point to lower blockIdx (in-order dispatch).
 __device__ __forceinline__ void load_tile_regs(const double* __restrict__ M, long long ld, double (&t)[16][4]) {
     const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
 #pragma unroll
@@ -493,57 +423,37 @@ __global__ void __launch_bounds__(256, 1) trsv_bwd_persistent2(const double* __r
     __syncthreads();
     if (threadIdx.x == 0) st_release(flags + b, 1);
 }
-bool g_trsv2_attr = false;
-int g_trsv_variant = -1;
-}  // namespace
+bool g_trsv_attr = false;
 
-// GPB200_TRSV=1 selects the round-1 kernels (critical tiles prefetched to L2 only); default: resident-tile kernels
-static bool trsv_use_v2() {
-    if (g_trsv_variant < 0) {
-        const char* e = getenv("GPB200_TRSV");
-        g_trsv_variant = e ? atoi(e) : 2;
-    }
-    if (g_trsv_variant != 2) return false;
-    if (!g_trsv2_attr) {
-        if (cudaFuncSetAttribute(trsv_fwd_persistent2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * T * T)) != cudaSuccess ||
-            cudaFuncSetAttribute(trsv_bwd_persistent2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * T * T)) != cudaSuccess) {
-            (void)cudaGetLastError();
-            g_trsv_variant = 1;
-            return false;
-        }
-        g_trsv2_attr = true;
-    }
-    return true;
+cudaError_t trsv_set_smem_attr() {
+    if (g_trsv_attr) return cudaSuccess;
+    const int bytes = (int)(sizeof(double) * T * T);
+    cudaError_t e = cudaFuncSetAttribute(trsv_fwd_persistent2, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(trsv_bwd_persistent2, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) g_trsv_attr = true;
+    return e;
 }
-void trsv_set_variant(int v) { g_trsv_variant = (v == 2) ? 2 : 1; }
+}  // namespace
 
 // flags: int[Npad/128 + 1] scratch (last entry = watchdog error flag); returns cudaErrorLaunchFailure-free:
 // the caller reads flags[nb] after the stream sync.
 cudaError_t trsv_lower_fwd_fused(const double* F, int64_t ldf, const double* Dinv, const double* r, double* y, int64_t Npad,
                                  int* flags, cudaStream_t st, int64_t* launches) {
     const int nb = (int)(Npad / T);
-    cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(int) * (nb + 1), st);
+    cudaError_t e = trsv_set_smem_attr();
     if (e != cudaSuccess) return e;
-    if (trsv_use_v2()) {
-        trsv_fwd_persistent2<<<nb, 256, sizeof(double) * T * T, st>>>(F, ldf, Dinv, r, y, flags, flags + nb);
-        if (launches) ++*launches;
-        return cudaGetLastError();
-    }
-    trsv_fwd_persistent<<<nb, 256, 0, st>>>(F, ldf, Dinv, r, y, flags, flags + nb);
+    if ((e = cudaMemsetAsync(flags, 0, sizeof(int) * (nb + 1), st)) != cudaSuccess) return e;
+    trsv_fwd_persistent2<<<nb, 256, sizeof(double) * T * T, st>>>(F, ldf, Dinv, r, y, flags, flags + nb);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t trsv_lower_bwd_fused(const double* F, int64_t ldf, const double* DinvT, const double* z, double* a, int64_t Npad,
                                  int* flags, cudaStream_t st, int64_t* launches) {
     const int nb = (int)(Npad / T);
-    cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(int) * (nb + 1), st);
+    cudaError_t e = trsv_set_smem_attr();
     if (e != cudaSuccess) return e;
-    if (trsv_use_v2()) {
-        trsv_bwd_persistent2<<<nb, 256, sizeof(double) * T * T, st>>>(F, ldf, DinvT, z, a, flags, flags + nb, nb);
-        if (launches) ++*launches;
-        return cudaGetLastError();
-    }
-    trsv_bwd_persistent<<<nb, 256, 0, st>>>(F, ldf, DinvT, z, a, flags, flags + nb, nb);
+    if ((e = cudaMemsetAsync(flags, 0, sizeof(int) * (nb + 1), st)) != cudaSuccess) return e;
+    trsv_bwd_persistent2<<<nb, 256, sizeof(double) * T * T, st>>>(F, ldf, DinvT, z, a, flags, flags + nb, nb);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

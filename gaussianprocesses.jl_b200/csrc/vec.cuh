@@ -41,5 +41,3 @@ cudaError_t spd_from_cov_launch(double* dst, int64_t ldd, const double* src, int
 cudaError_t add_rowvec_launch(double* A, int64_t ld, const double* v, int64_t nrows, int64_t ncols, cudaStream_t st);
 // out[a * nv + b] = src[idx[a] * ld + idx[b]]   (principal sub-matrix on an index set; cross-validation folds)
 cudaError_t gather_block_launch(double* out, const double* src, int64_t ld, const long long* idx, int64_t nv, cudaStream_t st);
-// single-launch solves: 2 (default) = critical tiles resident in registers / shared memory, 1 = round-1 kernels (L2 prefetch)
-void trsv_set_variant(int v);

@@ -165,20 +165,15 @@ int64_t gpb200_launch_count(gpb200_handle* h);
  *   "nb"         outer Cholesky block: 0 (default) = fully recursive, else 128*2^k <= 4096 (right-looking panels)
  *   "gemm"       0 = TMA/mbarrier DMMA kernel (default), 1 = simple-loader kernel (bring-up / cross-check)
  *   "lookahead"  1 (default) = next diagonal tile factored on a side stream behind the Schur update
- *   "trsv_fused" single-launch flag-synchronised triangular solves: 2 (default) = critical tiles resident in registers / shared
- *                memory, 1 = round-1 kernels (L2 prefetch only), 0 = one launch per block step
+ *   "trsv_fused" 1 (default) = single-launch flag-synchronised triangular solves, 0 = one launch per block step
  *   "profile"    1 = CUDA events around every GEMM launch (see gpb200_get_timings)
  *   "dist_nb"    multi-GPU: width of an owned block column, 0 = auto (~N/(8*ranks))
  *   "p2p"        multi-GPU: 1 = fused panel push over peer memory (after gpb200_ipc_import), 0 = NCCL broadcast
  *   "gram_fast"  1 (default) = TMA-staged SEIso Gram / trace kernels (gram_fast.cu) when the kernel is one SEIso leaf over
  *                <= 8 dimensions, 0 = always the generic kernel-program kernels (cross-check)
- *   "leaf"       1 (default) = blocked 128 x 128 diagonal-tile kernel (16-column panels, 74.5 us), 0 = column-per-barrier kernel
- *                (123 us; cross-check); process-wide
  *   "capacity"   rows reserved by the next gpb200_set_data (>= N) so that gpb200_append can extend the factor in place
  *   "shard"      multi-GPU storage of the two N x N buffers: 1 = row-sharded (each rank maps only its own block rows),
  *                0 = replicated, -1 (default) = sharded only when the replicated form would not fit the device
- *   "shard_la"   1 (default) = look-ahead schedules of the row-sharded Cholesky / inverse (panel chain on a side stream),
- *                0 = the plain one-stream schedules (cross-check)
  *   "shard_rb"   row-sharded ownership block in 128-row tiles (panel width 128*rb): 0 auto, 1, 2, 4, 8
  * Returns GPB200_EINVAL for unknown keys or values.                                           */
 int  gpb200_set_option(gpb200_handle* h, const char* key, int64_t value);

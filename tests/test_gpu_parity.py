@@ -263,8 +263,9 @@ def test_engine_stream_profile_and_options(engine):
         assert m2 == mll and np.array_equal(a2, alpha)
     with pytest.raises(ValueError):
         engine.set_option("nb", 300)
-    with pytest.raises(ValueError):
-        engine.set_option("no_such_option", 1)
+    for key, value in (("no_such_option", 1), ("leaf", 0), ("shard_la", 0), ("trsv_fused", 2)):
+        with pytest.raises(ValueError):
+            engine.set_option(key, value)
     pk = engine.fp64_peak()
     assert 5.0 < pk["dmma_tflops"] < 80.0 and 5.0 < pk["dfma_tflops"] < 80.0
     assert engine.launch_count() > 0
@@ -415,37 +416,30 @@ def test_elastic_append_matches_batch_fit():
         gp.append(np.zeros((3, 2)), [0.0, 1.0])
 
 
-def test_blocked_diagonal_tile_kernel_matches_column_kernel(engine):
-    """potrf_base.cu: the blocked 128 x 128 leaf (16-column panels, option "leaf" = 1) against the column-per-barrier leaf and
-    the oracle: factor, inverted tiles (through solve / K^-1), log-determinant, and the not-positive-definite report."""
+def test_diagonal_tile_kernel_matches_oracle(engine):
+    """potrf_base.cu: the blocked 128 x 128 leaf (16-column panels) against the oracle: factor, inverted tiles (through
+    solve / K^-1), log-determinant."""
     import gpb200
     X, y, _ = make_data(1000, 3, 41)
     k = gpb200.Mat52Iso(0.0, 0.2) + gpb200.SEIso(0.4, -0.1)
     theta, _ = _setup(engine, k, X, nb=0, gemm=0)
     o = orc.fit(k.spec(), X, y, -1.2)
-    out = {}
-    for leaf in (0, 1):
-        engine.set_option("leaf", leaf)
-        engine.factorize(theta, -1.2)
-        U = engine.factor_upper()
-        alpha, mll = engine.mll(y)
-        engine.grad_prepare()
-        out[leaf] = (U, alpha, mll, engine.logdet(), engine.inverse())
-    engine.set_option("leaf", 1)
+    engine.factorize(theta, -1.2)
+    U = engine.factor_upper()
+    alpha, mll = engine.mll(y)
+    engine.grad_prepare()
+    ld, Kinv = engine.logdet(), engine.inverse()
     Ky = orc.gram(k.spec(), X, -1.2)
-    for leaf in (0, 1):
-        U, alpha, mll, ld, Kinv = out[leaf]
-        assert np.max(np.abs(U.T @ U - Ky)) <= 1e-12 * np.max(np.abs(Ky))
-        assert abs(mll - o["mll"]) <= RTOL * abs(o["mll"]) and _rel(alpha, o["alpha"]) < RTOL
-        assert abs(ld - np.linalg.slogdet(Ky)[1]) <= 1e-11 * abs(ld)
-        assert np.max(np.abs(Kinv @ Ky - np.eye(1000))) <= 1e-9
-    assert _rel(out[1][0], out[0][0]) < 1e-12
+    assert np.max(np.abs(U.T @ U - Ky)) <= 1e-12 * np.max(np.abs(Ky))
+    assert abs(mll - o["mll"]) <= RTOL * abs(o["mll"]) and _rel(alpha, o["alpha"]) < RTOL
+    assert abs(ld - np.linalg.slogdet(Ky)[1]) <= 1e-11 * abs(ld)
+    assert np.max(np.abs(Kinv @ Ky - np.eye(1000))) <= 1e-9
 
 
 def test_triangular_solve_variants_agree(engine):
-    """alpha = K_y^-1 r (src/GPE.jl:208) through the three schedules of the blocked solves: one launch per block step,
-    the round-1 single-launch kernels, and the resident-tile single-launch kernels (diagonal tile in registers, neighbour
-    tile in shared memory) -- same arithmetic order, so the results agree to the last bits; all match the oracle."""
+    """alpha = K_y^-1 r (src/GPE.jl:208) through the two schedules of the blocked solves: one launch per block step and
+    the single-launch kernels (diagonal tile in registers, neighbour tile in shared memory) -- same arithmetic order, so
+    the results agree to the last bits; both match the oracle."""
     import gpb200
     X, y, _ = make_data(3000, 3, 51)
     k = gpb200.SEIso(0.2, 0.1) + gpb200.Mat12Iso(0.5, -0.4)
@@ -453,11 +447,9 @@ def test_triangular_solve_variants_agree(engine):
     engine.factorize(theta, -0.9)
     o = orc.fit(k.spec(), X, y, -0.9)
     res = {}
-    for v in (0, 1, 2):
+    for v in (0, 1):
         engine.set_option("trsv_fused", v)
         alpha, mll = engine.mll(y)
         res[v] = (alpha, mll, engine.solve(np.cos(X[:, 1])))
         assert _rel(alpha, o["alpha"]) < RTOL and abs(mll - o["mll"]) <= RTOL * abs(o["mll"])
-    engine.set_option("trsv_fused", 2)
-    for v in (0, 1):
-        assert _rel(res[v][0], res[2][0]) < 1e-13 and _rel(res[v][2], res[2][2]) < 1e-13
+    assert _rel(res[0][0], res[1][0]) < 1e-13 and _rel(res[0][2], res[1][2]) < 1e-13
