@@ -242,7 +242,7 @@ bool g_gemm_attr = false;
 
 }  // namespace
 
-cudaError_t fsa_gemm_launch(const FsaGemmItem* items, int n, cudaStream_t st) {
+cudaError_t fsa_gemm_launch(const FsaGemmItem* items, int n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     if (!g_gemm_attr) {
         cudaError_t e = cudaFuncSetAttribute(fsa_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_G);
@@ -250,82 +250,95 @@ cudaError_t fsa_gemm_launch(const FsaGemmItem* items, int n, cudaStream_t st) {
         g_gemm_attr = true;
     }
     fsa_gemm_kernel<<<n, GEMM_THREADS, SMEM_G, st>>>(items);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t fsa_gram_launch(const KProg& P, const double* xb, int d, const FsaGramItem* items, int n, const double* mask,
-                            double diag_add, cudaStream_t st) {
+                            double diag_add, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_gram_kernel<<<n, 256, 0, st>>>(P, xb, d, items, mask, diag_add);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t fsa_bdmv_launch(int mode, const double* packed, const int* rblk, const long long* bstart, const int* bsize,
-                            const long long* boff, const double* v, double* y, long long Np, cudaStream_t st) {
+                            const long long* boff, const double* v, double* y, long long Np, cudaStream_t st, int64_t* launches) {
     if (Np <= 0) return cudaSuccess;
     fsa_bdmv_kernel<<<(unsigned)((Np + 7) / 8), 256, 0, st>>>(mode, packed, rblk, bstart, bsize, boff, v, y, Np);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t fsa_mask_launch(double* A, long long ld, long long nrows, long long ncols, const double* rowmask,
-                            const double* colmask, cudaStream_t st) {
+                            const double* colmask, cudaStream_t st, int64_t* launches) {
     if (nrows <= 0 || ncols <= 0) return cudaSuccess;
     const unsigned gx = (unsigned)std::min<long long>((ncols + 255) / 256, 64);
     fsa_mask_kernel<<<dim3(gx, (unsigned)nrows), 256, 0, st>>>(A, ld, nrows, ncols, rowmask, colmask);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t fsa_permute_launch(int scatter, const double* src, const long long* pos, long long n, double* dst, cudaStream_t st) {
+cudaError_t fsa_permute_launch(int scatter, const double* src, const long long* pos, long long n, double* dst, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_permute_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(scatter, src, pos, n, dst);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t fsa_resid_launch(double* out, const double* a, const double* b, const double* mask, long long n, cudaStream_t st) {
+cudaError_t fsa_resid_launch(double* out, const double* a, const double* b, const double* mask, long long n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_resid_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out, a, b, mask, n);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t fsa_outer_launch(const FsaGramItem* items, int n, const double* a, cudaStream_t st) {
+cudaError_t fsa_outer_launch(const FsaGramItem* items, int n, const double* a, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_outer_kernel<<<n, 256, 0, st>>>(items, a);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t fsa_trace_launch(const KProg& P, const double* xb, int d, const FsaGramItem* items, int n, const double* mask,
-                             double* part, double* out, cudaStream_t st) {
+                             double* part, double* out, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaMemsetAsync(out, 0, sizeof(double) * P.n_theta, st);
     fsa_trace_kernel<<<n, 256, 0, st>>>(P, xb, d, items, mask, part);
+    if (launches) ++*launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     fsa_trace_reduce_kernel<<<P.n_theta, 256, 0, st>>>(part, n, P.n_theta, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t fsa_axpy_t_launch(double* C, long long ldc, const double* A, long long lda, long long nrows, long long ncols,
-                              double alpha, cudaStream_t st) {
+                              double alpha, cudaStream_t st, int64_t* launches) {
     if (nrows <= 0 || ncols <= 0) return cudaSuccess;
     dim3 grid((unsigned)((ncols + 31) / 32), (unsigned)((nrows + 31) / 32));
     fsa_axpy_t_kernel<<<grid, dim3(32, 8), 0, st>>>(C, ldc, A, lda, nrows, ncols, alpha);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t fsa_crossgram_launch(const KProg& P, const double* xs, const double* xb, int d, const FsaGramItem* items, int n,
-                                 const double* mask, cudaStream_t st) {
+                                 const double* mask, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_crossgram_kernel<<<n, 256, 0, st>>>(P, xs, xb, d, items, mask);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t fsa_rowdot_launch(const FsaRowItem* items, int n, cudaStream_t st) {
+cudaError_t fsa_rowdot_launch(const FsaRowItem* items, int n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_rowdot_kernel<<<n, 256, 0, st>>>(items);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t fsa_var_launch(double* out, const double* q, const double* g2, const double* r2neg, long long n, cudaStream_t st) {
+cudaError_t fsa_var_launch(double* out, const double* q, const double* g2, const double* r2neg, long long n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_var_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out, q, g2, r2neg, n);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

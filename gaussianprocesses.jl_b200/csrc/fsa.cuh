@@ -19,7 +19,7 @@ struct FsaGemmItem {
     int lower;
     double alpha, beta;
 };
-cudaError_t fsa_gemm_launch(const FsaGemmItem* items, int n, cudaStream_t st);
+cudaError_t fsa_gemm_launch(const FsaGemmItem* items, int n, cudaStream_t st, int64_t* launches);
 
 // One tile of a block's Gram matrix: dst[i][j] = k(x_{row_i+i}, x_{row_j+j}) over padded rows, + diag_add on the real
 // diagonal, identity on padding rows (mask 0); diag != 0: only i >= j is written.
@@ -31,7 +31,7 @@ struct FsaGramItem {
     int pad_;
 };
 cudaError_t fsa_gram_launch(const KProg& P, const double* xb, int d, const FsaGramItem* items, int n, const double* mask,
-                            double diag_add, cudaStream_t st);
+                            double diag_add, cudaStream_t st, int64_t* launches);
 
 // Block-diagonal row products over the Np padded rows (row r lies in block rblk[r], which starts at padded row bstart[b],
 // has B_b = bsize[b] rows and its packed matrix at offset boff[b]); r_l = r - bstart:
@@ -40,28 +40,28 @@ cudaError_t fsa_gram_launch(const KProg& P, const double* xb, int d, const FsaGr
 //   mode 2: y[r] = sum_{k <= r_l} M[r_l][k]^2                  (squared row norms of the lower triangle)
 // one warp per row, fixed summation order.
 cudaError_t fsa_bdmv_launch(int mode, const double* packed, const int* rblk, const long long* bstart, const int* bsize,
-                            const long long* boff, const double* v, double* y, long long Np, cudaStream_t st);
+                            const long long* boff, const double* v, double* y, long long Np, cudaStream_t st, int64_t* launches);
 // A[i][j] = 0 where rowmask[i] == 0 (rowmask may be NULL) or colmask[j] == 0 (colmask may be NULL), i < nrows, j < ncols
 cudaError_t fsa_mask_launch(double* A, long long ld, long long nrows, long long ncols, const double* rowmask,
-                            const double* colmask, cudaStream_t st);
+                            const double* colmask, cudaStream_t st, int64_t* launches);
 // dst[pos[i]] = src[i] (scatter 1) or dst[i] = src[pos[i]] (scatter 0), i < n
-cudaError_t fsa_permute_launch(int scatter, const double* src, const long long* pos, long long n, double* dst, cudaStream_t st);
+cudaError_t fsa_permute_launch(int scatter, const double* src, const long long* pos, long long n, double* dst, cudaStream_t st, int64_t* launches);
 // out[i] = mask[i] * (a[i] - b[i])
-cudaError_t fsa_resid_launch(double* out, const double* a, const double* b, const double* mask, long long n, cudaStream_t st);
+cudaError_t fsa_resid_launch(double* out, const double* a, const double* b, const double* mask, long long n, cudaStream_t st, int64_t* launches);
 // dst[i][j] += a[row_i + i] * a[row_j + j] on every item tile (the alpha_i alpha_i' part of the FSA gradient weights)
-cudaError_t fsa_outer_launch(const FsaGramItem* items, int n, const double* a, cudaStream_t st);
+cudaError_t fsa_outer_launch(const FsaGramItem* items, int n, const double* a, cudaStream_t st, int64_t* launches);
 // Block-diagonal weighted gradient trace: out[p] = sum over the item tiles of sum_ij dst[i][j] dk(x_{row_i+i}, x_{row_j+j})/dθ_p
 // over real rows (mask != 0), for all P = P.n_theta parameters in one pass; the kernel derivatives are recomputed from x.
 // part: n * n_theta scratch; per-tile partials are summed in a fixed order (two runs agree bit for bit).
 cudaError_t fsa_trace_launch(const KProg& P, const double* xb, int d, const FsaGramItem* items, int n, const double* mask,
-                             double* part, double* out, cudaStream_t st);
+                             double* part, double* out, cudaStream_t st, int64_t* launches);
 // C[i][j] += alpha * A[j][i], i < nrows, j < ncols
 cudaError_t fsa_axpy_t_launch(double* C, long long ldc, const double* A, long long lda, long long nrows, long long ncols,
-                              double alpha, cudaStream_t st);
+                              double alpha, cudaStream_t st, int64_t* launches);
 // Prediction pieces.  One tile of a test-block x training-block cross-Gram: dst[i][j] = k(xs_{row_i+i}, xb_{row_j+j}) with
 // xs / xb the staged test / padded training inputs, 0 on training padding rows (mask 0).
 cudaError_t fsa_crossgram_launch(const KProg& P, const double* xs, const double* xb, int d, const FsaGramItem* items, int n,
-                                 const double* mask, cudaStream_t st);
+                                 const double* mask, cudaStream_t st, int64_t* launches);
 // Row products of 128-row tiles: out[i] = sum_{k < K} A[i][k] v[k] (sq = 0) or sum_{k < K} A[i][k]^2 (sq = 1), i < 128
 struct FsaRowItem {
     const double* A;
@@ -71,6 +71,6 @@ struct FsaRowItem {
     int K;
     int sq;
 };
-cudaError_t fsa_rowdot_launch(const FsaRowItem* items, int n, cudaStream_t st);
+cudaError_t fsa_rowdot_launch(const FsaRowItem* items, int n, cudaStream_t st, int64_t* launches);
 // out[i] = q[i] - g2[i] - r2neg[i]: k** - |V*|^2 - |G|^2 + |R|^2 from q = k** - |V*|^2 and r2neg = -|R|^2
-cudaError_t fsa_var_launch(double* out, const double* q, const double* g2, const double* r2neg, long long n, cudaStream_t st);
+cudaError_t fsa_var_launch(double* out, const double* q, const double* g2, const double* r2neg, long long n, cudaStream_t st, int64_t* launches);

@@ -436,7 +436,7 @@ bool gemm_make_tensor_map_plain(CUtensorMap* out, const double* base, int64_t ro
     return r == CUDA_SUCCESS;
 }
 
-cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream) {
+cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream, int64_t* launches) {
     GemmKP p;
     p.A = d.A.buf.base; p.Asub = d.A.sub.base; p.B = d.B.buf.base; p.Bsub = d.B.sub.base;
     p.lda = d.A.buf.ld; p.ldb = d.B.buf.ld;
@@ -486,5 +486,6 @@ cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream) {
     } else {
         gpb200_dgemm_nt_simple<<<grid, SIMPLE_THREADS, SMEM_SIMPLE, stream>>>(p);
     }
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

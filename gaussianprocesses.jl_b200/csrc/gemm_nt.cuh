@@ -57,7 +57,7 @@ static inline GemmDesc gemm_desc_default() {
 }
 
 // impl: 0 = TMA + mbarrier warp-specialised kernel, 1 = simple synchronous kernel.
-cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream);
+cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream, int64_t* launches);
 // one-time per process (sets max dynamic smem)
 cudaError_t gemm_nt_init();
 // Build a TMA descriptor for a row-major [rows x cols] FP64 buffer, box 16 x 128, swizzle 128B.

@@ -340,17 +340,16 @@ double gemm_exec_flops(const GemmDesc& d) {
 }
 
 cudaError_t launch_gemm(gpb200_handle* h, const GemmDesc& d) {
-    ++h->launches;
     const int impl = h->tma_ok ? h->gemm_impl : 1;
     cudaStream_t stc = h->st_cur ? h->st_cur : h->st;
-    if (!h->profile || stc != h->st) return gemm_nt_launch(d, impl, stc);
+    if (!h->profile || stc != h->st) return gemm_nt_launch(d, impl, stc, &h->launches);
     if (h->pev_used + 2 > h->pev.size()) {
         const size_t old = h->pev.size();
         h->pev.resize(old + 512);
         for (size_t i = old; i < h->pev.size(); ++i) cudaEventCreate(&h->pev[i]);
     }
     cudaEventRecord(h->pev[h->pev_used++], h->st);
-    cudaError_t e = gemm_nt_launch(d, impl, h->st);
+    cudaError_t e = gemm_nt_launch(d, impl, h->st, &h->launches);
     cudaEventRecord(h->pev[h->pev_used++], h->st);
     h->gemm_flops_exec += gemm_exec_flops(d);
     ++h->gemm_launches;
@@ -436,13 +435,12 @@ cudaError_t merge_inverse(gpb200_handle* h, int p, int n1, int n2, int batch) {
 // block size, so ~98% of the flops run with K >= 1024 (near-peak DMMA activity); only the
 // 128-wide leaves (tile factorisation + TRSM through the inverted tile) are latency bound.
 cudaError_t leaf_launch(gpb200_handle* h, int p, cudaStream_t st) {
-    ++h->launches;
     PotrfPeers pp{};
     if (h->push_panel) {
         pp.n = h->n_peer;
         for (int q = 0; q < h->n_peer; ++q) { pp.F[q] = h->peer_F[q]; pp.Dinv[q] = h->peer_Dinv[q]; pp.DinvT[q] = h->peer_DinvT[q]; pp.logd[q] = h->peer_logd[q]; }
     }
-    return potrf128_launch(h->G, h->ld, h->F, h->ld, h->Dinv, h->DinvT, h->logd, h->info_dev, p, 1, TILE, st, &pp);
+    return potrf128_launch(h->G, h->ld, h->F, h->ld, h->Dinv, h->DinvT, h->logd, h->info_dev, p, 1, TILE, st, &h->launches, &pp);
 }
 
 // `leaf_done`: the tile at p was already factored by the look-ahead chain on the side stream (join it first).
@@ -733,16 +731,16 @@ int cholesky_dist_p2p(gpb200_handle* h) {
         cudaError_t e = chol_panel(h, bp(b), bn(b), NB);
         h->push_panel = false;
         CK(e);
-        ++h->launches;
         signal_peers_kernel<<<1, 32, 0, h->st>>>(h->peer_sig_dev, h->n_peer, base + b + 1);
+        ++h->launches;
         CK(cudaGetLastError());
         return GPB200_OK;
     };
     if (owner(0) == me) { int rc = factor_and_publish(0); if (rc) return rc; }
     for (int b = 0; b < nblk; ++b) {
         if (owner(b) != me) {
-            ++h->launches;
             wait_signal_kernel<<<1, 1, 0, h->st>>>(h->sig + owner(b), base + b + 1, h->sig + 8);
+            ++h->launches;
             CK(cudaGetLastError());
         }
         bool did_next = false;
@@ -807,8 +805,8 @@ int inverse_dist(gpb200_handle* h) {
         if ((size_t)per_rank > h->ag_send_elems || (size_t)per_rank * R > h->ag_recv_elems)
             return fail(h, GPB200_ECUDA, "inverse_dist: exchange buffers too small");
         dim3 blk(32, 32), grd((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)batch);
-        h->launches += 2;
         pack_slices_kernel<<<grd, blk, 0, h->st>>>(h->G, h->ld, h->ag_send, (int)s, wr, R, me, Np);
+        ++h->launches;
         CK(cudaGetLastError());
         CK(cudaEventRecord(h->ev_x, h->st));
         CK(cudaStreamWaitEvent(h->st_comm, h->ev_x, 0));
@@ -817,6 +815,7 @@ int inverse_dist(gpb200_handle* h) {
         CK(cudaStreamWaitEvent(h->st, h->ev_y, 0));
         dim3 grd2((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)(batch * R));
         unpack_slices_kernel<<<grd2, blk, 0, h->st>>>(h->G, h->ld, h->ag_recv, per_rank, (int)s, wr, Np, R, me);
+        ++h->launches;
         CK(cudaGetLastError());
     }
     // W'W on this rank's tile rows only (K^-1 stays distributed; the trace needs no more)
@@ -962,17 +961,17 @@ bool use_seiso_fast(gpb200_handle* h, SeIsoFast* sf) {
 cudaError_t launch_gram(gpb200_handle* h, double* G, int64_t ldg, int own_tiles, int nranks, int rank, int own_axis) {
     SeIsoFast sf;
     if (use_seiso_fast(h, &sf))
-        return gram_seiso_tma_launch(&h->mapX, &h->mapXT, h->dxp, sf, h->N, h->Npad, h->noise_var, h->n_noise, h->nugget, G, ldg, h->st,
+        return gram_seiso_tma_launch(&h->mapX, &h->mapXT, h->dxp, sf, h->N, h->Npad, h->noise_var, h->n_noise, h->nugget, G, ldg, h->st, &h->launches,
                                      own_tiles, nranks, rank, own_axis);
-    return gram_lower_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, h->noise_var, h->n_noise, h->nugget, G, ldg, h->st,
+    return gram_lower_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, h->noise_var, h->n_noise, h->nugget, G, ldg, h->st, &h->launches,
                              own_tiles, nranks, rank, own_axis);
 }
 cudaError_t launch_trace(gpb200_handle* h, int bm_mod, int bm_rem, int bm_div) {
     SeIsoFast sf;
     if (use_seiso_fast(h, &sf))
-        return trace_seiso_tma_launch(&h->mapX, &h->mapXT, h->dxp, sf, h->N, h->Npad, h->alpha, h->G, h->ld, h->part, h->trace_out, h->st,
+        return trace_seiso_tma_launch(&h->mapX, &h->mapXT, h->dxp, sf, h->N, h->Npad, h->alpha, h->G, h->ld, h->part, h->trace_out, h->st, &h->launches,
                                       bm_mod, bm_rem, bm_div);
-    return trace_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, h->alpha, h->G, h->ld, h->part, h->trace_out, h->st,
+    return trace_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, h->alpha, h->G, h->ld, h->part, h->trace_out, h->st, &h->launches,
                         bm_mod, bm_rem, bm_div);
 }
 
@@ -1200,8 +1199,7 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
         CK(cudaMemcpy2DAsync(h->xp, sizeof(double) * h->dxp, x, sizeof(double) * ldx, sizeof(double) * d, N,
                              cudaMemcpyHostToDevice, h->st));
         if (!h->xpt) CK(cudaMalloc(&h->xpt, sizeof(double) * Npad * h->dxp));
-        ++h->launches;
-        CK(shard_transpose(h->xpt, Npad, h->xp, h->dxp, Npad, h->dxp, h->st));
+        CK(shard_transpose(h->xpt, Npad, h->xp, h->dxp, Npad, h->dxp, h->st, &h->launches));
         h->xmap_ok = gemm_make_tensor_map_plain(&h->mapX, h->xp, N, h->dxp, h->dxp, TILE, h->dxp) &&
                      gemm_make_tensor_map_plain(&h->mapXT, h->xpt, h->dxp, N, Npad, h->dxp, TILE);
     }
@@ -1300,10 +1298,7 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
     if (h->sharded) {
         // row-sharded storage: own rows of the Gram matrix, then the all-gathered-panel Cholesky (shard_impl.cuh)
         CK(cudaEventRecord(h->ev0, h->st));
-        for (auto* q : L) {
-            ++q->launches;
-            SCK(q, launch_gram(q, q->G, q->ld, q->rb, q->nranks, q->rank, 1));
-        }
+        for (auto* q : L) SCK(q, launch_gram(q, q->G, q->ld, q->rb, q->nranks, q->rank, 1));
         CK(cudaEventRecord(h->ev1, h->st));
         { int rc = shard_cholesky_la(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
         CK(cudaEventRecord(h->ev2, h->st));
@@ -1324,7 +1319,6 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
     }
 
     CK(cudaEventRecord(h->ev0, h->st));
-    ++h->launches;
     if (h->nranks > 1) {
         int rc = dist_alloc(h);
         if (rc) return rc;
@@ -1364,8 +1358,7 @@ int gpb200_logdet(gpb200_handle* h, double* logdet) {
     if (!h || !logdet) return GPB200_EINVAL;
     if (!h->factored) return fail(h, GPB200_ESTATE, "logdet: factorize first");
     CK(cudaSetDevice(h->device));
-    ++h->launches;
-    CK(sum_launch(h->logd, h->Npad, h->scal, h->st));
+    CK(sum_launch(h->logd, h->Npad, h->scal, h->st, &h->launches));
     CK(cudaMemcpyAsync(logdet, h->scal, sizeof(double), cudaMemcpyDeviceToHost, h->st));
     CK(cudaStreamSynchronize(h->st));
     return GPB200_OK;
@@ -1409,9 +1402,8 @@ int gpb200_mll(gpb200_handle* h, const double* y_minus_mean, double* alpha, doub
         CK(cudaMemcpyAsync(h->r1, h->r0, sizeof(double) * h->Npad, cudaMemcpyDeviceToDevice, h->st));
         CK(solve_device(h, h->r1, h->y1, h->alpha));
     }
-    h->launches += 2;
-    CK(dot_launch(h->r0, h->alpha, h->Npad, h->scal + 0, h->st));
-    CK(sum_launch(h->logd, h->Npad, h->scal + 1, h->st));
+    CK(dot_launch(h->r0, h->alpha, h->Npad, h->scal + 0, h->st, &h->launches));
+    CK(sum_launch(h->logd, h->Npad, h->scal + 1, h->st, &h->launches));
     double s[2];
     CK(cudaMemcpyAsync(s, h->scal, sizeof(double) * 2, cudaMemcpyDeviceToHost, h->st));
     if (alpha) CK(cudaMemcpyAsync(alpha, h->alpha, sizeof(double) * h->N, cudaMemcpyDeviceToHost, h->st));
@@ -1469,15 +1461,11 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     CK(cudaEventRecord(h->ev0, h->st));
     if (h->sharded) {
         // fused trace over the own rows of K^-1 (block-cyclic tile rows), P+1 partial sums summed over the ranks
-        for (auto* q : Lg) {
-            q->launches += 2;
-            SCK(q, launch_trace(q, q->nranks, q->rank, q->rb));
-        }
+        for (auto* q : Lg) SCK(q, launch_trace(q, q->nranks, q->rank, q->rb));
         int rc = coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out; }, (size_t)trace_num_acc(h->prog));
         if (rc) { if (Lg[0] != h) h->err = Lg[0]->err; return rc; }
     } else {
-    h->launches += 2;
-    CK(launch_trace(h, h->nranks, h->rank, 1));
+        CK(launch_trace(h, h->nranks, h->rank, 1));
     }
     if (!h->sharded && h->nranks > 1) {                    // P+1 partial sums, summed over ranks
         CK(cudaEventRecord(h->ev_x, h->st));
@@ -1536,16 +1524,13 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
             if (rc) { if (q != h) h->err = q->err; return rc; }
             SCK(q, cudaMemcpy2DAsync(q->xs, sizeof(double) * q->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * q->d, Mc,
                                      cudaMemcpyHostToDevice, q->st));
-            ++q->launches;
-            SCK(q, crossgram_launch(q->prog, q->xs, q->d, Mc, Mpad, q->x, q->d, q->N, q->Npad, q->d, q->Kst, q->Npad, q->st));
+            SCK(q, crossgram_launch(q->prog, q->xs, q->d, Mc, Mpad, q->x, q->d, q->N, q->Npad, q->d, q->Kst, q->Npad, q->st, &q->launches));
             if (need_v) {
-                ++q->launches;
-                SCK(q, kdiag_launch(q->prog, q->xs, q->d, Mc, q->pvar, q->st));           // running variance starts at k**
-                if (cov) { ++q->launches; SCK(q, gram_full_launch(q->prog, q->xs, q->d, Mc, Mpad, q->d, q->Kss, Mpad, q->st)); }
+                SCK(q, kdiag_launch(q->prog, q->xs, q->d, Mc, q->pvar, q->st, &q->launches));           // running variance starts at k**
+                if (cov) SCK(q, gram_full_launch(q->prog, q->xs, q->d, Mc, Mpad, q->d, q->Kss, Mpad, q->st, &q->launches));
             }
         }
-        ++h->launches;
-        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st));          // GP.jl:26
+        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));          // GP.jl:26
         CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
         if (need_v) {
             int rc = shard_predict_solve(Lp, (int)Mpad, Mc, var != nullptr, cov != nullptr);
@@ -1563,21 +1548,18 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
         if (rc) return rc;
         CK(cudaMemcpy2DAsync(h->xs, sizeof(double) * h->d, xs + m0 * ldxs, sizeof(double) * ldxs,
                              sizeof(double) * h->d, Mc, cudaMemcpyHostToDevice, h->st));
-        h->launches += 2;
-        CK(crossgram_launch(h->prog, h->xs, h->d, Mc, Mpad, h->x, h->d, h->N, h->Npad, h->d, h->Kst, h->Npad, h->st));
-        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st));          // GP.jl:26
+        CK(crossgram_launch(h->prog, h->xs, h->d, Mc, Mpad, h->x, h->d, h->N, h->Npad, h->d, h->Kst, h->Npad, h->st, &h->launches));
+        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));          // GP.jl:26
         CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
         if (need_v) {
             CK(trsm_rec(h, (int)Mpad, 0, (int)h->Npad));                                   // whiten!, GP.jl:27
             if (var) {
-                h->launches += 2;
-                CK(kdiag_launch(h->prog, h->xs, h->d, Mc, h->pkdiag, h->st));
-                CK(rowvar_launch(h->Kst, h->Npad, h->pkdiag, Mc, h->Npad, h->pvar, h->st));
+                CK(kdiag_launch(h->prog, h->xs, h->d, Mc, h->pkdiag, h->st, &h->launches));
+                CK(rowvar_launch(h->Kst, h->Npad, h->pkdiag, Mc, h->Npad, h->pvar, h->st, &h->launches));
                 CK(cudaMemcpyAsync(var + m0, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
             }
             if (cov) {                                                                      // GP.jl:51-54
-                ++h->launches;
-                CK(gram_full_launch(h->prog, h->xs, h->d, Mc, Mpad, h->d, h->Kss, Mpad, h->st));
+                CK(gram_full_launch(h->prog, h->xs, h->d, Mc, Mpad, h->d, h->Kss, Mpad, h->st, &h->launches));
                 GemmBuf bk{h->tma_ok ? &h->mapKst : nullptr, h->Kst, h->Npad};
                 GemmDesc g = gemm_desc_default();
                 g.A = GemmOperand{bk, bufNone(), 0, 0};
@@ -1623,14 +1605,15 @@ int gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, con
     }
     gpb200_handle* sb = h->sub;
     sb->st = h->st;
+    const int64_t sub_launches = sb->launches;
     if (!sb->has_data || sb->N != M) {
         std::vector<double> dummy((size_t)M, 0.0);
         rc = gpb200_set_data(sb, M, 1, dummy.data(), 1);
         if (rc) { h->err = "rand: " + sb->err; return rc; }
     }
-    ++h->launches;
-    CK(spd_from_cov_launch(sb->G, sb->ld, h->Kss, Mpad, M, Mpad, nugget, h->st));
+    CK(spd_from_cov_launch(sb->G, sb->ld, h->Kss, Mpad, M, Mpad, nugget, h->st, &h->launches));
     rc = chol_inplace(sb);
+    h->launches += sb->launches - sub_launches;                 // the sub-engine's kernels run for this call
     if (rc) { h->err = "rand: predictive covariance + nugget is not positive definite: " + sb->err; return rc; }
     // draws: Zt (nsamp x M, zero padded) on the device
     if (Spad > h->rz_rows || Mpad > h->rz_cols) {
@@ -1653,8 +1636,7 @@ int gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, con
         g.flags = GEMM_KHI_N;
         CK(launch_gemm(h, g));
     }
-    ++h->launches;
-    CK(add_rowvec_launch(h->rout, ldz, h->pmu, nsamp, M, h->st));                          // + mu (K*' alpha part)
+    CK(add_rowvec_launch(h->rout, ldz, h->pmu, nsamp, M, h->st, &h->launches));                          // + mu (K*' alpha part)
     CK(cudaMemcpy2DAsync(samples, sizeof(double) * M, h->rout, sizeof(double) * ldz, sizeof(double) * M, nsamp, cudaMemcpyDeviceToHost, h->st));
     CK(cudaStreamSynchronize(h->st));
     return GPB200_OK;
@@ -1682,8 +1664,7 @@ int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) 
     h->xmap_ok = false;
     if (h->xp) {
         CK(cudaMemcpy2DAsync(h->xp + Nold * h->dxp, sizeof(double) * h->dxp, xnew, sizeof(double) * ldx, sizeof(double) * d, k, cudaMemcpyHostToDevice, h->st));
-        ++h->launches;
-        CK(shard_transpose(h->xpt, Np, h->xp, h->dxp, Np, h->dxp, h->st));
+        CK(shard_transpose(h->xpt, Np, h->xp, h->dxp, Np, h->dxp, h->st, &h->launches));
         h->xmap_ok = gemm_make_tensor_map_plain(&h->mapX, h->xp, Nnew, h->dxp, h->dxp, TILE, h->dxp) &&
                      gemm_make_tensor_map_plain(&h->mapXT, h->xpt, h->dxp, Nnew, Np, h->dxp, TILE);
     }
@@ -1691,9 +1672,8 @@ int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) 
     h->inv_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
     const int init = INT_MAX;
     CK(cudaMemcpyAsync(h->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, h->st));
-    ++h->launches;
     // Gram rows >= c0 (columns <= row), identity beyond the new N
-    CK(gram_lower_launch(h->prog, h->x, d, d, Nnew, Np, h->noise_var, 1, h->nugget, h->G, h->ld, h->st, 0, 1, 0, 0, c0 / TILE));
+    CK(gram_lower_launch(h->prog, h->x, d, d, Nnew, Np, h->noise_var, 1, h->nugget, h->G, h->ld, h->st, &h->launches, 0, 1, 0, 0, c0 / TILE));
     cudaError_t e = cudaSuccess;
     if (c0 > 0) {
         // rows >= c0 of G against the existing factor: G[r, 0:c0] <- G[r, 0:c0] L11^-T, then keep them as rows of L
@@ -1755,8 +1735,7 @@ static int cv_prepare(gpb200_handle* h) {
             return fail(h, GPB200_ECUDA, "cv: cuTensorMapEncodeTiled failed");
     }
     if (!h->g_sym) {
-        ++h->launches;
-        CK(symmetrize_launch(h->G, h->ld, h->Npad, h->st));      // lower K^-1 -> full symmetric (the W' scratch above it is dead)
+        CK(symmetrize_launch(h->G, h->ld, h->Npad, h->st, &h->launches));      // lower K^-1 -> full symmetric (the W' scratch above it is dead)
         h->g_sym = true;
     }
     return GPB200_OK;
@@ -1774,8 +1753,7 @@ int gpb200_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double
     GemmBuf bD{h->tma_ok ? &h->mapCvD : nullptr, h->cvD, h->Npad}, bY{h->tma_ok ? &h->mapCvY : nullptr, h->cvY, h->Npad};
     const double* Yt = h->cvY;
     if (param >= 0) {
-        ++h->launches;
-        CK(gram_grad_full_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, param, h->cvD, h->Npad, h->st));
+        CK(gram_grad_full_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, param, h->cvD, h->Npad, h->st, &h->launches));
         GemmDesc g = gemm_desc_default();                           // Y' = K^-1 D   (both symmetric: NT form)
         g.A = GemmOperand{bufG(h), bufNone(), 0, 0};
         g.B = GemmOperand{bD, bufNone(), 0, 0};
@@ -1784,9 +1762,8 @@ int gpb200_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double
     } else {
         Yt = h->G;                                                  // noise: Z = K^-1 (crossvalidation.jl:124-126)
     }
-    h->launches += 2;
-    CK(rowdot_launch(Yt, h->Npad, h->alpha, h->N, h->Npad, h->r1, h->st));              // Z_j alpha
-    CK(rowdot2_launch(h->G, Yt, h->Npad, h->N, h->Npad, h->y1, h->st));                 // diag(Z_j K^-1) = rowwise <K^-1_i, Y'_i>
+    CK(rowdot_launch(Yt, h->Npad, h->alpha, h->N, h->Npad, h->r1, h->st, &h->launches));              // Z_j alpha
+    CK(rowdot2_launch(h->G, Yt, h->Npad, h->N, h->Npad, h->y1, h->st, &h->launches));                 // diag(Z_j K^-1) = rowwise <K^-1_i, Y'_i>
     {   // M_j = Y' K^-1  -> cvD (fold sub-blocks)
         GemmDesc g = gemm_desc_default();
         g.A = GemmOperand{param >= 0 ? bY : bufG(h), bufNone(), 0, 0};
@@ -1820,8 +1797,7 @@ int gpb200_cv_block(gpb200_handle* h, int32_t which, int64_t nV, const int64_t* 
     }
     static_assert(sizeof(long long) == sizeof(int64_t), "index width");
     CK(cudaMemcpyAsync(h->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, h->st));
-    ++h->launches;
-    CK(gather_block_launch(h->cvblk, which == 0 ? h->G : h->cvD, h->Npad, h->cvidx, nV, h->st));
+    CK(gather_block_launch(h->cvblk, which == 0 ? h->G : h->cvD, h->Npad, h->cvidx, nV, h->st, &h->launches));
     CK(cudaMemcpyAsync(out, h->cvblk, sizeof(double) * nV * nV, cudaMemcpyDeviceToHost, h->st));
     CK(cudaStreamSynchronize(h->st));
     return GPB200_OK;
@@ -1908,7 +1884,7 @@ int gpb200_dgemm_nt_device(gpb200_handle* h, int impl, int64_t M, int64_t N, int
     g.alpha = alpha; g.beta = beta;
     g.flags = lower_only ? GEMM_LOWER_ONLY : 0;
     CK(cudaEventRecord(h->ev0, h->st));
-    for (int r = 0; r < reps; ++r) { ++h->launches; CK(gemm_nt_launch(g, impl, h->st)); }
+    for (int r = 0; r < reps; ++r) CK(gemm_nt_launch(g, impl, h->st, &h->launches));
     CK(cudaEventRecord(h->ev1, h->st));
     CK(cudaStreamSynchronize(h->st));
     if (ms) *ms = ev_ms(h->ev0, h->ev1);
@@ -1919,7 +1895,7 @@ int gpb200_fp64_peak(gpb200_handle* h, double* tflops_dmma, double* tflops_dfma)
     if (!h) return GPB200_EINVAL;
     CK(cudaSetDevice(h->device));
     double t[2] = {0, 0};
-    CK(fp64_peak_measure(h->st, t));
+    CK(fp64_peak_measure(h->st, &h->launches, t));
     if (tflops_dmma) *tflops_dmma = t[0];
     if (tflops_dfma) *tflops_dfma = t[1];
     return GPB200_OK;
@@ -2189,13 +2165,11 @@ int gpb200_fitc_set_kernel(gpb200_fitc* f, int32_t n_ops, const int32_t* ops, in
 
 // K_fu chunk (rows r0..r0+nc of x against the inducing points) into bufA [Nc x Mpad]
 static cudaError_t fitc_kfu(gpb200_fitc* f, const double* xrows, int64_t nc) {
-    ++f->eu->launches;
-    return crossgram_launch(f->eu->prog, xrows, f->d, nc, f->Nc, f->eu->x, f->d, f->M, f->Mpad, f->d, f->bufA, f->Mpad, f->eu->st);
+    return crossgram_launch(f->eu->prog, xrows, f->d, nc, f->Nc, f->eu->x, f->d, f->M, f->Mpad, f->d, f->bufA, f->Mpad, f->eu->st, &f->eu->launches);
 }
 // K_uf chunk into bufB [Mpad x Nc]
 static cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc) {
-    ++f->eu->launches;
-    return crossgram_launch(f->eu->prog, f->eu->x, f->d, f->M, f->Mpad, xrows, f->d, nc, f->Nc, f->d, f->bufB, f->Nc, f->eu->st);
+    return crossgram_launch(f->eu->prog, f->eu->x, f->d, f->M, f->Mpad, xrows, f->d, nc, f->Nc, f->d, f->bufB, f->Nc, f->eu->st, &f->eu->launches);
 }
 
 int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise) {
@@ -2216,8 +2190,7 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
     const double zero = 0.0;
     FCK(cudaMemcpyAsync(es->noise_var, &zero, sizeof(double), cudaMemcpyHostToDevice, st));
     es->n_noise = 1; es->nugget = 2e-10;
-    ++es->launches;
-    if (f->rank == 0) FCK(gram_lower_launch(es->prog, es->x, f->d, f->d, f->M, f->Mpad, es->noise_var, 1, 2e-10, es->G, es->ld, st));
+    if (f->rank == 0) FCK(gram_lower_launch(es->prog, es->x, f->d, f->d, f->M, f->Mpad, es->noise_var, 1, 2e-10, es->G, es->ld, st, &es->launches));
     else FCK(cudaMemsetAsync(es->G, 0, sizeof(double) * (size_t)f->Mpad * (size_t)f->Mpad, st));     // K_uu (+ nuggets, identity padding) enters the sum once
     f->noise_var = exp(2.0 * log_noise);
     if (f->mode == 3) return fsa_factorize(f);
@@ -2230,19 +2203,16 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
             // Lambda_i = sigma^2 + K_ii - |L_uu^-1 K_ui|^2   (fitc.jl:146-148)
             FCK(fitc_kfu(f, xr, nc));
             FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
-            eu->launches += 3;
-            FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->tmpc, st));
-            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, nc, f->Mpad, f->tmpc2, st));
-            FCK(ew_launch(0, nc, f->lam + r0, f->tmpc2, nullptr, nullptr, f->noise_var, st));
+            FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, nc, f->Mpad, f->tmpc2, st, &eu->launches));
+            FCK(ew_launch(0, nc, f->lam + r0, f->tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
         } else {
             // SoR / DTC: Lambda = sigma^2 I   (subsetofregressors.jl:100: exp(-2 logNoise) * Kuf * Kfu + Kuu)
-            ++eu->launches;
-            FCK(ew_launch(0, nc, f->lam + r0, f->zeroc, nullptr, nullptr, f->noise_var, st));
+            FCK(ew_launch(0, nc, f->lam + r0, f->zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
         }
         // Sigma_QR += K_uf Lambda^-1 K_fu   (fitc.jl:150), as (K_uf Lambda^-1/2)(K_uf Lambda^-1/2)'
         FCK(fitc_kuf(f, xr, nc));
-        ++eu->launches;
-        FCK(scale_launch(0, f->bufB, f->Nc, f->Mpad, nc, f->lam + r0, st));
+        FCK(scale_launch(0, f->bufB, f->Nc, f->Mpad, nc, f->lam + r0, st, &eu->launches));
         GemmDesc g = gemm_desc_default();
         g.A = GemmOperand{bB, bufNone(), 0, 0};
         g.B = GemmOperand{bB, bufNone(), 0, 0};
@@ -2272,11 +2242,10 @@ int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, d
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
         FCK(fitc_kuf(f, f->x + r0 * f->d, nc));
-        eu->launches += 3;
         FCK(cudaMemsetAsync(f->w, 0, sizeof(double) * f->Nc, st));
-        FCK(ew_launch(1, nc, f->w, f->y + r0, f->lam + r0, nullptr, 0.0, st));
-        FCK(rowdot_launch(f->bufB, f->Nc, f->w, f->M, f->Nc, f->tmpm, st));
-        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st));
+        FCK(ew_launch(1, nc, f->w, f->y + r0, f->lam + r0, nullptr, 0.0, st, &eu->launches));
+        FCK(rowdot_launch(f->bufB, f->Nc, f->w, f->M, f->Nc, f->tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
     }
     { int rca = fitc_allreduce(f, f->bvec, (size_t)f->Mpad); if (rca) return rca; }              // b summed over the ranks' rows
     // u = Sigma_QR^-1 b   (== get_alpha_u, fitc.jl:279-286)
@@ -2286,16 +2255,14 @@ int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, d
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
         FCK(fitc_kfu(f, f->x + r0 * f->d, nc));
-        eu->launches += 2;
-        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, nc, f->Mpad, f->tmpc, st));
-        FCK(ew_launch(3, nc, f->alpha + r0, f->y + r0, f->tmpc, f->lam + r0, 0.0, st));
+        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, nc, f->Mpad, f->tmpc, st, &eu->launches));
+        FCK(ew_launch(3, nc, f->alpha + r0, f->y + r0, f->tmpc, f->lam + r0, 0.0, st, &eu->launches));
     }
-    eu->launches += 5;
-    FCK(dot_launch(f->y, f->alpha, f->N, f->scal + 0, st));
-    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st));
-    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st));
-    FCK(ew_launch(4, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st));
-    FCK(sum_launch(f->tmpn, f->N, f->scal + 3, st));
+    FCK(dot_launch(f->y, f->alpha, f->N, f->scal + 0, st, &eu->launches));
+    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st, &eu->launches));
+    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st, &eu->launches));
+    FCK(ew_launch(4, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(sum_launch(f->tmpn, f->N, f->scal + 3, st, &eu->launches));
     double s[5];
     if (f->nranks > 1) {
         // r'alpha, sum log Lambda and N are sums over the ranks' rows; the two M x M log-determinants are replicated
@@ -2331,16 +2298,14 @@ int gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise) {
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
         FCK(fitc_kfu(f, f->x + r0 * f->d, nc));
-        eu->launches += 2;
-        FCK(scale_launch(1, f->bufA, f->Mpad, nc, f->Mpad, f->lam + r0, st));
+        FCK(scale_launch(1, f->bufA, f->Mpad, nc, f->Mpad, f->lam + r0, st, &eu->launches));
         FCK(trsm_rec_buf(es, bA, (int)f->Nc, 0, (int)f->Mpad));
-        FCK(rowvar_launch(f->bufA, f->Mpad, f->zeroc, nc, f->Mpad, f->tmpn + r0, st));     // = -|row|^2
+        FCK(rowvar_launch(f->bufA, f->Mpad, f->zeroc, nc, f->Mpad, f->tmpn + r0, st, &eu->launches));     // = -|row|^2
     }
-    eu->launches += 4;
-    FCK(sum_launch(f->tmpn, f->N, f->scal + 0, st));
-    FCK(dot_launch(f->alpha, f->alpha, f->N, f->scal + 1, st));
-    FCK(ew_launch(5, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st));
-    FCK(sum_launch(f->tmpn, f->N, f->scal + 2, st));
+    FCK(sum_launch(f->tmpn, f->N, f->scal + 0, st, &eu->launches));
+    FCK(dot_launch(f->alpha, f->alpha, f->N, f->scal + 1, st, &eu->launches));
+    FCK(ew_launch(5, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(sum_launch(f->tmpn, f->N, f->scal + 2, st, &eu->launches));
     { int rca = fitc_allreduce(f, f->scal, 3); if (rca) return rca; }                             // sums over the ranks' rows
     double s[3];
     FCK(cudaMemcpyAsync(s, f->scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
@@ -2365,21 +2330,19 @@ int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ld
         FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * f->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * f->d,
                               mc, cudaMemcpyHostToDevice, st));
         FCK(fitc_kfu(f, f->xs, mc));
-        ++eu->launches;
-        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st));
+        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st, &eu->launches));
         FCK(cudaMemcpyAsync(mu + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
         if (var) {
             FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
             FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
             FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
-            eu->launches += 4;
-            FCK(kdiag_launch(eu->prog, f->xs, f->d, mc, f->tmpc, st));
-            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st));       // k_xx - q
-            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st));          // -s
+            FCK(kdiag_launch(eu->prog, f->xs, f->d, mc, f->tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st, &eu->launches));       // k_xx - q
+            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st, &eu->launches));          // -s
             if (f->mode == 2) {                                                             // SoR: K_xu S^-1 K_ux only (sor.jl:302-321)
                 FCK(cudaMemsetAsync(f->tmpc2, 0, sizeof(double) * mc, st));
             }
-            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st));               // [k_xx - q] + s
+            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st, &eu->launches));               // [k_xx - q] + s
             FCK(cudaMemcpyAsync(var + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
         }
         FCK(cudaStreamSynchronize(st));
@@ -2410,15 +2373,13 @@ int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
     GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
     FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * f->d, xs, sizeof(double) * ldxs, sizeof(double) * f->d, Ms, cudaMemcpyHostToDevice, st));
     FCK(fitc_kfu(f, f->xs, Ms));                                         // bufA = K*u  (Ms x Mpad, zero padded rows)
-    ++eu->launches;
-    FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, Ms, f->Mpad, f->tmpc, st));
+    FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, Ms, f->Mpad, f->tmpc, st, &eu->launches));
     FCK(cudaMemcpyAsync(mu, f->tmpc, sizeof(double) * Ms, cudaMemcpyDeviceToHost, st));
     FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
     FCK(trsm_rec_buf(es, bB2, (int)Mspad, 0, (int)f->Mpad));             // B = K*u L_s^-T
-    ++eu->launches;
     if (f->mode != 2) {
         FCK(trsm_rec_buf(eu, bA, (int)Mspad, 0, (int)f->Mpad));         // A = K*u L_uu^-T
-        FCK(gram_full_launch(eu->prog, f->xs, f->d, Ms, Mspad, f->d, f->Kss, Mspad, st));
+        FCK(gram_full_launch(eu->prog, f->xs, f->d, Ms, Mspad, f->d, f->Kss, Mspad, st, &eu->launches));
         GemmDesc g = gemm_desc_default();
         g.A = GemmOperand{bA, bufNone(), 0, 0};
         g.B = GemmOperand{bA, bufNone(), 0, 0};
@@ -2479,9 +2440,8 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     // explicit K_uu^-1 and Sigma_QR^-1 (full symmetric) in the sub-engines' G buffers
     FSUB(gpb200_grad_prepare(eu), eu);
     FSUB(gpb200_grad_prepare(es), es);
-    eu->launches += 2;
-    FCK(symmetrize_launch(eu->G, eu->ld, Mp, st));
-    FCK(symmetrize_launch(es->G, es->ld, Mp, st));
+    FCK(symmetrize_launch(eu->G, eu->ld, Mp, st, &eu->launches));
+    FCK(symmetrize_launch(es->G, es->ld, Mp, st, &eu->launches));
     const bool tma = eu->tma_ok;
     GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bAt{tma ? &f->mapAt : nullptr, f->bufA, Nc};
     GemmBuf bCt{tma ? &f->mapCt : nullptr, f->bufC, Nc};
@@ -2491,11 +2451,10 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
         const int64_t nc = std::min(Nc, f->N - r0);
         FCK(fitc_kuf(f, f->x + r0 * f->d, nc));
-        eu->launches += 2;
         FCK(cudaMemsetAsync(f->w, 0, sizeof(double) * Nc, st));
         FCK(cudaMemcpyAsync(f->w, f->alpha + r0, sizeof(double) * nc, cudaMemcpyDeviceToDevice, st));
-        FCK(rowdot_launch(f->bufB, Nc, f->w, f->M, Nc, f->tmpm, st));
-        FCK(ew_launch(2, f->M, f->rhsm, f->tmpm, nullptr, nullptr, 0.0, st));
+        FCK(rowdot_launch(f->bufB, Nc, f->w, f->M, Nc, f->tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->rhsm, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
     }
     { int rca = fitc_allreduce(f, f->rhsm, (size_t)Mp); if (rca) return rca; }                    // K_uf alpha over all rows
     FCK(solve_device(eu, f->rhsm, f->tmpm, f->betav));
@@ -2513,9 +2472,8 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
             g.C = f->bufB; g.ldc = Mp; g.M = (int)Nc; g.N = (int)Mp; g.K = (int)Mp;
             FCK(launch_gemm(es, g));
         }
-        eu->launches += 2;
-        FCK(rowdot2_launch(f->bufA, f->bufB, Mp, nc, Mp, f->tmpc, st));
-        if (f->mode == 0) FCK(fitc_g_launch(nc, f->alpha + r0, f->lam + r0, f->tmpc, f->gvec + r0, st));
+        FCK(rowdot2_launch(f->bufA, f->bufB, Mp, nc, Mp, f->tmpc, st, &eu->launches));
+        if (f->mode == 0) FCK(fitc_g_launch(nc, f->alpha + r0, f->lam + r0, f->tmpc, f->gvec + r0, st, &eu->launches));
         else FCK(cudaMemsetAsync(f->gvec + r0, 0, sizeof(double) * nc, st));       // SoR part only (sor.jl:219-253)
         {   // P1 = K_fu K_uu^-1 -> bufC
             GemmDesc g = gemm_desc_default();
@@ -2524,21 +2482,18 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
             g.C = f->bufC; g.ldc = Mp; g.M = (int)Nc; g.N = (int)Mp; g.K = (int)Mp;
             FCK(launch_gemm(eu, g));
         }
-        eu->launches += 4;
-        FCK(fitc_wfu_launch(f->bufB, f->bufC, Mp, nc, f->M, f->alpha + r0, f->lam + r0, f->gvec + r0, f->betav, st));
-        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufB, Mp, f->gpart, f->gtmp, st));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st));
+        FCK(fitc_wfu_launch(f->bufB, f->bufC, Mp, nc, f->M, f->alpha + r0, f->lam + r0, f->gvec + r0, f->betav, st, &eu->launches));
+        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufB, Mp, f->gpart, f->gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         if (f->mode != 0) continue;                                       // no Lambda-derivative terms for SoR / DTC
         // diagonal term sum_i g_i dK_ii/dθ_p (scratch: bufC as np x nc)
-        FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->gvec + r0, f->bufC, st));
-        for (int p = 0; p < np; ++p) { ++eu->launches; FCK(sum_launch(f->bufC + (size_t)p * nc, nc, f->gtmp + p, st)); }
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st));
+        FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->gvec + r0, f->bufC, st, &eu->launches));
+        for (int p = 0; p < np; ++p) FCK(sum_launch(f->bufC + (size_t)p * nc, nc, f->gtmp + p, st, &eu->launches));
+        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         // H += K_uf diag(g) K_fu
-        ++eu->launches;
-        FCK(crossgram_launch(eu->prog, eu->x, f->d, f->M, Mp, xr, f->d, nc, Nc, f->d, f->bufA, Nc, st));   // bufA = K_uf chunk (Mpad x Nc)
+        FCK(crossgram_launch(eu->prog, eu->x, f->d, f->M, Mp, xr, f->d, nc, Nc, f->d, f->bufA, Nc, st, &eu->launches));   // bufA = K_uf chunk (Mpad x Nc)
         FCK(cudaMemcpyAsync(f->bufC, f->bufA, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
-        ++eu->launches;
-        FCK(colscale_launch(f->bufC, Nc, Mp, nc, f->gvec + r0, st));
+        FCK(colscale_launch(f->bufC, Nc, Mp, nc, f->gvec + r0, st, &eu->launches));
         {
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bAt, bufNone(), 0, 0};
@@ -2561,10 +2516,9 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
         g.C = f->Wbuf;
         FCK(launch_gemm(eu, g));
     }
-    eu->launches += 4;
-    FCK(fitc_wuu_launch(f->Wbuf, f->Wbuf, eu->G, es->G, Mp, f->M, f->betav, st));
-    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st));
-    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st));
+    FCK(fitc_wuu_launch(f->Wbuf, f->Wbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
+    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
+    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
@@ -2887,12 +2841,6 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     return GPB200_OK;
 }
 
-static cudaError_t fsa_gemm(gpb200_fitc* f, const FsaLaunch& l) {
-    if (l.n == 0) return cudaSuccess;
-    ++f->eu->launches;
-    return fsa_gemm_launch(f->fsa->gitems + l.off, l.n, f->eu->st);
-}
-
 static int fsa_check(gpb200_fitc* f, const char* who) {
     if (f->nranks > 1) { f->err = std::string(who) + ": FSA is single-GPU only"; return GPB200_EINVAL; }
     if (!f->fsa) { f->err = std::string(who) + ": FSA needs gpb200_fitc_set_blocks after set_data"; return GPB200_ESTATE; }
@@ -2913,28 +2861,22 @@ static int fsa_factorize(gpb200_fitc* f) {
         const double* xr = s->xb + ch.r0 * f->d;
         // V = K_fu L_uu^-T (padding rows zero), then Lambda_i = K_ii + (sigma^2 + 1e-10) I - V_i V_i'
         FCK(fitc_kfu(f, xr, ch.rows));
-        ++eu->launches;
-        FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st));
+        FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
         FCK(trsm_rec_buf(eu, bA, (int)Nc, 0, (int)Mp));
-        ++eu->launches;
-        FCK(fsa_gram_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gram.off, ch.gram.n, s->mask, f->noise_var + 1e-10, st));
-        FCK(fsa_gemm(f, ch.vv));
+        FCK(fsa_gram_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gram.off, ch.gram.n, s->mask, f->noise_var + 1e-10, st, &eu->launches));
+        FCK(fsa_gemm_launch(s->gitems + ch.vv.off, ch.vv.n, st, &eu->launches));
         // batched block Cholesky + inverse
         for (int k = 0; k < s->max_tiles; ++k) {
-            if (ch.leaf[k].n > 0) {
-                ++eu->launches;
-                FCK(potrf128_ptr_launch(s->litems + ch.leaf[k].off, ch.leaf[k].n, s->info, st));
-            }
-            FCK(fsa_gemm(f, ch.panel[k]));
-            FCK(fsa_gemm(f, ch.trail[k]));
-            FCK(fsa_gemm(f, ch.inv1[k]));
-            FCK(fsa_gemm(f, ch.inv2[k]));
+            FCK(potrf128_ptr_launch(s->litems + ch.leaf[k].off, ch.leaf[k].n, s->info, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->gitems + ch.panel[k].off, ch.panel[k].n, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->gitems + ch.trail[k].off, ch.trail[k].n, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->gitems + ch.inv1[k].off, ch.inv1[k].n, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->gitems + ch.inv2[k].off, ch.inv2[k].n, st, &eu->launches));
         }
         // W' = K_uf L_Lambda^-T, Sigma_QR += W' W
         FCK(fitc_kuf(f, xr, ch.rows));
-        ++eu->launches;
-        FCK(fsa_mask_launch(f->bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st));
-        FCK(fsa_gemm(f, ch.wt));
+        FCK(fsa_mask_launch(f->bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+        FCK(fsa_gemm_launch(s->gitems + ch.wt.off, ch.wt.n, st, &eu->launches));
         GemmDesc g = gemm_desc_default();
         g.A = GemmOperand{bWt, bufNone(), 0, 0};
         g.B = GemmOperand{bWt, bufNone(), 0, 0};
@@ -2964,33 +2906,29 @@ static int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, do
     const int64_t Np = s->Np, Mp = f->Mpad;
     FCK(cudaMemcpyAsync(f->y, y_minus_mean, sizeof(double) * f->N, cudaMemcpyHostToDevice, st));
     FCK(cudaMemsetAsync(s->r, 0, sizeof(double) * Np, st));
-    eu->launches += 3;
-    FCK(fsa_permute_launch(1, f->y, s->pos, f->N, s->r, st));
-    FCK(fsa_bdmv_launch(0, s->X, s->rblk, s->bstart, s->bsize, s->boff, s->r, s->t1, Np, st));
-    FCK(fsa_bdmv_launch(1, s->LT, s->rblk, s->bstart, s->bsize, s->boff, s->t1, s->t2, Np, st));     // t2 = Lambda^-1 r
+    FCK(fsa_permute_launch(1, f->y, s->pos, f->N, s->r, st, &eu->launches));
+    FCK(fsa_bdmv_launch(0, s->X, s->rblk, s->bstart, s->bsize, s->boff, s->r, s->t1, Np, st, &eu->launches));
+    FCK(fsa_bdmv_launch(1, s->LT, s->rblk, s->bstart, s->bsize, s->boff, s->t1, s->t2, Np, st, &eu->launches));     // t2 = Lambda^-1 r
     FCK(cudaMemsetAsync(f->bvec, 0, sizeof(double) * Mp, st));
     for (const FsaChunk& ch : s->chunks) {
         FCK(fitc_kuf(f, s->xb + ch.r0 * f->d, ch.rows));
-        eu->launches += 2;
-        FCK(rowdot_launch(f->bufB, f->Nc, s->t2 + ch.r0, f->M, ch.rows, f->tmpm, st));
-        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st));
+        FCK(rowdot_launch(f->bufB, f->Nc, s->t2 + ch.r0, f->M, ch.rows, f->tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
     }
     FCK(cudaMemcpyAsync(f->rhsm, f->bvec, sizeof(double) * Mp, cudaMemcpyDeviceToDevice, st));
     FCK(solve_device(es, f->rhsm, f->tmpm, f->uvec));
     for (const FsaChunk& ch : s->chunks) {
         FCK(fitc_kfu(f, s->xb + ch.r0 * f->d, ch.rows));
-        ++eu->launches;
-        FCK(rowdot_launch(f->bufA, Mp, f->uvec, ch.rows, Mp, s->t1 + ch.r0, st));
+        FCK(rowdot_launch(f->bufA, Mp, f->uvec, ch.rows, Mp, s->t1 + ch.r0, st, &eu->launches));
     }
-    eu->launches += 8;
-    FCK(fsa_resid_launch(s->t1, s->r, s->t1, s->mask, Np, st));                                      // r - K_fu u, padding 0
-    FCK(fsa_bdmv_launch(0, s->X, s->rblk, s->bstart, s->bsize, s->boff, s->t1, s->t2, Np, st));
-    FCK(fsa_bdmv_launch(1, s->LT, s->rblk, s->bstart, s->bsize, s->boff, s->t2, s->a, Np, st));      // alpha (padded order)
-    FCK(fsa_permute_launch(0, s->a, s->pos, f->N, f->alpha, st));
-    FCK(dot_launch(s->r, s->a, Np, f->scal + 0, st));
-    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st));
-    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st));
-    FCK(sum_launch(s->logd, Np, f->scal + 3, st));
+    FCK(fsa_resid_launch(s->t1, s->r, s->t1, s->mask, Np, st, &eu->launches));                                      // r - K_fu u, padding 0
+    FCK(fsa_bdmv_launch(0, s->X, s->rblk, s->bstart, s->bsize, s->boff, s->t1, s->t2, Np, st, &eu->launches));
+    FCK(fsa_bdmv_launch(1, s->LT, s->rblk, s->bstart, s->bsize, s->boff, s->t2, s->a, Np, st, &eu->launches));      // alpha (padded order)
+    FCK(fsa_permute_launch(0, s->a, s->pos, f->N, f->alpha, st, &eu->launches));
+    FCK(dot_launch(s->r, s->a, Np, f->scal + 0, st, &eu->launches));
+    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st, &eu->launches));
+    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st, &eu->launches));
+    FCK(sum_launch(s->logd, Np, f->scal + 3, st, &eu->launches));
     double sc[4];
     FCK(cudaMemcpyAsync(sc, f->scal, sizeof(double) * 4, cudaMemcpyDeviceToHost, st));
     if (alpha) FCK(cudaMemcpyAsync(alpha, f->alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
@@ -3013,19 +2951,16 @@ static int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise) {
     GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, Mp};
     for (const FsaChunk& ch : s->chunks) {
         FCK(fitc_kuf(f, s->xb + ch.r0 * f->d, ch.rows));
-        ++eu->launches;
-        FCK(fsa_mask_launch(f->bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st));
-        FCK(fsa_gemm(f, ch.wt));                                              // W' = K_uf X'               (bufA, Mpad x Nc)
-        FCK(fsa_gemm(f, ch.z));                                               // Z = X' W = Lambda^-1 K_fu  (bufB, Nc x Mpad)
+        FCK(fsa_mask_launch(f->bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+        FCK(fsa_gemm_launch(s->gitems + ch.wt.off, ch.wt.n, st, &eu->launches));  // W' = K_uf X'               (bufA, Mpad x Nc)
+        FCK(fsa_gemm_launch(s->gitems + ch.z.off, ch.z.n, st, &eu->launches));    // Z = X' W = Lambda^-1 K_fu  (bufB, Nc x Mpad)
         FCK(trsm_rec_buf(es, bB2, (int)ch.rows, 0, (int)Mp));                 // Y = Z L_s^-T
-        ++eu->launches;
-        FCK(rowvar_launch(f->bufB, Mp, f->zeroc, ch.rows, Mp, s->t1 + ch.r0, st));   // -|Y_r|^2
+        FCK(rowvar_launch(f->bufB, Mp, f->zeroc, ch.rows, Mp, s->t1 + ch.r0, st, &eu->launches));   // -|Y_r|^2
     }
-    eu->launches += 4;
-    FCK(sum_launch(s->t1, Np, f->scal + 0, st));
-    FCK(dot_launch(s->a, s->a, Np, f->scal + 1, st));
-    FCK(fsa_bdmv_launch(2, s->X, s->rblk, s->bstart, s->bsize, s->boff, nullptr, s->t2, Np, st));
-    FCK(sum_launch(s->t2, Np, f->scal + 2, st));
+    FCK(sum_launch(s->t1, Np, f->scal + 0, st, &eu->launches));
+    FCK(dot_launch(s->a, s->a, Np, f->scal + 1, st, &eu->launches));
+    FCK(fsa_bdmv_launch(2, s->X, s->rblk, s->bstart, s->bsize, s->boff, nullptr, s->t2, Np, st, &eu->launches));
+    FCK(sum_launch(s->t2, Np, f->scal + 2, st, &eu->launches));
     double sc[3];
     FCK(cudaMemcpyAsync(sc, f->scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
@@ -3056,10 +2991,9 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
         const double* xr = s->xb + ch.r0 * f->d;
         const int64_t nc = ch.rows;
         FCK(fitc_kuf(f, xr, nc));
-        ++eu->launches;
-        FCK(fsa_mask_launch(f->bufB, Nc, Mp, nc, nullptr, s->mask + ch.r0, st));
-        FCK(fsa_gemm(f, ch.wt));                                // W' = K_uf X'                   (bufA, Mpad x Nc)
-        FCK(fsa_gemm(f, ch.z));                                 // Z = Lambda^-1 K_fu             (bufB, Nc x Mpad)
+        FCK(fsa_mask_launch(f->bufB, Nc, Mp, nc, nullptr, s->mask + ch.r0, st, &eu->launches));
+        FCK(fsa_gemm_launch(s->gitems + ch.wt.off, ch.wt.n, st, &eu->launches));  // W' = K_uf X'                   (bufA, Mpad x Nc)
+        FCK(fsa_gemm_launch(s->gitems + ch.z.off, ch.z.n, st, &eu->launches));    // Z = Lambda^-1 K_fu             (bufB, Nc x Mpad)
         {   // P2 = Z S^-1 -> bufC
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bB2, bufNone(), 0, 0};
@@ -3069,16 +3003,14 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
         }
         FCK(trsm_rec_buf(es, bB2, (int)nc, 0, (int)Mp));       // Y = Z L_s^-T                   (bufB)
         // G_i = -Lambda_i^-1 + Y_i Y_i' + alpha_i alpha_i'  (Gpk), then sum_i <G_i, dK_ii/dθ_p>
-        FCK(fsa_gemm(f, ch.ginv));
-        FCK(fsa_gemm(f, ch.gyy));
-        eu->launches += 4;
-        FCK(fsa_outer_launch(s->gramitems + ch.gtiles.off, ch.gtiles.n, s->a, st));
-        FCK(fsa_trace_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gtiles.off, ch.gtiles.n, s->mask, s->gpart, f->gtmp, st));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st));
+        FCK(fsa_gemm_launch(s->gitems + ch.ginv.off, ch.ginv.n, st, &eu->launches));
+        FCK(fsa_gemm_launch(s->gitems + ch.gyy.off, ch.gyy.n, st, &eu->launches));
+        FCK(fsa_outer_launch(s->gramitems + ch.gtiles.off, ch.gtiles.n, s->a, st, &eu->launches));
+        FCK(fsa_trace_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gtiles.off, ch.gtiles.n, s->mask, s->gpart, f->gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         // P1' = K_uu^-1 K_uf (bufB, Mpad x Nc) from K_fu (bufA)
         FCK(fitc_kfu(f, xr, nc));
-        ++eu->launches;
-        FCK(fsa_mask_launch(f->bufA, Mp, nc, Mp, s->mask + ch.r0, nullptr, st));
+        FCK(fsa_mask_launch(f->bufA, Mp, nc, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
         {
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bufG(eu), bufNone(), 0, 0};
@@ -3087,12 +3019,11 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
             FCK(launch_gemm(eu, g));
         }
         // W_fu = 2 alpha beta' - 2 P2 - 2 G_bd P1  (bufC); P1' G_bd -> bufA (Mpad x Nc)
-        eu->launches += 4;
-        FCK(fitc_wfu_launch(f->bufC, f->bufA, Mp, nc, f->M, s->a + ch.r0, s->ones, f->zeroc, f->betav, st));   // g = 0: P1 unused
-        FCK(fsa_gemm(f, ch.gp1t));
-        FCK(fsa_axpy_t_launch(f->bufC, Mp, f->bufA, Nc, nc, Mp, -2.0, st));
-        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufC, Mp, f->gpart, f->gtmp, st));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st));
+        FCK(fitc_wfu_launch(f->bufC, f->bufA, Mp, nc, f->M, s->a + ch.r0, s->ones, f->zeroc, f->betav, st, &eu->launches));   // g = 0: P1 unused
+        FCK(fsa_gemm_launch(s->gitems + ch.gp1t.off, ch.gp1t.n, st, &eu->launches));
+        FCK(fsa_axpy_t_launch(f->bufC, Mp, f->bufA, Nc, nc, Mp, -2.0, st, &eu->launches));
+        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufC, Mp, f->gpart, f->gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         {   // H += P1' G_bd P1 = K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bBt, bufNone(), 0, 0};
@@ -3102,10 +3033,9 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
             FCK(launch_gemm(eu, g));
         }
     }
-    eu->launches += 4;
-    FCK(fitc_wuu_launch(f->Wbuf, f->Hbuf, eu->G, es->G, Mp, f->M, f->betav, st));
-    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st));
-    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st));
+    FCK(fitc_wuu_launch(f->Wbuf, f->Hbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
+    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
+    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
@@ -3286,11 +3216,6 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
     FCK(upload(s->pg, s->pg_cap, gi));
     FCK(upload(s->px, s->px_cap, xi));
     FCK(upload(s->pr, s->pr_cap, ri));
-    auto pgemm = [&](const FsaLaunch& l) -> cudaError_t {
-        if (l.n == 0) return cudaSuccess;
-        ++eu->launches;
-        return fsa_gemm_launch(s->pg + l.off, l.n, st);
-    };
     GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, Mp};
     GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, Mp};
     GemmBuf bVs{eu->tma_ok ? &s->mapVs : nullptr, s->Vs, Mp};
@@ -3298,42 +3223,38 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
     for (const Sub& sb : subs) {
         const int64_t row0 = sb.t0 * TILE, mq = (sb.t1 - sb.t0) * TILE;
         FCK(cudaMemcpyAsync(f->xs, xsp.data() + row0 * d, sizeof(double) * mq * d, cudaMemcpyHostToDevice, st));
-        eu->launches += 5;
-        FCK(crossgram_launch(eu->prog, f->xs, d, mq, mq, eu->x, d, f->M, Mp, d, f->bufB, Mp, st));     // K_*u
-        FCK(rowdot_launch(f->bufB, Mp, f->uvec, mq, Mp, mu1, st));                                       // K_*u u
+        FCK(crossgram_launch(eu->prog, f->xs, d, mq, mq, eu->x, d, f->M, Mp, d, f->bufB, Mp, st, &eu->launches));     // K_*u
+        FCK(rowdot_launch(f->bufB, Mp, f->uvec, mq, Mp, mu1, st, &eu->launches));                                       // K_*u u
         FCK(cudaMemcpyAsync(s->Vs, f->bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));
         FCK(trsm_rec_buf(eu, bVs, (int)mq, 0, (int)Mp));                                                 // V_*'
-        FCK(kdiag_launch(eu->prog, f->xs, d, mq, r2, st));
-        FCK(rowvar_launch(s->Vs, Mp, r2, mq, Mp, q, st));                                                 // k** - |V_*|^2
+        FCK(kdiag_launch(eu->prog, f->xs, d, mq, r2, st, &eu->launches));
+        FCK(rowvar_launch(s->Vs, Mp, r2, mq, Mp, q, st, &eu->launches));                                                 // k** - |V_*|^2
         FCK(cudaMemsetAsync(mu2, 0, sizeof(double) * mq, st));
         FCK(cudaMemsetAsync(g2, 0, sizeof(double) * mq, st));
         for (const Pass& ps : sb.passes) {
             const FsaChunk& ch = s->chunks[(size_t)ps.chunk];
             const double* xr = s->xb + ch.r0 * d;
             FCK(fitc_kfu(f, xr, ch.rows));                                                                 // V of the training chunk
-            eu->launches += 6;
-            FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st));
+            FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
             FCK(trsm_rec_buf(eu, bA, (int)Nc, 0, (int)Mp));
-            FCK(fsa_crossgram_launch(eu->prog, f->xs, s->xb, d, s->px + ps.xg.off, ps.xg.n, s->mask, st));
-            FCK(pgemm(ps.vv));
-            FCK(fsa_rowdot_launch(s->pr + ps.mu2.off, ps.mu2.n, st));
-            FCK(pgemm(ps.gg));
-            FCK(fsa_rowdot_launch(s->pr + ps.g2.off, ps.g2.n, st));
-            FCK(pgemm(ps.hh));
-            FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->bufA, Nc, st));   // K_uf of the chunk
-            FCK(fsa_mask_launch(f->bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st));
-            FCK(pgemm(ps.kh));
+            FCK(fsa_crossgram_launch(eu->prog, f->xs, s->xb, d, s->px + ps.xg.off, ps.xg.n, s->mask, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->pg + ps.vv.off, ps.vv.n, st, &eu->launches));
+            FCK(fsa_rowdot_launch(s->pr + ps.mu2.off, ps.mu2.n, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->pg + ps.gg.off, ps.gg.n, st, &eu->launches));
+            FCK(fsa_rowdot_launch(s->pr + ps.g2.off, ps.g2.n, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->pg + ps.hh.off, ps.hh.n, st, &eu->launches));
+            FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->bufA, Nc, st, &eu->launches));   // K_uf of the chunk
+            FCK(fsa_mask_launch(f->bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+            FCK(fsa_gemm_launch(s->pg + ps.kh.off, ps.kh.n, st, &eu->launches));
         }
         FCK(trsm_rec_buf(es, bB2, (int)mq, 0, (int)Mp));                                                  // R = (K_*u - G W) L_s^-T
-        eu->launches += 3;
-        FCK(rowvar_launch(f->bufB, Mp, f->zeroc, mq, Mp, r2, st));
-        FCK(fsa_var_launch(vp, q, g2, r2, mq, st));
-        FCK(ew_launch(2, mq, mu1, mu2, nullptr, nullptr, 0.0, st));
+        FCK(rowvar_launch(f->bufB, Mp, f->zeroc, mq, Mp, r2, st, &eu->launches));
+        FCK(fsa_var_launch(vp, q, g2, r2, mq, st, &eu->launches));
+        FCK(ew_launch(2, mq, mu1, mu2, nullptr, nullptr, 0.0, st, &eu->launches));
         FCK(cudaMemcpyAsync(mu_p.data() + row0, mu1, sizeof(double) * mq, cudaMemcpyDeviceToHost, st));
         if (var) FCK(cudaMemcpyAsync(var_p.data() + row0, vp, sizeof(double) * mq, cudaMemcpyDeviceToHost, st));
         if (cov) {
-            ++eu->launches;
-            FCK(gram_full_launch(eu->prog, f->xs, d, mq, mq, d, f->Kss, mq, st));
+            FCK(gram_full_launch(eu->prog, f->xs, d, mq, mq, d, f->Kss, mq, st, &eu->launches));
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bVs, bufNone(), 0, 0};
             g.B = GemmOperand{bVs, bufNone(), 0, 0};
@@ -3344,7 +3265,7 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
             g.B = GemmOperand{bB2, bufNone(), 0, 0};
             g.alpha = 1.0;
             FCK(launch_gemm(es, g));                                                                      // + R R'
-            FCK(pgemm(sb.ggt));                                                                           // - G G'
+            FCK(fsa_gemm_launch(s->pg + sb.ggt.off, sb.ggt.n, st, &eu->launches));  // - G G'
             FCK(cudaMemcpyAsync(cov_p.data(), f->Kss, sizeof(double) * mq * mq, cudaMemcpyDeviceToHost, st));
         }
         FCK(cudaStreamSynchronize(st));

@@ -466,7 +466,7 @@ cudaError_t ensure_smem(K kern, size_t bytes) {
 
 cudaError_t gram_lower_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad,
                               const double* noise_var, int64_t n_noise, double nugget, double* G, int64_t ldg,
-                              cudaStream_t st, int own_tiles, int nranks, int rank, int own_axis, int bm_min) {
+                              cudaStream_t st, int64_t* launches, int own_tiles, int nranks, int rank, int own_axis, int bm_min) {
     const int T = (int)(Npad / TB);
     dim3 grid(T, T);
     const size_t sm = xtile_smem(d);
@@ -478,11 +478,12 @@ cudaError_t gram_lower_launch(const KProg& P, const double* x, int64_t ldx, int 
         if ((e = ensure_smem(gram_lower_kernel<false>, sm)) != cudaSuccess) return e;
         gram_lower_kernel<false><<<grid, NT, sm, st>>>(P, x, ldx, d, N, Npad, noise_var, n_noise, nugget, G, ldg, own_tiles, nranks, rank, own_axis, bm_min);
     }
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t crossgram_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, const double* x,
-                             int64_t ldx, int64_t N, int64_t Npad, int d, double* Kst, int64_t ldk, cudaStream_t st) {
+                             int64_t ldx, int64_t N, int64_t Npad, int d, double* Kst, int64_t ldk, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)(Npad / TB), (unsigned)(Mpad / TB));
     const size_t sm = xtile_smem(d);
     cudaError_t e;
@@ -493,11 +494,12 @@ cudaError_t crossgram_launch(const KProg& P, const double* xs, int64_t ldxs, int
         if ((e = ensure_smem(crossgram_kernel<false>, sm)) != cudaSuccess) return e;
         crossgram_kernel<false><<<grid, NT, sm, st>>>(P, xs, ldxs, M, x, ldx, N, d, Kst, ldk);
     }
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t gram_full_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, int d,
-                             double* Kss, int64_t ldk, cudaStream_t st) {
+                             double* Kss, int64_t ldk, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)(Mpad / TB), (unsigned)(Mpad / TB));
     const size_t sm = xtile_smem(d);
     cudaError_t e;
@@ -508,11 +510,13 @@ cudaError_t gram_full_launch(const KProg& P, const double* xs, int64_t ldxs, int
         if ((e = ensure_smem(gram_full_kernel<false>, sm)) != cudaSuccess) return e;
         gram_full_kernel<false><<<grid, NT, sm, st>>>(P, xs, ldxs, M, d, Kss, ldk);
     }
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t kdiag_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, double* out, cudaStream_t st) {
+cudaError_t kdiag_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, double* out, cudaStream_t st, int64_t* launches) {
     kdiag_kernel<<<(unsigned)((M + 127) / 128), 128, 0, st>>>(P, xs, ldxs, M, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
@@ -520,7 +524,7 @@ int trace_num_acc(const KProg& P) { return P.fast ? 3 : P.n_theta + 1; }
 
 cudaError_t trace_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad,
                          const double* alpha, const double* Kinv, int64_t ldg, double* part, double* out,
-                         cudaStream_t st, int bm_mod, int bm_rem, int bm_div) {
+                         cudaStream_t st, int64_t* launches, int bm_mod, int bm_rem, int bm_div) {
     if (bm_div < 1) bm_div = 1;
     const int T = (int)(Npad / TB);
     const int tiles = T * (T + 1) / 2;
@@ -534,15 +538,17 @@ cudaError_t trace_launch(const KProg& P, const double* x, int64_t ldx, int d, in
         if ((e = ensure_smem(trace_kernel<false>, sm)) != cudaSuccess) return e;
         trace_kernel<false><<<tiles, NT, sm, st>>>(P, x, ldx, d, N, alpha, Kinv, ldg, part, tiles, bm_mod, bm_rem, bm_div);
     }
+    if (launches) ++*launches;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     reduce_partials_kernel<<<nacc, 256, 0, st>>>(part, tiles, nacc, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 // acc_out[p] += sum over the N1 x N2 rectangle of W[i,m] dk(x1_i,x2_m)/dθ_p ; part: [tiles][n_theta] scratch
 cudaError_t trace_rect_launch(const KProg& P, const double* x1, int64_t ldx1, int64_t N1, const double* x2, int64_t ldx2,
                               int64_t N2, int d, const double* W, int64_t ldw, double* part, double* tmp_out,
-                              cudaStream_t st) {
+                              cudaStream_t st, int64_t* launches) {
     const int tm = (int)((N1 + TB - 1) / TB), tn = (int)((N2 + TB - 1) / TB);
     const int nacc = P.fast ? 2 : P.n_theta;
     const size_t sm = xtile_smem(d) + (size_t)(8 * nacc) * sizeof(double);
@@ -555,23 +561,27 @@ cudaError_t trace_rect_launch(const KProg& P, const double* x1, int64_t ldx1, in
         if ((e = ensure_smem(trace_rect_kernel<false>, sm)) != cudaSuccess) return e;
         trace_rect_kernel<false><<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part);
     }
+    if (launches) ++*launches;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     reduce_partials_kernel<<<nacc, 256, 0, st>>>(part, tm * tn, nacc, tmp_out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t kdiag_grad_launch(const KProg& P, const double* x, int64_t ldx, int64_t N, const double* gvec, double* out,
-                              cudaStream_t st) {
+                              cudaStream_t st, int64_t* launches) {
     kdiag_grad_kernel<<<(unsigned)((N + 127) / 128), 128, 0, st>>>(P, x, ldx, N, gvec, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad, int j,
-                                  double* D, int64_t ldd, cudaStream_t st) {
+                                  double* D, int64_t ldd, cudaStream_t st, int64_t* launches) {
     if (j < 0 || j >= P.n_theta) return cudaErrorInvalidValue;
     dim3 grid((unsigned)(Npad / TB), (unsigned)(Npad / TB));
     const size_t sm = xtile_smem(d);
     cudaError_t e;
     if ((e = ensure_smem(gram_grad_full_kernel, sm)) != cudaSuccess) return e;
     gram_grad_full_kernel<<<grid, NT, sm, st>>>(P, x, ldx, N, d, j, D, ldd);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

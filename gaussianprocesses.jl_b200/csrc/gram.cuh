@@ -7,27 +7,27 @@
 // lower tiles of K_y (+ noise on the diagonal, identity in the padding) into G (row-major, ld = ldg)
 cudaError_t gram_lower_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad,
                               const double* noise_var, int64_t n_noise, double nugget, double* G, int64_t ldg,
-                              cudaStream_t st, int own_tiles = 0, int nranks = 1, int rank = 0, int own_axis = 0, int bm_min = 0);
+                              cudaStream_t st, int64_t* launches, int own_tiles = 0, int nranks = 1, int rank = 0, int own_axis = 0, int bm_min = 0);
 // Kst[m, n] = k(xs_m, x_n), M_pad x N_pad, zero padding
 cudaError_t crossgram_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, const double* x,
-                             int64_t ldx, int64_t N, int64_t Npad, int d, double* Kst, int64_t ldk, cudaStream_t st);
+                             int64_t ldx, int64_t N, int64_t Npad, int d, double* Kst, int64_t ldk, cudaStream_t st, int64_t* launches);
 // Kss[m, m'] = k(xs_m, xs_m'), full M_pad x M_pad
 cudaError_t gram_full_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, int d,
-                             double* Kss, int64_t ldk, cudaStream_t st);
-cudaError_t kdiag_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, double* out, cudaStream_t st);
+                             double* Kss, int64_t ldk, cudaStream_t st, int64_t* launches);
+cudaError_t kdiag_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, double* out, cudaStream_t st, int64_t* launches);
 // number of accumulators per tile: n_theta + 1 (last = tr(A))
 int trace_num_acc(const KProg& P);
 // part: [tiles][nacc] scratch; out: [nacc] = {dmll_kernel[0..n_theta), tr(A)}
 cudaError_t trace_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad,
                          const double* alpha, const double* Kinv, int64_t ldg, double* part, double* out,
-                         cudaStream_t st, int bm_mod = 1, int bm_rem = 0, int bm_div = 1);
+                         cudaStream_t st, int64_t* launches, int bm_mod = 1, int bm_rem = 0, int bm_div = 1);
 // FITC gradient pieces: rectangular weighted trace (tmp_out[p] = sum W .* dK/dθ_p over the rectangle; part must hold
 // ceil(N1/128)*ceil(N2/128)*n_theta doubles) and g_i * dk(x_i,x_i)/dθ_p written as out[p*N + i]
 cudaError_t trace_rect_launch(const KProg& P, const double* x1, int64_t ldx1, int64_t N1, const double* x2, int64_t ldx2,
                               int64_t N2, int d, const double* W, int64_t ldw, double* part, double* tmp_out,
-                              cudaStream_t st);
+                              cudaStream_t st, int64_t* launches);
 cudaError_t kdiag_grad_launch(const KProg& P, const double* x, int64_t ldx, int64_t N, const double* gvec, double* out,
-                              cudaStream_t st);
+                              cudaStream_t st, int64_t* launches);
 // D[i, k] = dk(x_i, x_k)/dtheta_j, full N_pad x N_pad (zero padding)  -- grad_slice! (src/kernels/kernels.jl:96-131)
 cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad, int j,
-                                  double* D, int64_t ldd, cudaStream_t st);
+                                  double* D, int64_t ldd, cudaStream_t st, int64_t* launches);

@@ -326,7 +326,7 @@ bool seiso_fast_prepare(double l2, double s2, SeIsoFast* out) {
 
 cudaError_t gram_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* mapXT, int dx, const SeIsoFast& sf, int64_t N, int64_t Npad,
                                   const double* noise_var, int64_t n_noise, double nugget, double* G, int64_t ldg,
-                                  cudaStream_t st, int own_tiles, int nranks, int rank, int own_axis) {
+                                  cudaStream_t st, int64_t* launches, int own_tiles, int nranks, int rank, int own_axis) {
     const int T = (int)(Npad / TB);
     const int tiles = T * (T + 1) / 2;
     switch (dx) {
@@ -336,12 +336,13 @@ cudaError_t gram_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* ma
     case 8: gram_seiso_tma_kernel<8><<<tiles, NT, 0, st>>>(*mapX, *mapXT, sf, N, noise_var, n_noise, nugget, G, ldg, own_tiles, nranks, rank, own_axis); break;
     default: return cudaErrorInvalidValue;
     }
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t trace_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* mapXT, int dx, const SeIsoFast& sf, int64_t N, int64_t Npad,
                                    const double* alpha, const double* Kinv, int64_t ldg, double* part, double* out,
-                                   cudaStream_t st, int bm_mod, int bm_rem, int bm_div) {
+                                   cudaStream_t st, int64_t* launches, int bm_mod, int bm_rem, int bm_div) {
     const int T = (int)(Npad / TB);
     const int tiles = T * (T + 1) / 2;
     if (bm_div < 1) bm_div = 1;
@@ -352,8 +353,10 @@ cudaError_t trace_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* m
     case 8: trace_seiso_tma_kernel<8><<<tiles, NT, 0, st>>>(*mapX, *mapXT, sf, N, alpha, Kinv, ldg, part, bm_mod, bm_rem, bm_div); break;
     default: return cudaErrorInvalidValue;
     }
+    if (launches) ++*launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     reduce_partials3_kernel<<<3, 256, 0, st>>>(part, tiles, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

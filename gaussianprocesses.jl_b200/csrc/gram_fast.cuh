@@ -16,8 +16,8 @@ bool seiso_fast_prepare(double l2, double s2, SeIsoFast* out);
 // mapXT: descriptor of the transposed copy [dx x N] (row pitch Npad), box dx x 128
 cudaError_t gram_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* mapXT, int dx, const SeIsoFast& sf, int64_t N, int64_t Npad,
                                   const double* noise_var, int64_t n_noise, double nugget, double* G, int64_t ldg,
-                                  cudaStream_t st, int own_tiles, int nranks, int rank, int own_axis);
+                                  cudaStream_t st, int64_t* launches, int own_tiles, int nranks, int rank, int own_axis);
 // part: [tiles][3] scratch; out[0..2] = {dmll/dll, dmll/dlsigma, tr(A)} (same contract as trace_launch's fast path)
 cudaError_t trace_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* mapXT, int dx, const SeIsoFast& sf, int64_t N, int64_t Npad,
                                    const double* alpha, const double* Kinv, int64_t ldg, double* part, double* out,
-                                   cudaStream_t st, int bm_mod, int bm_rem, int bm_div);
+                                   cudaStream_t st, int64_t* launches, int bm_mod, int bm_rem, int bm_div);

@@ -326,7 +326,7 @@ bool g_attr_set_blk = false, g_attr_set_ptr = false;
 }  // namespace
 
 cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf, double* Dinv, double* DinvT,
-                            double* logd, int* info, int p0, int ntiles, int tile_stride, cudaStream_t st,
+                            double* logd, int* info, int p0, int ntiles, int tile_stride, cudaStream_t st, int64_t* launches,
                             const PotrfPeers* peers) {
     PotrfPeers pp{};
     if (peers) pp = *peers;
@@ -336,10 +336,11 @@ cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf
         g_attr_set_blk = true;
     }
     potrf128_blk_kernel<<<ntiles, NTB, SMEM_BLK, st>>>(G, ldg, F, ldf, Dinv, DinvT, logd, info, p0, tile_stride, pp);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st) {
+cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     if (!g_attr_set_ptr) {
         cudaError_t e = cudaFuncSetAttribute(potrf128_ptr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BLK);
@@ -347,5 +348,6 @@ cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cud
         g_attr_set_ptr = true;
     }
     potrf128_ptr_kernel<<<n, NTB, SMEM_BLK, st>>>(items, info);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

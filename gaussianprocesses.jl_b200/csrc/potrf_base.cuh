@@ -12,7 +12,7 @@ struct PotrfPeers {
 };
 // tiles at diagonal offsets p0 + b*tile_stride, b < ntiles.  *info must be initialised to INT_MAX.
 cudaError_t potrf128_launch(const double* G, int64_t ldg, double* F, int64_t ldf, double* Dinv, double* DinvT,
-                            double* logd, int* info, int p0, int ntiles, int tile_stride, cudaStream_t st,
+                            double* logd, int* info, int p0, int ntiles, int tile_stride, cudaStream_t st, int64_t* launches,
                             const PotrfPeers* peers = nullptr);
 // pointer-table entry point (batched block-diagonal factorisation, fsa.cu): tile b of the launch reads the lower triangle of
 // items[b].G and writes W = L^-1 (clean lower) to items[b].Dinv, W' (clean upper) to items[b].DinvT, all three with leading
@@ -27,4 +27,4 @@ struct Potrf128Item {
     int info_base;
     int pad_;
 };
-cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st);
+cudaError_t potrf128_ptr_launch(const Potrf128Item* items, int n, int* info, cudaStream_t st, int64_t* launches);

@@ -247,8 +247,7 @@ int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n) {
     for (int q = 0; q < R; ++q) {
         for (int p = 0; p < R; ++p)
             if (p != q) SCK(L[q], cudaStreamWaitEvent(L[q]->st, copied[p], 0));
-        ++L[q]->launches;
-        SCK(L[q], shard_sum_ranks(vec(L[q]), L[q]->red, (int64_t)n, R, (int64_t)n, L[q]->st));
+        SCK(L[q], shard_sum_ranks(vec(L[q]), L[q]->red, (int64_t)n, R, (int64_t)n, L[q]->st, &L[q]->launches));
     }
     return GPB200_OK;
 }
@@ -273,8 +272,7 @@ int coll_allreduce_min_info(const Locals& L) {
     for (int q = 0; q < R; ++q) {
         for (int p = 0; p < R; ++p)
             if (p != q) SCK(L[q], cudaStreamWaitEvent(L[q]->st, copied[p], 0));
-        ++L[q]->launches;
-        SCK(L[q], shard_min_ranks(L[q]->info_dev, L[q]->redi, R, L[q]->st));
+        SCK(L[q], shard_min_ranks(L[q]->info_dev, L[q]->redi, R, L[q]->st, &L[q]->launches));
     }
     return GPB200_OK;
 }
@@ -468,8 +466,7 @@ int shard_cholesky_la(const Locals& L) {
                 cudaError_t e = chol_panel(q, c0, nb, NBp);
                 q->row_lim = 0; q->lookahead = la;
                 if (e != cudaSuccess) { q->err = std::string("chol_panel: ") + cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
-                ++q->launches;
-                e = shard_copy_lower(q->P[pb] + (size_t)c0 * NBp, NBp, q->F + (size_t)c0 * q->ld + c0, q->ld, nb, q->st);
+                e = shard_copy_lower(q->P[pb] + (size_t)c0 * NBp, NBp, q->F + (size_t)c0 * q->ld + c0, q->ld, nb, q->st, &q->launches);
                 if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
             }
             if (rc) break;
@@ -486,18 +483,15 @@ int shard_cholesky_la(const Locals& L) {
             const size_t per = (size_t)maxown * TILE * NBp;
             for (auto* q : L) {
                 cudaError_t e = shard_trsm_rows(q, c0, r1, 0, nb, pb);
-                ++q->launches;
-                if (e == cudaSuccess) e = shard_scatter_rows(q->G, q->F, q->ld, Np, c0, nb, t1, q->Sbuf + (size_t)q->rank * per, NBp, own_of(q), q->st);
+                if (e == cudaSuccess) e = shard_scatter_rows(q->G, q->F, q->ld, Np, c0, nb, t1, q->Sbuf + (size_t)q->rank * per, NBp, own_of(q), q->st, &q->launches);
                 if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
             }
             if (rc) break;
             if ((rc = coll_allgather(L, [&](gpb200_handle* q) { return (void*)q->Sbuf; }, sizeof(double) * per))) break;
             for (auto* q : L) {
-                ++q->launches;
-                cudaError_t e = shard_unpack_panel(q->P[pb], NBp, Np, nb, t1, q->Sbuf, (int64_t)per, own_of(q), q->st);
+                cudaError_t e = shard_unpack_panel(q->P[pb], NBp, Np, nb, t1, q->Sbuf, (int64_t)per, own_of(q), q->st, &q->launches);
                 if (e == cudaSuccess && q->rank == o) {
-                    ++q->launches;
-                    e = shard_transpose(q->F + (size_t)c0 * q->ld + r1, q->ld, q->P[pb] + (size_t)r1 * NBp, NBp, Np - r1, nb, q->st);
+                    e = shard_transpose(q->F + (size_t)c0 * q->ld + r1, q->ld, q->P[pb] + (size_t)r1 * NBp, NBp, Np - r1, nb, q->st, &q->launches);
                 }
                 if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
             }
@@ -563,9 +557,8 @@ int shard_solve(const Locals& L, double* gpb200_handle::*rhs, double* gpb200_han
             double* r = q->*rhs; double* y = q->*ybuf;
             double* t = q->tblk;                     // nb-vector scratch
             if (c0 > 0) {
-                q->launches += 2;
-                SCK(q, rowdot_launch(q->F + (size_t)c0 * q->ld, q->ld, y, nb, c0, t, q->st));
-                SCK(q, ew_launch(6, nb, t, r + c0, t, nullptr, 0.0, q->st));                 // t = r_k - L[k, <k] y
+                SCK(q, rowdot_launch(q->F + (size_t)c0 * q->ld, q->ld, y, nb, c0, t, q->st, &q->launches));
+                SCK(q, ew_launch(6, nb, t, r + c0, t, nullptr, 0.0, q->st, &q->launches));                 // t = r_k - L[k, <k] y
             } else {
                 SCK(q, cudaMemcpyAsync(t, r, sizeof(double) * nb, cudaMemcpyDeviceToDevice, q->st));
             }
@@ -581,9 +574,8 @@ int shard_solve(const Locals& L, double* gpb200_handle::*rhs, double* gpb200_han
             double* y = q->*ybuf; double* a = q->*out;
             double* t = q->tblk;
             if (r1 < Np) {
-                q->launches += 2;
-                SCK(q, rowdot_launch(q->F + (size_t)c0 * q->ld + r1, q->ld, a + r1, nb, Np - r1, t, q->st));
-                SCK(q, ew_launch(6, nb, t, y + c0, t, nullptr, 0.0, q->st));                 // t = y_k - U[k, >k] a
+                SCK(q, rowdot_launch(q->F + (size_t)c0 * q->ld + r1, q->ld, a + r1, nb, Np - r1, t, q->st, &q->launches));
+                SCK(q, ew_launch(6, nb, t, y + c0, t, nullptr, 0.0, q->st, &q->launches));                 // t = y_k - U[k, >k] a
             } else {
                 SCK(q, cudaMemcpyAsync(t, y + c0, sizeof(double) * nb, cudaMemcpyDeviceToDevice, q->st));
             }
@@ -651,8 +643,7 @@ int shard_inverse_la(const Locals& L) {
                 if (q->rank != o) continue;
                 cudaError_t e = cudaSuccess;
                 if (ncols > 0) {
-                    ++q->launches;
-                    e = shard_transpose(q->Sbuf + (size_t)r1 * NBp, NBp, q->G + (size_t)j0 * q->ld + r1, q->ld, nb, ncols, q->st);
+                    e = shard_transpose(q->Sbuf + (size_t)r1 * NBp, NBp, q->G + (size_t)j0 * q->ld + r1, q->ld, nb, ncols, q->st, &q->launches);
                     GemmDesc g = gemm_desc_default();
                     g.A = GemmOperand{bufS(q), bufNone(), r1, 0};
                     g.B = GemmOperand{bufG(q), bufDinvT(q), j0, j0};
@@ -663,8 +654,7 @@ int shard_inverse_la(const Locals& L) {
                     g.flags = GEMM_KLO_N;
                     if (e == cudaSuccess) e = launch_gemm(q, g);
                 }
-                ++q->launches;
-                if (e == cudaSuccess) e = shard_pack_wblock(q->P[2 * set], NBp, q->G, q->ld, q->Dinv, j0, nb, q->st);
+                if (e == cudaSuccess) e = shard_pack_wblock(q->P[2 * set], NBp, q->G, q->ld, q->Dinv, j0, nb, q->st, &q->launches);
                 if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
             }
             if (rc) break;
@@ -672,9 +662,8 @@ int shard_inverse_la(const Locals& L) {
                                  sizeof(double) * (size_t)(Np - j0) * NBp))) break;
             for (size_t i = 0; i < nl; ++i) {
                 gpb200_handle* q = L[i];
-                ++q->launches;
                 cudaError_t e = shard_transpose(q->XRbig[xb] + (size_t)(j0 - j0L) * Np + j0, Np, q->P[2 * set] + (size_t)j0 * NBp, NBp,
-                                                Np - j0, nb, q->st);
+                                                Np - j0, nb, q->st, &q->launches);
                 if (e == cudaSuccess && k > 0 && q->rank == (k - 1) % R) {
                     // narrow TRTRI update: the accumulator rows of block k-1 (the next panel to be finalised)
                     if (ev_trtri1[i]) e = cudaStreamWaitEvent(q->st, ev_trtri1[i], 0);           // main(k+1)'s TRTRI part adds into the same rows
@@ -748,7 +737,7 @@ int shard_predict_solve(const Locals& L, int Mpad, int64_t Mc, bool want_var, bo
         }
         SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->P[0]; }, sizeof(double) * (size_t)Mpad * NBp));
         for (auto* q : L) {
-            if (want_var) { ++q->launches; SCK(q, rowvar_launch(q->P[0], NBp, q->pvar, Mc, nb, q->pvar, q->st)); }
+            if (want_var) SCK(q, rowvar_launch(q->P[0], NBp, q->pvar, Mc, nb, q->pvar, q->st, &q->launches));
             if (r1 < Np) {
                 GemmDesc g = gemm_desc_default();
                 g.A = GemmOperand{bufP(q, 0), bufNone(), 0, 0};

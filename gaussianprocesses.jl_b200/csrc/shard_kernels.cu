@@ -82,53 +82,60 @@ __global__ void min_ranks_kernel(int* __restrict__ out, const int* __restrict__ 
 }
 }  // namespace
 
-cudaError_t shard_copy_lower(double* dst, int64_t ldd, const double* src, int64_t lds, int n, cudaStream_t st) {
+cudaError_t shard_copy_lower(double* dst, int64_t ldd, const double* src, int64_t lds, int n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     dim3 grid((n + 127) / 128, n);
     copy_lower_kernel<<<grid, 128, 0, st>>>(dst, ldd, src, lds, n);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t shard_scatter_rows(const double* G, double* F, int64_t ld, int64_t Npad, int c0, int nb, int t1, double* S_me,
-                               int nbp, ShardOwn own, cudaStream_t st) {
+                               int nbp, ShardOwn own, cudaStream_t st, int64_t* launches) {
     const long long n_tiles = Npad / T;
     if (t1 >= n_tiles || nb <= 0) return cudaSuccess;
     dim3 grid((nb + 127) / 128, (unsigned)(n_tiles - t1));
     scatter_rows_kernel<<<grid, 256, 0, st>>>(G, F, ld, c0, nb, t1, S_me, nbp, own,
                                               shard_own_before(t1, own.me, own.rb, own.R), n_tiles);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t shard_unpack_panel(double* P, int nbp, int64_t Npad, int nb, int t1, const double* S, int64_t per_rank,
-                               ShardOwn own, cudaStream_t st) {
+                               ShardOwn own, cudaStream_t st, int64_t* launches) {
     const long long n_tiles = Npad / T;
     if (t1 >= n_tiles || nb <= 0) return cudaSuccess;
     dim3 grid((nb + 127) / 128, (unsigned)(n_tiles - t1));
     unpack_panel_kernel<<<grid, 256, 0, st>>>(P, nbp, nb, t1, S, per_rank, own, n_tiles);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t shard_transpose(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, cudaStream_t st) {
+cudaError_t shard_transpose(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, cudaStream_t st, int64_t* launches) {
     if (rows <= 0 || cols <= 0) return cudaSuccess;
     // grid.y is limited to 65535 blocks of 32 rows = 2M rows: enough for N <= 2^21
     dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32)), block(32, 8);
     transpose_kernel<<<grid, block, 0, st>>>(dst, ldd, src, lds, rows, cols);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t shard_pack_wblock(double* P, int nbp, const double* G, int64_t ld, const double* Dinv, int j0, int nb, cudaStream_t st) {
+cudaError_t shard_pack_wblock(double* P, int nbp, const double* G, int64_t ld, const double* Dinv, int j0, int nb, cudaStream_t st, int64_t* launches) {
     if (nb <= 0) return cudaSuccess;
     dim3 grid((nb + 127) / 128, nb);
     pack_wblock_kernel<<<grid, 128, 0, st>>>(P, nbp, G, ld, Dinv, j0, nb);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t shard_sum_ranks(double* out, const double* in, int64_t stride, int nranks, int64_t n, cudaStream_t st) {
+cudaError_t shard_sum_ranks(double* out, const double* in, int64_t stride, int nranks, int64_t n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     sum_ranks_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out, in, stride, nranks, n);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t shard_min_ranks(int* out, const int* in, int nranks, cudaStream_t st) {
+cudaError_t shard_min_ranks(int* out, const int* in, int nranks, cudaStream_t st, int64_t* launches) {
     min_ranks_kernel<<<1, 1, 0, st>>>(out, in, nranks);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

@@ -19,19 +19,19 @@ __host__ __device__ inline long long shard_own_before(long long t, int q, int rb
 }
 
 // dst (n x n, ld ldd) = lower triangle of src (ld lds), zeros above the diagonal
-cudaError_t shard_copy_lower(double* dst, int64_t ldd, const double* src, int64_t lds, int n, cudaStream_t st);
+cudaError_t shard_copy_lower(double* dst, int64_t ldd, const double* src, int64_t lds, int n, cudaStream_t st, int64_t* launches);
 // own tile rows t >= t1 (rows r >= 128*t1): F[r, c0..c0+nb) = G[r, c0..c0+nb);  S_me[(li(r)), 0..nb) = same (ld nbp),
 // li = local index of the row among this rank's rows >= 128*t1
 cudaError_t shard_scatter_rows(const double* G, double* F, int64_t ld, int64_t Npad, int c0, int nb, int t1, double* S_me,
-                               int nbp, ShardOwn own, cudaStream_t st);
+                               int nbp, ShardOwn own, cudaStream_t st, int64_t* launches);
 // all rows r >= 128*t1: P[r, 0..nb) = S[owner(r)][li(r)][0..nb) ; S regions of `per_rank` doubles each
 cudaError_t shard_unpack_panel(double* P, int nbp, int64_t Npad, int nb, int t1, const double* S, int64_t per_rank,
-                               ShardOwn own, cudaStream_t st);
+                               ShardOwn own, cudaStream_t st, int64_t* launches);
 // dst[j * ldd + i] = src[i * lds + j], i < rows, j < cols
-cudaError_t shard_transpose(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, cudaStream_t st);
+cudaError_t shard_transpose(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, cudaStream_t st, int64_t* launches);
 // P[(j0 + c), i] (ld nbp) = W_JJ[c, i] for c >= i (strictly-lower tiles from G, diagonal tiles from Dinv), 0 for c < i
-cudaError_t shard_pack_wblock(double* P, int nbp, const double* G, int64_t ld, const double* Dinv, int j0, int nb, cudaStream_t st);
+cudaError_t shard_pack_wblock(double* P, int nbp, const double* G, int64_t ld, const double* Dinv, int j0, int nb, cudaStream_t st, int64_t* launches);
 // out[i] = sum_q in[q * stride + i]  (fixed rank order), i < n
-cudaError_t shard_sum_ranks(double* out, const double* in, int64_t stride, int nranks, int64_t n, cudaStream_t st);
+cudaError_t shard_sum_ranks(double* out, const double* in, int64_t stride, int nranks, int64_t n, cudaStream_t st, int64_t* launches);
 // out[0] = min_q in[q]
-cudaError_t shard_min_ranks(int* out, const int* in, int nranks, cudaStream_t st);
+cudaError_t shard_min_ranks(int* out, const int* in, int nranks, cudaStream_t st, int64_t* launches);

@@ -155,7 +155,7 @@ __global__ void dfma_peak_kernel(double* out, int iters) {
 }
 }  // namespace
 
-cudaError_t fp64_peak_measure(cudaStream_t st, double* tflops) {
+cudaError_t fp64_peak_measure(cudaStream_t st, int64_t* launches, double* tflops) {
     int dev = 0, sms = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -169,10 +169,12 @@ cudaError_t fp64_peak_measure(cudaStream_t st, double* tflops) {
     for (int rep = 0; rep < 3; ++rep) {
         cudaEventRecord(e0, st);
         dmma_peak_kernel<<<sms, warps * 32, 0, st>>>(out, iters);
+        if (launches) ++*launches;
         cudaEventRecord(e1, st); cudaEventSynchronize(e1);
         float ms; cudaEventElapsedTime(&ms, e0, e1); if (rep && ms < best[0]) best[0] = ms;
         cudaEventRecord(e0, st);
         dfma_peak_kernel<<<sms, warps * 32, 0, st>>>(out, iters);
+        if (launches) ++*launches;
         cudaEventRecord(e1, st); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1); if (rep && ms < best[1]) best[1] = ms;
     }
@@ -260,47 +262,55 @@ __global__ void fitc_wuu_kernel(double* __restrict__ Wuu, const double* __restri
     if (i < n && j < n) Wuu[i * ld + j] = T[i * ld + j] - beta[i] * beta[j] + Kinv[i * ld + j] - Sinv[i * ld + j];
 }
 }  // namespace
-cudaError_t rowdot2_launch(const double* A, const double* B, int64_t ld, int64_t nrows, int64_t ncols, double* q, cudaStream_t st) {
+cudaError_t rowdot2_launch(const double* A, const double* B, int64_t ld, int64_t nrows, int64_t ncols, double* q, cudaStream_t st, int64_t* launches) {
     if (nrows <= 0) return cudaSuccess;
     rowdot2_kernel<<<(unsigned)nrows, 256, 0, st>>>(A, B, ld, ncols, q);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t fitc_g_launch(int64_t n, const double* alpha, const double* lam, const double* q, double* g, cudaStream_t st) {
+cudaError_t fitc_g_launch(int64_t n, const double* alpha, const double* lam, const double* q, double* g, cudaStream_t st, int64_t* launches) {
     fitc_g_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, alpha, lam, q, g);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t fitc_wfu_launch(double* P2, const double* P1, int64_t ld, int64_t nrows, int64_t ncols, const double* alpha,
-                            const double* lam, const double* g, const double* beta, cudaStream_t st) {
+                            const double* lam, const double* g, const double* beta, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
     fitc_wfu_kernel<<<grid, 256, 0, st>>>(P2, P1, ld, nrows, ncols, alpha, lam, g, beta);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t colscale_launch(double* A, int64_t ld, int64_t nrows, int64_t ncols, const double* v, cudaStream_t st) {
+cudaError_t colscale_launch(double* A, int64_t ld, int64_t nrows, int64_t ncols, const double* v, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
     colscale_kernel<<<grid, 256, 0, st>>>(A, ld, nrows, ncols, v);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t symmetrize_launch(double* A, int64_t ld, int64_t n, cudaStream_t st) {
+cudaError_t symmetrize_launch(double* A, int64_t ld, int64_t n, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)((n + 255) / 256), (unsigned)n);
     symmetrize_kernel<<<grid, 256, 0, st>>>(A, ld, n);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t fitc_wuu_launch(double* Wuu, const double* T, const double* Kinv, const double* Sinv, int64_t ld, int64_t n,
-                            const double* beta, cudaStream_t st) {
+                            const double* beta, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)((n + 255) / 256), (unsigned)n);
     fitc_wuu_kernel<<<grid, 256, 0, st>>>(Wuu, T, Kinv, Sinv, ld, n, beta);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t ew_launch(int op, int64_t n, double* out, const double* a, const double* b, const double* c, double s, cudaStream_t st) {
+cudaError_t ew_launch(int op, int64_t n, double* out, const double* a, const double* b, const double* c, double s, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     ew_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, n, out, a, b, c, s);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t scale_launch(int mode, double* A, int64_t ld, int64_t nrows, int64_t ncols, const double* v, cudaStream_t st) {
+cudaError_t scale_launch(int mode, double* A, int64_t ld, int64_t nrows, int64_t ncols, const double* v, cudaStream_t st, int64_t* launches) {
     if (nrows <= 0 || ncols <= 0) return cudaSuccess;
     dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
     scale_kernel<<<grid, 256, 0, st>>>(mode, A, ld, nrows, ncols, v);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
@@ -476,26 +486,31 @@ cudaError_t trsv_lower_bwd(const double* F, int64_t ldf, const double* DinvT, do
     }
     return cudaGetLastError();
 }
-cudaError_t dot_launch(const double* a, const double* b, int64_t n, double* out, cudaStream_t st) {
+cudaError_t dot_launch(const double* a, const double* b, int64_t n, double* out, cudaStream_t st, int64_t* launches) {
     dot_kernel<<<1, 1024, 0, st>>>(a, b, n, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t sum_launch(const double* a, int64_t n, double* out, cudaStream_t st) {
+cudaError_t sum_launch(const double* a, int64_t n, double* out, cudaStream_t st, int64_t* launches) {
     sum_kernel<<<1, 1024, 0, st>>>(a, n, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t rowdot_launch(const double* Kst, int64_t ldk, const double* alpha, int64_t M, int64_t N, double* mu, cudaStream_t st) {
+cudaError_t rowdot_launch(const double* Kst, int64_t ldk, const double* alpha, int64_t M, int64_t N, double* mu, cudaStream_t st, int64_t* launches) {
     if (M <= 0) return cudaSuccess;
     rowdot_kernel<<<(unsigned)M, 256, 0, st>>>(Kst, ldk, alpha, N, mu);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t rowvar_launch(const double* Vt, int64_t ldk, const double* kdiag, int64_t M, int64_t N, double* var, cudaStream_t st) {
+cudaError_t rowvar_launch(const double* Vt, int64_t ldk, const double* kdiag, int64_t M, int64_t N, double* var, cudaStream_t st, int64_t* launches) {
     if (M <= 0) return cudaSuccess;
     rowvar_kernel<<<(unsigned)M, 256, 0, st>>>(Vt, ldk, kdiag, N, var);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t exp2x_launch(const double* ln, int64_t n, double* out, cudaStream_t st) {
+cudaError_t exp2x_launch(const double* ln, int64_t n, double* out, cudaStream_t st, int64_t* launches) {
     exp2x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ln, n, out);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
@@ -516,14 +531,16 @@ __global__ void add_rowvec_kernel(double* __restrict__ A, long long ld, const do
     if (j < ncols && i < nrows) A[i * ld + j] += v[j];
 }
 }  // namespace
-cudaError_t spd_from_cov_launch(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t n, int64_t npad, double nugget, cudaStream_t st) {
+cudaError_t spd_from_cov_launch(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t n, int64_t npad, double nugget, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)((npad + 255) / 256), (unsigned)npad);
     spd_from_cov_kernel<<<grid, 256, 0, st>>>(dst, ldd, src, lds, n, npad, nugget);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t add_rowvec_launch(double* A, int64_t ld, const double* v, int64_t nrows, int64_t ncols, cudaStream_t st) {
+cudaError_t add_rowvec_launch(double* A, int64_t ld, const double* v, int64_t nrows, int64_t ncols, cudaStream_t st, int64_t* launches) {
     dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
     add_rowvec_kernel<<<grid, 256, 0, st>>>(A, ld, v, nrows, ncols);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }
 
@@ -533,9 +550,10 @@ __global__ void gather_block_kernel(double* __restrict__ out, const double* __re
     if (b < nv) out[a * nv + b] = src[idx[a] * ld + idx[b]];
 }
 }  // namespace
-cudaError_t gather_block_launch(double* out, const double* src, int64_t ld, const long long* idx, int64_t nv, cudaStream_t st) {
+cudaError_t gather_block_launch(double* out, const double* src, int64_t ld, const long long* idx, int64_t nv, cudaStream_t st, int64_t* launches) {
     if (nv <= 0) return cudaSuccess;
     dim3 grid((unsigned)((nv + 255) / 256), (unsigned)nv);
     gather_block_kernel<<<grid, 256, 0, st>>>(out, src, ld, idx, nv);
+    if (launches) ++*launches;
     return cudaGetLastError();
 }

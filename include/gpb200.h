@@ -159,7 +159,8 @@ int  gpb200_get_inverse_diag(gpb200_handle* h, double* diag);
  * [6] number of DMMA GEMM launches  [7] sum of their device durations (ms, CUDA events around
  * every launch)  [8] FP64 flops those launches executed (tile-granular)                       */
 int  gpb200_get_timings(gpb200_handle* h, double* ms, int32_t n);
-/* number of kernel launches issued by this handle since creation */
+/* number of kernels enqueued by calls on this handle since creation (gpb200_rand includes its M x M sub-engine's
+ * Cholesky); cudaMemsetAsync and copies are not counted */
 int64_t gpb200_launch_count(gpb200_handle* h);
 /* tuning knobs (string key):
  *   "nb"         outer Cholesky block: 0 (default) = fully recursive, else 128*2^k <= 4096 (right-looking panels)
@@ -281,6 +282,8 @@ int  gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* bloc
  * grouped by block and each group padded to a multiple of 128, to fit one staging chunk (GPB200_EINVAL otherwise).      */
 int  gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
                              double* mu_minus_mean, double* var, double* cov);
+/* number of kernels enqueued by calls on this handle since creation, on both M x M sub-engines; cudaMemsetAsync and
+ * copies are not counted */
 int64_t gpb200_fitc_launch_count(gpb200_fitc* f);
 
 #ifdef __cplusplus
