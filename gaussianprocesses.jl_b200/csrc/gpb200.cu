@@ -45,6 +45,7 @@
 #include "shard_kernels.cuh"
 #include "vec.cuh"
 #include "fsa.cuh"
+#include "gpa.cuh"
 
 namespace {
 constexpr int TILE = 128;
@@ -63,7 +64,7 @@ struct VmBuf {
 struct gpb200_handle {
     int device = 0;
     cudaStream_t st = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr;
     int64_t N = 0, Npad = 0, ld = 0;
     int d = 0;
     double* x = nullptr;
@@ -74,6 +75,8 @@ struct gpb200_handle {
     double *noise_var = nullptr, *r0 = nullptr, *r1 = nullptr, *y1 = nullptr, *alpha = nullptr, *scal = nullptr;
     double *part = nullptr, *trace_out = nullptr;
     double* tblk = nullptr;                    // Npad scratch vector (block right-hand sides of the sharded solves)
+    double* ZdT = nullptr;                     // gpb200_gpa_grad: Npad x 128 clean upper diagonal tiles of Z' (allocated on first use)
+    CUtensorMap mapZdT{};
     // TMA-staged SEIso kernels (gram_fast.cu): inputs stored [Npad x dxp] with an even, zero-padded dxp <= 8
     double *xp = nullptr, *xpt = nullptr;      // [Npad x dxp] and its transpose [dxp x Npad]
     int dxp = 0;
@@ -287,7 +290,7 @@ void free_data(gpb200_handle* h) {
     free_FG(h);
     double** ptrs[] = {&h->x, &h->Dinv, &h->DinvT, &h->logd, &h->noise_var, &h->r0, &h->r1,
                        &h->y1, &h->alpha, &h->scal, &h->part, &h->trace_out, &h->xs, &h->Kst, &h->Kss,
-                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt};
+                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt, &h->ZdT};
     h->xmap_ok = false;
     if (h->cvD) cudaFree(h->cvD);
     if (h->cvY) cudaFree(h->cvY);
@@ -493,9 +496,9 @@ cudaError_t cholesky(gpb200_handle* h) {
     return cudaSuccess;
 }
 
-// K_y^-1 from the factor: level-parallel triangular inverse (all pairs of adjacent s x s diagonal
-// blocks merged at once, s = 128, 256, ...: 2 batched GEMM launches per level), then W'W.
-cudaError_t inverse_from_factor(gpb200_handle* h) {
+// W = L^-1 from the factor: level-parallel triangular inverse (all pairs of adjacent s x s diagonal blocks merged at once,
+// s = 128, 256, ...: 2 batched GEMM launches per level).  Leaves W in G's strict-lower tiles and W' in its strict-upper tiles.
+cudaError_t inverse_merges(gpb200_handle* h) {
     const int Np = (int)h->Npad;
     cudaError_t e;
     for (long long s = TILE; s < Np; s *= 2) {
@@ -503,6 +506,14 @@ cudaError_t inverse_from_factor(gpb200_handle* h) {
         const int n2 = (int)((Np - s < s) ? Np - s : s);
         if ((e = merge_inverse(h, 0, (int)s, n2, batch)) != cudaSuccess) return e;
     }
+    return cudaSuccess;
+}
+
+// K_y^-1 from the factor: the merges, then W'W.
+cudaError_t inverse_from_factor(gpb200_handle* h) {
+    const int Np = (int)h->Npad;
+    cudaError_t e;
+    if ((e = inverse_merges(h)) != cudaSuccess) return e;
     GemmDesc g = gemm_desc_default();
     g.A = GemmOperand{bufG(h), bufDinvT(h), 0, 0};
     g.B = GemmOperand{bufG(h), bufDinvT(h), 0, 0};
@@ -1033,7 +1044,7 @@ int gpb200_create(gpb200_handle** out, int device) {
     };
     if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
     if ((e = cudaStreamCreateWithFlags(&h->st, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
-    cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1); cudaEventCreate(&h->ev2); cudaEventCreate(&h->ev3);
+    cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1); cudaEventCreate(&h->ev2); cudaEventCreate(&h->ev3); cudaEventCreate(&h->ev4);
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -1068,6 +1079,7 @@ void gpb200_destroy(gpb200_handle* h) {
     if (h->ev1) cudaEventDestroy(h->ev1);
     if (h->ev2) cudaEventDestroy(h->ev2);
     if (h->ev3) cudaEventDestroy(h->ev3);
+    if (h->ev4) cudaEventDestroy(h->ev4);
     if (h->ev_la0) cudaEventDestroy(h->ev_la0);
     if (h->ev_la2) cudaEventDestroy(h->ev_la2);
     if (h->st_side) cudaStreamDestroy(h->st_side);
@@ -1483,6 +1495,84 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     h->ms[4] = ev_ms(h->ev0, h->ev1);
     if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = out[p];
     if (trA) *trA = out[np];
+    return GPB200_OK;
+}
+
+// ---- GPA (src/GPA.jl): whitened latent variables f = L v + mu, gradient through the Cholesky factor ------------------------
+static int gpa_check(gpb200_handle* h, const char* who) {
+    if (h->nranks > 1 || h->sharded || h->grp) return fail(h, GPB200_EINVAL, (std::string(who) + ": single-GPU handles only").c_str());
+    if (!h->factored) return fail(h, GPB200_ESTATE, (std::string(who) + ": factorize first").c_str());
+    return GPB200_OK;
+}
+
+int gpb200_unwhiten(gpb200_handle* h, const double* v, double* f) {
+    if (!h) return GPB200_EINVAL;
+    if (!v || !f) return fail(h, GPB200_EINVAL, "unwhiten: null v or f");
+    int rc = gpa_check(h, "unwhiten");
+    if (rc) return rc;
+    CK(cudaSetDevice(h->device));
+    if ((rc = upload_padded(h, h->r0, v))) return rc;
+    CK(gpa_trmv_launch(h->F, h->ld, h->r0, h->y1, h->Npad, h->st, &h->launches));
+    CK(cudaMemcpyAsync(f, h->y1, sizeof(double) * h->N, cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
+    return GPB200_OK;
+}
+
+// u = L' g; then, for the kernel gradient, W = L^-1 (the inverse merges), Z' by the scans of gpa.cu, G_lower = -S = -W' Z (one
+// NT GEMM with the k range of K^-1 = W'W), and the trace kernels with alpha = 0 (A = alpha alpha' - G = S): 1/2 sum S dK.
+int gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, double* dll_process, double* dll_kernel) {
+    if (!h) return GPB200_EINVAL;
+    if (!v || !dl_df) return fail(h, GPB200_EINVAL, "gpa_grad: null v or dl_df");
+    int rc = gpa_check(h, "gpa_grad");
+    if (rc) return rc;
+    CK(cudaSetDevice(h->device));
+    if ((rc = upload_padded(h, h->r0, v))) return rc;
+    if ((rc = upload_padded(h, h->r1, dl_df))) return rc;
+    CK(gpa_trmv_t_launch(h->F, h->ld, h->r1, h->y1, h->Npad, h->st, &h->launches));
+    if (dll_process) CK(cudaMemcpyAsync(dll_process, h->y1, sizeof(double) * h->N, cudaMemcpyDeviceToHost, h->st));
+    if (!dll_kernel) {
+        CK(cudaStreamSynchronize(h->st));
+        return GPB200_OK;
+    }
+    // G and F's strict-upper tiles are overwritten: K^-1, its mirror, M_j and alpha are gone
+    h->inv_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
+    const int Np = (int)h->Npad;
+    if (!h->ZdT) {
+        CK(cudaMalloc(&h->ZdT, sizeof(double) * h->Npad * TILE));
+        if (h->tma_ok && !gemm_make_tensor_map(&h->mapZdT, h->ZdT, h->Npad, TILE, TILE)) {
+            cudaFree(h->ZdT); h->ZdT = nullptr;
+            return fail(h, GPB200_ECUDA, "gpa_grad: cuTensorMapEncodeTiled failed for the diagonal tiles of Z'");
+        }
+    }
+    CK(cudaEventRecord(h->ev0, h->st));
+    CK(inverse_merges(h));
+    CK(cudaEventRecord(h->ev1, h->st));
+    CK(gpa_scan_launch(h->G, h->ld, h->DinvT, h->y1, h->r0, h->F, h->ZdT, h->Npad, h->st, &h->launches));
+    CK(cudaEventRecord(h->ev2, h->st));
+    {
+        GemmDesc g = gemm_desc_default();                       // G[a,b] = -sum_{i >= a} W'[a,i] Z'[b,i]   (a >= b)
+        g.A = GemmOperand{bufG(h), bufDinvT(h), 0, 0};
+        g.B = GemmOperand{bufF(h), GemmBuf{h->tma_ok ? &h->mapZdT : nullptr, h->ZdT, TILE}, 0, 0};
+        g.C = h->G; g.ldc = h->ld; g.c_row0 = 0; g.c_col0 = 0;
+        g.M = Np; g.N = Np; g.K = Np;
+        g.alpha = -1.0;
+        g.flags = GEMM_LOWER_ONLY | GEMM_KLO_M;
+        CK(launch_gemm(h, g));
+    }
+    CK(cudaEventRecord(h->ev3, h->st));
+    CK(cudaMemsetAsync(h->alpha, 0, sizeof(double) * h->Npad, h->st));
+    CK(launch_trace(h, 1, 0, 1));
+    CK(cudaEventRecord(h->ev4, h->st));
+    const int np = h->prog.n_theta;
+    std::vector<double> out((size_t)np + 1);
+    CK(cudaMemcpyAsync(out.data(), h->trace_out, sizeof(double) * (np + 1), cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
+    profile_collect(h);
+    h->ms[3] = ev_ms(h->ev0, h->ev1);
+    h->ms[9] = ev_ms(h->ev1, h->ev2);
+    h->ms[10] = ev_ms(h->ev2, h->ev3);
+    h->ms[4] = ev_ms(h->ev3, h->ev4);
+    for (int p = 0; p < np; ++p) dll_kernel[p] = out[p];
     return GPB200_OK;
 }
 

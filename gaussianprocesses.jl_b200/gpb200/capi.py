@@ -40,6 +40,8 @@ _SIGNATURES = {
     "gpb200_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
     "gpb200_rand": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, C.c_int64, _dp, C.c_double, _dp, _dp]),
     "gpb200_append": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
+    "gpb200_unwhiten": (C.c_int, [_H, _dp, _dp]),
+    "gpb200_gpa_grad": (C.c_int, [_H, _dp, _dp, _dp, _dp]),
     "gpb200_cv_param": (C.c_int, [_H, C.c_int32, _dp, _dp, _dp]),
     "gpb200_cv_block": (C.c_int, [_H, C.c_int32, C.c_int64, C.POINTER(C.c_int64), _dp]),
     "gpb200_get_gram": (C.c_int, [_H, _dp]),
@@ -246,6 +248,28 @@ class Engine:
         self._check(self._lib.gpb200_append(self._h, k, _as_dp(xnew_pm), d), "append")
         self.N += k
 
+    def unwhiten(self, v):
+        """f = L v with L the factor of the last factorize (GPA's latent variables, src/GPA.jl:106,125)."""
+        v = np.ascontiguousarray(v, dtype=np.float64)
+        if v.shape != (self.N,):
+            raise ValueError("unwhiten: v must have length N")
+        f = np.empty(self.N)
+        self._check(self._lib.gpb200_unwhiten(self._h, _as_dp(v), _as_dp(f)), "unwhiten")
+        return f
+
+    def gpa_grad(self, v, dl_df, process=True, kern=True):
+        """GPA gradient pieces (src/GPA.jl:164-173, 200): (L' dl_df or None, full kernel-parameter gradient or None).
+        The kernel part overwrites K^-1 and the resident alpha on the device."""
+        v = np.ascontiguousarray(v, dtype=np.float64)
+        g = np.ascontiguousarray(dl_df, dtype=np.float64)
+        if v.shape != (self.N,) or g.shape != (self.N,):
+            raise ValueError("gpa_grad: v and dl_df must have length N")
+        u = np.empty(self.N) if process else None
+        gk = np.empty(max(self.n_theta, 1)) if kern else None
+        self._check(self._lib.gpb200_gpa_grad(self._h, _as_dp(v), _as_dp(g), _as_dp(u) if process else None,
+                                              _as_dp(gk) if kern else None), "gpa_grad")
+        return u, (gk[:self.n_theta].copy() if kern else None)
+
     def cv_param(self, param, alpha=None):
         """(Z_j alpha, diag(Z_j K^-1)) for kernel parameter `param` (index into the full parameter vector) or -1 = noise."""
         za, dg = np.empty(self.N), np.empty(self.N)
@@ -297,7 +321,7 @@ class Engine:
         ms = np.zeros(12)
         self._check(self._lib.gpb200_get_timings(self._h, _as_dp(ms), 12), "get_timings")
         return dict(gram=ms[0], cholesky=ms[1], solve_mll=ms[2], inverse=ms[3], trace=ms[4], predict=ms[5],
-                    gemm_launches=ms[6], gemm_ms=ms[7], gemm_flops=ms[8])
+                    gemm_launches=ms[6], gemm_ms=ms[7], gemm_flops=ms[8], gpa_scan=ms[9], gpa_product=ms[10])
 
     def set_stream(self, cuda_stream):
         """Run on the caller's CUDA stream (int handle, e.g. torch.cuda.current_stream().cuda_stream); 0/None = private."""

@@ -399,6 +399,10 @@ class GPE:
 
 
 def GP(x, y, mean, kernel, logNoise=-2.0, **kw):                   # GPE.jl:119
+    from .likelihoods import Likelihood
+    if isinstance(logNoise, Likelihood):                           # GP(x, y, mean, kernel, lik) == GPA (GPA.jl:93-94)
+        from .gpa import GPA
+        return GPA(x, y, mean, kernel, logNoise, **kw)
     return GPE(x, y, mean, kernel, logNoise, **kw)
 
 

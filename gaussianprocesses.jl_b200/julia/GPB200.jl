@@ -120,7 +120,7 @@ dim(a::B200PDMat) = a.n
 
 # update_cK! (src/GPE.jl:169-186).  Two methods, typed like the reference's pair (logNoise::Real / ::AbstractVector)
 # so that they are strictly more specific than update_cK!(::AbstractPDMat, ..., ::CovarianceStrategy).
-function b200_update!(cK::B200PDMat, x::AbstractMatrix, kernel::Kernel, ln::Vector{Float64})
+function b200_update!(cK::B200PDMat, x::AbstractMatrix, kernel::Kernel, ln::Vector{Float64}; nugget::Float64 = 0.0)
     d, n = size(x)
     if objectid(x) != cK.xid || (d, n) != cK.xsize       # fit!/push!/append! replace or grow x; optimiser steps do not
         X = Matrix{Float64}(x)                   # Adjoint / SubArray / ElasticArray -> dense d x N (gotcha 1)
@@ -136,7 +136,7 @@ function b200_update!(cK::B200PDMat, x::AbstractMatrix, kernel::Kernel, ln::Vect
     end
     cK.exposed = exposed; cK.ntheta = length(theta)
     check(cK, ccall((:gpb200_factorize, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Int64, Float64),
-                    cK.handle, theta, ln, length(ln), 0.0), "factorize")          # rc > 0 -> PosDefException
+                    cK.handle, theta, ln, length(ln), nugget), "factorize")       # rc > 0 -> PosDefException
     return cK
 end
 update_cK!(cK::B200PDMat, x::AbstractMatrix, kernel::Kernel, logNoise::Real, data::KernelData, ::B200Covariance) =
@@ -495,6 +495,150 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::Abs
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
 end
 
-export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE
+# ---- GPA: non-Gaussian likelihoods (src/GPA.jl) ----------------------------------------------------------------------------
+# The reference's GPA types cK as PDMat{Float64,Matrix{Float64}} (GPA.jl:33), so a device factor cannot be slotted into it.
+# B200GPA carries GPA's fields and methods over a B200PDMat; the likelihoods are the reference's own (log_dens,
+# dlog_dens_df, dlog_dens_dθ, predict_obs), only the factor, f = L v and the gradient through the factor are on the device.
+# mcmc / ess / optimize! drive it through get_params / set_params! / update_target_and_dtarget! like a GPA.
+import GaussianProcesses: GPBase, Likelihood, log_dens, dlog_dens_df, dlog_dens_dθ, predict_obs, set_params!, predict_y,
+                          update_target_and_dtarget!, get_params_kwargs, grad_stack
+
+mutable struct B200GPA{X<:AbstractMatrix,Y<:AbstractVector,M<:Mean,K<:Kernel,L<:Likelihood} <: GPBase
+    x::X
+    y::Y
+    mean::M
+    kernel::K
+    lik::L
+    dim::Int
+    nobs::Int
+    v::Vector{Float64}            # whitened latent variables, f = L v + μ
+    μ::Vector{Float64}
+    cK::B200PDMat
+    ll::Float64
+    dll::Vector{Float64}
+    target::Float64
+    dtarget::Vector{Float64}
+end
+
+function B200GPA(x::AbstractMatrix, y::AbstractVector{<:Real}, mean::Mean, kernel::Kernel, lik::Likelihood; device::Int = 0)
+    dim, nobs = size(x)
+    length(y) == nobs || throw(ArgumentError("Input and output observations must have consistent dimensions."))   # GPA.jl:45
+    gp = B200GPA(x, y, mean, kernel, lik, dim, nobs, zeros(nobs), zeros(nobs), B200PDMat(device, nobs), NaN, Float64[], NaN,
+                 Float64[])
+    return initialise_target!(gp)
+end
+
+# f = L v (gpb200_unwhiten): unwhiten(gp.cK, gp.v) of GPA.jl:106,125,159,294
+function unwhiten_dev(cK::B200PDMat, v::AbstractVector)
+    f = Vector{Float64}(undef, cK.n)
+    check(cK, ccall((:gpb200_unwhiten, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}), cK.handle, Vector{Float64}(v), f), "unwhiten")
+    return f
+end
+
+function initialise_target!(gp::B200GPA)                                           # GPA.jl:101-109, 245-250
+    gp.μ = mean(gp.mean, gp.x)
+    b200_update!(gp.cK, gp.x, gp.kernel, Float64[-400.0]; nugget=1e-6)             # PDMat(Σ + 1e-6 I): exp(-800) == 0
+    gp.ll = sum(log_dens(gp.lik, unwhiten_dev(gp.cK, gp.v) + gp.μ, gp.y))
+    gp.target = gp.ll - (sum(abs2, gp.v) + log(2π) * gp.nobs) / 2
+    return gp
+end
+
+function update_target!(gp::B200GPA; process::Bool=true, lik::Bool=true, domean::Bool=true, kern::Bool=true)   # GPA.jl:261-266
+    kern && b200_update!(gp.cK, gp.x, gp.kernel, Float64[-20.0])                  # update_cK!(::GPA), GPA.jl:111-114
+    gp.μ = mean(gp.mean, gp.x)
+    gp.ll = sum(log_dens(gp.lik, unwhiten_dev(gp.cK, gp.v) + gp.μ, gp.y))
+    gp.target = gp.ll - (sum(abs2, gp.v) + log(2π) * gp.nobs) / 2
+    return gp
+end
+
+# update_dll! + update_dtarget! (GPA.jl:183-228, 268-272): [L' dl_df; Σ dlog_dens_dθ; dmll_mean!; dll_kern!] - [v; 0...]
+function update_dtarget!(gp::B200GPA; process::Bool=true, lik::Bool=true, domean::Bool=true, kern::Bool=true)
+    cK = gp.cK
+    f = unwhiten_dev(cK, gp.v) + gp.μ
+    dl_df = Vector{Float64}(dlog_dens_df(gp.lik, f, gp.y))
+    u = Vector{Float64}(undef, gp.nobs)
+    gk = Vector{Float64}(undef, max(cK.ntheta, 1))
+    if process || kern
+        if process && kern
+            check(cK, ccall((:gpb200_gpa_grad, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                            cK.handle, gp.v, dl_df, u, gk), "gpa_grad")
+        elseif process
+            check(cK, ccall((:gpb200_gpa_grad, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                            cK.handle, gp.v, dl_df, u, Ptr{Float64}(C_NULL)), "gpa_grad")
+        else
+            check(cK, ccall((:gpb200_gpa_grad, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                            cK.handle, gp.v, dl_df, Ptr{Float64}(C_NULL), gk), "gpa_grad")
+        end
+    end
+    dll = Float64[]
+    process && append!(dll, u)
+    if lik && num_params(gp.lik) > 0
+        append!(dll, vec(sum(dlog_dens_dθ(gp.lik, f, gp.y), dims=1)))
+    end
+    if domean && num_params(gp.mean) > 0
+        append!(dll, grad_stack(gp.mean, gp.x)' * dl_df)                          # dmll_mean!(dll, mean, x, dl_df)
+    end
+    kern && append!(dll, gk[cK.exposed])
+    gp.dll = dll
+    gp.dtarget = copy(dll)
+    process && (gp.dtarget[1:gp.nobs] .-= gp.v)                                    # prior_gradlogpdf: -v (GPA.jl:384-385)
+    return gp
+end
+
+function update_target_and_dtarget!(gp::B200GPA; kwargs...)                       # GPA.jl:283-291
+    update_target!(gp; kwargs...)
+    update_dtarget!(gp; kwargs...)
+end
+update_target_and_dtarget!(gp::B200GPA, precomp; kwargs...) = update_target_and_dtarget!(gp; kwargs...)   # mcmc.jl:17
+init_precompute(gp::B200GPA) = nothing
+get_params_kwargs(::B200GPA; kwargs...) = delete!(Dict(kwargs), :noise)           # optimize.jl:2
+
+function get_params(gp::B200GPA; lik::Bool=true, domean::Bool=true, kern::Bool=true)   # GPA.jl:336-349
+    params = copy(gp.v)
+    lik && num_params(gp.lik) > 0 && append!(params, get_params(gp.lik))
+    domean && num_params(gp.mean) > 0 && append!(params, get_params(gp.mean))
+    kern && append!(params, get_params(gp.kernel))
+    return params
+end
+
+function num_params(gp::B200GPA; lik::Bool=true, domean::Bool=true, kern::Bool=true)   # GPA.jl:351-357
+    n = length(gp.v)
+    lik && (n += num_params(gp.lik))
+    domean && (n += num_params(gp.mean))
+    kern && (n += num_params(gp.kernel))
+    return n
+end
+
+function set_params!(gp::B200GPA, hyp::AbstractVector; process::Bool=true, lik::Bool=true, domean::Bool=true, kern::Bool=true)
+    nl, nm, nk = num_params(gp.lik), num_params(gp.mean), num_params(gp.kernel)    # GPA.jl:359-381
+    i = 1
+    if process
+        gp.v = hyp[1:gp.nobs]; i += gp.nobs
+    end
+    if lik && nl > 0
+        set_params!(gp.lik, hyp[i:i+nl-1]); i += nl
+    end
+    if domean && nm > 0
+        set_params!(gp.mean, hyp[i:i+nm-1]); i += nm
+    end
+    if kern
+        set_params!(gp.kernel, hyp[i:i+nk-1]); i += nk
+    end
+end
+
+# predict_full(gp::GPA, x) (GPA.jl:294): alpha = cK \ unwhiten(cK, v), then the batched device predictMVN
+function predict_f(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)
+    alpha = gp.cK \ unwhiten_dev(gp.cK, gp.v)
+    μ, σ2 = predict_raw(gp.cK, x, alpha, full_cov)
+    μ .+= mean(gp.mean, x)
+    return full_cov ? (μ, σ2) : (μ, max.(σ2, 0.0))                                 # GP.jl:75
+end
+
+function predict_y(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)        # GPA.jl:303-306
+    μ, σ2 = predict_f(gp, x; full_cov=full_cov)
+    return predict_obs(gp.lik, μ, σ2)
+end
+
+export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA
 
 end # module

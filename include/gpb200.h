@@ -136,6 +136,20 @@ int  gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, co
  * gpb200_set_data; GPB200_EINVAL when the capacity is exceeded (the shim refits, like ElasticPDMats.resize!).             */
 int  gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx);
 
+/* ---- GPA: GP with a non-Gaussian likelihood (src/GPA.jl), latent f = L v + mu over K = L L' ---------------------------------
+ * The likelihood stays on the host (O(N)); the handle supplies the O(N^2) / O(N^3) pieces.  Call gpb200_factorize first
+ * (update_cK!(::GPA), GPA.jl:111-114: log_noise = -20).  Single GPU: GPB200_EINVAL on multi-rank, row-sharded and grouped
+ * handles; GPB200_ESTATE before factorize.                                                                                  */
+/* unwhiten(cK, v) (src/GPA.jl:106,125,159,294): f[N] = L v, L the factor of the last gpb200_factorize */
+int  gpb200_unwhiten(gpb200_handle* h, const double* v, double* f);
+/* GPA gradient (src/GPA.jl:164-173,200; src/chol_utils.jl:15-39), after gpb200_factorize:
+ * dll_process[N] = L' dl_df (may be NULL); dll_kernel[P] = dll_kern! for Lbar = tril(dl_df v') (may be NULL: no O(N^3) work).
+ * The kernel gradient is 1/2 sum_ij S_ij dK_ij/dtheta_p with S = W' M_s W, W = L^-1, M_s[i,j] = u[max(i,j)] v[min(i,j)],
+ * u = L' dl_df: the inverse merges, two scans and one triangular NT GEMM (N^3/3 + N^3/3 flop) instead of the reference's
+ * level-2 reverse pass.  It overwrites K_y^-1 and the resident alpha: grad_kernel / cv_* then need grad_prepare / mll again
+ * (GPB200_ESTATE otherwise).  The factor, logdet, solve, mll, predict, rand and append are unaffected.                   */
+int  gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, double* dll_process, double* dll_kernel);
+
 /* ---- cross-validation on the resident inverse (src/crossvalidation.jl; after gpb200_grad_prepare, single GPU) ------------
  * Per hyper-parameter the reference forms Z_j = inv(Sigma) dK_j and Z_j inv(Sigma) as host matrices (crossvalidation.jl:86-108,
  * 270-283).  gpb200_cv_param does the two N^3 products on the device and returns the two vectors the LOO formulas need:
@@ -154,7 +168,8 @@ int  gpb200_get_inverse(gpb200_handle* h, double* Kinv);  /* N x N, after gpb200
  * (src/crossvalidation.jl:8-13, 37-49: sigma_i^2 = 1/[K^-1]_ii, mu_i = y_i - alpha_i sigma_i^2)  */
 int  gpb200_get_inverse_diag(gpb200_handle* h, double* diag);
 /* per-phase device times (ms) of the last calls:
- * [0] gram  [1] cholesky  [2] solve+mll  [3] inverse (trtri+lauum)  [4] trace  [5] predict
+ * [0] gram  [1] cholesky  [2] solve+mll  [3] inverse (trtri+lauum; gpb200_gpa_grad: the merges only)  [4] trace  [5] predict
+ * [9] gpb200_gpa_grad's scans  [10] its S = W'Z GEMM
  * with option "profile"=1, accumulated since the option was set:
  * [6] number of DMMA GEMM launches  [7] sum of their device durations (ms, CUDA events around
  * every launch)  [8] FP64 flops those launches executed (tile-granular)                       */
