@@ -73,8 +73,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) fsa_gemm_kernel(const FsaGemm
             double* cp = it.C + (long long)r * it.ldc + c;
             double v0 = it.alpha * acc[i][j][0], v1 = it.alpha * acc[i][j][1];
             if (it.beta != 0.0) {
+                // rounded as gemm_nt.cu's epilogue (alpha * acc, then one fma with beta * C): left to contraction, some
+                // paths of this kernel became fma(alpha, acc, beta * C) and differed from the NT GEMM in the last bit
                 const double2 old = *reinterpret_cast<const double2*>(cp);
-                v0 += it.beta * old.x; v1 += it.beta * old.y;
+                v0 = fma(it.beta, old.x, v0); v1 = fma(it.beta, old.y, v1);
             }
             if (!it.lower || c + 1 <= r) *reinterpret_cast<double2*>(cp) = make_double2(v0, v1);
             else if (c <= r) cp[0] = v0;

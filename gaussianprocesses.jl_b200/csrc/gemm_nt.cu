@@ -455,6 +455,11 @@ cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream, int
     p.alpha = d.alpha; p.beta = d.beta;
     if (d.M <= 0 || d.N <= 0) return cudaSuccess;
     if ((d.M % BM) || (d.N % BN) || (d.K % BK)) return cudaErrorInvalidValue;
+    // the diagonal mask applies to C only: a peer copy or Ct of a LOWER_ONLY launch would get the diagonal tiles' upper halves
+    // wrong (peers) or written (Ct)
+    if ((d.flags & GEMM_LOWER_ONLY) && (d.n_peer > 0 || d.Ct != nullptr)) return cudaErrorInvalidValue;
+    // the TMA kernel reads a sub buffer through its own descriptor only
+    if (impl == 0 && ((d.A.sub.base && !d.A.sub.map) || (d.B.sub.base && !d.B.sub.map))) return cudaErrorInvalidValue;
     const int tm = d.M / BM, tn = d.N / BN;
     if ((d.flags & GEMM_LOWER_ONLY) && tm < tn) return cudaErrorInvalidValue;
     // one CTA per tile (LOWER_ONLY: per tile of the lower trapezoid), walked in L2-friendly groups

@@ -45,7 +45,7 @@ struct GemmDesc {
     int bn_mod, bn_rem; // same for tile columns
     int bm_div, bm_off; // block-cyclic ownership: bm_div tiles per block (0/1: tile-cyclic), bm_off = global tile index of tile row 0
     int bn_div, bn_off;
-    int n_peer;         // fused broadcast: C is additionally stored to these peer-mapped buffers (not with LOWER_ONLY)
+    int n_peer;         // fused broadcast: C is additionally stored to these peer-mapped buffers (LOWER_ONLY: rejected, as Ct is)
     double* Cpeer[7];
 };
 
@@ -57,6 +57,8 @@ static inline GemmDesc gemm_desc_default() {
 }
 
 // impl: 0 = TMA + mbarrier warp-specialised kernel, 1 = simple synchronous kernel.
+// cudaErrorInvalidValue, nothing launched: M / N / K not multiples of 128 / 128 / 16, LOWER_ONLY with tm < tn, with n_peer > 0
+// or with Ct; impl 0 without a main-buffer map or with a sub buffer that has no map.
 cudaError_t gemm_nt_launch(const GemmDesc& d, int impl, cudaStream_t stream, int64_t* launches);
 // one-time per process (sets max dynamic smem)
 cudaError_t gemm_nt_init();

@@ -1981,6 +1981,134 @@ int gpb200_dgemm_nt_device(gpb200_handle* h, int impl, int64_t M, int64_t N, int
     return GPB200_OK;
 }
 
+int gpb200_gemm_nt_desc(gpb200_handle* h, int impl, const int64_t* desc, int32_t n, double alpha, double beta) {
+    if (!h || !desc || n != GPB200_GEMM_DESC_LEN || (impl != 0 && impl != 1)) return GPB200_EINVAL;
+    const int64_t* f = desc;
+    const int64_t* bufs = desc + 27;                       // (pointer, rows, cols, ld): A, A.sub, B, B.sub, C, Ct, 7 peers
+    for (int i = 0; i < 27; ++i)
+        if (f[i] < INT_MIN || f[i] > INT_MAX) return fail(h, GPB200_EINVAL, "gemm_nt_desc: field out of int range");
+    for (int b = 0; b < 13; ++b) {
+        const int64_t* q = bufs + 4 * b;
+        if (q[0] && ((q[0] & 15) || (q[3] & 1) || q[1] < 0 || q[2] < 0 || q[2] > q[3]))
+            return fail(h, GPB200_EINVAL, "gemm_nt_desc: buffers need 16-byte aligned pointers, even ld >= cols");
+    }
+    const int64_t* qa = bufs; const int64_t* qas = bufs + 4; const int64_t* qb = bufs + 8; const int64_t* qbs = bufs + 12;
+    if (!qa[0] || !qb[0] || !bufs[16]) return fail(h, GPB200_EINVAL, "gemm_nt_desc: A, B and C are required");
+    if (f[1] % TILE || f[2] % TILE || f[3] % 16 || f[1] < 0 || f[2] < 0 || f[3] < 0)
+        return fail(h, GPB200_EINVAL, "gemm_nt_desc: M, N multiples of 128, K multiple of 16");
+    for (const int64_t* s : {qas, qbs})
+        if (s[0] && (s[3] != TILE || ((s[1] || s[2]) && (s[1] % TILE || s[2] != TILE))))
+            return fail(h, GPB200_EINVAL, "gemm_nt_desc: sub buffers are [Npad x 128] with ld 128");
+    if (f[18] < 0 || f[18] > 7) return fail(h, GPB200_EINVAL, "gemm_nt_desc: n_peer in [0, 7]");
+    CK(cudaSetDevice(h->device));
+    // descriptors as the engine builds them: 16 x 128 boxes with 128B swizzle over the whole buffer; a sub buffer's map
+    // covers [Npad x 128].  rows = cols = 0 passes a buffer without a map (the engine's buffers when TMA is unavailable).
+    CUtensorMap maps[4];
+    const int64_t* ops[4] = {qa, qas, qb, qbs};
+    GemmBuf gb[4];
+    for (int i = 0; i < 4; ++i) {
+        const int64_t* q = ops[i];
+        const double* base = reinterpret_cast<const double*>(q[0]);
+        const bool want = q[0] && (q[1] > 0 || q[2] > 0);
+        if (want && !gemm_make_tensor_map(&maps[i], base, q[1], q[2], q[3]))
+            return fail(h, GPB200_ECUDA, "gemm_nt_desc: TMA descriptor could not be built");
+        gb[i] = q[0] ? GemmBuf{want ? &maps[i] : nullptr, base, q[3]} : bufNone();
+    }
+    GemmDesc g = gemm_desc_default();
+    g.A = GemmOperand{gb[0], gb[1], (int)f[19], (int)f[20]};
+    g.B = GemmOperand{gb[2], gb[3], (int)f[21], (int)f[22]};
+    g.C = reinterpret_cast<double*>(bufs[16]); g.ldc = bufs[19]; g.c_row0 = (int)f[23]; g.c_col0 = (int)f[24];
+    g.Ct = reinterpret_cast<double*>(bufs[20]); g.ldct = bufs[23]; g.ct_row0 = (int)f[25]; g.ct_col0 = (int)f[26];
+    g.flags = (int)f[0]; g.M = (int)f[1]; g.N = (int)f[2]; g.K = (int)f[3];
+    g.batch = (int)f[4]; g.zstep = (int)f[5]; g.m_lim = (int)f[6]; g.n_lim = (int)f[7]; g.k_lim = (int)f[8];
+    g.klo_off = (int)f[9]; g.bm_mod = (int)f[10]; g.bm_rem = (int)f[11]; g.bn_mod = (int)f[12]; g.bn_rem = (int)f[13];
+    g.bm_div = (int)f[14]; g.bm_off = (int)f[15]; g.bn_div = (int)f[16]; g.bn_off = (int)f[17];
+    g.n_peer = (int)f[18];
+    for (int q = 0; q < g.n_peer; ++q) {
+        const int64_t* pq = bufs + 4 * (6 + q);
+        if (!pq[0]) return fail(h, GPB200_EINVAL, "gemm_nt_desc: missing peer buffer");
+        g.Cpeer[q] = reinterpret_cast<double*>(pq[0]);
+    }
+    g.alpha = alpha; g.beta = beta;
+    if (g.batch < 1) return fail(h, GPB200_EINVAL, "gemm_nt_desc: batch >= 1");
+    if ((impl == 0 && (!gb[0].map || !gb[2].map)) || (g.flags & ~63))
+        return fail(h, GPB200_EINVAL, "gemm_nt_desc: impl 0 needs maps of A and B; unknown flag");
+    const cudaError_t e = gemm_nt_launch(g, impl, h->st, &h->launches);
+    if (e == cudaErrorInvalidValue) { (void)cudaGetLastError(); return fail(h, GPB200_EINVAL, "gemm_nt_desc: rejected by gemm_nt_launch"); }
+    CK(e);
+    CK(cudaStreamSynchronize(h->st));
+    return GPB200_OK;
+}
+
+int gpb200_fsa_gemm_items(gpb200_handle* h, const int64_t* items, const double* alpha_beta, int32_t n) {
+    if (!h || n < 0 || (n > 0 && (!items || !alpha_beta))) return GPB200_EINVAL;
+    std::vector<FsaGemmItem> v(n);
+    for (int i = 0; i < n; ++i) {
+        const int64_t* q = items + 8 * i;                  // C, A, B, ldc, lda, ldb, K, lower
+        if (!q[0] || !q[1] || !q[2] || ((q[0] | q[1] | q[2]) & 15) || ((q[3] | q[4] | q[5]) & 1) || q[6] < 0 || q[6] % 16 ||
+            q[6] > INT_MAX)
+            return fail(h, GPB200_EINVAL, "fsa_gemm_items: 16-byte aligned pointers, even ld, K a multiple of 16");
+        v[i] = FsaGemmItem{reinterpret_cast<double*>(q[0]), reinterpret_cast<const double*>(q[1]),
+                           reinterpret_cast<const double*>(q[2]), q[3], q[4], q[5], (int)q[6], (int)(q[7] != 0),
+                           alpha_beta[2 * i], alpha_beta[2 * i + 1]};
+    }
+    if (n == 0) return GPB200_OK;
+    CK(cudaSetDevice(h->device));
+    FsaGemmItem* d = nullptr;
+    CK(cudaMalloc(&d, sizeof(FsaGemmItem) * n));
+    cudaError_t e = cudaMemcpyAsync(d, v.data(), sizeof(FsaGemmItem) * n, cudaMemcpyHostToDevice, h->st);
+    if (e == cudaSuccess) e = fsa_gemm_launch(d, n, h->st, &h->launches);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
+    cudaFree(d);
+    CK(e);
+    return GPB200_OK;
+}
+
+int gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t n, int32_t* info) {
+    if (!h || !args || !info || (mode != 0 && mode != 1)) return GPB200_EINVAL;
+    if (mode == 0 && n != 39) return fail(h, GPB200_EINVAL, "potrf_tiles: mode 0 takes 39 arguments");
+    if (mode == 1 && (n <= 0 || n % 6)) return fail(h, GPB200_EINVAL, "potrf_tiles: mode 1 takes 6 arguments per tile");
+    CK(cudaSetDevice(h->device));
+    int* dinfo = nullptr;
+    Potrf128Item* ditems = nullptr;
+    const int big = INT_MAX;
+    CK(cudaMalloc(&dinfo, sizeof(int)));
+    cudaError_t e = cudaMemcpyAsync(dinfo, &big, sizeof(int), cudaMemcpyHostToDevice, h->st);
+    if (mode == 0) {
+        // G, ldg, F, ldf, Dinv, DinvT, logd, p0, ntiles, tile_stride, n_peer, then per peer (F, Dinv, DinvT, logd)
+        const int64_t* a = args;
+        PotrfPeers pp{};
+        pp.n = (int)std::min<int64_t>(std::max<int64_t>(a[10], 0), 7);
+        for (int q = 0; q < pp.n; ++q) {
+            pp.F[q] = reinterpret_cast<double*>(a[11 + 4 * q]); pp.Dinv[q] = reinterpret_cast<double*>(a[12 + 4 * q]);
+            pp.DinvT[q] = reinterpret_cast<double*>(a[13 + 4 * q]); pp.logd[q] = reinterpret_cast<double*>(a[14 + 4 * q]);
+        }
+        if (e == cudaSuccess && a[8] > 0)
+            e = potrf128_launch(reinterpret_cast<const double*>(a[0]), a[1], reinterpret_cast<double*>(a[2]), a[3],
+                                reinterpret_cast<double*>(a[4]), reinterpret_cast<double*>(a[5]), reinterpret_cast<double*>(a[6]),
+                                dinfo, (int)a[7], (int)a[8], (int)a[9], h->st, &h->launches, &pp);
+    } else {
+        const int nt = n / 6;
+        std::vector<Potrf128Item> v(nt);
+        for (int i = 0; i < nt; ++i) {
+            const int64_t* q = args + 6 * i;               // G, Dinv, DinvT, logd, ld, info_base
+            v[i] = Potrf128Item{reinterpret_cast<const double*>(q[0]), reinterpret_cast<double*>(q[1]),
+                                reinterpret_cast<double*>(q[2]), reinterpret_cast<double*>(q[3]), q[4], (int)q[5], 0};
+        }
+        if (e == cudaSuccess) e = cudaMalloc(&ditems, sizeof(Potrf128Item) * nt);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ditems, v.data(), sizeof(Potrf128Item) * nt, cudaMemcpyHostToDevice, h->st);
+        if (e == cudaSuccess) e = potrf128_ptr_launch(ditems, nt, dinfo, h->st, &h->launches);
+    }
+    int hinfo = big;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&hinfo, dinfo, sizeof(int), cudaMemcpyDeviceToHost, h->st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
+    cudaFree(dinfo);
+    if (ditems) cudaFree(ditems);
+    CK(e);
+    *info = hinfo;
+    return GPB200_OK;
+}
+
 int gpb200_fp64_peak(gpb200_handle* h, double* tflops_dmma, double* tflops_dfma) {
     if (!h) return GPB200_EINVAL;
     CK(cudaSetDevice(h->device));

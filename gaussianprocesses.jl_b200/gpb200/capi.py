@@ -56,6 +56,9 @@ _SIGNATURES = {
     "gpb200_dgemm_nt_device": (C.c_int, [_H, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_void_p,
                                          C.c_int64, C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_int64,
                                          C.c_int, C.c_int, _dp]),
+    "gpb200_gemm_nt_desc": (C.c_int, [_H, C.c_int, _lp, C.c_int32, C.c_double, C.c_double]),
+    "gpb200_fsa_gemm_items": (C.c_int, [_H, _lp, _dp, C.c_int32]),
+    "gpb200_potrf_tiles": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _ip]),
     "gpb200_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "gpb200_ipc_export": (C.c_int, [_H, C.c_void_p]),
     "gpb200_ipc_import": (C.c_int, [_H, C.c_int, C.c_void_p]),
@@ -371,6 +374,31 @@ class Engine:
                                                      C.c_void_p(dB), ldb, float(beta), C.c_void_p(dC), ldc,
                                                      1 if lower_only else 0, int(reps), C.byref(ms)), "dgemm_nt")
         return ms.value
+
+    GEMM_DESC_LEN = 79
+
+    def gemm_nt_desc(self, impl, desc, alpha, beta):
+        """One NT GEMM launch from the flat descriptor of include/gpb200.h (GPB200_GEMM_DESC_LEN int64)."""
+        d = np.ascontiguousarray(desc, dtype=np.int64)
+        self._check(self._lib.gpb200_gemm_nt_desc(self._h, int(impl), d.ctypes.data_as(_lp), d.size, float(alpha),
+                                                  float(beta)), "gemm_nt_desc")
+
+    def fsa_gemm_items(self, items, alpha_beta):
+        """items: (n, 8) int64 rows (C, A, B, ldc, lda, ldb, K, lower); alpha_beta: (n, 2)."""
+        it = np.ascontiguousarray(items, dtype=np.int64).reshape(-1, 8)
+        ab = np.ascontiguousarray(alpha_beta, dtype=np.float64).reshape(-1, 2)
+        if ab.shape[0] != it.shape[0]:
+            raise ValueError("fsa_gemm_items: one (alpha, beta) per item")
+        self._check(self._lib.gpb200_fsa_gemm_items(self._h, it.ctypes.data_as(_lp), _as_dp(ab), it.shape[0]),
+                    "fsa_gemm_items")
+
+    def potrf_tiles(self, mode, args):
+        """Diagonal-tile leaf (mode 0: strided tiles, 39 arguments; mode 1: 6 per item).  Returns the device info word."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        info = C.c_int32()
+        self._check(self._lib.gpb200_potrf_tiles(self._h, int(mode), a.ctypes.data_as(_lp), a.size, C.byref(info)),
+                    "potrf_tiles")
+        return int(info.value)
 
 
 class FitcEngine:

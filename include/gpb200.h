@@ -210,6 +210,29 @@ int  gpb200_dgemm_nt_device(gpb200_handle* h, int impl, int64_t M, int64_t N, in
                             double alpha, const double* dA, int64_t lda,
                             const double* dB, int64_t ldb, double beta,
                             double* dC, int64_t ldc, int lower_only, int reps, double* ms);
+/* One launch of the NT GEMM from a complete descriptor (csrc/gemm_nt.cuh GemmDesc), synchronous.  desc holds
+ * GPB200_GEMM_DESC_LEN int64 (n must equal it):
+ *   [0] flags  [1] M  [2] N  [3] K  [4] batch  [5] zstep  [6] m_lim  [7] n_lim  [8] k_lim  [9] klo_off
+ *   [10] bm_mod  [11] bm_rem  [12] bn_mod  [13] bn_rem  [14] bm_div  [15] bm_off  [16] bn_div  [17] bn_off  [18] n_peer
+ *   [19] A.row0  [20] A.col0  [21] B.row0  [22] B.col0  [23] c_row0  [24] c_col0  [25] ct_row0  [26] ct_col0
+ *   [27 + 4 b ..] buffer b = (device pointer, rows, cols, ld) for b = 0 A, 1 A.sub, 2 B, 3 B.sub, 4 C, 5 Ct, 6..12 peers;
+ *                 pointer 0 = absent.  A, A.sub, B, B.sub get TMA descriptors as the engine builds them (whole buffer,
+ *                 16 x 128 box, 128B swizzle; a sub buffer is [Npad x 128] with ld 128); rows = cols = 0 passes the
+ *                 buffer without one.
+ * GPB200_EINVAL, nothing launched: M, N not multiples of 128, K not a multiple of 16, an odd ld or unaligned pointer,
+ * impl 0 with a buffer that has no descriptor, and every descriptor gemm_nt_launch rejects (LOWER_ONLY with tm < tn,
+ * with n_peer > 0 or with Ct).                                                                                       */
+#define GPB200_GEMM_DESC_LEN 79
+int  gpb200_gemm_nt_desc(gpb200_handle* h, int impl, const int64_t* desc, int32_t n, double alpha, double beta);
+/* One launch of the grouped tile GEMM of the FSA strategy (csrc/fsa.cuh FsaGemmItem) over n items, synchronous:
+ * items[8 i ..] = (C, A, B, ldc, lda, ldb, K, lower), alpha_beta[2 i ..] = (alpha, beta).                            */
+int  gpb200_fsa_gemm_items(gpb200_handle* h, const int64_t* items, const double* alpha_beta, int32_t n);
+/* One launch of the 128 x 128 diagonal-tile leaf (csrc/potrf_base.cuh), synchronous; *info = the device info word
+ * (INT_MAX: every pivot positive).
+ *   mode 0 (potrf128_launch), n = 39: G, ldg, F, ldf, Dinv, DinvT, logd, p0, ntiles, tile_stride, n_peer, then
+ *          (F, Dinv, DinvT, logd) for each of the 7 peer sets;
+ *   mode 1 (potrf128_ptr_launch), n = 6 per tile: G, Dinv, DinvT, logd, ld, info_base.                                */
+int  gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t n, int32_t* info);
 
 /* ---- multi-GPU (one process per GPU; NCCL over NVLink) -------------------------------------- */
 /* rank 0 obtains a 128-byte NCCL unique id, the host side broadcasts it (torch.distributed /
