@@ -1739,17 +1739,10 @@ int gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, con
 //   Gram rows r >= c0;  L[r, 0:c0] = K[r, 0:c0] L11^-T (whitening TRSM against the existing factor);
 //   Schur complement of the trailing block (one GEMM with K = c0);  Cholesky of that small trailing block --
 // i.e. O(k N^2) instead of O(N^3).  Returns GPB200_EINVAL if N + k exceeds the capacity (the caller refits).
-int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) {
-    if (!h) return GPB200_EINVAL;
-    if (k <= 0 || !xnew || ldx < h->d) return fail(h, GPB200_EINVAL, "append: bad k, x or ldx");
-    if (!h->factored) return fail(h, GPB200_ESTATE, "append: factorize first");
-    if (h->nranks > 1) return fail(h, GPB200_ESTATE, "append: single-GPU handles only");
-    if (h->n_noise != 1) return fail(h, GPB200_ESTATE, "append: scalar logNoise only (per-point noise needs a refit)");
-    if (h->N + k > h->Npad) return fail(h, GPB200_EINVAL, "append: capacity exceeded (set option \"capacity\" before set_data, or refit)");
-    CK(cudaSetDevice(h->device));
+// Row-sharded handles run the same steps over the ranks (shard_append in shard_impl.cuh).
+static int append_inputs(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) {
     const int64_t Nold = h->N, Nnew = Nold + k;
     const int d = h->d, Np = (int)h->Npad;
-    const int c0 = (int)(Nold / TILE * TILE);                       // first tile row that changes
     CK(cudaMemcpy2DAsync(h->x + Nold * d, sizeof(double) * d, xnew, sizeof(double) * ldx, sizeof(double) * d, k, cudaMemcpyHostToDevice, h->st));
     h->xmap_ok = false;
     if (h->xp) {
@@ -1760,6 +1753,45 @@ int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) 
     }
     h->N = Nnew;
     h->inv_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
+    return GPB200_OK;
+}
+
+int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) {
+    if (!h) return GPB200_EINVAL;
+    if (k <= 0 || !xnew || ldx < h->d) return fail(h, GPB200_EINVAL, "append: bad k, x or ldx");
+    if (!h->factored) return fail(h, GPB200_ESTATE, "append: factorize first");
+    if (h->nranks > 1 && !h->sharded)
+        return fail(h, GPB200_ESTATE, "append: multi-rank handles need row-sharded storage (option \"shard\" = 1)");
+    Locals L{h};
+    if (h->sharded) { int rc = shard_entry(h, L); if (rc) return rc; }
+    if (h->n_noise != 1) return fail(h, GPB200_ESTATE, "append: scalar logNoise only (per-point noise needs a refit)");
+    if (h->N + k > h->Npad) return fail(h, GPB200_EINVAL, "append: capacity exceeded (set option \"capacity\" before set_data, or refit)");
+    CK(cudaSetDevice(h->device));
+    const int64_t Nold = h->N;
+    if (h->sharded) {
+        for (auto* q : L)
+            if (!q->factored || q->N != Nold || q->Npad != h->Npad)
+                return fail(h, GPB200_ESTATE, "append: every handle of the group needs the same factorized data");
+        for (auto* q : L) { int rc = append_inputs(q, k, xnew, ldx); if (rc) { if (q != h) h->err = q->err; return rc; } }
+        int rc = shard_append(L, Nold);
+        if (rc) { for (auto* q : L) if (q != h && !q->err.empty()) { h->err = q->err; break; } return rc; }
+        int info = 0;
+        CK(cudaMemcpyAsync(&info, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
+        if ((rc = sync_all(L))) return rc;
+        for (auto* q : L) profile_collect(q);
+        if (info != INT_MAX) {
+            for (auto* q : L) q->factored = false;
+            char buf[128];
+            snprintf(buf, sizeof buf, "append: extended matrix is not positive definite; leading minor %d", info);
+            h->err = buf;
+            return info > h->N ? (int)h->N : info;
+        }
+        return GPB200_OK;
+    }
+    { int rc = append_inputs(h, k, xnew, ldx); if (rc) return rc; }
+    const int64_t Nnew = h->N;
+    const int d = h->d, Np = (int)h->Npad;
+    const int c0 = (int)(Nold / TILE * TILE);                       // first tile row that changes
     const int init = INT_MAX;
     CK(cudaMemcpyAsync(h->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, h->st));
     // Gram rows >= c0 (columns <= row), identity beyond the new N

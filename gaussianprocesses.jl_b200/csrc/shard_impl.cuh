@@ -24,6 +24,9 @@
 //              path, K^-1 never leaves the rank that owns the row.
 //   predict    V' = K*' L^-T with the columns of V' (training rows) owned like the rows of L; variance accumulated from
 //              the broadcast blocks, identical on every rank.
+//   append     rebuild from the ownership block b0 of the first touched tile: own Gram rows >= b0; V = K[b0.., :b0] L11^-T
+//              solved like the predict (the block owner also keeps each block's transpose as U rows of its old rows); own
+//              rows of V into L; Schur complement of the own rows (K = b0); the Cholesky above from block b0 / NBp on.
 // Collectives: NCCL (one process per GPU) or, for an in-process group of virtual ranks on ONE device
 // (gpb200_group_create: lets a 1-GPU box run the multi-rank schedules), event-ordered device-to-device copies.
 
@@ -440,7 +443,8 @@ cudaError_t shard_trsm_rows(gpb200_handle* h, int c0, int r1, int off, int n, in
 // R-way split TRSM, the all-gather) runs on the high-priority side stream while the main stream applies the PREVIOUS panel
 // to the bulk of the trailing matrix.  Per panel the main stream first updates only the columns of the next block ("narrow"
 // update, K = NBp, a few hundred tiles), hands over to the chain, then does the rest.  Panel buffers alternate (P[k & 1]).
-int shard_cholesky_la(const Locals& L) {
+// `kb0` > 0 factors only the trailing matrix from block kb0 on (append: the blocks before it are already factored).
+int shard_cholesky_la(const Locals& L, int kb0 = 0) {
     gpb200_handle* h0 = L[0];
     const int Np = (int)h0->Npad, R = h0->nranks, NBp = shard_panel_width(h0);
     const int nblk = (Np + NBp - 1) / NBp;
@@ -452,7 +456,7 @@ int shard_cholesky_la(const Locals& L) {
         SCK(q, cudaStreamWaitEvent(q->st_side, e, 0));
     }
     std::vector<cudaEvent_t> ev_panel(L.size());
-    for (int k = 0; k < nblk; ++k) {
+    for (int k = kb0; k < nblk; ++k) {
         const int c0 = k * NBp, nb = std::min(NBp, Np - c0), o = k % R, r1 = c0 + nb, pb = k & 1;
         const int t1 = r1 / TILE;
         // ---------------- chain of panel k, on the side streams ----------------
@@ -759,4 +763,86 @@ int shard_predict_solve(const Locals& L, int Mpad, int64_t Mc, bool want_var, bo
         }
     }
     return GPB200_OK;
+}
+
+// ---- append: V = K[b0.., 0..b0) L11^-T for the Mv rows from b0 on, solved like the test points of shard_predict_solve -------
+// Kst (Mv x Npad) holds K[b0.., 0..b0) on every rank.  Per old column block the owner solves it, keeps its transpose as the
+// U part of its own old rows (F[c0.., b0..b0+Mv)) and broadcasts it; every rank copies the block into its Kst, which ends
+// as the replicated V, and applies it to its own later columns below b0.
+int shard_append_solve(const Locals& L, int b0, int Mv) {
+    gpb200_handle* h0 = L[0];
+    const int R = h0->nranks, NBp = shard_panel_width(h0);
+    for (int k = 0; k * NBp < b0; ++k) {
+        const int c0 = k * NBp, o = k % R, r1 = c0 + NBp;
+        for (auto* q : L) {
+            if (q->rank != o) continue;
+            GemmBuf bk{q->tma_ok ? &q->mapKst : nullptr, q->Kst, q->Npad};
+            SCK(q, trsm_rec_buf(q, bk, Mv, c0, NBp));
+            SCK(q, cudaMemcpy2DAsync(q->P[0], sizeof(double) * NBp, q->Kst + c0, sizeof(double) * q->Npad, sizeof(double) * NBp,
+                                     (size_t)Mv, cudaMemcpyDeviceToDevice, q->st));
+            SCK(q, shard_transpose(q->F + (size_t)c0 * q->ld + b0, q->ld, q->P[0], NBp, Mv, NBp, q->st, &q->launches));
+        }
+        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->P[0]; }, sizeof(double) * (size_t)Mv * NBp));
+        for (auto* q : L) {
+            if (q->rank != o)
+                SCK(q, cudaMemcpy2DAsync(q->Kst + c0, sizeof(double) * q->Npad, q->P[0], sizeof(double) * NBp, sizeof(double) * NBp,
+                                         (size_t)Mv, cudaMemcpyDeviceToDevice, q->st));
+            if (r1 < b0) {
+                GemmDesc g = gemm_desc_default();
+                g.A = GemmOperand{bufP(q, 0), bufNone(), 0, 0};
+                g.B = GemmOperand{bufF(q), bufNone(), r1, c0};
+                g.C = q->Kst; g.ldc = q->Npad; g.c_row0 = 0; g.c_col0 = r1;
+                g.M = Mv; g.N = b0 - r1; g.K = NBp;
+                g.alpha = -1.0; g.beta = 1.0;
+                own_cols_filter(q, g, r1);
+                SCK(q, launch_gemm(q, g));
+            }
+        }
+    }
+    return GPB200_OK;
+}
+
+// Extend the factor by the points the caller placed at rows Nold..N of x on every rank (gpb200_append).  The rebuild starts at
+// the ownership block b0 holding row Nold, so every panel factored again is one whole block with one owner; rows < b0 of L,
+// their Dinv / DinvT / logd and their U part left of b0 stay.  Rows >= N up to Npad keep identity rows of L, so only the Mv
+// rows b0 .. N (rounded up to a tile) carry V.
+int shard_append(const Locals& L, int64_t Nold) {
+    gpb200_handle* h0 = L[0];
+    const int Np = (int)h0->Npad, NBp = shard_panel_width(h0);
+    const int b0 = (int)(Nold / NBp * NBp);
+    const int Mv = (int)((h0->N + TILE - 1) / TILE * TILE) - b0;
+    const int init = INT_MAX;
+    for (auto* q : L) {
+        SCK(q, cudaMemcpyAsync(q->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, q->st));
+        // own Gram rows >= b0 (columns <= row), identity beyond the new N
+        SCK(q, gram_lower_launch(q->prog, q->x, q->d, q->d, q->N, Np, q->noise_var, 1, q->nugget, q->G, q->ld, q->st, &q->launches,
+                                 q->rb, q->nranks, q->rank, 1, b0 / TILE));
+    }
+    if (b0 > 0) {
+        for (auto* q : L) {
+            SRC(ensure_predict_ws(q, Mv, false));
+            SCK(q, crossgram_launch(q->prog, q->x + (size_t)b0 * q->d, q->d, q->N - b0, Mv, q->x, q->d, b0, b0, q->d, q->Kst, q->Npad,
+                                    q->st, &q->launches));
+        }
+        SRC(shard_append_solve(L, b0, Mv));
+        for (auto* q : L) {
+            // own rows of V are the rows of L left of b0
+            for (long long t = b0 / TILE; t < (b0 + Mv) / TILE; ++t)
+                if (owner_of_tile(q, t) == q->rank)
+                    SCK(q, cudaMemcpy2DAsync(q->F + (size_t)t * TILE * q->ld, sizeof(double) * q->ld, q->Kst + (size_t)(t * TILE - b0) * q->Npad,
+                                             sizeof(double) * q->Npad, sizeof(double) * b0, TILE, cudaMemcpyDeviceToDevice, q->st));
+            // Schur complement of the own rows: G[r, c] -= V_r V_c',  r >= c >= b0
+            GemmBuf bv{q->tma_ok ? &q->mapKst : nullptr, q->Kst, q->Npad};
+            GemmDesc g = gemm_desc_default();
+            g.A = GemmOperand{bv, bufNone(), 0, 0};
+            g.B = GemmOperand{bv, bufNone(), 0, 0};
+            g.C = q->G; g.ldc = q->ld; g.c_row0 = b0; g.c_col0 = b0;
+            g.M = Mv; g.N = Mv; g.K = b0;
+            g.alpha = -1.0; g.beta = 1.0;
+            g.flags = GEMM_LOWER_ONLY;
+            own_rows_filter(q, g, b0);
+            SCK(q, launch_gemm(q, g));
+        }
+    }
+    return shard_cholesky_la(L, b0 / NBp);
 }

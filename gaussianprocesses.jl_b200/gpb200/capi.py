@@ -593,6 +593,13 @@ class LocalGroupEngine:
     def rand(self, *a, **k):
         return self.lead.rand(*a, **k)
 
+    def append(self, xnew_pm):
+        """the leader extends every rank's inputs and the distributed factor (ElasticGPE append!)"""
+        self.lead.append(xnew_pm)
+        for e in self.engines[1:]:
+            e.N = self.lead.N
+        self.N = self.lead.N
+
     def timings(self):
         return self.lead.timings()
 

@@ -133,7 +133,10 @@ int  gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, co
 /* append!(gp::ElasticGPE, x, y) (src/GPEelastic.jl:13-22): k more observations (xnew: d x k column-major) with UNCHANGED
  * hyper-parameters; the factor is extended in place (rows from the first touched tile on are rebuilt: O(k N^2)), alpha / mll are
  * then refreshed with gpb200_mll on the longer y.  Needs room reserved by option "capacity" (ElasticGPE's capacity) before
- * gpb200_set_data; GPB200_EINVAL when the capacity is exceeded (the shim refits, like ElasticPDMats.resize!).             */
+ * gpb200_set_data; GPB200_EINVAL when the capacity is exceeded (the shim refits, like ElasticPDMats.resize!).
+ * Row-sharded handles extend the distributed factor: an in-process group through its leader, NCCL ranks (option "shard" = 1)
+ * collectively; the rebuild starts at the ownership block of the first touched tile.  Replicated multi-rank handles and
+ * vector logNoise return GPB200_ESTATE; a non-positive-definite extension returns the leading minor and clears the factor. */
 int  gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx);
 
 /* ---- GPA: GP with a non-Gaussian likelihood (src/GPA.jl), latent f = L v + mu over K = L L' ---------------------------------
