@@ -242,30 +242,35 @@ bool nccl_load() {
     return g_nccl.ok;
 }
 
-#define CK(call)                                                                                   \
-    do {                                                                                           \
-        cudaError_t e_ = (call);                                                                   \
-        if (e_ != cudaSuccess) {                                                                   \
-            char buf_[512];                                                                        \
-            snprintf(buf_, sizeof buf_, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,       \
-                     cudaGetErrorString(e_));                                                      \
-            h->err = buf_;                                                                         \
-            (void)cudaGetLastError();                                                              \
-            return GPB200_ECUDA;                                                                   \
-        }                                                                                          \
-    } while (0)
+// "<call> failed at file:line: reason" into `err`; a CUDA failure also clears the error the runtime keeps for the next
+// cudaGetLastError.  Returns `code`.
+int check_failed(std::string& err, int code, const char* call, const char* file, int line, const char* reason) {
+    char buf[512];
+    snprintf(buf, sizeof buf, "%s failed at %s:%d: %s", call, file, line, reason);
+    err = buf;
+    if (code == GPB200_ECUDA) (void)cudaGetLastError();
+    return code;
+}
+int cuda_rc(std::string& err, cudaError_t e, const char* call, const char* file, int line) {
+    return e == cudaSuccess ? GPB200_OK : check_failed(err, GPB200_ECUDA, call, file, line, cudaGetErrorString(e));
+}
+int nccl_rc(std::string& err, ncclResult_t r, const char* call, const char* file, int line) {
+    return r == ncclSuccess ? GPB200_OK
+                            : check_failed(err, GPB200_ENCCL, call, file, line, g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "nccl error");
+}
+// a failure on rank q: in an in-process group the caller holds the leader (shard_entry), so q's message is copied there
+int rank_failed(gpb200_handle* q, int rc) {
+    if (rc && q->grp && q != q->grp->hs[0]) q->grp->hs[0]->err = q->err;
+    return rc;
+}
 
-#define CKN(call)                                                                                  \
-    do {                                                                                           \
-        ncclResult_t r_ = (call);                                                                  \
-        if (r_ != ncclSuccess) {                                                                   \
-            char buf_[512];                                                                        \
-            snprintf(buf_, sizeof buf_, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,       \
-                     g_nccl.GetErrorString ? g_nccl.GetErrorString(r_) : "nccl error");            \
-            h->err = buf_;                                                                         \
-            return GPB200_ENCCL;                                                                   \
-        }                                                                                          \
-    } while (0)
+#define TRY(rc)        do { if (int rc_ = (rc)) return rc_; } while (0)
+#define CK(call)       TRY(cuda_rc(h->err, (call), #call, __FILE__, __LINE__))
+#define CKN(call)      TRY(nccl_rc(h->err, (call), #call, __FILE__, __LINE__))
+#define SCK(q, call)   TRY(rank_failed(q, cuda_rc((q)->err, (call), #call, __FILE__, __LINE__)))
+#define SCKN(q, call)  TRY(rank_failed(q, nccl_rc((q)->err, (call), #call, __FILE__, __LINE__)))
+#define FCK(call)      TRY(cuda_rc(f->err, (call), #call, __FILE__, __LINE__))
+#define FCKN(call)     TRY(nccl_rc(f->err, (call), #call, __FILE__, __LINE__))
 
 int fail(gpb200_handle* h, int code, const char* msg) {
     if (h) h->err = msg;
@@ -480,14 +485,14 @@ cudaError_t chol_panel(gpb200_handle* h, int p, int n, int s, bool leaf_done = f
     return chol_panel(h, p + hs, cols, hs);
 }
 
-cudaError_t cholesky(gpb200_handle* h) {
+// right-looking outer loop over the columns from p0 on, `nb`-wide panels (0 = one panel spanning the rest: fully recursive)
+cudaError_t cholesky(gpb200_handle* h, int p0, int nb) {
     const int Np = (int)h->Npad;
-    // outer block: option "nb" (0 = one panel spanning the matrix: fully recursive)
     int NB = TILE;
-    const int want = h->nb > 0 ? h->nb : Np;
+    const int want = nb > 0 ? nb : Np;
     while (NB < want && NB < Np) NB *= 2;
     cudaError_t e;
-    for (int p = 0; p < Np; p += NB) {
+    for (int p = p0; p < Np; p += NB) {
         const int n = (Np - p < NB) ? Np - p : NB;
         if ((e = chol_panel(h, p, n, NB)) != cudaSuccess) return e;
         const int rem = Np - p - n;
@@ -938,26 +943,6 @@ cudaError_t trsm_rec(gpb200_handle* h, int Mpad, int c0, int n) {
     return trsm_rec_buf(h, bk, Mpad, c0, n);
 }
 
-// factor whatever SPD matrix sits in the lower tiles of h->G (padding must be identity)
-int chol_inplace(gpb200_handle* h) {
-    h->factored = h->inv_ready = h->alpha_ready = false;
-    const int init = INT_MAX;
-    CK(cudaMemcpyAsync(h->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, h->st));
-    CK(cholesky(h));
-    int info = 0;
-    CK(cudaMemcpyAsync(&info, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
-    CK(cudaStreamSynchronize(h->st));
-    profile_collect(h);
-    if (info != INT_MAX) {
-        char buf[128];
-        snprintf(buf, sizeof buf, "matrix is not positive definite; leading minor %d", info);
-        h->err = buf;
-        return info > h->N ? (int)h->N : info;
-    }
-    h->factored = true;
-    return GPB200_OK;
-}
-
 float ev_ms(cudaEvent_t a, cudaEvent_t b) {
     float ms = 0.f;
     cudaEventElapsedTime(&ms, a, b);
@@ -993,6 +978,7 @@ cudaError_t launch_trace(gpb200_handle* h, int bm_mod, int bm_rem, int bm_div) {
 int shard_entry(gpb200_handle* h, Locals& L) {
     L = locals(h);
     if (h->grp && L[0] != h) return fail(h, GPB200_ESTATE, "in-process group: call collective entry points on the leader (rank 0) handle");
+    for (auto* q : L) q->err.clear();          // a message on any rank after this call comes from this call
     return GPB200_OK;
 }
 // debug getters with sharded storage: rows this rank owns, zeros elsewhere (the caller adds the ranks' pieces)
@@ -1010,6 +996,42 @@ int copy_own_rows(gpb200_handle* h, double* dst_host, const double* src_dev) {
 int sync_all(const Locals& L) {
     for (auto* q : L) SCK(q, cudaStreamSynchronize(q->st));
     return GPB200_OK;
+}
+
+// Every factorisation schedule runs between these two.  factor_begin: no failing pivot yet on any rank (info = INT_MAX).
+// factor_end: the first failing pivot is read on the leader once every rank has finished; `factored` of every rank follows
+// it.  Returns GPB200_OK or the leading minor clipped to N, with "<what>matrix is not positive definite; ..." as the message.
+int factor_begin(const Locals& L) {
+    const int init = INT_MAX;
+    for (auto* q : L) SCK(q, cudaMemcpyAsync(q->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, q->st));
+    return GPB200_OK;
+}
+int factor_end(const Locals& L, const char* what, bool p2p_ran) {
+    gpb200_handle* h = L[0];
+    int info = 0;
+    CK(cudaMemcpyAsync(&info, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    TRY(sync_all(L));
+    for (auto* q : L) profile_collect(q);
+    if (p2p_ran) {
+        int wd = 0;
+        CK(cudaMemcpy(&wd, h->sig + 8, sizeof(int), cudaMemcpyDeviceToHost));
+        if (wd) return fail(h, GPB200_ECUDA, "panel signal watchdog fired (a peer never published its panel)");
+    }
+    for (auto* q : L) q->factored = info == INT_MAX;
+    if (info == INT_MAX) return GPB200_OK;
+    char buf[128];
+    snprintf(buf, sizeof buf, "%smatrix is not positive definite; leading minor %d", what, info);
+    h->err = buf;
+    return info > h->N ? (int)h->N : info;
+}
+
+// factor whatever SPD matrix sits in the lower tiles of h->G (padding must be identity)
+int chol_inplace(gpb200_handle* h) {
+    h->factored = h->inv_ready = h->alpha_ready = false;
+    const Locals L{h};
+    TRY(factor_begin(L));
+    CK(cholesky(h, 0, h->nb));
+    return factor_end(L, "", false);
 }
 
 }  // namespace
@@ -1295,8 +1317,7 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
     }
     Locals L;
     { int rc = shard_entry(h, L); if (rc) return rc; }
-    for (auto* q : L) { int rc = ensure_storage(q); if (rc) { if (q != h) h->err = q->err; return rc; } }
-    const int init = INT_MAX;
+    for (auto* q : L) TRY(rank_failed(q, ensure_storage(q)));
     for (auto* q : L) {                                    // (an in-process group: every virtual rank gets the arguments)
         if (!q->has_data || !q->has_kernel || q->prog.n_theta != h->prog.n_theta || q->N != h->N)
             return fail(h, GPB200_ESTATE, "factorize: every handle of the group needs the same set_data / set_kernel");
@@ -1305,65 +1326,29 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
         kprog_set_theta(q->prog, theta);
         SCK(q, cudaMemcpyAsync(q->noise_var, nv.data(), sizeof(double) * n_noise, cudaMemcpyHostToDevice, q->st));
         q->n_noise = n_noise; q->nugget = extra_nugget;
-        SCK(q, cudaMemcpyAsync(q->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, q->st));
     }
+    TRY(factor_begin(L));
+    CK(cudaEventRecord(h->ev0, h->st));
     if (h->sharded) {
         // row-sharded storage: own rows of the Gram matrix, then the all-gathered-panel Cholesky (shard_impl.cuh)
-        CK(cudaEventRecord(h->ev0, h->st));
         for (auto* q : L) SCK(q, launch_gram(q, q->G, q->ld, q->rb, q->nranks, q->rank, 1));
         CK(cudaEventRecord(h->ev1, h->st));
-        { int rc = shard_cholesky_la(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
-        CK(cudaEventRecord(h->ev2, h->st));
-        int info_s = 0;
-        CK(cudaMemcpyAsync(&info_s, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
-        { int rc = sync_all(L); if (rc) return rc; }
-        for (auto* q : L) profile_collect(q);
-        h->ms[0] = ev_ms(h->ev0, h->ev1);
-        h->ms[1] = ev_ms(h->ev1, h->ev2);
-        if (info_s != INT_MAX) {
-            char buf[128];
-            snprintf(buf, sizeof buf, "matrix is not positive definite; leading minor %d", info_s);
-            h->err = buf;
-            return info_s > h->N ? (int)h->N : info_s;
-        }
-        for (auto* q : L) q->factored = true;
-        return GPB200_OK;
-    }
-
-    CK(cudaEventRecord(h->ev0, h->st));
-    if (h->nranks > 1) {
-        int rc = dist_alloc(h);
-        if (rc) return rc;
-        const int NBd = dist_block(h);
-        CK(launch_gram(h, h->G, h->ld, NBd / TILE, h->nranks, h->rank, 0));
+        TRY(shard_cholesky_la(L));
+    } else if (h->nranks > 1) {
+        TRY(dist_alloc(h));
+        CK(launch_gram(h, h->G, h->ld, dist_block(h) / TILE, h->nranks, h->rank, 0));
         CK(cudaEventRecord(h->ev1, h->st));
-        rc = h->p2p ? cholesky_dist_p2p(h) : cholesky_dist(h);
-        if (rc) return rc;
+        TRY(h->p2p ? cholesky_dist_p2p(h) : cholesky_dist(h));
     } else {
         CK(launch_gram(h, h->G, h->ld, 0, 1, 0, 0));
         CK(cudaEventRecord(h->ev1, h->st));
-        CK(cholesky(h));
+        CK(cholesky(h, 0, h->nb));
     }
     CK(cudaEventRecord(h->ev2, h->st));
-    int info = 0;
-    CK(cudaMemcpyAsync(&info, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
-    CK(cudaStreamSynchronize(h->st));
-    profile_collect(h);
+    const int rc = factor_end(L, "", !h->sharded && h->p2p);
     h->ms[0] = ev_ms(h->ev0, h->ev1);
     h->ms[1] = ev_ms(h->ev1, h->ev2);
-    if (h->p2p) {
-        int wd = 0;
-        CK(cudaMemcpy(&wd, h->sig + 8, sizeof(int), cudaMemcpyDeviceToHost));
-        if (wd) return fail(h, GPB200_ECUDA, "panel signal watchdog fired (a peer never published its panel)");
-    }
-    if (info != INT_MAX) {
-        char buf[128];
-        snprintf(buf, sizeof buf, "matrix is not positive definite; leading minor %d", info);
-        h->err = buf;
-        return info > h->N ? (int)h->N : info;
-    }
-    h->factored = true;
-    return GPB200_OK;
+    return rc;
 }
 
 int gpb200_logdet(gpb200_handle* h, double* logdet) {
@@ -1383,8 +1368,8 @@ int gpb200_solve(gpb200_handle* h, const double* rhs, double* out) {
     if (h->sharded) {
         Locals L;
         { int rc = shard_entry(h, L); if (rc) return rc; }
-        for (auto* q : L) { int rc = upload_padded(q, q->r1, rhs); if (rc) return rc; }
-        { int rc = shard_solve(L, &gpb200_handle::r1, &gpb200_handle::y1, &gpb200_handle::r0); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
+        for (auto* q : L) TRY(rank_failed(q, upload_padded(q, q->r1, rhs)));
+        TRY(shard_solve(L, &gpb200_handle::r1, &gpb200_handle::y1, &gpb200_handle::r0));
         CK(cudaMemcpyAsync(out, h->r0, sizeof(double) * h->N, cudaMemcpyDeviceToHost, h->st));
         return sync_all(L);
     }
@@ -1406,9 +1391,8 @@ int gpb200_mll(gpb200_handle* h, const double* y_minus_mean, double* alpha, doub
     int rc = upload_padded(h, h->r0, y_minus_mean);
     if (rc) return rc;
     if (h->sharded) {
-        for (auto* q : Ls) if (q != h) { rc = upload_padded(q, q->r0, y_minus_mean); if (rc) return rc; }
-        rc = shard_solve(Ls, &gpb200_handle::r0, &gpb200_handle::y1, &gpb200_handle::alpha);
-        if (rc) { if (Ls[0] != h) h->err = Ls[0]->err; return rc; }
+        for (auto* q : Ls) if (q != h) TRY(rank_failed(q, upload_padded(q, q->r0, y_minus_mean)));
+        TRY(shard_solve(Ls, &gpb200_handle::r0, &gpb200_handle::y1, &gpb200_handle::alpha));
         for (auto* q : Ls) q->alpha_ready = true;
     } else {
         CK(cudaMemcpyAsync(h->r1, h->r0, sizeof(double) * h->Npad, cudaMemcpyDeviceToDevice, h->st));
@@ -1421,7 +1405,7 @@ int gpb200_mll(gpb200_handle* h, const double* y_minus_mean, double* alpha, doub
     if (alpha) CK(cudaMemcpyAsync(alpha, h->alpha, sizeof(double) * h->N, cudaMemcpyDeviceToHost, h->st));
     CK(cudaEventRecord(h->ev1, h->st));
     CK(cudaStreamSynchronize(h->st));
-    if (h->sharded) { int rcs = sync_all(Ls); if (rcs) return rcs; }
+    if (h->sharded) TRY(sync_all(Ls));
     h->ms[2] = ev_ms(h->ev0, h->ev1);
     if (!h->sharded) { int rcw = check_trsv_watchdog(h); if (rcw) return rcw; }
     *mll = -(s[0] + s[1] + LOG2PI * (double)h->N) / 2.0;    // src/GPE.jl:210
@@ -1439,9 +1423,9 @@ int gpb200_grad_prepare(gpb200_handle* h) {
     if (h->sharded) {
         Locals L;
         { int rc = shard_entry(h, L); if (rc) return rc; }
-        { int rc = shard_inverse_la(L); if (rc) { if (L[0] != h) h->err = L[0]->err; return rc; } }
+        TRY(shard_inverse_la(L));
         CK(cudaEventRecord(h->ev1, h->st));
-        { int rc = sync_all(L); if (rc) return rc; }
+        TRY(sync_all(L));
         for (auto* q : L) { profile_collect(q); q->inv_ready = true; }
         h->ms[3] = ev_ms(h->ev0, h->ev1);
         return GPB200_OK;
@@ -1465,8 +1449,7 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     if (h->sharded) { int rc = shard_entry(h, Lg); if (rc) return rc; } else Lg = Locals{h};
     if (alpha) {
         for (auto* q : Lg) {
-            int rc = upload_padded(q, q->alpha, alpha);
-            if (rc) return rc;
+            TRY(rank_failed(q, upload_padded(q, q->alpha, alpha)));
             q->alpha_ready = true;
         }
     }
@@ -1474,8 +1457,7 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     if (h->sharded) {
         // fused trace over the own rows of K^-1 (block-cyclic tile rows), P+1 partial sums summed over the ranks
         for (auto* q : Lg) SCK(q, launch_trace(q, q->nranks, q->rank, q->rb));
-        int rc = coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out; }, (size_t)trace_num_acc(h->prog));
-        if (rc) { if (Lg[0] != h) h->err = Lg[0]->err; return rc; }
+        TRY(coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out; }, (size_t)trace_num_acc(h->prog)));
     } else {
         CK(launch_trace(h, h->nranks, h->rank, 1));
     }
@@ -1491,7 +1473,7 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     std::vector<double> out((size_t)np + 1);
     CK(cudaMemcpyAsync(out.data(), h->trace_out, sizeof(double) * (np + 1), cudaMemcpyDeviceToHost, h->st));
     CK(cudaStreamSynchronize(h->st));
-    if (h->sharded) { int rcs = sync_all(Lg); if (rcs) return rcs; }
+    if (h->sharded) TRY(sync_all(Lg));
     h->ms[4] = ev_ms(h->ev0, h->ev1);
     if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = out[p];
     if (trA) *trA = out[np];
@@ -1602,7 +1584,7 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
     Locals Lp;
     if (h->sharded) {
         int rc = shard_entry(h, Lp); if (rc) return rc;
-        if (alpha) for (auto* q : Lp) if (q != h) { rc = upload_padded(q, q->alpha, alpha); if (rc) return rc; }
+        if (alpha) for (auto* q : Lp) if (q != h) TRY(rank_failed(q, upload_padded(q, q->alpha, alpha)));
     }
     CK(cudaEventRecord(h->ev2, h->st));
     for (int64_t m0 = 0; h->sharded && m0 < M; m0 += cap) {
@@ -1610,8 +1592,7 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
         const int64_t Mc = (M - m0 < cap) ? M - m0 : cap;
         const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
         for (auto* q : Lp) {
-            int rc = ensure_predict_ws(q, Mc, cov != nullptr);
-            if (rc) { if (q != h) h->err = q->err; return rc; }
+            TRY(rank_failed(q, ensure_predict_ws(q, Mc, cov != nullptr)));
             SCK(q, cudaMemcpy2DAsync(q->xs, sizeof(double) * q->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * q->d, Mc,
                                      cudaMemcpyHostToDevice, q->st));
             SCK(q, crossgram_launch(q->prog, q->xs, q->d, Mc, Mpad, q->x, q->d, q->N, q->Npad, q->d, q->Kst, q->Npad, q->st, &q->launches));
@@ -1623,13 +1604,12 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
         CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));          // GP.jl:26
         CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
         if (need_v) {
-            int rc = shard_predict_solve(Lp, (int)Mpad, Mc, var != nullptr, cov != nullptr);
-            if (rc) { if (Lp[0] != h) h->err = Lp[0]->err; return rc; }
+            TRY(shard_predict_solve(Lp, (int)Mpad, Mc, var != nullptr, cov != nullptr));
             if (var) CK(cudaMemcpyAsync(var + m0, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
             if (cov && !h->cov_keep_device) CK(cudaMemcpy2DAsync(cov, sizeof(double) * M, h->Kss, sizeof(double) * Mpad, sizeof(double) * M, M,
                                           cudaMemcpyDeviceToHost, h->st));
         }
-        { int rc = sync_all(Lp); if (rc) return rc; }
+        TRY(sync_all(Lp));
     }
     for (int64_t m0 = 0; !h->sharded && m0 < M; m0 += cap) {
         const int64_t Mc = (M - m0 < cap) ? M - m0 : cap;
@@ -1772,28 +1752,16 @@ int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) 
         for (auto* q : L)
             if (!q->factored || q->N != Nold || q->Npad != h->Npad)
                 return fail(h, GPB200_ESTATE, "append: every handle of the group needs the same factorized data");
-        for (auto* q : L) { int rc = append_inputs(q, k, xnew, ldx); if (rc) { if (q != h) h->err = q->err; return rc; } }
-        int rc = shard_append(L, Nold);
-        if (rc) { for (auto* q : L) if (q != h && !q->err.empty()) { h->err = q->err; break; } return rc; }
-        int info = 0;
-        CK(cudaMemcpyAsync(&info, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
-        if ((rc = sync_all(L))) return rc;
-        for (auto* q : L) profile_collect(q);
-        if (info != INT_MAX) {
-            for (auto* q : L) q->factored = false;
-            char buf[128];
-            snprintf(buf, sizeof buf, "append: extended matrix is not positive definite; leading minor %d", info);
-            h->err = buf;
-            return info > h->N ? (int)h->N : info;
-        }
-        return GPB200_OK;
+        for (auto* q : L) TRY(rank_failed(q, append_inputs(q, k, xnew, ldx)));
+        TRY(factor_begin(L));
+        TRY(shard_append(L, Nold));
+        return factor_end(L, "append: extended ", false);
     }
-    { int rc = append_inputs(h, k, xnew, ldx); if (rc) return rc; }
+    TRY(append_inputs(h, k, xnew, ldx));
     const int64_t Nnew = h->N;
     const int d = h->d, Np = (int)h->Npad;
     const int c0 = (int)(Nold / TILE * TILE);                       // first tile row that changes
-    const int init = INT_MAX;
-    CK(cudaMemcpyAsync(h->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, h->st));
+    TRY(factor_begin(L));
     // Gram rows >= c0 (columns <= row), identity beyond the new N
     CK(gram_lower_launch(h->prog, h->x, d, d, Nnew, Np, h->noise_var, 1, h->nugget, h->G, h->ld, h->st, &h->launches, 0, 1, 0, 0, c0 / TILE));
     cudaError_t e = cudaSuccess;
@@ -1814,23 +1782,8 @@ int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) 
         CK(schur_update(h, c0, Np - c0, Np - c0, 0, c0));
     }
     // factor the trailing block tile by tile (right-looking, 128-wide panels)
-    for (int p = c0; p < Np; p += TILE) {
-        CK(chol_panel(h, p, TILE, TILE));
-        const int rem = Np - p - TILE;
-        if (rem > 0) CK(schur_update(h, p + TILE, rem, rem, p, TILE));
-    }
-    int info = 0;
-    CK(cudaMemcpyAsync(&info, h->info_dev, sizeof(int), cudaMemcpyDeviceToHost, h->st));
-    CK(cudaStreamSynchronize(h->st));
-    profile_collect(h);
-    if (info != INT_MAX) {
-        h->factored = false;
-        char buf[128];
-        snprintf(buf, sizeof buf, "append: extended matrix is not positive definite; leading minor %d", info);
-        h->err = buf;
-        return info > h->N ? (int)h->N : info;
-    }
-    return GPB200_OK;
+    CK(cholesky(h, c0, TILE));
+    return factor_end(L, "append: extended ", false);
 }
 
 // ---- cross-validation on the resident inverse (src/crossvalidation.jl) --------------------------------------------
@@ -2274,31 +2227,10 @@ int gpb200_group_create(gpb200_handle** hs, int n) {
 // staging buffers and only M x M state persists (H7 of SURVEY.md §7.2): per chunk a cross-Gram, a
 // recursive TRSM against L_uu for diag(Q_ff), and one rank-Nc SYRK into Sigma_QR -- all on the DMMA GEMM.
 // ================================================================================================
-#define FCK(call)                                                                                  \
-    do {                                                                                           \
-        cudaError_t e_ = (call);                                                                   \
-        if (e_ != cudaSuccess) {                                                                   \
-            char buf_[512];                                                                        \
-            snprintf(buf_, sizeof buf_, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,       \
-                     cudaGetErrorString(e_));                                                      \
-            f->err = buf_;                                                                         \
-            (void)cudaGetLastError();                                                              \
-            return GPB200_ECUDA;                                                                   \
-        }                                                                                          \
-    } while (0)
 #define FSUB(call, who)                                                                            \
     do {                                                                                           \
         int rc_ = (call);                                                                          \
         if (rc_ != GPB200_OK) { f->err = std::string(#call) + ": " + (who)->err; return rc_; }     \
-    } while (0)
-
-#define FCKN(call)                                                                                 \
-    do {                                                                                           \
-        ncclResult_t r_ = (call);                                                                  \
-        if (r_ != ncclSuccess) {                                                                   \
-            f->err = std::string(#call) + ": " + (g_nccl.GetErrorString ? g_nccl.GetErrorString(r_) : "nccl error"); \
-            return GPB200_ENCCL;                                                                   \
-        }                                                                                          \
     } while (0)
 // in-place sum over the ranks of a device vector (no-op on one rank)
 static int fitc_allreduce(gpb200_fitc* f, double* v, size_t n) {

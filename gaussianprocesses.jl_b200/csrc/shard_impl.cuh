@@ -130,31 +130,6 @@ bool multi_rank(gpb200_handle* h) { return h->nranks > 1; }
 ShardOwn own_of(gpb200_handle* h) { return ShardOwn{h->nranks, h->rank, h->rb}; }
 int owner_of_tile(gpb200_handle* h, long long t) { return (int)((t / h->rb) % h->nranks); }
 
-#define SCK(hh, call)                                                                               \
-    do {                                                                                            \
-        cudaError_t e_ = (call);                                                                    \
-        if (e_ != cudaSuccess) {                                                                    \
-            char buf_[512];                                                                         \
-            snprintf(buf_, sizeof buf_, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); \
-            (hh)->err = buf_;                                                                       \
-            (void)cudaGetLastError();                                                               \
-            return GPB200_ECUDA;                                                                    \
-        }                                                                                           \
-    } while (0)
-#define SCKN(hh, call)                                                                              \
-    do {                                                                                            \
-        ncclResult_t r_ = (call);                                                                   \
-        if (r_ != ncclSuccess) {                                                                    \
-            char buf_[512];                                                                         \
-            snprintf(buf_, sizeof buf_, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,        \
-                     g_nccl.GetErrorString ? g_nccl.GetErrorString(r_) : "nccl error");             \
-            (hh)->err = buf_;                                                                       \
-            return GPB200_ENCCL;                                                                    \
-        }                                                                                           \
-    } while (0)
-#define SRC(call)                                                                                   \
-    do { int rc_ = (call); if (rc_ != GPB200_OK) return rc_; } while (0)
-
 cudaEvent_t ring_event(gpb200_handle* h) {
     if (h->evring.empty()) {
         h->evring.resize(128);
@@ -343,8 +318,8 @@ int alloc_FG_sharded(gpb200_handle* h) {
     for (long long t = 0; t < tiles; ++t)
         if (owner_of_tile(h, t) == h->rank) want.push_back({(size_t)t * TILE * rowb, (size_t)TILE * rowb});
     h->sharded = true;                                          // so that a failure below is cleaned up by free_FG
-    SRC(vm_alloc(h, h->vmF, Np * rowb, want));
-    SRC(vm_alloc(h, h->vmG, Np * rowb, want));
+    TRY(vm_alloc(h, h->vmF, Np * rowb, want));
+    TRY(vm_alloc(h, h->vmG, Np * rowb, want));
     h->F = (double*)h->vmF.base;
     h->G = (double*)h->vmG.base;
     const size_t nbp = (size_t)shard_panel_width(h);
@@ -450,7 +425,7 @@ int shard_cholesky_la(const Locals& L, int kb0 = 0) {
     const int nblk = (Np + NBp - 1) / NBp;
     const long long tiles = Np / TILE;
     for (auto* q : L) {
-        if (!q->st_side) return fail(q, GPB200_ECUDA, "sharded look-ahead needs the side stream");
+        if (!q->st_side) return rank_failed(q, fail(q, GPB200_ECUDA, "sharded look-ahead needs the side stream"));
         cudaEvent_t e = ring_event(q);                       // the chain starts after the Gram build
         SCK(q, cudaEventRecord(e, q->st));
         SCK(q, cudaStreamWaitEvent(q->st_side, e, 0));
@@ -469,9 +444,9 @@ int shard_cholesky_la(const Locals& L, int kb0 = 0) {
                 q->lookahead = 0; q->row_lim = r1;
                 cudaError_t e = chol_panel(q, c0, nb, NBp);
                 q->row_lim = 0; q->lookahead = la;
-                if (e != cudaSuccess) { q->err = std::string("chol_panel: ") + cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
+                if (e != cudaSuccess) { q->err = std::string("chol_panel: ") + cudaGetErrorString(e); rc = rank_failed(q, GPB200_ECUDA); break; }
                 e = shard_copy_lower(q->P[pb] + (size_t)c0 * NBp, NBp, q->F + (size_t)c0 * q->ld + c0, q->ld, nb, q->st, &q->launches);
-                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
+                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = rank_failed(q, GPB200_ECUDA); break; }
             }
             if (rc) break;
             if ((rc = coll_group_begin(L))) break;
@@ -488,7 +463,7 @@ int shard_cholesky_la(const Locals& L, int kb0 = 0) {
             for (auto* q : L) {
                 cudaError_t e = shard_trsm_rows(q, c0, r1, 0, nb, pb);
                 if (e == cudaSuccess) e = shard_scatter_rows(q->G, q->F, q->ld, Np, c0, nb, t1, q->Sbuf + (size_t)q->rank * per, NBp, own_of(q), q->st, &q->launches);
-                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
+                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = rank_failed(q, GPB200_ECUDA); break; }
             }
             if (rc) break;
             if ((rc = coll_allgather(L, [&](gpb200_handle* q) { return (void*)q->Sbuf; }, sizeof(double) * per))) break;
@@ -497,17 +472,17 @@ int shard_cholesky_la(const Locals& L, int kb0 = 0) {
                 if (e == cudaSuccess && q->rank == o) {
                     e = shard_transpose(q->F + (size_t)c0 * q->ld + r1, q->ld, q->P[pb] + (size_t)r1 * NBp, NBp, Np - r1, nb, q->st, &q->launches);
                 }
-                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
+                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = rank_failed(q, GPB200_ECUDA); break; }
             }
         } while (false);
         if (!rc) {
             for (size_t i = 0; i < L.size(); ++i) {
                 ev_panel[i] = ring_event(L[i]);
-                if (cudaEventRecord(ev_panel[i], L[i]->st) != cudaSuccess) { L[i]->err = "cudaEventRecord failed"; rc = GPB200_ECUDA; }
+                if (cudaEventRecord(ev_panel[i], L[i]->st) != cudaSuccess) { L[i]->err = "cudaEventRecord failed"; rc = rank_failed(L[i], GPB200_ECUDA); }
             }
         }
         for (auto* q : L) std::swap(q->st, q->st_side);           // back to the main streams
-        if (rc) { if (L[0]->err.empty()) for (auto* q : L) if (!q->err.empty()) { L[0]->err = q->err; break; } return rc; }
+        if (rc) return rc;
         if (r1 >= Np) {
             for (size_t i = 0; i < L.size(); ++i) SCK(L[i], cudaStreamWaitEvent(L[i]->st, ev_panel[i], 0));
             break;
@@ -568,7 +543,7 @@ int shard_solve(const Locals& L, double* gpb200_handle::*rhs, double* gpb200_han
             }
             SCK(q, trsv_lower_fwd(q->F + (size_t)c0 * q->ld + c0, q->ld, q->Dinv + (size_t)c0 * TILE, t, y + c0, nb, q->st, &q->launches));
         }
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->*ybuf + c0); }, sizeof(double) * (size_t)nb));
+        TRY(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->*ybuf + c0); }, sizeof(double) * (size_t)nb));
     }
     // backward: U a = y on the rows of U = L' (upper part of F)
     for (int k = nblk - 1; k >= 0; --k) {
@@ -585,7 +560,7 @@ int shard_solve(const Locals& L, double* gpb200_handle::*rhs, double* gpb200_han
             }
             SCK(q, trsv_lower_bwd(q->F + (size_t)c0 * q->ld + c0, q->ld, q->DinvT + (size_t)c0 * TILE, t, a + c0, nb, q->st, &q->launches));
         }
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->*out + c0); }, sizeof(double) * (size_t)nb));
+        TRY(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->*out + c0); }, sizeof(double) * (size_t)nb));
     }
     return GPB200_OK;
 }
@@ -602,7 +577,7 @@ int shard_inverse_la(const Locals& L) {
     const int nblk = (Np + NBp - 1) / NBp;
     const size_t nl = L.size();
     for (auto* q : L) {
-        if (!q->st_side) return fail(q, GPB200_ECUDA, "sharded look-ahead needs the side stream");
+        if (!q->st_side) return rank_failed(q, fail(q, GPB200_ECUDA, "sharded look-ahead needs the side stream"));
         for (auto& run : q->vmG.runs) SCK(q, cudaMemsetAsync((char*)q->G + run.first, 0, run.second, q->st));
         // W_kk = L_kk^-1 of the own diagonal blocks, level by level (strictly-lower tiles -> G lower, transposed -> G upper;
         // the diagonal tiles stay in Dinv / DinvT, substituted by the GEMM producer)
@@ -659,7 +634,7 @@ int shard_inverse_la(const Locals& L) {
                     if (e == cudaSuccess) e = launch_gemm(q, g);
                 }
                 if (e == cudaSuccess) e = shard_pack_wblock(q->P[2 * set], NBp, q->G, q->ld, q->Dinv, j0, nb, q->st, &q->launches);
-                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
+                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = rank_failed(q, GPB200_ECUDA); break; }
             }
             if (rc) break;
             if ((rc = coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->P[2 * set] + (size_t)j0 * NBp); },
@@ -679,17 +654,17 @@ int shard_inverse_la(const Locals& L) {
                     g.alpha = 1.0; g.beta = 1.0;
                     if (e == cudaSuccess) e = launch_gemm(q, g);
                 }
-                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = GPB200_ECUDA; break; }
+                if (e != cudaSuccess) { q->err = cudaGetErrorString(e); rc = rank_failed(q, GPB200_ECUDA); break; }
             }
         } while (false);
         if (!rc) {
             for (size_t i = 0; i < nl; ++i) {
                 ev_panel[i] = ring_event(L[i]);
-                if (cudaEventRecord(ev_panel[i], L[i]->st) != cudaSuccess) { L[i]->err = "cudaEventRecord failed"; rc = GPB200_ECUDA; }
+                if (cudaEventRecord(ev_panel[i], L[i]->st) != cudaSuccess) { L[i]->err = "cudaEventRecord failed"; rc = rank_failed(L[i], GPB200_ECUDA); }
             }
         }
         for (auto* q : L) std::swap(q->st, q->st_side);
-        if (rc) { if (L[0]->err.empty()) for (auto* q : L) if (!q->err.empty()) { L[0]->err = q->err; break; } return rc; }
+        if (rc) return rc;
         // ---------------- main streams: bulk of panel k ----------------
         for (size_t i = 0; i < nl; ++i) {
             gpb200_handle* q = L[i];
@@ -739,7 +714,7 @@ int shard_predict_solve(const Locals& L, int Mpad, int64_t Mc, bool want_var, bo
             SCK(q, cudaMemcpy2DAsync(q->P[0], sizeof(double) * NBp, q->Kst + c0, sizeof(double) * q->Npad, sizeof(double) * nb,
                                      (size_t)Mpad, cudaMemcpyDeviceToDevice, q->st));
         }
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->P[0]; }, sizeof(double) * (size_t)Mpad * NBp));
+        TRY(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->P[0]; }, sizeof(double) * (size_t)Mpad * NBp));
         for (auto* q : L) {
             if (want_var) SCK(q, rowvar_launch(q->P[0], NBp, q->pvar, Mc, nb, q->pvar, q->st, &q->launches));
             if (r1 < Np) {
@@ -782,7 +757,7 @@ int shard_append_solve(const Locals& L, int b0, int Mv) {
                                      (size_t)Mv, cudaMemcpyDeviceToDevice, q->st));
             SCK(q, shard_transpose(q->F + (size_t)c0 * q->ld + b0, q->ld, q->P[0], NBp, Mv, NBp, q->st, &q->launches));
         }
-        SRC(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->P[0]; }, sizeof(double) * (size_t)Mv * NBp));
+        TRY(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->P[0]; }, sizeof(double) * (size_t)Mv * NBp));
         for (auto* q : L) {
             if (q->rank != o)
                 SCK(q, cudaMemcpy2DAsync(q->Kst + c0, sizeof(double) * q->Npad, q->P[0], sizeof(double) * NBp, sizeof(double) * NBp,
@@ -811,20 +786,16 @@ int shard_append(const Locals& L, int64_t Nold) {
     const int Np = (int)h0->Npad, NBp = shard_panel_width(h0);
     const int b0 = (int)(Nold / NBp * NBp);
     const int Mv = (int)((h0->N + TILE - 1) / TILE * TILE) - b0;
-    const int init = INT_MAX;
-    for (auto* q : L) {
-        SCK(q, cudaMemcpyAsync(q->info_dev, &init, sizeof(int), cudaMemcpyHostToDevice, q->st));
-        // own Gram rows >= b0 (columns <= row), identity beyond the new N
+    for (auto* q : L)        // own Gram rows >= b0 (columns <= row), identity beyond the new N
         SCK(q, gram_lower_launch(q->prog, q->x, q->d, q->d, q->N, Np, q->noise_var, 1, q->nugget, q->G, q->ld, q->st, &q->launches,
                                  q->rb, q->nranks, q->rank, 1, b0 / TILE));
-    }
     if (b0 > 0) {
         for (auto* q : L) {
-            SRC(ensure_predict_ws(q, Mv, false));
+            TRY(rank_failed(q, ensure_predict_ws(q, Mv, false)));
             SCK(q, crossgram_launch(q->prog, q->x + (size_t)b0 * q->d, q->d, q->N - b0, Mv, q->x, q->d, b0, b0, q->d, q->Kst, q->Npad,
                                     q->st, &q->launches));
         }
-        SRC(shard_append_solve(L, b0, Mv));
+        TRY(shard_append_solve(L, b0, Mv));
         for (auto* q : L) {
             // own rows of V are the rows of L left of b0
             for (long long t = b0 / TILE; t < (b0 + Mv) / TILE; ++t)
