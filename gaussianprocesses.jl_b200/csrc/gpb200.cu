@@ -89,7 +89,7 @@ struct gpb200_handle {
     bool cv_m_ok = false;                                       // cvD holds M_j = Z_j K^-1 of the last cv_param call
     double *cvD = nullptr, *cvY = nullptr;
     CUtensorMap mapCvD{}, mapCvY{};
-    double* cvblk = nullptr; long long* cvidx = nullptr; int64_t cvblk_cap = 0;
+    double* cvblk = nullptr; long long* cvidx = nullptr; int64_t cvblk_cap = 0, cvidx_cap = 0;   // capacities in elements
     // posterior sampling (gpb200_rand): M x M sub-engine for chol(Sigma* + nugget I), normal draws / samples staging
     gpb200_handle* sub = nullptr;
     bool cov_keep_device = false;              // predict: leave the full covariance in Kss (no D2H)
@@ -153,6 +153,8 @@ struct gpb200_handle {
     int rb = 4;                                // effective ownership block (tiles); panel width NBp = 128 * rb
     int row_lim = 0;                           // chol_panel: rows below this limit only (diagonal block of a sharded panel); 0 = Npad
     VmBuf vmF, vmG;
+    VmBuf vmCvY, vmCvM;                        // cross-validation work matrices (Y' = K^-1 dK_j, lower triangle of M_j), own rows only
+    CUtensorMap mapShCvY{}, mapShCvM{};
     double* P[4] = {nullptr, nullptr, nullptr, nullptr};   // panel buffers, Npad x NBp (global row order); P[1], P[3] double as NBp x Npad row panels
     double* Sbuf = nullptr;                    // all-gather staging: nranks regions of S_per_rank doubles; scratch of the inverse sweep
     size_t S_per_rank = 0;
@@ -301,7 +303,7 @@ void free_data(gpb200_handle* h) {
     if (h->cvY) cudaFree(h->cvY);
     if (h->cvblk) cudaFree(h->cvblk);
     if (h->cvidx) cudaFree(h->cvidx);
-    h->cvD = h->cvY = h->cvblk = nullptr; h->cvidx = nullptr; h->cvblk_cap = 0; h->g_sym = false; h->cv_m_ok = false;
+    h->cvD = h->cvY = h->cvblk = nullptr; h->cvidx = nullptr; h->cvblk_cap = h->cvidx_cap = 0; h->g_sym = false; h->cv_m_ok = false;
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     if (h->info_dev) { cudaFree(h->info_dev); h->info_dev = nullptr; }
     if (h->flags) { cudaFree(h->flags); h->flags = nullptr; }
@@ -1791,9 +1793,16 @@ int gpb200_append(gpb200_handle* h, int64_t k, const double* xnew, int64_t ldx) 
 // (crossvalidation.jl:86-108, 270-283).  Here K_y^-1 already sits on the device after gpb200_grad_prepare; per parameter:
 // D = dK_j (recomputed from x), Y' = K^-1 D, M_j = Y' K^-1 -- two NT DMMA GEMMs -- and the two N-vectors every LOO / fold
 // formula needs: Z_j alpha = Y' alpha and diag(M_j).  Fold formulas read principal sub-blocks through gpb200_cv_block.
-static int cv_prepare(gpb200_handle* h) {
+// Row-sharded handles run the same steps over the ranks (shard_cv_* in shard_impl.cuh) and keep only the lower triangle of M_j.
+static int cv_check(gpb200_handle* h) {
     if (!h->inv_ready) return fail(h, GPB200_ESTATE, "cv: grad_prepare first (K_y^-1 must be resident)");
-    if (h->nranks > 1) return fail(h, GPB200_ESTATE, "cv: K^-1 is distributed over the ranks; single-GPU handles only");
+    if (h->nranks > 1 && !h->sharded)
+        return fail(h, GPB200_ESTATE, "cv: K^-1 is distributed over the ranks; multi-rank handles need row-sharded storage (option \"shard\" = 1)");
+    return GPB200_OK;
+}
+
+static int cv_prepare(gpb200_handle* h) {
+    TRY(cv_check(h));
     const size_t nn = sizeof(double) * (size_t)h->Npad * (size_t)h->Npad;
     if (!h->cvD || !h->cvY) {
         if (h->cvD) { cudaFree(h->cvD); h->cvD = nullptr; }
@@ -1816,11 +1825,64 @@ static int cv_prepare(gpb200_handle* h) {
     return GPB200_OK;
 }
 
+// the N-vectors of the compact own-row values in Sbuf (`width` per row): all-gathered, read back on this rank, unpacked
+static int shard_own_vectors(const Locals& L, size_t per, int width, double* out0, double* out1) {
+    gpb200_handle* h = L[0];
+    TRY(coll_allgather(L, [&](gpb200_handle* q) { return (void*)q->Sbuf; }, sizeof(double) * per));
+    std::vector<double> buf(per * (size_t)h->nranks);
+    CK(cudaMemcpyAsync(buf.data(), h->Sbuf, sizeof(double) * buf.size(), cudaMemcpyDeviceToHost, h->st));
+    TRY(sync_all(L));
+    unpack_own_rows(h, buf, per, width, 0, out0);
+    if (out1) unpack_own_rows(h, buf, per, width, 1, out1);
+    return GPB200_OK;
+}
+
+static int shard_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double* Zj_alpha, double* diag_ZjSinv) {
+    Locals L;
+    TRY(shard_entry(h, L));
+    TRY(cv_check(h));
+    TRY(shard_cv_alloc(L));
+    if (!h->g_sym) {
+        TRY(shard_cv_symmetrize(L));
+        h->g_sym = true;
+    }
+    if (alpha) {
+        for (auto* q : L) {
+            TRY(rank_failed(q, upload_padded(q, q->alpha, alpha)));
+            q->alpha_ready = true;
+        }
+    }
+    h->cv_m_ok = false;
+    if (param >= 0) TRY(shard_cv_y(L, param));
+    const size_t per = 2 * (size_t)shard_own_rows(h->N, ShardOwn{h->nranks, 0, h->rb});      // rank 0 owns the most rows
+    for (auto* q : L)
+        SCK(q, shard_rowdot_own(param >= 0 ? cv_y(q) : q->G, q->G, q->ld, q->Npad, q->alpha, q->N, own_of(q), q->Sbuf + (size_t)q->rank * per,
+                                q->st, &q->launches));
+    TRY(shard_cv_m(L, param < 0));
+    TRY(shard_own_vectors(L, per, 2, Zj_alpha, diag_ZjSinv));
+    for (auto* q : L) profile_collect(q);
+    h->cv_m_ok = true;
+    return GPB200_OK;
+}
+
+// principal sub-block workspace: nV indices, `elems` doubles
+static int ensure_cv_block_ws(gpb200_handle* h, int64_t nV, int64_t elems) {
+    if (nV <= h->cvidx_cap && elems <= h->cvblk_cap) return GPB200_OK;
+    if (h->cvblk) cudaFree(h->cvblk);
+    if (h->cvidx) cudaFree(h->cvidx);
+    h->cvblk = nullptr; h->cvidx = nullptr; h->cvblk_cap = h->cvidx_cap = 0;
+    CK(cudaMalloc(&h->cvblk, sizeof(double) * elems));
+    CK(cudaMalloc(&h->cvidx, sizeof(long long) * nV));
+    h->cvblk_cap = elems; h->cvidx_cap = nV;
+    return GPB200_OK;
+}
+
 int gpb200_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double* Zj_alpha, double* diag_ZjSinv) {
     if (!h || !Zj_alpha || !diag_ZjSinv) return GPB200_EINVAL;
     if (param < -1 || param >= h->prog.n_theta) return fail(h, GPB200_EINVAL, "cv_param: parameter index out of range");
     if (!alpha && !h->alpha_ready) return fail(h, GPB200_ESTATE, "cv_param: no alpha (call mll or pass alpha)");
     CK(cudaSetDevice(h->device));
+    if (h->sharded) return shard_cv_param(h, param, alpha, Zj_alpha, diag_ZjSinv);
     int rc = cv_prepare(h);
     if (rc) return rc;
     if (alpha) { rc = upload_padded(h, h->alpha, alpha); if (rc) return rc; h->alpha_ready = true; }
@@ -1857,20 +1919,32 @@ int gpb200_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double
 int gpb200_cv_block(gpb200_handle* h, int32_t which, int64_t nV, const int64_t* idx, double* out) {
     if (!h || !idx || !out || nV <= 0 || which < 0 || which > 1) return GPB200_EINVAL;
     CK(cudaSetDevice(h->device));
+    static_assert(sizeof(long long) == sizeof(int64_t), "index width");
+    if (h->sharded) {
+        // every rank reads the entries whose row (of the stored lower triangle) it owns, zeros elsewhere; one sum over the ranks
+        Locals L;
+        TRY(shard_entry(h, L));
+        TRY(cv_check(h));
+        if (which == 1 && !h->cv_m_ok) return fail(h, GPB200_ESTATE, "cv_block: which = 1 reads M_j of the last cv_param call; call cv_param first");
+        for (int64_t a = 0; a < nV; ++a)
+            if (idx[a] < 0 || idx[a] >= h->N) return fail(h, GPB200_EINVAL, "cv_block: index out of range");
+        const size_t nn = (size_t)nV * (size_t)nV;
+        const int64_t elems = (int64_t)nn * (1 + (h->grp ? h->nranks : 0));       // + the group's all-reduce scratch
+        for (auto* q : L) {
+            TRY(rank_failed(q, ensure_cv_block_ws(q, nV, elems)));
+            SCK(q, cudaMemcpyAsync(q->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, q->st));
+            SCK(q, shard_gather_block_own(q->cvblk, which == 0 ? q->G : cv_m(q), q->ld, q->cvidx, nV, own_of(q), q->st, &q->launches));
+        }
+        TRY(coll_allreduce_sum(L, [&](gpb200_handle* q) { return q->cvblk; }, nn, [&](gpb200_handle* q) { return q->cvblk + nn; }));
+        CK(cudaMemcpyAsync(out, h->cvblk, sizeof(double) * nn, cudaMemcpyDeviceToHost, h->st));
+        return sync_all(L);
+    }
     int rc = cv_prepare(h);
     if (rc) return rc;
     if (which == 1 && !h->cv_m_ok) return fail(h, GPB200_ESTATE, "cv_block: which = 1 reads M_j of the last cv_param call; call cv_param first");
     for (int64_t a = 0; a < nV; ++a)
         if (idx[a] < 0 || idx[a] >= h->N) return fail(h, GPB200_EINVAL, "cv_block: index out of range");
-    if (nV > h->cvblk_cap) {
-        if (h->cvblk) cudaFree(h->cvblk);
-        if (h->cvidx) cudaFree(h->cvidx);
-        h->cvblk = nullptr; h->cvidx = nullptr; h->cvblk_cap = 0;
-        CK(cudaMalloc(&h->cvblk, sizeof(double) * nV * nV));
-        CK(cudaMalloc(&h->cvidx, sizeof(long long) * nV));
-        h->cvblk_cap = nV;
-    }
-    static_assert(sizeof(long long) == sizeof(int64_t), "index width");
+    TRY(ensure_cv_block_ws(h, nV, nV * nV));
     CK(cudaMemcpyAsync(h->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, h->st));
     CK(gather_block_launch(h->cvblk, which == 0 ? h->G : h->cvD, h->Npad, h->cvidx, nV, h->st, &h->launches));
     CK(cudaMemcpyAsync(out, h->cvblk, sizeof(double) * nV * nV, cudaMemcpyDeviceToHost, h->st));
@@ -1933,8 +2007,16 @@ int gpb200_get_inverse(gpb200_handle* h, double* Kinv) {
 int gpb200_get_inverse_diag(gpb200_handle* h, double* diag) {
     if (!h || !diag) return GPB200_EINVAL;
     if (!h->inv_ready) return fail(h, GPB200_ESTATE, "get_inverse_diag: grad_prepare first");
-    if (h->nranks > 1) return fail(h, GPB200_ESTATE, "get_inverse_diag: K^-1 is distributed over the ranks");
+    if (h->nranks > 1 && !h->sharded)
+        return fail(h, GPB200_ESTATE, "get_inverse_diag: K^-1 is distributed over the ranks; multi-rank handles need row-sharded storage (option \"shard\" = 1)");
     CK(cudaSetDevice(h->device));
+    if (h->sharded) {           // own diagonal entries (copies), all-gathered
+        Locals L;
+        TRY(shard_entry(h, L));
+        const size_t per = (size_t)shard_own_rows(h->N, ShardOwn{h->nranks, 0, h->rb});
+        for (auto* q : L) SCK(q, shard_diag_own(q->G, q->ld, q->N, own_of(q), q->Sbuf + (size_t)q->rank * per, q->st, &q->launches));
+        return shard_own_vectors(L, per, 1, diag, nullptr);
+    }
     // strided gather of G[i,i]: pitch (ld+1) doubles, one double per row
     CK(cudaMemcpy2DAsync(diag, sizeof(double), h->G, sizeof(double) * (h->ld + 1), sizeof(double), h->N,
                          cudaMemcpyDeviceToHost, h->st));
@@ -2198,6 +2280,8 @@ int gpb200_storage_info(gpb200_handle* h, int64_t* out, int32_t n) {
     v[3] = h->sharded ? h->rb : 0;
     v[4] = h->nranks;
     v[5] = h->rank;
+    v[7] = h->sharded ? (int64_t)(vm_mapped_bytes(h->vmCvY) + vm_mapped_bytes(h->vmCvM))
+                      : (h->cvD && h->cvY ? 2 * (int64_t)sizeof(double) * h->Npad * h->Npad : 0);
     for (int i = 0; i < n && i < 8; ++i) out[i] = v[i];
     return GPB200_OK;
 }

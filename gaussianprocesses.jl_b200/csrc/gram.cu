@@ -225,10 +225,12 @@ __global__ void __launch_bounds__(NT) gram_full_kernel(const __grid_constant__ K
 }
 
 // dK/dtheta_j as a full symmetric matrix (N_pad x N_pad, zero padding): grad_slice! of the reference
-// (/root/reference/src/kernels/kernels.jl:96-131), needed by the cross-validation gradients (src/crossvalidation.jl:67-170, 253-341)
+// (/root/reference/src/kernels/kernels.jl:96-131), needed by the cross-validation gradients (src/crossvalidation.jl:67-170, 253-341).
+// Tile row blockIdx.y holds global tile row bm0 + blockIdx.y: a row-sharded handle generates D in row batches (D points at row bm0 * 128).
 __global__ void __launch_bounds__(NT) gram_grad_full_kernel(const __grid_constant__ KProg P, const double* __restrict__ x, long long ldx,
-                                                            long long N, int d, int j, double* __restrict__ D, long long ldd) {
-    const int bm = blockIdx.y, bn = blockIdx.x;
+                                                            long long N, int d, int j, double* __restrict__ D, long long ldd, int bm0) {
+    const int bm = bm0 + blockIdx.y, bn = blockIdx.x;
+    D += (long long)blockIdx.y * TB * ldd;
     extern __shared__ double sm[];
     const int ds = d | 1;
     double* sXi = sm;
@@ -249,7 +251,7 @@ __global__ void __launch_bounds__(NT) gram_grad_full_kernel(const __grid_constan
             const long long gj = (long long)bn * TB + c;
             double v = 0.0;
             if (gi < N && gj < N) { kprog_eval<true>(P, xi, sXj + c * ds, gbuf); v = gbuf[j]; }
-            D[gi * ldd + gj] = v;
+            D[r * ldd + gj] = v;
         }
     }
 }
@@ -575,13 +577,16 @@ cudaError_t kdiag_grad_launch(const KProg& P, const double* x, int64_t ldx, int6
 }
 
 cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad, int j,
-                                  double* D, int64_t ldd, cudaStream_t st, int64_t* launches) {
+                                  double* D, int64_t ldd, cudaStream_t st, int64_t* launches, int64_t row0, int64_t rows) {
     if (j < 0 || j >= P.n_theta) return cudaErrorInvalidValue;
-    dim3 grid((unsigned)(Npad / TB), (unsigned)(Npad / TB));
+    if (rows < 0) rows = Npad - row0;
+    if (row0 < 0 || row0 % TB || rows % TB || row0 + rows > Npad) return cudaErrorInvalidValue;
+    if (rows == 0) return cudaSuccess;
+    dim3 grid((unsigned)(Npad / TB), (unsigned)(rows / TB));
     const size_t sm = xtile_smem(d);
     cudaError_t e;
     if ((e = ensure_smem(gram_grad_full_kernel, sm)) != cudaSuccess) return e;
-    gram_grad_full_kernel<<<grid, NT, sm, st>>>(P, x, ldx, N, d, j, D, ldd);
+    gram_grad_full_kernel<<<grid, NT, sm, st>>>(P, x, ldx, N, d, j, D, ldd, (int)(row0 / TB));
     if (launches) ++*launches;
     return cudaGetLastError();
 }

@@ -28,6 +28,7 @@ cudaError_t trace_rect_launch(const KProg& P, const double* x1, int64_t ldx1, in
                               cudaStream_t st, int64_t* launches);
 cudaError_t kdiag_grad_launch(const KProg& P, const double* x, int64_t ldx, int64_t N, const double* gvec, double* out,
                               cudaStream_t st, int64_t* launches);
-// D[i, k] = dk(x_i, x_k)/dtheta_j, full N_pad x N_pad (zero padding)  -- grad_slice! (src/kernels/kernels.jl:96-131)
+// D[i, k] = dk(x_i, x_k)/dtheta_j, full N_pad x N_pad (zero padding)  -- grad_slice! (src/kernels/kernels.jl:96-131).
+// Rows row0 .. row0 + rows only (multiples of 128; rows < 0: to Npad), row row0 + r stored at D[r * ldd].
 cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad, int j,
-                                  double* D, int64_t ldd, cudaStream_t st, int64_t* launches);
+                                  double* D, int64_t ldd, cudaStream_t st, int64_t* launches, int64_t row0 = 0, int64_t rows = -1);

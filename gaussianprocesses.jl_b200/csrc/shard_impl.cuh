@@ -27,6 +27,8 @@
 //   append     rebuild from the ownership block b0 of the first touched tile: own Gram rows >= b0; V = K[b0.., :b0] L11^-T
 //              solved like the predict (the block owner also keeps each block's transpose as U rows of its old rows); own
 //              rows of V into L; Schur complement of the own rows (K = b0); the Cholesky above from block b0 / NBp on.
+//   CV         own rows of K^-1 completed to full rows once, then per parameter own rows of Y' = K^-1 dK_j and of the lower
+//              triangle of M_j = Y' K^-1 (see the section at the end; tests/test_shard_cv_model.py).
 // Collectives: NCCL (one process per GPU) or, for an in-process group of virtual ranks on ONE device
 // (gpb200_group_create: lets a 1-GPU box run the multi-rank schedules), event-ordered device-to-device copies.
 
@@ -201,9 +203,10 @@ int coll_allgather(const Locals& L, BufFn base, size_t per_bytes) {
             if (q != p) SCK(L[p], cudaStreamWaitEvent(L[p]->st, done[q], 0));
     return GPB200_OK;
 }
-// vec(q)[0..n) <- sum over ranks (n <= 4096); local groups sum in rank order (deterministic)
-template <class BufFn>
-int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n) {
+// vec(q)[0..n) <- sum over ranks; local groups gather the R vectors into scratch(q) (R * n doubles) and sum them in rank
+// order (deterministic)
+template <class BufFn, class ScratchFn>
+int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n, ScratchFn scratch) {
     gpb200_handle* h0 = L[0];
     const int R = h0->nranks;
     if (R <= 1 || n == 0) return GPB200_OK;
@@ -211,13 +214,12 @@ int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n) {
         SCKN(h0, g_nccl.AllReduce(vec(h0), vec(h0), n, ncclDouble, ncclSum, h0->comm, h0->st));
         return GPB200_OK;
     }
-    if (n > 4096) return fail(h0, GPB200_EINVAL, "coll_allreduce_sum: vector too long for the group scratch");
     std::vector<cudaEvent_t> ready(R), copied(R);
     for (int q = 0; q < R; ++q) { ready[q] = ring_event(L[q]); SCK(L[q], cudaEventRecord(ready[q], L[q]->st)); }
     for (int q = 0; q < R; ++q) {
         for (int p = 0; p < R; ++p) {
             if (p != q) SCK(L[q], cudaStreamWaitEvent(L[q]->st, ready[p], 0));
-            SCK(L[q], cudaMemcpyAsync(L[q]->red + (size_t)p * n, vec(L[p]), sizeof(double) * n, cudaMemcpyDeviceToDevice, L[q]->st));
+            SCK(L[q], cudaMemcpyAsync(scratch(L[q]) + (size_t)p * n, vec(L[p]), sizeof(double) * n, cudaMemcpyDeviceToDevice, L[q]->st));
         }
         copied[q] = ring_event(L[q]);
         SCK(L[q], cudaEventRecord(copied[q], L[q]->st));
@@ -225,9 +227,15 @@ int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n) {
     for (int q = 0; q < R; ++q) {
         for (int p = 0; p < R; ++p)
             if (p != q) SCK(L[q], cudaStreamWaitEvent(L[q]->st, copied[p], 0));
-        SCK(L[q], shard_sum_ranks(vec(L[q]), L[q]->red, (int64_t)n, R, (int64_t)n, L[q]->st, &L[q]->launches));
+        SCK(L[q], shard_sum_ranks(vec(L[q]), scratch(L[q]), (int64_t)n, R, (int64_t)n, L[q]->st, &L[q]->launches));
     }
     return GPB200_OK;
+}
+// the same through the group scratch `red` (n <= 4096)
+template <class BufFn>
+int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n) {
+    if (L[0]->grp && n > 4096) return fail(L[0], GPB200_EINVAL, "coll_allreduce_sum: vector too long for the group scratch");
+    return coll_allreduce_sum(L, vec, n, [](gpb200_handle* q) { return q->red; });
 }
 int coll_allreduce_min_info(const Locals& L) {
     gpb200_handle* h0 = L[0];
@@ -277,10 +285,12 @@ void shard_free_buffers(gpb200_handle* h) {
     h->Sbuf = h->red = nullptr; h->redi = nullptr; h->S_per_rank = 0;
 }
 
-// free F / G whatever their mode
+// free F / G whatever their mode (with the row-sharded cross-validation work matrices, which share their layout)
 void free_FG(gpb200_handle* h) {
     if (h->sharded) {
         vm_free(h->vmF); vm_free(h->vmG);
+        vm_free(h->vmCvY); vm_free(h->vmCvM);
+        h->g_sym = h->cv_m_ok = false;
         shard_free_buffers(h);
     } else {
         if (h->F) cudaFree(h->F);
@@ -309,14 +319,21 @@ int alloc_FG_replicated(gpb200_handle* h) {
     return GPB200_OK;
 }
 
+// byte ranges of the own 128-row tiles of an Npad x Npad row-major matrix
+std::vector<std::pair<size_t, size_t>> own_row_runs(gpb200_handle* h) {
+    const size_t rowb = (size_t)h->Npad * sizeof(double);
+    std::vector<std::pair<size_t, size_t>> want;
+    for (long long t = 0; t < h->Npad / TILE; ++t)
+        if (owner_of_tile(h, t) == h->rank) want.push_back({(size_t)t * TILE * rowb, (size_t)TILE * rowb});
+    return want;
+}
+
 int alloc_FG_sharded(gpb200_handle* h) {
     const size_t Np = (size_t)h->Npad;
     const size_t rowb = Np * sizeof(double);
     h->rb = shard_pick_rb(h);
-    std::vector<std::pair<size_t, size_t>> want;
+    const auto want = own_row_runs(h);
     const long long tiles = (long long)(Np / TILE);
-    for (long long t = 0; t < tiles; ++t)
-        if (owner_of_tile(h, t) == h->rank) want.push_back({(size_t)t * TILE * rowb, (size_t)TILE * rowb});
     h->sharded = true;                                          // so that a failure below is cleaned up by free_FG
     TRY(vm_alloc(h, h->vmF, Np * rowb, want));
     TRY(vm_alloc(h, h->vmG, Np * rowb, want));
@@ -816,4 +833,152 @@ int shard_append(const Locals& L, int64_t Nold) {
         }
     }
     return shard_cholesky_la(L, b0 / NBp);
+}
+
+// ---- cross-validation (gpb200_cv_param / cv_block / get_inverse_diag) ------------------------------------------------------
+// After the inverse sweep the lower part of an own row of G holds K^-1; its upper part is dead scratch.  Per grad_prepare the
+// rows are completed once (shard_cv_symmetrize); per parameter j (tests/test_shard_cv_model.py is the numpy specification):
+//   Y' own rows = K^-1[own, :] dK_j, dK_j generated by every rank itself in row batches of up to xr_batch * NBp rows (NT:
+//   dK_j is symmetric), no communication; Z_j alpha and diag(Z_j K^-1) are row-local (<Y'_i, alpha>, <K^-1_i, Y'_i>);
+//   M_j = Y' K^-1 own rows, lower triangle only (symmetric): the K^-1 row panels are broadcast batch by batch.
+// Communication: N^2 / 2 doubles once per grad_prepare, N^2 per cv_param, plus the N-vectors.
+double* cv_y(gpb200_handle* h) { return (double*)h->vmCvY.base; }
+double* cv_m(gpb200_handle* h) { return (double*)h->vmCvM.base; }
+GemmBuf bufCvY(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapShCvY : nullptr, cv_y(h), h->Npad}; }
+GemmBuf bufXRbig(gpb200_handle* h, int set) { return GemmBuf{h->tma_ok ? &h->mapXRbig[set] : nullptr, h->XRbig[set], h->Npad}; }
+
+// Y' and M_j of every rank, backed on the own rows like F and G; all ranks or none
+int shard_cv_alloc(const Locals& L) {
+    bool have = true;
+    for (auto* q : L) have = have && q->vmCvY.base && q->vmCvM.base;
+    if (have) return GPB200_OK;
+    for (auto* q : L) { SCK(q, cudaStreamSynchronize(q->st)); vm_free(q->vmCvY); vm_free(q->vmCvM); }
+    for (auto* q : L) {
+        const size_t total = sizeof(double) * (size_t)q->Npad * (size_t)q->Npad;
+        const auto want = own_row_runs(q);
+        int rc = vm_alloc(q, q->vmCvY, total, want);
+        if (!rc) rc = vm_alloc(q, q->vmCvM, total, want);
+        if (!rc && q->tma_ok && !(gemm_make_tensor_map(&q->mapShCvY, cv_y(q), q->Npad, q->Npad, q->Npad) &&
+                                  gemm_make_tensor_map(&q->mapShCvM, cv_m(q), q->Npad, q->Npad, q->Npad)))
+            rc = fail(q, GPB200_ECUDA, "cv: cuTensorMapEncodeTiled failed");
+        if (rc) {
+            for (auto* p : L) { vm_free(p->vmCvY); vm_free(p->vmCvM); }
+            return rank_failed(q, rc);
+        }
+    }
+    return GPB200_OK;
+}
+
+// every own row of G <- the full row of K^-1: the owner of panel k broadcasts K^-1[k, 0..c0) (staged in XRbig[0]); every rank
+// writes its transpose into the upper part of its own rows < c0; the owner mirrors inside the diagonal block
+int shard_cv_symmetrize(const Locals& L) {
+    gpb200_handle* h0 = L[0];
+    const int Np = (int)h0->Npad, R = h0->nranks, NBp = shard_panel_width(h0);
+    for (int k = 0; k * NBp < Np; ++k) {
+        const int c0 = k * NBp, nb = std::min(NBp, Np - c0), o = k % R;
+        if (c0 > 0) {
+            for (auto* q : L)
+                if (q->rank == o)
+                    SCK(q, cudaMemcpy2DAsync(q->XRbig[0], sizeof(double) * c0, q->G + (size_t)c0 * q->ld, sizeof(double) * q->ld,
+                                             sizeof(double) * c0, nb, cudaMemcpyDeviceToDevice, q->st));
+            TRY(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)q->XRbig[0]; }, sizeof(double) * (size_t)nb * c0));
+            for (auto* q : L)
+                SCK(q, shard_transpose_own(q->G + c0, q->ld, q->XRbig[0], c0, nb, c0, own_of(q), q->st, &q->launches));
+        }
+        for (auto* q : L)
+            if (q->rank == o) SCK(q, symmetrize_launch(q->G + (size_t)c0 * q->ld + c0, q->ld, nb, q->st, &q->launches));
+    }
+    return GPB200_OK;
+}
+
+// own rows of Y' = K^-1 dK_param, dK generated row batch by row batch into XRbig[0]
+int shard_cv_y(const Locals& L, int param) {
+    gpb200_handle* h0 = L[0];
+    const int Np = (int)h0->Npad, rows_b = h0->xr_batch * shard_panel_width(h0);
+    for (int n0 = 0; n0 < Np; n0 += rows_b) {
+        const int nr = std::min(rows_b, Np - n0);
+        for (auto* q : L) {
+            SCK(q, gram_grad_full_launch(q->prog, q->x, q->d, q->d, q->N, q->Npad, param, q->XRbig[0], q->Npad, q->st, &q->launches, n0, nr));
+            GemmDesc g = gemm_desc_default();
+            g.A = GemmOperand{bufG(q), bufNone(), 0, 0};
+            g.B = GemmOperand{bufXRbig(q, 0), bufNone(), 0, 0};
+            g.C = cv_y(q); g.ldc = q->Npad; g.c_row0 = 0; g.c_col0 = n0;
+            g.M = Np; g.N = nr; g.K = Np;
+            own_rows_filter(q, g, 0);
+            SCK(q, launch_gemm(q, g));
+        }
+    }
+    return GPB200_OK;
+}
+
+// own rows of the lower triangle of M_j = Y' K^-1 (Y' = K^-1 itself for the noise): per batch of K^-1 row panels (rows n0 ..
+// n0 + nr) the owners broadcast them into XRbig[b & 1] on the side streams, then one lower-trapezoid GEMM on the main streams.
+// The broadcast of batch b + 1 may run while the GEMM of batch b does; batch b + 2 reuses the set once GEMM b is done.
+int shard_cv_m(const Locals& L, bool noise) {
+    gpb200_handle* h0 = L[0];
+    const int Np = (int)h0->Npad, R = h0->nranks, NBp = shard_panel_width(h0), rows_b = h0->xr_batch * NBp;
+    const size_t nl = L.size();
+    // [set * nl + i]: the GEMM of the last batch that read XRbig[set] is done.  A ring event: between its record and its wait
+    // each rank takes at most 2 * (xr_batch + 1) <= 66 of the 128 ring events (one per panel broadcast, one per batch)
+    std::vector<cudaEvent_t> ev_free(2 * nl, nullptr);
+    int rc = GPB200_OK;
+    for (auto* q : L) {                                        // the side streams start after the main streams' work so far
+        cudaEvent_t e = ring_event(q);
+        if (cudaEventRecord(e, q->st) != cudaSuccess || cudaStreamWaitEvent(q->st_side, e, 0) != cudaSuccess) {
+            q->err = "cudaEventRecord failed"; rc = rank_failed(q, GPB200_ECUDA); break;
+        }
+    }
+    std::vector<cudaEvent_t> ev_ready(nl);
+    for (int b = 0, n0 = 0; !rc && n0 < Np; ++b, n0 += rows_b) {
+        const int nr = std::min(rows_b, Np - n0), set = b & 1;
+        for (size_t i = 0; i < nl; ++i) std::swap(L[i]->st, L[i]->st_side);
+        rc = [&]() -> int {
+            for (size_t i = 0; i < nl; ++i)
+                if (ev_free[set * nl + i]) SCK(L[i], cudaStreamWaitEvent(L[i]->st, ev_free[set * nl + i], 0));
+            for (int k = n0 / NBp; k * NBp < n0 + nr; ++k) {
+                const int c0 = k * NBp, nb = std::min(NBp, Np - c0), o = k % R;
+                for (auto* q : L)
+                    if (q->rank == o)
+                        SCK(q, cudaMemcpyAsync(q->XRbig[set] + (size_t)(c0 - n0) * Np, q->G + (size_t)c0 * q->ld,
+                                               sizeof(double) * (size_t)nb * Np, cudaMemcpyDeviceToDevice, q->st));
+                TRY(coll_bcast(L, o, [&](gpb200_handle* q) { return (void*)(q->XRbig[set] + (size_t)(c0 - n0) * Np); },
+                               sizeof(double) * (size_t)nb * Np));
+            }
+            for (size_t i = 0; i < nl; ++i) {
+                ev_ready[i] = ring_event(L[i]);
+                SCK(L[i], cudaEventRecord(ev_ready[i], L[i]->st));
+            }
+            return GPB200_OK;
+        }();
+        for (size_t i = 0; i < nl; ++i) std::swap(L[i]->st, L[i]->st_side);
+        if (rc) break;
+        rc = [&]() -> int {
+            for (size_t i = 0; i < nl; ++i) {
+                gpb200_handle* q = L[i];
+                SCK(q, cudaStreamWaitEvent(q->st, ev_ready[i], 0));
+                GemmDesc g = gemm_desc_default();
+                g.A = GemmOperand{noise ? bufG(q) : bufCvY(q), bufNone(), n0, 0};
+                g.B = GemmOperand{bufXRbig(q, set), bufNone(), 0, 0};
+                g.C = cv_m(q); g.ldc = q->Npad; g.c_row0 = n0; g.c_col0 = n0;
+                g.M = Np - n0; g.N = nr; g.K = Np;
+                g.flags = GEMM_LOWER_ONLY;
+                own_rows_filter(q, g, n0);
+                SCK(q, launch_gemm(q, g));
+                ev_free[set * nl + i] = ring_event(q);
+                SCK(q, cudaEventRecord(ev_free[set * nl + i], q->st));
+            }
+            return GPB200_OK;
+        }();
+    }
+    return rc;
+}
+
+// own rows r < N of the tiles covering 0 .. N, compact (shard_kernels.cuh) in region q of the all-gathered buffer -> out[r]
+void unpack_own_rows(gpb200_handle* h, const std::vector<double>& buf, size_t per, int width, int k, double* out) {
+    for (int64_t i = 0; i < h->N; ++i) {
+        const long long t = i / TILE;
+        const int q = owner_of_tile(h, t);
+        const long long li = shard_own_before(t, q, h->rb, h->nranks) * TILE + i % TILE;
+        out[i] = buf[(size_t)q * per + (size_t)li * width + k];
+    }
 }

@@ -80,6 +80,67 @@ __global__ void min_ranks_kernel(int* __restrict__ out, const int* __restrict__ 
     for (int q = 1; q < nranks; ++q) m = min(m, in[q]);
     out[0] = m;
 }
+
+// global tile index of this rank's lt-th own tile
+__device__ __forceinline__ long long own_tile(long long lt, const ShardOwn& own) {
+    return (lt / own.rb) * ((long long)own.rb * own.R) + (long long)own.me * own.rb + lt % own.rb;
+}
+
+// 32 x 32 blocks as in transpose_kernel; a block whose destination rows lie in another rank's tile exits (32 | 128: uniform)
+__global__ void transpose_own_kernel(double* __restrict__ dst, long long ldd, const double* __restrict__ src, long long lds,
+                                     long long rows, long long cols, ShardOwn own) {
+    __shared__ double tile[32][33];
+    const long long i0 = (long long)blockIdx.y * 32, j0 = (long long)blockIdx.x * 32;
+    if ((int)((j0 / T / own.rb) % own.R) != own.me) return;
+    for (int y = threadIdx.y; y < 32; y += 8) {
+        const long long i = i0 + y, j = j0 + threadIdx.x;
+        tile[y][threadIdx.x] = (i < rows && j < cols) ? src[i * lds + j] : 0.0;
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < 32; y += 8) {
+        const long long j = j0 + y, i = i0 + threadIdx.x;
+        if (i < rows && j < cols) dst[j * ldd + i] = tile[threadIdx.x][y];
+    }
+}
+
+// one CTA per own row (compact index li): the reduction order of rowdot_kernel / rowdot2_kernel (vec.cu), so every value is
+// bitwise the one a single-GPU handle computes from the same rows
+__global__ void __launch_bounds__(256) rowdot_own_kernel(const double* __restrict__ Y, const double* __restrict__ G, long long ld,
+                                                         long long ncols, const double* __restrict__ alpha, long long N, ShardOwn own,
+                                                         double* __restrict__ out) {
+    __shared__ double s[256], s2[256];
+    const long long li = blockIdx.x;
+    const long long r = own_tile(li / T, own) * T + li % T;
+    double v = 0.0, v2 = 0.0;
+    if (r < N) {
+        const double* ry = Y + r * ld;
+        const double* rg = G + r * ld;
+        for (long long c = threadIdx.x; c < ncols; c += 256) v += ry[c] * alpha[c];
+        for (long long c = threadIdx.x; c < ncols; c += 256) v2 += rg[c] * ry[c];
+    }
+    s[threadIdx.x] = v; s2[threadIdx.x] = v2;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) { s[threadIdx.x] += s[threadIdx.x + o]; s2[threadIdx.x] += s2[threadIdx.x + o]; }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) { out[2 * li] = s[0]; out[2 * li + 1] = s2[0]; }
+}
+
+__global__ void diag_own_kernel(const double* __restrict__ G, long long ld, long long n_own_rows, ShardOwn own, double* __restrict__ out) {
+    const long long li = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (li >= n_own_rows) return;
+    const long long r = own_tile(li / T, own) * T + li % T;
+    out[li] = G[r * ld + r];
+}
+
+__global__ void gather_block_own_kernel(double* __restrict__ out, const double* __restrict__ src, long long ld,
+                                        const long long* __restrict__ idx, long long nv, ShardOwn own) {
+    const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x, a = blockIdx.y;
+    if (b >= nv) return;
+    const long long r = max(idx[a], idx[b]), c = min(idx[a], idx[b]);
+    out[a * nv + b] = ((int)((r / T / own.rb) % own.R) == own.me) ? src[r * ld + c] : 0.0;
+}
 }  // namespace
 
 cudaError_t shard_copy_lower(double* dst, int64_t ldd, const double* src, int64_t lds, int n, cudaStream_t st, int64_t* launches) {
@@ -136,6 +197,45 @@ cudaError_t shard_sum_ranks(double* out, const double* in, int64_t stride, int n
 }
 cudaError_t shard_min_ranks(int* out, const int* in, int nranks, cudaStream_t st, int64_t* launches) {
     min_ranks_kernel<<<1, 1, 0, st>>>(out, in, nranks);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_transpose_own(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, ShardOwn own,
+                                cudaStream_t st, int64_t* launches) {
+    if (rows <= 0 || cols <= 0) return cudaSuccess;
+    dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32)), block(32, 8);
+    transpose_own_kernel<<<grid, block, 0, st>>>(dst, ldd, src, lds, rows, cols, own);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+int64_t shard_own_rows(int64_t n, ShardOwn own) {
+    return shard_own_before((n + T - 1) / T, own.me, own.rb, own.R) * T;
+}
+
+cudaError_t shard_rowdot_own(const double* Y, const double* G, int64_t ld, int64_t ncols, const double* alpha, int64_t N, ShardOwn own,
+                             double* out, cudaStream_t st, int64_t* launches) {
+    const int64_t n = shard_own_rows(N, own);
+    if (n <= 0) return cudaSuccess;
+    rowdot_own_kernel<<<(unsigned)n, 256, 0, st>>>(Y, G, ld, ncols, alpha, N, own, out);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_diag_own(const double* G, int64_t ld, int64_t N, ShardOwn own, double* out, cudaStream_t st, int64_t* launches) {
+    const int64_t n = shard_own_rows(N, own);
+    if (n <= 0) return cudaSuccess;
+    diag_own_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(G, ld, n, own, out);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_gather_block_own(double* out, const double* src, int64_t ld, const long long* idx, int64_t nv, ShardOwn own,
+                                   cudaStream_t st, int64_t* launches) {
+    if (nv <= 0) return cudaSuccess;
+    dim3 grid((unsigned)((nv + 255) / 256), (unsigned)nv);
+    gather_block_own_kernel<<<grid, 256, 0, st>>>(out, src, ld, idx, nv, own);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

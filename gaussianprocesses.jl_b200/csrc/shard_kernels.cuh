@@ -35,3 +35,20 @@ cudaError_t shard_pack_wblock(double* P, int nbp, const double* G, int64_t ld, c
 cudaError_t shard_sum_ranks(double* out, const double* in, int64_t stride, int nranks, int64_t n, cudaStream_t st, int64_t* launches);
 // out[0] = min_q in[q]
 cudaError_t shard_min_ranks(int* out, const int* in, int nranks, cudaStream_t st, int64_t* launches);
+
+// ---- cross-validation on row-sharded storage.  "Compact" vectors hold one entry per own row, own tiles in ascending order:
+// own row r of tile t sits at li = shard_own_before(t, me) * 128 + r % 128.
+// dst[j * ldd + i] = src[i * lds + j] for i < rows, j < cols, only where destination row j lies in an own tile
+cudaError_t shard_transpose_own(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, ShardOwn own,
+                                cudaStream_t st, int64_t* launches);
+// own rows in the tiles covering rows 0 .. n (length of the compact vectors)
+int64_t shard_own_rows(int64_t n, ShardOwn own);
+// own rows r < N: out[2 li] = <Y_r, alpha>, out[2 li + 1] = <G_r, Y_r> over ncols columns (0 for padding rows)
+cudaError_t shard_rowdot_own(const double* Y, const double* G, int64_t ld, int64_t ncols, const double* alpha, int64_t N, ShardOwn own,
+                             double* out, cudaStream_t st, int64_t* launches);
+// out[li] = G[r, r] for the own rows r of the tiles covering 0 .. N
+cudaError_t shard_diag_own(const double* G, int64_t ld, int64_t N, ShardOwn own, double* out, cudaStream_t st, int64_t* launches);
+// out[a * nv + b] = src[max(ia, ib) * ld + min(ia, ib)] where that row is own, else 0 (i* = idx[*]): summed over the ranks, the
+// exactly symmetric principal sub-block of a matrix whose lower triangle is stored
+cudaError_t shard_gather_block_own(double* out, const double* src, int64_t ld, const long long* idx, int64_t nv, ShardOwn own,
+                                   cudaStream_t st, int64_t* launches);

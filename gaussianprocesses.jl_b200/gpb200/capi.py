@@ -312,7 +312,7 @@ class Engine:
         v = (C.c_int64 * 8)()
         self._check(self._lib.gpb200_storage_info(self._h, v, 8), "storage_info")
         return dict(sharded=bool(v[0]), bytes_F=int(v[1]), bytes_G=int(v[2]), rb=int(v[3]), nranks=int(v[4]), rank=int(v[5]),
-                    tma=bool(v[6]))
+                    tma=bool(v[6]), bytes_cv=int(v[7]))
 
     def _own_rows_inverse(self):
         """sharded storage: this rank's rows of K^-1 (lower part valid), zeros elsewhere"""
@@ -593,6 +593,15 @@ class LocalGroupEngine:
     def rand(self, *a, **k):
         return self.lead.rand(*a, **k)
 
+    def cv_param(self, *a, **k):
+        return self.lead.cv_param(*a, **k)
+
+    def cv_block(self, *a, **k):
+        return self.lead.cv_block(*a, **k)
+
+    def inverse_diag(self):
+        return self.lead.inverse_diag()
+
     def append(self, xnew_pm):
         """the leader extends every rank's inputs and the distributed factor (ElasticGPE append!)"""
         self.lead.append(xnew_pm)
@@ -616,6 +625,3 @@ class LocalGroupEngine:
     def inverse(self):
         K = sum(e._own_rows_inverse() for e in self.engines)
         return np.tril(K) + np.tril(K, -1).T
-
-    def inverse_diag(self):
-        return np.diag(self.inverse()).copy()

@@ -153,14 +153,19 @@ int  gpb200_unwhiten(gpb200_handle* h, const double* v, double* f);
  * (GPB200_ESTATE otherwise).  The factor, logdet, solve, mll, predict, rand and append are unaffected.                   */
 int  gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, double* dll_process, double* dll_kernel);
 
-/* ---- cross-validation on the resident inverse (src/crossvalidation.jl; after gpb200_grad_prepare, single GPU) ------------
+/* ---- cross-validation on the resident inverse (src/crossvalidation.jl; after gpb200_grad_prepare) ------------------------
  * Per hyper-parameter the reference forms Z_j = inv(Sigma) dK_j and Z_j inv(Sigma) as host matrices (crossvalidation.jl:86-108,
  * 270-283).  gpb200_cv_param does the two N^3 products on the device and returns the two vectors the LOO formulas need:
  * Zj_alpha[N] = Z_j alpha and diag_ZjSinv[N] = diag(Z_j inv(Sigma)); `param` indexes the kernel's full parameter vector, -1 is the
- * noise variance (Z = inv(Sigma), crossvalidation.jl:124-126).  M_j = Z_j inv(Sigma) stays resident for gpb200_cv_block.        */
+ * noise variance (Z = inv(Sigma), crossvalidation.jl:124-126).  M_j = Z_j inv(Sigma) stays resident for gpb200_cv_block.
+ * Row-sharded handles (in-process groups, or NCCL ranks with option "shard" = 1) run the same steps over the ranks: every rank
+ * keeps its own rows of Z_j and of the lower triangle of M_j (3 N^3 flop split over the ranks instead of 4 N^3); call the
+ * leader of a group.  Replicated multi-rank handles return GPB200_ESTATE.  Repeated calls return bitwise equal vectors.      */
 int  gpb200_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double* Zj_alpha, double* diag_ZjSinv);
 /* principal sub-matrix on the index set idx[nV] (0-based) of inv(Sigma) (which = 0) or of the last M_j (which = 1), row-major
- * nV x nV: `Matrix(invΣ)[V,V]` / `ZjΣinv[V,V]` of predict_CVfold / gradient_fold (crossvalidation.jl:180-191, 248-262)     */
+ * nV x nV: `Matrix(invΣ)[V,V]` / `ZjΣinv[V,V]` of predict_CVfold / gradient_fold (crossvalidation.jl:180-191, 248-262).
+ * which = 1 before a gpb200_cv_param since the last factorize / append / grad_prepare: GPB200_ESTATE.  Row-sharded handles read
+ * every entry from the stored lower triangle and sum the ranks' pieces: the block is exactly symmetric.                    */
 int  gpb200_cv_block(gpb200_handle* h, int32_t which, int64_t nV, const int64_t* idx, double* out);
 
 /* ---- debug / introspection (Base.Matrix(::P), mat(::P), tests) ----------------------------- */
@@ -168,7 +173,8 @@ int  gpb200_get_gram(gpb200_handle* h, double* K);        /* N x N, K_y rebuilt 
 int  gpb200_get_factor(gpb200_handle* h, double* U);      /* N x N column-major upper U, K_y=U'U */
 int  gpb200_get_inverse(gpb200_handle* h, double* Kinv);  /* N x N, after gpb200_grad_prepare    */
 /* diag(K_y^-1)[N] after gpb200_grad_prepare: all predict_LOO / logp_LOO need besides alpha
- * (src/crossvalidation.jl:8-13, 37-49: sigma_i^2 = 1/[K^-1]_ii, mu_i = y_i - alpha_i sigma_i^2)  */
+ * (src/crossvalidation.jl:8-13, 37-49: sigma_i^2 = 1/[K^-1]_ii, mu_i = y_i - alpha_i sigma_i^2).  Row-sharded handles copy
+ * the own diagonal entries and all-gather them; replicated multi-rank handles return GPB200_ESTATE.                         */
 int  gpb200_get_inverse_diag(gpb200_handle* h, double* diag);
 /* per-phase device times (ms) of the last calls:
  * [0] gram  [1] cholesky  [2] solve+mll  [3] inverse (trtri+lauum; gpb200_gpa_grad: the merges only)  [4] trace  [5] predict
@@ -259,7 +265,9 @@ int  gpb200_ipc_import(gpb200_handle* h, int nranks, const char* all_blobs);
 int  gpb200_group_create(gpb200_handle** hs, int n);
 /* storage of the two N x N buffers of this handle: out[0] = 1 if row-sharded, out[1] / out[2] = bytes of F / G physically
  * backed on this device, out[3] = ownership block (tiles), out[4] = ranks, out[5] = rank, out[6] = 1 if the GEMMs run on
- * TMA descriptors (0: plain-load fallback)  (cf. test/memory.jl:14-19)                                              */
+ * TMA descriptors (0: plain-load fallback), out[7] = bytes of the cross-validation work matrices physically backed on this
+ * device (0 before the first gpb200_cv_param; 2 Npad^2 8 on one GPU, the own rows of two such matrices when row-sharded)
+ * (cf. test/memory.jl:14-19)                                                                                         */
 int  gpb200_storage_info(gpb200_handle* h, int64_t* out, int32_t n);
 
 /* ---- sparse FITC strategy (src/sparse/fully_indep_train_conditional.jl) ------------------------
