@@ -46,6 +46,7 @@
 #include "vec.cuh"
 #include "fsa.cuh"
 #include "gpa.cuh"
+#include "fitc_cv.cuh"
 
 namespace {
 constexpr int TILE = 128;
@@ -195,6 +196,22 @@ struct gpb200_fitc {
     CUtensorMap mapAt{}, mapC{}, mapCt{}, mapH{}, mapT{};
     bool grad_ws = false;
     double* Kss = nullptr; int64_t Kss_rows = 0;      // full predictive covariance (gpb200_fitc_predict_cov)
+    // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
+    // buffer the likelihood, gradient and prediction schedules keep):
+    //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
+    //   cvCh Nc x Mpad: Ch = L^-1 K_fu S^-1;  cvP Nc x Mpad: Ch Q (pass 2) or E (fold blocks)
+    //   Mpad x Mpad: cvDuu = dK_uu, cvDp = dK_uu K_uu^-1, cvR = K_uf L^-1 G, cvH = K_uf L^-1 Delta L^-1 K_fu, cvQ = H - R - R'
+    double *cvG = nullptr, *cvGt = nullptr, *cvCh = nullptr, *cvP = nullptr;
+    double *cvDuu = nullptr, *cvDp = nullptr, *cvR = nullptr, *cvH = nullptr, *cvQ = nullptr;
+    double *cvalpha = nullptr, *cvdel = nullptr, *cvilam = nullptr, *cvza = nullptr, *cvdg = nullptr;   // N + Nc
+    double *cvda = nullptr, *cvq = nullptr, *cvlamV = nullptr, *cvdelV = nullptr, *cvxs = nullptr;     // Nc (cvxs: Nc x d)
+    double* cvm = nullptr;                            // 8 x Mpad: K_uf alpha, G' alpha, K_uf L^-1 Delta alpha, beta, R beta, w, tmp
+    double* cvout = nullptr; int64_t cvout_rows = 0;  // fold block (padded nV x padded nV)
+    long long* cvidx = nullptr;
+    CUtensorMap mapCvG{}, mapCvGt{}, mapCvCh{}, mapCvP{}, mapCvDuu{}, mapCvDp{}, mapCvQ{};
+    bool cv_ws = false;
+    bool cv_m_ok = false;                             // cvDp / cvQ / cvdel hold the state of the last cv_param since factorize
+    int cv_param = 0;
     // multi-GPU (gpb200_fitc_comm_init): the N observations are sharded over the ranks, every M x M object is replicated;
     // exchanged: one all-reduce of the M x M accumulator Sigma_QR (and of H for the kernel gradient), M-vectors, scalars
     ncclComm_t comm = nullptr;
@@ -2331,6 +2348,17 @@ static int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, do
 static int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise);
 static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel);
 
+// cross-validation workspace (gpb200_fitc_cv_*): it depends on N, Nc and Mpad only
+static void fitc_cv_free(gpb200_fitc* f) {
+    double** ptrs[] = {&f->cvG, &f->cvGt, &f->cvCh, &f->cvP, &f->cvDuu, &f->cvDp, &f->cvR, &f->cvH, &f->cvQ, &f->cvalpha,
+                       &f->cvdel, &f->cvilam, &f->cvza, &f->cvdg, &f->cvda, &f->cvq, &f->cvlamV, &f->cvdelV, &f->cvxs,
+                       &f->cvm, &f->cvout};
+    for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
+    if (f->cvidx) cudaFree(f->cvidx);
+    f->cvidx = nullptr; f->cvout_rows = 0;
+    f->cv_ws = f->cv_m_ok = false;
+}
+
 int gpb200_fitc_comm_init(gpb200_fitc* f, int nranks, int rank, const char* id128) {
     if (!f || !id128 || nranks < 1 || rank < 0 || rank >= nranks) return GPB200_EINVAL;
     if (!nccl_load()) { f->err = "libnccl.so.2 could not be loaded"; return GPB200_ENCCL; }
@@ -2354,6 +2382,7 @@ void gpb200_fitc_destroy(gpb200_fitc* f) {
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     if (f->Kss) cudaFree(f->Kss);
     fsa_free(f);
+    fitc_cv_free(f);
     if (f->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(f->comm);
     if (f->es) { f->es->st = nullptr; f->es->own_stream = false; gpb200_destroy(f->es); }
     if (f->eu) gpb200_destroy(f->eu);
@@ -2391,6 +2420,7 @@ int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, 
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     f->grad_ws = false;
     fsa_free(f);                                      // the FSA blocks refer to the old observations
+    fitc_cv_free(f);
     f->N = N; f->M = M; f->d = d; f->Mpad = f->eu->Npad;
     // chunk of data rows: two staging buffers of ~2 GB each at most
     int64_t nc = (int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE;
@@ -2444,7 +2474,7 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
     if (!isfinite(log_noise)) { f->err = "fitc_factorize: non-finite logNoise"; return GPB200_EINVAL; }
     if (f->mode == 3) { int rc3 = fsa_check(f, "fitc_factorize"); if (rc3) return rc3; }
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = false;
+    f->factored = f->alpha_ready = f->cv_m_ok = false;
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     // K_uu + 1e-10 I and its factor (fitc.jl:139-141)
@@ -2789,6 +2819,237 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
+    return GPB200_OK;
+}
+
+// ================================================================================================
+// Cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance), one GPU.
+// Sigma = Lambda + K_fu K_uu^-1 K_uf is the matrix gpb200_fitc_mll inverts; nothing N x N is formed.  With S = Sigma_QR,
+// L = Lambda and the explicit K_uu^-1, S^-1 of the sub-engines (grad_prepare, as gpb200_fitc_grad_kernel):
+//   Sigma^-1 = L^-1 - Ch K_uf L^-1,   Ch = L^-1 K_fu S^-1 = Sigma^-1 K_fu K_uu^-1   (row-local)
+//   [Sigma^-1]_ii = 1/L_i - k_i S^-1 k_i' / L_i^2
+// Per hyper-parameter j: dSigma_j = Delta + G C' + C G',  C = K_fu K_uu^-1,  G = dK_fu - 1/2 K_fu Dp,  Dp = dK_uu K_uu^-1,
+// Delta = diag(dk_ii - 2 G_i.C_i) (FITC), 0 (SoR / DTC kernel parameters), I (noise variance; G = 0).  Then
+//   Sigma^-1 dSigma_j Sigma^-1 = diag(Delta / L^2) + E Ch' + Ch E',   E = L^-1 G - L^-2 Delta K_fu + 1/2 Ch Q,
+//   Q = H - R - R',  R = K_uf L^-1 G,  H = K_uf L^-1 Delta L^-1 K_fu      (both M x M)
+//   Z_j alpha = Delta alpha / L + L^-1 G beta + Ch w,   beta = K_uu^-1 K_uf alpha,  w = G'alpha - K_uf L^-1 Delta alpha - R beta
+// Pass 1 streams the chunks once to accumulate R, H and the M-vectors, pass 2 streams them again for the two N-vectors; a
+// fold block reads the same quantities on the gathered rows V only.
+// ================================================================================================
+static int fitc_cv_check(gpb200_fitc* f, const char* who) {
+    if (f->mode == 3) { f->err = std::string(who) + ": cross-validation is not available for FSA (mode 3)"; return GPB200_EINVAL; }
+    if (f->nranks > 1) {
+        f->err = std::string(who) + ": cross-validation runs on one GPU; this handle has " + std::to_string(f->nranks) + " ranks";
+        return GPB200_EINVAL;
+    }
+    if (!f->factored || !f->alpha_ready) { f->err = std::string(who) + ": factorize and mll first"; return GPB200_ESTATE; }
+    return GPB200_OK;
+}
+
+// workspace on first use; K_uu^-1 and S^-1 as full symmetric matrices in the sub-engines' G (the state grad_kernel builds)
+static int fitc_cv_prepare(gpb200_fitc* f) {
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N;
+    if (!f->cv_ws) {
+        for (double** p : {&f->cvG, &f->cvGt, &f->cvCh, &f->cvP}) FCK(cudaMalloc(p, sizeof(double) * Nc * Mp));
+        for (double** p : {&f->cvDuu, &f->cvDp, &f->cvR, &f->cvH, &f->cvQ}) FCK(cudaMalloc(p, sizeof(double) * Mp * Mp));
+        for (double** p : {&f->cvalpha, &f->cvdel, &f->cvilam, &f->cvza, &f->cvdg}) FCK(cudaMalloc(p, sizeof(double) * (N + Nc)));
+        for (double** p : {&f->cvda, &f->cvq, &f->cvlamV, &f->cvdelV}) FCK(cudaMalloc(p, sizeof(double) * Nc));
+        FCK(cudaMalloc(&f->cvxs, sizeof(double) * Nc * f->d));
+        FCK(cudaMalloc(&f->cvm, sizeof(double) * 8 * Mp));
+        FCK(cudaMalloc(&f->cvidx, sizeof(long long) * Nc));
+        FCK(cudaMemsetAsync(f->cvalpha, 0, sizeof(double) * (N + Nc), st));      // zero tail: chunk vectors are read Nc wide
+        if (eu->tma_ok) {
+            const bool ok = gemm_make_tensor_map(&f->mapCvGt, f->cvGt, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapCvCh, f->cvCh, Nc, Mp, Mp) &&
+                            gemm_make_tensor_map(&f->mapCvP, f->cvP, Nc, Mp, Mp) && gemm_make_tensor_map(&f->mapCvDuu, f->cvDuu, Mp, Mp, Mp) &&
+                            gemm_make_tensor_map(&f->mapCvDp, f->cvDp, Mp, Mp, Mp) && gemm_make_tensor_map(&f->mapCvQ, f->cvQ, Mp, Mp, Mp);
+            if (!ok) { f->err = "fitc_cv: cuTensorMapEncodeTiled failed"; return GPB200_ECUDA; }
+        }
+        f->cv_ws = true;
+    }
+    FSUB(gpb200_grad_prepare(eu), eu);
+    FSUB(gpb200_grad_prepare(es), es);
+    FCK(symmetrize_launch(eu->G, eu->ld, Mp, st, &eu->launches));
+    FCK(symmetrize_launch(es->G, es->ld, Mp, st, &eu->launches));
+    return GPB200_OK;
+}
+
+// C[M x N] (+)= alpha A B' on the engine's DMMA GEMM
+static cudaError_t fitc_gemm(gpb200_fitc* f, GemmBuf a, GemmBuf b, double* c, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                             double alpha, double beta, double* ct = nullptr, int64_t ldct = 0) {
+    GemmDesc g = gemm_desc_default();
+    g.A = GemmOperand{a, bufNone(), 0, 0};
+    g.B = GemmOperand{b, bufNone(), 0, 0};
+    g.C = c; g.ldc = ldc; g.M = (int)M; g.N = (int)N; g.K = (int)K;
+    g.alpha = alpha; g.beta = beta;
+    g.Ct = ct; g.ldct = ldct;
+    return launch_gemm(f->eu, g);
+}
+
+int gpb200_fitc_get_inverse_diag(gpb200_fitc* f, double* diag) {
+    if (!f || !diag) return GPB200_EINVAL;
+    TRY(fitc_cv_check(f, "fitc_get_inverse_diag"));
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cv_prepare(f));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc;
+    const bool tma = eu->tma_ok;
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp};
+    for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, f->N - r0);
+        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));                                                   // bufA = K_fu
+        FCK(fitc_gemm(f, bA, bufG(es), f->cvCh, Mp, Nc, Mp, Mp, 1.0, 0.0));                      // K_fu S^-1
+        FCK(rowdot2_launch(f->bufA, f->cvCh, Mp, nc, Mp, f->cvq, st, &eu->launches));
+        FCK(fitc_cv_invdiag_launch(nc, f->lam + r0, f->cvq, f->cvdg + r0, st, &eu->launches));
+    }
+    FCK(cudaMemcpyAsync(diag, f->cvdg, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_cv_param(gpb200_fitc* f, int32_t param, const double* alpha, double* Zj_alpha, double* diag_ZjSinv) {
+    if (!f || !Zj_alpha || !diag_ZjSinv) return GPB200_EINVAL;
+    TRY(fitc_cv_check(f, "fitc_cv_param"));
+    const int np = f->eu->prog.n_theta;
+    if (param < -1 || param >= np) {
+        f->err = "fitc_cv_param: param must be -1 (noise variance) or a kernel parameter index below " + std::to_string(np);
+        return GPB200_EINVAL;
+    }
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cv_prepare(f));
+    f->cv_m_ok = false;
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N, M = f->M;
+    const int d = f->d;
+    const bool tma = eu->tma_ok, noise = param < 0;
+    const int kind = noise ? 2 : (f->mode == 0 ? 0 : 1);
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bB{tma ? &f->mapB : nullptr, f->bufB, Nc};
+    GemmBuf bGt{tma ? &f->mapCvGt : nullptr, f->cvGt, Nc}, bCh{tma ? &f->mapCvCh : nullptr, f->cvCh, Mp};
+    GemmBuf bDuu{tma ? &f->mapCvDuu : nullptr, f->cvDuu, Mp}, bDp{tma ? &f->mapCvDp : nullptr, f->cvDp, Mp};
+    GemmBuf bQ{tma ? &f->mapCvQ : nullptr, f->cvQ, Mp};
+    double *kta = f->cvm, *gta = f->cvm + Mp, *uD = f->cvm + 2 * Mp, *beta = f->cvm + 3 * Mp;
+    double *rb = f->cvm + 4 * Mp, *w = f->cvm + 5 * Mp, *tmp = f->cvm + 6 * Mp;
+    if (alpha) FCK(cudaMemcpyAsync(f->cvalpha, alpha, sizeof(double) * N, cudaMemcpyHostToDevice, st));
+    else FCK(cudaMemcpyAsync(f->cvalpha, f->alpha, sizeof(double) * N, cudaMemcpyDeviceToDevice, st));
+    FCK(ew_launch(5, N, f->cvilam, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));              // 1 / Lambda
+    FCK(cudaMemsetAsync(f->cvm, 0, sizeof(double) * 8 * Mp, st));
+    FCK(cudaMemsetAsync(f->cvR, 0, sizeof(double) * Mp * Mp, st));
+    FCK(cudaMemsetAsync(f->cvH, 0, sizeof(double) * Mp * Mp, st));
+    if (!noise) {   // Dp = dK_uu K_uu^-1
+        FCK(gram_grad_full_launch(eu->prog, eu->x, d, d, M, Mp, param, f->cvDuu, Mp, st, &eu->launches));
+        FCK(fitc_gemm(f, bDuu, bufG(eu), f->cvDp, Mp, Mp, Mp, Mp, 1.0, 0.0));
+    }
+    // pass 1: Delta, R, H, K_uf alpha, G'alpha, K_uf L^-1 Delta alpha
+    for (int64_t r0 = 0; r0 < N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, N - r0);
+        const double* xr = f->x + r0 * d;
+        FCK(fitc_kfu(f, xr, nc));                                                                     // bufA = K_fu
+        if (!noise) {
+            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cvG, Mp, st, &eu->launches));
+            if (kind == 0) FCK(fitc_gemm(f, bA, bufG(eu), f->bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));     // bufB = C (Nc x Mpad)
+            FCK(fitc_gemm(f, bA, bDp, f->cvG, Mp, Nc, Mp, Mp, -0.5, 1.0, f->cvGt, Nc));              // G and G'
+        }
+        FCK(fitc_cv_delta_launch(kind, eu->prog, xr, d, param, f->cvG, f->bufB, Mp, Mp, nc, Nc, f->cvalpha + r0, f->cvdel + r0,
+                                 f->cvda, st, &eu->launches));
+        FCK(fitc_kuf(f, xr, nc));                                                                     // bufB = K_uf
+        FCK(rowdot_launch(f->bufB, Nc, f->cvalpha + r0, M, Nc, tmp, st, &eu->launches));
+        FCK(ew_launch(2, M, kta, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(colscale_launch(f->bufB, Nc, Mp, nc, f->cvilam + r0, st, &eu->launches));                // K_uf L^-1
+        FCK(rowdot_launch(f->bufB, Nc, f->cvda, M, Nc, tmp, st, &eu->launches));
+        FCK(ew_launch(2, M, uD, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        if (!noise) {
+            FCK(rowdot_launch(f->cvGt, Nc, f->cvalpha + r0, M, Nc, tmp, st, &eu->launches));
+            FCK(ew_launch(2, M, gta, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
+            FCK(fitc_gemm(f, bB, bGt, f->cvR, Mp, Mp, Mp, Nc, 1.0, 1.0));                           // R += K_uf L^-1 G
+        }
+        if (kind != 1) {                                                                              // H += K_uf L^-1 Delta L^-1 K_fu
+            FCK(cudaMemcpyAsync(f->cvGt, f->bufB, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
+            FCK(colscale_launch(f->cvGt, Nc, Mp, nc, f->cvdel + r0, st, &eu->launches));
+            FCK(fitc_gemm(f, bB, bGt, f->cvH, Mp, Mp, Mp, Nc, 1.0, 1.0));
+        }
+    }
+    FCK(rowdot_launch(eu->G, eu->ld, kta, M, Mp, beta, st, &eu->launches));                         // beta = K_uu^-1 K_uf alpha
+    FCK(rowdot_launch(f->cvR, Mp, beta, M, Mp, rb, st, &eu->launches));
+    FCK(fitc_cv_wvec_launch(M, w, gta, uD, rb, st, &eu->launches));
+    FCK(fitc_cv_qs_launch(f->cvQ, f->cvH, f->cvR, Mp, Mp, st, &eu->launches));
+    // pass 2: the two N-vectors
+    for (int64_t r0 = 0; r0 < N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, N - r0);
+        const double* xr = f->x + r0 * d;
+        FCK(fitc_kfu(f, xr, nc));
+        if (!noise) {
+            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cvG, Mp, st, &eu->launches));
+            FCK(fitc_gemm(f, bA, bDp, f->cvG, Mp, Nc, Mp, Mp, -0.5, 1.0));
+        }
+        FCK(fitc_gemm(f, bA, bufG(es), f->cvCh, Mp, Nc, Mp, Mp, 1.0, 0.0));
+        FCK(scale_launch(1, f->cvCh, Mp, nc, Mp, f->lam + r0, st, &eu->launches));                  // Ch = L^-1 K_fu S^-1
+        FCK(fitc_gemm(f, bCh, bQ, f->cvP, Mp, Nc, Mp, Mp, 1.0, 0.0));                                // Ch Q
+        FCK(fitc_cv_rows_launch(noise ? nullptr : f->cvG, f->cvCh, f->bufA, f->cvP, Mp, nc, Mp, f->lam + r0, f->cvdel + r0,
+                                f->cvalpha + r0, beta, w, f->cvza + r0, f->cvdg + r0, st, &eu->launches));
+    }
+    FCK(cudaMemcpyAsync(Zj_alpha, f->cvza, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(diag_ZjSinv, f->cvdg, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    f->cv_param = param;
+    f->cv_m_ok = true;
+    return GPB200_OK;
+}
+
+int gpb200_fitc_cv_block(gpb200_fitc* f, int32_t which, int64_t nV, const int64_t* idx, double* out) {
+    if (!f || !idx || !out) return GPB200_EINVAL;
+    TRY(fitc_cv_check(f, "fitc_cv_block"));
+    if (which != 0 && which != 1) { f->err = "fitc_cv_block: which must be 0 (Sigma^-1) or 1 (the last cv_param's M_j)"; return GPB200_EINVAL; }
+    if (nV < 1 || nV > f->Nc) {
+        f->err = "fitc_cv_block: nV must lie in 1.." + std::to_string(f->Nc) + " (one staging chunk)";
+        return GPB200_EINVAL;
+    }
+    for (int64_t r = 0; r < nV; ++r)
+        if (idx[r] < 0 || idx[r] >= f->N) { f->err = "fitc_cv_block: index out of range"; return GPB200_EINVAL; }
+    if (which == 1 && !f->cv_m_ok) { f->err = "fitc_cv_block: which = 1 needs a fitc_cv_param since the last factorize"; return GPB200_ESTATE; }
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cv_prepare(f));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, M = f->M;
+    const int d = f->d;
+    const int64_t nVp = (nV + TILE - 1) / TILE * TILE;
+    const bool tma = eu->tma_ok;
+    if (nVp > f->cvout_rows) {
+        if (f->cvout) cudaFree(f->cvout);
+        f->cvout = nullptr; f->cvout_rows = 0;
+        FCK(cudaMalloc(&f->cvout, sizeof(double) * nVp * nVp));
+        f->cvout_rows = nVp;
+    }
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bB2{tma ? &f->mapB2 : nullptr, f->bufB, Mp};
+    GemmBuf bCh{tma ? &f->mapCvCh : nullptr, f->cvCh, Mp}, bP{tma ? &f->mapCvP : nullptr, f->cvP, Mp};
+    GemmBuf bDp{tma ? &f->mapCvDp : nullptr, f->cvDp, Mp}, bQ{tma ? &f->mapCvQ : nullptr, f->cvQ, Mp};
+    FCK(cudaMemcpyAsync(f->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, st));
+    FCK(fitc_cv_gather_launch(nV, f->cvidx, f->x, d, d, f->cvxs, f->lam, f->cvlamV, which == 1 ? f->cvdel : nullptr, f->cvdelV,
+                              st, &eu->launches));
+    FCK(crossgram_launch(eu->prog, f->cvxs, d, nV, nVp, eu->x, d, M, Mp, d, f->bufA, Mp, st, &eu->launches));   // K_V
+    FCK(fitc_gemm(f, bA, bufG(es), f->cvCh, Mp, nVp, Mp, Mp, 1.0, 0.0));
+    FCK(scale_launch(1, f->cvCh, Mp, nV, Mp, f->cvlamV, st, &eu->launches));                       // Ch_V
+    if (which == 0) {   // Sigma^-1[V,V] = diag(1/L_V) - Ch_V (L_V^-1 K_V)'
+        FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * nVp * Mp, cudaMemcpyDeviceToDevice, st));
+        FCK(scale_launch(1, f->bufB, Mp, nV, Mp, f->cvlamV, st, &eu->launches));
+        FCK(fitc_gemm(f, bCh, bB2, f->cvout, nVp, nVp, nVp, Mp, -1.0, 0.0));
+    } else {            // (Sigma^-1 dSigma_j Sigma^-1)[V,V] = diag(Delta_V / L_V^2) + E_V Ch_V' + Ch_V E_V'
+        const bool noise = f->cv_param < 0;
+        if (!noise) {
+            FCK(crossgram_grad_launch(eu->prog, f->cvxs, d, nV, nVp, eu->x, d, M, Mp, d, f->cv_param, f->cvG, Mp, st, &eu->launches));
+            FCK(fitc_gemm(f, bA, bDp, f->cvG, Mp, nVp, Mp, Mp, -0.5, 1.0));
+        }
+        FCK(fitc_gemm(f, bCh, bQ, f->cvP, Mp, nVp, Mp, Mp, 0.5, 0.0));
+        FCK(fitc_cv_eblock_launch(f->cvP, noise ? nullptr : f->cvG, f->bufA, Mp, nV, Mp, f->cvlamV, f->cvdelV, st, &eu->launches));
+        FCK(fitc_gemm(f, bP, bCh, f->cvout, nVp, nVp, nVp, Mp, 1.0, 0.0));
+        FCK(fitc_gemm(f, bCh, bP, f->cvout, nVp, nVp, nVp, Mp, 1.0, 1.0));
+    }
+    FCK(fitc_cv_diag_launch(f->cvout, nVp, nV, which, f->cvlamV, f->cvdelV, st, &eu->launches));
+    FCK(cudaMemcpy2DAsync(out, sizeof(double) * nV, f->cvout, sizeof(double) * nVp, sizeof(double) * nV, nV, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
 

@@ -256,6 +256,38 @@ __global__ void __launch_bounds__(NT) gram_grad_full_kernel(const __grid_constan
     }
 }
 
+// dK(x1, x2)/dtheta_j as a rectangular matrix (N1_pad x N2_pad, zero padding): the cross-validation schedule of the sparse
+// engine regenerates dK_fu / dK_Vu per chunk from it (gpb200_fitc_cv_param, gpb200_fitc_cv_block).
+__global__ void __launch_bounds__(NT) crossgram_grad_kernel(const __grid_constant__ KProg P, const double* __restrict__ x1,
+                                                            long long ldx1, long long N1, const double* __restrict__ x2,
+                                                            long long ldx2, long long N2, int d, int j, double* __restrict__ D,
+                                                            long long ldd) {
+    const int bm = blockIdx.y, bn = blockIdx.x;
+    extern __shared__ double sm[];
+    const int ds = d | 1;
+    double* sXi = sm;
+    double* sXj = sm + TB * ds;
+    load_xtile(sXi, x1, ldx1, d, ds, (long long)bm * TB, N1);
+    load_xtile(sXj, x2, ldx2, d, ds, (long long)bn * TB, N2);
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double gbuf[GPB200_MAX_THETA];
+#pragma unroll 1
+    for (int rr = 0; rr < 16; ++rr) {
+        const int r = warp * 16 + rr;
+        const long long gi = (long long)bm * TB + r;
+        const double* xi = sXi + r * ds;
+#pragma unroll 1
+        for (int b = 0; b < 4; ++b) {
+            const int c = (b >> 1) * 64 + lane * 2 + (b & 1);
+            const long long gj = (long long)bn * TB + c;
+            double v = 0.0;
+            if (gi < N1 && gj < N2) { kprog_eval<true>(P, xi, sXj + c * ds, gbuf); v = gbuf[j]; }
+            D[gi * ldd + gj] = v;
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // fused gradient trace over the lower triangle of Kinv (tile-per-CTA):
 //   part[tile][p]        = sum_{i>j in tile} A_ij dK_ij/dθ_p + 1/2 sum_{i==j} A_ii dK_ii/dθ_p
@@ -587,6 +619,19 @@ cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, 
     cudaError_t e;
     if ((e = ensure_smem(gram_grad_full_kernel, sm)) != cudaSuccess) return e;
     gram_grad_full_kernel<<<grid, NT, sm, st>>>(P, x, ldx, N, d, j, D, ldd, (int)(row0 / TB));
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t crossgram_grad_launch(const KProg& P, const double* x1, int64_t ldx1, int64_t N1, int64_t N1pad, const double* x2,
+                                  int64_t ldx2, int64_t N2, int64_t N2pad, int d, int j, double* D, int64_t ldd, cudaStream_t st,
+                                  int64_t* launches) {
+    if (j < 0 || j >= P.n_theta || N1pad % TB || N2pad % TB) return cudaErrorInvalidValue;
+    dim3 grid((unsigned)(N2pad / TB), (unsigned)(N1pad / TB));
+    const size_t sm = xtile_smem(d);
+    cudaError_t e;
+    if ((e = ensure_smem(crossgram_grad_kernel, sm)) != cudaSuccess) return e;
+    crossgram_grad_kernel<<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, j, D, ldd);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

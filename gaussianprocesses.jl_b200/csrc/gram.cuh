@@ -32,3 +32,8 @@ cudaError_t kdiag_grad_launch(const KProg& P, const double* x, int64_t ldx, int6
 // Rows row0 .. row0 + rows only (multiples of 128; rows < 0: to Npad), row row0 + r stored at D[r * ldd].
 cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad, int j,
                                   double* D, int64_t ldd, cudaStream_t st, int64_t* launches, int64_t row0 = 0, int64_t rows = -1);
+// D[m, n] = dk(x1_m, x2_n)/dtheta_j, N1_pad x N2_pad (multiples of 128), zero padding: the rectangular form for the sparse
+// engine's cross-validation (dK_fu of a chunk of training rows against the inducing points)
+cudaError_t crossgram_grad_launch(const KProg& P, const double* x1, int64_t ldx1, int64_t N1, int64_t N1pad, const double* x2,
+                                  int64_t ldx2, int64_t N2, int64_t N2pad, int d, int j, double* D, int64_t ldd, cudaStream_t st,
+                                  int64_t* launches);

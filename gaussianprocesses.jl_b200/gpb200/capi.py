@@ -77,6 +77,9 @@ _SIGNATURES = {
     "gpb200_fitc_set_mode": (C.c_int, [_H, C.c_int]),
     "gpb200_fitc_set_blocks": (C.c_int, [_H, C.c_int64, _lp, _lp]),
     "gpb200_fitc_predict_fsa": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _lp, _dp, _dp, _dp]),
+    "gpb200_fitc_get_inverse_diag": (C.c_int, [_H, _dp]),
+    "gpb200_fitc_cv_param": (C.c_int, [_H, C.c_int32, _dp, _dp, _dp]),
+    "gpb200_fitc_cv_block": (C.c_int, [_H, C.c_int32, C.c_int64, C.POINTER(C.c_int64), _dp]),
     "gpb200_fitc_launch_count": (C.c_int64, [_H]),
     "gpb200_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
     "gpb200_group_create": (C.c_int, [C.POINTER(_H), C.c_int]),
@@ -528,6 +531,28 @@ class FitcEngine:
                                                       _as_dp(var) if var is not None else None,
                                                       _as_dp(cov) if cov is not None else None), "fitc_predict_fsa")
         return mu, (cov if full_cov else var)
+
+    # -- cross-validation (modes 0-2, one GPU; after factorize + mll) ---------------------------------------------------
+    def inverse_diag(self):
+        """diag(Sigma^-1)[N]."""
+        d = np.empty(self.N)
+        self._check(self._lib.gpb200_fitc_get_inverse_diag(self._h, _as_dp(d)), "fitc_get_inverse_diag")
+        return d
+
+    def cv_param(self, param, alpha=None):
+        """(Z_j alpha, diag(Z_j Sigma^-1)) for kernel parameter `param` (index into the full parameter vector) or -1 = noise."""
+        za, dg = np.empty(self.N), np.empty(self.N)
+        ap = _as_dp(np.ascontiguousarray(alpha, dtype=np.float64)) if alpha is not None else None
+        self._check(self._lib.gpb200_fitc_cv_param(self._h, int(param), ap, _as_dp(za), _as_dp(dg)), "fitc_cv_param")
+        return za, dg
+
+    def cv_block(self, which, idx):
+        """Sigma^-1[V,V] (which 0) or (Z_j Sigma^-1)[V,V] of the last cv_param (which 1)."""
+        idx = np.ascontiguousarray(idx, dtype=np.int64)
+        out = np.empty((idx.size, idx.size))
+        self._check(self._lib.gpb200_fitc_cv_block(self._h, int(which), idx.size, idx.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                   _as_dp(out)), "fitc_cv_block")
+        return out
 
     def launch_count(self):
         return int(self._lib.gpb200_fitc_launch_count(self._h))

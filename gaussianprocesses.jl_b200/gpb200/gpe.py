@@ -236,9 +236,13 @@ class GPE:
             return mu, s2 + nv * np.eye(s2.shape[0])
         return mu, s2 + nv
 
+    def _cv_prepare(self):
+        """the engine state the cross-validation calls read: K_y^-1 (the sparse strategies prepare their own M x M inverses)"""
+        self._eng.grad_prepare()
+
     def predict_LOO(self):
         """predict_LOO(gp) (src/crossvalidation.jl:8-36): leave-one-out means / variances from diag(K_y^-1) and alpha."""
-        self._eng.grad_prepare()
+        self._cv_prepare()
         s2 = 1.0 / self._eng.inverse_diag()
         return -self.alpha * s2 + self.y, s2
 
@@ -275,7 +279,7 @@ class GPE:
     def predict_CVfold(self, folds):
         """predict_CVfold(gp, folds) (src/crossvalidation.jl:180-218): per fold V the predictive mean / covariance of y_V given
         the other observations, from the principal sub-block inv(Σ)[V,V] read off the device."""
-        self._eng.grad_prepare()
+        self._cv_prepare()
         mus, Sigs = [], []
         for V in folds:
             V = np.asarray(V, dtype=np.int64)
@@ -308,7 +312,7 @@ class GPE:
         """dlogpdθ_CVfold(gp, folds; noise, domean, kern) (src/crossvalidation.jl:264-341)."""
         if domean and self.mean.num_params() > 0:
             raise NotImplementedError("I don't know how to do means yet")          # crossvalidation.jl:330
-        self._eng.grad_prepare()
+        self._cv_prepare()
         inv_blocks = [self._eng.cv_block(0, np.asarray(V, dtype=np.int64)) for V in folds]
         out = []
         if noise:

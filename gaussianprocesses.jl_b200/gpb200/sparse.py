@@ -7,7 +7,7 @@ import math
 import numpy as np
 
 from . import capi
-from .gpe import _as_dxn
+from .gpe import GPE, _as_dxn
 from .kernels import flatten
 from .means import MeanZero
 
@@ -97,6 +97,21 @@ class FITC:
             return mu, s2 + self.noise_variance() * np.eye(s2.shape[0])       # GPE.jl:412 (ScalMat)
         return mu, s2 + self.noise_variance()
 
+    # ---- cross-validation (src/crossvalidation.jl with cK the sparse covariance) ----------------------------------------
+    # GPE's host assembly, unchanged: the engine's inverse_diag / cv_param / cv_block stream the N rows against the M x M
+    # inverses instead of reading a resident N x N inverse.
+    def _cv_prepare(self):
+        """the sparse engine's CV entry points prepare their own M x M inverses"""
+
+    predict_LOO = GPE.predict_LOO
+    logp_LOO = GPE.logp_LOO
+    _loo_component = GPE._loo_component
+    dlogp_LOO = GPE.dlogp_LOO
+    predict_CVfold = GPE.predict_CVfold
+    logp_CVfold = GPE.logp_CVfold
+    _fold_component = GPE._fold_component
+    dlogp_CVfold = GPE.dlogp_CVfold
+
 
 class DTC(FITC):
     """Deterministic Training Conditional (src/sparse/determ_train_conditional.jl): SoR likelihood, FITC-style
@@ -151,6 +166,9 @@ class FSA(FITC):
             self._eng.set_blocks(self._block_ptr, self._idx)
             self._pending_blocks = False
         return super().update_mll()
+
+    def _cv_prepare(self):
+        raise ValueError("cross-validation is not available for FSA")
 
     def predict_f(self, x, blockindpred, full_cov=False):
         """predict_f(gp, x, blockindpred; full_cov) (:456-477): test block j (0-based index arrays over the columns of x) is

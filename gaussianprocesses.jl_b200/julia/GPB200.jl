@@ -495,6 +495,83 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::Abs
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
 end
 
+# ---- cross-validation on the sparse covariances (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) -------------
+# The reference starts every function from inv(gp.cK), which its sparse PDMats do not define.  gpb200_fitc_get_inverse_diag /
+# _cv_param / _cv_block return the same vectors and blocks as the dense entry points, streaming the N rows against the two
+# M x M inverses; nothing N x N is formed.  FSA handles return ArgumentError.  The assembly is the dense methods' above.
+function GaussianProcesses.predict_LOO(cK::B200SparsePDMat, alpha::AbstractVector{<:Real}, y::AbstractVector{<:Real})
+    d = Vector{Float64}(undef, cK.n)
+    checks(cK, ccall((:gpb200_fitc_get_inverse_diag, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}), cK.handle, d), "fitc_get_inverse_diag")
+    σi2 = 1 ./ d
+    return -alpha .* σi2 .+ y, σi2
+end
+
+function cv_param(cK::B200SparsePDMat, j::Integer, alpha::AbstractVector)
+    Zjα = Vector{Float64}(undef, cK.n); dg = Vector{Float64}(undef, cK.n)
+    checks(cK, ccall((:gpb200_fitc_cv_param, LIB), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                     cK.handle, j, Vector{Float64}(alpha), Zjα, dg), "fitc_cv_param")
+    return Zjα, dg
+end
+
+function cv_block(cK::B200SparsePDMat, which::Integer, V::AbstractVector{Int})
+    idx = Vector{Int64}(V .- 1); B = Matrix{Float64}(undef, length(V), length(V))
+    checks(cK, ccall((:gpb200_fitc_cv_block, LIB), Cint, (Ptr{Cvoid}, Int32, Int64, Ptr{Int64}, Ptr{Float64}),
+                     cK.handle, which, length(V), idx, B), "fitc_cv_block")
+    return B
+end
+
+function dlogpdθ_LOO(gp::GPE{X,Y,M,K,CS,D,P}; noise::Bool, domean::Bool, kern::Bool) where {X,Y,M,K,CS<:B200Sparse,D,P}
+    cK = gp.cK; y = gp.y; alpha = gp.alpha
+    domean && num_params(gp.mean) > 0 && throw("I don't know how to do means yet")  # crossvalidation.jl:162
+    μi, σi2 = predict_LOO(cK, alpha, y)
+    out = Float64[]
+    if noise
+        Zjα, dg = cv_param(cK, -1, alpha)
+        push!(out, -loo_component(y, alpha, σi2, μi, Zjα, dg) / 2 * 2 * exp(2 * get_value(gp.logNoise)))
+    end
+    if kern
+        for j in cK.exposed
+            Zjα, dg = cv_param(cK, j - 1, alpha)
+            push!(out, -loo_component(y, alpha, σi2, μi, Zjα, dg) / 2)
+        end
+    end
+    return out
+end
+
+function predict_CVfold(cK::B200SparsePDMat, alpha::AbstractVector{<:Real}, y::AbstractVector{<:Real}, folds::Folds)
+    μ = Vector{Float64}[]; Σ = Matrix{Float64}[]
+    for V in folds
+        ΣVT = inv(Symmetric(cv_block(cK, 0, V)))
+        push!(μ, y[V] - ΣVT * alpha[V]); push!(Σ, Matrix(ΣVT))
+    end
+    return μ, Σ
+end
+
+function fold_component(cK::B200SparsePDMat, alpha, Zjα, V, ΣVTinv)
+    ZVV = cv_block(cK, 1, V)
+    C = cholesky(Symmetric(ΣVTinv))
+    ΣVTα = C \ alpha[V]
+    return -2 * dot(ΣVTα, Zjα[V]) + dot(ΣVTα, ZVV * ΣVTα) + tr(C \ ZVV)
+end
+
+function dlogpdθ_CVfold(gp::GPE{X,Y,M,K,CS,D,P}, folds::Folds; noise::Bool, domean::Bool, kern::Bool) where {X,Y,M,K,CS<:B200Sparse,D,P}
+    cK = gp.cK; alpha = gp.alpha
+    domean && num_params(gp.mean) > 0 && throw("I don't know how to do means yet")  # crossvalidation.jl:330
+    blocks = [cv_block(cK, 0, V) for V in folds]
+    out = Float64[]
+    if noise
+        Zjα, _ = cv_param(cK, -1, alpha)
+        push!(out, -sum(fold_component(cK, alpha, Zjα, V, B) for (V, B) in zip(folds, blocks)) / 2 * 2 * exp(2 * get_value(gp.logNoise)))
+    end
+    if kern
+        for j in cK.exposed
+            Zjα, _ = cv_param(cK, j - 1, alpha)
+            push!(out, -sum(fold_component(cK, alpha, Zjα, V, B) for (V, B) in zip(folds, blocks)) / 2)
+        end
+    end
+    return out
+end
+
 # ---- GPA: non-Gaussian likelihoods (src/GPA.jl) ----------------------------------------------------------------------------
 # The reference's GPA types cK as PDMat{Float64,Matrix{Float64}} (GPA.jl:33), so a device factor cannot be slotted into it.
 # B200GPA carries GPA's fields and methods over a B200PDMat; the likelihoods are the reference's own (log_dens,

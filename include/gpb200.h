@@ -331,6 +331,25 @@ int  gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* bloc
  * grouped by block and each group padded to a multiple of 128, to fit one staging chunk (GPB200_EINVAL otherwise).      */
 int  gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
                              double* mu_minus_mean, double* var, double* cov);
+/* ---- cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) ---------------
+ * The dense entry points gpb200_get_inverse_diag / gpb200_cv_param / gpb200_cv_block for modes 0 (FITC), 1 (DTC: SoR's
+ * covariance) and 2 (SoR), after gpb200_fitc_factorize and gpb200_fitc_mll.  Sigma = Lambda + K_fu K_uu^-1 K_uf is the matrix
+ * gpb200_fitc_mll inverts; nothing N x N is formed: every quantity comes from K_uu^-1, Sigma_QR^-1 (M x M) and the rows of
+ * K_fu and dK_fu regenerated chunk by chunk.  gpb200_fitc_cv_param costs two streaming passes over the N rows (~14 N M^2
+ * flop on the DMMA GEMM for a FITC kernel parameter), a fold block O(nV M^2 + nV^2 M).  The likelihood, gradient and
+ * prediction state of the handle is not touched: their results stay bitwise equal.  Repeated calls are bitwise equal.
+ * GPB200_ESTATE before factorize + mll; GPB200_EINVAL for mode 3 (FSA), for a handle with more than one rank
+ * (gpb200_fitc_comm_init), for a bad `param`, `which` or index, and for nV above one staging chunk.                    */
+/* diag(Sigma^-1)[N]: all predict_LOO / logp_LOO need besides alpha (crossvalidation.jl:8-49) */
+int  gpb200_fitc_get_inverse_diag(gpb200_fitc* f, double* diag);
+/* Zj_alpha[N] = Z_j alpha and diag_ZjSinv[N] = diag(Z_j Sigma^-1) with Z_j = Sigma^-1 dSigma/dtheta_j; `param` indexes the
+ * kernel's full parameter vector, -1 is the noise variance (dSigma = I).  alpha[N] may be NULL: the alpha of the last
+ * gpb200_fitc_mll.  The M x M state of this parameter stays resident for gpb200_fitc_cv_block(which = 1).                */
+int  gpb200_fitc_cv_param(gpb200_fitc* f, int32_t param, const double* alpha, double* Zj_alpha, double* diag_ZjSinv);
+/* principal sub-matrix on idx[nV] (0-based), row-major nV x nV, of Sigma^-1 (which = 0) or of Z_j Sigma^-1 for the parameter
+ * of the last gpb200_fitc_cv_param (which = 1; GPB200_ESTATE without one since the last factorize).  nV <= the staging chunk
+ * (32768 rows at most, fewer for large M: 2e9 / (8 Mpad) rounded down to 128).                                            */
+int  gpb200_fitc_cv_block(gpb200_fitc* f, int32_t which, int64_t nV, const int64_t* idx, double* out);
 /* number of kernels enqueued by calls on this handle since creation, on both M x M sub-engines; cudaMemsetAsync and
  * copies are not counted */
 int64_t gpb200_fitc_launch_count(gpb200_fitc* f);
