@@ -50,6 +50,7 @@
 
 namespace {
 constexpr int TILE = 128;
+constexpr int TRSV_FUSED_CTAS_PER_SM = 4;      // single-launch solves run for Npad/128 <= this x SMs (see solve_device)
 constexpr double LOG2PI = 1.8378770664093453;
 std::string g_create_error;
 }  // namespace
@@ -868,7 +869,10 @@ int inverse_dist(gpb200_handle* h) {
 // alpha-type solve on device vectors: out = K_y^-1 rhs ; rhs (Npad, zero padded) is destroyed
 cudaError_t solve_device(gpb200_handle* h, double* rhs, double* tmp, double* out) {
     const int nb = (int)(h->Npad / TILE);
-    // single-launch flag-synchronised solves need all Npad/128 CTAs co-resident (8 CTAs of 256 threads per SM)
+    // single-launch flag-synchronised solves: each CTA stages a 128 KB tile in dynamic shared memory, so one CTA fits per
+    // SM.  Every wait points to a lower blockIdx, so for nb above the SM count correctness rests on in-order CTA dispatch
+    // (a CTA waits only on CTAs dispatched before it, which run or have retired).  max_resident_ctas (TRSV_FUSED_CTAS_PER_SM
+    // per SM) is a chosen limit on nb, not a residency count; above it the per-step schedule runs.
     if (h->trsv_fused && h->flags && nb <= h->max_resident_ctas) {
         cudaError_t e = trsv_lower_fwd_fused(h->F, h->ld, h->Dinv, rhs, tmp, h->Npad, h->flags, h->st, &h->launches);
         if (e != cudaSuccess) return e;
@@ -1229,7 +1233,9 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
         {
             int sms = 0;
             CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-            h->max_resident_ctas = sms * 4;            // conservative: 4 CTAs of 256 threads per SM
+            // a chosen limit on the block count of the single-launch solves, not a residency count: one CTA fits per
+            // SM, and above the SM count the schedule relies on in-order CTA dispatch (see solve_device)
+            h->max_resident_ctas = sms * TRSV_FUSED_CTAS_PER_SM;
         }
         const int64_t T = Npad / TILE;
         CK(cudaMalloc(&h->part, sizeof(double) * (size_t)(T * (T + 1) / 2) * (GPB200_MAX_THETA + 1)));
@@ -2193,6 +2199,94 @@ int gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t 
     return GPB200_OK;
 }
 
+int gpb200_trsv_tiles(gpb200_handle* h, int schedule, int direction, const int64_t* args, int32_t n, int32_t* watchdog) {
+    if (!h || !args || !watchdog || (schedule != 0 && schedule != 1) || (direction != 0 && direction != 1)) return GPB200_EINVAL;
+    if (n != 6) return fail(h, GPB200_EINVAL, "trsv_tiles: 6 arguments (F, ldf, Dinv or DinvT, rhs, out, Npad)");
+    const int64_t ldf = args[1], Npad = args[5];
+    if (!args[0] || !args[2] || !args[3] || !args[4] || ((args[0] | args[2] | args[3] | args[4]) & 15))
+        return fail(h, GPB200_EINVAL, "trsv_tiles: 16-byte aligned device pointers");
+    if (Npad <= 0 || Npad % TILE || ldf <= 0 || ldf % 2)
+        return fail(h, GPB200_EINVAL, "trsv_tiles: Npad a positive multiple of 128, ldf positive and even");
+    const int nb = (int)(Npad / TILE);
+    CK(cudaSetDevice(h->device));
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+    if (schedule == 1 && nb > sms * TRSV_FUSED_CTAS_PER_SM)
+        return fail(h, GPB200_EINVAL, "trsv_tiles: the single-launch schedule runs for Npad/128 <= 4 x SMs only");
+    const double* F = reinterpret_cast<const double*>(args[0]);
+    const double* D = reinterpret_cast<const double*>(args[2]);
+    double* rhs = reinterpret_cast<double*>(args[3]);
+    double* out = reinterpret_cast<double*>(args[4]);
+    *watchdog = 0;
+    if (schedule == 0) {
+        CK(direction == 0 ? trsv_lower_fwd(F, ldf, D, rhs, out, Npad, h->st, &h->launches)
+                          : trsv_lower_bwd(F, ldf, D, rhs, out, Npad, h->st, &h->launches));
+        CK(cudaStreamSynchronize(h->st));
+        return GPB200_OK;
+    }
+    int* flags = nullptr;
+    CK(cudaMalloc(&flags, sizeof(int) * (nb + 1)));
+    cudaError_t e = direction == 0 ? trsv_lower_fwd_fused(F, ldf, D, rhs, out, Npad, flags, h->st, &h->launches)
+                                   : trsv_lower_bwd_fused(F, ldf, D, rhs, out, Npad, flags, h->st, &h->launches);
+    int wd = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&wd, flags + nb, sizeof(int), cudaMemcpyDeviceToHost, h->st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
+    cudaFree(flags);
+    CK(e);
+    *watchdog = wd;
+    return GPB200_OK;
+}
+
+int gpb200_gpa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n) {
+    if (!h || !args || which < 0 || which > 2) return GPB200_EINVAL;
+    const int want = which == 2 ? 8 : 5;
+    if (n != want) return fail(h, GPB200_EINVAL, "gpa_kernels: 5 arguments (trmv, trmv_t) or 8 (scan)");
+    const int64_t ld = args[1], Npad = args[want - 1];
+    if (Npad <= 0 || Npad % TILE || ld < Npad) return fail(h, GPB200_EINVAL, "gpa_kernels: Npad a positive multiple of 128, ld >= Npad");
+    for (int i = 0; i < want - 1; ++i)
+        if (i != 1 && !args[i]) return fail(h, GPB200_EINVAL, "gpa_kernels: null device pointer");
+    CK(cudaSetDevice(h->device));
+    auto cp = [&](int i) { return reinterpret_cast<const double*>(args[i]); };
+    auto mp = [&](int i) { return reinterpret_cast<double*>(args[i]); };
+    cudaError_t e;
+    if (which == 0) e = gpa_trmv_launch(cp(0), ld, cp(2), mp(3), Npad, h->st, &h->launches);
+    else if (which == 1) e = gpa_trmv_t_launch(cp(0), ld, cp(2), mp(3), Npad, h->st, &h->launches);
+    else e = gpa_scan_launch(cp(0), ld, cp(2), cp(3), cp(4), mp(5), mp(6), Npad, h->st, &h->launches);
+    if (e == cudaErrorInvalidValue) { (void)cudaGetLastError(); return fail(h, GPB200_EINVAL, "gpa_kernels: rejected by the launch"); }
+    CK(e);
+    CK(cudaStreamSynchronize(h->st));
+    return GPB200_OK;
+}
+
+int gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int32_t n) {
+    if (!h || !args || which < 0 || which > 4) return GPB200_EINVAL;
+    static const int want[5] = {4, 3, 6, 6, 6};
+    if (n != want[which]) return fail(h, GPB200_EINVAL, "row_reductions: dot 4, sum 3, rowdot / rowvar / rowdot2 6 arguments");
+    auto cp = [&](int i) { return reinterpret_cast<const double*>(args[i]); };
+    auto mp = [&](int i) { return reinterpret_cast<double*>(args[i]); };
+    cudaError_t e;
+    if (which <= 1) {
+        const int64_t len = args[which == 0 ? 2 : 1];
+        const int outi = which == 0 ? 3 : 2;
+        if (len < 0 || !args[0] || !args[outi] || (which == 0 && !args[1]))
+            return fail(h, GPB200_EINVAL, "row_reductions: n >= 0 and non-null pointers");
+        CK(cudaSetDevice(h->device));
+        e = which == 0 ? dot_launch(cp(0), cp(1), len, mp(3), h->st, &h->launches) : sum_launch(cp(0), len, mp(2), h->st, &h->launches);
+    } else {
+        // rowdot (K, ldk, alpha, M, N, mu), rowvar (V, ldk, kdiag, M, N, var), rowdot2 (A, B, ld, M, N, q)
+        const int64_t ld = which == 4 ? args[2] : args[1], M = args[3], N = args[4];
+        if (M < 0 || N < 0 || ld < N || !args[0] || !args[which == 4 ? 1 : 2] || !args[5])
+            return fail(h, GPB200_EINVAL, "row_reductions: M, N >= 0, ld >= N and non-null pointers");
+        CK(cudaSetDevice(h->device));
+        if (which == 2) e = rowdot_launch(cp(0), ld, cp(2), M, N, mp(5), h->st, &h->launches);
+        else if (which == 3) e = rowvar_launch(cp(0), ld, cp(2), M, N, mp(5), h->st, &h->launches);
+        else e = rowdot2_launch(cp(0), cp(1), ld, M, N, mp(5), h->st, &h->launches);
+    }
+    CK(e);
+    CK(cudaStreamSynchronize(h->st));
+    return GPB200_OK;
+}
+
 int gpb200_fp64_peak(gpb200_handle* h, double* tflops_dmma, double* tflops_dfma) {
     if (!h) return GPB200_EINVAL;
     CK(cudaSetDevice(h->device));
@@ -2574,6 +2668,7 @@ int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, d
     FCK(cudaMemcpyAsync(s, f->scal, sizeof(double) * 5, cudaMemcpyDeviceToHost, st));
     if (alpha) FCK(cudaMemcpyAsync(alpha, f->alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(es), es);                                   // the solve for u above
     f->Ntotal = f->nranks > 1 ? s[4] : (double)f->N;
     const double ld = s[1] - s[2] + s[3];
     if (logdet) *logdet = ld;
@@ -2818,6 +2913,7 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta above
     for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
     return GPB200_OK;
 }
@@ -3460,6 +3556,7 @@ static int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, do
     FCK(cudaMemcpyAsync(sc, f->scal, sizeof(double) * 4, cudaMemcpyDeviceToHost, st));
     if (alpha) FCK(cudaMemcpyAsync(alpha, f->alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(es), es);                                   // the solve for u above
     f->Ntotal = (double)f->N;
     const double ld = sc[1] - sc[2] + sc[3];
     if (logdet) *logdet = ld;
@@ -3566,6 +3663,7 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta in gpb200_fitc_grad_kernel
     for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
     return GPB200_OK;
 }

@@ -59,6 +59,9 @@ _SIGNATURES = {
     "gpb200_gemm_nt_desc": (C.c_int, [_H, C.c_int, _lp, C.c_int32, C.c_double, C.c_double]),
     "gpb200_fsa_gemm_items": (C.c_int, [_H, _lp, _dp, C.c_int32]),
     "gpb200_potrf_tiles": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _ip]),
+    "gpb200_trsv_tiles": (C.c_int, [_H, C.c_int, C.c_int, _lp, C.c_int32, _ip]),
+    "gpb200_gpa_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
+    "gpb200_row_reductions": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
     "gpb200_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "gpb200_ipc_export": (C.c_int, [_H, C.c_void_p]),
     "gpb200_ipc_import": (C.c_int, [_H, C.c_int, C.c_void_p]),
@@ -402,6 +405,25 @@ class Engine:
         self._check(self._lib.gpb200_potrf_tiles(self._h, int(mode), a.ctypes.data_as(_lp), a.size, C.byref(info)),
                     "potrf_tiles")
         return int(info.value)
+
+    def trsv_tiles(self, schedule, direction, args):
+        """Blocked triangular solve (schedule 0: per block step, 1: single launch; direction 0: L^-1, 1: L^-T) on
+        (F, ldf, Dinv or DinvT, rhs, out, Npad).  Returns the watchdog word."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        wd = C.c_int32()
+        self._check(self._lib.gpb200_trsv_tiles(self._h, int(schedule), int(direction), a.ctypes.data_as(_lp), a.size,
+                                                C.byref(wd)), "trsv_tiles")
+        return int(wd.value)
+
+    def gpa_kernels(self, which, args):
+        """GPA kernel (0 trmv, 1 trmv_t, 2 scan) on the device buffers of include/gpb200.h."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        self._check(self._lib.gpb200_gpa_kernels(self._h, int(which), a.ctypes.data_as(_lp), a.size), "gpa_kernels")
+
+    def row_reductions(self, which, args):
+        """Fixed-order reduction (0 dot, 1 sum, 2 rowdot, 3 rowvar, 4 rowdot2) on the device buffers of include/gpb200.h."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        self._check(self._lib.gpb200_row_reductions(self._h, int(which), a.ctypes.data_as(_lp), a.size), "row_reductions")
 
 
 class FitcEngine:

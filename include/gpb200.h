@@ -242,6 +242,26 @@ int  gpb200_fsa_gemm_items(gpb200_handle* h, const int64_t* items, const double*
  *          (F, Dinv, DinvT, logd) for each of the 7 peer sets;
  *   mode 1 (potrf128_ptr_launch), n = 6 per tile: G, Dinv, DinvT, logd, ld, info_base.                                */
 int  gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t n, int32_t* info);
+/* The blocked triangular solves (csrc/vec.cuh) on caller buffers, synchronous, launched as the engine launches them.
+ * args (n = 6): F, ldf, Dinv (direction 0: out = L^-1 rhs) or DinvT (direction 1: out = L^-T rhs), rhs, out, Npad.
+ * schedule 0: one launch per 128-block step (rhs is overwritten); schedule 1: the single-launch flag-synchronised kernel
+ * (rhs is only read), Npad/128 <= 4 x SMs.  *watchdog = the watchdog word of the single-launch kernel (a flags buffer
+ * owned by the call; 0 for schedule 0 and for every run in which each ready-flag arrived).
+ * GPB200_EINVAL, nothing launched: bad schedule / direction / n, Npad not a positive multiple of 128, ldf odd or not
+ * positive, a null or not 16-byte aligned pointer, schedule 1 above its block limit.                                  */
+int  gpb200_trsv_tiles(gpb200_handle* h, int schedule, int direction, const int64_t* args, int32_t n, int32_t* watchdog);
+/* The GPA kernels (csrc/gpa.cuh), synchronous, launched as the engine launches them:
+ *   which 0 gpa_trmv_launch   (n = 5): F, ldf, v, f, Npad
+ *   which 1 gpa_trmv_t_launch (n = 5): F, ldf, g, u, Npad
+ *   which 2 gpa_scan_launch   (n = 8): G, ld, DinvT, u, v, F, ZdT, Npad
+ * GPB200_EINVAL, nothing launched: bad which / n, Npad not a positive multiple of 128, ld < Npad, a null pointer.      */
+int  gpb200_gpa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n);
+/* The fixed-order reductions (csrc/vec.cuh), synchronous, launched as the engine launches them:
+ *   which 0 dot (n = 4): a, b, len, out     which 1 sum (n = 3): a, len, out
+ *   which 2 rowdot (n = 6): K, ldk, alpha, M, N, mu     which 3 rowvar (n = 6): V, ldk, kdiag, M, N, var
+ *   which 4 rowdot2 (n = 6): A, B, ld, M, N, q
+ * GPB200_EINVAL, nothing launched: bad which / n, a negative length, ld < N, a null pointer.                           */
+int  gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int32_t n);
 
 /* ---- multi-GPU (one process per GPU; NCCL over NVLink) -------------------------------------- */
 /* rank 0 obtains a 128-byte NCCL unique id, the host side broadcasts it (torch.distributed /
