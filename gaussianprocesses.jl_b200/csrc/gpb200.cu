@@ -197,6 +197,9 @@ struct gpb200_fitc {
     CUtensorMap mapAt{}, mapC{}, mapCt{}, mapH{}, mapT{};
     bool grad_ws = false;
     double* Kss = nullptr; int64_t Kss_rows = 0;      // full predictive covariance (gpb200_fitc_predict_cov)
+    // posterior sampling (gpb200_fitc_rand): the Ms x Ms sub-engine and the staging of the draws are eu's (rand_from_cov)
+    bool cov_keep_device = false;                     // predict_fsa: leave Sigma* in caller order on the device (fsa->Sc)
+    double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
     // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
     // buffer the likelihood, gradient and prediction schedules keep):
     //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
@@ -1057,6 +1060,64 @@ int chol_inplace(gpb200_handle* h) {
     return factor_end(L, "", false);
 }
 
+// make_posdef!(Sigma; nugget), cholesky and unwhiten! of rand(gp, X, n) on h's stream, from Sigma (M x M, leading dimension
+// ldc) and mu (M) on the device.  h owns the M x M sub-engine and the staging of the draws; the sub-engine's kernels are
+// counted on h.  Events on h: ev0 before make_posdef!, ev1 after the Cholesky, ev3 / ev2 around unwhiten! + mu (the upload
+// of z lies between ev1 and ev3).
+int rand_from_cov(gpb200_handle* h, int64_t M, const double* cov, int64_t ldc, const double* mu, int64_t nsamp,
+                  const double* z, double nugget, double* samples) {
+    const int64_t Mpad = (M + TILE - 1) / TILE * TILE, Spad = (nsamp + TILE - 1) / TILE * TILE;
+    int rc;
+    // sub-engine of size M (shares this handle's stream)
+    if (!h->sub) {
+        rc = gpb200_create(&h->sub, h->device);
+        if (rc) return fail(h, rc, "rand: could not create the M x M sub-engine");
+        cudaStreamDestroy(h->sub->st);
+        h->sub->own_stream = false;
+    }
+    gpb200_handle* sb = h->sub;
+    sb->st = h->st;
+    const int64_t sub_launches = sb->launches;
+    if (!sb->has_data || sb->N != M) {
+        std::vector<double> dummy((size_t)M, 0.0);
+        rc = gpb200_set_data(sb, M, 1, dummy.data(), 1);
+        if (rc) { h->err = "rand: " + sb->err; return rc; }
+    }
+    CK(cudaEventRecord(h->ev0, h->st));
+    CK(spd_from_cov_launch(sb->G, sb->ld, cov, ldc, M, Mpad, nugget, h->st, &h->launches));
+    rc = chol_inplace(sb);
+    h->launches += sb->launches - sub_launches;                 // the sub-engine's kernels run for this call
+    if (rc) { h->err = "rand: predictive covariance + nugget is not positive definite: " + sb->err; return rc; }
+    CK(cudaEventRecord(h->ev1, h->st));
+    // draws: Zt (nsamp x M, zero padded) on the device
+    if (Spad > h->rz_rows || Mpad > h->rz_cols) {
+        if (h->rz) cudaFree(h->rz);
+        if (h->rout) cudaFree(h->rout);
+        h->rz = h->rout = nullptr; h->rz_rows = h->rz_cols = 0;
+        CK(cudaMalloc(&h->rz, sizeof(double) * Spad * Mpad));
+        CK(cudaMalloc(&h->rout, sizeof(double) * Spad * Mpad));
+        h->rz_rows = Spad; h->rz_cols = Mpad;
+    }
+    const int64_t ldz = h->rz_cols;
+    if (h->tma_ok && !gemm_make_tensor_map(&h->mapRz, h->rz, h->rz_rows, ldz, ldz)) return fail(h, GPB200_ECUDA, "rand: tensor map");
+    CK(cudaMemsetAsync(h->rz, 0, sizeof(double) * h->rz_rows * ldz, h->st));
+    CK(cudaMemcpy2DAsync(h->rz, sizeof(double) * ldz, z, sizeof(double) * M, sizeof(double) * M, nsamp, cudaMemcpyHostToDevice, h->st));
+    CK(cudaEventRecord(h->ev3, h->st));
+    {   // out[s, m] = sum_{k <= m} Zt[s, k] L[m, k]       (unwhiten!: L Z)
+        GemmDesc g = gemm_desc_default();
+        g.A = GemmOperand{GemmBuf{h->tma_ok ? &h->mapRz : nullptr, h->rz, ldz}, bufNone(), 0, 0};
+        g.B = GemmOperand{bufF(sb), bufNone(), 0, 0};
+        g.C = h->rout; g.ldc = ldz; g.M = (int)Spad; g.N = (int)Mpad; g.K = (int)Mpad;
+        g.flags = GEMM_KHI_N;
+        CK(launch_gemm(h, g));
+    }
+    CK(add_rowvec_launch(h->rout, ldz, mu, nsamp, M, h->st, &h->launches));                              // + mu
+    CK(cudaEventRecord(h->ev2, h->st));
+    CK(cudaMemcpy2DAsync(samples, sizeof(double) * M, h->rout, sizeof(double) * ldz, sizeof(double) * M, nsamp, cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
+    return GPB200_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1690,51 +1751,7 @@ int gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, con
     int rc = gpb200_predict(h, M, xs, ldxs, alpha, mu_minus_mean, nullptr, &cov_flag);
     h->cov_keep_device = false;
     if (rc) return rc;
-    const int64_t Mpad = (M + TILE - 1) / TILE * TILE, Spad = (nsamp + TILE - 1) / TILE * TILE;
-    // sub-engine of size M (shares this handle's stream)
-    if (!h->sub) {
-        rc = gpb200_create(&h->sub, h->device);
-        if (rc) return fail(h, rc, "rand: could not create the M x M sub-engine");
-        cudaStreamDestroy(h->sub->st);
-        h->sub->own_stream = false;
-    }
-    gpb200_handle* sb = h->sub;
-    sb->st = h->st;
-    const int64_t sub_launches = sb->launches;
-    if (!sb->has_data || sb->N != M) {
-        std::vector<double> dummy((size_t)M, 0.0);
-        rc = gpb200_set_data(sb, M, 1, dummy.data(), 1);
-        if (rc) { h->err = "rand: " + sb->err; return rc; }
-    }
-    CK(spd_from_cov_launch(sb->G, sb->ld, h->Kss, Mpad, M, Mpad, nugget, h->st, &h->launches));
-    rc = chol_inplace(sb);
-    h->launches += sb->launches - sub_launches;                 // the sub-engine's kernels run for this call
-    if (rc) { h->err = "rand: predictive covariance + nugget is not positive definite: " + sb->err; return rc; }
-    // draws: Zt (nsamp x M, zero padded) on the device
-    if (Spad > h->rz_rows || Mpad > h->rz_cols) {
-        if (h->rz) cudaFree(h->rz);
-        if (h->rout) cudaFree(h->rout);
-        h->rz = h->rout = nullptr; h->rz_rows = h->rz_cols = 0;
-        CK(cudaMalloc(&h->rz, sizeof(double) * Spad * Mpad));
-        CK(cudaMalloc(&h->rout, sizeof(double) * Spad * Mpad));
-        h->rz_rows = Spad; h->rz_cols = Mpad;
-    }
-    const int64_t ldz = h->rz_cols;
-    if (h->tma_ok && !gemm_make_tensor_map(&h->mapRz, h->rz, h->rz_rows, ldz, ldz)) return fail(h, GPB200_ECUDA, "rand: tensor map");
-    CK(cudaMemsetAsync(h->rz, 0, sizeof(double) * h->rz_rows * ldz, h->st));
-    CK(cudaMemcpy2DAsync(h->rz, sizeof(double) * ldz, z, sizeof(double) * M, sizeof(double) * M, nsamp, cudaMemcpyHostToDevice, h->st));
-    {   // out[s, m] = sum_{k <= m} Zt[s, k] L[m, k]       (unwhiten!: L Z)
-        GemmDesc g = gemm_desc_default();
-        g.A = GemmOperand{GemmBuf{h->tma_ok ? &h->mapRz : nullptr, h->rz, ldz}, bufNone(), 0, 0};
-        g.B = GemmOperand{bufF(sb), bufNone(), 0, 0};
-        g.C = h->rout; g.ldc = ldz; g.M = (int)Spad; g.N = (int)Mpad; g.K = (int)Mpad;
-        g.flags = GEMM_KHI_N;
-        CK(launch_gemm(h, g));
-    }
-    CK(add_rowvec_launch(h->rout, ldz, h->pmu, nsamp, M, h->st, &h->launches));                          // + mu (K*' alpha part)
-    CK(cudaMemcpy2DAsync(samples, sizeof(double) * M, h->rout, sizeof(double) * ldz, sizeof(double) * M, nsamp, cudaMemcpyDeviceToHost, h->st));
-    CK(cudaStreamSynchronize(h->st));
-    return GPB200_OK;
+    return rand_from_cov(h, M, h->Kss, (M + TILE - 1) / TILE * TILE, h->pmu, nsamp, z, nugget, samples);
 }
 
 // ---- ElasticGPE append! (src/GPEelastic.jl:13-22): extend the factor by k new observations -----------------------------
@@ -2745,12 +2762,8 @@ int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ld
 // predictMVN with the FULL predictive covariance (fitc.jl:324-332 -> determ_train_conditional.jl:41-59 ->
 // subsetofregressors.jl:302-321):  Sigma* = K** - K*u K_uu^-1 Ku* + K*u S^-1 Ku*   (FITC, DTC);   K*u S^-1 Ku*   (SoR)
 // = K** - A A' + B B' with A = K*u L_uu^-T, B = K*u L_s^-T: two whitening TRSMs and two NT GEMMs.  Ms <= one staging chunk.
-int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* cov) {
-    if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu || !cov) return GPB200_EINVAL;
-    if (!f->factored || !f->alpha_ready) { f->err = "fitc_predict_cov: factorize and mll first"; return GPB200_ESTATE; }
-    if (f->mode == 3) { f->err = "fitc_predict_cov: FSA predictions need test blocks"; return GPB200_EINVAL; }
-    if (Ms > f->Nc) { f->err = "fitc_predict_cov: too many test points for one staging chunk"; return GPB200_EINVAL; }
-    FCK(cudaSetDevice(f->device));
+// Sigma* into f->Kss (leading dimension Ms rounded up to 128) and mu into f->tmpc and mu[Ms], on eu's stream; Ms <= Nc
+static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
@@ -2788,8 +2801,19 @@ int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
         g.alpha = 1.0; g.beta = 1.0;
         FCK(launch_gemm(es, g));
     }
-    FCK(cudaMemcpy2DAsync(cov, sizeof(double) * Ms, f->Kss, sizeof(double) * Mspad, sizeof(double) * Ms, Ms, cudaMemcpyDeviceToHost, st));
-    FCK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* cov) {
+    if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu || !cov) return GPB200_EINVAL;
+    if (!f->factored || !f->alpha_ready) { f->err = "fitc_predict_cov: factorize and mll first"; return GPB200_ESTATE; }
+    if (f->mode == 3) { f->err = "fitc_predict_cov: FSA predictions need test blocks"; return GPB200_EINVAL; }
+    if (Ms > f->Nc) { f->err = "fitc_predict_cov: too many test points for one staging chunk"; return GPB200_EINVAL; }
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cov_build(f, Ms, xs, ldxs, mu));
+    const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
+    FCK(cudaMemcpy2DAsync(cov, sizeof(double) * Ms, f->Kss, sizeof(double) * Mspad, sizeof(double) * Ms, Ms, cudaMemcpyDeviceToHost, f->eu->st));
+    FCK(cudaStreamSynchronize(f->eu->st));
     return GPB200_OK;
 }
 
@@ -3199,6 +3223,9 @@ struct Fsa {
     CUtensorMap mapVs{};
     FsaGemmItem* pg = nullptr; FsaGramItem* px = nullptr; FsaRowItem* pr = nullptr;
     size_t pg_cap = 0, px_cap = 0, pr_cap = 0;
+    // gpb200_fitc_rand: Sigma* gathered into the caller's order (Ms x Ms, dense) through the test-point permutation pp
+    double* Sc = nullptr; long long* pp = nullptr;
+    size_t Sc_cap = 0, pp_cap = 0;
 };
 
 static void fsa_free(gpb200_fitc* f) {
@@ -3206,7 +3233,7 @@ static void fsa_free(gpb200_fitc* f) {
     Fsa* s = f->fsa;
     void* ptrs[] = {s->xb, s->mask, s->X, s->LT, s->logd, s->r, s->a, s->t1, s->t2, s->pos, s->bstart, s->boff,
                     s->rblk, s->bsize, s->info, s->gitems, s->litems, s->gramitems, s->Gpk, s->gpart, s->ones,
-                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr};
+                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr, s->Sc, s->pp};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete s;
     f->fsa = nullptr;
@@ -3844,7 +3871,8 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
     GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, Mp};
     GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, Mp};
     GemmBuf bVs{eu->tma_ok ? &s->mapVs : nullptr, s->Vs, Mp};
-    std::vector<double> mu_p((size_t)Msp), var_p(var ? (size_t)Msp : 0), cov_p(cov ? (size_t)Msp * Msp : 0);
+    const bool cov_host = cov && !f->cov_keep_device;
+    std::vector<double> mu_p((size_t)Msp), var_p(var ? (size_t)Msp : 0), cov_p(cov_host ? (size_t)Msp * Msp : 0);
     for (const Sub& sb : subs) {
         const int64_t row0 = sb.t0 * TILE, mq = (sb.t1 - sb.t0) * TILE;
         FCK(cudaMemcpyAsync(f->xs, xsp.data() + row0 * d, sizeof(double) * mq * d, cudaMemcpyHostToDevice, st));
@@ -3891,17 +3919,76 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
             g.alpha = 1.0;
             FCK(launch_gemm(es, g));                                                                      // + R R'
             FCK(fsa_gemm_launch(s->pg + sb.ggt.off, sb.ggt.n, st, &eu->launches));  // - G G'
-            FCK(cudaMemcpyAsync(cov_p.data(), f->Kss, sizeof(double) * mq * mq, cudaMemcpyDeviceToHost, st));
+            if (cov_host) FCK(cudaMemcpyAsync(cov_p.data(), f->Kss, sizeof(double) * mq * mq, cudaMemcpyDeviceToHost, st));
         }
         FCK(cudaStreamSynchronize(st));
+    }
+    if (cov && !cov_host) {
+        // Sigma* (one sub-chunk: leading dimension Msp) and mu in the caller's order on the device, as the host loop below
+        // reorders them
+        if ((size_t)(Ms * Ms) > s->Sc_cap) {
+            if (s->Sc) cudaFree(s->Sc);
+            s->Sc = nullptr; s->Sc_cap = 0;
+            FCK(cudaMalloc(&s->Sc, sizeof(double) * Ms * Ms));
+            s->Sc_cap = (size_t)(Ms * Ms);
+        }
+        FCK(upload(s->pp, s->pp_cap, ppos));
+        FCK(gather_block_launch(s->Sc, f->Kss, Msp, s->pp, Ms, st, &eu->launches));
+        FCK(fsa_permute_launch(0, mu1, s->pp, Ms, f->tmpc, st, &eu->launches));
     }
     for (int64_t i = 0; i < Ms; ++i) {
         const size_t r = (size_t)ppos[(size_t)i];
         mu[i] = mu_p[r];
         if (var) var[i] = var_p[r];
-        if (cov)
+        if (cov_host)
             for (int64_t j = 0; j < Ms; ++j) cov[i * Ms + j] = cov_p[r * (size_t)Msp + (size_t)ppos[(size_t)j]];
     }
+    return GPB200_OK;
+}
+
+// rand(gp, X, n) (src/GP.jl:120-146) with a sparse cK: Sigma* is the covariance predict_cov (modes 0-2) or predict_fsa
+// (mode 3) returns, built on the device and kept there; make_posdef!, the Cholesky and unwhiten! are gpb200_rand's
+// (rand_from_cov on eu, whose Ms x Ms sub-engine shares the handle's stream).  The likelihood, gradient, prediction and
+// cross-validation state is only read.
+int gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of, int64_t nsamp,
+                     const double* z, double nugget, double* mu_minus_mean, double* samples) {
+    if (!f) return GPB200_EINVAL;
+    if (Ms <= 0 || nsamp <= 0 || !xs || ldxs < f->d || !z || !mu_minus_mean || !samples) {
+        f->err = "fitc_rand: bad Ms, nsamp, xs, ldxs, z, mu or samples"; return GPB200_EINVAL;
+    }
+    if (!(nugget >= 0.0)) { f->err = "fitc_rand: nugget must be >= 0"; return GPB200_EINVAL; }
+    if ((f->mode == 3) != (block_of != nullptr)) {
+        f->err = "fitc_rand: block_of is required in FSA mode (3) and must be NULL otherwise"; return GPB200_EINVAL;
+    }
+    if (!f->factored || !f->alpha_ready) { f->err = "fitc_rand: factorize and mll first"; return GPB200_ESTATE; }
+    if (f->mode != 3 && Ms > f->Nc) { f->err = "fitc_rand: too many test points for one staging chunk"; return GPB200_EINVAL; }
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle* eu = f->eu;
+    cudaEvent_t ev_start = eu->ev4;                      // rand_from_cov records ev0 .. ev3
+    FCK(cudaEventRecord(ev_start, eu->st));
+    const double* cov;
+    int64_t ldc;
+    if (f->mode == 3) {
+        static double cov_flag;                          // non-null marker: Sigma* stays on the device
+        f->cov_keep_device = true;
+        const int rc = gpb200_fitc_predict_fsa(f, Ms, xs, ldxs, block_of, mu_minus_mean, nullptr, &cov_flag);
+        f->cov_keep_device = false;
+        if (rc) return rc;
+        cov = f->fsa->Sc; ldc = Ms;
+    } else {
+        TRY(fitc_cov_build(f, Ms, xs, ldxs, mu_minus_mean));
+        cov = f->Kss; ldc = (Ms + TILE - 1) / TILE * TILE;
+    }
+    FSUB(rand_from_cov(eu, Ms, cov, ldc, f->tmpc, nsamp, z, nugget, samples), eu);
+    f->rand_ms[0] = ev_ms(ev_start, eu->ev0);
+    f->rand_ms[1] = ev_ms(eu->ev0, eu->ev1);
+    f->rand_ms[2] = ev_ms(eu->ev3, eu->ev2);
+    return GPB200_OK;
+}
+
+int gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n) {
+    if (!f || !ms || n < 0) return GPB200_EINVAL;
+    for (int32_t i = 0; i < n && i < 3; ++i) ms[i] = f->rand_ms[i];
     return GPB200_OK;
 }
 

@@ -84,6 +84,8 @@ _SIGNATURES = {
     "gpb200_fitc_cv_param": (C.c_int, [_H, C.c_int32, _dp, _dp, _dp]),
     "gpb200_fitc_cv_block": (C.c_int, [_H, C.c_int32, C.c_int64, C.POINTER(C.c_int64), _dp]),
     "gpb200_fitc_launch_count": (C.c_int64, [_H]),
+    "gpb200_fitc_rand": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _lp, C.c_int64, _dp, C.c_double, _dp, _dp]),
+    "gpb200_fitc_get_timings": (C.c_int, [_H, _dp, C.c_int32]),
     "gpb200_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
     "gpb200_group_create": (C.c_int, [C.POINTER(_H), C.c_int]),
     "gpb200_storage_info": (C.c_int, [_H, C.POINTER(C.c_int64), C.c_int32]),
@@ -574,6 +576,32 @@ class FitcEngine:
         out = np.empty((idx.size, idx.size))
         self._check(self._lib.gpb200_fitc_cv_block(self._h, int(which), idx.size, idx.ctypes.data_as(C.POINTER(C.c_int64)),
                                                    _as_dp(out)), "fitc_cv_block")
+        return out
+
+    def rand(self, xs_pm, z, nugget=1e-10, block_of=None):
+        """z: (nsamp, Ms) standard-normal draws (== Julia's Ms x nsamp column-major); block_of[Ms] in FSA mode only (as in
+        predict_fsa).  Returns (mu_minus_mean[Ms], samples (nsamp, Ms))."""
+        xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
+        z = np.ascontiguousarray(z, dtype=np.float64)
+        Ms, d = xs_pm.shape
+        if d != self.d or z.ndim != 2 or z.shape[1] != Ms:
+            raise ValueError("fitc_rand: inconsistent dimensions")
+        bp = None
+        if block_of is not None:
+            block_of = np.ascontiguousarray(block_of, dtype=np.int64)
+            if block_of.shape != (Ms,):
+                raise ValueError("fitc_rand: block_of must have one entry per test point")
+            bp = block_of.ctypes.data_as(_lp)
+        mu = np.empty(Ms)
+        out = np.empty_like(z)
+        self._check(self._lib.gpb200_fitc_rand(self._h, Ms, _as_dp(xs_pm), d, bp, z.shape[0], _as_dp(z), float(nugget),
+                                               _as_dp(mu), _as_dp(out)), "fitc_rand")
+        return mu, out
+
+    def rand_timings(self):
+        """device times (ms) of the last rand: Sigma* build, make_posdef! + Cholesky, unwhiten! + mu"""
+        out = np.zeros(3)
+        self._check(self._lib.gpb200_fitc_get_timings(self._h, _as_dp(out), 3), "fitc_get_timings")
         return out
 
     def launch_count(self):

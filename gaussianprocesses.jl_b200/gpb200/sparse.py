@@ -1,7 +1,8 @@
 """FITC -- host mirror of the reference's sparse strategy `FITC(x, Xu, y, mean, kern, logNoise)`
 (src/sparse/fully_indep_train_conditional.jl:335-338 == GPE(..., FullyIndepStrat(Xu))), over the
 gpb200_fitc_* entry points: update_cK!, alpha / mll / logdet, dmll_noise, dmll_mean!, dmll_kern!,
-predict_f / predict_y.  DTC, SoR and FSA are modes of the same engine."""
+predict_f / predict_y, rand, and GPE's parameter protocol (get_params / set_params / update_target* / optimize).
+DTC, SoR and FSA are modes of the same engine."""
 import math
 
 import numpy as np
@@ -45,8 +46,9 @@ class FITC:
         self.dmll = None
         self.update_mll()
 
-    def update_mll(self):
-        """update_mll! (src/GPE.jl:202-212) with cK::FullyIndepPDMat."""
+    def update_mll(self, noise=True, domean=True, kern=True):
+        """update_mll! (src/GPE.jl:202-212) with cK::FullyIndepPDMat.  The flags are GPE's (update_target passes them);
+        the sparse factorisation is rebuilt whatever they say."""
         self._eng.factorize(flatten(self.kernel, self.dim)[2], self.logNoise)
         mu = self.mean.mean(self._xpm)
         self.alpha, self.mll, self.logdet = self._eng.mll(self.y - mu)
@@ -76,6 +78,21 @@ class FITC:
     def update_mll_and_dmll(self, **kw):
         self.update_mll()
         return self.update_dmll(**kw)
+
+    # ---- GPE's parameter protocol, [noise; mean; kernel] (src/GPE.jl:346-510), and optimize! (src/optimize.jl) -----------
+    # logNoise is a scalar here; FixedKernel parameters are neither returned nor set, their gradients are dropped
+    # (update_dmll's `_exposed`), exactly as for GPE.
+    get_params = GPE.get_params
+    num_params = GPE.num_params
+    set_params = GPE.set_params
+    initialise_target = GPE.initialise_target
+    update_target = GPE.update_target
+    update_target_and_dtarget = GPE.update_target_and_dtarget
+    optimize = GPE.optimize
+
+    # rand(gp, X, n) (src/GP.jl:120-146): GPE's host side; the engine builds Sigma* = predict_f(x; full_cov=true)'s
+    # covariance on the device and factors it there.  Returns a (npred, n) array.
+    rand = GPE.rand
 
     def noise_variance(self):
         return math.exp(2.0 * self.logNoise)
@@ -160,7 +177,7 @@ class FSA(FITC):
         self._pending_blocks = True
         super().__init__(x, Xu, y, mean=mean, kernel=kernel, logNoise=logNoise, device=device)
 
-    def update_mll(self):
+    def update_mll(self, noise=True, domean=True, kern=True):
         """update_mll! with cK::FullScalePDMat (update_cK! :197-230, `\\` :105-108, logdet :142)."""
         if self._pending_blocks:
             self._eng.set_blocks(self._block_ptr, self._idx)
@@ -189,6 +206,21 @@ class FSA(FITC):
         if full_cov:
             return mu, s2 + self.noise_variance() * np.eye(s2.shape[0])
         return mu, s2 + self.noise_variance()
+
+    def rand(self, x, blockindpred, n=1, nugget=1e-10, rng=None):
+        """rand(gp, X, n) with the test blocks of predict_f(x, blockindpred; full_cov=true): n posterior draws, (npred, n).
+        That covariance is positive semi-definite when every test point is paired with the same training block; over
+        several test blocks predictMVN (:413-447) mixes the exact K** with Lambda_xf on the paired blocks only, the matrix
+        is in general indefinite and PosDefException is raised, as in the reference."""
+        rng = np.random.default_rng() if rng is None else rng
+        x = _as_dxn(x)
+        if x.shape[0] != self.dim:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        block_of = test_block_of(blockindpred, x.shape[1])
+        xs = np.ascontiguousarray(x.T)
+        z = rng.standard_normal((int(n), xs.shape[0]))
+        _, draws = self._eng.rand(xs, z, nugget=nugget, block_of=block_of)
+        return (draws + self.mean.mean(xs)[None, :]).T
 
 
 def test_block_of(blockindpred, npred):

@@ -479,11 +479,7 @@ end
 function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::AbstractVector; full_cov::Bool=false) where {X,Y,M,K,CS<:B200FSA,D,P}
     size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
     Xs = Matrix{Float64}(x); Ms = size(Xs, 2)
-    block_of = fill(Int64(-1), Ms)                                                 # 0-based training block of each test point
-    for (j, b) in enumerate(blockindpred), i in b
-        block_of[i] == -1 || throw(ArgumentError("test point $i lies in two prediction blocks"))
-        block_of[i] = j - 1
-    end
+    block_of = test_block_of(blockindpred, Ms)
     mu = Vector{Float64}(undef, Ms)
     var = full_cov ? Float64[] : Vector{Float64}(undef, Ms)
     Σ = full_cov ? Matrix{Float64}(undef, Ms, Ms) : Matrix{Float64}(undef, 0, 0)
@@ -493,6 +489,41 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::Abs
            "fitc_predict_fsa")
     full_cov && return mu .+ mean(gp.mean, Xs), Σ                                 # Σ is symmetric: row- = column-major
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
+end
+
+# 0-based training block of each test point (-1: none) from 1-based test blocks
+function test_block_of(blockindpred::AbstractVector, Ms::Int)
+    block_of = fill(Int64(-1), Ms)
+    for (j, b) in enumerate(blockindpred), i in b
+        block_of[i] == -1 || throw(ArgumentError("test point $i lies in two prediction blocks"))
+        block_of[i] = j - 1
+    end
+    return block_of
+end
+
+# rand(gp, X, n) (src/GP.jl:120-146) with a sparse cK on the device: Sigma* of predict_f(x; full_cov=true) stays there,
+# make_posdef!(Sigma*; nugget) and unwhiten! follow the dense rand! above (gpb200_fitc_rand); block_of is C_NULL outside FSA
+function sparse_rand!(gp::GPE, x::AbstractMatrix, block_of, A::DenseMatrix, nugget)
+    size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
+    Xs = Matrix{Float64}(x); Ms = size(Xs, 2); n = size(A, 2)
+    Z = randn(Ms, n); mu = Vector{Float64}(undef, Ms); S = Matrix{Float64}(undef, Ms, n)
+    checks(gp.cK, ccall((:gpb200_fitc_rand, LIB), Cint,
+                        (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Int64}, Int64, Ptr{Float64}, Float64, Ptr{Float64}, Ptr{Float64}),
+                        gp.cK.handle, Ms, Xs, size(Xs, 1), block_of, n, Z, Float64(nugget), mu, S), "fitc_rand")
+    A .= S .+ mean(gp.mean, Xs)
+    return A
+end
+function Random.rand!(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, A::DenseMatrix; nugget=1e-10) where {X,Y,M,K,CS<:B200Sparse,D,P}
+    return sparse_rand!(gp, x, C_NULL, A, nugget)
+end
+# FSA: the draws use predict_f(gp, x, blockindpred; full_cov=true)'s covariance
+function Random.rand!(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::AbstractVector, A::DenseMatrix;
+                      nugget=1e-10) where {X,Y,M,K,CS<:B200FSA,D,P}
+    return sparse_rand!(gp, x, test_block_of(blockindpred, size(x, 2)), A, nugget)
+end
+function Random.rand(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::AbstractVector, n::Int=1;
+                     nugget=1e-10) where {X,Y,M,K,CS<:B200FSA,D,P}
+    return Random.rand!(gp, x, blockindpred, Matrix{Float64}(undef, size(x, 2), n); nugget=nugget)
 end
 
 # ---- cross-validation on the sparse covariances (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) -------------

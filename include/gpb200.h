@@ -351,6 +351,24 @@ int  gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* bloc
  * grouped by block and each group padded to a multiple of 128, to fit one staging chunk (GPB200_EINVAL otherwise).      */
 int  gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
                              double* mu_minus_mean, double* var, double* cov);
+/* rand(gp, X, n) (src/GP.jl:120-146) with a sparse cK, on the device, with gpb200_rand's conventions: z and samples are
+ * Ms x nsamp column-major, mu_minus_mean[Ms] is the predictive mean without mean(x*).  Sigma* is exactly the covariance of
+ * gpb200_fitc_predict_cov (modes 0-2; block_of must be NULL; Ms <= one staging chunk) or of gpb200_fitc_predict_fsa (mode 3;
+ * block_of[Ms] required, as there; the grouped, padded test blocks must fit one staging chunk); it stays on the device.
+ * (FSA's Sigma* is positive semi-definite when all test points pair with one training block; over several blocks it is in
+ * general indefinite, and k > 0 is returned as the reference's cholesky would.)
+ * make_posdef!(Sigma*; nugget), its Cholesky on an Ms x Ms sub-engine of the handle (created on first use), unwhiten! as one
+ * NT GEMM and + mu follow gpb200_rand; the sub-engine's kernels count in gpb200_fitc_launch_count.  After factorize + mll
+ * (GPB200_ESTATE otherwise).  GPB200_EINVAL: bad Ms, nsamp or ldxs, a NULL xs, z, mu_minus_mean or samples, nugget < 0,
+ * block_of given in modes 0-2 or missing in mode 3, too many test points.  Returns k > 0 when Sigma* + nugget I is not
+ * positive definite; the handle stays usable.  The likelihood, gradient, prediction and cross-validation results of the
+ * handle are unchanged (bitwise).  With several ranks (gpb200_fitc_comm_init) every rank holds the replicated M x M state
+ * and draws on its own, as predict_cov does; that case has not been run on more than one GPU.                          */
+int  gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
+                      int64_t nsamp, const double* z, double nugget, double* mu_minus_mean, double* samples);
+/* device times (ms) of the last successful gpb200_fitc_rand: [0] Sigma* build (with mu), [1] make_posdef! + Cholesky,
+ * [2] unwhiten! GEMM + mu (CUDA events; n <= 3 entries are written)                                                    */
+int  gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n);
 /* ---- cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) ---------------
  * The dense entry points gpb200_get_inverse_diag / gpb200_cv_param / gpb200_cv_block for modes 0 (FITC), 1 (DTC: SoR's
  * covariance) and 2 (SoR), after gpb200_fitc_factorize and gpb200_fitc_mll.  Sigma = Lambda + K_fu K_uu^-1 K_uf is the matrix
