@@ -66,7 +66,7 @@ struct VmBuf {
 struct gpb200_handle {
     int device = 0;
     cudaStream_t st = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr, ev5 = nullptr;
     int64_t N = 0, Npad = 0, ld = 0;
     int d = 0;
     double* x = nullptr;
@@ -109,6 +109,7 @@ struct gpb200_handle {
     // predict workspace
     double *xs = nullptr, *Kst = nullptr, *Kss = nullptr, *pmu = nullptr, *pvar = nullptr, *pkdiag = nullptr;
     int64_t xs_cap = 0, Kst_rows = 0, Kss_rows = 0;
+    double* pdx = nullptr; int64_t pdx_rows = 0;   // gpb200_predict_grad: dmu (Mpad x d), then dvar (Mpad x d)
     CUtensorMap mapKst{};
     // options
     int nb = 0;                 // outer Cholesky block; 0 = fully recursive (one panel)
@@ -118,7 +119,7 @@ struct gpb200_handle {
     cudaStream_t st_cur = nullptr;             // stream launch_gemm / the leaf use right now (st or st_side)
     cudaEvent_t ev_la0 = nullptr, ev_la2 = nullptr;
     // stats
-    double ms[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    double ms[16] = {};
     int64_t launches = 0;
     bool own_stream = true;
     // per-launch GEMM profiling (option "profile"): event pairs + executed flops of every GEMM launch
@@ -197,6 +198,7 @@ struct gpb200_fitc {
     CUtensorMap mapAt{}, mapC{}, mapCt{}, mapH{}, mapT{};
     bool grad_ws = false;
     double* Kss = nullptr; int64_t Kss_rows = 0;      // full predictive covariance (gpb200_fitc_predict_cov)
+    double* pdx = nullptr;                            // gpb200_fitc_predict_grad: dmu, dvar of a chunk (2 x Nc x d; first use)
     // posterior sampling (gpb200_fitc_rand): the Ms x Ms sub-engine and the staging of the draws are eu's (rand_from_cov)
     bool cov_keep_device = false;                     // predict_fsa: leave Sigma* in caller order on the device (fsa->Sc)
     double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
@@ -318,7 +320,7 @@ void free_data(gpb200_handle* h) {
     free_FG(h);
     double** ptrs[] = {&h->x, &h->Dinv, &h->DinvT, &h->logd, &h->noise_var, &h->r0, &h->r1,
                        &h->y1, &h->alpha, &h->scal, &h->part, &h->trace_out, &h->xs, &h->Kst, &h->Kss,
-                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt, &h->ZdT};
+                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt, &h->ZdT, &h->pdx};
     h->xmap_ok = false;
     if (h->cvD) cudaFree(h->cvD);
     if (h->cvY) cudaFree(h->cvY);
@@ -335,7 +337,7 @@ void free_data(gpb200_handle* h) {
     if (h->ag_send) cudaFree(h->ag_send);
     if (h->ag_recv) cudaFree(h->ag_recv);
     h->ag_send = h->ag_recv = nullptr; h->pack_elems = h->ag_send_elems = h->ag_recv_elems = 0;
-    h->xs_cap = h->Kst_rows = h->Kss_rows = 0;
+    h->xs_cap = h->Kst_rows = h->Kss_rows = h->pdx_rows = 0;
     h->has_data = h->factored = h->inv_ready = h->alpha_ready = false;
 }
 
@@ -969,6 +971,36 @@ cudaError_t trsm_rec(gpb200_handle* h, int Mpad, int c0, int n) {
     return trsm_rec_buf(h, bk, Mpad, c0, n);
 }
 
+// Vt[:, c0..c0+n) <- Vt[:, c0..c0+n) L[c0.., c0..]^-1, the mirror of trsm_rec_buf: the second half is solved first, then
+// X1 -= X2 L21 as an NT GEMM whose B operand is L21' -- rows of U = L' in F's strict-upper tiles, which the caller has filled
+// (mirror_lower_tiles_launch) -- and the leaves multiply by DinvT = (L_tt^-1)'.
+cudaError_t trsm_right_rec_buf(gpb200_handle* h, GemmBuf bk, int rows, int c0, int n) {
+    double* kb = const_cast<double*>(bk.base);
+    if (n == TILE) {
+        GemmDesc g = gemm_desc_default();
+        g.A = GemmOperand{bk, bufNone(), 0, c0};
+        g.B = GemmOperand{bufDinvT(h), bufNone(), c0, 0};
+        g.C = kb; g.ldc = bk.ld; g.c_row0 = 0; g.c_col0 = c0;
+        g.M = rows; g.N = TILE; g.K = TILE;
+        return launch_gemm(h, g);
+    }
+    int n1 = TILE;
+    while (n1 * 2 < n) n1 *= 2;
+    const int n2 = n - n1;
+    cudaError_t e;
+    if ((e = trsm_right_rec_buf(h, bk, rows, c0 + n1, n2)) != cudaSuccess) return e;
+    {
+        GemmDesc g = gemm_desc_default();
+        g.A = GemmOperand{bk, bufNone(), 0, c0 + n1};
+        g.B = GemmOperand{bufF(h), bufNone(), c0, c0 + n1};
+        g.C = kb; g.ldc = bk.ld; g.c_row0 = 0; g.c_col0 = c0;
+        g.M = rows; g.N = n1; g.K = n2;
+        g.alpha = -1.0; g.beta = 1.0;
+        if ((e = launch_gemm(h, g)) != cudaSuccess) return e;
+    }
+    return trsm_right_rec_buf(h, bk, rows, c0, n1);
+}
+
 float ev_ms(cudaEvent_t a, cudaEvent_t b) {
     float ms = 0.f;
     cudaEventElapsedTime(&ms, a, b);
@@ -1151,6 +1183,7 @@ int gpb200_create(gpb200_handle** out, int device) {
     if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
     if ((e = cudaStreamCreateWithFlags(&h->st, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
     cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1); cudaEventCreate(&h->ev2); cudaEventCreate(&h->ev3); cudaEventCreate(&h->ev4);
+    cudaEventCreate(&h->ev5);
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -1186,6 +1219,7 @@ void gpb200_destroy(gpb200_handle* h) {
     if (h->ev2) cudaEventDestroy(h->ev2);
     if (h->ev3) cudaEventDestroy(h->ev3);
     if (h->ev4) cudaEventDestroy(h->ev4);
+    if (h->ev5) cudaEventDestroy(h->ev5);
     if (h->ev_la0) cudaEventDestroy(h->ev_la0);
     if (h->ev_la2) cudaEventDestroy(h->ev_la2);
     if (h->st_side) cudaStreamDestroy(h->st_side);
@@ -1265,7 +1299,7 @@ int gpb200_set_stream(gpb200_handle* h, void* stream) {
 
 int gpb200_get_timings(gpb200_handle* h, double* ms, int32_t n) {
     if (!h || !ms) return GPB200_EINVAL;
-    for (int i = 0; i < n && i < 12; ++i) ms[i] = h->ms[i];
+    for (int i = 0; i < n && i < 16; ++i) ms[i] = h->ms[i];
     return GPB200_OK;
 }
 
@@ -1734,6 +1768,83 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
     CK(cudaStreamSynchronize(h->st));
     profile_collect(h);
     h->ms[5] = ev_ms(h->ev2, h->ev3);
+    return GPB200_OK;
+}
+
+// Predictive gradients (for ForwardDiff.Dual test inputs of predict_f): mu and var through the same launches as gpb200_predict,
+// then, with W' = V' L^-1 = K*' K^-1 (rows w_m' = (K^-1 k*_m)'),
+//   dmu[m, :] = sum_i dk(x*_m, x_i)/dx*_m alpha_i,   dvar[m, :] = 2 dk(x*_m, x*_m)/dx*_m - 2 sum_i dk(x*_m, x_i)/dx*_m W'[m, i].
+// F's strict-upper tiles are scratch between calls (inverse merges, GPA's Z'); every call that solves for W' first fills
+// them with L' (one O(N^2) pass).  Timing slots 11..15: cross-Gram + mean, V' + variance, transpose, W', contraction.
+int gpb200_predict_grad(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, const double* alpha,
+                        double* mu, double* var, double* dmu, double* dvar) {
+    if (!h) return GPB200_EINVAL;
+    if (h->nranks > 1 || h->sharded || h->grp) return fail(h, GPB200_EINVAL, "predict_grad: single GPU handles only");
+    if (!h->factored) return fail(h, GPB200_ESTATE, "predict_grad: factorize first");
+    if (M <= 0 || !xs || ldxs < h->d || !mu || !dmu) return fail(h, GPB200_EINVAL, "predict_grad: bad M, xs, ldxs, mu or dmu");
+    if (!var != !dvar) return fail(h, GPB200_EINVAL, "predict_grad: var and dvar must be given together");
+    if (!alpha && !h->alpha_ready) return fail(h, GPB200_ESTATE, "predict_grad: no alpha (call mll or pass alpha)");
+    CK(cudaSetDevice(h->device));
+    if (alpha) {
+        int rc = upload_padded(h, h->alpha, alpha);
+        if (rc) return rc;
+        h->alpha_ready = true;
+    }
+    int64_t cap = (int64_t)(16.0e9 / (8.0 * (double)h->Npad)) / TILE * TILE;       // as gpb200_predict
+    if (const char* env = getenv("GPB200_PREDICT_CHUNK")) {
+        const int64_t v = atoll(env) / TILE * TILE;
+        if (v >= TILE && v < cap) cap = v;
+    }
+    if (cap < TILE) cap = TILE;
+    const int d = h->d;
+    for (int i = 11; i < 16; ++i) h->ms[i] = 0.0;
+    for (int64_t m0 = 0; m0 < M; m0 += cap) {
+        const int64_t Mc = (M - m0 < cap) ? M - m0 : cap;
+        const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
+        int rc = ensure_predict_ws(h, Mc, false);
+        if (rc) return rc;
+        if (Mpad > h->pdx_rows) {
+            if (h->pdx) cudaFree(h->pdx);
+            h->pdx = nullptr; h->pdx_rows = 0;
+            CK(cudaMalloc(&h->pdx, sizeof(double) * 2 * Mpad * d));
+            h->pdx_rows = Mpad;
+        }
+        double* ddmu = h->pdx;
+        double* ddvar = h->pdx + h->pdx_rows * d;
+        CK(cudaEventRecord(h->ev0, h->st));
+        CK(cudaMemcpy2DAsync(h->xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d, Mc,
+                             cudaMemcpyHostToDevice, h->st));
+        CK(crossgram_launch(h->prog, h->xs, d, Mc, Mpad, h->x, d, h->N, h->Npad, d, h->Kst, h->Npad, h->st, &h->launches));
+        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));
+        CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+        CK(cudaEventRecord(h->ev1, h->st));
+        if (var) {
+            CK(trsm_rec(h, (int)Mpad, 0, (int)h->Npad));                                   // V' = K*' L^-T
+            CK(kdiag_launch(h->prog, h->xs, d, Mc, h->pkdiag, h->st, &h->launches));
+            CK(rowvar_launch(h->Kst, h->Npad, h->pkdiag, Mc, h->Npad, h->pvar, h->st, &h->launches));
+            CK(cudaMemcpyAsync(var + m0, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+        }
+        CK(cudaEventRecord(h->ev2, h->st));
+        if (var && m0 == 0) CK(mirror_lower_tiles_launch(h->F, h->ld, h->Npad, h->st, &h->launches));   // L' into F's upper tiles
+        CK(cudaEventRecord(h->ev5, h->st));
+        if (var) {
+            GemmBuf bk{h->tma_ok ? &h->mapKst : nullptr, h->Kst, h->Npad};
+            CK(trsm_right_rec_buf(h, bk, (int)Mpad, 0, (int)h->Npad));                     // W' = V' L^-1
+        }
+        CK(cudaEventRecord(h->ev3, h->st));
+        CK(crossgram_dx_launch(h->prog, h->xs, d, Mc, h->x, d, h->N, d, h->alpha, var ? h->Kst : nullptr, nullptr, h->Npad, 1.0,
+                               ddmu, ddvar, h->st, &h->launches));
+        CK(cudaEventRecord(h->ev4, h->st));
+        CK(cudaMemcpyAsync(dmu + m0 * d, ddmu, sizeof(double) * Mc * d, cudaMemcpyDeviceToHost, h->st));
+        if (var) CK(cudaMemcpyAsync(dvar + m0 * d, ddvar, sizeof(double) * Mc * d, cudaMemcpyDeviceToHost, h->st));
+        CK(cudaStreamSynchronize(h->st));
+        h->ms[11] += ev_ms(h->ev0, h->ev1);
+        h->ms[12] += ev_ms(h->ev1, h->ev2);
+        h->ms[13] += ev_ms(h->ev2, h->ev5);
+        h->ms[14] += ev_ms(h->ev5, h->ev3);
+        h->ms[15] += ev_ms(h->ev3, h->ev4);
+    }
+    profile_collect(h);
     return GPB200_OK;
 }
 
@@ -2489,7 +2600,7 @@ void gpb200_fitc_destroy(gpb200_fitc* f) {
     if (f->eu && f->eu->st) cudaStreamSynchronize(f->eu->st);
     double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
                        &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
-                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp};
+                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx};
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     if (f->Kss) cudaFree(f->Kss);
     fsa_free(f);
@@ -2527,7 +2638,7 @@ int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, 
     cudaStream_t st = f->eu->st;
     double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
                        &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
-                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp};
+                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx};
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     f->grad_ws = false;
     fsa_free(f);                                      // the FSA blocks refer to the old observations
@@ -2758,6 +2869,61 @@ int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ld
     return GPB200_OK;
 }
 
+// Predictive gradients of the sparse models (predict_f with ForwardDiff.Dual inputs): mu and var through
+// gpb200_fitc_predict's launches (A = K*u L_uu^-T in bufA, B = K*u L_s^-T in bufB), then W' = A L_uu^-1 - B L_s^-1
+// (= K*u K_uu^-1 - K*u Sigma_QR^-1; SoR: - B L_s^-1) by the right-side TRSM on the two M x M sub-engines, whose F holds L'
+// in its strict-upper tiles for the call, and the contraction over the inducing points with alpha = u:
+//   dmu[m, :] = sum_j dk(x*_m, u_j)/dx*_m u_j,   dvar[m, :] = 2c dk(x*_m, x*_m)/dx*_m - 2 sum_j dk(x*_m, u_j)/dx*_m W'[m, j]
+// with c = 1 (FITC, DTC) or 0 (SoR, whose variance has no k_xx).  Single GPU, modes 0-2.
+int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* var,
+                             double* dmu, double* dvar) {
+    if (!f) return GPB200_EINVAL;
+    if (!f->factored || !f->alpha_ready) { f->err = "fitc_predict_grad: factorize and mll first"; return GPB200_ESTATE; }
+    if (f->mode == 3) { f->err = "fitc_predict_grad: not available for FSA"; return GPB200_EINVAL; }
+    if (f->nranks > 1) { f->err = "fitc_predict_grad: single GPU handles only"; return GPB200_EINVAL; }
+    if (Ms <= 0 || !xs || ldxs < f->d || !mu || !dmu) { f->err = "fitc_predict_grad: bad Ms, xs, ldxs, mu or dmu"; return GPB200_EINVAL; }
+    if (!var != !dvar) { f->err = "fitc_predict_grad: var and dvar must be given together"; return GPB200_EINVAL; }
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int d = f->d;
+    if (!f->pdx) FCK(cudaMalloc(&f->pdx, sizeof(double) * 2 * f->Nc * d));
+    double* ddmu = f->pdx;
+    double* ddvar = f->pdx + f->Nc * d;
+    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
+    if (var) {
+        FCK(mirror_lower_tiles_launch(eu->F, eu->ld, eu->Npad, st, &eu->launches));
+        FCK(mirror_lower_tiles_launch(es->F, es->ld, es->Npad, st, &eu->launches));
+    }
+    for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
+        const int64_t mc = std::min(f->Nc, Ms - m0);
+        FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d,
+                              mc, cudaMemcpyHostToDevice, st));
+        FCK(fitc_kfu(f, f->xs, mc));
+        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st, &eu->launches));
+        FCK(cudaMemcpyAsync(mu + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        if (var) {                                                          // as gpb200_fitc_predict
+            FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(kdiag_launch(eu->prog, f->xs, d, mc, f->tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st, &eu->launches));
+            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st, &eu->launches));
+            if (f->mode == 2) FCK(cudaMemsetAsync(f->tmpc2, 0, sizeof(double) * mc, st));
+            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st, &eu->launches));
+            FCK(cudaMemcpyAsync(var + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+            if (f->mode != 2) FCK(trsm_right_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));      // A L_uu^-1
+            FCK(trsm_right_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));                        // B L_s^-1
+        }
+        FCK(crossgram_dx_launch(eu->prog, f->xs, d, mc, eu->x, d, f->M, d, f->uvec, (var && f->mode != 2) ? f->bufA : nullptr,
+                                var ? f->bufB : nullptr, f->Mpad, f->mode == 2 ? 0.0 : 1.0, ddmu, ddvar, st, &eu->launches));
+        FCK(cudaMemcpyAsync(dmu + m0 * d, ddmu, sizeof(double) * mc * d, cudaMemcpyDeviceToHost, st));
+        if (var) FCK(cudaMemcpyAsync(dvar + m0 * d, ddvar, sizeof(double) * mc * d, cudaMemcpyDeviceToHost, st));
+        FCK(cudaStreamSynchronize(st));
+    }
+    return GPB200_OK;
+}
 
 // predictMVN with the FULL predictive covariance (fitc.jl:324-332 -> determ_train_conditional.jl:41-59 ->
 // subsetofregressors.jl:302-321):  Sigma* = K** - K*u K_uu^-1 Ku* + K*u S^-1 Ku*   (FITC, DTC);   K*u S^-1 Ku*   (SoR)
@@ -3277,7 +3443,7 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
         const int64_t cap = std::min<int64_t>((int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE, 32768);
         if (cap > f->Nc) {
             double** ptrs[] = {&f->xs, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2, &f->bufA, &f->bufB, &f->bufC, &f->Hbuf, &f->Wbuf,
-                               &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp};
+                               &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx};
             for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
             f->grad_ws = false;
             const int64_t nc = cap;

@@ -488,6 +488,65 @@ __global__ void kdiag_grad_kernel(const __grid_constant__ KProg P, const double*
     for (int p = 0; p < P.n_theta; ++p) out[(long long)p * N + i] = gi * gbuf[p];
 }
 
+// predictive gradients, one CTA per test point m (x* staged in shared memory):
+//   dmu[m, :]  = sum_i dk(xs_m, z_i)/dxs_m a_i
+//   dvar[m, :] = 2c dk(xs_m, xs_m)/dxs_m - 2 sum_i dk(xs_m, z_i)/dxs_m W[m, i],  W = W1 - W2 (either may be null; both
+//   null: dmu only -- the sparse models pass W1 = A L_uu^-1 and W2 = B L_s^-1, SoR only W2)
+// Thread t takes i = t, t + DX_NT, ... in order, then every coordinate is summed over the threads by one fixed tree, so a
+// row's result does not depend on the launch it belongs to.  The d-vector accumulators are indexed by the leaves' input
+// dimensions at run time and live in local memory.
+constexpr int DX_NT = 128;
+__global__ void __launch_bounds__(DX_NT) crossgram_dx_kernel(const __grid_constant__ KProg P, const double* __restrict__ xs,
+                                                             long long ldxs, const double* __restrict__ z, long long ldz,
+                                                             long long n, int d, const double* __restrict__ a,
+                                                             const double* __restrict__ W1, const double* __restrict__ W2,
+                                                             long long ldw, double c,
+                                                             double* __restrict__ dmu, double* __restrict__ dvar) {
+    __shared__ double sx[GPB200_MAX_DIMS];
+    __shared__ double red[DX_NT];
+    const long long m = blockIdx.x;
+    const int t = threadIdx.x;
+    for (int k = t; k < d; k += DX_NT) sx[k] = xs[m * ldxs + k];
+    __syncthreads();
+    double gm[GPB200_MAX_DIMS], gv[GPB200_MAX_DIMS];
+    for (int k = 0; k < d; ++k) { gm[k] = 0.0; gv[k] = 0.0; }
+    const bool W = W1 || W2;
+    const double* w1 = W1 ? W1 + m * ldw : nullptr;
+    const double* w2 = W2 ? W2 + m * ldw : nullptr;
+    // the k(x*, x*) term enters thread 0's sum as -c dk(x*, x*)/dx*, so that dvar = -2 (sum)
+    if (W && t == 0 && c != 0.0) kprog_eval_dx(P, sx, sx, 0.0, gm, -c, gv);
+    for (long long i = t; i < n; i += DX_NT) {
+        const double wi = (w1 ? w1[i] : 0.0) - (w2 ? w2[i] : 0.0);
+        kprog_eval_dx(P, sx, z + i * ldz, a[i], gm, wi, W ? gv : nullptr);
+    }
+    for (int k = 0; k < d; ++k) {
+        for (int which = 0; which < (W ? 2 : 1); ++which) {
+            red[t] = which ? gv[k] : gm[k];
+            __syncthreads();
+            for (int s = DX_NT / 2; s > 0; s >>= 1) {
+                if (t < s) red[t] += red[t + s];
+                __syncthreads();
+            }
+            if (t == 0) {
+                if (which) dvar[m * d + k] = -2.0 * red[0];
+                else dmu[m * d + k] = red[0];
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// strict-upper tiles of the Npad x Npad matrix F <- transpose of its strict-lower tiles (diagonal tiles untouched)
+__global__ void mirror_lower_tiles_kernel(double* __restrict__ F, long long ld) {
+    __shared__ double tl[32][33];
+    const int bx = blockIdx.x, by = blockIdx.y;             // 32 x 32 block (by, bx) of the lower source
+    if ((bx * 32) / TB >= (by * 32) / TB) return;
+    const long long r0 = (long long)by * 32, c0 = (long long)bx * 32;
+    for (int r = threadIdx.y; r < 32; r += 8) tl[r][threadIdx.x] = F[(r0 + r) * ld + c0 + threadIdx.x];
+    __syncthreads();
+    for (int r = threadIdx.y; r < 32; r += 8) F[(c0 + r) * ld + r0 + threadIdx.x] = tl[threadIdx.x][r];
+}
+
 size_t xtile_smem(int d) { return (size_t)2 * TB * (d | 1) * sizeof(double); }
 
 template <typename K>
@@ -632,6 +691,24 @@ cudaError_t crossgram_grad_launch(const KProg& P, const double* x1, int64_t ldx1
     cudaError_t e;
     if ((e = ensure_smem(crossgram_grad_kernel, sm)) != cudaSuccess) return e;
     crossgram_grad_kernel<<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, j, D, ldd);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t crossgram_dx_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, const double* z, int64_t ldz, int64_t n,
+                                int d, const double* a, const double* W1, const double* W2, int64_t ldw, double c, double* dmu,
+                                double* dvar, cudaStream_t st, int64_t* launches) {
+    if (M <= 0) return cudaSuccess;
+    if (d <= 0 || d > GPB200_MAX_DIMS || ((W1 || W2) && !dvar)) return cudaErrorInvalidValue;
+    crossgram_dx_kernel<<<(unsigned)M, DX_NT, 0, st>>>(P, xs, ldxs, z, ldz, n, d, a, W1, W2, ldw, c, dmu, dvar);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t mirror_lower_tiles_launch(double* F, int64_t ld, int64_t Npad, cudaStream_t st, int64_t* launches) {
+    if (Npad <= TB) return cudaSuccess;
+    dim3 grid((unsigned)(Npad / 32), (unsigned)(Npad / 32)), block(32, 8);
+    mirror_lower_tiles_kernel<<<grid, block, 0, st>>>(F, ld);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

@@ -37,3 +37,11 @@ cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, 
 cudaError_t crossgram_grad_launch(const KProg& P, const double* x1, int64_t ldx1, int64_t N1, int64_t N1pad, const double* x2,
                                   int64_t ldx2, int64_t N2, int64_t N2pad, int d, int j, double* D, int64_t ldd, cudaStream_t st,
                                   int64_t* launches);
+// predictive gradients (M x d outputs, point-major):  dmu[m, :] = sum_i dk(xs_m, z_i)/dxs_m a_i ;  with W = W1 - W2 (either may
+// be null; row m at W + m * ldw, n columns read): dvar[m, :] = 2c dk(xs_m, xs_m)/dxs_m - 2 sum_i dk(xs_m, z_i)/dxs_m W[m, i].
+// Both null: dmu only.  Fixed-order sums.
+cudaError_t crossgram_dx_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, const double* z, int64_t ldz, int64_t n,
+                                int d, const double* a, const double* W1, const double* W2, int64_t ldw, double c, double* dmu,
+                                double* dvar, cudaStream_t st, int64_t* launches);
+// F[j, i] = F[i, j] for every element of the strict-lower 128-tiles of the Npad x Npad matrix F (diagonal tiles untouched)
+cudaError_t mirror_lower_tiles_launch(double* F, int64_t ld, int64_t Npad, cudaStream_t st, int64_t* launches);

@@ -249,4 +249,99 @@ __device__ __forceinline__ double kprog_eval(const KProg& P, const double* xi, c
     return val[P.n_ops - 1];
 }
 
+// Input derivative of one leaf: g1[dims[p]] += s1 * dk(xi, xj)/dxi_p and, if g2, g2[dims[p]] += s2 * the same.  Indexing by
+// the global input dimension makes a Masked leaf map itself.  At r = 0 the stationary leaves return the limit of the
+// derivative (0, from formulas that carry the difference xi - xj as a factor; Periodic through the guarded sin(2u)/r),
+// Mat12 returns 0 where its derivative is undefined; Noise and Const are constant in xi.
+static __device__ __noinline__ void kp_leaf_dx(const KProg& P, int q, const double* xi, const double* xj, double s1, double* g1,
+                                               double s2, double* g2) {
+    const int* dims = P.dims + P.doff[q];
+    const int nd = P.nd[q];
+    const double* c = P.par + P.toff[q];
+    const int nth = P.nth[q];
+    const int op = P.op[q];
+    // dk/dxi_p = f * w_p * (xi_p - xj_p) for the stationary leaves (w_p = 1 for the isotropic ones), xj_p * w_p for Lin / Poly
+    double f = 0.0;
+    bool ard = false, lin = false;                  // ard: w_p = c[p] (1 / c[p]^2 for LinArd)
+    switch (op) {
+    case GPB200_OP_SE_ISO:
+        f = -c[1] * exp(-0.5 * kp_sqdist(dims, nd, xi, xj) / c[0]) / c[0]; break;
+    case GPB200_OP_SE_ARD:
+        f = -c[nth - 1] * exp(-kp_wsqdist(dims, nd, c, xi, xj) / 2.0); ard = true; break;
+    case GPB200_OP_MAT12_ISO: {
+        const double r = sqrt(kp_sqdist(dims, nd, xi, xj));
+        f = (r == 0.0) ? 0.0 : -c[1] * exp(-r / c[0]) / (c[0] * r);
+    } break;
+    case GPB200_OP_MAT32_ISO: {
+        const double s = sqrt(3.0) * sqrt(kp_sqdist(dims, nd, xi, xj)) / c[0];
+        f = -3.0 * c[1] * exp(-s) / (c[0] * c[0]);
+    } break;
+    case GPB200_OP_MAT52_ISO: {
+        const double s = sqrt(5.0) * sqrt(kp_sqdist(dims, nd, xi, xj)) / c[0];
+        f = -5.0 / 3.0 * c[1] * (1.0 + s) * exp(-s) / (c[0] * c[0]);
+    } break;
+    case GPB200_OP_MAT12_ARD: case GPB200_OP_MAT32_ARD: case GPB200_OP_MAT52_ARD: {
+        const double r = sqrt(kp_wsqdist(dims, nd, c, xi, xj)), sv = c[nth - 1];
+        if (op == GPB200_OP_MAT12_ARD) f = (r == 0.0) ? 0.0 : -sv * exp(-r) / r;
+        else if (op == GPB200_OP_MAT32_ARD) f = -3.0 * sv * exp(-sqrt(3.0) * r);
+        else { const double s = sqrt(5.0) * r; f = -5.0 / 3.0 * sv * (1.0 + s) * exp(-s); }
+        ard = true;
+    } break;
+    case GPB200_OP_RQ_ISO: {
+        const double part = 1.0 + kp_sqdist(dims, nd, xi, xj) / (2.0 * c[2] * c[0]);
+        f = -c[1] * exp(-(c[2] + 1.0) * log(part)) / c[0];
+    } break;
+    case GPB200_OP_RQ_ARD: {
+        const double al = c[nth - 1], part = 1.0 + kp_wsqdist(dims, nd, c, xi, xj) / (2.0 * al);
+        f = -c[nth - 2] * exp(-(al + 1.0) * log(part)); ard = true;
+    } break;
+    case GPB200_OP_PERIODIC: {
+        const double r = sqrt(kp_sqdist(dims, nd, xi, xj));
+        const double l2 = c[0], sv = c[1], per = c[2], pi = 3.141592653589793, t = 2.0 / l2;
+        double sn, cs;
+        sincos(pi * r / per, &sn, &cs);
+        const double s2r = (r == 0.0) ? 2.0 * pi / per : 2.0 * sn * cs / r;       // sin(2u) / r, u = pi r / per
+        f = -sv * exp(-t * (sn * sn)) * t * (pi / per) * s2r;
+    } break;
+    case GPB200_OP_LIN_ISO: f = 1.0 / c[0]; lin = true; break;
+    case GPB200_OP_LIN_ARD: f = 1.0; lin = ard = true; break;
+    case GPB200_OP_POLY: {
+        const int deg = P.extra[q];
+        const double base = c[0] + kp_dot(dims, nd, xi, xj);
+        double pw1 = 1.0;
+        for (int e = 0; e < deg - 1; ++e) pw1 *= base;
+        f = (deg >= 1) ? c[1] * deg * pw1 : 0.0; lin = true;
+    } break;
+    default: return;                                // Noise, Const
+    }
+    for (int p = 0; p < nd; ++p) {
+        const int k = dims[p];
+        const double w = !ard ? 1.0 : (op == GPB200_OP_LIN_ARD) ? 1.0 / (c[p] * c[p]) : c[p];
+        const double v = f * w * (lin ? xj[k] : xi[k] - xj[k]);
+        g1[k] += s1 * v;
+        if (g2) g2[k] += s2 * v;
+    }
+}
+
+// dk(xi, xj)/dxi of the full program, accumulated as kp_leaf_dx does: one forward sweep for the node values, the adjoint
+// sweep of kprog_eval, then every leaf's input derivative scaled by its adjoint.
+__device__ __forceinline__ void kprog_eval_dx(const KProg& P, const double* xi, const double* xj, double s1, double* g1,
+                                              double s2, double* g2) {
+    if (P.n_ops == 1) { kp_leaf_dx(P, 0, xi, xj, s1, g1, s2, g2); return; }
+    double val[GPB200_MAX_OPS], adj[GPB200_MAX_OPS];
+    for (int q = 0; q < P.n_ops; ++q) {
+        const int op = P.op[q];
+        if (op == GPB200_OP_SUM) val[q] = val[P.left[q]] + val[q - 1];
+        else if (op == GPB200_OP_PROD) val[q] = val[P.left[q]] * val[q - 1];
+        else val[q] = kp_leaf<false>(P, q, xi, xj, nullptr);
+    }
+    adj[P.n_ops - 1] = 1.0;
+    for (int q = P.n_ops - 1; q >= 0; --q) {
+        const int op = P.op[q];
+        if (op == GPB200_OP_SUM) { adj[P.left[q]] = adj[q]; adj[q - 1] = adj[q]; }
+        else if (op == GPB200_OP_PROD) { adj[P.left[q]] = adj[q] * val[q - 1]; adj[q - 1] = adj[q] * val[P.left[q]]; }
+        else kp_leaf_dx(P, q, xi, xj, s1 * adj[q], g1, s2 * adj[q], g2);
+    }
+}
+
 #endif  // __CUDACC__

@@ -38,6 +38,7 @@ _SIGNATURES = {
     "gpb200_grad_prepare": (C.c_int, [_H]),
     "gpb200_grad_kernel": (C.c_int, [_H, _dp, _dp, _dp]),
     "gpb200_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
+    "gpb200_predict_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp, _dp]),
     "gpb200_rand": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, C.c_int64, _dp, C.c_double, _dp, _dp]),
     "gpb200_append": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
     "gpb200_unwhiten": (C.c_int, [_H, _dp, _dp]),
@@ -75,6 +76,7 @@ _SIGNATURES = {
     "gpb200_fitc_grad_noise": (C.c_int, [_H, _dp]),
     "gpb200_fitc_grad_kernel": (C.c_int, [_H, _dp]),
     "gpb200_fitc_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp]),
+    "gpb200_fitc_predict_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
     "gpb200_fitc_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
     "gpb200_fitc_predict_cov": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp]),
     "gpb200_fitc_set_mode": (C.c_int, [_H, C.c_int]),
@@ -236,6 +238,21 @@ class Engine:
                                              _as_dp(cov) if full_cov else None), "predict")
         return mu, var, cov
 
+    def predict_grad(self, xs_pm, alpha=None, want_var=True):
+        """(mu_minus_mean[M], var[M] or None, dmu (M, d), dvar (M, d) or None): predictions and their gradients with respect to
+        the test inputs; var unclamped, the mean function's part left to the caller."""
+        xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
+        M, d = xs_pm.shape
+        if d != self.d:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        mu, dmu = np.empty(M), np.empty((M, d))
+        var = np.empty(M) if want_var else None
+        dvar = np.empty((M, d)) if want_var else None
+        ap = _as_dp(np.ascontiguousarray(alpha, dtype=np.float64)) if alpha is not None else None
+        self._check(self._lib.gpb200_predict_grad(self._h, M, _as_dp(xs_pm), d, ap, _as_dp(mu), _as_dp(var) if want_var else None,
+                                                  _as_dp(dmu), _as_dp(dvar) if want_var else None), "predict_grad")
+        return mu, var, dmu, dvar
+
     def rand(self, xs_pm, z, nugget=1e-10, alpha=None):
         """z: (nsamp, M) standard-normal draws (== Julia's M x nsamp column-major).  Returns (mu_minus_mean[M], samples (nsamp, M))."""
         xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
@@ -329,10 +346,12 @@ class Engine:
         return np.tril(K)
 
     def timings(self):
-        ms = np.zeros(12)
-        self._check(self._lib.gpb200_get_timings(self._h, _as_dp(ms), 12), "get_timings")
+        ms = np.zeros(16)
+        self._check(self._lib.gpb200_get_timings(self._h, _as_dp(ms), 16), "get_timings")
         return dict(gram=ms[0], cholesky=ms[1], solve_mll=ms[2], inverse=ms[3], trace=ms[4], predict=ms[5],
-                    gemm_launches=ms[6], gemm_ms=ms[7], gemm_flops=ms[8], gpa_scan=ms[9], gpa_product=ms[10])
+                    gemm_launches=ms[6], gemm_ms=ms[7], gemm_flops=ms[8], gpa_scan=ms[9], gpa_product=ms[10],
+                    pgrad_crossgram=ms[11], pgrad_trsm=ms[12], pgrad_transpose=ms[13], pgrad_trsm_right=ms[14],
+                    pgrad_contract=ms[15])
 
     def set_stream(self, cuda_stream):
         """Run on the caller's CUDA stream (int handle, e.g. torch.cuda.current_stream().cuda_stream); 0/None = private."""
@@ -512,6 +531,22 @@ class FitcEngine:
                                                   _as_dp(var) if want_var else None), "fitc_predict")
         return mu, var
 
+    def predict_grad(self, xs_pm, alpha=None, want_var=True):
+        """as Engine.predict_grad: (mu_minus_mean, var or None, dmu (Ms, d), dvar (Ms, d) or None); alpha must be None (the
+        sparse engine's own u is used)"""
+        if alpha is not None:
+            raise ValueError("fitc_predict_grad: the sparse engine predicts from its own u")
+        xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
+        Ms, d = xs_pm.shape
+        if d != self.d:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        mu, dmu = np.empty(Ms), np.empty((Ms, d))
+        var = np.empty(Ms) if want_var else None
+        dvar = np.empty((Ms, d)) if want_var else None
+        self._check(self._lib.gpb200_fitc_predict_grad(self._h, Ms, _as_dp(xs_pm), d, _as_dp(mu), _as_dp(var) if want_var else None,
+                                                       _as_dp(dmu), _as_dp(dvar) if want_var else None), "fitc_predict_grad")
+        return mu, var, dmu, dvar
+
     def comm_init(self, nranks, rank, id128):
         ib = C.create_string_buffer(bytes(id128), 128)
         self._check(self._lib.gpb200_fitc_comm_init(self._h, int(nranks), int(rank), C.cast(ib, C.c_char_p)), "fitc_comm_init")
@@ -667,6 +702,9 @@ class LocalGroupEngine:
 
     def rand(self, *a, **k):
         return self.lead.rand(*a, **k)
+
+    def predict_grad(self, *a, **k):
+        return self.lead.predict_grad(*a, **k)
 
     def cv_param(self, *a, **k):
         return self.lead.cv_param(*a, **k)

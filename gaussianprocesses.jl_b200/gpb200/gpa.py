@@ -10,7 +10,7 @@ import math
 import numpy as np
 
 from . import capi
-from .gpe import _as_dxn
+from .gpe import _as_dxn, _predict_f_grad
 from .kernels import Kernel, flatten
 from .likelihoods import Likelihood
 from .means import Mean, MeanZero
@@ -181,6 +181,11 @@ class GPA:
         if full_cov:
             return mu, cov
         return mu, np.maximum(var, 0.0)                                 # GP.jl:75
+
+    def predict_f_grad(self, x):
+        """predict_f(gp, x) and its gradients with respect to the test inputs: (mu, s2, dmu, ds2), as GPE.predict_f_grad, with
+        alpha = K^-1 L v."""
+        return _predict_f_grad(self._eng, self._xs(x), self._alpha(), self.mean)
 
     def predict_y(self, x):
         """predict_y(gp::GPA, x) (GPA.jl:303-306): predict_obs(lik, predict_f(gp, x)...) -- means and variances."""

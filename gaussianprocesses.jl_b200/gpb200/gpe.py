@@ -229,6 +229,15 @@ class GPE:
         mu = allgather_concat(mu, counts) + self.mean.mean(xs)
         return mu, np.maximum(allgather_concat(var, counts), 0.0)                # GP.jl:75
 
+    def predict_f_grad(self, x):
+        """predict_f(gp, x) with its gradients with respect to the test inputs, on the device: (mu, s2, dmu, ds2), dmu and ds2
+        of shape (dim, M) with column m = d mu_m / d x_m and d s2_m / d x_m -- what ForwardDiff gives through predict_f with
+        Dual inputs, including the clamp s2 = max(var, 0) (ds2 = 0 where it acts).  Single-GPU engines only."""
+        x = _as_dxn(x)
+        if x.shape[0] != self.dim:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        return _predict_f_grad(self._eng, np.ascontiguousarray(x.T), None, self.mean)
+
     def predict_y(self, x, full_cov=False):                        # GPE.jl:408-416
         mu, s2 = self.predict_f(x, full_cov=full_cov)
         nv = self.noise_variance()
@@ -400,6 +409,16 @@ class GPE:
         self.set_params(res.x, **flags)
         self.update_target()
         return res
+
+
+def _predict_f_grad(eng, xs, alpha, mean):
+    """shared by GPE and GPA: device predictions + gradients, the mean's share added on the host, GP.jl:75's clamp"""
+    mu, var, dmu, dvar = eng.predict_grad(xs, alpha, want_var=True)
+    mu = mu + mean.mean(xs)
+    dmu = dmu + mean.grad_x(xs)
+    neg = var < 0.0
+    dvar[neg] = 0.0
+    return mu, np.maximum(var, 0.0), np.ascontiguousarray(dmu.T), np.ascontiguousarray(dvar.T)
 
 
 def GP(x, y, mean, kernel, logNoise=-2.0, **kw):                   # GPE.jl:119

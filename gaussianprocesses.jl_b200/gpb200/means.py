@@ -19,6 +19,10 @@ class Mean:
     def grad_stack(self, X):
         raise NotImplementedError
 
+    def grad_x(self, X):
+        """d mean(x_i) / d x_i as an (N, d) array (the mean's part of the predictive-mean gradient)."""
+        raise NotImplementedError
+
 
 class MeanZero(Mean):                     # mZero.jl
     def mean(self, X):
@@ -26,6 +30,9 @@ class MeanZero(Mean):                     # mZero.jl
 
     def grad_stack(self, X):
         return np.zeros((X.shape[0], 0))
+
+    def grad_x(self, X):
+        return np.zeros(X.shape)
 
     def spec(self):
         return ("MeanZero",)
@@ -49,6 +56,9 @@ class MeanConst(Mean):                    # mConst.jl
     def grad_stack(self, X):
         return np.ones((X.shape[0], 1))
 
+    def grad_x(self, X):
+        return np.zeros(X.shape)
+
     def spec(self):
         return ("MeanConst", self.beta)
 
@@ -67,6 +77,9 @@ class MeanLin(Mean):                      # mLin.jl
 
     def mean(self, X):
         return X @ self.beta
+
+    def grad_x(self, X):
+        return np.broadcast_to(self.beta, X.shape).copy()
 
     def grad_stack(self, X):
         return np.array(X, dtype=np.float64)

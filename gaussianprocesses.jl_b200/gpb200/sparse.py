@@ -8,7 +8,7 @@ import math
 import numpy as np
 
 from . import capi
-from .gpe import GPE, _as_dxn
+from .gpe import GPE, _as_dxn, _predict_f_grad
 from .kernels import flatten
 from .means import MeanZero
 
@@ -108,6 +108,13 @@ class FITC:
         mu, var = self._eng.predict(xs)
         return mu + self.mean.mean(xs), np.maximum(var, 0.0)          # GP.jl:75
 
+    def predict_f_grad(self, x):
+        """predict_f(gp, x) and its gradients with respect to the test inputs, (mu, s2, dmu, ds2) as GPE.predict_f_grad"""
+        x = _as_dxn(x)
+        if x.shape[0] != self.dim:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        return _predict_f_grad(self._eng, np.ascontiguousarray(x.T), None, self.mean)
+
     def predict_y(self, x, full_cov=False):
         mu, s2 = self.predict_f(x, full_cov=full_cov)
         if full_cov:
@@ -200,6 +207,9 @@ class FSA(FITC):
         mu, s2 = self._eng.predict_fsa(xs, block_of, full_cov=full_cov)
         mu = mu + self.mean.mean(xs)
         return (mu, s2) if full_cov else (mu, np.maximum(s2, 0.0))
+
+    def predict_f_grad(self, x):
+        raise ValueError("predict_f_grad: not available for FSA (its predictions pair test points with training blocks)")
 
     def predict_y(self, x, blockindpred, full_cov=False):
         mu, s2 = self.predict_f(x, blockindpred, full_cov=full_cov)

@@ -25,6 +25,7 @@ using ElasticArrays: ElasticArray
 import PDMats: AbstractPDMat, dim
 import Base: \, size, Matrix
 import LinearAlgebra: logdet, tr
+import ForwardDiff                                      # a dependency of GaussianProcesses.jl (src/GaussianProcesses.jl:19)
 
 const LIB = get(ENV, "GPB200_LIB", "libgpb200.so")
 
@@ -326,6 +327,33 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=fa
     return mu .+ mean(gp.mean, Matrix{Float64}(x)), max.(s, 0.0)                   # src/GP.jl:75
 end
 
+# predict_f with ForwardDiff.Dual test inputs (acquisition-function gradients): the device computes mu, var and their
+# gradients with respect to each test point (d x M), and the outputs are rebuilt as Duals -- partials of mu_m are
+# sum_p dmu[p, m] * partials(x[p, m]).  The mean goes through the reference's own mean(gp.mean, x) on the Duals, and
+# max.(var, 0.0) acts on Duals as in src/GP.jl:75.  Nested Duals keep the Float64 conversion error; full_cov=true throws.
+const DualMatrix{T} = AbstractMatrix{<:ForwardDiff.Dual{T,Float64}}
+
+function dual_outputs(x::DualMatrix{T}, v::Vector{Float64}, g::Matrix{Float64}) where T
+    return [ForwardDiff.Dual{T}(v[m], sum(g[p, m] * ForwardDiff.partials(x[p, m]) for p in 1:size(x, 1))) for m in eachindex(v)]
+end
+
+function predict_grad_raw(cK::B200PDMat, x::DualMatrix, alpha::AbstractVector)
+    X = Matrix{Float64}(ForwardDiff.value.(x)); d, M = size(X)
+    mu = Vector{Float64}(undef, M); var = Vector{Float64}(undef, M)
+    dmu = Matrix{Float64}(undef, d, M); dvar = Matrix{Float64}(undef, d, M)
+    check(cK, ccall((:gpb200_predict_grad, LIB), Cint,
+                    (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                    cK.handle, M, X, d, Vector{Float64}(alpha), mu, var, dmu, dvar), "predict_grad")
+    return dual_outputs(x, mu, dmu), dual_outputs(x, var, dvar)
+end
+
+function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::DualMatrix; full_cov::Bool=false) where {X,Y,M,K,CS<:B200Covariance,D,P}
+    size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
+    full_cov && throw(ArgumentError("predict_f: full_cov=true is not supported with Dual inputs"))
+    mu, s = predict_grad_raw(gp.cK, x, gp.alpha)
+    return mu .+ mean(gp.mean, x), max.(s, 0.0)                                    # src/GP.jl:75
+end
+
 # predictMVN (src/GP.jl:39-49): mean + FULL predictive covariance through gpb200_predict(cov != NULL); this is what
 # predict_full / predict_f(full_cov=true) / rand(gp, X) reach.
 function predictMVN(xpred::AbstractMatrix, xtrain::AbstractMatrix, ytrain::AbstractVector, kernel::Kernel, meanf::Mean,
@@ -473,6 +501,19 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=fa
     checks(gp.cK, ccall((:gpb200_fitc_predict, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Float64}, Ptr{Float64}),
                         gp.cK.handle, Ms, Xs, size(Xs, 1), mu, var), "fitc_predict")
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
+end
+
+# Dual test inputs on FITC / DTC / SoR (see predict_grad_raw above); FSA keeps the Float64 conversion error
+function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::DualMatrix; full_cov::Bool=false) where {X,Y,M,K,CS<:B200Sparse,D,P}
+    size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
+    full_cov && throw(ArgumentError("predict_f: full_cov=true is not supported with Dual inputs"))
+    Xs = Matrix{Float64}(ForwardDiff.value.(x)); d, Ms = size(Xs)
+    mu = Vector{Float64}(undef, Ms); var = Vector{Float64}(undef, Ms)
+    dmu = Matrix{Float64}(undef, d, Ms); dvar = Matrix{Float64}(undef, d, Ms)
+    checks(gp.cK, ccall((:gpb200_fitc_predict_grad, LIB), Cint,
+                        (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                        gp.cK.handle, Ms, Xs, d, mu, var, dmu, dvar), "fitc_predict_grad")
+    return dual_outputs(x, mu, dmu) .+ mean(gp.mean, x), max.(dual_outputs(x, var, dvar), 0.0)
 end
 
 # predict_f(gp, x, blockindpred; full_cov) full_scale_approximation.jl:456-477: test block j is paired with training block j
@@ -740,6 +781,13 @@ function predict_f(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)
     μ, σ2 = predict_raw(gp.cK, x, alpha, full_cov)
     μ .+= mean(gp.mean, x)
     return full_cov ? (μ, σ2) : (μ, max.(σ2, 0.0))                                 # GP.jl:75
+end
+
+function predict_f(gp::B200GPA, x::DualMatrix; full_cov::Bool=false)           # Dual inputs: see predict_grad_raw
+    full_cov && throw(ArgumentError("predict_f: full_cov=true is not supported with Dual inputs"))
+    alpha = gp.cK \ unwhiten_dev(gp.cK, gp.v)
+    μ, σ2 = predict_grad_raw(gp.cK, x, alpha)
+    return μ .+ mean(gp.mean, x), max.(σ2, 0.0)
 end
 
 function predict_y(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)        # GPA.jl:303-306

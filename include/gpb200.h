@@ -123,6 +123,17 @@ int  gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kern
 int  gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs,
                     const double* alpha, double* mu_minus_mean, double* var, double* cov);
 
+/* Predictive gradients with respect to the test inputs (predict_f with ForwardDiff.Dual inputs): mu_minus_mean[M] and var[M]
+ * bitwise equal to gpb200_predict's on the same handle, and dmu / dvar (M x d point-major == Julia's d x M column-major)
+ *   dmu[m, p]  = sum_i dk(x*_m, x_i)/dx*_{m,p} alpha_i                     (the mean's own gradient is the caller's)
+ *   dvar[m, p] = 2 dk(x*_m, x*_m)/dx*_{m,p} - 2 sum_i dk(x*_m, x_i)/dx*_{m,p} (K^-1 k*_m)_i     (var NOT clamped)
+ * var and dvar are given together or both NULL (then only the cross-Gram and the contraction run, no solve).  Where x*_m
+ * coincides with a training input the stationary kernels contribute the limit of their derivative (0) rather than the NaN
+ * of differentiating through sqrt(0).  Single-GPU handles only (GPB200_EINVAL otherwise); chunked as gpb200_predict.
+ * Uses F's strict-upper tiles as scratch (they hold L' during the call).                                                 */
+int  gpb200_predict_grad(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, const double* alpha,
+                         double* mu_minus_mean, double* var, double* dmu, double* dvar);
+
 /* rand(gp, X, n) (src/GP.jl:120-146): n posterior draws at the M test points, on the device: predictMVN's full covariance,
  * make_posdef!(Sigma; nugget) (Cholesky of the M x M matrix), unwhiten!(Sigma, Z) and + mu.  z and samples are M x nsamp
  * column-major (Julia `randn(M, n)` / the returned matrix); mu_minus_mean[M] as in gpb200_predict (the shim adds mean(x*) to
@@ -179,6 +190,8 @@ int  gpb200_get_inverse_diag(gpb200_handle* h, double* diag);
 /* per-phase device times (ms) of the last calls:
  * [0] gram  [1] cholesky  [2] solve+mll  [3] inverse (trtri+lauum; gpb200_gpa_grad: the merges only)  [4] trace  [5] predict
  * [9] gpb200_gpa_grad's scans  [10] its S = W'Z GEMM
+ * gpb200_predict_grad (summed over chunks): [11] cross-Gram + mean  [12] V' = K*' L^-T + variance  [13] L' into F's upper
+ * tiles  [14] W' = V' L^-1  [15] gradient contraction
  * with option "profile"=1, accumulated since the option was set:
  * [6] number of DMMA GEMM launches  [7] sum of their device durations (ms, CUDA events around
  * every launch)  [8] FP64 flops those launches executed (tile-granular)                       */
@@ -320,6 +333,13 @@ int  gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise);
 int  gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel);
 /* mu_minus_mean[Ms], var[Ms] (may be NULL; not clamped) */
 int  gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean, double* var);
+/* Predictive gradients of FITC / DTC / SoR with respect to the test inputs, as gpb200_predict_grad (same layouts, var and
+ * dvar together or both NULL): mu_minus_mean and var bitwise equal to gpb200_fitc_predict's, and
+ *   dvar[m, p] = 2c dk(x*_m, x*_m)/dx*_{m,p} - 2 sum_j dk(x*_m, u_j)/dx*_{m,p} W'[m, j],  W' = K*u K_uu^-1 - K*u Sigma_QR^-1
+ * (c = 1; SoR: W' = -K*u Sigma_QR^-1, c = 0), dmu[m, p] = sum_j dk(x*_m, u_j)/dx*_{m,p} (Sigma_QR^-1 K_uf Lambda^-1 y)_j.
+ * GPB200_ESTATE before factorize + mll; GPB200_EINVAL for FSA (mode 3) and multi-rank handles ("single GPU").         */
+int  gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean,
+                              double* var, double* dmu, double* dvar);
 /* predictMVN with the full covariance cov[Ms x Ms] (fitc.jl:324-332, dtc.jl:41-59, sor.jl:302-321); Ms <= 32768 */
 int  gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean, double* cov);
 /* 0 = FITC (default), 1 = DTC (src/sparse/determ_train_conditional.jl), 2 = SoR
