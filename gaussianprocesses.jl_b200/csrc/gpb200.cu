@@ -2415,6 +2415,181 @@ int gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int3
     return GPB200_OK;
 }
 
+// A local copy of the handle's kernel program at log-scale theta (the handle's own theta and factor stay as they are).
+// The program must exist, theta must have n_theta entries and every input dimension the program reads must be < d.
+static int local_prog(gpb200_handle* h, const char* what, const double* theta, int32_t ntheta, int64_t d, KProg& P) {
+    if (!h->has_kernel) return fail(h, GPB200_ESTATE, (std::string(what) + ": set_kernel first").c_str());
+    if (ntheta != h->prog.n_theta || (ntheta > 0 && !theta)) return fail(h, GPB200_EINVAL, (std::string(what) + ": theta has n_theta entries").c_str());
+    if (d < 1) return fail(h, GPB200_EINVAL, (std::string(what) + ": d >= 1").c_str());
+    P = h->prog;
+    for (int q = 0; q < P.n_ops; ++q)
+        if (P.op[q] != GPB200_OP_SUM && P.op[q] != GPB200_OP_PROD)
+            for (int k = 0; k < P.nd[q]; ++k)
+                if (P.dims[P.doff[q] + k] >= d) return fail(h, GPB200_EINVAL, (std::string(what) + ": the program reads a dimension >= d").c_str());
+    kprog_set_theta(P, theta);
+    return GPB200_OK;
+}
+
+// Copies a host item list to a new device array (the caller frees it after the synchronize); none for an empty list.
+static cudaError_t items_to_device(const void* src, size_t bytes, void** d, cudaStream_t st) {
+    *d = nullptr;
+    if (!bytes) return cudaSuccess;
+    cudaError_t e = cudaMalloc(d, bytes);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(*d, src, bytes, cudaMemcpyHostToDevice, st);
+    return e;
+}
+
+int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
+    if (!h || (n > 0 && !args) || which < 0 || which > 10 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    // fixed arguments before the flattened items, and the item stride (0: no items)
+    static const int head[11] = {3, 9, 6, 5, 5, 1, 5, 6, 4, 0, 5};
+    static const int stride[11] = {5, 0, 0, 0, 0, 5, 5, 0, 5, 6, 0};
+    const int hd = head[which], sd = stride[which];
+    if (sd ? (n < hd || (n - hd) % sd) : n != hd) return fail(h, GPB200_EINVAL, "fsa_kernels: wrong argument count for this kernel");
+    const int ni = sd ? (n - hd) / sd : 0;
+    auto ptr = [&](int i) { return reinterpret_cast<double*>(args[i]); };
+    std::vector<FsaGramItem> gitems(sd == 5 ? ni : 0);
+    std::vector<FsaRowItem> ritems(sd == 6 ? ni : 0);
+    for (int k = 0; k < ni; ++k) {
+        const int64_t* q = args + hd + sd * k;
+        if (sd == 5) {                                   // dst, ld, row_i, row_j, diag
+            if (!q[0] || q[1] < TILE || q[2] < 0 || q[3] < 0)
+                return fail(h, GPB200_EINVAL, "fsa_kernels: item with a null dst, ld < 128 or a negative row");
+            gitems[k] = FsaGramItem{reinterpret_cast<double*>(q[0]), q[1], q[2], q[3], (int)(q[4] != 0), 0};
+        } else {                                         // A, v, out, lda, K, sq
+            if (!q[0] || !q[2] || (!q[5] && !q[1]) || q[4] < 0 || q[4] > INT_MAX || q[3] < q[4])
+                return fail(h, GPB200_EINVAL, "fsa_kernels: row item with a null pointer, K < 0 or lda < K");
+            ritems[k] = FsaRowItem{reinterpret_cast<const double*>(q[0]), reinterpret_cast<const double*>(q[1]),
+                                   reinterpret_cast<double*>(q[2]), q[3], (int)q[4], (int)(q[5] != 0)};
+        }
+    }
+    auto need = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (!args[i]) return false;
+        return true;
+    };
+    KProg P{};
+    const bool prog = which == 0 || which == 6 || which == 8;
+    if (prog) {
+        const int64_t d = args[which == 8 ? 2 : 1];
+        const int32_t want = h->prog.n_theta + (which == 0 ? 1 : 0);
+        if (h->has_kernel && nf != want) return fail(h, GPB200_EINVAL, "fsa_kernels: fargs = theta (+ diag_add for fsa_gram)");
+        TRY(local_prog(h, "fsa_kernels", fargs, h->prog.n_theta, d, P));
+    } else if (nf != (which == 7 ? 1 : 0)) {
+        return fail(h, GPB200_EINVAL, "fsa_kernels: fargs = alpha for fsa_axpy_t, none otherwise");
+    }
+    bool ok = true;
+    switch (which) {
+    case 0: ok = need({0, 2}); break;                                        // xb, d, mask | items
+    case 1: ok = need({1, 2, 3, 4, 5, 7}) && (args[0] == 2 || args[6]) && args[0] >= 0 && args[0] <= 2 && args[8] >= 0; break;
+    case 2: ok = need({0}) && args[1] >= args[3] && args[2] >= 0 && args[3] >= 0; break;     // A, ld, nrows, ncols, rowmask, colmask
+    case 3: ok = need({1, 2, 4}) && (args[0] == 0 || args[0] == 1) && args[3] >= 0; break;   // scatter, src, pos, n, dst
+    case 4: ok = need({0, 1, 2, 3}) && args[4] >= 0; break;                  // out, a, b, mask, n
+    case 5: ok = need({0}); break;                                           // a | items
+    case 6: ok = need({0, 2, 4}) && (ni == 0 || args[3]); break;             // xb, d, mask, part, out | items
+    case 7: ok = need({0, 2}) && args[4] >= 0 && args[5] >= 0 && args[1] >= args[5] && args[3] >= args[4]; break;  // C, ldc, A, lda, nrows, ncols
+    case 8: ok = need({0, 1, 3}); break;                                     // xs, xb, d, mask | items
+    case 9: break;                                                           // items only
+    case 10: ok = need({0, 1, 2, 3}) && args[4] >= 0; break;                 // out, q, g2, r2neg, n
+    }
+    if (!ok) return fail(h, GPB200_EINVAL, "fsa_kernels: a null pointer, a negative size, a bad mode or ld below the row width");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = h->st;
+    int64_t* L = &h->launches;
+    FsaGramItem* dg = nullptr;
+    FsaRowItem* dr = nullptr;
+    cudaError_t e = sd == 6 ? items_to_device(ritems.data(), sizeof(FsaRowItem) * ritems.size(), reinterpret_cast<void**>(&dr), st)
+                            : items_to_device(gitems.data(), sizeof(FsaGramItem) * gitems.size(), reinterpret_cast<void**>(&dg), st);
+    if (e == cudaSuccess) {
+        switch (which) {
+        case 0: e = fsa_gram_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), fargs[nf - 1], st, L); break;
+        case 1: e = fsa_bdmv_launch((int)args[0], ptr(1), reinterpret_cast<const int*>(args[2]), reinterpret_cast<const long long*>(args[3]),
+                                    reinterpret_cast<const int*>(args[4]), reinterpret_cast<const long long*>(args[5]), ptr(6), ptr(7),
+                                    args[8], st, L); break;
+        case 2: e = fsa_mask_launch(ptr(0), args[1], args[2], args[3], ptr(4), ptr(5), st, L); break;
+        case 3: e = fsa_permute_launch((int)args[0], ptr(1), reinterpret_cast<const long long*>(args[2]), args[3], ptr(4), st, L); break;
+        case 4: e = fsa_resid_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
+        case 5: e = fsa_outer_launch(dg, ni, ptr(0), st, L); break;
+        case 6: e = fsa_trace_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), ptr(3), ptr(4), st, L); break;
+        case 7: e = fsa_axpy_t_launch(ptr(0), args[1], ptr(2), args[3], args[4], args[5], fargs[0], st, L); break;
+        case 8: e = fsa_crossgram_launch(P, ptr(0), ptr(1), (int)args[2], dg, ni, ptr(3), st, L); break;
+        case 9: e = fsa_rowdot_launch(dr, ni, st, L); break;
+        case 10: e = fsa_var_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
+        }
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (dg) cudaFree(dg);
+    if (dr) cudaFree(dr);
+    CK(e);
+    return GPB200_OK;
+}
+
+int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
+    if (!h || !args || which < 0 || which > 13 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    static const int want[14] = {14, 14, 4, 8, 5, 5, 10, 6, 5, 6, 5, 9, 7, 3};
+    if (n != want[which]) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: wrong argument count for this kernel");
+    const int64_t* a = args;
+    auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
+    auto need = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (!a[i]) return false;
+        return true;
+    };
+    KProg P{};
+    if (which == 0) {
+        // kind, x, ldx, d, j, G, C, ld, ncols, nrows, rows_pad, alpha, delta, da
+        TRY(local_prog(h, "fitc_cv_kernels", fargs, nf, a[3], P));
+    } else if (nf != 0) {
+        return fail(h, GPB200_EINVAL, "fitc_cv_kernels: fargs = theta for delta, none otherwise");
+    }
+    bool ok = true;
+    switch (which) {
+    case 0: ok = a[0] >= 0 && a[0] <= 2 && a[9] >= 0 && a[10] >= 0 && need({11, 12, 13}) &&
+                 (a[0] != 0 || (need({1, 5, 6}) && a[2] >= a[3] && a[4] >= 0 && a[4] < P.n_theta && a[8] >= 0 && a[7] >= a[8]));
+            break;
+    // G, Ch, K, P, ld, nrows, ncols, lam, delta, alpha, beta, w, zja, dg   (G = 0: beta unread)
+    case 1: ok = need({1, 2, 3, 7, 8, 9, 11, 12, 13}) && (!a[0] || a[10]) && a[5] >= 0 && a[6] >= 0 && a[4] >= a[6]; break;
+    case 2: ok = need({1, 2, 3}) && a[0] >= 0; break;                                  // n, lam, q, out
+    case 3: ok = need({0, 2, 6, 7}) && a[4] >= 0 && a[5] >= 0 && a[3] >= a[5]; break;   // E, G, K, ld, nrows, ncols, lam, delta
+    case 4: ok = need({0, 1, 2}) && a[4] >= 0 && a[3] >= a[4]; break;                  // Q, H, R, ld, n
+    case 5: ok = need({1, 2, 3, 4}) && a[0] >= 0; break;                               // n, w, a, b, c
+    // nv, idx, x, ldx, d, xout, lam, lamout, delta, delout   (delta = 0: delout unwritten)
+    case 6: ok = need({1, 2, 5, 6, 7}) && (!a[8] || a[9]) && a[0] >= 0 && a[4] >= 0 && a[4] <= INT_MAX && a[3] >= a[4]; break;
+    case 7: ok = need({0, 4}) && (a[3] == 0 || (a[3] == 1 && a[5])) && a[2] >= 0 && a[1] >= a[2]; break;   // out, ld, nv, which, lam, delta
+    case 8: ok = need({0, 4}) && a[2] >= 0 && a[3] >= 0 && a[1] >= a[3]; break;       // colscale: A, ld, nrows, ncols, v
+    case 9: ok = need({1, 5}) && (a[0] == 0 || a[0] == 1) && a[3] >= 0 && a[4] >= 0 && a[2] >= a[4]; break;   // scale: mode, A, ld, nrows, ncols, v
+    case 10: ok = need({1, 2, 3, 4}) && a[0] >= 0; break;                             // fitc_g: n, alpha, lam, q, g
+    case 11: ok = need({0, 1, 5, 6, 7, 8}) && a[3] >= 0 && a[4] >= 0 && a[2] >= a[4]; break;   // fitc_wfu: P2, P1, ld, nrows, ncols, alpha, lam, g, beta
+    case 12: ok = need({0, 1, 2, 3, 6}) && a[5] >= 0 && a[4] >= a[5]; break;          // fitc_wuu: Wuu, T, Kinv, Sinv, ld, n, beta
+    case 13: ok = need({0}) && a[2] >= 0 && a[1] >= a[2]; break;                       // symmetrize: A, ld, n
+    }
+    if (!ok) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: a null pointer, a negative size, a bad mode or ld below the row width");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = h->st;
+    int64_t* L = &h->launches;
+    cudaError_t e = cudaSuccess;
+    switch (which) {
+    case 0: e = fitc_cv_delta_launch((int)a[0], P, ptr(1), a[2], (int)a[4], ptr(5), ptr(6), a[7], a[8], a[9], a[10], ptr(11), ptr(12),
+                                     ptr(13), st, L); break;
+    case 1: e = fitc_cv_rows_launch(ptr(0), ptr(1), ptr(2), ptr(3), a[4], a[5], a[6], ptr(7), ptr(8), ptr(9), ptr(10), ptr(11), ptr(12),
+                                    ptr(13), st, L); break;
+    case 2: e = fitc_cv_invdiag_launch(a[0], ptr(1), ptr(2), ptr(3), st, L); break;
+    case 3: e = fitc_cv_eblock_launch(ptr(0), ptr(1), ptr(2), a[3], a[4], a[5], ptr(6), ptr(7), st, L); break;
+    case 4: e = fitc_cv_qs_launch(ptr(0), ptr(1), ptr(2), a[3], a[4], st, L); break;
+    case 5: e = fitc_cv_wvec_launch(a[0], ptr(1), ptr(2), ptr(3), ptr(4), st, L); break;
+    case 6: e = fitc_cv_gather_launch(a[0], reinterpret_cast<const long long*>(a[1]), ptr(2), a[3], (int)a[4], ptr(5), ptr(6), ptr(7),
+                                      ptr(8), ptr(9), st, L); break;
+    case 7: e = fitc_cv_diag_launch(ptr(0), a[1], a[2], (int)a[3], ptr(4), ptr(5), st, L); break;
+    case 8: e = colscale_launch(ptr(0), a[1], a[2], a[3], ptr(4), st, L); break;
+    case 9: e = scale_launch((int)a[0], ptr(1), a[2], a[3], a[4], ptr(5), st, L); break;
+    case 10: e = fitc_g_launch(a[0], ptr(1), ptr(2), ptr(3), ptr(4), st, L); break;
+    case 11: e = fitc_wfu_launch(ptr(0), ptr(1), a[2], a[3], a[4], ptr(5), ptr(6), ptr(7), ptr(8), st, L); break;
+    case 12: e = fitc_wuu_launch(ptr(0), ptr(1), ptr(2), ptr(3), a[4], a[5], ptr(6), st, L); break;
+    case 13: e = symmetrize_launch(ptr(0), a[1], a[2], st, L); break;
+    }
+    CK(e);
+    CK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+
 int gpb200_fp64_peak(gpb200_handle* h, double* tflops_dmma, double* tflops_dfma) {
     if (!h) return GPB200_EINVAL;
     CK(cudaSetDevice(h->device));

@@ -269,24 +269,28 @@ cudaError_t rowdot2_launch(const double* A, const double* B, int64_t ld, int64_t
     return cudaGetLastError();
 }
 cudaError_t fitc_g_launch(int64_t n, const double* alpha, const double* lam, const double* q, double* g, cudaStream_t st, int64_t* launches) {
+    if (n <= 0) return cudaSuccess;
     fitc_g_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, alpha, lam, q, g);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t fitc_wfu_launch(double* P2, const double* P1, int64_t ld, int64_t nrows, int64_t ncols, const double* alpha,
                             const double* lam, const double* g, const double* beta, cudaStream_t st, int64_t* launches) {
+    if (nrows <= 0 || ncols <= 0) return cudaSuccess;
     dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
     fitc_wfu_kernel<<<grid, 256, 0, st>>>(P2, P1, ld, nrows, ncols, alpha, lam, g, beta);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t colscale_launch(double* A, int64_t ld, int64_t nrows, int64_t ncols, const double* v, cudaStream_t st, int64_t* launches) {
+    if (nrows <= 0 || ncols <= 0) return cudaSuccess;
     dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
     colscale_kernel<<<grid, 256, 0, st>>>(A, ld, nrows, ncols, v);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 cudaError_t symmetrize_launch(double* A, int64_t ld, int64_t n, cudaStream_t st, int64_t* launches) {
+    if (n <= 0) return cudaSuccess;
     dim3 grid((unsigned)((n + 255) / 256), (unsigned)n);
     symmetrize_kernel<<<grid, 256, 0, st>>>(A, ld, n);
     if (launches) ++*launches;
@@ -294,6 +298,7 @@ cudaError_t symmetrize_launch(double* A, int64_t ld, int64_t n, cudaStream_t st,
 }
 cudaError_t fitc_wuu_launch(double* Wuu, const double* T, const double* Kinv, const double* Sinv, int64_t ld, int64_t n,
                             const double* beta, cudaStream_t st, int64_t* launches) {
+    if (n <= 0) return cudaSuccess;
     dim3 grid((unsigned)((n + 255) / 256), (unsigned)n);
     fitc_wuu_kernel<<<grid, 256, 0, st>>>(Wuu, T, Kinv, Sinv, ld, n, beta);
     if (launches) ++*launches;

@@ -63,6 +63,8 @@ _SIGNATURES = {
     "gpb200_trsv_tiles": (C.c_int, [_H, C.c_int, C.c_int, _lp, C.c_int32, _ip]),
     "gpb200_gpa_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
     "gpb200_row_reductions": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
+    "gpb200_fsa_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
+    "gpb200_fitc_cv_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "gpb200_ipc_export": (C.c_int, [_H, C.c_void_p]),
     "gpb200_ipc_import": (C.c_int, [_H, C.c_int, C.c_void_p]),
@@ -445,6 +447,25 @@ class Engine:
         """Fixed-order reduction (0 dot, 1 sum, 2 rowdot, 3 rowvar, 4 rowdot2) on the device buffers of include/gpb200.h."""
         a = np.ascontiguousarray(args, dtype=np.int64).ravel()
         self._check(self._lib.gpb200_row_reductions(self._h, int(which), a.ctypes.data_as(_lp), a.size), "row_reductions")
+
+    FSA_KERNELS = ("gram", "bdmv", "mask", "permute", "resid", "outer", "trace", "axpy_t", "crossgram", "rowdot", "var")
+    FITC_CV_KERNELS = ("delta", "rows", "invdiag", "eblock", "qs", "wvec", "gather", "diag", "colscale", "scale", "fitc_g",
+                       "fitc_wfu", "fitc_wuu", "symmetrize")
+
+    def fsa_kernels(self, name, args, fargs=()):
+        """One FSA block-diagonal kernel (include/gpb200.h) by name, on device buffers: args = the int64 arguments followed
+        by the flattened items, fargs = theta (and diag_add) or alpha."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
+        self._check(self._lib.gpb200_fsa_kernels(self._h, self.FSA_KERNELS.index(name), a.ctypes.data_as(_lp), a.size,
+                                                 _as_dp(f), f.size), "fsa_kernels")
+
+    def fitc_cv_kernels(self, name, args, fargs=()):
+        """One sparse cross-validation row kernel or FITC element kernel (include/gpb200.h) by name, on device buffers."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
+        self._check(self._lib.gpb200_fitc_cv_kernels(self._h, self.FITC_CV_KERNELS.index(name), a.ctypes.data_as(_lp),
+                                                     a.size, _as_dp(f), f.size), "fitc_cv_kernels")
 
 
 class FitcEngine:

@@ -275,6 +275,46 @@ int  gpb200_gpa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
  *   which 4 rowdot2 (n = 6): A, B, ld, M, N, q
  * GPB200_EINVAL, nothing launched: bad which / n, a negative length, ld < N, a null pointer.                           */
 int  gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int32_t n);
+/* The FSA block-diagonal kernels (csrc/fsa.cuh) on caller buffers, synchronous, each through its launch wrapper (one
+ * launch, two for fsa_trace; sizes <= 0 launch nothing, as the wrappers do).  Item lists follow the fixed arguments,
+ * flattened: FsaGramItem = (dst, ld, row_i, row_j, diag), FsaRowItem = (A, v, out, lda, K, sq).  The kernels that
+ * evaluate the kernel program use the program of the last gpb200_set_kernel at fargs = log-scale theta (n_theta
+ * entries); the handle's own theta and factor are left alone.
+ *   which 0  fsa_gram      : xb, d, mask | Gram items        fargs = theta, diag_add
+ *   which 1  fsa_bdmv      : mode, packed, rblk (int32), bstart, bsize (int32), boff, v (mode 2: unused), y, Np
+ *   which 2  fsa_mask      : A, ld, nrows, ncols, rowmask, colmask (either may be 0)
+ *   which 3  fsa_permute   : scatter, src, pos, n, dst
+ *   which 4  fsa_resid     : out, a, b, mask, n
+ *   which 5  fsa_outer     : a | Gram items
+ *   which 6  fsa_trace     : xb, d, mask, part (items x n_theta), out | Gram items      fargs = theta
+ *                            (no items: out[0 .. n_theta) is zeroed and nothing is launched)
+ *   which 7  fsa_axpy_t    : C, ldc, A, lda, nrows, ncols                             fargs = alpha
+ *   which 8  fsa_crossgram : xs, xb, d, mask | Gram items                             fargs = theta
+ *   which 9  fsa_rowdot    : | row items (v unused when sq != 0)
+ *   which 10 fsa_var       : out, q, g2, r2neg, n
+ * GPB200_EINVAL, nothing launched: bad which / n / nf, theta not of n_theta entries, a program dimension >= d, a null
+ * pointer the kernel dereferences, a negative size or row, a bad mode, an item ld < 128, lda < K, ld < ncols.
+ * GPB200_ESTATE: a kernel-program call before gpb200_set_kernel.                                                    */
+int  gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
+/* The sparse cross-validation row kernels (csrc/fitc_cv.cuh) and the FITC element kernels that run between the same
+ * GEMMs (csrc/vec.cuh), synchronous, one launch each through its wrapper (sizes <= 0 launch nothing):
+ *   which 0  delta      : kind, x, ldx, d, j, G, C, ld, ncols, nrows, rows_pad, alpha, delta, da   fargs = theta
+ *                         (the program of the last gpb200_set_kernel; x, G, C and j are read for kind 0 only)
+ *   which 1  rows       : G (0 = none), Ch, K, P, ld, nrows, ncols, lam, delta, alpha, beta, w, zja, dg
+ *   which 2  invdiag    : n, lam, q, out
+ *   which 3  eblock     : E, G (0 = none), K, ld, nrows, ncols, lam, delta
+ *   which 4  qs         : Q, H, R, ld, n
+ *   which 5  wvec       : n, w, a, b, c
+ *   which 6  gather     : nv, idx, x, ldx, d, xout, lam, lamout, delta (0 = none), delout
+ *   which 7  diag       : out, ld, nv, which (0: 1/lam, 1: delta/lam^2), lam, delta
+ *   which 8  colscale   : A, ld, nrows, ncols, v
+ *   which 9  scale      : mode, A, ld, nrows, ncols, v
+ *   which 10 fitc_g     : n, alpha, lam, q, g
+ *   which 11 fitc_wfu   : P2, P1, ld, nrows, ncols, alpha, lam, g, beta
+ *   which 12 fitc_wuu   : Wuu, T, Kinv, Sinv, ld, n, beta
+ *   which 13 symmetrize : A, ld, n
+ * GPB200_EINVAL, nothing launched: as gpb200_fsa_kernels, plus j outside [0, n_theta) and ldx < d.                   */
+int  gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
 
 /* ---- multi-GPU (one process per GPU; NCCL over NVLink) -------------------------------------- */
 /* rank 0 obtains a 128-byte NCCL unique id, the host side broadcasts it (torch.distributed /
