@@ -240,6 +240,51 @@ __global__ void fsa_var_kernel(double* out, const double* q, const double* g2, c
     if (i < n) out[i] = q[i] - g2[i] - r2neg[i];
 }
 
+// Thread t takes the inducing points j = t, t + DX_NT, ..., then the block rows i = t, t + DX_NT, ..., in order; the d-vector
+// accumulators are indexed by the leaves' input dimensions at run time and live in local memory (as crossgram_dx_kernel's).
+constexpr int DX_NT = 128;
+__global__ void __launch_bounds__(DX_NT) fsa_crossgram_dx_kernel(
+        const __grid_constant__ KProg P, const double* __restrict__ xs, const double* __restrict__ z,
+        const double* __restrict__ xb, int d, long long M, const double* __restrict__ u, const double* __restrict__ Wb,
+        const double* __restrict__ S1, const double* __restrict__ S2, long long ldw, const double* __restrict__ mask,
+        const double* __restrict__ alpha, const double* __restrict__ E, long long lde, const FsaDxItem* __restrict__ items,
+        double* __restrict__ dmu, double* __restrict__ dvar) {
+    __shared__ double sx[GPB200_MAX_DIMS];
+    __shared__ double red[DX_NT];
+    const FsaDxItem it = items[blockIdx.x];
+    const int t = threadIdx.x;
+    for (int k = t; k < d; k += DX_NT) sx[k] = xs[it.row * d + k];
+    __syncthreads();
+    double gm[GPB200_MAX_DIMS], gv[GPB200_MAX_DIMS];
+    for (int k = 0; k < d; ++k) { gm[k] = 0.0; gv[k] = 0.0; }
+    const bool V = dvar != nullptr;
+    // dk(x*, x*)/dx* = 2 dk(x*, x')/dx* at x' = x*, into thread 0's variance sum only
+    if (V && t == 0) kprog_eval_dx(P, sx, sx, 2.0, gv, 0.0, nullptr);
+    const double* w = Wb ? Wb + it.row * ldw : nullptr;
+    const double* s1 = V ? S1 + it.row * ldw : nullptr;
+    const double* s2 = V ? S2 + it.row * ldw : nullptr;
+    for (long long j = t; j < M; j += DX_NT)
+        kprog_eval_dx(P, sx, z + j * d, u[j] - (w ? w[j] : 0.0), gm, V ? 2.0 * (s1[j] - s2[j]) : 0.0, V ? gv : nullptr);
+    const double* e = V ? E + it.row * lde : nullptr;
+    for (long long i = t; i < it.nb; i += DX_NT) {
+        const long long gi = it.b0 + i;
+        if (mask[gi] == 0.0) continue;
+        kprog_eval_dx(P, sx, xb + gi * d, alpha[gi], gm, V ? e[i] : 0.0, V ? gv : nullptr);
+    }
+    for (int k = 0; k < d; ++k) {
+        for (int which = 0; which < (V ? 2 : 1); ++which) {
+            red[t] = which ? gv[k] : gm[k];
+            __syncthreads();
+            for (int s = DX_NT / 2; s > 0; s >>= 1) {
+                if (t < s) red[t] += red[t + s];
+                __syncthreads();
+            }
+            if (t == 0) (which ? dvar : dmu)[it.out * d + k] = red[0];
+            __syncthreads();
+        }
+    }
+}
+
 bool g_gemm_attr = false;
 
 }  // namespace
@@ -341,6 +386,16 @@ cudaError_t fsa_rowdot_launch(const FsaRowItem* items, int n, cudaStream_t st, i
 cudaError_t fsa_var_launch(double* out, const double* q, const double* g2, const double* r2neg, long long n, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_var_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out, q, g2, r2neg, n);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t fsa_crossgram_dx_launch(const KProg& P, const double* xs, const double* z, const double* xb, int d, long long M,
+                                    const double* u, const double* Wb, const double* S1, const double* S2, long long ldw,
+                                    const double* mask, const double* alpha, const double* E, long long lde,
+                                    const FsaDxItem* items, int n, double* dmu, double* dvar, cudaStream_t st, int64_t* launches) {
+    if (n <= 0) return cudaSuccess;
+    fsa_crossgram_dx_kernel<<<n, DX_NT, 0, st>>>(P, xs, z, xb, d, M, u, Wb, S1, S2, ldw, mask, alpha, E, lde, items, dmu, dvar);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

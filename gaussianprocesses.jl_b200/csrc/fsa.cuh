@@ -74,3 +74,19 @@ struct FsaRowItem {
 cudaError_t fsa_rowdot_launch(const FsaRowItem* items, int n, cudaStream_t st, int64_t* launches);
 // out[i] = q[i] - g2[i] - r2neg[i]: k** - |V*|^2 - |G|^2 + |R|^2 from q = k** - |V*|^2 and r2neg = -|R|^2
 cudaError_t fsa_var_launch(double* out, const double* q, const double* g2, const double* r2neg, long long n, cudaStream_t st, int64_t* launches);
+// Predictive gradients of block-paired predictions, one CTA per item (one real test point):
+//   dmu[out, :]  = sum_{j < M} dk(x*, z_j)/dx* (u_j - Wb[row, j]) + sum_i dk(x*, xb_i)/dx* alpha_i
+//   dvar[out, :] = dk(x*, x*)/dx* + sum_{j < M} dk(x*, z_j)/dx* 2 (S1[row, j] - S2[row, j]) + sum_i dk(x*, xb_i)/dx* E[row, i - b0]
+// with x* = xs[row], i over the real rows (mask != 0) of the paired block [b0, b0 + nb) of the padded training inputs xb.
+// Wb may be null (0); dvar null: dmu only (S1, S2, E unread).  xs, z and xb have leading dimension d, the coefficient rows
+// ldw, E lde.  Every coordinate is summed by one fixed tree, so a row's result does not depend on the launch it is in.
+struct FsaDxItem {
+    long long row;          // row of xs and of the coefficient rows Wb / S1 / S2 / E
+    long long out;          // row of dmu / dvar
+    long long b0;           // first padded training row of the paired block
+    long long nb;           // padded rows of the paired block (0: unpaired)
+};
+cudaError_t fsa_crossgram_dx_launch(const KProg& P, const double* xs, const double* z, const double* xb, int d, long long M,
+                                    const double* u, const double* Wb, const double* S1, const double* S2, long long ldw,
+                                    const double* mask, const double* alpha, const double* E, long long lde,
+                                    const FsaDxItem* items, int n, double* dmu, double* dvar, cudaStream_t st, int64_t* launches);

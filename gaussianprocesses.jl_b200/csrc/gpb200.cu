@@ -202,6 +202,8 @@ struct gpb200_fitc {
     // posterior sampling (gpb200_fitc_rand): the Ms x Ms sub-engine and the staging of the draws are eu's (rand_from_cov)
     bool cov_keep_device = false;                     // predict_fsa: leave Sigma* in caller order on the device (fsa->Sc)
     double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
+    double fsag_ms[4] = {0, 0, 0, 0};                 // last predict_fsa_grad, summed over test chunks: predict_fsa's
+                                                      // launches, s + second sweep, K_uu^-1 TRSMs, contraction
     // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
     // buffer the likelihood, gradient and prediction schedules keep):
     //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
@@ -2440,19 +2442,26 @@ static cudaError_t items_to_device(const void* src, size_t bytes, void** d, cuda
 }
 
 int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
-    if (!h || (n > 0 && !args) || which < 0 || which > 10 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    if (!h || (n > 0 && !args) || which < 0 || which > 11 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
     // fixed arguments before the flattened items, and the item stride (0: no items)
-    static const int head[11] = {3, 9, 6, 5, 5, 1, 5, 6, 4, 0, 5};
-    static const int stride[11] = {5, 0, 0, 0, 0, 5, 5, 0, 5, 6, 0};
+    static const int head[12] = {3, 9, 6, 5, 5, 1, 5, 6, 4, 0, 5, 16};
+    static const int stride[12] = {5, 0, 0, 0, 0, 5, 5, 0, 5, 6, 0, 4};
     const int hd = head[which], sd = stride[which];
     if (sd ? (n < hd || (n - hd) % sd) : n != hd) return fail(h, GPB200_EINVAL, "fsa_kernels: wrong argument count for this kernel");
     const int ni = sd ? (n - hd) / sd : 0;
     auto ptr = [&](int i) { return reinterpret_cast<double*>(args[i]); };
     std::vector<FsaGramItem> gitems(sd == 5 ? ni : 0);
     std::vector<FsaRowItem> ritems(sd == 6 ? ni : 0);
+    std::vector<FsaDxItem> ditems(sd == 4 ? ni : 0);
+    int64_t max_nb = 0;
     for (int k = 0; k < ni; ++k) {
         const int64_t* q = args + hd + sd * k;
-        if (sd == 5) {                                   // dst, ld, row_i, row_j, diag
+        if (sd == 4) {                                   // row, out, b0, nb
+            if (q[0] < 0 || q[1] < 0 || q[2] < 0 || q[3] < 0)
+                return fail(h, GPB200_EINVAL, "fsa_kernels: crossgram_dx item with a negative row, out, b0 or nb");
+            ditems[k] = FsaDxItem{q[0], q[1], q[2], q[3]};
+            max_nb = std::max(max_nb, q[3]);
+        } else if (sd == 5) {                            // dst, ld, row_i, row_j, diag
             if (!q[0] || q[1] < TILE || q[2] < 0 || q[3] < 0)
                 return fail(h, GPB200_EINVAL, "fsa_kernels: item with a null dst, ld < 128 or a negative row");
             gitems[k] = FsaGramItem{reinterpret_cast<double*>(q[0]), q[1], q[2], q[3], (int)(q[4] != 0), 0};
@@ -2468,9 +2477,10 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
         return true;
     };
     KProg P{};
-    const bool prog = which == 0 || which == 6 || which == 8;
+    const bool prog = which == 0 || which == 6 || which == 8 || which == 11;
     if (prog) {
-        const int64_t d = args[which == 8 ? 2 : 1];
+        const int64_t d = args[which == 8 ? 2 : which == 11 ? 3 : 1];
+        if (which == 11 && d > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "fsa_kernels: d above GPB200_MAX_DIMS");
         const int32_t want = h->prog.n_theta + (which == 0 ? 1 : 0);
         if (h->has_kernel && nf != want) return fail(h, GPB200_EINVAL, "fsa_kernels: fargs = theta (+ diag_add for fsa_gram)");
         TRY(local_prog(h, "fsa_kernels", fargs, h->prog.n_theta, d, P));
@@ -2490,6 +2500,11 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
     case 8: ok = need({0, 1, 3}); break;                                     // xs, xb, d, mask | items
     case 9: break;                                                           // items only
     case 10: ok = need({0, 1, 2, 3}) && args[4] >= 0; break;                 // out, q, g2, r2neg, n
+    case 11:    // xs, z, xb, d, M, u, Wb, S1, S2, ldw, mask, alpha, E, lde, dmu, dvar | items
+        ok = need({0, 14}) && args[4] >= 0 && (args[4] == 0 || (args[1] && args[5])) && (max_nb == 0 || need({2, 10, 11})) &&
+             (!args[6] || args[9] >= args[4]) &&
+             (!args[15] || (need({7, 8}) && args[9] >= args[4] && (max_nb == 0 || (args[12] && args[13] >= max_nb))));
+        break;
     }
     if (!ok) return fail(h, GPB200_EINVAL, "fsa_kernels: a null pointer, a negative size, a bad mode or ld below the row width");
     CK(cudaSetDevice(h->device));
@@ -2497,8 +2512,10 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
     int64_t* L = &h->launches;
     FsaGramItem* dg = nullptr;
     FsaRowItem* dr = nullptr;
-    cudaError_t e = sd == 6 ? items_to_device(ritems.data(), sizeof(FsaRowItem) * ritems.size(), reinterpret_cast<void**>(&dr), st)
-                            : items_to_device(gitems.data(), sizeof(FsaGramItem) * gitems.size(), reinterpret_cast<void**>(&dg), st);
+    FsaDxItem* dd = nullptr;
+    cudaError_t e = sd == 6   ? items_to_device(ritems.data(), sizeof(FsaRowItem) * ritems.size(), reinterpret_cast<void**>(&dr), st)
+                    : sd == 4 ? items_to_device(ditems.data(), sizeof(FsaDxItem) * ditems.size(), reinterpret_cast<void**>(&dd), st)
+                              : items_to_device(gitems.data(), sizeof(FsaGramItem) * gitems.size(), reinterpret_cast<void**>(&dg), st);
     if (e == cudaSuccess) {
         switch (which) {
         case 0: e = fsa_gram_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), fargs[nf - 1], st, L); break;
@@ -2514,11 +2531,14 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
         case 8: e = fsa_crossgram_launch(P, ptr(0), ptr(1), (int)args[2], dg, ni, ptr(3), st, L); break;
         case 9: e = fsa_rowdot_launch(dr, ni, st, L); break;
         case 10: e = fsa_var_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
+        case 11: e = fsa_crossgram_dx_launch(P, ptr(0), ptr(1), ptr(2), (int)args[3], args[4], ptr(5), ptr(6), ptr(7), ptr(8),
+                                             args[9], ptr(10), ptr(11), ptr(12), args[13], dd, ni, ptr(14), ptr(15), st, L); break;
         }
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (dg) cudaFree(dg);
     if (dr) cudaFree(dr);
+    if (dd) cudaFree(dd);
     CK(e);
     return GPB200_OK;
 }
@@ -3567,6 +3587,12 @@ struct Fsa {
     // gpb200_fitc_rand: Sigma* gathered into the caller's order (Ms x Ms, dense) through the test-point permutation pp
     double* Sc = nullptr; long long* pp = nullptr;
     size_t Sc_cap = 0, pp_cap = 0;
+    // gpb200_fitc_predict_fsa_grad (first use): the s K_ub' tiles of the test rows (Nc x 2048), Z = K_*u + E K_fu / 2
+    // (Nc x Mpad), dmu / dvar in the caller's order (2 x Ms x d) and the contraction's items
+    double *Tb = nullptr, *Zb = nullptr, *pdx = nullptr;
+    CUtensorMap mapZb{};
+    FsaDxItem* pdi = nullptr;
+    size_t pdx_cap = 0, pdi_cap = 0;
 };
 
 static void fsa_free(gpb200_fitc* f) {
@@ -3574,7 +3600,7 @@ static void fsa_free(gpb200_fitc* f) {
     Fsa* s = f->fsa;
     void* ptrs[] = {s->xb, s->mask, s->X, s->LT, s->logd, s->r, s->a, s->t1, s->t2, s->pos, s->bstart, s->boff,
                     s->rblk, s->bsize, s->info, s->gitems, s->litems, s->gramitems, s->Gpk, s->gpart, s->ones,
-                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr, s->Sc, s->pp};
+                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr, s->Sc, s->pp, s->Tb, s->Zb, s->pdx, s->pdi};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete s;
     f->fsa = nullptr;
@@ -4042,8 +4068,20 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
 // (from Sigma^-1 = Lambda^-1 - Lambda^-1 K_fu S^-1 K_uf Lambda^-1 and S = K_uu + K_uf Lambda^-1 K_fu; C = 0 is the FITC formula).
 // G G' is block-diagonal in the test blocks.  Test points are grouped by paired block, each group padded to 128 rows, and
 // streamed in chunks of at most Nc padded rows; per chunk, the training chunks of the paired blocks are revisited (V, K_uf).
-int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
-                            double* mu, double* var, double* cov) {
+//
+// dmu != null (gpb200_fitc_predict_fsa_grad; cov null): the same launches give mu and var, then per test chunk the
+// gradients with respect to the test inputs.  With c = C row m, h = H row m, D_u / D_b / D_** the input derivatives of
+// k(x*, u_j), k(x*, x_i) (i in the paired block b) and k(x*, x*), and s = S^-1 r~' (= R L_s^-1, r~ = K_*u - C Lambda_b^-1 K_bu):
+//   dmu  = D_u (u - beta) + D_b alpha_b ,               beta = K_uu^-1 K_ub alpha_b
+//   dvar = D_** + D_u 2 (s - K_uu^-1 Z) + D_b e ,       e = -2 (h + s K_ub Lambda_b^-1) ,  Z = k_u + K_ub e / 2
+// (dc = D_b - D_u K_uu^-1 K_ub; c = 0 gives the FITC formula).  s comes from the right-side TRSM on es after R; a second
+// sweep over the paired training chunks regenerates K_fu / K_uf and forms s K_ub' (the C tiles' shape, into Tb), its
+// product with Lambda_b^-1 = X'X through Gb, e (over H, in the C tiles), then Z += e K_bu / 2 and alpha_b K_bu (A read
+// with lda = 0, every row of a test tile the same alpha_b) into the Mpad-wide test rows of Zb and Vs; beta is formed per
+// test row rather than once per block, so that it shares the row layout, the GEMM shape and the two K_uu^-1 TRSMs of Z.
+// One fsa_crossgram_dx launch per chunk writes dmu / dvar into the caller's order.
+static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of, double* mu,
+                       double* var, double* cov, double* dmu, double* dvar) {
     if (!f || Ms <= 0 || !xs || !block_of || !mu) return GPB200_EINVAL;
     if (f->mode != 3) { f->err = "fitc_predict_fsa: the handle is not in FSA mode (3)"; return GPB200_EINVAL; }
     if (!f->fsa || !f->factored || !f->alpha_ready) { f->err = "fitc_predict_fsa: set_blocks, factorize and mll first"; return GPB200_ESTATE; }
@@ -4093,10 +4131,24 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
             f->err = "fitc_predict_fsa: cuTensorMapEncodeTiled failed"; return GPB200_ECUDA;
         }
     }
+    const bool grad = dmu != nullptr, gvar = grad && var;
+    if (gvar && !s->Zb) {
+        FCK(cudaMalloc(&s->Tb, sizeof(double) * Nc * LDC));
+        FCK(cudaMalloc(&s->Zb, sizeof(double) * Nc * Mp));
+        if (eu->tma_ok && !gemm_make_tensor_map(&s->mapZb, s->Zb, Nc, Mp, Mp)) {
+            f->err = "fitc_predict_fsa_grad: cuTensorMapEncodeTiled failed"; return GPB200_ECUDA;
+        }
+    }
+    if (grad && (size_t)(2 * Ms * d) > s->pdx_cap) {
+        if (s->pdx) cudaFree(s->pdx);
+        s->pdx = nullptr; s->pdx_cap = 0;
+        FCK(cudaMalloc(&s->pdx, sizeof(double) * 2 * Ms * d));
+        s->pdx_cap = (size_t)(2 * Ms * d);
+    }
     double *mu1 = s->pvec, *mu2 = mu1 + Nc, *q = mu2 + Nc, *g2 = q + Nc, *r2 = g2 + Nc, *vp = r2 + Nc;
-    // work lists of every (test chunk, training chunk) pair
-    struct Pass { int chunk; FsaLaunch xg, vv, gg, hh, kh; FsaLaunch mu2, g2; };
-    struct Sub { int64_t t0, t1; std::vector<Pass> passes; FsaLaunch ggt; };
+    // work lists of every (test chunk, training chunk) pair; t1 .. ak: the gradient's second sweep
+    struct Pass { int chunk; FsaLaunch xg, vv, gg, hh, kh; FsaLaunch mu2, g2; FsaLaunch t1, tx, ee, ek, ak; };
+    struct Sub { int64_t t0, t1; std::vector<Pass> passes; FsaLaunch ggt, dx; };
     std::vector<Sub> subs;
     std::vector<FsaGemmItem> gi; std::vector<FsaGramItem> xi; std::vector<FsaRowItem> ri;
     auto gemm = [&](double* C, long long ldc, const double* A, long long lda, const double* B, long long ldb, int64_t K,
@@ -4177,6 +4229,47 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
                          f->bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], -1.0, 1.0);
             });
             ps.kh.n = (int)((int64_t)gi.size() - ps.kh.off);
+            if (gvar) {
+                ps.t1.off = (int64_t)gi.size();                 // T = s K_ub'  (bufB = s, bufA = K_fu of the chunk)
+                each([&](int64_t b, int64_t tl) {
+                    for (int c = 0; c < s->bsize_h[(size_t)b] / TILE; ++c)
+                        gemm(s->Tb + tl * TILE * LDC + c * TILE, LDC, f->bufB + tl * TILE * Mp, Mp,
+                             f->bufA + (s->bstart_h[(size_t)b] - ch.r0 + c * TILE) * Mp, Mp, Mp, 1.0, 0.0);
+                });
+                ps.t1.n = (int)((int64_t)gi.size() - ps.t1.off);
+                ps.tx.off = (int64_t)gi.size();                 // T X'  (into the G tiles)
+                each([&](int64_t b, int64_t tl) {
+                    const int B = s->bsize_h[(size_t)b];
+                    for (int c = 0; c < B / TILE; ++c)
+                        gemm(s->Gb + tl * TILE * LDC + c * TILE, LDC, s->Tb + tl * TILE * LDC, LDC,
+                             s->X + s->boff_h[(size_t)b] + (int64_t)c * TILE * B, B, (int64_t)(c + 1) * TILE, 1.0, 0.0);
+                });
+                ps.tx.n = (int)((int64_t)gi.size() - ps.tx.off);
+                ps.ee.off = (int64_t)gi.size();                 // e = -2 (H + T X' X)  (over H in the C tiles)
+                each([&](int64_t b, int64_t tl) {
+                    const int B = s->bsize_h[(size_t)b];
+                    for (int c = 0; c < B / TILE; ++c)
+                        gemm(s->Cb + tl * TILE * LDC + c * TILE, LDC, s->Gb + tl * TILE * LDC + c * TILE, LDC,
+                             s->LT + s->boff_h[(size_t)b] + (int64_t)c * TILE * B + c * TILE, B, B - (int64_t)c * TILE, -2.0, -2.0);
+                });
+                ps.ee.n = (int)((int64_t)gi.size() - ps.ee.off);
+                ps.ek.off = (int64_t)gi.size();                 // Z += e K_bu / 2  (bufA = K_uf of the chunk)
+                each([&](int64_t b, int64_t tl) {
+                    for (int64_t u = 0; u < Mp / TILE; ++u)
+                        gemm(s->Zb + tl * TILE * Mp + u * TILE, Mp, s->Cb + tl * TILE * LDC, LDC,
+                             f->bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], 0.5, 1.0);
+                });
+                ps.ek.n = (int)((int64_t)gi.size() - ps.ek.off);
+            }
+            if (grad) {
+                ps.ak.off = (int64_t)gi.size();                 // alpha_b K_bu on every row of the tile (into Vs)
+                each([&](int64_t b, int64_t tl) {
+                    for (int64_t u = 0; u < Mp / TILE; ++u)
+                        gemm(s->Vs + tl * TILE * Mp + u * TILE, Mp, s->a + s->bstart_h[(size_t)b], 0,
+                             f->bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], 1.0, 0.0);
+                });
+                ps.ak.n = (int)((int64_t)gi.size() - ps.ak.off);
+            }
             sb.passes.push_back(ps);
             t = te;
         }
@@ -4195,6 +4288,21 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
         subs.push_back(std::move(sb));
         t0 = subs.back().t1;
     }
+    std::vector<FsaDxItem> di;                                   // the contraction: one item per real test point
+    if (grad) {
+        std::vector<int64_t> at((size_t)Msp, -1);
+        for (int64_t i = 0; i < Ms; ++i) at[(size_t)ppos[(size_t)i]] = i;
+        for (Sub& sb : subs) {
+            sb.dx.off = (int64_t)di.size();
+            for (int64_t r = sb.t0 * TILE; r < sb.t1 * TILE; ++r) {
+                const int64_t i = at[(size_t)r];
+                if (i < 0) continue;
+                const int64_t b = key[(size_t)i];
+                di.push_back(FsaDxItem{r - sb.t0 * TILE, i, b < nb ? s->bstart_h[(size_t)b] : 0, b < nb ? s->bsize_h[(size_t)b] : 0});
+            }
+            sb.dx.n = (int)((int64_t)di.size() - sb.dx.off);
+        }
+    }
     auto upload = [&](auto*& dst, size_t& cap, const auto& v) -> cudaError_t {
         using T = typename std::decay_t<decltype(v)>::value_type;
         if (v.size() > cap) {
@@ -4209,17 +4317,28 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
     FCK(upload(s->pg, s->pg_cap, gi));
     FCK(upload(s->px, s->px_cap, xi));
     FCK(upload(s->pr, s->pr_cap, ri));
+    if (grad) FCK(upload(s->pdi, s->pdi_cap, di));
     GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, Mp};
     GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, Mp};
     GemmBuf bVs{eu->tma_ok ? &s->mapVs : nullptr, s->Vs, Mp};
+    GemmBuf bZb{eu->tma_ok ? &s->mapZb : nullptr, s->Zb, Mp};
     const bool cov_host = cov && !f->cov_keep_device;
     std::vector<double> mu_p((size_t)Msp), var_p(var ? (size_t)Msp : 0), cov_p(cov_host ? (size_t)Msp * Msp : 0);
+    double* ddmu = grad ? s->pdx : nullptr;
+    double* ddvar = grad ? s->pdx + Ms * d : nullptr;
+    if (grad) {
+        for (double& t : f->fsag_ms) t = 0.0;
+        FCK(mirror_lower_tiles_launch(eu->F, eu->ld, eu->Npad, st, &eu->launches));      // L' for the right-side TRSMs
+        if (var) FCK(mirror_lower_tiles_launch(es->F, es->ld, es->Npad, st, &eu->launches));
+    }
     for (const Sub& sb : subs) {
         const int64_t row0 = sb.t0 * TILE, mq = (sb.t1 - sb.t0) * TILE;
+        if (grad) FCK(cudaEventRecord(eu->ev0, st));
         FCK(cudaMemcpyAsync(f->xs, xsp.data() + row0 * d, sizeof(double) * mq * d, cudaMemcpyHostToDevice, st));
         FCK(crossgram_launch(eu->prog, f->xs, d, mq, mq, eu->x, d, f->M, Mp, d, f->bufB, Mp, st, &eu->launches));     // K_*u
         FCK(rowdot_launch(f->bufB, Mp, f->uvec, mq, Mp, mu1, st, &eu->launches));                                       // K_*u u
         FCK(cudaMemcpyAsync(s->Vs, f->bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));
+        if (gvar) FCK(cudaMemcpyAsync(s->Zb, f->bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));      // Z = K_*u
         FCK(trsm_rec_buf(eu, bVs, (int)mq, 0, (int)Mp));                                                 // V_*'
         FCK(kdiag_launch(eu->prog, f->xs, d, mq, r2, st, &eu->launches));
         FCK(rowvar_launch(s->Vs, Mp, r2, mq, Mp, q, st, &eu->launches));                                                 // k** - |V_*|^2
@@ -4247,6 +4366,38 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
         FCK(ew_launch(2, mq, mu1, mu2, nullptr, nullptr, 0.0, st, &eu->launches));
         FCK(cudaMemcpyAsync(mu_p.data() + row0, mu1, sizeof(double) * mq, cudaMemcpyDeviceToHost, st));
         if (var) FCK(cudaMemcpyAsync(var_p.data() + row0, vp, sizeof(double) * mq, cudaMemcpyDeviceToHost, st));
+        if (grad) {
+            FCK(cudaEventRecord(eu->ev1, st));
+            if (var) FCK(trsm_right_rec_buf(es, bB2, (int)mq, 0, (int)Mp));                             // s = R L_s^-1
+            FCK(cudaMemsetAsync(s->Vs, 0, sizeof(double) * mq * Mp, st));
+            for (const Pass& ps : sb.passes) {                                                           // second sweep
+                const FsaChunk& ch = s->chunks[(size_t)ps.chunk];
+                const double* xr = s->xb + ch.r0 * d;
+                if (var) {
+                    FCK(fitc_kfu(f, xr, ch.rows));                                                       // K_fu of the chunk
+                    FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
+                    FCK(fsa_gemm_launch(s->pg + ps.t1.off, ps.t1.n, st, &eu->launches));
+                    FCK(fsa_gemm_launch(s->pg + ps.tx.off, ps.tx.n, st, &eu->launches));
+                    FCK(fsa_gemm_launch(s->pg + ps.ee.off, ps.ee.n, st, &eu->launches));
+                }
+                FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->bufA, Nc, st, &eu->launches));
+                FCK(fsa_mask_launch(f->bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+                if (var) FCK(fsa_gemm_launch(s->pg + ps.ek.off, ps.ek.n, st, &eu->launches));
+                FCK(fsa_gemm_launch(s->pg + ps.ak.off, ps.ak.n, st, &eu->launches));
+            }
+            FCK(cudaEventRecord(eu->ev2, st));
+            FCK(trsm_rec_buf(eu, bVs, (int)mq, 0, (int)Mp));                                             // beta
+            FCK(trsm_right_rec_buf(eu, bVs, (int)mq, 0, (int)Mp));
+            if (var) {
+                FCK(trsm_rec_buf(eu, bZb, (int)mq, 0, (int)Mp));                                         // K_uu^-1 Z
+                FCK(trsm_right_rec_buf(eu, bZb, (int)mq, 0, (int)Mp));
+            }
+            FCK(cudaEventRecord(eu->ev3, st));
+            FCK(fsa_crossgram_dx_launch(eu->prog, f->xs, eu->x, s->xb, d, f->M, f->uvec, s->Vs, f->bufB, s->Zb, Mp, s->mask,
+                                        s->a, s->Cb, LDC, s->pdi + sb.dx.off, sb.dx.n, ddmu, var ? ddvar : nullptr, st,
+                                        &eu->launches));
+            FCK(cudaEventRecord(eu->ev4, st));
+        }
         if (cov) {
             FCK(gram_full_launch(eu->prog, f->xs, d, mq, mq, d, f->Kss, mq, st, &eu->launches));
             GemmDesc g = gemm_desc_default();
@@ -4262,6 +4413,17 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
             FCK(fsa_gemm_launch(s->pg + sb.ggt.off, sb.ggt.n, st, &eu->launches));  // - G G'
             if (cov_host) FCK(cudaMemcpyAsync(cov_p.data(), f->Kss, sizeof(double) * mq * mq, cudaMemcpyDeviceToHost, st));
         }
+        FCK(cudaStreamSynchronize(st));
+        if (grad) {
+            f->fsag_ms[0] += ev_ms(eu->ev0, eu->ev1);
+            f->fsag_ms[1] += ev_ms(eu->ev1, eu->ev2);
+            f->fsag_ms[2] += ev_ms(eu->ev2, eu->ev3);
+            f->fsag_ms[3] += ev_ms(eu->ev3, eu->ev4);
+        }
+    }
+    if (grad) {
+        FCK(cudaMemcpyAsync(dmu, ddmu, sizeof(double) * Ms * d, cudaMemcpyDeviceToHost, st));
+        if (var) FCK(cudaMemcpyAsync(dvar, ddvar, sizeof(double) * Ms * d, cudaMemcpyDeviceToHost, st));
         FCK(cudaStreamSynchronize(st));
     }
     if (cov && !cov_host) {
@@ -4285,6 +4447,24 @@ int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
             for (int64_t j = 0; j < Ms; ++j) cov[i * Ms + j] = cov_p[r * (size_t)Msp + (size_t)ppos[(size_t)j]];
     }
     return GPB200_OK;
+}
+
+int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
+                            double* mu, double* var, double* cov) {
+    return fsa_predict(f, Ms, xs, ldxs, block_of, mu, var, cov, nullptr, nullptr);
+}
+
+int gpb200_fitc_predict_fsa_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
+                                 double* mu, double* var, double* dmu, double* dvar) {
+    if (!f) return GPB200_EINVAL;
+    if (f->mode != 3) { f->err = "fitc_predict_fsa_grad: the handle is not in FSA mode (3)"; return GPB200_EINVAL; }
+    if (f->nranks > 1) { f->err = "fitc_predict_fsa_grad: single GPU handles only"; return GPB200_EINVAL; }
+    if (!f->fsa || !f->factored || !f->alpha_ready) { f->err = "fitc_predict_fsa_grad: set_blocks, factorize and mll first"; return GPB200_ESTATE; }
+    if (Ms <= 0 || !xs || ldxs < f->d || !block_of || !mu || !dmu) {
+        f->err = "fitc_predict_fsa_grad: bad Ms, xs, ldxs, block_of, mu or dmu"; return GPB200_EINVAL;
+    }
+    if (!var != !dvar) { f->err = "fitc_predict_fsa_grad: var and dvar must be given together"; return GPB200_EINVAL; }
+    return fsa_predict(f, Ms, xs, ldxs, block_of, mu, var, nullptr, dmu, dvar);
 }
 
 // rand(gp, X, n) (src/GP.jl:120-146) with a sparse cK: Sigma* is the covariance predict_cov (modes 0-2) or predict_fsa
@@ -4330,6 +4510,7 @@ int gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs,
 int gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n) {
     if (!f || !ms || n < 0) return GPB200_EINVAL;
     for (int32_t i = 0; i < n && i < 3; ++i) ms[i] = f->rand_ms[i];
+    for (int32_t i = 3; i < n && i < 7; ++i) ms[i] = f->fsag_ms[i - 3];
     return GPB200_OK;
 }
 

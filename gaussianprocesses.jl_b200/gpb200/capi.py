@@ -84,6 +84,7 @@ _SIGNATURES = {
     "gpb200_fitc_set_mode": (C.c_int, [_H, C.c_int]),
     "gpb200_fitc_set_blocks": (C.c_int, [_H, C.c_int64, _lp, _lp]),
     "gpb200_fitc_predict_fsa": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _lp, _dp, _dp, _dp]),
+    "gpb200_fitc_predict_fsa_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _lp, _dp, _dp, _dp, _dp]),
     "gpb200_fitc_get_inverse_diag": (C.c_int, [_H, _dp]),
     "gpb200_fitc_cv_param": (C.c_int, [_H, C.c_int32, _dp, _dp, _dp]),
     "gpb200_fitc_cv_block": (C.c_int, [_H, C.c_int32, C.c_int64, C.POINTER(C.c_int64), _dp]),
@@ -448,7 +449,8 @@ class Engine:
         a = np.ascontiguousarray(args, dtype=np.int64).ravel()
         self._check(self._lib.gpb200_row_reductions(self._h, int(which), a.ctypes.data_as(_lp), a.size), "row_reductions")
 
-    FSA_KERNELS = ("gram", "bdmv", "mask", "permute", "resid", "outer", "trace", "axpy_t", "crossgram", "rowdot", "var")
+    FSA_KERNELS = ("gram", "bdmv", "mask", "permute", "resid", "outer", "trace", "axpy_t", "crossgram", "rowdot", "var",
+                   "crossgram_dx")
     FITC_CV_KERNELS = ("delta", "rows", "invdiag", "eblock", "qs", "wvec", "gather", "diag", "colscale", "scale", "fitc_g",
                        "fitc_wfu", "fitc_wuu", "symmetrize")
 
@@ -612,6 +614,24 @@ class FitcEngine:
                                                       _as_dp(cov) if cov is not None else None), "fitc_predict_fsa")
         return mu, (cov if full_cov else var)
 
+    def predict_fsa_grad(self, xs_pm, block_of, want_var=True):
+        """FSA predictions and their gradients with respect to the test inputs: (mu_minus_mean, var or None, dmu (Ms, d),
+        dvar (Ms, d) or None), mu and var bitwise those of predict_fsa."""
+        xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
+        Ms, d = xs_pm.shape
+        if d != self.d:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        block_of = np.ascontiguousarray(block_of, dtype=np.int64)
+        if block_of.shape != (Ms,):
+            raise ValueError("fitc_predict_fsa_grad: block_of must have one entry per test point")
+        mu, dmu = np.empty(Ms), np.empty((Ms, d))
+        var = np.empty(Ms) if want_var else None
+        dvar = np.empty((Ms, d)) if want_var else None
+        self._check(self._lib.gpb200_fitc_predict_fsa_grad(self._h, Ms, _as_dp(xs_pm), d, block_of.ctypes.data_as(_lp),
+                                                           _as_dp(mu), _as_dp(var) if want_var else None, _as_dp(dmu),
+                                                           _as_dp(dvar) if want_var else None), "fitc_predict_fsa_grad")
+        return mu, var, dmu, dvar
+
     # -- cross-validation (modes 0-2, one GPU; after factorize + mll) ---------------------------------------------------
     def inverse_diag(self):
         """diag(Sigma^-1)[N]."""
@@ -659,6 +679,13 @@ class FitcEngine:
         out = np.zeros(3)
         self._check(self._lib.gpb200_fitc_get_timings(self._h, _as_dp(out), 3), "fitc_get_timings")
         return out
+
+    def predict_fsa_grad_timings(self):
+        """device times (ms) of the last predict_fsa_grad, summed over its test chunks: predict_fsa's launches, s and the
+        second block sweep, the K_uu^-1 TRSMs, the contraction"""
+        out = np.zeros(7)
+        self._check(self._lib.gpb200_fitc_get_timings(self._h, _as_dp(out), 7), "fitc_get_timings")
+        return out[3:].copy()
 
     def launch_count(self):
         return int(self._lib.gpb200_fitc_launch_count(self._h))

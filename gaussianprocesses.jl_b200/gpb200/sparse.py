@@ -208,8 +208,21 @@ class FSA(FITC):
         mu = mu + self.mean.mean(xs)
         return (mu, s2) if full_cov else (mu, np.maximum(s2, 0.0))
 
-    def predict_f_grad(self, x):
-        raise ValueError("predict_f_grad: not available for FSA (its predictions pair test points with training blocks)")
+    def predict_f_grad(self, x, blockindpred=None):
+        """predict_f(gp, x, blockindpred) and its gradients with respect to the test inputs, (mu, s2, dmu, ds2) as
+        GPE.predict_f_grad: dmu / ds2 are (dim, M), s2 is clamped at 0 (GP.jl:75) and ds2 is 0 where the clamp acts."""
+        if blockindpred is None:
+            raise ValueError("predict_f_grad: FSA pairs test points with training blocks; pass blockindpred")
+        x = _as_dxn(x)
+        if x.shape[0] != self.dim:
+            raise ValueError("Gaussian Process object and input observations do not have consistent dimensions")
+        block_of = test_block_of(blockindpred, x.shape[1])
+        xs = np.ascontiguousarray(x.T)
+        mu, var, dmu, dvar = self._eng.predict_fsa_grad(xs, block_of, want_var=True)
+        mu = mu + self.mean.mean(xs)
+        dmu = dmu + self.mean.grad_x(xs)
+        dvar[var < 0.0] = 0.0
+        return mu, np.maximum(var, 0.0), np.ascontiguousarray(dmu.T), np.ascontiguousarray(dvar.T)
 
     def predict_y(self, x, blockindpred, full_cov=False):
         mu, s2 = self.predict_f(x, blockindpred, full_cov=full_cov)

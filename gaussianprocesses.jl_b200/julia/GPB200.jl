@@ -503,7 +503,7 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=fa
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
 end
 
-# Dual test inputs on FITC / DTC / SoR (see predict_grad_raw above); FSA keeps the Float64 conversion error
+# Dual test inputs on FITC / DTC / SoR (see predict_grad_raw above); FSA's take the test blocks (below)
 function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::DualMatrix; full_cov::Bool=false) where {X,Y,M,K,CS<:B200Sparse,D,P}
     size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
     full_cov && throw(ArgumentError("predict_f: full_cov=true is not supported with Dual inputs"))
@@ -530,6 +530,20 @@ function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, blockindpred::Abs
            "fitc_predict_fsa")
     full_cov && return mu .+ mean(gp.mean, Xs), Σ                                 # Σ is symmetric: row- = column-major
     return mu .+ mean(gp.mean, Xs), max.(var, 0.0)
+end
+
+# Dual test inputs with test blocks: values and gradients from gpb200_fitc_predict_fsa_grad, the Duals rebuilt from them
+function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::DualMatrix, blockindpred::AbstractVector; full_cov::Bool=false) where {X,Y,M,K,CS<:B200FSA,D,P}
+    size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
+    full_cov && throw(ArgumentError("predict_f: full_cov=true is not supported with Dual inputs"))
+    Xs = Matrix{Float64}(ForwardDiff.value.(x)); d, Ms = size(Xs)
+    block_of = test_block_of(blockindpred, Ms)
+    mu = Vector{Float64}(undef, Ms); var = Vector{Float64}(undef, Ms)
+    dmu = Matrix{Float64}(undef, d, Ms); dvar = Matrix{Float64}(undef, d, Ms)
+    checks(gp.cK, ccall((:gpb200_fitc_predict_fsa_grad, LIB), Cint,
+                        (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                        gp.cK.handle, Ms, Xs, d, block_of, mu, var, dmu, dvar), "fitc_predict_fsa_grad")
+    return dual_outputs(x, mu, dmu) .+ mean(gp.mean, x), max.(dual_outputs(x, var, dvar), 0.0)
 end
 
 # 0-based training block of each test point (-1: none) from 1-based test blocks

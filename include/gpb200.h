@@ -292,6 +292,9 @@ int  gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int
  *   which 8  fsa_crossgram : xs, xb, d, mask | Gram items                             fargs = theta
  *   which 9  fsa_rowdot    : | row items (v unused when sq != 0)
  *   which 10 fsa_var       : out, q, g2, r2neg, n
+ *   which 11 crossgram_dx  : xs, z, xb, d, M, u, Wb (0 = none), S1, S2, ldw, mask, alpha, E, lde, dmu, dvar (0: dmu only)
+ *                            | items (row, out, b0, nb)                                 fargs = theta
+ *                            (fsa_crossgram_dx, csrc/fsa.cuh: one CTA per item; xs, z, xb of leading dimension d)
  * GPB200_EINVAL, nothing launched: bad which / n / nf, theta not of n_theta entries, a program dimension >= d, a null
  * pointer the kernel dereferences, a negative size or row, a bad mode, an item ld < 128, lda < K, ld < ncols.
  * GPB200_ESTATE: a kernel-program call before gpb200_set_kernel.                                                    */
@@ -377,7 +380,8 @@ int  gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t l
  * dvar together or both NULL): mu_minus_mean and var bitwise equal to gpb200_fitc_predict's, and
  *   dvar[m, p] = 2c dk(x*_m, x*_m)/dx*_{m,p} - 2 sum_j dk(x*_m, u_j)/dx*_{m,p} W'[m, j],  W' = K*u K_uu^-1 - K*u Sigma_QR^-1
  * (c = 1; SoR: W' = -K*u Sigma_QR^-1, c = 0), dmu[m, p] = sum_j dk(x*_m, u_j)/dx*_{m,p} (Sigma_QR^-1 K_uf Lambda^-1 y)_j.
- * GPB200_ESTATE before factorize + mll; GPB200_EINVAL for FSA (mode 3) and multi-rank handles ("single GPU").         */
+ * GPB200_ESTATE before factorize + mll; GPB200_EINVAL for multi-rank handles ("single GPU") and in mode 3, whose
+ * gradients need test blocks (gpb200_fitc_predict_fsa_grad).                                                          */
 int  gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean,
                               double* var, double* dmu, double* dvar);
 /* predictMVN with the full covariance cov[Ms x Ms] (fitc.jl:324-332, dtc.jl:41-59, sor.jl:302-321); Ms <= 32768 */
@@ -411,6 +415,20 @@ int  gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* bloc
  * grouped by block and each group padded to a multiple of 128, to fit one staging chunk (GPB200_EINVAL otherwise).      */
 int  gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
                              double* mu_minus_mean, double* var, double* cov);
+/* Predictive gradients of FSA with respect to the test inputs (predict_f(gp, x, blockindpred) with ForwardDiff.Dual
+ * inputs), block_of and layouts as gpb200_fitc_predict_fsa and gpb200_fitc_predict_grad: mu_minus_mean[Ms] and var[Ms]
+ * bitwise equal to gpb200_fitc_predict_fsa's (same launches), dmu and dvar Ms x d point-major, var and dvar given together
+ * or both NULL.  With c = Lambda_xf row m (0 when unpaired), u = alpha_u, S = Sigma_QR, h = c Lambda_b^-1,
+ * s = S^-1 (k_u - K_ub h') and D_u, D_b, D_** the input derivatives of k(x*, u_j), k(x*, x_i) over the paired block and k(x*, x*):
+ *   dmu  = D_u (u - K_uu^-1 K_ub alpha_b) + D_b alpha_b
+ *   dvar = D_** + D_u (2 s - 2 K_uu^-1 k_u - K_uu^-1 K_ub e) + D_b e,   e = -2 Lambda_b^-1 (c' + K_bu s)
+ * Test points are streamed (no size limit).  Device memory grows on the first call with var by one staging chunk of
+ * test-row x block tiles (Nc x 128 * the largest block's tiles doubles) and one Nc x Mpad matrix, and by 2 Ms d doubles
+ * for the outputs.  GPB200_ESTATE before set_blocks + factorize + mll; GPB200_EINVAL outside mode 3, for multi-rank
+ * handles and for bad arguments.  gpb200_fitc_get_timings slots 3-6 hold its device-event split, summed over the test
+ * chunks: predict_fsa's launches, s and the second block sweep, the K_uu^-1 TRSMs, the contraction.                   */
+int  gpb200_fitc_predict_fsa_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
+                                  double* mu_minus_mean, double* var, double* dmu, double* dvar);
 /* rand(gp, X, n) (src/GP.jl:120-146) with a sparse cK, on the device, with gpb200_rand's conventions: z and samples are
  * Ms x nsamp column-major, mu_minus_mean[Ms] is the predictive mean without mean(x*).  Sigma* is exactly the covariance of
  * gpb200_fitc_predict_cov (modes 0-2; block_of must be NULL; Ms <= one staging chunk) or of gpb200_fitc_predict_fsa (mode 3;
@@ -427,7 +445,9 @@ int  gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64
 int  gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
                       int64_t nsamp, const double* z, double nugget, double* mu_minus_mean, double* samples);
 /* device times (ms) of the last successful gpb200_fitc_rand: [0] Sigma* build (with mu), [1] make_posdef! + Cholesky,
- * [2] unwhiten! GEMM + mu (CUDA events; n <= 3 entries are written)                                                    */
+ * [2] unwhiten! GEMM + mu; of the last gpb200_fitc_predict_fsa_grad, summed over its test chunks: [3] predict_fsa's
+ * launches, [4] s = R L_s^-1 and the second block sweep, [5] the K_uu^-1 TRSMs, [6] the contraction (CUDA events;
+ * n <= 7 entries are written)                                                                                           */
 int  gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n);
 /* ---- cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) ---------------
  * The dense entry points gpb200_get_inverse_diag / gpb200_cv_param / gpb200_cv_block for modes 0 (FITC), 1 (DTC: SoR's
