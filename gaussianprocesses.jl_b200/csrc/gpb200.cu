@@ -1012,7 +1012,7 @@ float ev_ms(cudaEvent_t a, cudaEvent_t b) {
 // Gram build / gradient trace dispatch: the TMA-staged SEIso kernels (gram_fast.cu) when the kernel program is the single
 // SEIso leaf over all (<= 8) input dimensions, else the generic kernel-program kernels (gram.cu)
 bool use_seiso_fast(gpb200_handle* h, SeIsoFast* sf) {
-    return h->gram_fast && h->prog.fast && h->xmap_ok && h->xp && seiso_fast_prepare(h->prog.par[0], h->prog.par[1], sf);
+    return h->gram_fast && kprog_fast(h->prog, h->d) && h->xmap_ok && h->xp && seiso_fast_prepare(h->prog.par[0], h->prog.par[1], sf);
 }
 cudaError_t launch_gram(gpb200_handle* h, double* G, int64_t ldg, int own_tiles, int nranks, int rank, int own_axis) {
     SeIsoFast sf;
@@ -1362,6 +1362,9 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
     CK(cudaStreamSynchronize(h->st));
     h->has_data = true;
     h->factored = h->inv_ready = h->alpha_ready = false;
+    // a kernel program that reads a dimension the new points do not have is dropped: factorize then asks for set_kernel
+    for (int i = 0; h->has_kernel && i < GPB200_MAX_DIMS; ++i)
+        if (h->prog.dims[i] >= d) h->has_kernel = false;
     return GPB200_OK;
 }
 
@@ -1408,9 +1411,9 @@ int gpb200_set_kernel(gpb200_handle* h, int32_t n_ops, const int32_t* ops, int32
         if (dims[i] < 0 || (h->has_data && dims[i] >= h->d)) return fail(h, GPB200_EINVAL, "set_kernel: dim index out of range");
         P.dims[i] = dims[i];
     }
-    // single SEIso leaf over dims 0..nd-1 == the whole input: specialised kernels
+    // single SEIso leaf over dims 0..nd-1: specialised kernels whenever nd is the input dimension (kprog_fast)
     P.fast = 0;
-    if (n_ops == 1 && P.op[0] == GPB200_OP_SE_ISO && h->has_data && P.nd[0] == h->d) {
+    if (n_ops == 1 && P.op[0] == GPB200_OP_SE_ISO) {
         bool ident = true;
         for (int i = 0; i < P.nd[0]; ++i) ident = ident && (P.dims[P.doff[0] + i] == i);
         P.fast = ident ? 1 : 0;
@@ -1579,14 +1582,14 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     if (h->sharded) {
         // fused trace over the own rows of K^-1 (block-cyclic tile rows), P+1 partial sums summed over the ranks
         for (auto* q : Lg) SCK(q, launch_trace(q, q->nranks, q->rank, q->rb));
-        TRY(coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out; }, (size_t)trace_num_acc(h->prog)));
+        TRY(coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out; }, (size_t)trace_num_acc(h->prog, h->d)));
     } else {
         CK(launch_trace(h, h->nranks, h->rank, 1));
     }
     if (!h->sharded && h->nranks > 1) {                    // P+1 partial sums, summed over ranks
         CK(cudaEventRecord(h->ev_x, h->st));
         CK(cudaStreamWaitEvent(h->st_comm, h->ev_x, 0));
-        CKN(g_nccl.AllReduce(h->trace_out, h->trace_out, (size_t)trace_num_acc(h->prog), ncclDouble, ncclSum, h->comm, h->st_comm));
+        CKN(g_nccl.AllReduce(h->trace_out, h->trace_out, (size_t)trace_num_acc(h->prog, h->d), ncclDouble, ncclSum, h->comm, h->st_comm));
         CK(cudaEventRecord(h->ev_y, h->st_comm));
         CK(cudaStreamWaitEvent(h->st, h->ev_y, 0));
     }
@@ -2539,6 +2542,101 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
     if (dg) cudaFree(dg);
     if (dr) cudaFree(dr);
     if (dd) cudaFree(dd);
+    CK(e);
+    return GPB200_OK;
+}
+
+int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
+    if (!h || (n > 0 && !args) || which < 0 || which > 10 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    static const int want[11] = {14, 11, 7, 5, 10, 12, 13, 11, 6, 13, 3};
+    if (n != want[which]) return fail(h, GPB200_EINVAL, "gram_kernels: wrong argument count for this kernel");
+    const int64_t* a = args;
+    auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
+    // every argument pointer non-null; a buffer accessed as double2 16-byte aligned with an even leading dimension
+    auto need = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (!a[i]) return false;
+        return true;
+    };
+    auto vec2 = [&](int p, int ld) { return a[p] % 16 == 0 && a[ld] % 2 == 0; };
+    auto padded = [&](int size, int pad) { return a[size] >= 0 && a[pad] >= a[size] && a[pad] % TILE == 0; };
+    KProg P{};
+    int64_t d = 1;
+    if (which != 10) {
+        static const int dpos[10] = {2, 8, 4, 2, 2, 8, 2, 6, 2, 6};
+        d = a[dpos[which]];
+        if (d < 1 || d > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "gram_kernels: d outside 1 .. GPB200_MAX_DIMS");
+        const int32_t extra = (which == 0 || which == 9) ? 1 : 0;       // nugget / c after theta
+        if (h->has_kernel && nf != h->prog.n_theta + extra)
+            return fail(h, GPB200_EINVAL, "gram_kernels: fargs = theta (+ nugget for gram_lower, c for crossgram_dx)");
+        TRY(local_prog(h, "gram_kernels", fargs, h->prog.n_theta, d, P));
+    } else if (nf != 0) {
+        return fail(h, GPB200_EINVAL, "gram_kernels: mirror_lower_tiles takes no fargs");
+    }
+    const int np = P.n_theta;
+    auto jok = [&](int i) { return a[i] >= 0 && a[i] < np; };
+    bool ok = true;
+    switch (which) {
+    case 0:     // x, ldx, d, N, Npad, noise_var, n_noise, G, ldg, own_tiles, nranks, rank, own_axis, bm_min
+        ok = need({0, 5, 7}) && a[1] >= d && padded(3, 4) && (a[6] == 1 || a[6] == a[3]) && vec2(7, 8) && a[8] >= a[4] &&
+             a[9] >= 0 && a[10] >= 1 && a[11] >= 0 && a[11] < a[10] && (a[12] == 0 || a[12] == 1) && a[13] >= 0;
+        break;
+    case 1:     // xs, ldxs, M, Mpad, x, ldx, N, Npad, d, Kst, ldk
+        ok = need({0, 4, 9}) && a[1] >= d && a[5] >= d && padded(2, 3) && padded(6, 7) && vec2(9, 10) && a[10] >= a[7];
+        break;
+    case 2:     // xs, ldxs, M, Mpad, d, Kss, ldk
+        ok = need({0, 5}) && a[1] >= d && padded(2, 3) && vec2(5, 6) && a[6] >= a[3];
+        break;
+    case 3:     // xs, ldxs, d, M, out
+        ok = need({0, 4}) && a[1] >= d && a[3] >= 0;
+        break;
+    case 4:     // x, ldx, d, N, Npad, j, D, ldd, row0, rows
+        ok = need({0, 6}) && a[1] >= d && padded(3, 4) && jok(5) && a[7] >= a[4] && a[8] >= 0 && a[8] % TILE == 0 &&
+             a[9] >= 0 && a[9] % TILE == 0 && a[8] + a[9] <= a[4];
+        break;
+    case 5:     // x1, ldx1, N1, N1pad, x2, ldx2, N2, N2pad, d, j, D, ldd
+        ok = need({0, 4, 10}) && a[1] >= d && a[5] >= d && padded(2, 3) && padded(6, 7) && jok(9) && a[11] >= a[7];
+        break;
+    case 6:     // x, ldx, d, N, Npad, alpha, Kinv, ldg, part, out, bm_mod, bm_rem, bm_div
+        ok = need({0, 5, 6, 8, 9}) && a[1] >= d && padded(3, 4) && vec2(6, 7) && a[7] >= a[4] && a[10] >= 1 &&
+             a[11] >= 0 && a[11] < a[10] && a[12] >= 1;
+        break;
+    case 7:     // x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part, out
+        ok = need({0, 3, 7, 9, 10}) && a[1] >= d && a[4] >= d && a[2] >= 0 && a[5] >= 0 && vec2(7, 8) && a[8] >= a[5];
+        break;
+    case 8:     // x, ldx, d, N, g, out
+        ok = need({0, 4, 5}) && a[1] >= d && a[3] >= 0;
+        break;
+    case 9:     // xs, ldxs, M, z, ldz, n, d, a, W1, W2, ldw, dmu, dvar
+        ok = need({0, 3, 7, 11}) && a[1] >= d && a[4] >= d && a[2] >= 0 && a[5] >= 0 && ((!a[8] && !a[9]) || (a[12] && a[10] >= a[5]));
+        break;
+    case 10:    // F, ld, Npad
+        ok = need({0}) && a[2] >= 0 && a[2] % TILE == 0 && a[1] >= a[2];
+        break;
+    }
+    if (!ok) return fail(h, GPB200_EINVAL, "gram_kernels: a null pointer, a negative size, a bad padding, leading dimension or "
+                                           "alignment, j outside [0, n_theta) or a bad ownership argument");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = h->st;
+    int64_t* L = &h->launches;
+    const int id = (int)d;
+    cudaError_t e = cudaSuccess;
+    switch (which) {
+    case 0: e = gram_lower_launch(P, ptr(0), a[1], id, a[3], a[4], ptr(5), a[6], fargs[nf - 1], ptr(7), a[8], st, L, (int)a[9],
+                                  (int)a[10], (int)a[11], (int)a[12], (int)a[13]); break;
+    case 1: e = crossgram_launch(P, ptr(0), a[1], a[2], a[3], ptr(4), a[5], a[6], a[7], id, ptr(9), a[10], st, L); break;
+    case 2: e = gram_full_launch(P, ptr(0), a[1], a[2], a[3], id, ptr(5), a[6], st, L); break;
+    case 3: e = kdiag_launch(P, ptr(0), a[1], a[3], ptr(4), st, L); break;
+    case 4: e = gram_grad_full_launch(P, ptr(0), a[1], id, a[3], a[4], (int)a[5], ptr(6), a[7], st, L, a[8], a[9]); break;
+    case 5: e = crossgram_grad_launch(P, ptr(0), a[1], a[2], a[3], ptr(4), a[5], a[6], a[7], id, (int)a[9], ptr(10), a[11], st, L); break;
+    case 6: e = trace_launch(P, ptr(0), a[1], id, a[3], a[4], ptr(5), ptr(6), a[7], ptr(8), ptr(9), st, L, (int)a[10], (int)a[11],
+                             (int)a[12]); break;
+    case 7: e = trace_rect_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], id, ptr(7), a[8], ptr(9), ptr(10), st, L); break;
+    case 8: e = kdiag_grad_launch(P, ptr(0), a[1], a[3], ptr(4), ptr(5), st, L); break;
+    case 9: e = crossgram_dx_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], id, ptr(7), ptr(8), ptr(9), a[10], fargs[nf - 1],
+                                    ptr(11), ptr(12), st, L); break;
+    case 10: e = mirror_lower_tiles_launch(ptr(0), a[1], a[2], st, L); break;
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     CK(e);
     return GPB200_OK;
 }

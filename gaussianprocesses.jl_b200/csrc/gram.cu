@@ -5,7 +5,10 @@
 //   cov!(cK, k, X1, X2, data)       src/kernels/kernels.jl:56-71   (rectangular, predict)
 //   dmll_kern!(dmll, k, X, data, A) src/GPE.jl:219-241             (1/2 sum_ij A_ij dK_ij/dθ)
 // and removes the N x N distance cache (IsotropicData.R, src/kernels/stationary.jl:34-40):
-// distances are recomputed from the 128 x d input tiles staged in shared memory.
+// distances are recomputed from the 128 x d input tiles staged in shared memory.  When two staged tiles (and a kernel's
+// reduction scratch) exceed the device's opt-in shared memory per block (d >= 110 on an H100), the tile kernels read the
+// points in place from global memory instead: the same values enter the same arithmetic, so the results are bitwise
+// those of the staged kernels (and of fsa_gram, which always reads global memory).  Padding rows are never read.
 //
 // Tile-per-CTA (128 x 128 outputs, 256 threads): the two input tiles are staged in shared memory
 // (row stride padded to an odd number of doubles -> conflict-free column reads), each warp owns 16
@@ -30,6 +33,20 @@ __device__ __forceinline__ void load_xtile(double* s, const double* __restrict__
     }
 }
 
+// The tile of points row0 .. row0+127 as (base, row stride): staged into s when `staged`, else x itself in global memory
+// (rows past the valid count are then not addressable, and every kernel guards them before it evaluates the program).
+struct XTile {
+    const double* p;
+    long long ld;
+    __device__ __forceinline__ const double* row(int r) const { return p + r * ld; }
+};
+__device__ __forceinline__ XTile xtile(bool staged, double* s, const double* x, long long ldx, int d, long long row0,
+                                       long long nrows_valid) {
+    if (!staged) return XTile{x + row0 * ldx, ldx};
+    load_xtile(s, x, ldx, d, d | 1, row0, nrows_valid);
+    return XTile{s, d | 1};
+}
+
 // ------------------------------------------------------------------------------------------
 // symmetric Gram, lower tiles:  G[i,j] = k(x_i,x_j) + [i==j] noise_i ; padding = identity
 // ------------------------------------------------------------------------------------------
@@ -38,7 +55,8 @@ __global__ void __launch_bounds__(NT) gram_lower_kernel(const __grid_constant__ 
                                                         long long ldx, int d, long long N, long long Npad,
                                                         const double* __restrict__ noise_var, long long n_noise,
                                                         double nugget, double* __restrict__ G, long long ldg,
-                                                        int own_tiles, int nranks, int rank, int own_axis, int bm_min) {
+                                                        int own_tiles, int nranks, int rank, int own_axis, int bm_min,
+                                                        int staged) {
     const int bm = blockIdx.y, bn = blockIdx.x;
     if (bn > bm || bm < bm_min) return;
     // multi-GPU ownership: block columns (replicated storage, own_axis 0) or block rows (row-sharded storage, own_axis 1)
@@ -47,14 +65,14 @@ __global__ void __launch_bounds__(NT) gram_lower_kernel(const __grid_constant__ 
     const int ds = d | 1;
     double* sXi = sm;
     double* sXj = sm + TB * ds;
-    load_xtile(sXi, x, ldx, d, ds, (long long)bm * TB, N);
-    load_xtile(sXj, x, ldx, d, ds, (long long)bn * TB, N);
+    const XTile ti = xtile(staged, sXi, x, ldx, d, (long long)bm * TB, N);
+    const XTile tj = xtile(staged, sXj, x, ldx, d, (long long)bn * TB, N);
     __syncthreads();
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double mh = 0.0, s2 = 0.0;
     if (FAST) { mh = -0.5 / P.par[0]; s2 = P.par[1]; }
-    if (FAST && d <= 8) {
+    if (FAST && d <= 8 && staged) {
         // register-cached variant: the lane's 4 column points live in registers, a row point is read
         // once per row (8 broadcast LDS) -> 2 LDS per output instead of 16: FP64-ALU bound, not LSU bound
         double xjr[4][8];
@@ -93,7 +111,7 @@ __global__ void __launch_bounds__(NT) gram_lower_kernel(const __grid_constant__ 
     for (int rr = 0; rr < 16; ++rr) {
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
             const int c0 = b * 64 + lane * 2;
@@ -102,14 +120,16 @@ __global__ void __launch_bounds__(NT) gram_lower_kernel(const __grid_constant__ 
             for (int e = 0; e < 2; ++e) {
                 const int c = c0 + e;
                 const long long gj = (long long)bn * TB + c;
-                const double* xj = sXj + c * ds;
-                double kv;
-                if (FAST) {
-                    double r2 = 0.0;
-                    for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
-                    kv = s2 * exp(mh * r2);
-                } else {
-                    kv = kprog_eval<false>(P, xi, xj, nullptr);
+                const double* xj = tj.row(c);
+                double kv = 0.0;
+                if (gi < N && gj < N) {                    // a padding row is never read
+                    if (FAST) {
+                        double r2 = 0.0;
+                        for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
+                        kv = s2 * exp(mh * r2);
+                    } else {
+                        kv = kprog_eval<false>(P, xi, xj, nullptr);
+                    }
                 }
                 if (gi >= N || gj >= N) kv = (gi == gj) ? 1.0 : 0.0;
                 else if (gi == gj) kv += ((n_noise == 1) ? noise_var[0] : noise_var[gi]) + nugget;
@@ -127,14 +147,12 @@ template <bool FAST>
 __global__ void __launch_bounds__(NT) crossgram_kernel(const __grid_constant__ KProg P, const double* __restrict__ xs,
                                                        long long ldxs, long long M, const double* __restrict__ x,
                                                        long long ldx, long long N, int d, double* __restrict__ Kst,
-                                                       long long ldk) {
+                                                       long long ldk, int staged) {
     const int bm = blockIdx.y, bn = blockIdx.x;
     extern __shared__ double sm[];
     const int ds = d | 1;
-    double* sXi = sm;
-    double* sXj = sm + TB * ds;
-    load_xtile(sXi, xs, ldxs, d, ds, (long long)bm * TB, M);
-    load_xtile(sXj, x, ldx, d, ds, (long long)bn * TB, N);
+    const XTile ti = xtile(staged, sm, xs, ldxs, d, (long long)bm * TB, M);
+    const XTile tj = xtile(staged, sm + TB * ds, x, ldx, d, (long long)bn * TB, N);
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double mh = 0.0, s2 = 0.0;
@@ -143,7 +161,7 @@ __global__ void __launch_bounds__(NT) crossgram_kernel(const __grid_constant__ K
     for (int rr = 0; rr < 16; ++rr) {
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
             const int c0 = b * 64 + lane * 2;
@@ -152,16 +170,17 @@ __global__ void __launch_bounds__(NT) crossgram_kernel(const __grid_constant__ K
             for (int e = 0; e < 2; ++e) {
                 const int c = c0 + e;
                 const long long gj = (long long)bn * TB + c;
-                const double* xj = sXj + c * ds;
-                double kv;
-                if (FAST) {
-                    double r2 = 0.0;
-                    for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
-                    kv = s2 * exp(mh * r2);
-                } else {
-                    kv = kprog_eval<false>(P, xi, xj, nullptr);
+                const double* xj = tj.row(c);
+                double kv = 0.0;
+                if (gi < M && gj < N) {                    // a padding row is never read
+                    if (FAST) {
+                        double r2 = 0.0;
+                        for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
+                        kv = s2 * exp(mh * r2);
+                    } else {
+                        kv = kprog_eval<false>(P, xi, xj, nullptr);
+                    }
                 }
-                if (gi >= M || gj >= N) kv = 0.0;
                 v[e] = kv;
             }
             *reinterpret_cast<double2*>(Kst + gi * ldk + (long long)bn * TB + c0) = make_double2(v[0], v[1]);
@@ -182,14 +201,12 @@ __global__ void kdiag_kernel(const __grid_constant__ KProg P, const double* __re
 template <bool FAST>
 __global__ void __launch_bounds__(NT) gram_full_kernel(const __grid_constant__ KProg P, const double* __restrict__ xs,
                                                        long long ldxs, long long M, int d, double* __restrict__ Kss,
-                                                       long long ldk) {
+                                                       long long ldk, int staged) {
     const int bm = blockIdx.y, bn = blockIdx.x;
     extern __shared__ double sm[];
     const int ds = d | 1;
-    double* sXi = sm;
-    double* sXj = sm + TB * ds;
-    load_xtile(sXi, xs, ldxs, d, ds, (long long)bm * TB, M);
-    load_xtile(sXj, xs, ldxs, d, ds, (long long)bn * TB, M);
+    const XTile ti = xtile(staged, sm, xs, ldxs, d, (long long)bm * TB, M);
+    const XTile tj = xtile(staged, sm + TB * ds, xs, ldxs, d, (long long)bn * TB, M);
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double mh = 0.0, s2 = 0.0;
@@ -198,7 +215,7 @@ __global__ void __launch_bounds__(NT) gram_full_kernel(const __grid_constant__ K
     for (int rr = 0; rr < 16; ++rr) {
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
             const int c0 = b * 64 + lane * 2;
@@ -207,16 +224,17 @@ __global__ void __launch_bounds__(NT) gram_full_kernel(const __grid_constant__ K
             for (int e = 0; e < 2; ++e) {
                 const int c = c0 + e;
                 const long long gj = (long long)bn * TB + c;
-                const double* xj = sXj + c * ds;
-                double kv;
-                if (FAST) {
-                    double r2 = 0.0;
-                    for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
-                    kv = s2 * exp(mh * r2);
-                } else {
-                    kv = kprog_eval<false>(P, xi, xj, nullptr);
+                const double* xj = tj.row(c);
+                double kv = 0.0;
+                if (gi < M && gj < M) {                    // a padding row is never read
+                    if (FAST) {
+                        double r2 = 0.0;
+                        for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
+                        kv = s2 * exp(mh * r2);
+                    } else {
+                        kv = kprog_eval<false>(P, xi, xj, nullptr);
+                    }
                 }
-                if (gi >= M || gj >= M) kv = 0.0;
                 v[e] = kv;
             }
             *reinterpret_cast<double2*>(Kss + gi * ldk + (long long)bn * TB + c0) = make_double2(v[0], v[1]);
@@ -228,15 +246,14 @@ __global__ void __launch_bounds__(NT) gram_full_kernel(const __grid_constant__ K
 // (/root/reference/src/kernels/kernels.jl:96-131), needed by the cross-validation gradients (src/crossvalidation.jl:67-170, 253-341).
 // Tile row blockIdx.y holds global tile row bm0 + blockIdx.y: a row-sharded handle generates D in row batches (D points at row bm0 * 128).
 __global__ void __launch_bounds__(NT) gram_grad_full_kernel(const __grid_constant__ KProg P, const double* __restrict__ x, long long ldx,
-                                                            long long N, int d, int j, double* __restrict__ D, long long ldd, int bm0) {
+                                                            long long N, int d, int j, double* __restrict__ D, long long ldd, int bm0,
+                                                            int staged) {
     const int bm = bm0 + blockIdx.y, bn = blockIdx.x;
     D += (long long)blockIdx.y * TB * ldd;
     extern __shared__ double sm[];
     const int ds = d | 1;
-    double* sXi = sm;
-    double* sXj = sm + TB * ds;
-    load_xtile(sXi, x, ldx, d, ds, (long long)bm * TB, N);
-    load_xtile(sXj, x, ldx, d, ds, (long long)bn * TB, N);
+    const XTile ti = xtile(staged, sm, x, ldx, d, (long long)bm * TB, N);
+    const XTile tj = xtile(staged, sm + TB * ds, x, ldx, d, (long long)bn * TB, N);
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double gbuf[GPB200_MAX_THETA];
@@ -244,13 +261,13 @@ __global__ void __launch_bounds__(NT) gram_grad_full_kernel(const __grid_constan
     for (int rr = 0; rr < 16; ++rr) {
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
 #pragma unroll 1
         for (int b = 0; b < 4; ++b) {
             const int c = (b >> 1) * 64 + lane * 2 + (b & 1);
             const long long gj = (long long)bn * TB + c;
             double v = 0.0;
-            if (gi < N && gj < N) { kprog_eval<true>(P, xi, sXj + c * ds, gbuf); v = gbuf[j]; }
+            if (gi < N && gj < N) { kprog_eval<true>(P, xi, tj.row(c), gbuf); v = gbuf[j]; }
             D[r * ldd + gj] = v;
         }
     }
@@ -261,14 +278,12 @@ __global__ void __launch_bounds__(NT) gram_grad_full_kernel(const __grid_constan
 __global__ void __launch_bounds__(NT) crossgram_grad_kernel(const __grid_constant__ KProg P, const double* __restrict__ x1,
                                                             long long ldx1, long long N1, const double* __restrict__ x2,
                                                             long long ldx2, long long N2, int d, int j, double* __restrict__ D,
-                                                            long long ldd) {
+                                                            long long ldd, int staged) {
     const int bm = blockIdx.y, bn = blockIdx.x;
     extern __shared__ double sm[];
     const int ds = d | 1;
-    double* sXi = sm;
-    double* sXj = sm + TB * ds;
-    load_xtile(sXi, x1, ldx1, d, ds, (long long)bm * TB, N1);
-    load_xtile(sXj, x2, ldx2, d, ds, (long long)bn * TB, N2);
+    const XTile ti = xtile(staged, sm, x1, ldx1, d, (long long)bm * TB, N1);
+    const XTile tj = xtile(staged, sm + TB * ds, x2, ldx2, d, (long long)bn * TB, N2);
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double gbuf[GPB200_MAX_THETA];
@@ -276,13 +291,13 @@ __global__ void __launch_bounds__(NT) crossgram_grad_kernel(const __grid_constan
     for (int rr = 0; rr < 16; ++rr) {
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
 #pragma unroll 1
         for (int b = 0; b < 4; ++b) {
             const int c = (b >> 1) * 64 + lane * 2 + (b & 1);
             const long long gj = (long long)bn * TB + c;
             double v = 0.0;
-            if (gi < N1 && gj < N2) { kprog_eval<true>(P, xi, sXj + c * ds, gbuf); v = gbuf[j]; }
+            if (gi < N1 && gj < N2) { kprog_eval<true>(P, xi, tj.row(c), gbuf); v = gbuf[j]; }
             D[gi * ldd + gj] = v;
         }
     }
@@ -299,7 +314,8 @@ template <bool FAST>
 __global__ void __launch_bounds__(NT) trace_kernel(const __grid_constant__ KProg P, const double* __restrict__ x,
                                                    long long ldx, int d, long long N, const double* __restrict__ alpha,
                                                    const double* __restrict__ Kinv, long long ldg,
-                                                   double* __restrict__ part, int tiles, int bm_mod, int bm_rem, int bm_div) {
+                                                   double* __restrict__ part, int tiles, int bm_mod, int bm_rem, int bm_div,
+                                                   int staged) {
     // triangular tile index
     const int lin = blockIdx.x;
     int bm = (int)((sqrt(8.0 * (double)lin + 1.0) - 1.0) * 0.5);
@@ -315,13 +331,11 @@ __global__ void __launch_bounds__(NT) trace_kernel(const __grid_constant__ KProg
 
     extern __shared__ double sm[];
     const int ds = d | 1;
-    double* sXi = sm;
-    double* sXj = sXi + TB * ds;
-    double* sAi = sXj + TB * ds;
+    double* sAi = sm + (staged ? 2 * TB * ds : 0);
     double* sAj = sAi + TB;
     double* sRed = sAj + TB;             // [8 warps][np+1]
-    load_xtile(sXi, x, ldx, d, ds, (long long)bm * TB, N);
-    load_xtile(sXj, x, ldx, d, ds, (long long)bn * TB, N);
+    const XTile ti = xtile(staged, sm, x, ldx, d, (long long)bm * TB, N);
+    const XTile tj = xtile(staged, sm + TB * ds, x, ldx, d, (long long)bn * TB, N);
     for (int i = threadIdx.x; i < TB; i += NT) {
         const long long gi = (long long)bm * TB + i, gj = (long long)bn * TB + i;
         sAi[i] = gi < N ? alpha[gi] : 0.0;
@@ -342,7 +356,7 @@ __global__ void __launch_bounds__(NT) trace_kernel(const __grid_constant__ KProg
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
         if (gi >= N) continue;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
         const double ai = sAi[r];
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
@@ -358,7 +372,7 @@ __global__ void __launch_bounds__(NT) trace_kernel(const __grid_constant__ KProg
                 const double kinv = e ? kin.y : kin.x;
                 const double A = ai * sAj[c] - kinv;
                 const double w = (gi == gj) ? 0.5 * A : A;
-                const double* xj = sXj + c * ds;
+                const double* xj = tj.row(c);
                 if (FAST) {
                     double r2 = 0.0;
                     for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
@@ -412,16 +426,14 @@ __global__ void __launch_bounds__(NT) trace_rect_kernel(const __grid_constant__ 
                                                         long long ldx1, long long N1, const double* __restrict__ x2,
                                                         long long ldx2, long long N2, int d,
                                                         const double* __restrict__ W, long long ldw,
-                                                        double* __restrict__ part) {
+                                                        double* __restrict__ part, int staged) {
     const int bm = blockIdx.y, bn = blockIdx.x;
     const int np = P.n_theta;
     extern __shared__ double sm[];
     const int ds = d | 1;
-    double* sXi = sm;
-    double* sXj = sXi + TB * ds;
-    double* sRed = sXj + TB * ds;
-    load_xtile(sXi, x1, ldx1, d, ds, (long long)bm * TB, N1);
-    load_xtile(sXj, x2, ldx2, d, ds, (long long)bn * TB, N2);
+    double* sRed = sm + (staged ? 2 * TB * ds : 0);
+    const XTile ti = xtile(staged, sm, x1, ldx1, d, (long long)bm * TB, N1);
+    const XTile tj = xtile(staged, sm + TB * ds, x2, ldx2, d, (long long)bn * TB, N2);
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double acc[FAST ? 2 : GPB200_MAX_THETA];
@@ -435,7 +447,7 @@ __global__ void __launch_bounds__(NT) trace_rect_kernel(const __grid_constant__ 
         const int r = warp * 16 + rr;
         const long long gi = (long long)bm * TB + r;
         if (gi >= N1) continue;
-        const double* xi = sXi + r * ds;
+        const double* xi = ti.row(r);
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
             const int c0 = b * 64 + lane * 2;
@@ -447,7 +459,7 @@ __global__ void __launch_bounds__(NT) trace_rect_kernel(const __grid_constant__ 
                 const long long gj = gj0 + e;
                 if (gj >= N2) continue;
                 const double w = e ? wv.y : wv.x;
-                const double* xj = sXj + (c0 + e) * ds;
+                const double* xj = tj.row(c0 + e);
                 if (FAST) {
                     double r2 = 0.0;
                     for (int k = 0; k < d; ++k) { const double df = xi[k] - xj[k]; r2 += df * df; }
@@ -549,8 +561,16 @@ __global__ void mirror_lower_tiles_kernel(double* __restrict__ F, long long ld) 
 
 size_t xtile_smem(int d) { return (size_t)2 * TB * (d | 1) * sizeof(double); }
 
+// Dynamic shared memory of a tile kernel: the two staged point tiles plus `extra` bytes of scratch when that fits the
+// device's opt-in limit per block (staged = 1), else the scratch alone, the points then being read in place (staged = 0).
 template <typename K>
-cudaError_t ensure_smem(K kern, size_t bytes) {
+cudaError_t tile_smem(K kern, int d, size_t extra, size_t& bytes, int& staged) {
+    int dev = 0, optin = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (e != cudaSuccess) return e;
+    staged = xtile_smem(d) + extra <= (size_t)optin;
+    bytes = (staged ? xtile_smem(d) : 0) + extra;
     if (bytes > 48 * 1024) return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     return cudaSuccess;
 }
@@ -561,15 +581,17 @@ cudaError_t gram_lower_launch(const KProg& P, const double* x, int64_t ldx, int 
                               const double* noise_var, int64_t n_noise, double nugget, double* G, int64_t ldg,
                               cudaStream_t st, int64_t* launches, int own_tiles, int nranks, int rank, int own_axis, int bm_min) {
     const int T = (int)(Npad / TB);
+    if (T <= 0) return cudaSuccess;
     dim3 grid(T, T);
-    const size_t sm = xtile_smem(d);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if (P.fast) {
-        if ((e = ensure_smem(gram_lower_kernel<true>, sm)) != cudaSuccess) return e;
-        gram_lower_kernel<true><<<grid, NT, sm, st>>>(P, x, ldx, d, N, Npad, noise_var, n_noise, nugget, G, ldg, own_tiles, nranks, rank, own_axis, bm_min);
+    if (kprog_fast(P, d)) {
+        if ((e = tile_smem(gram_lower_kernel<true>, d, 0, sm, stg)) != cudaSuccess) return e;
+        gram_lower_kernel<true><<<grid, NT, sm, st>>>(P, x, ldx, d, N, Npad, noise_var, n_noise, nugget, G, ldg, own_tiles, nranks, rank, own_axis, bm_min, stg);
     } else {
-        if ((e = ensure_smem(gram_lower_kernel<false>, sm)) != cudaSuccess) return e;
-        gram_lower_kernel<false><<<grid, NT, sm, st>>>(P, x, ldx, d, N, Npad, noise_var, n_noise, nugget, G, ldg, own_tiles, nranks, rank, own_axis, bm_min);
+        if ((e = tile_smem(gram_lower_kernel<false>, d, 0, sm, stg)) != cudaSuccess) return e;
+        gram_lower_kernel<false><<<grid, NT, sm, st>>>(P, x, ldx, d, N, Npad, noise_var, n_noise, nugget, G, ldg, own_tiles, nranks, rank, own_axis, bm_min, stg);
     }
     if (launches) ++*launches;
     return cudaGetLastError();
@@ -577,15 +599,17 @@ cudaError_t gram_lower_launch(const KProg& P, const double* x, int64_t ldx, int 
 
 cudaError_t crossgram_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, const double* x,
                              int64_t ldx, int64_t N, int64_t Npad, int d, double* Kst, int64_t ldk, cudaStream_t st, int64_t* launches) {
+    if (Mpad < TB || Npad < TB) return cudaSuccess;
     dim3 grid((unsigned)(Npad / TB), (unsigned)(Mpad / TB));
-    const size_t sm = xtile_smem(d);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if (P.fast) {
-        if ((e = ensure_smem(crossgram_kernel<true>, sm)) != cudaSuccess) return e;
-        crossgram_kernel<true><<<grid, NT, sm, st>>>(P, xs, ldxs, M, x, ldx, N, d, Kst, ldk);
+    if (kprog_fast(P, d)) {
+        if ((e = tile_smem(crossgram_kernel<true>, d, 0, sm, stg)) != cudaSuccess) return e;
+        crossgram_kernel<true><<<grid, NT, sm, st>>>(P, xs, ldxs, M, x, ldx, N, d, Kst, ldk, stg);
     } else {
-        if ((e = ensure_smem(crossgram_kernel<false>, sm)) != cudaSuccess) return e;
-        crossgram_kernel<false><<<grid, NT, sm, st>>>(P, xs, ldxs, M, x, ldx, N, d, Kst, ldk);
+        if ((e = tile_smem(crossgram_kernel<false>, d, 0, sm, stg)) != cudaSuccess) return e;
+        crossgram_kernel<false><<<grid, NT, sm, st>>>(P, xs, ldxs, M, x, ldx, N, d, Kst, ldk, stg);
     }
     if (launches) ++*launches;
     return cudaGetLastError();
@@ -593,27 +617,30 @@ cudaError_t crossgram_launch(const KProg& P, const double* xs, int64_t ldxs, int
 
 cudaError_t gram_full_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, int d,
                              double* Kss, int64_t ldk, cudaStream_t st, int64_t* launches) {
+    if (Mpad < TB) return cudaSuccess;
     dim3 grid((unsigned)(Mpad / TB), (unsigned)(Mpad / TB));
-    const size_t sm = xtile_smem(d);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if (P.fast) {
-        if ((e = ensure_smem(gram_full_kernel<true>, sm)) != cudaSuccess) return e;
-        gram_full_kernel<true><<<grid, NT, sm, st>>>(P, xs, ldxs, M, d, Kss, ldk);
+    if (kprog_fast(P, d)) {
+        if ((e = tile_smem(gram_full_kernel<true>, d, 0, sm, stg)) != cudaSuccess) return e;
+        gram_full_kernel<true><<<grid, NT, sm, st>>>(P, xs, ldxs, M, d, Kss, ldk, stg);
     } else {
-        if ((e = ensure_smem(gram_full_kernel<false>, sm)) != cudaSuccess) return e;
-        gram_full_kernel<false><<<grid, NT, sm, st>>>(P, xs, ldxs, M, d, Kss, ldk);
+        if ((e = tile_smem(gram_full_kernel<false>, d, 0, sm, stg)) != cudaSuccess) return e;
+        gram_full_kernel<false><<<grid, NT, sm, st>>>(P, xs, ldxs, M, d, Kss, ldk, stg);
     }
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 
 cudaError_t kdiag_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, double* out, cudaStream_t st, int64_t* launches) {
+    if (M <= 0) return cudaSuccess;
     kdiag_kernel<<<(unsigned)((M + 127) / 128), 128, 0, st>>>(P, xs, ldxs, M, out);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-int trace_num_acc(const KProg& P) { return P.fast ? 3 : P.n_theta + 1; }
+int trace_num_acc(const KProg& P, int d) { return kprog_fast(P, d) ? 3 : P.n_theta + 1; }
 
 cudaError_t trace_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad,
                          const double* alpha, const double* Kinv, int64_t ldg, double* part, double* out,
@@ -621,15 +648,18 @@ cudaError_t trace_launch(const KProg& P, const double* x, int64_t ldx, int d, in
     if (bm_div < 1) bm_div = 1;
     const int T = (int)(Npad / TB);
     const int tiles = T * (T + 1) / 2;
-    const int nacc = trace_num_acc(P);
-    const size_t sm = xtile_smem(d) + (size_t)(2 * TB + 8 * nacc) * sizeof(double);
+    const int nacc = trace_num_acc(P, d);
+    if (tiles <= 0) return cudaMemsetAsync(out, 0, sizeof(double) * nacc, st);
+    const size_t extra = (size_t)(2 * TB + 8 * nacc) * sizeof(double);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if (P.fast) {
-        if ((e = ensure_smem(trace_kernel<true>, sm)) != cudaSuccess) return e;
-        trace_kernel<true><<<tiles, NT, sm, st>>>(P, x, ldx, d, N, alpha, Kinv, ldg, part, tiles, bm_mod, bm_rem, bm_div);
+    if (kprog_fast(P, d)) {
+        if ((e = tile_smem(trace_kernel<true>, d, extra, sm, stg)) != cudaSuccess) return e;
+        trace_kernel<true><<<tiles, NT, sm, st>>>(P, x, ldx, d, N, alpha, Kinv, ldg, part, tiles, bm_mod, bm_rem, bm_div, stg);
     } else {
-        if ((e = ensure_smem(trace_kernel<false>, sm)) != cudaSuccess) return e;
-        trace_kernel<false><<<tiles, NT, sm, st>>>(P, x, ldx, d, N, alpha, Kinv, ldg, part, tiles, bm_mod, bm_rem, bm_div);
+        if ((e = tile_smem(trace_kernel<false>, d, extra, sm, stg)) != cudaSuccess) return e;
+        trace_kernel<false><<<tiles, NT, sm, st>>>(P, x, ldx, d, N, alpha, Kinv, ldg, part, tiles, bm_mod, bm_rem, bm_div, stg);
     }
     if (launches) ++*launches;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
@@ -643,16 +673,19 @@ cudaError_t trace_rect_launch(const KProg& P, const double* x1, int64_t ldx1, in
                               int64_t N2, int d, const double* W, int64_t ldw, double* part, double* tmp_out,
                               cudaStream_t st, int64_t* launches) {
     const int tm = (int)((N1 + TB - 1) / TB), tn = (int)((N2 + TB - 1) / TB);
-    const int nacc = P.fast ? 2 : P.n_theta;
-    const size_t sm = xtile_smem(d) + (size_t)(8 * nacc) * sizeof(double);
+    const int nacc = kprog_fast(P, d) ? 2 : P.n_theta;
+    if (tm <= 0 || tn <= 0) return cudaMemsetAsync(tmp_out, 0, sizeof(double) * nacc, st);
+    const size_t extra = (size_t)(8 * nacc) * sizeof(double);
     dim3 grid(tn, tm);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if (P.fast) {
-        if ((e = ensure_smem(trace_rect_kernel<true>, sm)) != cudaSuccess) return e;
-        trace_rect_kernel<true><<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part);
+    if (kprog_fast(P, d)) {
+        if ((e = tile_smem(trace_rect_kernel<true>, d, extra, sm, stg)) != cudaSuccess) return e;
+        trace_rect_kernel<true><<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part, stg);
     } else {
-        if ((e = ensure_smem(trace_rect_kernel<false>, sm)) != cudaSuccess) return e;
-        trace_rect_kernel<false><<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part);
+        if ((e = tile_smem(trace_rect_kernel<false>, d, extra, sm, stg)) != cudaSuccess) return e;
+        trace_rect_kernel<false><<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part, stg);
     }
     if (launches) ++*launches;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
@@ -662,6 +695,7 @@ cudaError_t trace_rect_launch(const KProg& P, const double* x1, int64_t ldx1, in
 }
 cudaError_t kdiag_grad_launch(const KProg& P, const double* x, int64_t ldx, int64_t N, const double* gvec, double* out,
                               cudaStream_t st, int64_t* launches) {
+    if (N <= 0) return cudaSuccess;
     kdiag_grad_kernel<<<(unsigned)((N + 127) / 128), 128, 0, st>>>(P, x, ldx, N, gvec, out);
     if (launches) ++*launches;
     return cudaGetLastError();
@@ -672,12 +706,13 @@ cudaError_t gram_grad_full_launch(const KProg& P, const double* x, int64_t ldx, 
     if (j < 0 || j >= P.n_theta) return cudaErrorInvalidValue;
     if (rows < 0) rows = Npad - row0;
     if (row0 < 0 || row0 % TB || rows % TB || row0 + rows > Npad) return cudaErrorInvalidValue;
-    if (rows == 0) return cudaSuccess;
+    if (rows == 0 || Npad < TB) return cudaSuccess;
     dim3 grid((unsigned)(Npad / TB), (unsigned)(rows / TB));
-    const size_t sm = xtile_smem(d);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if ((e = ensure_smem(gram_grad_full_kernel, sm)) != cudaSuccess) return e;
-    gram_grad_full_kernel<<<grid, NT, sm, st>>>(P, x, ldx, N, d, j, D, ldd, (int)(row0 / TB));
+    if ((e = tile_smem(gram_grad_full_kernel, d, 0, sm, stg)) != cudaSuccess) return e;
+    gram_grad_full_kernel<<<grid, NT, sm, st>>>(P, x, ldx, N, d, j, D, ldd, (int)(row0 / TB), stg);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
@@ -686,11 +721,13 @@ cudaError_t crossgram_grad_launch(const KProg& P, const double* x1, int64_t ldx1
                                   int64_t ldx2, int64_t N2, int64_t N2pad, int d, int j, double* D, int64_t ldd, cudaStream_t st,
                                   int64_t* launches) {
     if (j < 0 || j >= P.n_theta || N1pad % TB || N2pad % TB) return cudaErrorInvalidValue;
+    if (N1pad < TB || N2pad < TB) return cudaSuccess;
     dim3 grid((unsigned)(N2pad / TB), (unsigned)(N1pad / TB));
-    const size_t sm = xtile_smem(d);
+    size_t sm;
+    int stg;
     cudaError_t e;
-    if ((e = ensure_smem(crossgram_grad_kernel, sm)) != cudaSuccess) return e;
-    crossgram_grad_kernel<<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, j, D, ldd);
+    if ((e = tile_smem(crossgram_grad_kernel, d, 0, sm, stg)) != cudaSuccess) return e;
+    crossgram_grad_kernel<<<grid, NT, sm, st>>>(P, x1, ldx1, N1, x2, ldx2, N2, d, j, D, ldd, stg);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

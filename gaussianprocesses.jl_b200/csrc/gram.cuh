@@ -15,8 +15,8 @@ cudaError_t crossgram_launch(const KProg& P, const double* xs, int64_t ldxs, int
 cudaError_t gram_full_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, int64_t Mpad, int d,
                              double* Kss, int64_t ldk, cudaStream_t st, int64_t* launches);
 cudaError_t kdiag_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, double* out, cudaStream_t st, int64_t* launches);
-// number of accumulators per tile: n_theta + 1 (last = tr(A))
-int trace_num_acc(const KProg& P);
+// number of accumulators per tile: n_theta + 1 (last = tr(A)); 3 for the specialised SEIso program (kprog_fast)
+int trace_num_acc(const KProg& P, int d);
 // part: [tiles][nacc] scratch; out: [nacc] = {dmll_kernel[0..n_theta), tr(A)}
 cudaError_t trace_launch(const KProg& P, const double* x, int64_t ldx, int d, int64_t N, int64_t Npad,
                          const double* alpha, const double* Kinv, int64_t ldg, double* part, double* out,

@@ -12,7 +12,7 @@
 struct KProg {
     int n_ops;
     int n_theta;
-    int fast;                        // 1: single SEIso leaf over dims 0..nd-1 (specialised kernels)
+    int fast;                        // 1: single SEIso leaf over dims 0..nd-1 (see kprog_fast)
     int pad_;
     int op[GPB200_MAX_OPS];
     int toff[GPB200_MAX_OPS];
@@ -24,6 +24,10 @@ struct KProg {
     int dims[GPB200_MAX_DIMS];
     double par[GPB200_MAX_THETA];    // transformed parameters (host: exp of the log-scale theta)
 };
+
+// The specialised SEIso kernels apply when the program is one SEIso leaf over every input dimension in order.  P.fast
+// records the first part from the program alone; d is the input dimension of the points the launch reads.
+static inline bool kprog_fast(const KProg& P, int d) { return P.fast && P.nd[0] == d; }
 
 // Host-side transform theta (log scale) -> par (natural scale), mirrors the constructors
 // (se_iso.jl:10 SEIso(ll,lσ) = (exp(2ll), exp(2lσ)); se_ard.jl:13 iℓ2 = exp(-2ll); mat12_iso.jl:12

@@ -64,6 +64,7 @@ _SIGNATURES = {
     "gpb200_gpa_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
     "gpb200_row_reductions": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
     "gpb200_fsa_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
+    "gpb200_gram_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_fitc_cv_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "gpb200_ipc_export": (C.c_int, [_H, C.c_void_p]),
@@ -461,6 +462,17 @@ class Engine:
         f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
         self._check(self._lib.gpb200_fsa_kernels(self._h, self.FSA_KERNELS.index(name), a.ctypes.data_as(_lp), a.size,
                                                  _as_dp(f), f.size), "fsa_kernels")
+
+    GRAM_KERNELS = ("gram_lower", "crossgram", "gram_full", "kdiag", "gram_grad_full", "crossgram_grad", "trace",
+                    "trace_rect", "kdiag_grad", "crossgram_dx", "mirror_lower_tiles")
+
+    def gram_kernels(self, name, args, fargs=()):
+        """One dense Gram-family kernel (include/gpb200.h) by name, on device buffers: args = the int64 arguments,
+        fargs = theta (and the nugget or c)."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
+        self._check(self._lib.gpb200_gram_kernels(self._h, self.GRAM_KERNELS.index(name), a.ctypes.data_as(_lp), a.size,
+                                                  _as_dp(f), f.size), "gram_kernels")
 
     def fitc_cv_kernels(self, name, args, fargs=()):
         """One sparse cross-validation row kernel or FITC element kernel (include/gpb200.h) by name, on device buffers."""

@@ -299,6 +299,33 @@ int  gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int
  * pointer the kernel dereferences, a negative size or row, a bad mode, an item ld < 128, lda < K, ld < ncols.
  * GPB200_ESTATE: a kernel-program call before gpb200_set_kernel.                                                    */
 int  gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
+/* The dense Gram-family kernels (csrc/gram.cuh), synchronous, one call of the existing launch wrapper each, on device
+ * buffers (row-major, leading dimensions in doubles).  The kernels that evaluate the kernel program use the program of
+ * the last gpb200_set_kernel at fargs = log-scale theta (n_theta entries); the handle's own theta and factor are left
+ * alone.  A size of 0 launches nothing (trace and trace_rect then zero their outputs).
+ *   which 0  gram_lower         : x, ldx, d, N, Npad, noise_var, n_noise, G, ldg, own_tiles, nranks, rank, own_axis, bm_min
+ *                                 fargs = theta, nugget
+ *   which 1  crossgram          : xs, ldxs, M, Mpad, x, ldx, N, Npad, d, Kst, ldk
+ *   which 2  gram_full          : xs, ldxs, M, Mpad, d, Kss, ldk
+ *   which 3  kdiag              : xs, ldxs, d, M, out
+ *   which 4  gram_grad_full     : x, ldx, d, N, Npad, j, D, ldd, row0, rows
+ *   which 5  crossgram_grad     : x1, ldx1, N1, N1pad, x2, ldx2, N2, N2pad, d, j, D, ldd
+ *   which 6  trace (+ reduce)   : x, ldx, d, N, Npad, alpha, Kinv, ldg, part, out, bm_mod, bm_rem, bm_div
+ *                                 (out: n_theta + 1 entries, 3 for a single SEIso leaf over all d dimensions)
+ *   which 7  trace_rect         : x1, ldx1, N1, x2, ldx2, N2, d, W, ldw, part, out
+ *                                 (out: n_theta entries, 2 for a single SEIso leaf over all d dimensions)
+ *   which 8  kdiag_grad         : x, ldx, d, N, g, out                                   (out[p * N + i])
+ *   which 9  crossgram_dx       : xs, ldxs, M, z, ldz, n, d, a, W1 (0 = none), W2 (0 = none), ldw, dmu, dvar
+ *                                 fargs = theta, c
+ *   which 10 mirror_lower_tiles : F, ld, Npad                                            (no fargs)
+ * GPB200_EINVAL, nothing launched: bad which / n / nf, theta not of n_theta entries, d outside 1 .. GPB200_MAX_DIMS, a
+ * program dimension >= d, a null pointer (W1, W2 and, without them, dvar may be null), a negative size, a padded size
+ * that is not a multiple of 128 or is below its size, a leading dimension below the row width, an odd leading dimension
+ * or a pointer not 16-byte aligned for G, Kst, Kss, Kinv and W, j outside [0, n_theta), bad ownership arguments
+ * (nranks >= 1, 0 <= rank < nranks, own_axis 0 or 1; bm_mod, bm_div >= 1, 0 <= bm_rem < bm_mod), row0 or rows not a
+ * multiple of 128 or past Npad.
+ * GPB200_ESTATE: a kernel-program call before gpb200_set_kernel.                                                    */
+int  gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
 /* The sparse cross-validation row kernels (csrc/fitc_cv.cuh) and the FITC element kernels that run between the same
  * GEMMs (csrc/vec.cuh), synchronous, one launch each through its wrapper (sizes <= 0 launch nothing):
  *   which 0  delta      : kind, x, ldx, d, j, G, C, ld, ncols, nrows, rows_pad, alpha, delta, da   fargs = theta
