@@ -204,6 +204,12 @@ struct gpb200_fitc {
     double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
     double fsag_ms[4] = {0, 0, 0, 0};                 // last predict_fsa_grad, summed over test chunks: predict_fsa's
                                                       // launches, s + second sweep, K_uu^-1 TRSMs, contraction
+    // inducing-point gradient (gpb200_fitc_grad_kernel_inducing; first use): dmll/dXu accumulator (M x d), the events
+    // around the call (0, 1) and around each contraction launch (2k, 2k + 1 for k >= 1), and the device times of the last
+    // call: the contractions summed, the whole call
+    double* dxu = nullptr;
+    std::vector<cudaEvent_t> xu_ev;
+    double xu_ms[2] = {0, 0};
     // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
     // buffer the likelihood, gradient and prediction schedules keep):
     //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
@@ -2642,8 +2648,8 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
 }
 
 int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
-    if (!h || !args || which < 0 || which > 13 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
-    static const int want[14] = {14, 14, 4, 8, 5, 5, 10, 6, 5, 6, 5, 9, 7, 3};
+    if (!h || !args || which < 0 || which > 14 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    static const int want[15] = {14, 14, 4, 8, 5, 5, 10, 6, 5, 6, 5, 9, 7, 3, 13};
     if (n != want[which]) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: wrong argument count for this kernel");
     const int64_t* a = args;
     auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
@@ -2655,8 +2661,12 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
     if (which == 0) {
         // kind, x, ldx, d, j, G, C, ld, ncols, nrows, rows_pad, alpha, delta, da
         TRY(local_prog(h, "fitc_cv_kernels", fargs, nf, a[3], P));
+    } else if (which == 14) {
+        // u, ldu, M, z, ldz, n, d, W, ldw, sym, mask, out, accumulate
+        if (a[6] > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: d exceeds GPB200_MAX_DIMS");
+        TRY(local_prog(h, "fitc_cv_kernels", fargs, nf, a[6], P));
     } else if (nf != 0) {
-        return fail(h, GPB200_EINVAL, "fitc_cv_kernels: fargs = theta for delta, none otherwise");
+        return fail(h, GPB200_EINVAL, "fitc_cv_kernels: fargs = theta for delta and inducing_dx, none otherwise");
     }
     bool ok = true;
     switch (which) {
@@ -2678,6 +2688,8 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
     case 11: ok = need({0, 1, 5, 6, 7, 8}) && a[3] >= 0 && a[4] >= 0 && a[2] >= a[4]; break;   // fitc_wfu: P2, P1, ld, nrows, ncols, alpha, lam, g, beta
     case 12: ok = need({0, 1, 2, 3, 6}) && a[5] >= 0 && a[4] >= a[5]; break;          // fitc_wuu: Wuu, T, Kinv, Sinv, ld, n, beta
     case 13: ok = need({0}) && a[2] >= 0 && a[1] >= a[2]; break;                       // symmetrize: A, ld, n
+    case 14: ok = need({0, 3, 7, 11}) && a[2] >= 0 && a[5] >= 0 && a[1] >= a[6] && a[4] >= a[6] && a[8] >= a[2] &&
+                  (a[9] == 0 || (a[9] == 1 && a[5] == a[2])) && (a[12] == 0 || a[12] == 1); break;
     }
     if (!ok) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: a null pointer, a negative size, a bad mode or ld below the row width");
     CK(cudaSetDevice(h->device));
@@ -2702,6 +2714,8 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
     case 11: e = fitc_wfu_launch(ptr(0), ptr(1), a[2], a[3], a[4], ptr(5), ptr(6), ptr(7), ptr(8), st, L); break;
     case 12: e = fitc_wuu_launch(ptr(0), ptr(1), ptr(2), ptr(3), a[4], a[5], ptr(6), st, L); break;
     case 13: e = symmetrize_launch(ptr(0), a[1], a[2], st, L); break;
+    case 14: e = inducing_dx_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], (int)a[6], ptr(7), a[8], (int)a[9], ptr(10), ptr(11),
+                                    (int)a[12], st, L); break;
     }
     CK(e);
     CK(cudaStreamSynchronize(st));
@@ -2861,7 +2875,8 @@ static int fsa_check(gpb200_fitc* f, const char* who);
 static int fsa_factorize(gpb200_fitc* f);
 static int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, double* mll, double* logdet);
 static int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise);
-static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel);
+static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu);
+static size_t fsa_num_chunks(const gpb200_fitc* f);
 
 // cross-validation workspace (gpb200_fitc_cv_*): it depends on N, Nc and Mpad only
 static void fitc_cv_free(gpb200_fitc* f) {
@@ -2893,9 +2908,11 @@ void gpb200_fitc_destroy(gpb200_fitc* f) {
     if (f->eu && f->eu->st) cudaStreamSynchronize(f->eu->st);
     double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
                        &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
-                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx};
+                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx,
+                       &f->dxu};
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     if (f->Kss) cudaFree(f->Kss);
+    for (cudaEvent_t e : f->xu_ev) cudaEventDestroy(e);
     fsa_free(f);
     fitc_cv_free(f);
     if (f->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(f->comm);
@@ -2931,7 +2948,8 @@ int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, 
     cudaStream_t st = f->eu->st;
     double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
                        &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
-                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx};
+                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx,
+                       &f->dxu};
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     f->grad_ws = false;
     fsa_free(f);                                      // the FSA blocks refer to the old observations
@@ -3286,10 +3304,55 @@ int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
 // with S = Sigma_QR, L = Lambda; uses Sigma^-1 K_fu K_uu^-1 = L^-1 K_fu S^-1 and
 // K_uu^-1 K_uf Sigma^-1 K_fu K_uu^-1 = K_uu^-1 - S^-1 (both follow from S = K_uu + K_uf L^-1 K_fu).
 // All O(M^2 N) work is NT GEMMs against the explicit M x M inverses (grad_prepare of the sub-engines).
-int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
-    if (!f || !dmll_kernel) return GPB200_EINVAL;
-    if (!f->factored || !f->alpha_ready) { f->err = "fitc_grad_kernel: factorize and mll first"; return GPB200_ESTATE; }
+//
+// Inducing points (dmll_xu != null, gpb200_fitc_grad_kernel_inducing): moving u_j changes K_fu and K_uu only (k_ii and the
+// FSA blocks K_bb do not depend on Xu), so the same adjoints give
+//   dmll/du_j = 1/2 [ sum_i W_fu[i, j] dk(u_j, x_i)/du_j + sum_l (W_uu[j, l] + W_uu[l, j]) dk(u_j, u_l)/du_j ]
+// (W_uu is not exactly symmetric: it comes from two GEMMs).  One inducing_dx launch per chunk reads W_fu where
+// trace_rect reads it and accumulates into f->dxu in chunk order; one more after the chunk loop contracts W_uu + W_uu'.
+// Without dmll_xu the launches are exactly those of the kernel gradient alone; with it, they are the same launches plus
+// the contractions (and, on several ranks, one all-reduce of the M x d partial), which read and write nothing else.
+static int xu_event_pairs(gpb200_fitc* f, size_t pairs) {
+    while (f->xu_ev.size() < 2 * pairs) {
+        cudaEvent_t e;
+        FCK(cudaEventCreate(&e));
+        f->xu_ev.push_back(e);
+    }
+    return GPB200_OK;
+}
+
+// one contraction launch (slot k >= 1 of f->xu_ev) over n rows z against W (ld Mpad) into f->dxu
+static int xu_contract(gpb200_fitc* f, size_t k, const double* z, int64_t n, const double* W, int sym, const double* mask,
+                       int accumulate) {
+    gpb200_handle* eu = f->eu;
+    FCK(cudaEventRecord(f->xu_ev[2 * k], eu->st));
+    FCK(inducing_dx_launch(eu->prog, eu->x, f->d, f->M, z, f->d, n, f->d, W, f->Mpad, sym, mask, f->dxu, accumulate, eu->st,
+                           &eu->launches));
+    FCK(cudaEventRecord(f->xu_ev[2 * k + 1], eu->st));
+    return GPB200_OK;
+}
+
+// after the final synchronize: device times of the call and of its k_used contractions; dmll_xu = dxu / 2
+static int xu_finish(gpb200_fitc* f, size_t k_used, double* dmll_xu) {
+    std::vector<double> h((size_t)f->M * f->d);
+    FCK(cudaMemcpy(h.data(), f->dxu, sizeof(double) * h.size(), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < h.size(); ++i) dmll_xu[i] = 0.5 * h[i];
+    double c = 0.0;
+    for (size_t k = 1; k <= k_used; ++k) c += ev_ms(f->xu_ev[2 * k], f->xu_ev[2 * k + 1]);
+    f->xu_ms[0] = c;
+    f->xu_ms[1] = ev_ms(f->xu_ev[0], f->xu_ev[1]);
+    return GPB200_OK;
+}
+
+static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, const char* who) {
+    if (!f->factored || !f->alpha_ready) { f->err = std::string(who) + ": factorize and mll first"; return GPB200_ESTATE; }
     FCK(cudaSetDevice(f->device));
+    if (dmll_xu) {
+        const size_t chunks = f->mode == 3 ? fsa_num_chunks(f) : (size_t)((f->N + f->Nc - 1) / f->Nc);
+        TRY(xu_event_pairs(f, chunks + 2));
+        if (!f->dxu) FCK(cudaMalloc(&f->dxu, sizeof(double) * f->M * f->d));
+        FCK(cudaEventRecord(f->xu_ev[0], f->eu->st));
+    }
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int np = eu->prog.n_theta;
@@ -3334,7 +3397,8 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     FCK(solve_device(eu, f->rhsm, f->tmpm, f->betav));
     FCK(cudaMemsetAsync(f->gacc, 0, sizeof(double) * GPB200_MAX_THETA, st));
     FCK(cudaMemsetAsync(f->Hbuf, 0, sizeof(double) * Mp * Mp, st));
-    if (f->mode == 3) return fsa_grad_kernel(f, dmll_kernel);
+    if (f->mode == 3) return fsa_grad_kernel(f, dmll_kernel, dmll_xu);
+    size_t xk = 0;                                                        // contraction launches so far
     for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
         const int64_t nc = std::min(Nc, f->N - r0);
         const double* xr = f->x + r0 * f->d;
@@ -3359,6 +3423,7 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
         FCK(fitc_wfu_launch(f->bufB, f->bufC, Mp, nc, f->M, f->alpha + r0, f->lam + r0, f->gvec + r0, f->betav, st, &eu->launches));
         FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufB, Mp, f->gpart, f->gtmp, st, &eu->launches));
         FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufB, 0, nullptr, xk > 0)); ++xk; }
         if (f->mode != 0) continue;                                       // no Lambda-derivative terms for SoR / DTC
         // diagonal term sum_i g_i dK_ii/dθ_p (scratch: bufC as np x nc)
         FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->gvec + r0, f->bufC, st, &eu->launches));
@@ -3380,6 +3445,7 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     // multi-GPU: the per-row traces and H = K_uf diag(g) K_fu are sums over the ranks' rows; the M x M part below is replicated
     { int rca = fitc_allreduce(f, f->gacc, (size_t)np); if (rca) return rca; }
     { int rca = fitc_allreduce(f, f->Hbuf, (size_t)Mp * (size_t)Mp); if (rca) return rca; }
+    if (dmll_xu) { int rca = fitc_allreduce(f, f->dxu, (size_t)f->M * f->d); if (rca) return rca; }   // W_fu part over all rows
     {   // T = K_uu^-1 H ; Wbuf = K_uu^-1 T' = K_uu^-1 H K_uu^-1
         GemmDesc g = gemm_desc_default();
         g.A = GemmOperand{bufG(eu), bufNone(), 0, 0};
@@ -3393,11 +3459,43 @@ int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     FCK(fitc_wuu_launch(f->Wbuf, f->Wbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
     FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
     FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+    if (dmll_xu) {
+        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, 1)); ++xk;
+        FCK(cudaEventRecord(f->xu_ev[1], st));
+    }
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta above
-    for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
+    if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
+    if (dmll_xu) TRY(xu_finish(f, xk, dmll_xu));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
+    if (!f || !dmll_kernel) return GPB200_EINVAL;
+    return fitc_grad(f, dmll_kernel, nullptr, "fitc_grad_kernel");
+}
+
+int gpb200_fitc_grad_kernel_inducing(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
+    if (!f) return GPB200_EINVAL;
+    if (!dmll_xu) { f->err = "fitc_grad_kernel_inducing: dmll_xu is required"; return GPB200_EINVAL; }
+    return fitc_grad(f, dmll_kernel, dmll_xu, "fitc_grad_kernel_inducing");
+}
+
+// Replaces the inducing inputs of both sub-engines in place (same M and d: no buffer is reallocated); the training inputs,
+// the kernel program, the FSA blocks and every workspace are kept.  The factorisation, alpha and the cross-validation state
+// refer to the old Xu and are invalidated.
+int gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_t ldxu) {
+    if (!f) return GPB200_EINVAL;
+    if (!f->has_data) { f->err = "fitc_set_inducing: set_data first"; return GPB200_ESTATE; }
+    if (M != f->M || !xu || ldxu < f->d) {
+        f->err = "fitc_set_inducing: M must be set_data's, xu non-null and ldxu >= d"; return GPB200_EINVAL;
+    }
+    FCK(cudaSetDevice(f->device));
+    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    FSUB(gpb200_set_data(f->eu, M, f->d, xu, ldxu), f->eu);
+    FSUB(gpb200_set_data(f->es, M, f->d, xu, ldxu), f->es);
     return GPB200_OK;
 }
 
@@ -3692,6 +3790,8 @@ struct Fsa {
     FsaDxItem* pdi = nullptr;
     size_t pdx_cap = 0, pdi_cap = 0;
 };
+
+static size_t fsa_num_chunks(const gpb200_fitc* f) { return f->fsa ? f->fsa->chunks.size() : 0; }
 
 static void fsa_free(gpb200_fitc* f) {
     if (!f->fsa) return;
@@ -4092,7 +4192,7 @@ static int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise) {
 //   W_uu = -beta beta' + K_uu^-1 - S^-1 + K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
 // since dSigma = dQ + blockdiag(dK - dQ) and <alpha alpha' - Sigma^-1, blockdiag(D)> = <G_bd, D>.  Called by
 // gpb200_fitc_grad_kernel once K_uu^-1, S^-1 (full symmetric, sub-engines' G) and beta are in place, gacc and Hbuf zeroed.
-static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
+static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
     Fsa* s = f->fsa;
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
@@ -4103,6 +4203,7 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     GemmBuf bAt{tma ? &s->mapWt : nullptr, f->bufA, Nc};        // bufA as Mpad x Nc
     GemmBuf bB2{tma ? &f->mapB2 : nullptr, f->bufB, Mp};        // bufB as Nc x Mpad
     GemmBuf bBt{tma ? &f->mapB : nullptr, f->bufB, Nc};         // bufB as Mpad x Nc
+    size_t xk = 0;                                                // inducing-point contractions so far
     for (const FsaChunk& ch : s->chunks) {
         const double* xr = s->xb + ch.r0 * f->d;
         const int64_t nc = ch.rows;
@@ -4140,6 +4241,8 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
         FCK(fsa_axpy_t_launch(f->bufC, Mp, f->bufA, Nc, nc, Mp, -2.0, st, &eu->launches));
         FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufC, Mp, f->gpart, f->gtmp, st, &eu->launches));
         FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        // dmll/dXu: the padding rows of the chunk are skipped (mask 0); Xu is in the caller's order (never permuted)
+        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufC, 0, s->mask + ch.r0, xk > 0)); ++xk; }
         {   // H += P1' G_bd P1 = K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bBt, bufNone(), 0, 0};
@@ -4152,11 +4255,16 @@ static int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     FCK(fitc_wuu_launch(f->Wbuf, f->Hbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
     FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
     FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+    if (dmll_xu) {
+        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, xk > 0)); ++xk;
+        FCK(cudaEventRecord(f->xu_ev[1], st));
+    }
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta in gpb200_fitc_grad_kernel
-    for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
+    if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
+    if (dmll_xu) TRY(xu_finish(f, xk, dmll_xu));
     return GPB200_OK;
 }
 
@@ -4609,6 +4717,7 @@ int gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n) {
     if (!f || !ms || n < 0) return GPB200_EINVAL;
     for (int32_t i = 0; i < n && i < 3; ++i) ms[i] = f->rand_ms[i];
     for (int32_t i = 3; i < n && i < 7; ++i) ms[i] = f->fsag_ms[i - 3];
+    for (int32_t i = 7; i < n && i < 9; ++i) ms[i] = f->xu_ms[i - 7];
     return GPB200_OK;
 }
 

@@ -548,6 +548,44 @@ __global__ void __launch_bounds__(DX_NT) crossgram_dx_kernel(const __grid_consta
     }
 }
 
+// inducing-point gradient of the sparse mll, one CTA per inducing point j (u_j staged in shared memory):
+//   out[j, :] (=, or += when accumulate) sum_i W(i, j) dk(u_j, z_i)/du_j,   W(i, j) = W[i * ldw + j] (+ W[j * ldw + i] if sym)
+// W is read in place down column j (the adjoint W_fu of a chunk, Nc x Mpad, or W_uu with sym = W_uu + W_uu').  Rows with
+// mask[i] == 0 (FSA padding) are skipped, not weighted by 0.  Thread t takes i = t, t + DX_NT, ... in order and every
+// coordinate is summed over the threads by one fixed tree (crossgram_dx_kernel's order), so a launch's sum does not
+// depend on the grid; accumulate adds it to out in launch order.
+__global__ void __launch_bounds__(DX_NT) inducing_dx_kernel(const __grid_constant__ KProg P, const double* __restrict__ u,
+                                                            long long ldu, const double* __restrict__ z, long long ldz,
+                                                            long long n, int d, const double* __restrict__ W, long long ldw,
+                                                            int sym, const double* __restrict__ mask,
+                                                            double* __restrict__ out, int accumulate) {
+    __shared__ double su[GPB200_MAX_DIMS];
+    __shared__ double red[DX_NT];
+    const long long j = blockIdx.x;
+    const int t = threadIdx.x;
+    for (int k = t; k < d; k += DX_NT) su[k] = u[j * ldu + k];
+    __syncthreads();
+    double g[GPB200_MAX_DIMS];
+    for (int k = 0; k < d; ++k) g[k] = 0.0;
+    const double* wc = W + j;
+    const double* wr = W + j * ldw;
+    for (long long i = t; i < n; i += DX_NT) {
+        if (mask && mask[i] == 0.0) continue;
+        const double wi = sym ? wc[i * ldw] + wr[i] : wc[i * ldw];
+        kprog_eval_dx(P, su, z + i * ldz, wi, g, 0.0, nullptr);
+    }
+    for (int k = 0; k < d; ++k) {
+        red[t] = g[k];
+        __syncthreads();
+        for (int s = DX_NT / 2; s > 0; s >>= 1) {
+            if (t < s) red[t] += red[t + s];
+            __syncthreads();
+        }
+        if (t == 0) out[j * d + k] = accumulate ? out[j * d + k] + red[0] : red[0];
+        __syncthreads();
+    }
+}
+
 // strict-upper tiles of the Npad x Npad matrix F <- transpose of its strict-lower tiles (diagonal tiles untouched)
 __global__ void mirror_lower_tiles_kernel(double* __restrict__ F, long long ld) {
     __shared__ double tl[32][33];
@@ -738,6 +776,16 @@ cudaError_t crossgram_dx_launch(const KProg& P, const double* xs, int64_t ldxs, 
     if (M <= 0) return cudaSuccess;
     if (d <= 0 || d > GPB200_MAX_DIMS || ((W1 || W2) && !dvar)) return cudaErrorInvalidValue;
     crossgram_dx_kernel<<<(unsigned)M, DX_NT, 0, st>>>(P, xs, ldxs, z, ldz, n, d, a, W1, W2, ldw, c, dmu, dvar);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t inducing_dx_launch(const KProg& P, const double* u, int64_t ldu, int64_t M, const double* z, int64_t ldz, int64_t n,
+                               int d, const double* W, int64_t ldw, int sym, const double* mask, double* out, int accumulate,
+                               cudaStream_t st, int64_t* launches) {
+    if (M <= 0) return cudaSuccess;
+    if (d <= 0 || d > GPB200_MAX_DIMS || n < 0) return cudaErrorInvalidValue;
+    inducing_dx_kernel<<<(unsigned)M, DX_NT, 0, st>>>(P, u, ldu, z, ldz, n, d, W, ldw, sym, mask, out, accumulate);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

@@ -43,5 +43,10 @@ cudaError_t crossgram_grad_launch(const KProg& P, const double* x1, int64_t ldx1
 cudaError_t crossgram_dx_launch(const KProg& P, const double* xs, int64_t ldxs, int64_t M, const double* z, int64_t ldz, int64_t n,
                                 int d, const double* a, const double* W1, const double* W2, int64_t ldw, double c, double* dmu,
                                 double* dvar, cudaStream_t st, int64_t* launches);
+// inducing-point gradient (M x d output, point-major): out[j, :] = [out[j, :] if accumulate] + sum_i W(i, j) dk(u_j, z_i)/du_j
+// over the n rows z_i with mask[i] != 0 (mask may be null), W(i, j) = W[i * ldw + j] (+ W[j * ldw + i] if sym).  Fixed-order sums.
+cudaError_t inducing_dx_launch(const KProg& P, const double* u, int64_t ldu, int64_t M, const double* z, int64_t ldz, int64_t n,
+                               int d, const double* W, int64_t ldw, int sym, const double* mask, double* out, int accumulate,
+                               cudaStream_t st, int64_t* launches);
 // F[j, i] = F[i, j] for every element of the strict-lower 128-tiles of the Npad x Npad matrix F (diagonal tiles untouched)
 cudaError_t mirror_lower_tiles_launch(double* F, int64_t ld, int64_t Npad, cudaStream_t st, int64_t* launches);

@@ -78,6 +78,8 @@ _SIGNATURES = {
     "gpb200_fitc_mll": (C.c_int, [_H, _dp, _dp, _dp, _dp]),
     "gpb200_fitc_grad_noise": (C.c_int, [_H, _dp]),
     "gpb200_fitc_grad_kernel": (C.c_int, [_H, _dp]),
+    "gpb200_fitc_grad_kernel_inducing": (C.c_int, [_H, _dp, _dp]),
+    "gpb200_fitc_set_inducing": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
     "gpb200_fitc_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp]),
     "gpb200_fitc_predict_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
     "gpb200_fitc_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
@@ -453,7 +455,7 @@ class Engine:
     FSA_KERNELS = ("gram", "bdmv", "mask", "permute", "resid", "outer", "trace", "axpy_t", "crossgram", "rowdot", "var",
                    "crossgram_dx")
     FITC_CV_KERNELS = ("delta", "rows", "invdiag", "eblock", "qs", "wvec", "gather", "diag", "colscale", "scale", "fitc_g",
-                       "fitc_wfu", "fitc_wuu", "symmetrize")
+                       "fitc_wfu", "fitc_wuu", "symmetrize", "inducing_dx")
 
     def fsa_kernels(self, name, args, fargs=()):
         """One FSA block-diagonal kernel (include/gpb200.h) by name, on device buffers: args = the int64 arguments followed
@@ -529,6 +531,27 @@ class FitcEngine:
         g = np.empty(max(self.n_theta, 1))
         self._check(self._lib.gpb200_fitc_grad_kernel(self._h, _as_dp(g)), "fitc_grad_kernel")
         return g[:self.n_theta].copy()
+
+    def grad_kernel_inducing(self, want_kernel=True):
+        """one sweep: (dmll_kernel[n_theta] or None, dmll_xu (M, d)); dmll_kernel bitwise grad_kernel's"""
+        g = np.empty(max(self.n_theta, 1)) if want_kernel else None
+        gx = np.empty((self.M, self.d))
+        self._check(self._lib.gpb200_fitc_grad_kernel_inducing(self._h, _as_dp(g) if want_kernel else None, _as_dp(gx)),
+                    "fitc_grad_kernel_inducing")
+        return (g[:self.n_theta].copy() if want_kernel else None), gx
+
+    def set_inducing(self, xu_pm):
+        """replace the inducing points (M, d) in place; factorize + mll must follow"""
+        xu_pm = np.ascontiguousarray(xu_pm, dtype=np.float64)
+        if xu_pm.shape != (self.M, self.d):
+            raise ValueError("fitc_set_inducing: the inducing points must keep their shape (%d, %d)" % (self.M, self.d))
+        self._check(self._lib.gpb200_fitc_set_inducing(self._h, self.M, _as_dp(xu_pm), self.d), "fitc_set_inducing")
+
+    def grad_inducing_timings(self):
+        """device times (ms) of the last grad_kernel_inducing: the dmll/dXu contractions summed, the whole call"""
+        out = np.zeros(9)
+        self._check(self._lib.gpb200_fitc_get_timings(self._h, _as_dp(out), 9), "fitc_get_timings")
+        return out[7:].copy()
 
     def set_kernel(self, ops, dims, n_theta):
         self.n_theta = int(n_theta)

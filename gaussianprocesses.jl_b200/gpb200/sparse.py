@@ -8,7 +8,7 @@ import math
 import numpy as np
 
 from . import capi
-from .gpe import GPE, _as_dxn, _predict_f_grad
+from .gpe import GPE, _RejectedStep, _as_dxn, _predict_f_grad
 from .kernels import flatten
 from .means import MeanZero
 
@@ -63,32 +63,85 @@ class FITC:
         self.dmll = np.array(out)
         return self
 
-    def update_dmll(self, noise=True, domean=True, kern=True):
-        """update_dmll! (src/GPE.jl:298-324) with the FITC strategy: [noise; mean; kernel]."""
+    def update_dmll(self, noise=True, domean=True, kern=True, inducing=False):
+        """update_dmll! (src/GPE.jl:298-324) with the FITC strategy: [noise; mean; kernel].  inducing=True appends
+        dmll/dXu as vec(Xu) (one point after another); the kernel part and it come from one device sweep."""
         out = []
         if noise:
             out.append(self._eng.grad_noise())                                   # fitc.jl:243-257
         if domean and self.mean.num_params() > 0:
             out.extend(self.mean.grad_stack(self._xpm).T @ self.alpha)           # GPE.jl:282-288
-        if kern:
+        if inducing:
+            gk, gx = self._eng.grad_kernel_inducing(want_kernel=kern)
+            if kern:
+                out.extend(gk[self._exposed])
+            out.extend(gx.ravel())
+        elif kern:
             out.extend(self._eng.grad_kernel()[self._exposed])                   # fitc.jl:200-234 + sor.jl:219-253
         self.dmll = np.array(out)
         return self
 
-    def update_mll_and_dmll(self, **kw):
+    def update_mll_and_dmll(self, noise=True, domean=True, kern=True, inducing=False):
         self.update_mll()
-        return self.update_dmll(**kw)
+        return self.update_dmll(noise=noise, domean=domean, kern=kern, inducing=inducing)
 
     # ---- GPE's parameter protocol, [noise; mean; kernel] (src/GPE.jl:346-510), and optimize! (src/optimize.jl) -----------
     # logNoise is a scalar here; FixedKernel parameters are neither returned nor set, their gradients are dropped
-    # (update_dmll's `_exposed`), exactly as for GPE.
-    get_params = GPE.get_params
+    # (update_dmll's `_exposed`), exactly as for GPE.  inducing=True (not in the reference) appends vec(Xu), Julia's
+    # column-major vec of the dim x M matrix: [noise; mean; kernel; Xu].
+    def get_params(self, noise=True, domean=True, kern=True, inducing=False):
+        p = GPE.get_params(self, noise=noise, domean=domean, kern=kern)
+        return np.concatenate([p, self.Xu.T.ravel()]) if inducing else p
+
     num_params = GPE.num_params
-    set_params = GPE.set_params
+
+    def set_params(self, hyp, noise=True, domean=True, kern=True, inducing=False):
+        if not inducing:
+            return GPE.set_params(self, hyp, noise=noise, domean=domean, kern=kern)
+        hyp = np.asarray(hyp, dtype=np.float64)
+        nu = self.Xu.size
+        if hyp.size != self.num_params(noise=noise, domean=domean, kern=kern, inducing=True):
+            raise ValueError("wrong number of hyper-parameters")
+        GPE.set_params(self, hyp[:hyp.size - nu], noise=noise, domean=domean, kern=kern)
+        xu_pm = hyp[hyp.size - nu:].reshape(self.Xu.shape[1], self.dim)
+        self._eng.set_inducing(xu_pm)
+        self.Xu = np.ascontiguousarray(xu_pm.T)
+        return self
+
     initialise_target = GPE.initialise_target
     update_target = GPE.update_target
-    update_target_and_dtarget = GPE.update_target_and_dtarget
-    optimize = GPE.optimize
+
+    def update_target_and_dtarget(self, noise=True, domean=True, kern=True, inducing=False):
+        return GPE.update_target_and_dtarget(self, noise=noise, domean=domean, kern=kern, inducing=inducing)
+
+    def optimize(self, noise=True, domean=True, kern=True, inducing=False, maxiter=100, **kw):
+        """optimize!(gp) as GPE.optimize; inducing=True also moves the inducing points (Snelson & Ghahramani's
+        pseudo-inputs), with the same exception filter: a step that makes K_uu or Sigma_QR singular (two inducing points
+        meeting: PosDefException) is rejected and the parameters, Xu included, are rolled back."""
+        if not inducing:
+            return GPE.optimize(self, noise=noise, domean=domean, kern=kern, maxiter=maxiter, **kw)
+        from scipy.optimize import minimize
+
+        flags = dict(noise=noise, domean=domean, kern=kern, inducing=True)
+        best = {"f": None}
+
+        def fg(hyp):
+            prev = self.get_params(**flags)
+            try:
+                if not np.all(np.isfinite(hyp)):
+                    raise _RejectedStep("non-finite hyper-parameter")
+                self.set_params(hyp, **flags)
+                self.update_target_and_dtarget(**flags)
+                best["f"] = -self.target if best["f"] is None else min(best["f"], -self.target)
+                return -self.target, -self.dtarget
+            except (np.linalg.LinAlgError, _RejectedStep):            # as GPE.optimize
+                self.set_params(prev, **flags)
+                return 1e10 + 1e6 * abs(best["f"] or 0.0), np.asarray(hyp, dtype=np.float64) - prev
+
+        res = minimize(fg, self.get_params(**flags), jac=True, method="L-BFGS-B", options=dict(maxiter=maxiter), **kw)
+        self.set_params(res.x, **flags)
+        self.update_target()
+        return res
 
     # rand(gp, X, n) (src/GP.jl:120-146): GPE's host side; the engine builds Sigma* = predict_f(x; full_cov=true)'s
     # covariance on the device and factors it there.  Returns a (npred, n) array.

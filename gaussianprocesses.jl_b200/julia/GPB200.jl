@@ -488,6 +488,27 @@ function dmll_kern!(dmll::AbstractVector, gp, ::B200SparsePrecompute, ::B200Spar
     dmll .= g[gp.cK.exposed]
     return dmll
 end
+
+# Inducing points as parameters (not in the reference; Snelson & Ghahramani's pseudo-inputs).  set_inducing! moves the
+# strategy's Xu in place (same size) and on the device, without rebuilding the handle, then refreshes the target;
+# dmll_inducing returns dmll/dXu (dim x M) of the last update_target!, from one sweep of the kernel-gradient adjoints.
+function set_inducing!(gp::GPE{X,Y,M,K,CS,D,P}, Xu::AbstractMatrix) where {X,Y,M,K,CS<:B200SparseStrategy,D,P}
+    size(Xu) == size(gp.covstrat.inducing) ||
+        throw(ArgumentError("set_inducing!: Xu must keep the size $(size(gp.covstrat.inducing))"))
+    gp.covstrat.inducing .= Xu
+    U = Matrix{Float64}(gp.covstrat.inducing)
+    checks(gp.cK, ccall((:gpb200_fitc_set_inducing, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64),
+                        gp.cK.handle, size(U, 2), U, size(U, 1)), "fitc_set_inducing")
+    update_target!(gp)
+    return gp
+end
+function dmll_inducing(gp::GPE{X,Y,M,K,CS,D,P}) where {X,Y,M,K,CS<:B200SparseStrategy,D,P}
+    g = Matrix{Float64}(undef, size(gp.covstrat.inducing)...)
+    checks(gp.cK, ccall((:gpb200_fitc_grad_kernel_inducing, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}),
+                        gp.cK.handle, C_NULL, g), "fitc_grad_kernel_inducing")
+    return g
+end
+
 function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=false) where {X,Y,M,K,CS<:B200Sparse,D,P}
     size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
     Xs = Matrix{Float64}(x); Ms = size(Xs, 2)
@@ -809,6 +830,6 @@ function predict_y(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)        
     return predict_obs(gp.lik, μ, σ2)
 end
 
-export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA
+export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA, set_inducing!, dmll_inducing
 
 end # module

@@ -343,6 +343,9 @@ int  gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32
  *   which 11 fitc_wfu   : P2, P1, ld, nrows, ncols, alpha, lam, g, beta
  *   which 12 fitc_wuu   : Wuu, T, Kinv, Sinv, ld, n, beta
  *   which 13 symmetrize : A, ld, n
+ *   which 14 inducing_dx: u, ldu, M, z, ldz, n, d, W, ldw, sym, mask (0 = none), out, accumulate   fargs = theta
+ *                         out[j, :] (+)= sum_{i < n, mask[i] != 0} W(i, j) dk(u_j, z_i)/du_j, W(i, j) = W[i ldw + j]
+ *                         (+ W[j ldw + i] when sym = 1, which needs n = M); out is M x d point-major
  * GPB200_EINVAL, nothing launched: as gpb200_fsa_kernels, plus j outside [0, n_theta) and ldx < d.                   */
 int  gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
 
@@ -401,6 +404,23 @@ int  gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, 
 int  gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise);
 /* dmll_kernel[n_theta], full parameter vector of the un-fixed kernel tree (as gpb200_grad_kernel) */
 int  gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel);
+/* Gradient of the mll with respect to the inducing inputs (not in the reference; Snelson & Ghahramani's pseudo-inputs),
+ * all four modes.  One sweep gives dmll_kernel[n_theta] (may be NULL; when given, bitwise equal to gpb200_fitc_grad_kernel
+ * on the same handle: the same launches) and dmll_xu[M x d], point-major (Julia's d x M column-major):
+ *   dmll/du_j = 1/2 [ sum_i W_fu[i, j] dk(u_j, x_i)/du_j + sum_l (W_uu[j, l] + W_uu[l, j]) dk(u_j, u_l)/du_j ]
+ * with W_fu, W_uu the adjoints of the mll with respect to K_fu and K_uu that the kernel gradient already builds.  It adds one
+ * contraction launch per staging chunk and one for W_uu (FSA padding rows are skipped); with several ranks the W_fu part is
+ * all-reduced once (M d doubles).  Sums are in a fixed order: repeated calls are bitwise equal.  Device memory grows by
+ * M d doubles on the first call.  GPB200_ESTATE before factorize + mll; GPB200_EINVAL for a NULL dmll_xu.
+ * gpb200_fitc_get_timings slots 7-8 hold the last call's device times: the contractions, the whole call.            */
+int  gpb200_fitc_grad_kernel_inducing(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu);
+/* Replaces the inducing inputs (xu: d x M column-major, ld = ldxu) of both M x M sub-engines in place (not in the
+ * reference).  M must be gpb200_fitc_set_data's and ldxu >= d (GPB200_EINVAL otherwise); GPB200_ESTATE before set_data.
+ * The training inputs, the kernel program, the FSA blocks and their work lists and every workspace are kept; the
+ * factorisation, alpha and the cross-validation state are cleared.  After factorize + mll, alpha, mll and logdet are
+ * bitwise those of a fresh handle given the same xu to gpb200_fitc_set_data (and the same gpb200_fitc_set_blocks).
+ * With several ranks every rank passes the same xu.                                                                   */
+int  gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_t ldxu);
 /* mu_minus_mean[Ms], var[Ms] (may be NULL; not clamped) */
 int  gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean, double* var);
 /* Predictive gradients of FITC / DTC / SoR with respect to the test inputs, as gpb200_predict_grad (same layouts, var and
@@ -473,8 +493,9 @@ int  gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs
                       int64_t nsamp, const double* z, double nugget, double* mu_minus_mean, double* samples);
 /* device times (ms) of the last successful gpb200_fitc_rand: [0] Sigma* build (with mu), [1] make_posdef! + Cholesky,
  * [2] unwhiten! GEMM + mu; of the last gpb200_fitc_predict_fsa_grad, summed over its test chunks: [3] predict_fsa's
- * launches, [4] s = R L_s^-1 and the second block sweep, [5] the K_uu^-1 TRSMs, [6] the contraction (CUDA events;
- * n <= 7 entries are written)                                                                                           */
+ * launches, [4] s = R L_s^-1 and the second block sweep, [5] the K_uu^-1 TRSMs, [6] the contraction; of the last
+ * gpb200_fitc_grad_kernel_inducing: [7] its dmll/dXu contractions summed, [8] the whole call (CUDA events; n <= 9 entries
+ * are written)                                                                                                          */
 int  gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n);
 /* ---- cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) ---------------
  * The dense entry points gpb200_get_inverse_diag / gpb200_cv_param / gpb200_cv_block for modes 0 (FITC), 1 (DTC: SoR's
