@@ -73,6 +73,7 @@ struct gpb200_handle {
     KProg prog{};
     std::vector<double> theta;
     bool has_data = false, has_kernel = false, factored = false, inv_ready = false, alpha_ready = false;
+    bool s_ready = false;                      // G's lower triangle holds -S of gpb200_gpa_grad (A = S for gpb200_grad_inputs)
     double *F = nullptr, *G = nullptr, *Dinv = nullptr, *DinvT = nullptr, *logd = nullptr;
     double *noise_var = nullptr, *r0 = nullptr, *r1 = nullptr, *y1 = nullptr, *alpha = nullptr, *scal = nullptr;
     double *part = nullptr, *trace_out = nullptr;
@@ -110,6 +111,9 @@ struct gpb200_handle {
     double *xs = nullptr, *Kst = nullptr, *Kss = nullptr, *pmu = nullptr, *pvar = nullptr, *pkdiag = nullptr;
     int64_t xs_cap = 0, Kst_rows = 0, Kss_rows = 0;
     double* pdx = nullptr; int64_t pdx_rows = 0;   // gpb200_predict_grad: dmu (Mpad x d), then dvar (Mpad x d)
+    // gpb200_grad_inputs (first use, freed with the data): a caller's alpha (Npad), the N x d result (Npad x d), and in an
+    // in-process group the gathered ranks' results (nranks x Npad x d)
+    double* dxin = nullptr;
     CUtensorMap mapKst{};
     // options
     int nb = 0;                 // outer Cholesky block; 0 = fully recursive (one panel)
@@ -119,7 +123,7 @@ struct gpb200_handle {
     cudaStream_t st_cur = nullptr;             // stream launch_gemm / the leaf use right now (st or st_side)
     cudaEvent_t ev_la0 = nullptr, ev_la2 = nullptr;
     // stats
-    double ms[16] = {};
+    double ms[17] = {};
     int64_t launches = 0;
     bool own_stream = true;
     // per-launch GEMM profiling (option "profile"): event pairs + executed flops of every GEMM launch
@@ -328,7 +332,7 @@ void free_data(gpb200_handle* h) {
     free_FG(h);
     double** ptrs[] = {&h->x, &h->Dinv, &h->DinvT, &h->logd, &h->noise_var, &h->r0, &h->r1,
                        &h->y1, &h->alpha, &h->scal, &h->part, &h->trace_out, &h->xs, &h->Kst, &h->Kss,
-                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt, &h->ZdT, &h->pdx};
+                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt, &h->ZdT, &h->pdx, &h->dxin};
     h->xmap_ok = false;
     if (h->cvD) cudaFree(h->cvD);
     if (h->cvY) cudaFree(h->cvY);
@@ -346,7 +350,7 @@ void free_data(gpb200_handle* h) {
     if (h->ag_recv) cudaFree(h->ag_recv);
     h->ag_send = h->ag_recv = nullptr; h->pack_elems = h->ag_send_elems = h->ag_recv_elems = 0;
     h->xs_cap = h->Kst_rows = h->Kss_rows = h->pdx_rows = 0;
-    h->has_data = h->factored = h->inv_ready = h->alpha_ready = false;
+    h->has_data = h->factored = h->inv_ready = h->s_ready = h->alpha_ready = false;
 }
 
 GemmBuf bufF(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapF : nullptr, h->F, h->ld}; }
@@ -1093,7 +1097,7 @@ int factor_end(const Locals& L, const char* what, bool p2p_ran) {
 
 // factor whatever SPD matrix sits in the lower tiles of h->G (padding must be identity)
 int chol_inplace(gpb200_handle* h) {
-    h->factored = h->inv_ready = h->alpha_ready = false;
+    h->factored = h->inv_ready = h->s_ready = h->alpha_ready = false;
     const Locals L{h};
     TRY(factor_begin(L));
     CK(cholesky(h, 0, h->nb));
@@ -1212,7 +1216,7 @@ void gpb200_destroy(gpb200_handle* h) {
         for (auto* m : g->hs) { if (m->st) cudaStreamSynchronize(m->st); }
         for (auto* m : g->hs) {                 // the survivors become ordinary single-rank handles (storage re-allocated at their next factorize)
             m->grp = nullptr; m->nranks = 1; m->rank = 0;
-            m->factored = m->inv_ready = m->alpha_ready = false;
+            m->factored = m->inv_ready = m->s_ready = m->alpha_ready = false;
         }
         delete g;
     }
@@ -1250,13 +1254,13 @@ int gpb200_set_option(gpb200_handle* h, const char* key, int64_t value) {
     if (!strcmp(key, "nb")) {
         if (value != 0 && value != 128 && value != 256 && value != 512 && value != 1024 && value != 2048 && value != 4096)
             return fail(h, GPB200_EINVAL, "nb must be 0 (fully recursive) or 128 * 2^k <= 4096");
-        h->nb = (int)value; h->factored = h->inv_ready = false; return GPB200_OK;
+        h->nb = (int)value; h->factored = h->inv_ready = h->s_ready = false; return GPB200_OK;
     }
     if (!strcmp(key, "gemm")) { h->gemm_impl = value ? 1 : 0; return GPB200_OK; }
     if (!strcmp(key, "dist_nb")) {
         if (value != 0 && value != 128 && value != 256 && value != 512 && value != 1024 && value != 2048 && value != 4096)
             return fail(h, GPB200_EINVAL, "dist_nb must be 0 (auto) or 128 * 2^k <= 4096");
-        h->dist_nb = (int)value; h->factored = h->inv_ready = false; return GPB200_OK;
+        h->dist_nb = (int)value; h->factored = h->inv_ready = h->s_ready = false; return GPB200_OK;
     }
     if (!strcmp(key, "lookahead")) { h->lookahead = value ? 1 : 0; return GPB200_OK; }
     if (!strcmp(key, "gram_fast")) { h->gram_fast = value ? 1 : 0; return GPB200_OK; }
@@ -1266,11 +1270,11 @@ int gpb200_set_option(gpb200_handle* h, const char* key, int64_t value) {
     }
     if (!strcmp(key, "shard")) {                // storage of F / G with several ranks: -1 auto, 0 replicated, 1 row-sharded
         if (value < -1 || value > 1) return fail(h, GPB200_EINVAL, "shard must be -1 (auto), 0 or 1");
-        h->shard_opt = (int)value; h->factored = h->inv_ready = false; return GPB200_OK;
+        h->shard_opt = (int)value; h->factored = h->inv_ready = h->s_ready = false; return GPB200_OK;
     }
     if (!strcmp(key, "shard_rb")) {             // ownership block of the row-sharded storage in 128-row tiles (panel = 128 * rb)
         if (value != 0 && value != 1 && value != 2 && value != 4 && value != 8) return fail(h, GPB200_EINVAL, "shard_rb must be 0 (auto), 1, 2, 4 or 8");
-        h->shard_rb_opt = (int)value; h->factored = h->inv_ready = false; return GPB200_OK;
+        h->shard_rb_opt = (int)value; h->factored = h->inv_ready = h->s_ready = false; return GPB200_OK;
     }
     if (!strcmp(key, "trsv_fused")) {            // 0: one launch per block step; 1 (default): single-launch kernels
         if (value != 0 && value != 1) return fail(h, GPB200_EINVAL, "trsv_fused must be 0 or 1");
@@ -1307,7 +1311,7 @@ int gpb200_set_stream(gpb200_handle* h, void* stream) {
 
 int gpb200_get_timings(gpb200_handle* h, double* ms, int32_t n) {
     if (!h || !ms) return GPB200_EINVAL;
-    for (int i = 0; i < n && i < 16; ++i) ms[i] = h->ms[i];
+    for (int i = 0; i < n && i < 17; ++i) ms[i] = h->ms[i];
     return GPB200_OK;
 }
 
@@ -1367,7 +1371,7 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
     }
     CK(cudaStreamSynchronize(h->st));
     h->has_data = true;
-    h->factored = h->inv_ready = h->alpha_ready = false;
+    h->factored = h->inv_ready = h->s_ready = h->alpha_ready = false;
     // a kernel program that reads a dimension the new points do not have is dropped: factorize then asks for set_kernel
     for (int i = 0; h->has_kernel && i < GPB200_MAX_DIMS; ++i)
         if (h->prog.dims[i] >= d) h->has_kernel = false;
@@ -1427,7 +1431,7 @@ int gpb200_set_kernel(gpb200_handle* h, int32_t n_ops, const int32_t* ops, int32
     h->prog = P;
     h->theta.assign(n_theta, 0.0);
     h->has_kernel = true;
-    h->factored = h->inv_ready = false;
+    h->factored = h->inv_ready = h->s_ready = false;
     return GPB200_OK;
 }
 
@@ -1440,7 +1444,7 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
     for (int i = 0; i < h->prog.n_theta; ++i)
         if (!isfinite(theta[i])) return fail(h, GPB200_EINVAL, "factorize: non-finite hyper-parameter");
     CK(cudaSetDevice(h->device));
-    h->factored = h->inv_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
+    h->factored = h->inv_ready = h->s_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
     std::vector<double> nv((size_t)n_noise);
     for (int64_t i = 0; i < n_noise; ++i) {
         if (!isfinite(log_noise[i])) return fail(h, GPB200_EINVAL, "factorize: non-finite logNoise");
@@ -1452,7 +1456,7 @@ int gpb200_factorize(gpb200_handle* h, const double* theta, const double* log_no
     for (auto* q : L) {                                    // (an in-process group: every virtual rank gets the arguments)
         if (!q->has_data || !q->has_kernel || q->prog.n_theta != h->prog.n_theta || q->N != h->N)
             return fail(h, GPB200_ESTATE, "factorize: every handle of the group needs the same set_data / set_kernel");
-        q->factored = q->inv_ready = q->alpha_ready = false;
+        q->factored = q->inv_ready = q->s_ready = q->alpha_ready = false;
         for (int i = 0; i < q->prog.n_theta; ++i) q->theta[i] = theta[i];
         kprog_set_theta(q->prog, theta);
         SCK(q, cudaMemcpyAsync(q->noise_var, nv.data(), sizeof(double) * n_noise, cudaMemcpyHostToDevice, q->st));
@@ -1548,7 +1552,7 @@ int gpb200_grad_prepare(gpb200_handle* h) {
     if (!h) return GPB200_EINVAL;
     if (!h->factored) return fail(h, GPB200_ESTATE, "grad_prepare: factorize first");
     if (h->inv_ready) return GPB200_OK;
-    h->g_sym = false; h->cv_m_ok = false;
+    h->g_sym = false; h->cv_m_ok = false; h->s_ready = false;
     CK(cudaSetDevice(h->device));
     CK(cudaEventRecord(h->ev0, h->st));
     if (h->sharded) {
@@ -1648,7 +1652,7 @@ int gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, doub
         return GPB200_OK;
     }
     // G and F's strict-upper tiles are overwritten: K^-1, its mirror, M_j and alpha are gone
-    h->inv_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
+    h->inv_ready = h->s_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
     const int Np = (int)h->Npad;
     if (!h->ZdT) {
         CK(cudaMalloc(&h->ZdT, sizeof(double) * h->Npad * TILE));
@@ -1686,6 +1690,51 @@ int gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, doub
     h->ms[10] = ev_ms(h->ev2, h->ev3);
     h->ms[4] = ev_ms(h->ev3, h->ev4);
     for (int p = 0; p < np; ++p) dll_kernel[p] = out[p];
+    h->s_ready = true;
+    return GPB200_OK;
+}
+
+// Training-input gradient: out[i, :] = sum_j A_ij dk(x_i, x_j)/dx_i over the resident lower triangle of A (the inputs_dx
+// kernel of gram.cu reads each stored entry twice, once for its row point and once for its column point).  The tile rows
+// are split as in gpb200_grad_kernel's trace: replicated multi-rank handles sum rows t % nranks == rank and all-reduce the
+// N x d partials over NCCL; row-sharded handles sum their own rows and all-reduce through coll_allreduce_sum.  Reads F, G,
+// alpha and the cross-validation work matrices only: a caller's alpha goes to the dxin scratch.  Timing slot 16.
+int gpb200_grad_inputs(gpb200_handle* h, const double* alpha, double* dmll_x) {
+    if (!h) return GPB200_EINVAL;
+    if (!dmll_x) return fail(h, GPB200_EINVAL, "grad_inputs: null dmll_x");
+    if (h->s_ready && alpha) return fail(h, GPB200_EINVAL, "grad_inputs: after gpa_grad the contraction is with S; alpha must be NULL");
+    if (!h->s_ready && !h->inv_ready) return fail(h, GPB200_ESTATE, "grad_inputs: grad_prepare (or gpa_grad with the kernel gradient) first");
+    if (!h->s_ready && !alpha && !h->alpha_ready) return fail(h, GPB200_ESTATE, "grad_inputs: no alpha (call mll or pass alpha)");
+    CK(cudaSetDevice(h->device));
+    Locals L;
+    if (h->sharded) TRY(shard_entry(h, L)); else L = Locals{h};
+    const int64_t N = h->N, Npad = h->Npad, nd = Npad * h->d;
+    for (auto* q : L) {
+        if (!q->dxin) SCK(q, cudaMalloc(&q->dxin, sizeof(double) * (size_t)(Npad + nd * (1 + (q->grp ? q->nranks : 0)))));
+        if (alpha) TRY(rank_failed(q, upload_padded(q, q->dxin, alpha)));
+    }
+    auto res = [&](gpb200_handle* q) { return q->dxin + Npad; };
+    CK(cudaEventRecord(h->ev0, h->st));
+    for (auto* q : L) {
+        SeIsoFast sf;
+        const double* a = h->s_ready ? nullptr : alpha ? q->dxin : q->alpha;     // S state: A = -G = S
+        SCK(q, inputs_dx_launch(q->prog, use_seiso_fast(q, &sf), q->x, q->d, q->d, N, a, q->G, q->ld, res(q), q->st, &q->launches,
+                                q->nranks, q->rank, q->sharded ? q->rb : 1));
+    }
+    if (h->sharded) {
+        TRY(coll_allreduce_sum(L, res, (size_t)(N * h->d), [&](gpb200_handle* q) { return q->dxin + Npad + nd; }));
+    } else if (h->nranks > 1) {                            // N x d partial sums, summed over ranks
+        CK(cudaEventRecord(h->ev_x, h->st));
+        CK(cudaStreamWaitEvent(h->st_comm, h->ev_x, 0));
+        CKN(g_nccl.AllReduce(res(h), res(h), (size_t)(N * h->d), ncclDouble, ncclSum, h->comm, h->st_comm));
+        CK(cudaEventRecord(h->ev_y, h->st_comm));
+        CK(cudaStreamWaitEvent(h->st, h->ev_y, 0));
+    }
+    CK(cudaEventRecord(h->ev1, h->st));
+    CK(cudaMemcpyAsync(dmll_x, res(h), sizeof(double) * (size_t)(N * h->d), cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
+    if (h->sharded) TRY(sync_all(L));
+    h->ms[16] = ev_ms(h->ev0, h->ev1);
     return GPB200_OK;
 }
 
@@ -1896,7 +1945,7 @@ static int append_inputs(gpb200_handle* h, int64_t k, const double* xnew, int64_
                      gemm_make_tensor_map_plain(&h->mapXT, h->xpt, h->dxp, Nnew, Np, h->dxp, TILE);
     }
     h->N = Nnew;
-    h->inv_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
+    h->inv_ready = h->s_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
     return GPB200_OK;
 }
 
@@ -2811,7 +2860,7 @@ int gpb200_comm_init(gpb200_handle* h, int nranks, int rank, const char* id128) 
     if (!h->ev_x) CK(cudaEventCreateWithFlags(&h->ev_x, cudaEventDisableTiming));
     if (!h->ev_y) CK(cudaEventCreateWithFlags(&h->ev_y, cudaEventDisableTiming));
     h->nranks = nranks; h->rank = rank;
-    h->factored = h->inv_ready = false;
+    h->factored = h->inv_ready = h->s_ready = false;
     return GPB200_OK;
 }
 
@@ -2844,7 +2893,7 @@ int gpb200_group_create(gpb200_handle** hs, int n) {
     for (int i = 0; i < n; ++i) {
         g->hs.push_back(hs[i]);
         hs[i]->grp = g; hs[i]->nranks = n; hs[i]->rank = i;
-        hs[i]->factored = hs[i]->inv_ready = false;
+        hs[i]->factored = hs[i]->inv_ready = hs[i]->s_ready = false;
     }
     return GPB200_OK;
 }

@@ -586,6 +586,114 @@ __global__ void __launch_bounds__(DX_NT) inducing_dx_kernel(const __grid_constan
     }
 }
 
+// training-input gradient over the stored lower triangle of a symmetric A (A_ij = a_i a_j - G[i * ldg + j], a = alpha or 0
+// when alpha is null: A = alpha alpha' - K^-1 after grad_prepare, A = S after gpa_grad), one CTA per IX_PB points p0..:
+//   out[i, :] = sum_{j <= i} A_ij d1k(x_i, x_j)  +  sum_{l > i} A_li d1k(x_i, x_l)
+// (d1k: derivative in the first argument).  Row part: warp w takes rows p0 + w, p0 + w + 8, ..., its lanes run across the
+// columns j <= i of row i (coalesced), then one fixed shuffle tree per coordinate.  Column part: lane t owns column p0 + t,
+// warp w walks the rows l = w, w + 8, ... below it (each row's 32 columns are one coalesced read), then the 8 warps are
+// summed in warp order.  Both parts of a CTA cover together N entries per point, so the CTAs are balanced although the
+// triangle is not.  Only tile rows with ((tile / bm_div) % bm_mod) == bm_rem are read (trace_kernel's ownership); the
+// others contribute 0 here and come from the other ranks.  Rows and columns >= N are never read.  Fixed order throughout.
+// FAST: the single SEIso leaf with d <= 8, the d-vectors in registers; else kprog_eval_dx with a local-memory d-vector.
+constexpr int IX_PB = 32;
+template <bool FAST>
+__global__ void __launch_bounds__(NT) inputs_dx_kernel(const __grid_constant__ KProg P, const double* __restrict__ x, long long ldx,
+                                                       int d, long long N, const double* __restrict__ alpha,
+                                                       const double* __restrict__ G, long long ldg, double* __restrict__ out,
+                                                       int bm_mod, int bm_rem, int bm_div) {
+    constexpr int DR = FAST ? 8 : GPB200_MAX_DIMS;
+    __shared__ double red[NT / 32][IX_PB];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long p0 = (long long)blockIdx.x * IX_PB;
+    auto owned = [&](long long row) { return bm_mod <= 1 || ((row / TB / bm_div) % bm_mod) == bm_rem; };
+    double il2 = 0.0, mh = 0.0, s2 = 0.0;
+    if (FAST) { il2 = 1.0 / P.par[0]; mh = -0.5 / P.par[0]; s2 = P.par[1]; }
+    double acc[DR];
+    const int dk = FAST ? 8 : d;                          // accumulated coordinates (FAST: zero beyond d)
+    // A_ij d1k(x_i, x_j) into acc (xi: the point differentiated, xj: the other)
+    auto add = [&](const double* xi, const double* xj, double A) {
+        if (FAST) {
+            double df[8], r2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { df[k] = k < d ? xi[k] - xj[k] : 0.0; r2 += df[k] * df[k]; }
+            const double f = -s2 * exp(mh * r2) * il2 * A;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) acc[k] += f * df[k];
+        } else {
+            kprog_eval_dx(P, xi, xj, A, acc, 0.0, nullptr);
+        }
+    };
+
+    // ---- row part: j <= i in row i
+#pragma unroll 1
+    for (int rr = warp; rr < IX_PB; rr += NT / 32) {
+        const long long i = p0 + rr;
+        if (i >= N) break;
+#pragma unroll
+        for (int k = 0; k < dk; ++k) acc[k] = 0.0;
+        if (owned(i)) {
+            const double* xi = x + i * ldx;
+            double xr[FAST ? 8 : 1];
+            if (FAST) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) xr[k] = k < d ? xi[k] : 0.0;
+            }
+            const double ai = alpha ? alpha[i] : 0.0;
+            const double* gr = G + i * ldg;
+#pragma unroll 1
+            for (long long j = lane; j <= i; j += 32) {
+                const double A = (alpha ? ai * alpha[j] : 0.0) - gr[j];
+                add(FAST ? xr : xi, x + j * ldx, A);
+            }
+        }
+        for (int k = 0; k < dk; ++k) {
+            double v = acc[k];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+            if (lane == 0 && k < d) out[i * d + k] = v;
+        }
+    }
+
+    // ---- column part: l > j in column j = p0 + lane
+    const long long j = p0 + lane;
+#pragma unroll
+    for (int k = 0; k < dk; ++k) acc[k] = 0.0;
+    if (j < N) {
+        const double* xj = x + j * ldx;
+        double xc[FAST ? 8 : 1];
+        if (FAST) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) xc[k] = k < d ? xj[k] : 0.0;
+        }
+        const double aj = alpha ? alpha[j] : 0.0;
+        for (long long t0 = p0 / TB * TB; t0 < N; t0 += TB) {
+            if (!owned(t0)) continue;
+            const long long lend = t0 + TB < N ? t0 + TB : N;
+#pragma unroll 1
+            for (long long l = (t0 > p0 ? t0 : p0) + warp; l < lend; l += NT / 32) {
+                if (l <= j) continue;
+                const double A = (alpha ? alpha[l] * aj : 0.0) - G[l * ldg + j];
+                add(FAST ? xc : xj, x + l * ldx, A);
+            }
+        }
+    }
+    __syncthreads();                                      // the row part's out[] stores are visible to the whole CTA
+#pragma unroll
+    for (int k = 0; k < dk; ++k) {
+        if (k >= d) break;                                // uniform: the barriers below are reached by every thread
+        red[warp][lane] = acc[k];
+        __syncthreads();
+        if (warp == 0 && j < N) {
+            double v = 0.0;
+#pragma unroll
+            for (int w = 0; w < NT / 32; ++w) v += red[w][lane];
+            out[j * d + k] += v;
+        }
+        __syncthreads();
+    }
+}
+
 // strict-upper tiles of the Npad x Npad matrix F <- transpose of its strict-lower tiles (diagonal tiles untouched)
 __global__ void mirror_lower_tiles_kernel(double* __restrict__ F, long long ld) {
     __shared__ double tl[32][33];
@@ -786,6 +894,19 @@ cudaError_t inducing_dx_launch(const KProg& P, const double* u, int64_t ldu, int
     if (M <= 0) return cudaSuccess;
     if (d <= 0 || d > GPB200_MAX_DIMS || n < 0) return cudaErrorInvalidValue;
     inducing_dx_kernel<<<(unsigned)M, DX_NT, 0, st>>>(P, u, ldu, z, ldz, n, d, W, ldw, sym, mask, out, accumulate);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t inputs_dx_launch(const KProg& P, bool fast, const double* x, int64_t ldx, int d, int64_t N, const double* alpha,
+                             const double* G, int64_t ldg, double* out, cudaStream_t st, int64_t* launches, int bm_mod,
+                             int bm_rem, int bm_div) {
+    if (N <= 0) return cudaSuccess;
+    if (d <= 0 || d > GPB200_MAX_DIMS || (fast && (!kprog_fast(P, d) || d > 8))) return cudaErrorInvalidValue;
+    if (bm_div < 1) bm_div = 1;
+    const unsigned grid = (unsigned)((N + IX_PB - 1) / IX_PB);
+    if (fast) inputs_dx_kernel<true><<<grid, NT, 0, st>>>(P, x, ldx, d, N, alpha, G, ldg, out, bm_mod, bm_rem, bm_div);
+    else inputs_dx_kernel<false><<<grid, NT, 0, st>>>(P, x, ldx, d, N, alpha, G, ldg, out, bm_mod, bm_rem, bm_div);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

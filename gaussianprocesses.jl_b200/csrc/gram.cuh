@@ -48,5 +48,12 @@ cudaError_t crossgram_dx_launch(const KProg& P, const double* xs, int64_t ldxs, 
 cudaError_t inducing_dx_launch(const KProg& P, const double* u, int64_t ldu, int64_t M, const double* z, int64_t ldz, int64_t n,
                                int d, const double* W, int64_t ldw, int sym, const double* mask, double* out, int accumulate,
                                cudaStream_t st, int64_t* launches);
+// training-input gradient (N x d output, point-major), over the lower triangle of A = a a' - G (a = alpha, 0 when null):
+//   out[i, :] = sum_{j <= i} A_ij dk(x_i, x_j)/dx_i + sum_{l > i} A_li dk(x_i, x_l)/dx_i
+// reading only the tile rows t with ((t / bm_div) % bm_mod) == bm_rem (all when bm_mod <= 1; the others count 0) and no row
+// or column >= N.  fast: the single-SEIso specialisation (needs kprog_fast(P, d) and d <= 8).  Fixed-order sums.
+cudaError_t inputs_dx_launch(const KProg& P, bool fast, const double* x, int64_t ldx, int d, int64_t N, const double* alpha,
+                             const double* G, int64_t ldg, double* out, cudaStream_t st, int64_t* launches, int bm_mod,
+                             int bm_rem, int bm_div);
 // F[j, i] = F[i, j] for every element of the strict-lower 128-tiles of the Npad x Npad matrix F (diagonal tiles untouched)
 cudaError_t mirror_lower_tiles_launch(double* F, int64_t ld, int64_t Npad, cudaStream_t st, int64_t* launches);

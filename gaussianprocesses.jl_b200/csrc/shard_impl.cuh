@@ -298,7 +298,7 @@ void free_FG(gpb200_handle* h) {
     }
     h->F = h->G = nullptr;
     h->sharded = false;
-    h->factored = h->inv_ready = false;
+    h->factored = h->inv_ready = h->s_ready = false;
 }
 
 bool make_FG_maps(gpb200_handle* h) {

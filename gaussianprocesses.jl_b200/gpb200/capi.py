@@ -37,6 +37,7 @@ _SIGNATURES = {
     "gpb200_mll": (C.c_int, [_H, _dp, _dp, _dp]),
     "gpb200_grad_prepare": (C.c_int, [_H]),
     "gpb200_grad_kernel": (C.c_int, [_H, _dp, _dp, _dp]),
+    "gpb200_grad_inputs": (C.c_int, [_H, _dp, _dp]),
     "gpb200_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
     "gpb200_predict_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp, _dp]),
     "gpb200_rand": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, C.c_int64, _dp, C.c_double, _dp, _dp]),
@@ -230,6 +231,14 @@ class Engine:
         self._check(self._lib.gpb200_grad_kernel(self._h, ap, _as_dp(g), C.byref(tr)), "grad_kernel")
         return g[:self.n_theta].copy(), tr.value
 
+    def grad_inputs(self, alpha=None):
+        """(N, d): sum_j A_ij dk(x_i, x_j)/dx_i with A = alpha alpha' - K_y^-1 after grad_prepare, or A = S after gpa_grad
+        with the kernel gradient (alpha must then be None); the mean's part is the caller's"""
+        out = np.empty((self.N, self.d))
+        ap = _as_dp(np.ascontiguousarray(alpha, dtype=np.float64)) if alpha is not None else None
+        self._check(self._lib.gpb200_grad_inputs(self._h, ap, _as_dp(out)), "grad_inputs")
+        return out
+
     def predict(self, xs_pm, alpha=None, want_var=True, full_cov=False):
         xs_pm = np.ascontiguousarray(xs_pm, dtype=np.float64)
         M, d = xs_pm.shape
@@ -352,12 +361,12 @@ class Engine:
         return np.tril(K)
 
     def timings(self):
-        ms = np.zeros(16)
-        self._check(self._lib.gpb200_get_timings(self._h, _as_dp(ms), 16), "get_timings")
+        ms = np.zeros(17)
+        self._check(self._lib.gpb200_get_timings(self._h, _as_dp(ms), 17), "get_timings")
         return dict(gram=ms[0], cholesky=ms[1], solve_mll=ms[2], inverse=ms[3], trace=ms[4], predict=ms[5],
                     gemm_launches=ms[6], gemm_ms=ms[7], gemm_flops=ms[8], gpa_scan=ms[9], gpa_product=ms[10],
                     pgrad_crossgram=ms[11], pgrad_trsm=ms[12], pgrad_transpose=ms[13], pgrad_trsm_right=ms[14],
-                    pgrad_contract=ms[15])
+                    pgrad_contract=ms[15], grad_inputs=ms[16])
 
     def set_stream(self, cuda_stream):
         """Run on the caller's CUDA stream (int handle, e.g. torch.cuda.current_stream().cuda_stream); 0/None = private."""
@@ -779,6 +788,9 @@ class LocalGroupEngine:
 
     def grad_kernel(self, *a, **k):
         return self.lead.grad_kernel(*a, **k)
+
+    def grad_inputs(self, *a, **k):
+        return self.lead.grad_inputs(*a, **k)
 
     def predict(self, *a, **k):
         return self.lead.predict(*a, **k)

@@ -67,10 +67,11 @@ class GPA:
     def update_cK(self):
         """update_cK!(gp::GPA) (GPA.jl:111-114): Gram + exp(2 * -20) nugget + Cholesky on the device."""
         self._eng.factorize(flatten(self.kernel, self.dim)[2], -20.0)
+        self._inputs_moved = False
 
-    def update_ll(self, process=True, lik=True, domean=True, kern=True):
-        """update_ll!(gp) (GPA.jl:118-128)."""
-        if kern:
+    def update_ll(self, process=True, lik=True, domean=True, kern=True, inputs=False):
+        """update_ll!(gp) (GPA.jl:118-128).  After set_params(..., inputs=True) the factor is refreshed whatever kern says."""
+        if kern or getattr(self, "_inputs_moved", False):
             self.update_cK()
         self.mu = self.mean.mean(self._xpm)
         self.ll = float(np.sum(self.lik.log_dens(self._f(), self.y)))
@@ -84,18 +85,20 @@ class GPA:
         self.target = self.ll + self._prior_v()
         return self
 
-    def update_target(self, process=True, lik=True, domean=True, kern=True):      # GPA.jl:261-266
+    def update_target(self, process=True, lik=True, domean=True, kern=True, inputs=False):      # GPA.jl:261-266
         self.update_ll(process=process, lik=lik, domean=domean, kern=kern)
         self.target = self.ll + self._prior_v()
         return self
 
-    def update_dll(self, process=True, lik=True, domean=True, kern=True):
-        """update_dll!(gp, precomp) (GPA.jl:183-228): [L' dl_df; sum dlog_dens_dθ; dmll_mean!; dll_kern!]."""
+    def update_dll(self, process=True, lik=True, domean=True, kern=True, inputs=False):
+        """update_dll!(gp, precomp) (GPA.jl:183-228): [L' dl_df; sum dlog_dens_dθ; dmll_mean!; dll_kern!].  inputs=True (not
+        in the reference) appends dll/dX as vec(X): sum_j S_ij dk(x_i, x_j)/dx_i over the S that the kernel gradient forms on
+        the device, plus (dl_df)_i dm(x_i)/dx_i."""
         f = self._f()                                                   # precompute! (GPA.jl:158-163)
         dl_df = self.lik.dlog_dens_df(f, self.y)
         u, gk = None, None
-        if process or kern:
-            u, gk = self._eng.gpa_grad(self.v, dl_df, process=process, kern=kern)
+        if process or kern or inputs:
+            u, gk = self._eng.gpa_grad(self.v, dl_df, process=process, kern=kern or inputs)
         out = []
         if process:
             out.extend(u)
@@ -105,6 +108,8 @@ class GPA:
             out.extend(self.mean.grad_stack(self._xpm).T @ dl_df)
         if kern:
             out.extend(gk[self._exposed])                               # FixedKernel selection, fixed_kernel.jl:64-66
+        if inputs:
+            out.extend((self._eng.grad_inputs() + dl_df[:, None] * self.mean.grad_x(self._xpm)).ravel())
         self.dll = np.array(out, dtype=np.float64)
         return self
 
@@ -121,7 +126,8 @@ class GPA:
         return self
 
     # ---- parameters ----------------------------------------------------------------------
-    def get_params(self, lik=True, domean=True, kern=True):             # GPA.jl:336-349
+    def get_params(self, lik=True, domean=True, kern=True, inputs=False):             # GPA.jl:336-349
+        """inputs=True (not in the reference) appends vec(X), one point after another."""
         p = list(self.v)
         if lik and self.lik.num_params() > 0:
             p.extend(self.lik.get_params())
@@ -129,10 +135,12 @@ class GPA:
             p.extend(self.mean.get_params())
         if kern:
             p.extend(self.kernel.get_params())
+        if inputs:
+            p.extend(self._xpm.ravel())
         return np.array(p, dtype=np.float64)
 
-    def num_params(self, lik=True, domean=True, kern=True):             # GPA.jl:351-357
-        n = self.nobs
+    def num_params(self, lik=True, domean=True, kern=True, inputs=False):             # GPA.jl:351-357
+        n = self.nobs + (self.dim * self.nobs if inputs else 0)
         if lik:
             n += self.lik.num_params()
         if domean:
@@ -141,8 +149,19 @@ class GPA:
             n += self.kernel.num_params()
         return n
 
-    def set_params(self, hyp, process=True, lik=True, domean=True, kern=True):     # GPA.jl:359-381
+    def set_params(self, hyp, process=True, lik=True, domean=True, kern=True, inputs=False):     # GPA.jl:359-381
+        """inputs=True: the last dim * nobs entries are vec(X), uploaded in place; the next update_ll refactorises."""
         hyp = np.asarray(hyp, dtype=np.float64)
+        if inputs:
+            nx = self.dim * self.nobs
+            if hyp.size < nx:
+                raise ValueError("wrong number of parameters")
+            self.set_params(hyp[:hyp.size - nx], process=process, lik=lik, domean=domean, kern=kern)
+            xpm = np.ascontiguousarray(hyp[hyp.size - nx:].reshape(self.nobs, self.dim))
+            self._eng.set_data(xpm)
+            self._xpm, self.x = xpm, xpm.T
+            self._inputs_moved = True
+            return self
         i = 0
         if process:
             self.v = hyp[:self.nobs].copy()

@@ -145,20 +145,24 @@ class GPE:
     def update_cK(self):
         """update_cK!(gp) (src/GPE.jl:169-195): Gram + noise + Cholesky on the device."""
         self._eng.factorize(self._theta_full(), self.logNoise)
+        self._inputs_moved = False
 
     def update_mll(self, noise=True, domean=True, kern=True):
-        """update_mll!(gp) (src/GPE.jl:202-212)."""
-        if kern or noise:
+        """update_mll!(gp) (src/GPE.jl:202-212).  After set_params(..., inputs=True) the factor is refreshed whatever
+        kern and noise say: it belongs to the old inputs."""
+        if kern or noise or getattr(self, "_inputs_moved", False):
             self.update_cK()
         mu = self.mean.mean(self._xpm)
         self.alpha, self.mll = self._eng.mll(self.y - mu)
         return self
 
-    def update_dmll(self, noise=True, domean=True, kern=True):
-        """update_dmll!(gp, precomp) (src/GPE.jl:298-324)."""
+    def update_dmll(self, noise=True, domean=True, kern=True, inputs=False):
+        """update_dmll!(gp, precomp) (src/GPE.jl:298-324).  inputs=True (not in the reference) appends dmll/dX as vec(X), one
+        point after another: sum_j A_ij dk(x_i, x_j)/dx_i from the device plus alpha_i dm(x_i)/dx_i."""
         gk_full, trA = None, None
-        if noise or kern:                                         # mean-only gradient needs neither K^-1 nor the trace
+        if noise or kern or inputs:                               # mean-only gradient needs neither K^-1 nor the trace
             self._eng.grad_prepare()                              # precompute! -> get_ααinvcKI!
+        if noise or kern:
             gk_full, trA = self._eng.grad_kernel()                # dmll_kern! + tr(A)
         out = []
         if noise:
@@ -169,12 +173,15 @@ class GPE:
             out.extend(self.mean.grad_stack(self._xpm).T @ self.alpha)      # dmll_mean!, GPE.jl:282-288
         if kern:
             out.extend(gk_full[self._exposed])                     # FixedKernel selection, fixed_kernel.jl:64-66
+        if inputs:
+            gx = self._eng.grad_inputs() + self.alpha[:, None] * self.mean.grad_x(self._xpm)
+            out.extend(gx.ravel())
         self.dmll = np.array(out, dtype=np.float64)
         return self
 
-    def update_mll_and_dmll(self, **kw):                           # GPE.jl:332-335
-        self.update_mll(**kw)
-        self.update_dmll(**kw)
+    def update_mll_and_dmll(self, noise=True, domean=True, kern=True, inputs=False):     # GPE.jl:332-335
+        self.update_mll(noise=noise, domean=domean, kern=kern)
+        self.update_dmll(noise=noise, domean=domean, kern=kern, inputs=inputs)
         return self
 
     def initialise_target(self):                                   # GPE.jl:346-349 (no priors in this mirror)
@@ -347,7 +354,8 @@ class GPE:
         return (draws + self.mean.mean(xs)[None, :]).T
 
     # ---- parameters ----------------------------------------------------------------------
-    def get_params(self, noise=True, domean=True, kern=True):      # GPE.jl:447-458
+    def get_params(self, noise=True, domean=True, kern=True, inputs=False):      # GPE.jl:447-458
+        """inputs=True (not in the reference) appends vec(X), Julia's column-major vec of the dim x nobs matrix."""
         p = []
         if noise:
             p.extend(np.atleast_1d(self.logNoise))
@@ -355,13 +363,27 @@ class GPE:
             p.extend(self.mean.get_params())
         if kern:
             p.extend(self.kernel.get_params())
+        if inputs:
+            p.extend(self._xpm.ravel())
         return np.array(p, dtype=np.float64)
 
     def num_params(self, **kw):
         return self.get_params(**kw).size
 
-    def set_params(self, hyp, noise=True, domean=True, kern=True):  # GPE.jl:492-510
+    def set_params(self, hyp, noise=True, domean=True, kern=True, inputs=False):  # GPE.jl:492-510
+        """inputs=True: the last dim * nobs entries are vec(X); they are uploaded in place (same N and d: no device buffer
+        is reallocated) and the next update_mll refactorises."""
         hyp = np.asarray(hyp, dtype=np.float64)
+        if inputs:
+            nx = self.dim * self.nobs
+            if hyp.size != self.num_params(noise=noise, domean=domean, kern=kern) + nx:
+                raise ValueError("wrong number of hyper-parameters")
+            self.set_params(hyp[:hyp.size - nx], noise=noise, domean=domean, kern=kern)
+            xpm = np.ascontiguousarray(hyp[hyp.size - nx:].reshape(self.nobs, self.dim))
+            self._eng.set_data(xpm)
+            self._xpm, self.x = xpm, xpm.T
+            self._inputs_moved = True
+            return self
         i = 0
         if noise:
             n = np.size(self.logNoise)
@@ -380,13 +402,17 @@ class GPE:
         return self
 
     # ---- optimisation (src/optimize.jl:19-97) ----------------------------------------------
-    def optimize(self, noise=True, domean=True, kern=True, maxiter=100, **kw):
+    def optimize(self, noise=True, domean=True, kern=True, maxiter=100, inputs=False, **kw):
         """optimize!(gp): L-BFGS on -target with the reference's exception filter (PosDefException / ArgumentError ->
         rejected step, parameters rolled back, optimize.jl:46-87).  Optim.jl's line search backs off from the
-        reference's `Inf`; scipy's L-BFGS-B stops on it, so a large finite penalty plays that role here."""
+        reference's `Inf`; scipy's L-BFGS-B stops on it, so a large finite penalty plays that role here.  inputs=True also
+        moves the training inputs; a step that makes K_y singular (two inputs meeting under small noise) is rejected and
+        X rolled back with the rest."""
         from scipy.optimize import minimize
 
         flags = dict(noise=noise, domean=domean, kern=kern)
+        if inputs:
+            flags["inputs"] = True
         best = {"f": None}
 
         def fg(hyp):

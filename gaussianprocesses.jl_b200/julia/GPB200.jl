@@ -184,6 +184,28 @@ end
 dmll_noise(gp::GPE, pre::B200Precompute, ::B200Covariance) =                      # src/GPE.jl:273-281
     exp(2 * GaussianProcesses.get_value(gp.logNoise)) * pre.trA
 
+# Training inputs as parameters (not in the reference, which gets dmll/dX only by differentiating its Julia cov!):
+# dmll_inputs returns dmll/dX (dim x N) of the last update_target! -- sum_j A_ij dk(x_i, x_j)/dx_i on the device
+# (gpb200_grad_inputs over the resident A = alpha alpha' - K^-1) plus alpha_i dm(x_i)/dx_i, the mean's part through the
+# reference's own mean(gp.mean, x) on Duals.  For B200GPA: the target's gradient, sum_j S_ij dk(x_i, x_j)/dx_i over the S
+# of the last update_dtarget! (kern=true) plus (dl_df)_i dm(x_i)/dx_i.
+function mean_dx(m::Mean, x::AbstractMatrix)
+    g = Matrix{Float64}(undef, size(x)...)
+    for i in 1:size(x, 2)
+        g[:, i] = ForwardDiff.gradient(z -> mean(m, reshape(z, :, 1))[1], Vector{Float64}(x[:, i]))
+    end
+    return g
+end
+
+function dmll_inputs(gp::GPE{X,Y,M,K,CS,D,P}) where {X,Y,M,K,CS<:B200Covariance,D,P}
+    cK = gp.cK
+    check(cK, ccall((:gpb200_grad_prepare, LIB), Cint, (Ptr{Cvoid},), cK.handle), "grad_prepare")   # no-op when resident
+    g = Matrix{Float64}(undef, gp.dim, gp.nobs)
+    check(cK, ccall((:gpb200_grad_inputs, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}),
+                    cK.handle, Vector{Float64}(gp.alpha), g), "grad_inputs")
+    return g .+ mean_dx(gp.mean, gp.x) .* reshape(gp.alpha, 1, :)
+end
+
 # leave-one-out predictions (src/crossvalidation.jl:8-13) without materialising inv(Σ) on the host
 function GaussianProcesses.predict_LOO(cK::B200PDMat, alpha::AbstractVector{<:Real}, y::AbstractVector{<:Real})
     check(cK, ccall((:gpb200_grad_prepare, LIB), Cint, (Ptr{Cvoid},), cK.handle), "grad_prepare")
@@ -769,6 +791,15 @@ function update_dtarget!(gp::B200GPA; process::Bool=true, lik::Bool=true, domean
     return gp
 end
 
+function dmll_inputs(gp::B200GPA)
+    cK = gp.cK
+    g = Matrix{Float64}(undef, gp.dim, gp.nobs)
+    check(cK, ccall((:gpb200_grad_inputs, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}),
+                    cK.handle, C_NULL, g), "grad_inputs")                          # A = S: alpha must be NULL
+    dl_df = Vector{Float64}(dlog_dens_df(gp.lik, unwhiten_dev(cK, gp.v) + gp.μ, gp.y))
+    return g .+ mean_dx(gp.mean, gp.x) .* reshape(dl_df, 1, :)
+end
+
 function update_target_and_dtarget!(gp::B200GPA; kwargs...)                       # GPA.jl:283-291
     update_target!(gp; kwargs...)
     update_dtarget!(gp; kwargs...)
@@ -830,6 +861,6 @@ function predict_y(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)        
     return predict_obs(gp.lik, μ, σ2)
 end
 
-export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA, set_inducing!, dmll_inducing
+export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA, set_inducing!, dmll_inducing, dmll_inputs
 
 end # module

@@ -113,6 +113,18 @@ int  gpb200_grad_prepare(gpb200_handle* h);
  * dmll_kernel[p] = 1/2 sum_ij A_ij dK_ij/dtheta_p, A = alpha alpha' - K_y^-1;  *trA = tr(A).
  * `alpha` may be NULL to use the alpha left resident by gpb200_mll.                          */
 int  gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kernel, double* trA);
+/* dmll/dX (N x d, point-major == Julia's d x N column-major) of the kernel part: sum_j A_ij dk(x_i, x_j)/dx_i.
+ * After gpb200_grad_prepare: A = alpha alpha' - K_y^-1 (alpha as in gpb200_grad_kernel: given, or the resident one).
+ * After gpb200_gpa_grad with dll_kernel != NULL: A = S (alpha must be NULL).  Otherwise GPB200_ESTATE.
+ * Collective on multi-rank and row-sharded handles; every rank returns the full array.
+ * Not in the reference (which differentiates its Julia cov! automatically).  The noise terms do not depend on x; the mean's
+ * part alpha_i dm(x_i)/dx_i (GPA: (dl_df)_i dm(x_i)/dx_i) is the caller's.  At coincident inputs the stationary kernels
+ * contribute the limit of their derivative (0), as in gpb200_predict_grad.  Each stored entry of A's lower triangle is read
+ * twice, nothing else of G; the tile rows are split over the ranks as by gpb200_grad_kernel and the N x d partials are
+ * summed once.  Sums run in a fixed order: repeated calls are bitwise equal.  GPB200_EINVAL for a NULL dmll_x or an alpha
+ * in the S state.  Reads F, G and alpha only (a given alpha is not kept): every later call behaves as without this one.
+ * Device memory grows by (N + N d) doubles on the first call (in-process groups: + nranks N d for the sum).  Timing slot 16. */
+int  gpb200_grad_inputs(gpb200_handle* h, const double* alpha, double* dmll_x);
 
 /* ---- predictMVN / predict_f (src/GP.jl:25-79) ---------------------------------------------
  * xs: d x M column-major test inputs (leading dim ldxs).  mu_minus_mean[M] = K*' alpha;
@@ -192,10 +204,11 @@ int  gpb200_get_inverse_diag(gpb200_handle* h, double* diag);
  * [9] gpb200_gpa_grad's scans  [10] its S = W'Z GEMM
  * gpb200_predict_grad (summed over chunks): [11] cross-Gram + mean  [12] V' = K*' L^-T + variance  [13] L' into F's upper
  * tiles  [14] W' = V' L^-1  [15] gradient contraction
+ * [16] gpb200_grad_inputs (contraction and, on several ranks, the sum of the partials)
  * with option "profile"=1, accumulated since the option was set:
  * [6] number of DMMA GEMM launches  [7] sum of their device durations (ms, CUDA events around
  * every launch)  [8] FP64 flops those launches executed (tile-granular)                       */
-int  gpb200_get_timings(gpb200_handle* h, double* ms, int32_t n);
+int  gpb200_get_timings(gpb200_handle* h, double* ms, int32_t n);   /* writes min(n, 17) entries */
 /* number of kernels enqueued by calls on this handle since creation (gpb200_rand includes its M x M sub-engine's
  * Cholesky); cudaMemsetAsync and copies are not counted */
 int64_t gpb200_launch_count(gpb200_handle* h);
