@@ -1,0 +1,313 @@
+// engine.cuh -- private to the engine's translation units; not installed and not part of the ABI.
+//   gpb200.cu            the dense engine (gpb200_handle) and its C ABI: schedules, IPC / NCCL, in-process groups
+//   kernel_contracts.cu  the raw kernels exposed for the parity tests and the roofline bench (include/gpb200.h)
+//   fitc_engine.cu       the sparse handle (gpb200_fitc): FITC / DTC / SoR, sparse cross-validation, rand
+//   fsa_engine.cu        the FSA schedule of the sparse handle (mode 3)
+// It holds the handle structs, the error path, and the declarations of what one unit uses from another.
+#pragma once
+#include <cuda.h>
+#include <cuda_runtime.h>
+#include <nccl.h>
+#include <stdio.h>
+#include <string>
+#include <vector>
+
+#include "../../include/gpb200.h"
+#include "gemm_nt.cuh"
+#include "kprog.cuh"
+
+// a virtual address range backed by physical memory only where `runs` say so (CUDA VMM: cuMemAddressReserve / cuMemMap)
+struct VmBuf {
+    CUdeviceptr base = 0;
+    size_t va_size = 0;
+    std::vector<std::pair<size_t, size_t>> runs;          // (offset, bytes) of every mapped run
+    std::vector<CUmemGenericAllocationHandle> handles;    // one physical allocation per run
+};
+
+struct gpb200_handle {
+    int device = 0;
+    cudaStream_t st = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr, ev5 = nullptr;
+    int64_t N = 0, Npad = 0, ld = 0;
+    int d = 0;
+    double* x = nullptr;
+    KProg prog{};
+    std::vector<double> theta;
+    bool has_data = false, has_kernel = false, factored = false, inv_ready = false, alpha_ready = false;
+    bool s_ready = false;                      // G's lower triangle holds -S of gpb200_gpa_grad (A = S for gpb200_grad_inputs)
+    double *F = nullptr, *G = nullptr, *Dinv = nullptr, *DinvT = nullptr, *logd = nullptr;
+    double *noise_var = nullptr, *r0 = nullptr, *r1 = nullptr, *y1 = nullptr, *alpha = nullptr, *scal = nullptr;
+    double *part = nullptr, *trace_out = nullptr;
+    double* tblk = nullptr;                    // Npad scratch vector (block right-hand sides of the sharded solves)
+    double* ZdT = nullptr;                     // gpb200_gpa_grad: Npad x 128 clean upper diagonal tiles of Z' (allocated on first use)
+    CUtensorMap mapZdT{};
+    // TMA-staged SEIso kernels (gram_fast.cu): inputs stored [Npad x dxp] with an even, zero-padded dxp <= 8
+    double *xp = nullptr, *xpt = nullptr;      // [Npad x dxp] and its transpose [dxp x Npad]
+    int dxp = 0;
+    CUtensorMap mapX{}, mapXT{};
+    bool xmap_ok = false;
+    int64_t capacity = 0;                      // option "capacity": rows reserved for gpb200_append (ElasticGPE's capacity)
+    int gram_fast = 1;                         // option "gram_fast": 0 = always the generic kernels of gram.cu
+    // cross-validation (gpb200_cv_*): K_y^-1 mirrored to a full symmetric matrix in G; two N x N temporaries
+    bool g_sym = false;
+    bool cv_m_ok = false;                                       // cvD holds M_j = Z_j K^-1 of the last cv_param call
+    double *cvD = nullptr, *cvY = nullptr;
+    CUtensorMap mapCvD{}, mapCvY{};
+    double* cvblk = nullptr; long long* cvidx = nullptr; int64_t cvblk_cap = 0, cvidx_cap = 0;   // capacities in elements
+    // posterior sampling (gpb200_rand): M x M sub-engine for chol(Sigma* + nugget I), normal draws / samples staging
+    gpb200_handle* sub = nullptr;
+    bool cov_keep_device = false;              // predict: leave the full covariance in Kss (no D2H)
+    double *rz = nullptr, *rout = nullptr;
+    int64_t rz_rows = 0, rz_cols = 0;
+    CUtensorMap mapRz{};
+    int* info_dev = nullptr;
+    int* flags = nullptr;                      // ready-flags of the single-launch triangular solves (2 x (Npad/128 + 1))
+    int trsv_fused = 1;
+    int max_resident_ctas = 0;
+    int64_t n_noise = 1;
+    double nugget = 0.0;
+    CUtensorMap mapF{}, mapG{}, mapDinv{}, mapDinvT{};
+    bool tma_ok = false;
+    // predict workspace
+    double *xs = nullptr, *Kst = nullptr, *Kss = nullptr, *pmu = nullptr, *pvar = nullptr, *pkdiag = nullptr;
+    int64_t xs_cap = 0, Kst_rows = 0, Kss_rows = 0;
+    double* pdx = nullptr; int64_t pdx_rows = 0;   // gpb200_predict_grad: dmu (Mpad x d), then dvar (Mpad x d)
+    // gpb200_grad_inputs (first use, freed with the data): a caller's alpha (Npad), the N x d result (Npad x d), and in an
+    // in-process group the gathered ranks' results (nranks x Npad x d)
+    double* dxin = nullptr;
+    CUtensorMap mapKst{};
+    // options
+    int nb = 0;                 // outer Cholesky block; 0 = fully recursive (one panel)
+    int gemm_impl = 0;
+    int lookahead = 1;          // factor the next diagonal tile on a side stream while the Schur update runs
+    cudaStream_t st_side = nullptr;            // high-priority stream of the look-ahead chain
+    cudaStream_t st_cur = nullptr;             // stream launch_gemm / the leaf use right now (st or st_side)
+    cudaEvent_t ev_la0 = nullptr, ev_la2 = nullptr;
+    // stats
+    double ms[17] = {};
+    int64_t launches = 0;
+    bool own_stream = true;
+    // per-launch GEMM profiling (option "profile"): event pairs + executed flops of every GEMM launch
+    int profile = 0;
+    std::vector<cudaEvent_t> pev;
+    size_t pev_used = 0;
+    double gemm_flops_exec = 0.0;
+    int64_t gemm_launches = 0;
+    // multi-GPU (one process per GPU): replicated F/G, block-column ownership, NCCL over NVLink
+    int nranks = 1, rank = 0;
+    ncclComm_t comm = nullptr;
+    cudaStream_t st_comm = nullptr;
+    int dist_nb = 0;                           // width of an owned block column; 0 = auto (~Npad/(8*nranks))
+    double* pack[2] = {nullptr, nullptr};      // panel staging (double buffered)
+    size_t pack_elems = 0;
+    cudaEvent_t ev_packed[2] = {nullptr, nullptr}, ev_bcast[2] = {nullptr, nullptr}, ev_unpacked[2] = {nullptr, nullptr};
+    cudaEvent_t ev_x = nullptr, ev_y = nullptr;
+    double *ag_send = nullptr, *ag_recv = nullptr;
+    size_t ag_send_elems = 0, ag_recv_elems = 0;
+    // fused panel broadcast over NVLink peer memory (CUDA IPC): peers' F / Dinv / DinvT / logd / signal words
+    bool p2p = false;
+    int n_peer = 0;
+    int peer_rank[7] = {0, 0, 0, 0, 0, 0, 0};
+    double *peer_F[7] = {}, *peer_Dinv[7] = {}, *peer_DinvT[7] = {}, *peer_logd[7] = {};
+    int* peer_sig[7] = {};
+    int* sig = nullptr;                        // sig[q] = last panel published by rank q (epoch * 65536 + b + 1); sig[8] = watchdog
+    int epoch = 0;
+    int** peer_sig_dev = nullptr;              // device array: &peer_sig[q][rank]
+    bool push_panel = false;                   // set while the owner factors a panel: leaf + leaf TRSM also store to the peers
+    // ---- row-sharded storage (shard_impl.cuh): F / G are virtual address ranges, physical pages exist for owned rows only ----
+    int shard_opt = -1;                        // option "shard": -1 auto (when replicated F+G would not fit), 0 never, 1 always
+    int shard_rb_opt = 0;                      // option "shard_rb": ownership block in 128-row tiles (0 = auto)
+    bool sharded = false;                      // current storage mode of F / G
+    int rb = 4;                                // effective ownership block (tiles); panel width NBp = 128 * rb
+    int row_lim = 0;                           // chol_panel: rows below this limit only (diagonal block of a sharded panel); 0 = Npad
+    VmBuf vmF, vmG;
+    VmBuf vmCvY, vmCvM;                        // cross-validation work matrices (Y' = K^-1 dK_j, lower triangle of M_j), own rows only
+    CUtensorMap mapShCvY{}, mapShCvM{};
+    double* P[4] = {nullptr, nullptr, nullptr, nullptr};   // panel buffers, Npad x NBp (global row order); P[1], P[3] double as NBp x Npad row panels
+    double* Sbuf = nullptr;                    // all-gather staging: nranks regions of S_per_rank doubles; scratch of the inverse sweep
+    size_t S_per_rank = 0;
+    CUtensorMap mapP[4] = {}, mapXR[2] = {}, mapS{};
+    double* XRbig[2] = {nullptr, nullptr};     // row-panel forms X_J of a BATCH of panels (inverse sweep: batched LAUUM part)
+    int xr_batch = 1;                          // panels per batch
+    CUtensorMap mapXRbig[2] = {};
+    double* red = nullptr;                     // small reduction scratch (local group all-reduce)
+    int* redi = nullptr;
+    struct gpb200_group* grp = nullptr;        // in-process group of virtual ranks on one device (gpb200_group_create)
+    std::vector<cudaEvent_t> evring;
+    size_t evring_next = 0;
+    std::string err;
+};
+
+// in-process "communicator": R handles on one device acting as R ranks of the sharded schedules, driven in lock step by
+// one host thread.  Collectives are device-to-device copies ordered by events (shard_impl.cuh).
+struct gpb200_group {
+    std::vector<gpb200_handle*> hs;
+};
+
+
+// ---- FITC (sparse/fully_indep_train_conditional.jl): two dense M x M sub-engines + N-chunk streaming ----
+struct gpb200_fitc {
+    gpb200_handle* eu = nullptr;     // K_uu  (+1e-10 I)            -> L_uu
+    gpb200_handle* es = nullptr;     // Sigma_QR = K_uf L^-1 K_fu + K_uu (+1e-10 I) -> L_s
+    int device = 0;
+    int64_t N = 0, M = 0, Mpad = 0, Nc = 0;
+    int d = 0;
+    double *x = nullptr, *xs = nullptr, *lam = nullptr, *y = nullptr, *alpha = nullptr, *tmpn = nullptr;
+    double *w = nullptr, *tmpc = nullptr, *zeroc = nullptr, *tmpc2 = nullptr;          // Nc
+    double *bvec = nullptr, *uvec = nullptr, *tmpm = nullptr, *rhsm = nullptr, *scal = nullptr;   // Mpad
+    double *bufA = nullptr, *bufB = nullptr;   // Nc x Mpad (K_fu chunk) ; Mpad x Nc (K_uf chunk)
+    CUtensorMap mapA{}, mapB{}, mapB2{};
+    // kernel-gradient workspace (allocated on first use)
+    double *bufC = nullptr, *Hbuf = nullptr, *Wbuf = nullptr, *Tbuf = nullptr, *gvec = nullptr, *betav = nullptr;
+    double *gpart = nullptr, *gacc = nullptr, *gtmp = nullptr;
+    CUtensorMap mapAt{}, mapC{}, mapCt{}, mapH{}, mapT{};
+    bool grad_ws = false;
+    double* Kss = nullptr; int64_t Kss_rows = 0;      // full predictive covariance (gpb200_fitc_predict_cov)
+    double* pdx = nullptr;                            // gpb200_fitc_predict_grad: dmu, dvar of a chunk (2 x Nc x d; first use)
+    // posterior sampling (gpb200_fitc_rand): the Ms x Ms sub-engine and the staging of the draws are eu's (rand_from_cov)
+    bool cov_keep_device = false;                     // predict_fsa: leave Sigma* in caller order on the device (fsa->Sc)
+    double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
+    double fsag_ms[4] = {0, 0, 0, 0};                 // last predict_fsa_grad, summed over test chunks: predict_fsa's
+                                                      // launches, s + second sweep, K_uu^-1 TRSMs, contraction
+    // inducing-point gradient (gpb200_fitc_grad_kernel_inducing; first use): dmll/dXu accumulator (M x d), the events
+    // around the call (0, 1) and around each contraction launch (2k, 2k + 1 for k >= 1), and the device times of the last
+    // call: the contractions summed, the whole call
+    double* dxu = nullptr;
+    std::vector<cudaEvent_t> xu_ev;
+    double xu_ms[2] = {0, 0};
+    // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
+    // buffer the likelihood, gradient and prediction schedules keep):
+    //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
+    //   cvCh Nc x Mpad: Ch = L^-1 K_fu S^-1;  cvP Nc x Mpad: Ch Q (pass 2) or E (fold blocks)
+    //   Mpad x Mpad: cvDuu = dK_uu, cvDp = dK_uu K_uu^-1, cvR = K_uf L^-1 G, cvH = K_uf L^-1 Delta L^-1 K_fu, cvQ = H - R - R'
+    double *cvG = nullptr, *cvGt = nullptr, *cvCh = nullptr, *cvP = nullptr;
+    double *cvDuu = nullptr, *cvDp = nullptr, *cvR = nullptr, *cvH = nullptr, *cvQ = nullptr;
+    double *cvalpha = nullptr, *cvdel = nullptr, *cvilam = nullptr, *cvza = nullptr, *cvdg = nullptr;   // N + Nc
+    double *cvda = nullptr, *cvq = nullptr, *cvlamV = nullptr, *cvdelV = nullptr, *cvxs = nullptr;     // Nc (cvxs: Nc x d)
+    double* cvm = nullptr;                            // 8 x Mpad: K_uf alpha, G' alpha, K_uf L^-1 Delta alpha, beta, R beta, w, tmp
+    double* cvout = nullptr; int64_t cvout_rows = 0;  // fold block (padded nV x padded nV)
+    long long* cvidx = nullptr;
+    CUtensorMap mapCvG{}, mapCvGt{}, mapCvCh{}, mapCvP{}, mapCvDuu{}, mapCvDp{}, mapCvQ{};
+    bool cv_ws = false;
+    bool cv_m_ok = false;                             // cvDp / cvQ / cvdel hold the state of the last cv_param since factorize
+    int cv_param = 0;
+    // multi-GPU (gpb200_fitc_comm_init): the N observations are sharded over the ranks, every M x M object is replicated;
+    // exchanged: one all-reduce of the M x M accumulator Sigma_QR (and of H for the kernel gradient), M-vectors, scalars
+    ncclComm_t comm = nullptr;
+    int nranks = 1, rank = 0;
+    double Ntotal = 0.0;                              // observations over all ranks (mll's N log 2 pi)
+    int mode = 0;                    // 0 FITC, 1 DTC, 2 SoR (Lambda = sigma^2 I; SoR also drops K_xx - Q_xx from the predictive variance)
+    double noise_var = 0.0;
+    bool has_data = false, has_kernel = false, factored = false, alpha_ready = false;
+    std::string err;
+    struct Fsa* fsa = nullptr;       // mode 3 (FSA): training blocks and the packed block-diagonal factors (gpb200_fitc_set_blocks)
+};
+
+// shared by the units, not exported from libgpb200.so (each `namespace engine` block of the units repeats the attribute)
+namespace engine __attribute__((visibility("hidden"))) {
+
+constexpr int TILE = 128;
+constexpr int TRSV_FUSED_CTAS_PER_SM = 4;      // single-launch solves run for Npad/128 <= this x SMs (see solve_device)
+constexpr double LOG2PI = 1.8378770664093453;
+extern std::string g_create_error;     // message of the last failed gpb200_create (one instance, in gpb200.cu)
+
+// ---- NCCL, bound at run time (dlopen) so that single-GPU use has no NCCL dependency -------------
+struct NcclApi {
+    void* lib = nullptr;
+    ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
+    ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
+    ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
+    ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
+    ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
+    ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
+    const char* (*GetErrorString)(ncclResult_t) = nullptr;
+    ncclResult_t (*GroupStart)() = nullptr;
+    ncclResult_t (*GroupEnd)() = nullptr;
+    bool ok = false;
+};
+extern NcclApi g_nccl;                 // one instance, in gpb200.cu
+bool nccl_load();
+
+// "<call> failed at file:line: reason" into `err`; a CUDA failure also clears the error the runtime keeps for the next
+// cudaGetLastError.  Returns `code`.
+inline int check_failed(std::string& err, int code, const char* call, const char* file, int line, const char* reason) {
+    char buf[512];
+    snprintf(buf, sizeof buf, "%s failed at %s:%d: %s", call, file, line, reason);
+    err = buf;
+    if (code == GPB200_ECUDA) (void)cudaGetLastError();
+    return code;
+}
+inline int cuda_rc(std::string& err, cudaError_t e, const char* call, const char* file, int line) {
+    return e == cudaSuccess ? GPB200_OK : check_failed(err, GPB200_ECUDA, call, file, line, cudaGetErrorString(e));
+}
+inline int nccl_rc(std::string& err, ncclResult_t r, const char* call, const char* file, int line) {
+    return r == ncclSuccess ? GPB200_OK
+                            : check_failed(err, GPB200_ENCCL, call, file, line, g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "nccl error");
+}
+// a failure on rank q: in an in-process group the caller holds the leader (shard_entry), so q's message is copied there
+inline int rank_failed(gpb200_handle* q, int rc) {
+    if (rc && q->grp && q != q->grp->hs[0]) q->grp->hs[0]->err = q->err;
+    return rc;
+}
+
+#define TRY(rc)        do { if (int rc_ = (rc)) return rc_; } while (0)
+#define CK(call)       TRY(cuda_rc(h->err, (call), #call, __FILE__, __LINE__))
+#define CKN(call)      TRY(nccl_rc(h->err, (call), #call, __FILE__, __LINE__))
+#define SCK(q, call)   TRY(rank_failed(q, cuda_rc((q)->err, (call), #call, __FILE__, __LINE__)))
+#define SCKN(q, call)  TRY(rank_failed(q, nccl_rc((q)->err, (call), #call, __FILE__, __LINE__)))
+#define FCK(call)      TRY(cuda_rc(f->err, (call), #call, __FILE__, __LINE__))
+#define FCKN(call)     TRY(nccl_rc(f->err, (call), #call, __FILE__, __LINE__))
+
+inline int fail(gpb200_handle* h, int code, const char* msg) {
+    if (h) h->err = msg;
+    return code;
+}
+inline int fail(gpb200_fitc* f, int code, const std::string& msg) {
+    if (f) f->err = msg;
+    return code;
+}
+#define FSUB(call, who)                                                                            \
+    do {                                                                                           \
+        int rc_ = (call);                                                                          \
+        if (rc_ != GPB200_OK) { f->err = std::string(#call) + ": " + (who)->err; return rc_; }     \
+    } while (0)
+
+inline GemmBuf bufF(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapF : nullptr, h->F, h->ld}; }
+inline GemmBuf bufG(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapG : nullptr, h->G, h->ld}; }
+inline GemmBuf bufDinv(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapDinv : nullptr, h->Dinv, TILE}; }
+inline GemmBuf bufDinvT(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapDinvT : nullptr, h->DinvT, TILE}; }
+inline GemmBuf bufNone() { return GemmBuf{nullptr, nullptr, 0}; }
+
+// ---- dense engine (gpb200.cu) -------------------------------------------------------------------------------------
+cudaError_t launch_gemm(gpb200_handle* h, const GemmDesc& d);
+// C[M x N] (+)= alpha A B' on h's DMMA GEMM, A and B whole buffers from (0, 0), C (and the optional transposed copy Ct)
+// from (0, 0)
+cudaError_t gemm_whole(gpb200_handle* h, GemmBuf a, GemmBuf b, double* c, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                       double alpha, double beta, double* ct = nullptr, int64_t ldct = 0, int flags = 0);
+cudaError_t trsm_rec_buf(gpb200_handle* h, GemmBuf bk, int rows, int c0, int n);
+cudaError_t trsm_right_rec_buf(gpb200_handle* h, GemmBuf bk, int rows, int c0, int n);
+cudaError_t solve_device(gpb200_handle* h, double* rhs, double* tmp, double* out);
+int check_trsv_watchdog(gpb200_handle* h);
+int chol_inplace(gpb200_handle* h);
+int rand_from_cov(gpb200_handle* h, int64_t M, const double* cov, int64_t ldc, const double* mu, int64_t nsamp,
+                  const double* z, double nugget, double* samples);
+float ev_ms(cudaEvent_t a, cudaEvent_t b);
+
+// ---- FSA schedule of the sparse handle (fsa_engine.cu), called by the FITC entry points -----------------------------
+void fsa_free(gpb200_fitc* f);
+int fsa_check(gpb200_fitc* f, const char* who);
+int fsa_factorize(gpb200_fitc* f);
+int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, double* mll, double* logdet);
+int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise);
+int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu);
+size_t fsa_num_chunks(const gpb200_fitc* f);
+const double* fsa_cov(const gpb200_fitc* f);
+
+// ---- FITC (fitc_engine.cu), shared with the FSA schedule --------------------------------------------------------------
+cudaError_t fitc_kfu(gpb200_fitc* f, const double* xrows, int64_t nc);
+cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc);
+int xu_contract(gpb200_fitc* f, size_t k, const double* z, int64_t n, const double* W, int sym, const double* mask,
+                int accumulate);
+int xu_finish(gpb200_fitc* f, size_t k_used, double* dmll_xu);
+
+}  // namespace engine

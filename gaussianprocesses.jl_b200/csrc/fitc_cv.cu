@@ -1,5 +1,5 @@
 // fitc_cv.cu -- row kernels of the sparse engine's cross-validation (see fitc_cv.cuh).  The O(N M^2) work of the schedule
-// is DMMA GEMMs in gpb200.cu; these kernels are the O(N M) per-row epilogues between them.
+// is DMMA GEMMs in fitc_engine.cu; these kernels are the O(N M) per-row epilogues between them.
 #include "fitc_cv.cuh"
 
 namespace {

@@ -1,5 +1,5 @@
 // fitc_cv.cuh -- row kernels of the sparse engine's cross-validation schedule (gpb200_fitc_get_inverse_diag,
-// gpb200_fitc_cv_param, gpb200_fitc_cv_block; see fitc_cv.cu and the schedule in gpb200.cu).  Every reduction runs in a
+// gpb200_fitc_cv_param, gpb200_fitc_cv_block; see fitc_cv.cu and the schedule in fitc_engine.cu).  Every reduction runs in a
 // fixed order (one warp per row, lane-strided partial sums, xor butterfly), so repeated calls are bitwise equal.
 #pragma once
 #include <cuda_runtime.h>

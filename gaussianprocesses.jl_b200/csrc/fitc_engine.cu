@@ -1,0 +1,876 @@
+// fitc_engine.cu -- the sparse handle gpb200_fitc behind include/gpb200.h: FITC, DTC and SoR (modes 0-2), their
+// cross-validation and posterior draws.  The FSA schedule of the same handle (mode 3) is fsa_engine.cu.
+#include "engine.cuh"
+#include "fitc_cv.cuh"
+#include "gram.cuh"
+#include "vec.cuh"
+
+using namespace engine;
+
+extern "C" {
+// ================================================================================================
+// FITC -- Fully Independent Training Conditional (src/sparse/fully_indep_train_conditional.jl)
+//   update_cK! (:134-156), `\` (:33-36), logdet (:77), dmll_noise (:243-257), predictMVN (:324-332 ->
+//   determ_train_conditional.jl:41-59 -> subsetofregressors.jl:302-321).
+// The reference materialises K_uf (M x N) and several copies; here N is streamed in chunks through two
+// staging buffers and only M x M state persists (H7 of SURVEY.md §7.2): per chunk a cross-Gram, a
+// recursive TRSM against L_uu for diag(Q_ff), and one rank-Nc SYRK into Sigma_QR -- all on the DMMA GEMM.
+// ================================================================================================
+// in-place sum over the ranks of a device vector (no-op on one rank)
+static int fitc_allreduce(gpb200_fitc* f, double* v, size_t n) {
+    if (f->nranks <= 1 || n == 0) return GPB200_OK;
+    FCKN(g_nccl.AllReduce(v, v, n, ncclDouble, ncclSum, f->comm, f->eu->st));
+    return GPB200_OK;
+}
+
+// cross-validation workspace (gpb200_fitc_cv_*): it depends on N, Nc and Mpad only
+static void fitc_cv_free(gpb200_fitc* f) {
+    double** ptrs[] = {&f->cvG, &f->cvGt, &f->cvCh, &f->cvP, &f->cvDuu, &f->cvDp, &f->cvR, &f->cvH, &f->cvQ, &f->cvalpha,
+                       &f->cvdel, &f->cvilam, &f->cvza, &f->cvdg, &f->cvda, &f->cvq, &f->cvlamV, &f->cvdelV, &f->cvxs,
+                       &f->cvm, &f->cvout};
+    for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
+    if (f->cvidx) cudaFree(f->cvidx);
+    f->cvidx = nullptr; f->cvout_rows = 0;
+    f->cv_ws = f->cv_m_ok = false;
+}
+
+// every buffer that depends on the observations or the inducing points; the FSA blocks refer to the old observations too
+static void fitc_free_data(gpb200_fitc* f) {
+    double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
+                       &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
+                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx,
+                       &f->dxu};
+    for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
+    f->grad_ws = false;
+    fsa_free(f);
+    fitc_cv_free(f);
+}
+
+int gpb200_fitc_comm_init(gpb200_fitc* f, int nranks, int rank, const char* id128) {
+    if (!f || !id128 || nranks < 1 || rank < 0 || rank >= nranks) return GPB200_EINVAL;
+    if (!nccl_load()) return fail(f, GPB200_ENCCL, "libnccl.so.2 could not be loaded");
+    FCK(cudaSetDevice(f->device));
+    if (f->comm) { g_nccl.CommDestroy(f->comm); f->comm = nullptr; }
+    ncclUniqueId id;
+    memcpy(&id, id128, 128);
+    FCKN(g_nccl.CommInitRank(&f->comm, nranks, id, rank));
+    f->nranks = nranks; f->rank = rank;
+    f->factored = f->alpha_ready = false;
+    return GPB200_OK;
+}
+
+void gpb200_fitc_destroy(gpb200_fitc* f) {
+    if (!f) return;
+    cudaSetDevice(f->device);
+    if (f->eu && f->eu->st) cudaStreamSynchronize(f->eu->st);
+    fitc_free_data(f);
+    if (f->Kss) cudaFree(f->Kss);
+    for (cudaEvent_t e : f->xu_ev) cudaEventDestroy(e);
+    if (f->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(f->comm);
+    if (f->es) { f->es->st = nullptr; f->es->own_stream = false; gpb200_destroy(f->es); }
+    if (f->eu) gpb200_destroy(f->eu);
+    delete f;
+}
+
+int gpb200_fitc_create(gpb200_fitc** out, int device) {
+    if (!out) return GPB200_EINVAL;
+    *out = nullptr;
+    gpb200_fitc* f = new gpb200_fitc();
+    f->device = device;
+    int rc = gpb200_create(&f->eu, device);
+    if (rc == GPB200_OK) rc = gpb200_create(&f->es, device);
+    if (rc != GPB200_OK) { if (f->eu) gpb200_destroy(f->eu); delete f; return rc; }
+    // one stream for both sub-engines
+    cudaStreamDestroy(f->es->st);
+    f->es->st = f->eu->st; f->es->own_stream = false;
+    *out = f;
+    return GPB200_OK;
+}
+
+const char* gpb200_fitc_last_error(gpb200_fitc* f) { return f ? f->err.c_str() : g_create_error.c_str(); }
+
+int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, int64_t ldx, int64_t M,
+                         const double* xu, int64_t ldxu) {
+    if (!f) return GPB200_EINVAL;
+    if (N <= 0 || M <= 0 || d <= 0 || !x || !xu || ldx < d || ldxu < d) return fail(f, GPB200_EINVAL, "fitc_set_data: bad arguments");
+    FCK(cudaSetDevice(f->device));
+    FSUB(gpb200_set_data(f->eu, M, d, xu, ldxu), f->eu);
+    FSUB(gpb200_set_data(f->es, M, d, xu, ldxu), f->es);
+    cudaStream_t st = f->eu->st;
+    fitc_free_data(f);
+    f->N = N; f->M = M; f->d = d; f->Mpad = f->eu->Npad;
+    // chunk of data rows: two staging buffers of ~2 GB each at most
+    int64_t nc = (int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE;
+    const int64_t Nceil = (N + TILE - 1) / TILE * TILE;
+    if (nc > 32768) nc = 32768;                       // grid.y limit of the row-scaling kernel
+    if (nc > Nceil) nc = Nceil;
+    if (nc < TILE) nc = TILE;
+    f->Nc = nc;
+    FCK(cudaMalloc(&f->x, sizeof(double) * N * d));
+    FCK(cudaMalloc(&f->xs, sizeof(double) * nc * d));
+    for (double** p : {&f->lam, &f->y, &f->alpha, &f->tmpn}) FCK(cudaMalloc(p, sizeof(double) * (N + TILE)));
+    for (double** p : {&f->w, &f->tmpc, &f->zeroc, &f->tmpc2}) FCK(cudaMalloc(p, sizeof(double) * nc));
+    for (double** p : {&f->bvec, &f->uvec, &f->tmpm, &f->rhsm}) FCK(cudaMalloc(p, sizeof(double) * f->Mpad));
+    FCK(cudaMalloc(&f->scal, sizeof(double) * 16));
+    FCK(cudaMalloc(&f->bufA, sizeof(double) * nc * f->Mpad));
+    FCK(cudaMalloc(&f->bufB, sizeof(double) * nc * f->Mpad));
+    FCK(cudaMemsetAsync(f->zeroc, 0, sizeof(double) * nc, st));
+    FCK(cudaMemcpy2DAsync(f->x, sizeof(double) * d, x, sizeof(double) * ldx, sizeof(double) * d, N, cudaMemcpyHostToDevice, st));
+    if (f->eu->tma_ok) {
+        const bool ok = gemm_make_tensor_map(&f->mapA, f->bufA, nc, f->Mpad, f->Mpad) &&
+                        gemm_make_tensor_map(&f->mapB, f->bufB, f->Mpad, nc, nc) &&
+                        gemm_make_tensor_map(&f->mapB2, f->bufB, nc, f->Mpad, f->Mpad);
+        if (!ok) return fail(f, GPB200_ECUDA, "fitc_set_data: cuTensorMapEncodeTiled failed");
+    }
+    FCK(cudaStreamSynchronize(st));
+    f->has_data = true; f->factored = f->alpha_ready = false;
+    return GPB200_OK;
+}
+
+int gpb200_fitc_set_kernel(gpb200_fitc* f, int32_t n_ops, const int32_t* ops, int32_t n_dims, const int32_t* dims,
+                           int32_t n_theta) {
+    if (!f) return GPB200_EINVAL;
+    FSUB(gpb200_set_kernel(f->eu, n_ops, ops, n_dims, dims, n_theta), f->eu);
+    FSUB(gpb200_set_kernel(f->es, n_ops, ops, n_dims, dims, n_theta), f->es);
+    f->has_kernel = true; f->factored = f->alpha_ready = false;
+    return GPB200_OK;
+}
+}  // extern "C"
+
+namespace engine __attribute__((visibility("hidden"))) {
+// K_fu chunk (rows r0..r0+nc of x against the inducing points) into bufA [Nc x Mpad]
+cudaError_t fitc_kfu(gpb200_fitc* f, const double* xrows, int64_t nc) {
+    return crossgram_launch(f->eu->prog, xrows, f->d, nc, f->Nc, f->eu->x, f->d, f->M, f->Mpad, f->d, f->bufA, f->Mpad, f->eu->st, &f->eu->launches);
+}
+// K_uf chunk into bufB [Mpad x Nc]
+cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc) {
+    return crossgram_launch(f->eu->prog, f->eu->x, f->d, f->M, f->Mpad, xrows, f->d, nc, f->Nc, f->d, f->bufB, f->Nc, f->eu->st, &f->eu->launches);
+}
+
+// one contraction launch (slot k >= 1 of f->xu_ev) over n rows z against W (ld Mpad) into f->dxu
+int xu_contract(gpb200_fitc* f, size_t k, const double* z, int64_t n, const double* W, int sym, const double* mask,
+                int accumulate) {
+    gpb200_handle* eu = f->eu;
+    FCK(cudaEventRecord(f->xu_ev[2 * k], eu->st));
+    FCK(inducing_dx_launch(eu->prog, eu->x, f->d, f->M, z, f->d, n, f->d, W, f->Mpad, sym, mask, f->dxu, accumulate, eu->st,
+                           &eu->launches));
+    FCK(cudaEventRecord(f->xu_ev[2 * k + 1], eu->st));
+    return GPB200_OK;
+}
+
+// after the final synchronize: device times of the call and of its k_used contractions; dmll_xu = dxu / 2
+int xu_finish(gpb200_fitc* f, size_t k_used, double* dmll_xu) {
+    std::vector<double> h((size_t)f->M * f->d);
+    FCK(cudaMemcpy(h.data(), f->dxu, sizeof(double) * h.size(), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < h.size(); ++i) dmll_xu[i] = 0.5 * h[i];
+    double c = 0.0;
+    for (size_t k = 1; k <= k_used; ++k) c += ev_ms(f->xu_ev[2 * k], f->xu_ev[2 * k + 1]);
+    f->xu_ms[0] = c;
+    f->xu_ms[1] = ev_ms(f->xu_ev[0], f->xu_ev[1]);
+    return GPB200_OK;
+}
+}  // namespace engine
+
+extern "C" {
+int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise) {
+    if (!f) return GPB200_EINVAL;
+    if (!f->has_data || !f->has_kernel) return fail(f, GPB200_ESTATE, "fitc_factorize: set_data and set_kernel first");
+    if (!isfinite(log_noise)) return fail(f, GPB200_EINVAL, "fitc_factorize: non-finite logNoise");
+    if (f->mode == 3) TRY(fsa_check(f, "fitc_factorize"));
+    FCK(cudaSetDevice(f->device));
+    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    // K_uu + 1e-10 I and its factor (fitc.jl:139-141)
+    const double ln_off = -1000.0;                          // exp(2*ln) == 0: no noise on K_uu
+    FSUB(gpb200_factorize(eu, theta, &ln_off, 1, 1e-10), eu);
+    // Sigma_QR starts as K_uu (+ the second 1e-10 nugget of make_posdef!, fitc.jl:153)
+    kprog_set_theta(es->prog, theta);
+    for (int i = 0; i < es->prog.n_theta; ++i) es->theta[i] = theta[i];
+    const double zero = 0.0;
+    FCK(cudaMemcpyAsync(es->noise_var, &zero, sizeof(double), cudaMemcpyHostToDevice, st));
+    es->n_noise = 1; es->nugget = 2e-10;
+    if (f->rank == 0) FCK(gram_lower_launch(es->prog, es->x, f->d, f->d, f->M, f->Mpad, es->noise_var, 1, 2e-10, es->G, es->ld, st, &es->launches));
+    else FCK(cudaMemsetAsync(es->G, 0, sizeof(double) * (size_t)f->Mpad * (size_t)f->Mpad, st));     // K_uu (+ nuggets, identity padding) enters the sum once
+    f->noise_var = exp(2.0 * log_noise);
+    if (f->mode == 3) return fsa_factorize(f);
+    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    GemmBuf bB{eu->tma_ok ? &f->mapB : nullptr, f->bufB, f->Nc};
+    for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
+        const int64_t nc = std::min(f->Nc, f->N - r0);
+        const double* xr = f->x + r0 * f->d;
+        if (f->mode == 0) {
+            // Lambda_i = sigma^2 + K_ii - |L_uu^-1 K_ui|^2   (fitc.jl:146-148)
+            FCK(fitc_kfu(f, xr, nc));
+            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, nc, f->Mpad, f->tmpc2, st, &eu->launches));
+            FCK(ew_launch(0, nc, f->lam + r0, f->tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
+        } else {
+            // SoR / DTC: Lambda = sigma^2 I   (subsetofregressors.jl:100: exp(-2 logNoise) * Kuf * Kfu + Kuu)
+            FCK(ew_launch(0, nc, f->lam + r0, f->zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
+        }
+        // Sigma_QR += K_uf Lambda^-1 K_fu   (fitc.jl:150), as (K_uf Lambda^-1/2)(K_uf Lambda^-1/2)'
+        FCK(fitc_kuf(f, xr, nc));
+        FCK(scale_launch(0, f->bufB, f->Nc, f->Mpad, nc, f->lam + r0, st, &eu->launches));
+        FCK(gemm_whole(es, bB, bB, es->G, es->ld, f->Mpad, f->Mpad, f->Nc, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
+    }
+    // multi-GPU: Sigma_QR = K_uu + sum over ranks of K_uf L^-1 K_fu  -- the one M x M exchange of the FITC likelihood
+    TRY(fitc_allreduce(f, es->G, (size_t)f->Mpad * (size_t)f->Mpad));
+    int rc = chol_inplace(es);
+    if (rc != GPB200_OK) return fail(f, rc, "fitc_factorize (Sigma_QR): " + es->err);
+    f->factored = true;
+    return GPB200_OK;
+}
+
+// alpha = Sigma^-1 r (fitc.jl:33-36), logdet (fitc.jl:77), mll (GPE.jl:210)
+int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, double* mll, double* logdet) {
+    if (!f || !y_minus_mean || !mll) return GPB200_EINVAL;
+    if (!f->factored) return fail(f, GPB200_ESTATE, "fitc_mll: factorize first");
+    if (f->mode == 3) { FCK(cudaSetDevice(f->device)); return fsa_mll(f, y_minus_mean, alpha, mll, logdet); }
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    FCK(cudaMemcpyAsync(f->y, y_minus_mean, sizeof(double) * f->N, cudaMemcpyHostToDevice, st));
+    // b = K_uf Lambda^-1 r
+    FCK(cudaMemsetAsync(f->bvec, 0, sizeof(double) * f->Mpad, st));
+    for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
+        const int64_t nc = std::min(f->Nc, f->N - r0);
+        FCK(fitc_kuf(f, f->x + r0 * f->d, nc));
+        FCK(cudaMemsetAsync(f->w, 0, sizeof(double) * f->Nc, st));
+        FCK(ew_launch(1, nc, f->w, f->y + r0, f->lam + r0, nullptr, 0.0, st, &eu->launches));
+        FCK(rowdot_launch(f->bufB, f->Nc, f->w, f->M, f->Nc, f->tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+    }
+    TRY(fitc_allreduce(f, f->bvec, (size_t)f->Mpad));              // b summed over the ranks' rows
+    // u = Sigma_QR^-1 b   (== get_alpha_u, fitc.jl:279-286)
+    FCK(cudaMemcpyAsync(f->rhsm, f->bvec, sizeof(double) * f->Mpad, cudaMemcpyDeviceToDevice, st));
+    FCK(solve_device(es, f->rhsm, f->tmpm, f->uvec));
+    // alpha = Lambda^-1 (r - K_fu u)
+    for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
+        const int64_t nc = std::min(f->Nc, f->N - r0);
+        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));
+        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, nc, f->Mpad, f->tmpc, st, &eu->launches));
+        FCK(ew_launch(3, nc, f->alpha + r0, f->y + r0, f->tmpc, f->lam + r0, 0.0, st, &eu->launches));
+    }
+    FCK(dot_launch(f->y, f->alpha, f->N, f->scal + 0, st, &eu->launches));
+    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st, &eu->launches));
+    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st, &eu->launches));
+    FCK(ew_launch(4, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(sum_launch(f->tmpn, f->N, f->scal + 3, st, &eu->launches));
+    double s[5];
+    if (f->nranks > 1) {
+        // r'alpha, sum log Lambda and N are sums over the ranks' rows; the two M x M log-determinants are replicated
+        const double nloc = (double)f->N;
+        FCK(cudaMemcpyAsync(f->scal + 8, f->scal + 0, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->scal + 9, f->scal + 3, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->scal + 10, &nloc, sizeof(double), cudaMemcpyHostToDevice, st));
+        TRY(fitc_allreduce(f, f->scal + 8, 3));
+        FCK(cudaMemcpyAsync(f->scal + 0, f->scal + 8, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->scal + 3, f->scal + 9, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->scal + 4, f->scal + 10, sizeof(double), cudaMemcpyDeviceToDevice, st));
+    }
+    FCK(cudaMemcpyAsync(s, f->scal, sizeof(double) * 5, cudaMemcpyDeviceToHost, st));
+    if (alpha) FCK(cudaMemcpyAsync(alpha, f->alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(es), es);                                   // the solve for u above
+    f->Ntotal = f->nranks > 1 ? s[4] : (double)f->N;
+    const double ld = s[1] - s[2] + s[3];
+    if (logdet) *logdet = ld;
+    *mll = -(s[0] + ld + LOG2PI * f->Ntotal) / 2.0;
+    f->alpha_ready = true;
+    return GPB200_OK;
+}
+
+// dmll_noise (fitc.jl:243-257): sigma^2 * (alpha.alpha - sum 1/Lambda + |L_s^-1 K_uf Lambda^-1|_F^2)
+int gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise) {
+    if (!f || !dmll_noise) return GPB200_EINVAL;
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_grad_noise: factorize and mll first");
+    if (f->mode == 3) { FCK(cudaSetDevice(f->device)); return fsa_grad_noise(f, dmll_noise); }
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
+        const int64_t nc = std::min(f->Nc, f->N - r0);
+        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));
+        FCK(scale_launch(1, f->bufA, f->Mpad, nc, f->Mpad, f->lam + r0, st, &eu->launches));
+        FCK(trsm_rec_buf(es, bA, (int)f->Nc, 0, (int)f->Mpad));
+        FCK(rowvar_launch(f->bufA, f->Mpad, f->zeroc, nc, f->Mpad, f->tmpn + r0, st, &eu->launches));     // = -|row|^2
+    }
+    FCK(sum_launch(f->tmpn, f->N, f->scal + 0, st, &eu->launches));
+    FCK(dot_launch(f->alpha, f->alpha, f->N, f->scal + 1, st, &eu->launches));
+    FCK(ew_launch(5, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(sum_launch(f->tmpn, f->N, f->scal + 2, st, &eu->launches));
+    TRY(fitc_allreduce(f, f->scal, 3));                             // sums over the ranks' rows
+    double s[3];
+    FCK(cudaMemcpyAsync(s, f->scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    *dmll_noise = f->noise_var * (s[1] - s[2] - s[0]);
+    return GPB200_OK;
+}
+
+// predictive mean / variance (fitc.jl:324-332 -> dtc.jl:41-59 -> sor.jl:302-321):
+//   mu = K_xu u ;  var = k_xx - |L_uu^-1 k_ux|^2 + |L_s^-1 k_ux|^2
+int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* var) {
+    if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu) return GPB200_EINVAL;
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict: factorize and mll first");
+    if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict: FSA predictions need test blocks");
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
+    for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
+        const int64_t mc = std::min(f->Nc, Ms - m0);
+        FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * f->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * f->d,
+                              mc, cudaMemcpyHostToDevice, st));
+        FCK(fitc_kfu(f, f->xs, mc));
+        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st, &eu->launches));
+        FCK(cudaMemcpyAsync(mu + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        if (var) {
+            FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(kdiag_launch(eu->prog, f->xs, f->d, mc, f->tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st, &eu->launches));       // k_xx - q
+            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st, &eu->launches));          // -s
+            if (f->mode == 2) {                                                             // SoR: K_xu S^-1 K_ux only (sor.jl:302-321)
+                FCK(cudaMemsetAsync(f->tmpc2, 0, sizeof(double) * mc, st));
+            }
+            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st, &eu->launches));               // [k_xx - q] + s
+            FCK(cudaMemcpyAsync(var + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        }
+        FCK(cudaStreamSynchronize(st));
+    }
+    return GPB200_OK;
+}
+
+// Predictive gradients of the sparse models (predict_f with ForwardDiff.Dual inputs): mu and var through
+// gpb200_fitc_predict's launches (A = K*u L_uu^-T in bufA, B = K*u L_s^-T in bufB), then W' = A L_uu^-1 - B L_s^-1
+// (= K*u K_uu^-1 - K*u Sigma_QR^-1; SoR: - B L_s^-1) by the right-side TRSM on the two M x M sub-engines, whose F holds L'
+// in its strict-upper tiles for the call, and the contraction over the inducing points with alpha = u:
+//   dmu[m, :] = sum_j dk(x*_m, u_j)/dx*_m u_j,   dvar[m, :] = 2c dk(x*_m, x*_m)/dx*_m - 2 sum_j dk(x*_m, u_j)/dx*_m W'[m, j]
+// with c = 1 (FITC, DTC) or 0 (SoR, whose variance has no k_xx).  Single GPU, modes 0-2.
+int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* var,
+                             double* dmu, double* dvar) {
+    if (!f) return GPB200_EINVAL;
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict_grad: factorize and mll first");
+    if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict_grad: not available for FSA");
+    if (f->nranks > 1) return fail(f, GPB200_EINVAL, "fitc_predict_grad: single GPU handles only");
+    if (Ms <= 0 || !xs || ldxs < f->d || !mu || !dmu) return fail(f, GPB200_EINVAL, "fitc_predict_grad: bad Ms, xs, ldxs, mu or dmu");
+    if (!var != !dvar) return fail(f, GPB200_EINVAL, "fitc_predict_grad: var and dvar must be given together");
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int d = f->d;
+    if (!f->pdx) FCK(cudaMalloc(&f->pdx, sizeof(double) * 2 * f->Nc * d));
+    double* ddmu = f->pdx;
+    double* ddvar = f->pdx + f->Nc * d;
+    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
+    if (var) {
+        FCK(mirror_lower_tiles_launch(eu->F, eu->ld, eu->Npad, st, &eu->launches));
+        FCK(mirror_lower_tiles_launch(es->F, es->ld, es->Npad, st, &eu->launches));
+    }
+    for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
+        const int64_t mc = std::min(f->Nc, Ms - m0);
+        FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d,
+                              mc, cudaMemcpyHostToDevice, st));
+        FCK(fitc_kfu(f, f->xs, mc));
+        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st, &eu->launches));
+        FCK(cudaMemcpyAsync(mu + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        if (var) {                                                          // as gpb200_fitc_predict
+            FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
+            FCK(kdiag_launch(eu->prog, f->xs, d, mc, f->tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st, &eu->launches));
+            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st, &eu->launches));
+            if (f->mode == 2) FCK(cudaMemsetAsync(f->tmpc2, 0, sizeof(double) * mc, st));
+            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st, &eu->launches));
+            FCK(cudaMemcpyAsync(var + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+            if (f->mode != 2) FCK(trsm_right_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));      // A L_uu^-1
+            FCK(trsm_right_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));                        // B L_s^-1
+        }
+        FCK(crossgram_dx_launch(eu->prog, f->xs, d, mc, eu->x, d, f->M, d, f->uvec, (var && f->mode != 2) ? f->bufA : nullptr,
+                                var ? f->bufB : nullptr, f->Mpad, f->mode == 2 ? 0.0 : 1.0, ddmu, ddvar, st, &eu->launches));
+        FCK(cudaMemcpyAsync(dmu + m0 * d, ddmu, sizeof(double) * mc * d, cudaMemcpyDeviceToHost, st));
+        if (var) FCK(cudaMemcpyAsync(dvar + m0 * d, ddvar, sizeof(double) * mc * d, cudaMemcpyDeviceToHost, st));
+        FCK(cudaStreamSynchronize(st));
+    }
+    return GPB200_OK;
+}
+
+// predictMVN with the FULL predictive covariance (fitc.jl:324-332 -> determ_train_conditional.jl:41-59 ->
+// subsetofregressors.jl:302-321):  Sigma* = K** - K*u K_uu^-1 Ku* + K*u S^-1 Ku*   (FITC, DTC);   K*u S^-1 Ku*   (SoR)
+// = K** - A A' + B B' with A = K*u L_uu^-T, B = K*u L_s^-T: two whitening TRSMs and two NT GEMMs.  Ms <= one staging chunk.
+// Sigma* into f->Kss (leading dimension Ms rounded up to 128) and mu into f->tmpc and mu[Ms], on eu's stream; Ms <= Nc
+static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu) {
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
+    if (Mspad > f->Kss_rows) {
+        if (f->Kss) cudaFree(f->Kss);
+        f->Kss = nullptr; f->Kss_rows = 0;
+        FCK(cudaMalloc(&f->Kss, sizeof(double) * Mspad * Mspad));
+        f->Kss_rows = Mspad;
+    }
+    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
+    FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * f->d, xs, sizeof(double) * ldxs, sizeof(double) * f->d, Ms, cudaMemcpyHostToDevice, st));
+    FCK(fitc_kfu(f, f->xs, Ms));                                         // bufA = K*u  (Ms x Mpad, zero padded rows)
+    FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, Ms, f->Mpad, f->tmpc, st, &eu->launches));
+    FCK(cudaMemcpyAsync(mu, f->tmpc, sizeof(double) * Ms, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+    FCK(trsm_rec_buf(es, bB2, (int)Mspad, 0, (int)f->Mpad));             // B = K*u L_s^-T
+    if (f->mode != 2) {
+        FCK(trsm_rec_buf(eu, bA, (int)Mspad, 0, (int)f->Mpad));         // A = K*u L_uu^-T
+        FCK(gram_full_launch(eu->prog, f->xs, f->d, Ms, Mspad, f->d, f->Kss, Mspad, st, &eu->launches));
+        FCK(gemm_whole(eu, bA, bA, f->Kss, Mspad, Mspad, Mspad, f->Mpad, -1.0, 1.0));
+    } else {
+        FCK(cudaMemsetAsync(f->Kss, 0, sizeof(double) * Mspad * Mspad, st));
+    }
+    FCK(gemm_whole(es, bB2, bB2, f->Kss, Mspad, Mspad, Mspad, f->Mpad, 1.0, 1.0));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* cov) {
+    if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu || !cov) return GPB200_EINVAL;
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict_cov: factorize and mll first");
+    if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict_cov: FSA predictions need test blocks");
+    if (Ms > f->Nc) return fail(f, GPB200_EINVAL, "fitc_predict_cov: too many test points for one staging chunk");
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cov_build(f, Ms, xs, ldxs, mu));
+    const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
+    FCK(cudaMemcpy2DAsync(cov, sizeof(double) * Ms, f->Kss, sizeof(double) * Mspad, sizeof(double) * Ms, Ms, cudaMemcpyDeviceToHost, f->eu->st));
+    FCK(cudaStreamSynchronize(f->eu->st));
+    return GPB200_OK;
+}
+
+// Kernel-parameter gradient of the FITC mll: dmll_kern!(::FullyIndepStrat) (fitc.jl:200-234) on top of
+// dmll_kern!(::SubsetOfRegsStrategy) (subsetofregressors.jl:219-253), regrouped so that every
+// parameter shares the same three weighted traces (kernel derivatives recomputed on the fly):
+//   dmll_p = 1/2 [ <W_fu, dK_fu/dθ_p> + <W_uu, dK_uu/dθ_p> + sum_i g_i dK_ii/dθ_p ]
+//   g_i   = alpha_i^2 - (Sigma^-1)_ii ,  (Sigma^-1)_ii = 1/L_i - K_fu,i S^-1 K_uf,i / L_i^2      (trinvAB, fitc.jl:63-67)
+//   W_fu  = 2 alpha beta' - 2 L^-1 K_fu S^-1 - 2 diag(g) K_fu K_uu^-1 ,  beta = K_uu^-1 K_uf alpha   (sor.jl:147)
+//   W_uu  = -beta beta' + K_uu^-1 - S^-1 + K_uu^-1 (K_uf diag(g) K_fu) K_uu^-1
+// with S = Sigma_QR, L = Lambda; uses Sigma^-1 K_fu K_uu^-1 = L^-1 K_fu S^-1 and
+// K_uu^-1 K_uf Sigma^-1 K_fu K_uu^-1 = K_uu^-1 - S^-1 (both follow from S = K_uu + K_uf L^-1 K_fu).
+// All O(M^2 N) work is NT GEMMs against the explicit M x M inverses (grad_prepare of the sub-engines).
+//
+// Inducing points (dmll_xu != null, gpb200_fitc_grad_kernel_inducing): moving u_j changes K_fu and K_uu only (k_ii and the
+// FSA blocks K_bb do not depend on Xu), so the same adjoints give
+//   dmll/du_j = 1/2 [ sum_i W_fu[i, j] dk(u_j, x_i)/du_j + sum_l (W_uu[j, l] + W_uu[l, j]) dk(u_j, u_l)/du_j ]
+// (W_uu is not exactly symmetric: it comes from two GEMMs).  One inducing_dx launch per chunk reads W_fu where
+// trace_rect reads it and accumulates into f->dxu in chunk order; one more after the chunk loop contracts W_uu + W_uu'.
+// Without dmll_xu the launches are exactly those of the kernel gradient alone; with it, they are the same launches plus
+// the contractions (and, on several ranks, one all-reduce of the M x d partial), which read and write nothing else.
+static int xu_event_pairs(gpb200_fitc* f, size_t pairs) {
+    while (f->xu_ev.size() < 2 * pairs) {
+        cudaEvent_t e;
+        FCK(cudaEventCreate(&e));
+        f->xu_ev.push_back(e);
+    }
+    return GPB200_OK;
+}
+
+
+static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, const char* who) {
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, std::string(who) + ": factorize and mll first");
+    FCK(cudaSetDevice(f->device));
+    if (dmll_xu) {
+        const size_t chunks = f->mode == 3 ? fsa_num_chunks(f) : (size_t)((f->N + f->Nc - 1) / f->Nc);
+        TRY(xu_event_pairs(f, chunks + 2));
+        if (!f->dxu) FCK(cudaMalloc(&f->dxu, sizeof(double) * f->M * f->d));
+        FCK(cudaEventRecord(f->xu_ev[0], f->eu->st));
+    }
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int np = eu->prog.n_theta;
+    const int64_t Mp = f->Mpad, Nc = f->Nc;
+    if (!f->grad_ws) {
+        FCK(cudaMalloc(&f->bufC, sizeof(double) * Nc * Mp));
+        for (double** p : {&f->Hbuf, &f->Wbuf, &f->Tbuf}) FCK(cudaMalloc(p, sizeof(double) * Mp * Mp));
+        FCK(cudaMalloc(&f->gvec, sizeof(double) * (f->N + TILE)));
+        FCK(cudaMalloc(&f->betav, sizeof(double) * Mp));
+        const size_t tiles = (size_t)std::max((Nc / TILE) * (Mp / TILE), (Mp / TILE) * (Mp / TILE));
+        FCK(cudaMalloc(&f->gpart, sizeof(double) * tiles * GPB200_MAX_THETA));
+        FCK(cudaMalloc(&f->gacc, sizeof(double) * GPB200_MAX_THETA));
+        FCK(cudaMalloc(&f->gtmp, sizeof(double) * GPB200_MAX_THETA));
+        if (eu->tma_ok) {
+            const bool ok = gemm_make_tensor_map(&f->mapAt, f->bufA, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapC, f->bufC, Nc, Mp, Mp) &&
+                            gemm_make_tensor_map(&f->mapCt, f->bufC, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapH, f->Hbuf, Mp, Mp, Mp) &&
+                            gemm_make_tensor_map(&f->mapT, f->Tbuf, Mp, Mp, Mp);
+            if (!ok) return fail(f, GPB200_ECUDA, "fitc_grad_kernel: cuTensorMapEncodeTiled failed");
+        }
+        f->grad_ws = true;
+    }
+    // explicit K_uu^-1 and Sigma_QR^-1 (full symmetric) in the sub-engines' G buffers
+    FSUB(gpb200_grad_prepare(eu), eu);
+    FSUB(gpb200_grad_prepare(es), es);
+    FCK(symmetrize_launch(eu->G, eu->ld, Mp, st, &eu->launches));
+    FCK(symmetrize_launch(es->G, es->ld, Mp, st, &eu->launches));
+    const bool tma = eu->tma_ok;
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bAt{tma ? &f->mapAt : nullptr, f->bufA, Nc};
+    GemmBuf bCt{tma ? &f->mapCt : nullptr, f->bufC, Nc};
+    GemmBuf bH{tma ? &f->mapH : nullptr, f->Hbuf, Mp}, bT{tma ? &f->mapT : nullptr, f->Tbuf, Mp};
+    // beta = K_uu^-1 (K_uf alpha)
+    FCK(cudaMemsetAsync(f->rhsm, 0, sizeof(double) * Mp, st));
+    for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, f->N - r0);
+        FCK(fitc_kuf(f, f->x + r0 * f->d, nc));
+        FCK(cudaMemsetAsync(f->w, 0, sizeof(double) * Nc, st));
+        FCK(cudaMemcpyAsync(f->w, f->alpha + r0, sizeof(double) * nc, cudaMemcpyDeviceToDevice, st));
+        FCK(rowdot_launch(f->bufB, Nc, f->w, f->M, Nc, f->tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->rhsm, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+    }
+    TRY(fitc_allreduce(f, f->rhsm, (size_t)Mp));                    // K_uf alpha over all rows
+    FCK(solve_device(eu, f->rhsm, f->tmpm, f->betav));
+    FCK(cudaMemsetAsync(f->gacc, 0, sizeof(double) * GPB200_MAX_THETA, st));
+    FCK(cudaMemsetAsync(f->Hbuf, 0, sizeof(double) * Mp * Mp, st));
+    if (f->mode == 3) return fsa_grad_kernel(f, dmll_kernel, dmll_xu);
+    size_t xk = 0;                                                        // contraction launches so far
+    for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, f->N - r0);
+        const double* xr = f->x + r0 * f->d;
+        FCK(fitc_kfu(f, xr, nc));                                         // bufA = K_fu chunk
+        FCK(gemm_whole(es, bA, bufG(es), f->bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));         // P2 = K_fu S^-1 -> bufB (as Nc x Mpad)
+        FCK(rowdot2_launch(f->bufA, f->bufB, Mp, nc, Mp, f->tmpc, st, &eu->launches));
+        if (f->mode == 0) FCK(fitc_g_launch(nc, f->alpha + r0, f->lam + r0, f->tmpc, f->gvec + r0, st, &eu->launches));
+        else FCK(cudaMemsetAsync(f->gvec + r0, 0, sizeof(double) * nc, st));       // SoR part only (sor.jl:219-253)
+        FCK(gemm_whole(eu, bA, bufG(eu), f->bufC, Mp, Nc, Mp, Mp, 1.0, 0.0));         // P1 = K_fu K_uu^-1 -> bufC
+        FCK(fitc_wfu_launch(f->bufB, f->bufC, Mp, nc, f->M, f->alpha + r0, f->lam + r0, f->gvec + r0, f->betav, st, &eu->launches));
+        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufB, Mp, f->gpart, f->gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufB, 0, nullptr, xk > 0)); ++xk; }
+        if (f->mode != 0) continue;                                       // no Lambda-derivative terms for SoR / DTC
+        // diagonal term sum_i g_i dK_ii/dθ_p (scratch: bufC as np x nc)
+        FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->gvec + r0, f->bufC, st, &eu->launches));
+        for (int p = 0; p < np; ++p) FCK(sum_launch(f->bufC + (size_t)p * nc, nc, f->gtmp + p, st, &eu->launches));
+        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        // H += K_uf diag(g) K_fu
+        FCK(crossgram_launch(eu->prog, eu->x, f->d, f->M, Mp, xr, f->d, nc, Nc, f->d, f->bufA, Nc, st, &eu->launches));   // bufA = K_uf chunk (Mpad x Nc)
+        FCK(cudaMemcpyAsync(f->bufC, f->bufA, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
+        FCK(colscale_launch(f->bufC, Nc, Mp, nc, f->gvec + r0, st, &eu->launches));
+        FCK(gemm_whole(eu, bAt, bCt, f->Hbuf, Mp, Mp, Mp, Nc, 1.0, 1.0));
+    }
+    // multi-GPU: the per-row traces and H = K_uf diag(g) K_fu are sums over the ranks' rows; the M x M part below is replicated
+    TRY(fitc_allreduce(f, f->gacc, (size_t)np));
+    TRY(fitc_allreduce(f, f->Hbuf, (size_t)Mp * (size_t)Mp));
+    if (dmll_xu) TRY(fitc_allreduce(f, f->dxu, (size_t)f->M * f->d));   // W_fu part over all rows
+    // T = K_uu^-1 H ; Wbuf = K_uu^-1 T' = K_uu^-1 H K_uu^-1
+    FCK(gemm_whole(eu, bufG(eu), bH, f->Tbuf, Mp, Mp, Mp, Mp, 1.0, 0.0));
+    FCK(gemm_whole(eu, bufG(eu), bT, f->Wbuf, Mp, Mp, Mp, Mp, 1.0, 0.0));
+    FCK(fitc_wuu_launch(f->Wbuf, f->Wbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
+    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
+    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+    if (dmll_xu) {
+        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, 1)); ++xk;
+        FCK(cudaEventRecord(f->xu_ev[1], st));
+    }
+    std::vector<double> out((size_t)std::max(np, 1));
+    FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta above
+    if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
+    if (dmll_xu) TRY(xu_finish(f, xk, dmll_xu));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
+    if (!f || !dmll_kernel) return GPB200_EINVAL;
+    return fitc_grad(f, dmll_kernel, nullptr, "fitc_grad_kernel");
+}
+
+int gpb200_fitc_grad_kernel_inducing(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
+    if (!f) return GPB200_EINVAL;
+    if (!dmll_xu) return fail(f, GPB200_EINVAL, "fitc_grad_kernel_inducing: dmll_xu is required");
+    return fitc_grad(f, dmll_kernel, dmll_xu, "fitc_grad_kernel_inducing");
+}
+
+// Replaces the inducing inputs of both sub-engines in place (same M and d: no buffer is reallocated); the training inputs,
+// the kernel program, the FSA blocks and every workspace are kept.  The factorisation, alpha and the cross-validation state
+// refer to the old Xu and are invalidated.
+int gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_t ldxu) {
+    if (!f) return GPB200_EINVAL;
+    if (!f->has_data) return fail(f, GPB200_ESTATE, "fitc_set_inducing: set_data first");
+    if (M != f->M || !xu || ldxu < f->d) {
+        return fail(f, GPB200_EINVAL, "fitc_set_inducing: M must be set_data's, xu non-null and ldxu >= d");
+    }
+    FCK(cudaSetDevice(f->device));
+    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    FSUB(gpb200_set_data(f->eu, M, f->d, xu, ldxu), f->eu);
+    FSUB(gpb200_set_data(f->es, M, f->d, xu, ldxu), f->es);
+    return GPB200_OK;
+}
+
+// ================================================================================================
+// Cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance), one GPU.
+// Sigma = Lambda + K_fu K_uu^-1 K_uf is the matrix gpb200_fitc_mll inverts; nothing N x N is formed.  With S = Sigma_QR,
+// L = Lambda and the explicit K_uu^-1, S^-1 of the sub-engines (grad_prepare, as gpb200_fitc_grad_kernel):
+//   Sigma^-1 = L^-1 - Ch K_uf L^-1,   Ch = L^-1 K_fu S^-1 = Sigma^-1 K_fu K_uu^-1   (row-local)
+//   [Sigma^-1]_ii = 1/L_i - k_i S^-1 k_i' / L_i^2
+// Per hyper-parameter j: dSigma_j = Delta + G C' + C G',  C = K_fu K_uu^-1,  G = dK_fu - 1/2 K_fu Dp,  Dp = dK_uu K_uu^-1,
+// Delta = diag(dk_ii - 2 G_i.C_i) (FITC), 0 (SoR / DTC kernel parameters), I (noise variance; G = 0).  Then
+//   Sigma^-1 dSigma_j Sigma^-1 = diag(Delta / L^2) + E Ch' + Ch E',   E = L^-1 G - L^-2 Delta K_fu + 1/2 Ch Q,
+//   Q = H - R - R',  R = K_uf L^-1 G,  H = K_uf L^-1 Delta L^-1 K_fu      (both M x M)
+//   Z_j alpha = Delta alpha / L + L^-1 G beta + Ch w,   beta = K_uu^-1 K_uf alpha,  w = G'alpha - K_uf L^-1 Delta alpha - R beta
+// Pass 1 streams the chunks once to accumulate R, H and the M-vectors, pass 2 streams them again for the two N-vectors; a
+// fold block reads the same quantities on the gathered rows V only.
+// ================================================================================================
+static int fitc_cv_check(gpb200_fitc* f, const char* who) {
+    if (f->mode == 3) return fail(f, GPB200_EINVAL, std::string(who) + ": cross-validation is not available for FSA (mode 3)");
+    if (f->nranks > 1)
+        return fail(f, GPB200_EINVAL, std::string(who) + ": cross-validation runs on one GPU; this handle has " + std::to_string(f->nranks) + " ranks");
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, std::string(who) + ": factorize and mll first");
+    return GPB200_OK;
+}
+
+// workspace on first use; K_uu^-1 and S^-1 as full symmetric matrices in the sub-engines' G (the state grad_kernel builds)
+static int fitc_cv_prepare(gpb200_fitc* f) {
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N;
+    if (!f->cv_ws) {
+        for (double** p : {&f->cvG, &f->cvGt, &f->cvCh, &f->cvP}) FCK(cudaMalloc(p, sizeof(double) * Nc * Mp));
+        for (double** p : {&f->cvDuu, &f->cvDp, &f->cvR, &f->cvH, &f->cvQ}) FCK(cudaMalloc(p, sizeof(double) * Mp * Mp));
+        for (double** p : {&f->cvalpha, &f->cvdel, &f->cvilam, &f->cvza, &f->cvdg}) FCK(cudaMalloc(p, sizeof(double) * (N + Nc)));
+        for (double** p : {&f->cvda, &f->cvq, &f->cvlamV, &f->cvdelV}) FCK(cudaMalloc(p, sizeof(double) * Nc));
+        FCK(cudaMalloc(&f->cvxs, sizeof(double) * Nc * f->d));
+        FCK(cudaMalloc(&f->cvm, sizeof(double) * 8 * Mp));
+        FCK(cudaMalloc(&f->cvidx, sizeof(long long) * Nc));
+        FCK(cudaMemsetAsync(f->cvalpha, 0, sizeof(double) * (N + Nc), st));      // zero tail: chunk vectors are read Nc wide
+        if (eu->tma_ok) {
+            const bool ok = gemm_make_tensor_map(&f->mapCvGt, f->cvGt, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapCvCh, f->cvCh, Nc, Mp, Mp) &&
+                            gemm_make_tensor_map(&f->mapCvP, f->cvP, Nc, Mp, Mp) && gemm_make_tensor_map(&f->mapCvDuu, f->cvDuu, Mp, Mp, Mp) &&
+                            gemm_make_tensor_map(&f->mapCvDp, f->cvDp, Mp, Mp, Mp) && gemm_make_tensor_map(&f->mapCvQ, f->cvQ, Mp, Mp, Mp);
+            if (!ok) return fail(f, GPB200_ECUDA, "fitc_cv: cuTensorMapEncodeTiled failed");
+        }
+        f->cv_ws = true;
+    }
+    FSUB(gpb200_grad_prepare(eu), eu);
+    FSUB(gpb200_grad_prepare(es), es);
+    FCK(symmetrize_launch(eu->G, eu->ld, Mp, st, &eu->launches));
+    FCK(symmetrize_launch(es->G, es->ld, Mp, st, &eu->launches));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_get_inverse_diag(gpb200_fitc* f, double* diag) {
+    if (!f || !diag) return GPB200_EINVAL;
+    TRY(fitc_cv_check(f, "fitc_get_inverse_diag"));
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cv_prepare(f));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc;
+    const bool tma = eu->tma_ok;
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp};
+    for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, f->N - r0);
+        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));                                                   // bufA = K_fu
+        FCK(gemm_whole(f->eu, bA, bufG(es), f->cvCh, Mp, Nc, Mp, Mp, 1.0, 0.0));                      // K_fu S^-1
+        FCK(rowdot2_launch(f->bufA, f->cvCh, Mp, nc, Mp, f->cvq, st, &eu->launches));
+        FCK(fitc_cv_invdiag_launch(nc, f->lam + r0, f->cvq, f->cvdg + r0, st, &eu->launches));
+    }
+    FCK(cudaMemcpyAsync(diag, f->cvdg, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+
+int gpb200_fitc_cv_param(gpb200_fitc* f, int32_t param, const double* alpha, double* Zj_alpha, double* diag_ZjSinv) {
+    if (!f || !Zj_alpha || !diag_ZjSinv) return GPB200_EINVAL;
+    TRY(fitc_cv_check(f, "fitc_cv_param"));
+    const int np = f->eu->prog.n_theta;
+    if (param < -1 || param >= np)
+        return fail(f, GPB200_EINVAL, "fitc_cv_param: param must be -1 (noise variance) or a kernel parameter index below " + std::to_string(np));
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cv_prepare(f));
+    f->cv_m_ok = false;
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N, M = f->M;
+    const int d = f->d;
+    const bool tma = eu->tma_ok, noise = param < 0;
+    const int kind = noise ? 2 : (f->mode == 0 ? 0 : 1);
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bB{tma ? &f->mapB : nullptr, f->bufB, Nc};
+    GemmBuf bGt{tma ? &f->mapCvGt : nullptr, f->cvGt, Nc}, bCh{tma ? &f->mapCvCh : nullptr, f->cvCh, Mp};
+    GemmBuf bDuu{tma ? &f->mapCvDuu : nullptr, f->cvDuu, Mp}, bDp{tma ? &f->mapCvDp : nullptr, f->cvDp, Mp};
+    GemmBuf bQ{tma ? &f->mapCvQ : nullptr, f->cvQ, Mp};
+    double *kta = f->cvm, *gta = f->cvm + Mp, *uD = f->cvm + 2 * Mp, *beta = f->cvm + 3 * Mp;
+    double *rb = f->cvm + 4 * Mp, *w = f->cvm + 5 * Mp, *tmp = f->cvm + 6 * Mp;
+    if (alpha) FCK(cudaMemcpyAsync(f->cvalpha, alpha, sizeof(double) * N, cudaMemcpyHostToDevice, st));
+    else FCK(cudaMemcpyAsync(f->cvalpha, f->alpha, sizeof(double) * N, cudaMemcpyDeviceToDevice, st));
+    FCK(ew_launch(5, N, f->cvilam, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));              // 1 / Lambda
+    FCK(cudaMemsetAsync(f->cvm, 0, sizeof(double) * 8 * Mp, st));
+    FCK(cudaMemsetAsync(f->cvR, 0, sizeof(double) * Mp * Mp, st));
+    FCK(cudaMemsetAsync(f->cvH, 0, sizeof(double) * Mp * Mp, st));
+    if (!noise) {   // Dp = dK_uu K_uu^-1
+        FCK(gram_grad_full_launch(eu->prog, eu->x, d, d, M, Mp, param, f->cvDuu, Mp, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bDuu, bufG(eu), f->cvDp, Mp, Mp, Mp, Mp, 1.0, 0.0));
+    }
+    // pass 1: Delta, R, H, K_uf alpha, G'alpha, K_uf L^-1 Delta alpha
+    for (int64_t r0 = 0; r0 < N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, N - r0);
+        const double* xr = f->x + r0 * d;
+        FCK(fitc_kfu(f, xr, nc));                                                                     // bufA = K_fu
+        if (!noise) {
+            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cvG, Mp, st, &eu->launches));
+            if (kind == 0) FCK(gemm_whole(f->eu, bA, bufG(eu), f->bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));     // bufB = C (Nc x Mpad)
+            FCK(gemm_whole(f->eu, bA, bDp, f->cvG, Mp, Nc, Mp, Mp, -0.5, 1.0, f->cvGt, Nc));              // G and G'
+        }
+        FCK(fitc_cv_delta_launch(kind, eu->prog, xr, d, param, f->cvG, f->bufB, Mp, Mp, nc, Nc, f->cvalpha + r0, f->cvdel + r0,
+                                 f->cvda, st, &eu->launches));
+        FCK(fitc_kuf(f, xr, nc));                                                                     // bufB = K_uf
+        FCK(rowdot_launch(f->bufB, Nc, f->cvalpha + r0, M, Nc, tmp, st, &eu->launches));
+        FCK(ew_launch(2, M, kta, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(colscale_launch(f->bufB, Nc, Mp, nc, f->cvilam + r0, st, &eu->launches));                // K_uf L^-1
+        FCK(rowdot_launch(f->bufB, Nc, f->cvda, M, Nc, tmp, st, &eu->launches));
+        FCK(ew_launch(2, M, uD, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        if (!noise) {
+            FCK(rowdot_launch(f->cvGt, Nc, f->cvalpha + r0, M, Nc, tmp, st, &eu->launches));
+            FCK(ew_launch(2, M, gta, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bB, bGt, f->cvR, Mp, Mp, Mp, Nc, 1.0, 1.0));                           // R += K_uf L^-1 G
+        }
+        if (kind != 1) {                                                                              // H += K_uf L^-1 Delta L^-1 K_fu
+            FCK(cudaMemcpyAsync(f->cvGt, f->bufB, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
+            FCK(colscale_launch(f->cvGt, Nc, Mp, nc, f->cvdel + r0, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bB, bGt, f->cvH, Mp, Mp, Mp, Nc, 1.0, 1.0));
+        }
+    }
+    FCK(rowdot_launch(eu->G, eu->ld, kta, M, Mp, beta, st, &eu->launches));                         // beta = K_uu^-1 K_uf alpha
+    FCK(rowdot_launch(f->cvR, Mp, beta, M, Mp, rb, st, &eu->launches));
+    FCK(fitc_cv_wvec_launch(M, w, gta, uD, rb, st, &eu->launches));
+    FCK(fitc_cv_qs_launch(f->cvQ, f->cvH, f->cvR, Mp, Mp, st, &eu->launches));
+    // pass 2: the two N-vectors
+    for (int64_t r0 = 0; r0 < N; r0 += Nc) {
+        const int64_t nc = std::min(Nc, N - r0);
+        const double* xr = f->x + r0 * d;
+        FCK(fitc_kfu(f, xr, nc));
+        if (!noise) {
+            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cvG, Mp, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bA, bDp, f->cvG, Mp, Nc, Mp, Mp, -0.5, 1.0));
+        }
+        FCK(gemm_whole(f->eu, bA, bufG(es), f->cvCh, Mp, Nc, Mp, Mp, 1.0, 0.0));
+        FCK(scale_launch(1, f->cvCh, Mp, nc, Mp, f->lam + r0, st, &eu->launches));                  // Ch = L^-1 K_fu S^-1
+        FCK(gemm_whole(f->eu, bCh, bQ, f->cvP, Mp, Nc, Mp, Mp, 1.0, 0.0));                                // Ch Q
+        FCK(fitc_cv_rows_launch(noise ? nullptr : f->cvG, f->cvCh, f->bufA, f->cvP, Mp, nc, Mp, f->lam + r0, f->cvdel + r0,
+                                f->cvalpha + r0, beta, w, f->cvza + r0, f->cvdg + r0, st, &eu->launches));
+    }
+    FCK(cudaMemcpyAsync(Zj_alpha, f->cvza, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(diag_ZjSinv, f->cvdg, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    f->cv_param = param;
+    f->cv_m_ok = true;
+    return GPB200_OK;
+}
+
+int gpb200_fitc_cv_block(gpb200_fitc* f, int32_t which, int64_t nV, const int64_t* idx, double* out) {
+    if (!f || !idx || !out) return GPB200_EINVAL;
+    TRY(fitc_cv_check(f, "fitc_cv_block"));
+    if (which != 0 && which != 1) return fail(f, GPB200_EINVAL, "fitc_cv_block: which must be 0 (Sigma^-1) or 1 (the last cv_param's M_j)");
+    if (nV < 1 || nV > f->Nc)
+        return fail(f, GPB200_EINVAL, "fitc_cv_block: nV must lie in 1.." + std::to_string(f->Nc) + " (one staging chunk)");
+    for (int64_t r = 0; r < nV; ++r)
+        if (idx[r] < 0 || idx[r] >= f->N) return fail(f, GPB200_EINVAL, "fitc_cv_block: index out of range");
+    if (which == 1 && !f->cv_m_ok) return fail(f, GPB200_ESTATE, "fitc_cv_block: which = 1 needs a fitc_cv_param since the last factorize");
+    FCK(cudaSetDevice(f->device));
+    TRY(fitc_cv_prepare(f));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, M = f->M;
+    const int d = f->d;
+    const int64_t nVp = (nV + TILE - 1) / TILE * TILE;
+    const bool tma = eu->tma_ok;
+    if (nVp > f->cvout_rows) {
+        if (f->cvout) cudaFree(f->cvout);
+        f->cvout = nullptr; f->cvout_rows = 0;
+        FCK(cudaMalloc(&f->cvout, sizeof(double) * nVp * nVp));
+        f->cvout_rows = nVp;
+    }
+    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bB2{tma ? &f->mapB2 : nullptr, f->bufB, Mp};
+    GemmBuf bCh{tma ? &f->mapCvCh : nullptr, f->cvCh, Mp}, bP{tma ? &f->mapCvP : nullptr, f->cvP, Mp};
+    GemmBuf bDp{tma ? &f->mapCvDp : nullptr, f->cvDp, Mp}, bQ{tma ? &f->mapCvQ : nullptr, f->cvQ, Mp};
+    FCK(cudaMemcpyAsync(f->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, st));
+    FCK(fitc_cv_gather_launch(nV, f->cvidx, f->x, d, d, f->cvxs, f->lam, f->cvlamV, which == 1 ? f->cvdel : nullptr, f->cvdelV,
+                              st, &eu->launches));
+    FCK(crossgram_launch(eu->prog, f->cvxs, d, nV, nVp, eu->x, d, M, Mp, d, f->bufA, Mp, st, &eu->launches));   // K_V
+    FCK(gemm_whole(f->eu, bA, bufG(es), f->cvCh, Mp, nVp, Mp, Mp, 1.0, 0.0));
+    FCK(scale_launch(1, f->cvCh, Mp, nV, Mp, f->cvlamV, st, &eu->launches));                       // Ch_V
+    if (which == 0) {   // Sigma^-1[V,V] = diag(1/L_V) - Ch_V (L_V^-1 K_V)'
+        FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * nVp * Mp, cudaMemcpyDeviceToDevice, st));
+        FCK(scale_launch(1, f->bufB, Mp, nV, Mp, f->cvlamV, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bCh, bB2, f->cvout, nVp, nVp, nVp, Mp, -1.0, 0.0));
+    } else {            // (Sigma^-1 dSigma_j Sigma^-1)[V,V] = diag(Delta_V / L_V^2) + E_V Ch_V' + Ch_V E_V'
+        const bool noise = f->cv_param < 0;
+        if (!noise) {
+            FCK(crossgram_grad_launch(eu->prog, f->cvxs, d, nV, nVp, eu->x, d, M, Mp, d, f->cv_param, f->cvG, Mp, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bA, bDp, f->cvG, Mp, nVp, Mp, Mp, -0.5, 1.0));
+        }
+        FCK(gemm_whole(f->eu, bCh, bQ, f->cvP, Mp, nVp, Mp, Mp, 0.5, 0.0));
+        FCK(fitc_cv_eblock_launch(f->cvP, noise ? nullptr : f->cvG, f->bufA, Mp, nV, Mp, f->cvlamV, f->cvdelV, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bP, bCh, f->cvout, nVp, nVp, nVp, Mp, 1.0, 0.0));
+        FCK(gemm_whole(f->eu, bCh, bP, f->cvout, nVp, nVp, nVp, Mp, 1.0, 1.0));
+    }
+    FCK(fitc_cv_diag_launch(f->cvout, nVp, nV, which, f->cvlamV, f->cvdelV, st, &eu->launches));
+    FCK(cudaMemcpy2DAsync(out, sizeof(double) * nV, f->cvout, sizeof(double) * nVp, sizeof(double) * nV, nV, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+
+// rand(gp, X, n) (src/GP.jl:120-146) with a sparse cK: Sigma* is the covariance predict_cov (modes 0-2) or predict_fsa
+// (mode 3) returns, built on the device and kept there; make_posdef!, the Cholesky and unwhiten! are gpb200_rand's
+// (rand_from_cov on eu, whose Ms x Ms sub-engine shares the handle's stream).  The likelihood, gradient, prediction and
+// cross-validation state is only read.
+int gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of, int64_t nsamp,
+                     const double* z, double nugget, double* mu_minus_mean, double* samples) {
+    if (!f) return GPB200_EINVAL;
+    if (Ms <= 0 || nsamp <= 0 || !xs || ldxs < f->d || !z || !mu_minus_mean || !samples) {
+        return fail(f, GPB200_EINVAL, "fitc_rand: bad Ms, nsamp, xs, ldxs, z, mu or samples");
+    }
+    if (!(nugget >= 0.0)) return fail(f, GPB200_EINVAL, "fitc_rand: nugget must be >= 0");
+    if ((f->mode == 3) != (block_of != nullptr)) {
+        return fail(f, GPB200_EINVAL, "fitc_rand: block_of is required in FSA mode (3) and must be NULL otherwise");
+    }
+    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_rand: factorize and mll first");
+    if (f->mode != 3 && Ms > f->Nc) return fail(f, GPB200_EINVAL, "fitc_rand: too many test points for one staging chunk");
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle* eu = f->eu;
+    cudaEvent_t ev_start = eu->ev4;                      // rand_from_cov records ev0 .. ev3
+    FCK(cudaEventRecord(ev_start, eu->st));
+    const double* cov;
+    int64_t ldc;
+    if (f->mode == 3) {
+        static double cov_flag;                          // non-null marker: Sigma* stays on the device
+        f->cov_keep_device = true;
+        const int rc = gpb200_fitc_predict_fsa(f, Ms, xs, ldxs, block_of, mu_minus_mean, nullptr, &cov_flag);
+        f->cov_keep_device = false;
+        if (rc) return rc;
+        cov = fsa_cov(f); ldc = Ms;
+    } else {
+        TRY(fitc_cov_build(f, Ms, xs, ldxs, mu_minus_mean));
+        cov = f->Kss; ldc = (Ms + TILE - 1) / TILE * TILE;
+    }
+    FSUB(rand_from_cov(eu, Ms, cov, ldc, f->tmpc, nsamp, z, nugget, samples), eu);
+    f->rand_ms[0] = ev_ms(ev_start, eu->ev0);
+    f->rand_ms[1] = ev_ms(eu->ev0, eu->ev1);
+    f->rand_ms[2] = ev_ms(eu->ev3, eu->ev2);
+    return GPB200_OK;
+}
+
+int gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n) {
+    if (!f || !ms || n < 0) return GPB200_EINVAL;
+    for (int32_t i = 0; i < n && i < 3; ++i) ms[i] = f->rand_ms[i];
+    for (int32_t i = 3; i < n && i < 7; ++i) ms[i] = f->fsag_ms[i - 3];
+    for (int32_t i = 7; i < n && i < 9; ++i) ms[i] = f->xu_ms[i - 7];
+    return GPB200_OK;
+}
+
+int gpb200_fitc_set_mode(gpb200_fitc* f, int mode) {
+    if (!f || mode < 0 || mode > 3) return GPB200_EINVAL;
+    f->mode = mode; f->factored = f->alpha_ready = false;
+    return GPB200_OK;
+}
+
+int64_t gpb200_fitc_launch_count(gpb200_fitc* f) { return f ? f->eu->launches + f->es->launches : 0; }
+}  // extern "C"

@@ -1,4 +1,4 @@
-// fsa.cu -- kernels of the Full Scale Approximation's block-diagonal Lambda (see fsa.cuh and the FSA section of gpb200.cu).
+// fsa.cu -- kernels of the Full Scale Approximation's block-diagonal Lambda (see fsa.cuh and fsa_engine.cu).
 //
 // The hot path is the grouped tile GEMM: every CTA reads one work item (tile pointers, leading dimensions, K, alpha, beta)
 // from a device array, so one launch covers a list of aligned 128 x 128 tiles that belong to blocks of different sizes --

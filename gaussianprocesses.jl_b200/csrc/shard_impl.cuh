@@ -1,4 +1,4 @@
-// shard_impl.cuh -- ROW-SHARDED multi-GPU schedules (included by gpb200.cu inside its anonymous namespace).
+// shard_impl.cuh -- ROW-SHARDED multi-GPU schedules (included by gpb200.cu inside namespace engine).
 //
 // North-star: "for N beyond one GPU's HBM the Gram matrix is row-block sharded across the 8 GPUs and a 1-D block
 // Cholesky exchanges panels over NVLink with NCCL" (config C4: Mat32Iso N=131072 d=16, 137 GB per N x N matrix).

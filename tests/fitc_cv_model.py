@@ -1,5 +1,5 @@
 """numpy model of the sparse engine's cross-validation schedule (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block in
-csrc/gpb200.cu): the same M x M state, the same two streaming passes over row chunks of `chunk` rows, the same row
+csrc/fitc_engine.cu): the same M x M state, the same two streaming passes over row chunks of `chunk` rows, the same row
 epilogues.  Only K_uu^-1, S^-1 and per-chunk rows of K_fu / dK_fu are formed; the tests compare it against the dense
 inverse of Sigma (tests/fitc_cv_oracle.py)."""
 import math

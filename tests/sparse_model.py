@@ -6,7 +6,7 @@ element may be NaN) and returns what the kernel writes (functions that update a 
 updated copy; elements the kernel leaves alone come back unchanged).  Every function takes a dtype: np.float64 gives the
 float64 result, np.longdouble the extended-precision one.
 
-The FSA packed layout is restated from gpb200_fitc_set_blocks (csrc/gpb200.cu) by `Layout`: block b of n_b points is
+The FSA packed layout is restated from gpb200_fitc_set_blocks (csrc/fsa_engine.cu) by `Layout`: block b of n_b points is
 padded to B_b = ceil(n_b / 128) * 128 rows and starts at padded row bstart_b; its B_b x B_b matrix is stored row-major
 with leading dimension B_b at offset boff_b of the packed array; rblk maps a padded row to its block, mask is 1 on real
 rows and 0 on padding, pos maps a training point to its padded row.  The Gram item list holds the lower tiles of every

@@ -72,7 +72,7 @@ def _leaf_outputs(L, Np):
 
 
 def _merge_inverse(Np, p, n1, n2, batch):
-    """gpb200.cu merge_inverse (l. 407)"""
+    """merge_inverse (gpb200.cu)"""
     lim = Np - p - n1
     return [Desc(Operand("G", "DinvT", p, p), Operand("F", None, p + n1, p), "F", c_row0=p, c_col0=p + n1,
                  M=n1, N=n2, K=n1, flags=KLO_M, batch=batch, zstep=2 * n1, n_lim=lim),
@@ -82,7 +82,7 @@ def _merge_inverse(Np, p, n1, n2, batch):
 
 
 def _inverse_from_factor(Np):
-    """gpb200.cu inverse_merges (l. 501) + inverse_from_factor (l. 513)"""
+    """inverse_merges + inverse_from_factor (gpb200.cu)"""
     out = []
     s = T
     while s < Np:
@@ -136,19 +136,19 @@ def test_engine_panel_trsm_and_schur_update_reproduce_the_factor():
     K = _spd(Np, 7)
     L = np.linalg.cholesky(K)
     Dinv, _ = _leaf_outputs(L, Np)
-    # panel_trsm_leaf (l. 379): F[r0.., p..p+128) = G[r0.., p..p+128) W_pp'
+    # panel_trsm_leaf (gpb200.cu): F[r0.., p..p+128) = G[r0.., p..p+128) W_pp'
     d = Desc(Operand("G", None, T, p), Operand("Dinv", None, p, 0), "F", c_row0=T, c_col0=p, M=Np - T, N=T, K=T)
     after, _ = _run_poisoned([d], dict(G=np.tril(K), F=np.full((Np, Np), np.nan), Dinv=Dinv))
     assert np.max(np.abs(after["F"][T:, :T] - L[T:, :T])) <= 1e-12 * np.max(np.abs(L))
 
-    def schur(r0, rows, cols, extra=0):          # schur_update (l. 393)
+    def schur(r0, rows, cols, extra=0):          # schur_update (gpb200.cu)
         return Desc(Operand("F", None, r0, p), Operand("F", None, r0, p), "G", c_row0=r0, c_col0=r0,
                     M=rows, N=cols, K=k, alpha=-1.0, beta=1.0, flags=LOWER_ONLY | extra)
 
     r0, rows = p + k, Np - p - k
     S = K[r0:, r0:] - L[r0:, :k] @ L[r0:, :k].T
     for sched in ([schur(r0, rows, rows)],
-                  [schur(r0, T, T), schur(r0, rows, rows, SKIP_FIRST)],          # look-ahead split (chol_panel, l. 471-476)
+                  [schur(r0, T, T), schur(r0, rows, rows, SKIP_FIRST)],          # look-ahead split (chol_panel)
                   [schur(r0, rows, 2 * T), schur(r0 + 2 * T, rows - 2 * T, rows - 2 * T)]):   # trapezoid, then the rest
         after, written = _run_poisoned(sched, dict(F=np.tril(L), G=np.where(np.tri(Np, dtype=bool), K, np.nan)))
         got = after["G"][r0:, r0:]

@@ -121,14 +121,14 @@ def test_gemm_each_flag_alone(engine, impl, flags):
 def _engine_cases():
     Np = 640
     sq = dict(G=_sq(Np), F=_sq(Np), Dinv=(Np, T), DinvT=(Np, T))
-    # gpb200.cu panel_trsm_leaf (l. 379): F[r0.., p..) = G[r0.., p..) W_pp'
+    # panel_trsm_leaf (gpb200.cu): F[r0.., p..) = G[r0.., p..) W_pp'
     yield "panel_trsm_leaf", Desc(Operand("G", None, 256, 128), Operand("Dinv", None, 128, 0), "F", c_row0=256,
                                   c_col0=128, M=384, N=T, K=T), sq
-    # schur_update (l. 393) and its look-ahead remainder (l. 476)
+    # schur_update (gpb200.cu) and its look-ahead remainder (chol_panel)
     for extra in (0, SKIP_FIRST):
         yield "schur_update", Desc(Operand("F", None, 256, 0), Operand("F", None, 256, 0), "G", c_row0=256, c_col0=256,
                                    M=384, N=256, K=256, alpha=-1.0, beta=1.0, flags=LOWER_ONLY | extra), sq
-    # merge_inverse (l. 407) at Npad = 896: both launches of level s = 128 (batch 4, the last problem skipped) and of
+    # merge_inverse (gpb200.cu) at Npad = 896: both launches of level s = 128 (batch 4, the last problem skipped) and of
     # s = 256 (batch 2, the second problem clipped to one tile)
     Nm = 896
     sqm = dict(G=_sq(Nm), F=_sq(Nm), Dinv=(Nm, T), DinvT=(Nm, T))
@@ -139,19 +139,19 @@ def _engine_cases():
         yield "merge_inverse_W21", Desc(Operand("G", "Dinv", s, s), Operand("F", None, 0, s), "G", c_row0=s, c_col0=0,
                                         Ct="G", ct_row0=0, ct_col0=s, M=n2, N=s, K=n2, alpha=-1.0, flags=KHI_M,
                                         batch=batch, zstep=2 * s, m_lim=lim, k_lim=lim), sqm
-    # inverse_from_factor (l. 513): W'W, A = B = G with the DinvT tiles on the diagonal
+    # inverse_from_factor (gpb200.cu): W'W, A = B = G with the DinvT tiles on the diagonal
     yield "inverse_from_factor", Desc(Operand("G", "DinvT"), Operand("G", "DinvT"), "G", M=Np, N=Np, K=Np,
                                       flags=LOWER_ONLY | KLO_M), sq
-    # GPA product (l. 1559): B's diagonal tiles from a second sub buffer
+    # GPA product (gpb200_gpa_grad, gpb200.cu): B's diagonal tiles from a second sub buffer
     yield "gpa_product", Desc(Operand("G", "DinvT"), Operand("F", "ZdT"), "G", M=Np, N=Np, K=Np, alpha=-1.0,
                               flags=LOWER_ONLY | KLO_M), dict(sq, ZdT=(Np, T))
-    # rand (l. 1726): out = Z L'
+    # rand (rand_from_cov, gpb200.cu): out = Z L'
     yield "rand", Desc(Operand("Z"), Operand("F"), "O", M=256, N=Np, K=Np, flags=KHI_N), dict(Z=(256, Np), F=_sq(Np),
                                                                                                O=(256, Np))
-    # rank update of a symmetric block (l. 2438, FITC): C += B B', lower trapezoid
+    # rank update of a symmetric block (gpb200_fitc_factorize, fitc_engine.cu): C += B B', lower trapezoid
     yield "rank_update", Desc(Operand("B"), Operand("B"), "C", M=512, N=512, K=384, beta=1.0, flags=LOWER_ONLY), \
         dict(B=(512, 384), C=_sq(512))
-    # inverse_dist (l. 789-811): the two merge launches of level s = 256 split over 2 ranks (filtered grids, batch 2,
+    # inverse_dist (gpb200.cu): the two merge launches of level s = 256 split over 2 ranks (filtered grids, batch 2,
     # the second problem clipped)
     for me in range(2):
         yield "inverse_dist_T", Desc(Operand("G", "DinvT"), Operand("F", None, 256, 0), "F", c_row0=0, c_col0=256,
@@ -162,7 +162,7 @@ def _engine_cases():
                                        flags=KHI_M, bn_mod=2, bn_rem=me, batch=2, zstep=512, m_lim=Nm - 256,
                                        k_lim=Nm - 256), sqm
     for me in range(3):
-        # l. 838: W'W on the owned tile rows (compact grid, batch 1)
+        # inverse_dist: W'W on the owned tile rows (compact grid, batch 1)
         yield "inverse_dist_WtW", Desc(Operand("G", "DinvT"), Operand("G", "DinvT"), "G", M=Np, N=Np, K=Np,
                                        flags=LOWER_ONLY | KLO_M, bm_mod=3, bm_rem=me), sq
     # shard_impl.cuh: own_rows_filter (l. 402) on the leaf TRSM (l. 414), the narrow Schur update (l. 523), the TRTRI
