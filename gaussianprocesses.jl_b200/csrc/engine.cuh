@@ -175,6 +175,11 @@ struct gpb200_fitc {
     double* dxu = nullptr;
     std::vector<cudaEvent_t> xu_ev;
     double xu_ms[2] = {0, 0};
+    // training-input gradient (gpb200_fitc_grad_kernel_inputs; first use): dmll/dX accumulator (N x d, this rank's rows in
+    // the caller's order), the events around the call and its contractions (as xu_ev) and the device times of the last call
+    double* dx = nullptr;
+    std::vector<cudaEvent_t> x_ev;
+    double x_ms[2] = {0, 0};
     // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
     // buffer the likelihood, gradient and prediction schedules keep):
     //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
@@ -299,7 +304,8 @@ int fsa_check(gpb200_fitc* f, const char* who);
 int fsa_factorize(gpb200_fitc* f);
 int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, double* mll, double* logdet);
 int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise);
-int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu);
+int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double* dmll_x);
+int fsa_set_inputs(gpb200_fitc* f, const double* x, int64_t ldx);
 size_t fsa_num_chunks(const gpb200_fitc* f);
 const double* fsa_cov(const gpb200_fitc* f);
 
@@ -309,5 +315,8 @@ cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc);
 int xu_contract(gpb200_fitc* f, size_t k, const double* z, int64_t n, const double* W, int sym, const double* mask,
                 int accumulate);
 int xu_finish(gpb200_fitc* f, size_t k_used, double* dmll_xu);
+int x_rows(gpb200_fitc* f, size_t k, const double* xr, int64_t n, const double* W, const double* c, const double* mask,
+           const long long* map, double* out, int accumulate);
+int x_finish(gpb200_fitc* f, size_t k_used, double* dmll_x);
 
 }  // namespace engine

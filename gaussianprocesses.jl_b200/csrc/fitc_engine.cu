@@ -39,7 +39,7 @@ static void fitc_free_data(gpb200_fitc* f) {
     double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
                        &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
                        &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx,
-                       &f->dxu};
+                       &f->dxu, &f->dx};
     for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
     f->grad_ws = false;
     fsa_free(f);
@@ -66,6 +66,7 @@ void gpb200_fitc_destroy(gpb200_fitc* f) {
     fitc_free_data(f);
     if (f->Kss) cudaFree(f->Kss);
     for (cudaEvent_t e : f->xu_ev) cudaEventDestroy(e);
+    for (cudaEvent_t e : f->x_ev) cudaEventDestroy(e);
     if (f->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(f->comm);
     if (f->es) { f->es->st = nullptr; f->es->own_stream = false; gpb200_destroy(f->es); }
     if (f->eu) gpb200_destroy(f->eu);
@@ -167,6 +168,29 @@ int xu_finish(gpb200_fitc* f, size_t k_used, double* dmll_xu) {
     for (size_t k = 1; k <= k_used; ++k) c += ev_ms(f->xu_ev[2 * k], f->xu_ev[2 * k + 1]);
     f->xu_ms[0] = c;
     f->xu_ms[1] = ev_ms(f->xu_ev[0], f->xu_ev[1]);
+    return GPB200_OK;
+}
+
+// one row-contraction launch (slot k >= 1 of f->x_ev) over n rows xr against the W_fu rows W (ld Mpad): rows_dx_launch
+int x_rows(gpb200_fitc* f, size_t k, const double* xr, int64_t n, const double* W, const double* c, const double* mask,
+           const long long* map, double* out, int accumulate) {
+    gpb200_handle* eu = f->eu;
+    FCK(cudaEventRecord(f->x_ev[2 * k], eu->st));
+    FCK(rows_dx_launch(eu->prog, xr, f->d, n, eu->x, f->d, f->M, f->d, W, f->Mpad, c, mask, map, out, accumulate, eu->st,
+                       &eu->launches));
+    FCK(cudaEventRecord(f->x_ev[2 * k + 1], eu->st));
+    return GPB200_OK;
+}
+
+// after the final synchronize: device times of the call and of its k_used contractions; dmll_x = dx / 2
+int x_finish(gpb200_fitc* f, size_t k_used, double* dmll_x) {
+    const size_t n = (size_t)f->N * f->d;
+    FCK(cudaMemcpy(dmll_x, f->dx, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; ++i) dmll_x[i] *= 0.5;
+    double c = 0.0;
+    for (size_t k = 1; k <= k_used; ++k) c += ev_ms(f->x_ev[2 * k], f->x_ev[2 * k + 1]);
+    f->x_ms[0] = c;
+    f->x_ms[1] = ev_ms(f->x_ev[0], f->x_ev[1]);
     return GPB200_OK;
 }
 }  // namespace engine
@@ -466,24 +490,40 @@ int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
 // trace_rect reads it and accumulates into f->dxu in chunk order; one more after the chunk loop contracts W_uu + W_uu'.
 // Without dmll_xu the launches are exactly those of the kernel gradient alone; with it, they are the same launches plus
 // the contractions (and, on several ranks, one all-reduce of the M x d partial), which read and write nothing else.
-static int xu_event_pairs(gpb200_fitc* f, size_t pairs) {
-    while (f->xu_ev.size() < 2 * pairs) {
+//
+// Training inputs (dmll_x != null, gpb200_fitc_grad_kernel_inputs): x_i enters row i of K_fu, K_ii (FITC) and row and
+// column i of its FSA block K_bb, never K_uu, so with d1k the derivative in the first argument
+//   FITC:      dmll/dx_i = 1/2 [ sum_j W_fu[i, j] d1k(x_i, u_j) + 2 g_i d1k(x_i, x_i) ]
+//   DTC, SoR:  dmll/dx_i = 1/2   sum_j W_fu[i, j] d1k(x_i, u_j)
+//   FSA:       dmll/dx_i = 1/2 [ sum_j W_fu[i, j] d1k(x_i, u_j) + sum_{l in b(i)} (G_b[i, l] + G_b[l, i]) d1k(x_i, x_l) ]
+// (2 d1k(x, x) is the derivative of k(x, x): 0 for the stationary leaves; G_b is not exactly symmetric, it comes from GEMMs).
+// The mean's part alpha_i dm(x_i)/dx_i is the caller's.  One rows_dx launch per chunk reads W_fu where trace_rect reads it
+// (FITC with c = g); FSA adds one fsa_block_dx launch per chunk over the G_b tiles in Gpk, after fsa_outer completes them
+// and before the next chunk overwrites them, and writes in the caller's order through the inverse row map.  The rows are
+// the rank's own, so nothing is exchanged.  Without dmll_x the launch sequence is unchanged.
+static int event_pairs(gpb200_fitc* f, std::vector<cudaEvent_t>& ev, size_t pairs) {
+    while (ev.size() < 2 * pairs) {
         cudaEvent_t e;
         FCK(cudaEventCreate(&e));
-        f->xu_ev.push_back(e);
+        ev.push_back(e);
     }
     return GPB200_OK;
 }
 
 
-static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, const char* who) {
+static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double* dmll_x, const char* who) {
     if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, std::string(who) + ": factorize and mll first");
     FCK(cudaSetDevice(f->device));
+    const size_t chunks = f->mode == 3 ? fsa_num_chunks(f) : (size_t)((f->N + f->Nc - 1) / f->Nc);
     if (dmll_xu) {
-        const size_t chunks = f->mode == 3 ? fsa_num_chunks(f) : (size_t)((f->N + f->Nc - 1) / f->Nc);
-        TRY(xu_event_pairs(f, chunks + 2));
+        TRY(event_pairs(f, f->xu_ev, chunks + 2));
         if (!f->dxu) FCK(cudaMalloc(&f->dxu, sizeof(double) * f->M * f->d));
         FCK(cudaEventRecord(f->xu_ev[0], f->eu->st));
+    }
+    if (dmll_x) {
+        TRY(event_pairs(f, f->x_ev, 2 * chunks + 1));
+        if (!f->dx) FCK(cudaMalloc(&f->dx, sizeof(double) * f->N * f->d));
+        FCK(cudaEventRecord(f->x_ev[0], f->eu->st));
     }
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
@@ -529,8 +569,8 @@ static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, const
     FCK(solve_device(eu, f->rhsm, f->tmpm, f->betav));
     FCK(cudaMemsetAsync(f->gacc, 0, sizeof(double) * GPB200_MAX_THETA, st));
     FCK(cudaMemsetAsync(f->Hbuf, 0, sizeof(double) * Mp * Mp, st));
-    if (f->mode == 3) return fsa_grad_kernel(f, dmll_kernel, dmll_xu);
-    size_t xk = 0;                                                        // contraction launches so far
+    if (f->mode == 3) return fsa_grad_kernel(f, dmll_kernel, dmll_xu, dmll_x);
+    size_t xk = 0, rk = 0;                                                // Xu / X contraction launches so far
     for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
         const int64_t nc = std::min(Nc, f->N - r0);
         const double* xr = f->x + r0 * f->d;
@@ -544,6 +584,10 @@ static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, const
         FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufB, Mp, f->gpart, f->gtmp, st, &eu->launches));
         FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufB, 0, nullptr, xk > 0)); ++xk; }
+        if (dmll_x) {
+            TRY(x_rows(f, rk + 1, xr, nc, f->bufB, f->mode == 0 ? f->gvec + r0 : nullptr, nullptr, nullptr, f->dx + r0 * f->d, 0));
+            ++rk;
+        }
         if (f->mode != 0) continue;                                       // no Lambda-derivative terms for SoR / DTC
         // diagonal term sum_i g_i dK_ii/dθ_p (scratch: bufC as np x nc)
         FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->gvec + r0, f->bufC, st, &eu->launches));
@@ -569,24 +613,32 @@ static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, const
         TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, 1)); ++xk;
         FCK(cudaEventRecord(f->xu_ev[1], st));
     }
+    if (dmll_x) FCK(cudaEventRecord(f->x_ev[1], st));
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta above
     if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
     if (dmll_xu) TRY(xu_finish(f, xk, dmll_xu));
+    if (dmll_x) TRY(x_finish(f, rk, dmll_x));
     return GPB200_OK;
 }
 
 int gpb200_fitc_grad_kernel(gpb200_fitc* f, double* dmll_kernel) {
     if (!f || !dmll_kernel) return GPB200_EINVAL;
-    return fitc_grad(f, dmll_kernel, nullptr, "fitc_grad_kernel");
+    return fitc_grad(f, dmll_kernel, nullptr, nullptr, "fitc_grad_kernel");
 }
 
 int gpb200_fitc_grad_kernel_inducing(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
     if (!f) return GPB200_EINVAL;
     if (!dmll_xu) return fail(f, GPB200_EINVAL, "fitc_grad_kernel_inducing: dmll_xu is required");
-    return fitc_grad(f, dmll_kernel, dmll_xu, "fitc_grad_kernel_inducing");
+    return fitc_grad(f, dmll_kernel, dmll_xu, nullptr, "fitc_grad_kernel_inducing");
+}
+
+int gpb200_fitc_grad_kernel_inputs(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double* dmll_x) {
+    if (!f) return GPB200_EINVAL;
+    if (!dmll_x) return fail(f, GPB200_EINVAL, "fitc_grad_kernel_inputs: dmll_x is required");
+    return fitc_grad(f, dmll_kernel, dmll_xu, dmll_x, "fitc_grad_kernel_inputs");
 }
 
 // Replaces the inducing inputs of both sub-engines in place (same M and d: no buffer is reallocated); the training inputs,
@@ -602,6 +654,22 @@ int gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_
     f->factored = f->alpha_ready = f->cv_m_ok = false;
     FSUB(gpb200_set_data(f->eu, M, f->d, xu, ldxu), f->eu);
     FSUB(gpb200_set_data(f->es, M, f->d, xu, ldxu), f->es);
+    return GPB200_OK;
+}
+
+// Replaces the training inputs in place (same N and d: no buffer is reallocated); FSA rebuilds its padded copy through the
+// kept row map, so the blocks, their work lists and every workspace stay.  The factorisation, alpha and the cross-validation
+// state refer to the old inputs and are invalidated.
+int gpb200_fitc_set_inputs(gpb200_fitc* f, int64_t N, const double* x, int64_t ldx) {
+    if (!f) return GPB200_EINVAL;
+    if (!f->has_data) return fail(f, GPB200_ESTATE, "fitc_set_inputs: set_data first");
+    if (N != f->N || !x || ldx < f->d) return fail(f, GPB200_EINVAL, "fitc_set_inputs: N must be set_data's, x non-null and ldx >= d");
+    FCK(cudaSetDevice(f->device));
+    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    cudaStream_t st = f->eu->st;
+    FCK(cudaMemcpy2DAsync(f->x, sizeof(double) * f->d, x, sizeof(double) * ldx, sizeof(double) * f->d, N, cudaMemcpyHostToDevice, st));
+    if (f->fsa) TRY(fsa_set_inputs(f, x, ldx));
+    FCK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
 
@@ -863,6 +931,7 @@ int gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n) {
     for (int32_t i = 0; i < n && i < 3; ++i) ms[i] = f->rand_ms[i];
     for (int32_t i = 3; i < n && i < 7; ++i) ms[i] = f->fsag_ms[i - 3];
     for (int32_t i = 7; i < n && i < 9; ++i) ms[i] = f->xu_ms[i - 7];
+    for (int32_t i = 9; i < n && i < 11; ++i) ms[i] = f->x_ms[i - 9];
     return GPB200_OK;
 }
 

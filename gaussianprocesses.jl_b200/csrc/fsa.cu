@@ -285,6 +285,50 @@ __global__ void __launch_bounds__(DX_NT) fsa_crossgram_dx_kernel(
     }
 }
 
+// One CTA of TB threads per item (one 128-row tile row of a block), thread t owns row i = 128 tile + t of the block and walks
+// l = 0 .. n-1 in order: G[i][l] along its own row (cached lines), G[l][i] down column i (coalesced over the threads), x_l
+// the same for every thread.  No atomics and no cross-thread sums: a row's result does not depend on the launch.  FAST: the
+// single SEIso leaf with d <= 8, the d-vectors in registers; else kprog_eval_dx with a local-memory d-vector.
+template <bool FAST>
+__global__ void __launch_bounds__(TB) fsa_block_dx_kernel(const __grid_constant__ KProg P, const double* __restrict__ xb, int d,
+                                                         const FsaBlockDxItem* __restrict__ items, const long long* __restrict__ map,
+                                                         double* __restrict__ out, int accumulate) {
+    constexpr int DR = FAST ? 8 : GPB200_MAX_DIMS;
+    const FsaBlockDxItem it = items[blockIdx.x];
+    const long long i = (long long)it.tile * TB + threadIdx.x;
+    if (i >= it.n) return;
+    const int dk = FAST ? 8 : d;
+    double acc[DR];
+#pragma unroll
+    for (int k = 0; k < dk; ++k) acc[k] = 0.0;
+    const double* xi = xb + (it.row0 + i) * d;
+    const double* gr = it.G + i * it.B;
+    const double* gc = it.G + i;
+    if (FAST) {
+        const double il2 = 1.0 / P.par[0], mh = -0.5 / P.par[0], s2 = P.par[1];
+        double xr[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) xr[k] = k < d ? xi[k] : 0.0;
+#pragma unroll 1
+        for (long long l = 0; l < it.n; ++l) {
+            const double* xl = xb + (it.row0 + l) * d;
+            double df[8], r2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { df[k] = k < d ? xr[k] - xl[k] : 0.0; r2 += df[k] * df[k]; }
+            const double f = -s2 * exp(mh * r2) * il2 * (gr[l] + gc[l * it.B]);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) acc[k] += f * df[k];
+        }
+    } else {
+#pragma unroll 1
+        for (long long l = 0; l < it.n; ++l) kprog_eval_dx(P, xi, xb + (it.row0 + l) * d, gr[l] + gc[l * it.B], acc, 0.0, nullptr);
+    }
+    const long long r = map ? map[it.row0 + i] : it.row0 + i;
+#pragma unroll
+    for (int k = 0; k < dk; ++k)
+        if (k < d) out[r * d + k] = accumulate ? out[r * d + k] + acc[k] : acc[k];
+}
+
 bool g_gemm_attr = false;
 
 }  // namespace
@@ -396,6 +440,16 @@ cudaError_t fsa_crossgram_dx_launch(const KProg& P, const double* xs, const doub
                                     const FsaDxItem* items, int n, double* dmu, double* dvar, cudaStream_t st, int64_t* launches) {
     if (n <= 0) return cudaSuccess;
     fsa_crossgram_dx_kernel<<<n, DX_NT, 0, st>>>(P, xs, z, xb, d, M, u, Wb, S1, S2, ldw, mask, alpha, E, lde, items, dmu, dvar);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t fsa_block_dx_launch(const KProg& P, const double* xb, int d, const FsaBlockDxItem* items, int n, const long long* map,
+                                double* out, int accumulate, cudaStream_t st, int64_t* launches) {
+    if (n <= 0) return cudaSuccess;
+    if (d <= 0 || d > GPB200_MAX_DIMS) return cudaErrorInvalidValue;
+    if (kprog_fast(P, d) && d <= 8) fsa_block_dx_kernel<true><<<n, TB, 0, st>>>(P, xb, d, items, map, out, accumulate);
+    else fsa_block_dx_kernel<false><<<n, TB, 0, st>>>(P, xb, d, items, map, out, accumulate);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

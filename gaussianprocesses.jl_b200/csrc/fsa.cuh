@@ -90,3 +90,18 @@ cudaError_t fsa_crossgram_dx_launch(const KProg& P, const double* xs, const doub
                                     const double* u, const double* Wb, const double* S1, const double* S2, long long ldw,
                                     const double* mask, const double* alpha, const double* E, long long lde,
                                     const FsaDxItem* items, int n, double* dmu, double* dvar, cudaStream_t st, int64_t* launches);
+// Training-input gradient of the block-diagonal part: for every real row i (< n) of the item's 128-row tile row of a block
+// with B x B weights G (row-major, ld B; rows 0 .. n-1 real, the rest padding), whose row 0 is padded row row0 of xb,
+//   out[row(i), :] (=, or += when accumulate) sum_{l < n} (G[i][l] + G[l][i]) d1k(x_i, x_l)
+// (d1k: derivative in the first argument; the l = i term is G[i][i] times the derivative of k(x_i, x_i)), row(i) =
+// map[row0 + i] (map may be null: row0 + i).  One CTA per item, one thread per row, no atomics: fixed-order sums.
+struct FsaBlockDxItem {
+    const double* G;
+    long long row0;
+    int B;                  // padded block size, the leading dimension of G
+    int n;                  // real rows of the block
+    int tile;               // tile row: rows 128 tile .. 128 tile + 127
+    int pad_;
+};
+cudaError_t fsa_block_dx_launch(const KProg& P, const double* xb, int d, const FsaBlockDxItem* items, int n, const long long* map,
+                                double* out, int accumulate, cudaStream_t st, int64_t* launches);

@@ -39,6 +39,7 @@ struct FsaChunk {
     // kernel gradient: G_i = alpha_i alpha_i' - Lambda_i^-1 + Y_i Y_i' as full tiles of the chunk's blocks in Gpk
     FsaLaunch gtiles;                                   // FsaGramItem list: every tile (r, c) of every block, dst in Gpk
     FsaLaunch ginv, gyy, gp1t;                          // -X_r' X_c tiles ; += Y_r Y_c' ; (K_uu^-1 K_uf G_bd) (bufA, Mpad x Nc)
+    FsaLaunch bdx;                                      // training-input gradient: FsaBlockDxItem list, one per tile row of a block
 };
 struct Fsa {
     int64_t nblocks = 0, Np = 0, n_pad = 0, packed = 0;
@@ -47,6 +48,9 @@ struct Fsa {
     double *xb = nullptr, *mask = nullptr, *X = nullptr, *LT = nullptr, *logd = nullptr;
     double *r = nullptr, *a = nullptr, *t1 = nullptr, *t2 = nullptr;
     long long *pos = nullptr, *bstart = nullptr, *boff = nullptr;
+    long long* ipos = nullptr;                          // padded row -> caller index (-1 on padding): inverse of pos
+    FsaBlockDxItem* bdx = nullptr;
+    std::vector<long long> pos_h;                       // pos on the host: gpb200_fitc_set_inputs rebuilds xb through it
     int *rblk = nullptr, *bsize = nullptr, *info = nullptr;
     FsaGemmItem* gitems = nullptr;
     Potrf128Item* litems = nullptr;
@@ -132,7 +136,7 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     const int d = f->d;
     const int64_t Mp = f->Mpad, Nc = f->Nc;
     // host tables: padded layout, positions, the reordered inputs
-    std::vector<long long> bstart((size_t)nblocks), boff((size_t)nblocks), pos((size_t)N);
+    std::vector<long long> bstart((size_t)nblocks), boff((size_t)nblocks), pos((size_t)N), ipos;
     std::vector<int> bsize((size_t)nblocks), rblk((size_t)Np);
     std::vector<double> mask((size_t)Np, 0.0), xh((size_t)N * d), xb((size_t)Np * d, 0.0);
     FCK(cudaMemcpy(xh.data(), f->x, sizeof(double) * N * d, cudaMemcpyDeviceToHost));
@@ -158,6 +162,7 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     FCK(cudaMemsetAsync(s->X, 0, sizeof(double) * packed, st));
     FCK(cudaMemsetAsync(s->LT, 0, sizeof(double) * packed, st));
     FCK(cudaMalloc(&s->pos, sizeof(long long) * N));
+    FCK(cudaMalloc(&s->ipos, sizeof(long long) * Np));
     FCK(cudaMalloc(&s->bstart, sizeof(long long) * nblocks));
     FCK(cudaMalloc(&s->boff, sizeof(long long) * nblocks));
     FCK(cudaMalloc(&s->bsize, sizeof(int) * nblocks));
@@ -175,6 +180,9 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     FCK(cudaMemcpy(s->xb, xb.data(), sizeof(double) * Np * d, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->mask, mask.data(), sizeof(double) * Np, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->pos, pos.data(), sizeof(long long) * N, cudaMemcpyHostToDevice));
+    ipos.assign((size_t)Np, -1);
+    for (int64_t i = 0; i < N; ++i) ipos[(size_t)pos[(size_t)i]] = i;
+    FCK(cudaMemcpy(s->ipos, ipos.data(), sizeof(long long) * Np, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->bstart, bstart.data(), sizeof(long long) * nblocks, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->boff, boff.data(), sizeof(long long) * nblocks, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->bsize, bsize.data(), sizeof(int) * nblocks, cudaMemcpyHostToDevice));
@@ -182,12 +190,13 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     if (f->eu->tma_ok && !gemm_make_tensor_map(&s->mapWt, f->bufA, Mp, Nc, Nc)) {
         return fail(f, GPB200_ECUDA, "fitc_set_blocks: cuTensorMapEncodeTiled failed");
     }
-    s->bstart_h = bstart; s->boff_h = boff; s->bsize_h = bsize;
+    s->bstart_h = bstart; s->boff_h = boff; s->bsize_h = bsize; s->pos_h = pos;
     s->bchunk_h.assign((size_t)nblocks, 0);
     // work lists: staging chunks of whole blocks, then every launch of factorize / grad_noise as a range of items
     std::vector<FsaGemmItem> gi;
     std::vector<Potrf128Item> li;
     std::vector<FsaGramItem> gr;
+    std::vector<FsaBlockDxItem> bd;
     auto gemm = [&](double* C, long long ldc, const double* A, long long lda, const double* B, long long ldb, int64_t K,
                     double alpha, double beta, bool lower) {
         FsaGemmItem it{};
@@ -307,6 +316,12 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
                     gemm(f->bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, f->bufB + u * TILE * Nc + (bstart[b] - ch.r0), Nc,
                          Gt(b, r, 0), bsize[b], bsize[b], 1.0, 0.0, false);
         close_g(ch.gp1t);
+        ch.bdx.off = (int64_t)bd.size();                // the real tile rows of every block, G_b in Gpk as above
+        for (int64_t b = b0; b < b1; ++b) {
+            const int64_t n = block_ptr[b + 1] - block_ptr[b];
+            for (int r = 0; (int64_t)r * TILE < n; ++r) bd.push_back(FsaBlockDxItem{Gt(b, 0, 0), bstart[b], bsize[b], (int)n, r, 0});
+        }
+        ch.bdx.n = (int)((int64_t)bd.size() - ch.bdx.off);
         for (int64_t b = b0; b < b1; ++b) s->bchunk_h[(size_t)b] = (int)s->chunks.size();
         s->chunks.push_back(std::move(ch));
         b0 = b1;
@@ -317,6 +332,8 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     FCK(cudaMemcpy(s->gitems, gi.data(), sizeof(FsaGemmItem) * gi.size(), cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->litems, li.data(), sizeof(Potrf128Item) * li.size(), cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->gramitems, gr.data(), sizeof(FsaGramItem) * gr.size(), cudaMemcpyHostToDevice));
+    FCK(cudaMalloc(&s->bdx, sizeof(FsaBlockDxItem) * std::max<size_t>(bd.size(), 1)));
+    FCK(cudaMemcpy(s->bdx, bd.data(), sizeof(FsaBlockDxItem) * bd.size(), cudaMemcpyHostToDevice));
     FCK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
@@ -332,7 +349,7 @@ void fsa_free(gpb200_fitc* f) {
     Fsa* s = f->fsa;
     void* ptrs[] = {s->xb, s->mask, s->X, s->LT, s->logd, s->r, s->a, s->t1, s->t2, s->pos, s->bstart, s->boff,
                     s->rblk, s->bsize, s->info, s->gitems, s->litems, s->gramitems, s->Gpk, s->gpart, s->ones,
-                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr, s->Sc, s->pp, s->Tb, s->Zb, s->pdx, s->pdi};
+                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr, s->Sc, s->pp, s->Tb, s->Zb, s->pdx, s->pdi, s->ipos, s->bdx};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete s;
     f->fsa = nullptr;
@@ -467,7 +484,7 @@ int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise) {
 //   W_uu = -beta beta' + K_uu^-1 - S^-1 + K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
 // since dSigma = dQ + blockdiag(dK - dQ) and <alpha alpha' - Sigma^-1, blockdiag(D)> = <G_bd, D>.  Called by
 // gpb200_fitc_grad_kernel once K_uu^-1, S^-1 (full symmetric, sub-engines' G) and beta are in place, gacc and Hbuf zeroed.
-int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
+int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double* dmll_x) {
     Fsa* s = f->fsa;
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
@@ -478,7 +495,7 @@ int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
     GemmBuf bAt{tma ? &s->mapWt : nullptr, f->bufA, Nc};        // bufA as Mpad x Nc
     GemmBuf bB2{tma ? &f->mapB2 : nullptr, f->bufB, Mp};        // bufB as Nc x Mpad
     GemmBuf bBt{tma ? &f->mapB : nullptr, f->bufB, Nc};         // bufB as Mpad x Nc
-    size_t xk = 0;                                                // inducing-point contractions so far
+    size_t xk = 0, rk = 0;                                        // inducing-point / training-input contractions so far
     for (const FsaChunk& ch : s->chunks) {
         const double* xr = s->xb + ch.r0 * f->d;
         const int64_t nc = ch.rows;
@@ -494,6 +511,12 @@ int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
         FCK(fsa_outer_launch(s->gramitems + ch.gtiles.off, ch.gtiles.n, s->a, st, &eu->launches));
         FCK(fsa_trace_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gtiles.off, ch.gtiles.n, s->mask, s->gpart, f->gtmp, st, &eu->launches));
         FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        if (dmll_x) {                                               // the G_b part of dmll/dX, written in the caller's order
+            ++rk;
+            FCK(cudaEventRecord(f->x_ev[2 * rk], st));
+            FCK(fsa_block_dx_launch(eu->prog, s->xb, f->d, s->bdx + ch.bdx.off, ch.bdx.n, s->ipos, f->dx, 0, st, &eu->launches));
+            FCK(cudaEventRecord(f->x_ev[2 * rk + 1], st));
+        }
         // P1' = K_uu^-1 K_uf (bufB, Mpad x Nc) from K_fu (bufA)
         FCK(fitc_kfu(f, xr, nc));
         FCK(fsa_mask_launch(f->bufA, Mp, nc, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
@@ -506,6 +529,7 @@ int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
         FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         // dmll/dXu: the padding rows of the chunk are skipped (mask 0); Xu is in the caller's order (never permuted)
         if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufC, 0, s->mask + ch.r0, xk > 0)); ++xk; }
+        if (dmll_x) { TRY(x_rows(f, rk + 1, xr, nc, f->bufC, nullptr, s->mask + ch.r0, s->ipos + ch.r0, f->dx, 1)); ++rk; }
         FCK(gemm_whole(eu, bBt, bAt, f->Hbuf, Mp, Mp, Mp, nc, 1.0, 1.0));   // H += P1' G_bd P1 = K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
     }
     FCK(fitc_wuu_launch(f->Wbuf, f->Hbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
@@ -515,12 +539,24 @@ int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu) {
         TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, xk > 0)); ++xk;
         FCK(cudaEventRecord(f->xu_ev[1], st));
     }
+    if (dmll_x) FCK(cudaEventRecord(f->x_ev[1], st));
     std::vector<double> out((size_t)std::max(np, 1));
     FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta in gpb200_fitc_grad_kernel
     if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
     if (dmll_xu) TRY(xu_finish(f, xk, dmll_xu));
+    if (dmll_x) TRY(x_finish(f, rk, dmll_x));
+    return GPB200_OK;
+}
+
+// gpb200_fitc_set_inputs: the padded inputs xb through the row map of gpb200_fitc_set_blocks, built as it builds them
+int fsa_set_inputs(gpb200_fitc* f, const double* x, int64_t ldx) {
+    Fsa* s = f->fsa;
+    const int d = f->d;
+    std::vector<double> xb((size_t)s->Np * d, 0.0);
+    for (int64_t i = 0; i < f->N; ++i) memcpy(&xb[(size_t)s->pos_h[(size_t)i] * d], x + i * ldx, sizeof(double) * d);
+    FCK(cudaMemcpy(s->xb, xb.data(), sizeof(double) * s->Np * d, cudaMemcpyHostToDevice));
     return GPB200_OK;
 }
 

@@ -694,6 +694,61 @@ __global__ void __launch_bounds__(NT) inputs_dx_kernel(const __grid_constant__ K
     }
 }
 
+// training-input gradient of the sparse mll, one warp per training row i (RX_PB rows per CTA):
+//   out[row(i), :] (=, or += when accumulate) sum_{j < M} W[i * ldw + j] d1k(x_i, u_j) + 2 c_i d1k(x_i, x_i)
+// (d1k: derivative in the first argument; 2 d1k(x, x) is the derivative of k(x, x)).  W is the adjoint W_fu of a chunk
+// (row-major, ld Mpad): the lanes run across row i, so its reads are coalesced.  Rows with mask[i] == 0 (FSA padding) are
+// skipped, not weighted by 0: their output rows are neither read nor written.  row(i) = map[i] (the caller's order of an FSA
+// row) or i.  The c term enters lane 0 before its columns; each coordinate is then reduced by one fixed shuffle tree, so the
+// result does not depend on the grid.  FAST: the single SEIso leaf with d <= 8, the d-vectors in registers (its d1k(x, x)
+// is 0 and the c term is left out); else kprog_eval_dx with a local-memory d-vector.
+constexpr int RX_PB = NT / 32;
+template <bool FAST>
+__global__ void __launch_bounds__(NT) rows_dx_kernel(const __grid_constant__ KProg P, const double* __restrict__ x, long long ldx,
+                                                     long long n, const double* __restrict__ u, long long ldu, long long M, int d,
+                                                     const double* __restrict__ W, long long ldw, const double* __restrict__ c,
+                                                     const double* __restrict__ mask, const long long* __restrict__ map,
+                                                     double* __restrict__ out, int accumulate) {
+    constexpr int DR = FAST ? 8 : GPB200_MAX_DIMS;
+    const int lane = threadIdx.x & 31;
+    const long long i = (long long)blockIdx.x * RX_PB + (threadIdx.x >> 5);
+    if (i >= n || (mask && mask[i] == 0.0)) return;      // whole warps: no barrier below
+    const int dk = FAST ? 8 : d;
+    double acc[DR];
+#pragma unroll
+    for (int k = 0; k < dk; ++k) acc[k] = 0.0;
+    const double* xi = x + i * ldx;
+    const double* wr = W + i * ldw;
+    if (FAST) {
+        const double il2 = 1.0 / P.par[0], mh = -0.5 / P.par[0], s2 = P.par[1];
+        double xr[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) xr[k] = k < d ? xi[k] : 0.0;
+#pragma unroll 1
+        for (long long j = lane; j < M; j += 32) {
+            const double* uj = u + j * ldu;
+            double df[8], r2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { df[k] = k < d ? xr[k] - uj[k] : 0.0; r2 += df[k] * df[k]; }
+            const double f = -s2 * exp(mh * r2) * il2 * wr[j];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) acc[k] += f * df[k];
+        }
+    } else {
+        if (c && lane == 0) kprog_eval_dx(P, xi, xi, 2.0 * c[i], acc, 0.0, nullptr);
+#pragma unroll 1
+        for (long long j = lane; j < M; j += 32) kprog_eval_dx(P, xi, u + j * ldu, wr[j], acc, 0.0, nullptr);
+    }
+    const long long r = map ? map[i] : i;
+#pragma unroll
+    for (int k = 0; k < dk; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+        if (lane == 0 && k < d) out[r * d + k] = accumulate ? out[r * d + k] + v : v;
+    }
+}
+
 // strict-upper tiles of the Npad x Npad matrix F <- transpose of its strict-lower tiles (diagonal tiles untouched)
 __global__ void mirror_lower_tiles_kernel(double* __restrict__ F, long long ld) {
     __shared__ double tl[32][33];
@@ -907,6 +962,18 @@ cudaError_t inputs_dx_launch(const KProg& P, bool fast, const double* x, int64_t
     const unsigned grid = (unsigned)((N + IX_PB - 1) / IX_PB);
     if (fast) inputs_dx_kernel<true><<<grid, NT, 0, st>>>(P, x, ldx, d, N, alpha, G, ldg, out, bm_mod, bm_rem, bm_div);
     else inputs_dx_kernel<false><<<grid, NT, 0, st>>>(P, x, ldx, d, N, alpha, G, ldg, out, bm_mod, bm_rem, bm_div);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t rows_dx_launch(const KProg& P, const double* x, int64_t ldx, int64_t n, const double* u, int64_t ldu, int64_t M, int d,
+                           const double* W, int64_t ldw, const double* c, const double* mask, const long long* map, double* out,
+                           int accumulate, cudaStream_t st, int64_t* launches) {
+    if (n <= 0) return cudaSuccess;
+    if (d <= 0 || d > GPB200_MAX_DIMS || M < 0) return cudaErrorInvalidValue;
+    const unsigned grid = (unsigned)((n + RX_PB - 1) / RX_PB);
+    if (kprog_fast(P, d) && d <= 8) rows_dx_kernel<true><<<grid, NT, 0, st>>>(P, x, ldx, n, u, ldu, M, d, W, ldw, c, mask, map, out, accumulate);
+    else rows_dx_kernel<false><<<grid, NT, 0, st>>>(P, x, ldx, n, u, ldu, M, d, W, ldw, c, mask, map, out, accumulate);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

@@ -55,5 +55,13 @@ cudaError_t inducing_dx_launch(const KProg& P, const double* u, int64_t ldu, int
 cudaError_t inputs_dx_launch(const KProg& P, bool fast, const double* x, int64_t ldx, int d, int64_t N, const double* alpha,
                              const double* G, int64_t ldg, double* out, cudaStream_t st, int64_t* launches, int bm_mod,
                              int bm_rem, int bm_div);
+// training-input gradient of the sparse mll over n rows x_i (output rows point-major, d wide):
+//   out[row(i), :] (=, or += when accumulate) sum_{j < M} W[i * ldw + j] d1k(x_i, u_j) + 2 c_i d1k(x_i, x_i)
+// (d1k: derivative in the first argument; c may be null: 0), over the rows with mask[i] != 0 (mask may be null; the others
+// are neither read nor written), row(i) = map[i] (map may be null: i).  One warp per row; the single SEIso leaf with d <= 8
+// takes a register specialisation.  Fixed-order sums.
+cudaError_t rows_dx_launch(const KProg& P, const double* x, int64_t ldx, int64_t n, const double* u, int64_t ldu, int64_t M, int d,
+                           const double* W, int64_t ldw, const double* c, const double* mask, const long long* map, double* out,
+                           int accumulate, cudaStream_t st, int64_t* launches);
 // F[j, i] = F[i, j] for every element of the strict-lower 128-tiles of the Npad x Npad matrix F (diagonal tiles untouched)
 cudaError_t mirror_lower_tiles_launch(double* F, int64_t ld, int64_t Npad, cudaStream_t st, int64_t* launches);

@@ -278,21 +278,29 @@ static cudaError_t items_to_device(const void* src, size_t bytes, void** d, cuda
 }
 
 int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
-    if (!h || (n > 0 && !args) || which < 0 || which > 11 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    if (!h || (n > 0 && !args) || which < 0 || which > 12 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
     // fixed arguments before the flattened items, and the item stride (0: no items)
-    static const int head[12] = {3, 9, 6, 5, 5, 1, 5, 6, 4, 0, 5, 16};
-    static const int stride[12] = {5, 0, 0, 0, 0, 5, 5, 0, 5, 6, 0, 4};
+    static const int head[13] = {3, 9, 6, 5, 5, 1, 5, 6, 4, 0, 5, 16, 5};
+    static const int stride[13] = {5, 0, 0, 0, 0, 5, 5, 0, 5, 6, 0, 4, 5};
     const int hd = head[which], sd = stride[which];
     if (sd ? (n < hd || (n - hd) % sd) : n != hd) return fail(h, GPB200_EINVAL, "fsa_kernels: wrong argument count for this kernel");
     const int ni = sd ? (n - hd) / sd : 0;
     auto ptr = [&](int i) { return reinterpret_cast<double*>(args[i]); };
-    std::vector<FsaGramItem> gitems(sd == 5 ? ni : 0);
+    const bool bdx = which == 12;                        // block_dx items share the Gram items' stride
+    std::vector<FsaGramItem> gitems(sd == 5 && !bdx ? ni : 0);
+    std::vector<FsaBlockDxItem> bitems(bdx ? ni : 0);
     std::vector<FsaRowItem> ritems(sd == 6 ? ni : 0);
     std::vector<FsaDxItem> ditems(sd == 4 ? ni : 0);
     int64_t max_nb = 0;
     for (int k = 0; k < ni; ++k) {
         const int64_t* q = args + hd + sd * k;
-        if (sd == 4) {                                   // row, out, b0, nb
+        if (bdx) {                                       // G, row0, B, n, tile
+            if (!q[0] || q[1] < 0 || q[2] < TILE || q[2] % TILE || q[2] > INT_MAX || q[3] < 0 || q[3] > q[2] || q[4] < 0 ||
+                q[4] * TILE >= q[2])
+                return fail(h, GPB200_EINVAL, "fsa_kernels: block_dx item with a null G, a negative row0, B not a positive "
+                                              "multiple of 128, n outside [0, B] or a tile row past B");
+            bitems[k] = FsaBlockDxItem{reinterpret_cast<const double*>(q[0]), q[1], (int)q[2], (int)q[3], (int)q[4], 0};
+        } else if (sd == 4) {                            // row, out, b0, nb
             if (q[0] < 0 || q[1] < 0 || q[2] < 0 || q[3] < 0)
                 return fail(h, GPB200_EINVAL, "fsa_kernels: crossgram_dx item with a negative row, out, b0 or nb");
             ditems[k] = FsaDxItem{q[0], q[1], q[2], q[3]};
@@ -313,10 +321,10 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
         return true;
     };
     KProg P{};
-    const bool prog = which == 0 || which == 6 || which == 8 || which == 11;
+    const bool prog = which == 0 || which == 6 || which == 8 || which == 11 || which == 12;
     if (prog) {
         const int64_t d = args[which == 8 ? 2 : which == 11 ? 3 : 1];
-        if (which == 11 && d > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "fsa_kernels: d above GPB200_MAX_DIMS");
+        if ((which == 11 || which == 12) && d > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "fsa_kernels: d above GPB200_MAX_DIMS");
         const int32_t want = h->prog.n_theta + (which == 0 ? 1 : 0);
         if (h->has_kernel && nf != want) return fail(h, GPB200_EINVAL, "fsa_kernels: fargs = theta (+ diag_add for fsa_gram)");
         TRY(local_prog(h, "fsa_kernels", fargs, h->prog.n_theta, d, P));
@@ -341,6 +349,7 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
              (!args[6] || args[9] >= args[4]) &&
              (!args[15] || (need({7, 8}) && args[9] >= args[4] && (max_nb == 0 || (args[12] && args[13] >= max_nb))));
         break;
+    case 12: ok = need({0, 3}) && (args[4] == 0 || args[4] == 1); break;    // xb, d, map, out, accumulate | items
     }
     if (!ok) return fail(h, GPB200_EINVAL, "fsa_kernels: a null pointer, a negative size, a bad mode or ld below the row width");
     CK(cudaSetDevice(h->device));
@@ -349,7 +358,9 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
     FsaGramItem* dg = nullptr;
     FsaRowItem* dr = nullptr;
     FsaDxItem* dd = nullptr;
-    cudaError_t e = sd == 6   ? items_to_device(ritems.data(), sizeof(FsaRowItem) * ritems.size(), reinterpret_cast<void**>(&dr), st)
+    FsaBlockDxItem* db = nullptr;
+    cudaError_t e = bdx       ? items_to_device(bitems.data(), sizeof(FsaBlockDxItem) * bitems.size(), reinterpret_cast<void**>(&db), st)
+                    : sd == 6 ? items_to_device(ritems.data(), sizeof(FsaRowItem) * ritems.size(), reinterpret_cast<void**>(&dr), st)
                     : sd == 4 ? items_to_device(ditems.data(), sizeof(FsaDxItem) * ditems.size(), reinterpret_cast<void**>(&dd), st)
                               : items_to_device(gitems.data(), sizeof(FsaGramItem) * gitems.size(), reinterpret_cast<void**>(&dg), st);
     if (e == cudaSuccess) {
@@ -369,12 +380,15 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
         case 10: e = fsa_var_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
         case 11: e = fsa_crossgram_dx_launch(P, ptr(0), ptr(1), ptr(2), (int)args[3], args[4], ptr(5), ptr(6), ptr(7), ptr(8),
                                              args[9], ptr(10), ptr(11), ptr(12), args[13], dd, ni, ptr(14), ptr(15), st, L); break;
+        case 12: e = fsa_block_dx_launch(P, ptr(0), (int)args[1], db, ni, reinterpret_cast<const long long*>(args[2]), ptr(3),
+                                         (int)args[4], st, L); break;
         }
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (dg) cudaFree(dg);
     if (dr) cudaFree(dr);
     if (dd) cudaFree(dd);
+    if (db) cudaFree(db);
     CK(e);
     return GPB200_OK;
 }
@@ -475,8 +489,8 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
 }
 
 int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
-    if (!h || !args || which < 0 || which > 14 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
-    static const int want[15] = {14, 14, 4, 8, 5, 5, 10, 6, 5, 6, 5, 9, 7, 3, 13};
+    if (!h || !args || which < 0 || which > 15 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    static const int want[16] = {14, 14, 4, 8, 5, 5, 10, 6, 5, 6, 5, 9, 7, 3, 13, 14};
     if (n != want[which]) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: wrong argument count for this kernel");
     const int64_t* a = args;
     auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
@@ -492,8 +506,12 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
         // u, ldu, M, z, ldz, n, d, W, ldw, sym, mask, out, accumulate
         if (a[6] > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: d exceeds GPB200_MAX_DIMS");
         TRY(local_prog(h, "fitc_cv_kernels", fargs, nf, a[6], P));
+    } else if (which == 15) {
+        // x, ldx, n, u, ldu, M, d, W, ldw, c, mask, map, out, accumulate
+        if (a[6] > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: d exceeds GPB200_MAX_DIMS");
+        TRY(local_prog(h, "fitc_cv_kernels", fargs, nf, a[6], P));
     } else if (nf != 0) {
-        return fail(h, GPB200_EINVAL, "fitc_cv_kernels: fargs = theta for delta and inducing_dx, none otherwise");
+        return fail(h, GPB200_EINVAL, "fitc_cv_kernels: fargs = theta for delta, inducing_dx and rows_dx, none otherwise");
     }
     bool ok = true;
     switch (which) {
@@ -517,6 +535,8 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
     case 13: ok = need({0}) && a[2] >= 0 && a[1] >= a[2]; break;                       // symmetrize: A, ld, n
     case 14: ok = need({0, 3, 7, 11}) && a[2] >= 0 && a[5] >= 0 && a[1] >= a[6] && a[4] >= a[6] && a[8] >= a[2] &&
                   (a[9] == 0 || (a[9] == 1 && a[5] == a[2])) && (a[12] == 0 || a[12] == 1); break;
+    case 15: ok = need({0, 3, 7, 12}) && a[2] >= 0 && a[5] >= 0 && a[1] >= a[6] && a[4] >= a[6] && a[8] >= a[5] &&
+                  (a[13] == 0 || a[13] == 1); break;
     }
     if (!ok) return fail(h, GPB200_EINVAL, "fitc_cv_kernels: a null pointer, a negative size, a bad mode or ld below the row width");
     CK(cudaSetDevice(h->device));
@@ -543,6 +563,8 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
     case 13: e = symmetrize_launch(ptr(0), a[1], a[2], st, L); break;
     case 14: e = inducing_dx_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], (int)a[6], ptr(7), a[8], (int)a[9], ptr(10), ptr(11),
                                     (int)a[12], st, L); break;
+    case 15: e = rows_dx_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], (int)a[6], ptr(7), a[8], ptr(9), ptr(10),
+                                reinterpret_cast<const long long*>(a[11]), ptr(12), (int)a[13], st, L); break;
     }
     CK(e);
     CK(cudaStreamSynchronize(st));

@@ -81,6 +81,8 @@ _SIGNATURES = {
     "gpb200_fitc_grad_kernel": (C.c_int, [_H, _dp]),
     "gpb200_fitc_grad_kernel_inducing": (C.c_int, [_H, _dp, _dp]),
     "gpb200_fitc_set_inducing": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
+    "gpb200_fitc_grad_kernel_inputs": (C.c_int, [_H, _dp, _dp, _dp]),
+    "gpb200_fitc_set_inputs": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
     "gpb200_fitc_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp]),
     "gpb200_fitc_predict_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
     "gpb200_fitc_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
@@ -462,9 +464,9 @@ class Engine:
         self._check(self._lib.gpb200_row_reductions(self._h, int(which), a.ctypes.data_as(_lp), a.size), "row_reductions")
 
     FSA_KERNELS = ("gram", "bdmv", "mask", "permute", "resid", "outer", "trace", "axpy_t", "crossgram", "rowdot", "var",
-                   "crossgram_dx")
+                   "crossgram_dx", "block_dx")
     FITC_CV_KERNELS = ("delta", "rows", "invdiag", "eblock", "qs", "wvec", "gather", "diag", "colscale", "scale", "fitc_g",
-                       "fitc_wfu", "fitc_wuu", "symmetrize", "inducing_dx")
+                       "fitc_wfu", "fitc_wuu", "symmetrize", "inducing_dx", "rows_dx")
 
     def fsa_kernels(self, name, args, fargs=()):
         """One FSA block-diagonal kernel (include/gpb200.h) by name, on device buffers: args = the int64 arguments followed
@@ -555,6 +557,30 @@ class FitcEngine:
         if xu_pm.shape != (self.M, self.d):
             raise ValueError("fitc_set_inducing: the inducing points must keep their shape (%d, %d)" % (self.M, self.d))
         self._check(self._lib.gpb200_fitc_set_inducing(self._h, self.M, _as_dp(xu_pm), self.d), "fitc_set_inducing")
+
+    def grad_kernel_inputs(self, want_kernel=True, want_inducing=False):
+        """one sweep: (dmll_kernel[n_theta] or None, dmll_xu (M, d) or None, dmll_x (N, d)) without the mean's part;
+        dmll_kernel and dmll_xu bitwise those of grad_kernel and grad_kernel_inducing"""
+        g = np.empty(max(self.n_theta, 1)) if want_kernel else None
+        gu = np.empty((self.M, self.d)) if want_inducing else None
+        gx = np.empty((self.N, self.d))
+        self._check(self._lib.gpb200_fitc_grad_kernel_inputs(self._h, _as_dp(g) if want_kernel else None,
+                                                             _as_dp(gu) if want_inducing else None, _as_dp(gx)),
+                    "fitc_grad_kernel_inputs")
+        return (g[:self.n_theta].copy() if want_kernel else None), gu, gx
+
+    def set_inputs(self, x_pm):
+        """replace the training inputs (N, d) in place (FSA keeps its blocks by index); factorize + mll must follow"""
+        x_pm = np.ascontiguousarray(x_pm, dtype=np.float64)
+        if x_pm.shape != (self.N, self.d):
+            raise ValueError("fitc_set_inputs: the inputs must keep their shape (%d, %d)" % (self.N, self.d))
+        self._check(self._lib.gpb200_fitc_set_inputs(self._h, self.N, _as_dp(x_pm), self.d), "fitc_set_inputs")
+
+    def grad_inputs_timings(self):
+        """device times (ms) of the last grad_kernel_inputs: the dmll/dX contractions summed, the whole call"""
+        out = np.zeros(11)
+        self._check(self._lib.gpb200_fitc_get_timings(self._h, _as_dp(out), 11), "fitc_get_timings")
+        return out[9:].copy()
 
     def grad_inducing_timings(self):
         """device times (ms) of the last grad_kernel_inducing: the dmll/dXu contractions summed, the whole call"""

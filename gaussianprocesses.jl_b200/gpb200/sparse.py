@@ -30,6 +30,7 @@ class FITC:
         if self.Xu.shape[0] != self.dim or self.y.size != self.nobs:
             raise ValueError("Input and output observations must have consistent dimensions.")
         self._xpm = np.ascontiguousarray(self.x.T)
+        self._distributed = bool(distributed)
         self._eng = capi.FitcEngine(device)
         if distributed:
             import torch.distributed as dist
@@ -63,15 +64,24 @@ class FITC:
         self.dmll = np.array(out)
         return self
 
-    def update_dmll(self, noise=True, domean=True, kern=True, inducing=False):
+    def update_dmll(self, noise=True, domean=True, kern=True, inducing=False, inputs=False):
         """update_dmll! (src/GPE.jl:298-324) with the FITC strategy: [noise; mean; kernel].  inducing=True appends
-        dmll/dXu as vec(Xu) (one point after another); the kernel part and it come from one device sweep."""
+        dmll/dXu as vec(Xu) (one point after another); inputs=True then appends dmll/dX as vec(X) (on a distributed model:
+        this rank's points), the device's part plus alpha_i dm(x_i)/dx_i.  The kernel part and the point gradients come from
+        one device sweep."""
         out = []
         if noise:
             out.append(self._eng.grad_noise())                                   # fitc.jl:243-257
         if domean and self.mean.num_params() > 0:
             out.extend(self.mean.grad_stack(self._xpm).T @ self.alpha)           # GPE.jl:282-288
-        if inducing:
+        if inputs:
+            gk, gu, gx = self._eng.grad_kernel_inputs(want_kernel=kern, want_inducing=inducing)
+            if kern:
+                out.extend(gk[self._exposed])
+            if inducing:
+                out.extend(gu.ravel())
+            out.extend((gx + self.alpha[:, None] * self.mean.grad_x(self._xpm)).ravel())
+        elif inducing:
             gk, gx = self._eng.grad_kernel_inducing(want_kernel=kern)
             if kern:
                 out.extend(gk[self._exposed])
@@ -81,48 +91,65 @@ class FITC:
         self.dmll = np.array(out)
         return self
 
-    def update_mll_and_dmll(self, noise=True, domean=True, kern=True, inducing=False):
+    def update_mll_and_dmll(self, noise=True, domean=True, kern=True, inducing=False, inputs=False):
         self.update_mll()
-        return self.update_dmll(noise=noise, domean=domean, kern=kern, inducing=inducing)
+        return self.update_dmll(noise=noise, domean=domean, kern=kern, inducing=inducing, inputs=inputs)
 
     # ---- GPE's parameter protocol, [noise; mean; kernel] (src/GPE.jl:346-510), and optimize! (src/optimize.jl) -----------
     # logNoise is a scalar here; FixedKernel parameters are neither returned nor set, their gradients are dropped
     # (update_dmll's `_exposed`), exactly as for GPE.  inducing=True (not in the reference) appends vec(Xu), Julia's
-    # column-major vec of the dim x M matrix: [noise; mean; kernel; Xu].
-    def get_params(self, noise=True, domean=True, kern=True, inducing=False):
-        p = GPE.get_params(self, noise=noise, domean=domean, kern=kern)
-        return np.concatenate([p, self.Xu.T.ravel()]) if inducing else p
+    # column-major vec of the dim x M matrix, and inputs=True vec(X) of the dim x nobs matrix: [noise; mean; kernel; Xu; X].
+    def get_params(self, noise=True, domean=True, kern=True, inducing=False, inputs=False):
+        p = [GPE.get_params(self, noise=noise, domean=domean, kern=kern)]
+        if inducing:
+            p.append(self.Xu.T.ravel())
+        if inputs:
+            p.append(self._xpm.ravel())
+        return np.concatenate(p)
 
     num_params = GPE.num_params
 
-    def set_params(self, hyp, noise=True, domean=True, kern=True, inducing=False):
-        if not inducing:
+    def set_params(self, hyp, noise=True, domean=True, kern=True, inducing=False, inputs=False):
+        """inducing / inputs: the trailing vec(Xu) / vec(X) are moved on the engine in place (same sizes; FSA keeps its
+        blocks by index); the next update_mll refactorises."""
+        if not inducing and not inputs:
             return GPE.set_params(self, hyp, noise=noise, domean=domean, kern=kern)
         hyp = np.asarray(hyp, dtype=np.float64)
-        nu = self.Xu.size
-        if hyp.size != self.num_params(noise=noise, domean=domean, kern=kern, inducing=True):
+        nu = self.Xu.size if inducing else 0
+        nx = self.x.size if inputs else 0
+        if hyp.size != self.num_params(noise=noise, domean=domean, kern=kern, inducing=inducing, inputs=inputs):
             raise ValueError("wrong number of hyper-parameters")
-        GPE.set_params(self, hyp[:hyp.size - nu], noise=noise, domean=domean, kern=kern)
-        xu_pm = hyp[hyp.size - nu:].reshape(self.Xu.shape[1], self.dim)
-        self._eng.set_inducing(xu_pm)
-        self.Xu = np.ascontiguousarray(xu_pm.T)
+        n0 = hyp.size - nu - nx
+        GPE.set_params(self, hyp[:n0], noise=noise, domean=domean, kern=kern)
+        if inducing:
+            xu_pm = hyp[n0:n0 + nu].reshape(self.Xu.shape[1], self.dim)
+            self._eng.set_inducing(xu_pm)
+            self.Xu = np.ascontiguousarray(xu_pm.T)
+        if inputs:
+            xpm = np.ascontiguousarray(hyp[n0 + nu:].reshape(self.nobs, self.dim))
+            self._eng.set_inputs(xpm)
+            self._xpm, self.x = xpm, xpm.T
         return self
 
     initialise_target = GPE.initialise_target
     update_target = GPE.update_target
 
-    def update_target_and_dtarget(self, noise=True, domean=True, kern=True, inducing=False):
-        return GPE.update_target_and_dtarget(self, noise=noise, domean=domean, kern=kern, inducing=inducing)
+    def update_target_and_dtarget(self, noise=True, domean=True, kern=True, inducing=False, inputs=False):
+        return GPE.update_target_and_dtarget(self, noise=noise, domean=domean, kern=kern, inducing=inducing, inputs=inputs)
 
-    def optimize(self, noise=True, domean=True, kern=True, inducing=False, maxiter=100, **kw):
+    def optimize(self, noise=True, domean=True, kern=True, inducing=False, inputs=False, maxiter=100, **kw):
         """optimize!(gp) as GPE.optimize; inducing=True also moves the inducing points (Snelson & Ghahramani's
-        pseudo-inputs), with the same exception filter: a step that makes K_uu or Sigma_QR singular (two inducing points
-        meeting: PosDefException) is rejected and the parameters, Xu included, are rolled back."""
-        if not inducing:
+        pseudo-inputs) and inputs=True the training inputs, with the same exception filter: a step that makes K_uu,
+        Sigma_QR or an FSA block singular (PosDefException) is rejected and the parameters, Xu and X included, are rolled
+        back.  inputs=True is refused on a distributed model: each rank holds only its own slice of X."""
+        if inputs and self._distributed:
+            raise ValueError("optimize(inputs=True) needs every training input in one parameter vector; a distributed model "
+                             "holds only this rank's slice")
+        if not inducing and not inputs:
             return GPE.optimize(self, noise=noise, domean=domean, kern=kern, maxiter=maxiter, **kw)
         from scipy.optimize import minimize
 
-        flags = dict(noise=noise, domean=domean, kern=kern, inducing=True)
+        flags = dict(noise=noise, domean=domean, kern=kern, inducing=inducing, inputs=inputs)
         best = {"f": None}
 
         def fg(hyp):

@@ -531,6 +531,26 @@ function dmll_inducing(gp::GPE{X,Y,M,K,CS,D,P}) where {X,Y,M,K,CS<:B200SparseStr
     return g
 end
 
+# Training inputs as parameters of the sparse strategies (not in the reference).  set_inputs! moves gp.x in place (same
+# size; FSA keeps its blocks by index) and on the device, then refreshes the target; dmll_inputs returns dmll/dX (dim x N)
+# of the last update_target!: the device part from one sweep of the kernel-gradient adjoints (W_fu, FITC's g, the FSA
+# blocks' G_b) plus alpha_i dm(x_i)/dx_i through the reference's own mean on Duals, as for the dense strategies.
+function set_inputs!(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix) where {X,Y,M,K,CS<:B200SparseStrategy,D,P}
+    size(x) == size(gp.x) || throw(ArgumentError("set_inputs!: x must keep the size $(size(gp.x))"))
+    gp.x .= x
+    Xm = Matrix{Float64}(gp.x)
+    checks(gp.cK, ccall((:gpb200_fitc_set_inputs, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64),
+                        gp.cK.handle, size(Xm, 2), Xm, size(Xm, 1)), "fitc_set_inputs")
+    update_target!(gp)
+    return gp
+end
+function dmll_inputs(gp::GPE{X,Y,M,K,CS,D,P}) where {X,Y,M,K,CS<:B200SparseStrategy,D,P}
+    g = Matrix{Float64}(undef, gp.dim, gp.nobs)
+    checks(gp.cK, ccall((:gpb200_fitc_grad_kernel_inputs, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                        gp.cK.handle, C_NULL, C_NULL, g), "fitc_grad_kernel_inputs")
+    return g .+ mean_dx(gp.mean, gp.x) .* reshape(gp.alpha, 1, :)
+end
+
 function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=false) where {X,Y,M,K,CS<:B200Sparse,D,P}
     size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
     Xs = Matrix{Float64}(x); Ms = size(Xs, 2)
@@ -861,6 +881,6 @@ function predict_y(gp::B200GPA, x::AbstractMatrix; full_cov::Bool=false)        
     return predict_obs(gp.lik, μ, σ2)
 end
 
-export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA, set_inducing!, dmll_inducing, dmll_inputs
+export B200Covariance, B200Sparse, B200FSA, B200ElasticGPE, B200GPA, set_inducing!, dmll_inducing, dmll_inputs, set_inputs!
 
 end # module

@@ -308,6 +308,10 @@ int  gpb200_row_reductions(gpb200_handle* h, int which, const int64_t* args, int
  *   which 11 crossgram_dx  : xs, z, xb, d, M, u, Wb (0 = none), S1, S2, ldw, mask, alpha, E, lde, dmu, dvar (0: dmu only)
  *                            | items (row, out, b0, nb)                                 fargs = theta
  *                            (fsa_crossgram_dx, csrc/fsa.cuh: one CTA per item; xs, z, xb of leading dimension d)
+ *   which 12 block_dx      : xb, d, map (0 = none), out, accumulate | items (G, row0, B, n, tile)   fargs = theta
+ *                            out[row(i), :] (+)= sum_{l < n} (G[i B + l] + G[l B + i]) dk(x_i, x_l)/dx_i for the real rows
+ *                            i = 128 tile .. min(n, 128 tile + 128) - 1 of each item, x_i = xb row row0 + i (leading
+ *                            dimension d), row(i) = map[row0 + i] or row0 + i; out point-major (fsa_block_dx, csrc/fsa.cuh)
  * GPB200_EINVAL, nothing launched: bad which / n / nf, theta not of n_theta entries, a program dimension >= d, a null
  * pointer the kernel dereferences, a negative size or row, a bad mode, an item ld < 128, lda < K, ld < ncols.
  * GPB200_ESTATE: a kernel-program call before gpb200_set_kernel.                                                    */
@@ -359,6 +363,11 @@ int  gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32
  *   which 14 inducing_dx: u, ldu, M, z, ldz, n, d, W, ldw, sym, mask (0 = none), out, accumulate   fargs = theta
  *                         out[j, :] (+)= sum_{i < n, mask[i] != 0} W(i, j) dk(u_j, z_i)/du_j, W(i, j) = W[i ldw + j]
  *                         (+ W[j ldw + i] when sym = 1, which needs n = M); out is M x d point-major
+ *   which 15 rows_dx    : x, ldx, n, u, ldu, M, d, W, ldw, c (0 = none), mask (0 = none), map (0 = none), out, accumulate
+ *                         fargs = theta
+ *                         out[row(i), :] (+)= sum_{j < M} W[i ldw + j] dk(x_i, u_j)/dx_i + 2 c_i dk(x_i, x')/dx_i at x' = x_i
+ *                         over the rows i < n with mask[i] != 0 (the others are not written), row(i) = map[i] or i; out
+ *                         point-major (rows_dx_launch, csrc/gram.cuh)
  * GPB200_EINVAL, nothing launched: as gpb200_fsa_kernels, plus j outside [0, n_theta) and ldx < d.                   */
 int  gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
 
@@ -434,6 +443,28 @@ int  gpb200_fitc_grad_kernel_inducing(gpb200_fitc* f, double* dmll_kernel, doubl
  * bitwise those of a fresh handle given the same xu to gpb200_fitc_set_data (and the same gpb200_fitc_set_blocks).
  * With several ranks every rank passes the same xu.                                                                   */
 int  gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_t ldxu);
+/* Gradient of the mll with respect to the training inputs (not in the reference; latent-input and input-warping models),
+ * all four modes.  One sweep gives dmll_x[N x d], point-major (Julia's d x N column-major; on several ranks the rank's own
+ * rows), and optionally dmll_kernel[n_theta] and dmll_xu[M x d] (either may be NULL; when given, bitwise equal to those of
+ * gpb200_fitc_grad_kernel and gpb200_fitc_grad_kernel_inducing: the same launches).  With W_fu, g and G_b the adjoints of
+ * the mll with respect to K_fu, the FITC diagonal K_ii and the FSA blocks K_bb that the kernel gradient builds, and d1k the
+ * derivative of k in its first argument:
+ *   FITC:      dmll/dx_i = 1/2 [ sum_j W_fu[i, j] d1k(x_i, u_j) + 2 g_i d1k(x_i, x_i) ]
+ *   DTC, SoR:  dmll/dx_i = 1/2   sum_j W_fu[i, j] d1k(x_i, u_j)
+ *   FSA:       dmll/dx_i = 1/2 [ sum_j W_fu[i, j] d1k(x_i, u_j) + sum_{l in b(i)} (G_b[i, l] + G_b[l, i]) d1k(x_i, x_l) ]
+ * The mean's part alpha_i dm(x_i)/dx_i is left to the caller.  It adds one row-contraction launch per staging chunk (FSA:
+ * two, the block contraction and the row contraction); these read the adjoints and write nothing else, and nothing is
+ * exchanged between ranks for X.  Sums are in a fixed order: repeated calls are bitwise equal.  Device memory grows by
+ * N d doubles on the first call.  GPB200_ESTATE before factorize + mll; GPB200_EINVAL for a NULL dmll_x.
+ * gpb200_fitc_get_timings slots 9-10 hold the last call's device times: the X contractions summed, the whole call.   */
+int  gpb200_fitc_grad_kernel_inputs(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double* dmll_x);
+/* Replaces the training inputs (x: d x N column-major, ld = ldx) in place (not in the reference).  N must be
+ * gpb200_fitc_set_data's and ldx >= d (GPB200_EINVAL otherwise); GPB200_ESTATE before set_data.  FSA keeps its blocks (by
+ * index), their work lists and every workspace, and rebuilds its reordered copy of the inputs.  The factorisation, alpha
+ * and the cross-validation state are cleared.  After factorize + mll, alpha, mll and logdet are bitwise those of a fresh
+ * handle given the same x to gpb200_fitc_set_data (and the same gpb200_fitc_set_blocks).  With several ranks every rank
+ * passes its own slice.  No kernel is launched.                                                                        */
+int  gpb200_fitc_set_inputs(gpb200_fitc* f, int64_t N, const double* x, int64_t ldx);
 /* mu_minus_mean[Ms], var[Ms] (may be NULL; not clamped) */
 int  gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean, double* var);
 /* Predictive gradients of FITC / DTC / SoR with respect to the test inputs, as gpb200_predict_grad (same layouts, var and
@@ -507,7 +538,8 @@ int  gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs
 /* device times (ms) of the last successful gpb200_fitc_rand: [0] Sigma* build (with mu), [1] make_posdef! + Cholesky,
  * [2] unwhiten! GEMM + mu; of the last gpb200_fitc_predict_fsa_grad, summed over its test chunks: [3] predict_fsa's
  * launches, [4] s = R L_s^-1 and the second block sweep, [5] the K_uu^-1 TRSMs, [6] the contraction; of the last
- * gpb200_fitc_grad_kernel_inducing: [7] its dmll/dXu contractions summed, [8] the whole call (CUDA events; n <= 9 entries
+ * gpb200_fitc_grad_kernel_inducing: [7] its dmll/dXu contractions summed, [8] the whole call; of the last
+ * gpb200_fitc_grad_kernel_inputs: [9] its dmll/dX contractions summed, [10] the whole call (CUDA events; n <= 11 entries
  * are written)                                                                                                          */
 int  gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n);
 /* ---- cross-validation on the sparse engine (src/crossvalidation.jl with cK a FITC / DTC / SoR covariance) ---------------
