@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../../include/gpb200.h"
+#include "devbuf.cuh"
 #include "gemm_nt.cuh"
 #include "kprog.cuh"
 
@@ -30,19 +31,21 @@ struct gpb200_handle {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr, ev5 = nullptr;
     int64_t N = 0, Npad = 0, ld = 0;
     int d = 0;
-    double* x = nullptr;
+    DevBuf<double> x;
     KProg prog{};
     std::vector<double> theta;
     bool has_data = false, has_kernel = false, factored = false, inv_ready = false, alpha_ready = false;
     bool s_ready = false;                      // G's lower triangle holds -S of gpb200_gpa_grad (A = S for gpb200_grad_inputs)
-    double *F = nullptr, *G = nullptr, *Dinv = nullptr, *DinvT = nullptr, *logd = nullptr;
-    double *noise_var = nullptr, *r0 = nullptr, *r1 = nullptr, *y1 = nullptr, *alpha = nullptr, *scal = nullptr;
-    double *part = nullptr, *trace_out = nullptr;
-    double* tblk = nullptr;                    // Npad scratch vector (block right-hand sides of the sharded solves)
-    double* ZdT = nullptr;                     // gpb200_gpa_grad: Npad x 128 clean upper diagonal tiles of Z' (allocated on first use)
+    double *F = nullptr, *G = nullptr;         // Frep / Grep (replicated) or the VMM ranges vmF / vmG (row-sharded)
+    DevBuf<double> Frep, Grep;
+    DevBuf<double> Dinv, DinvT, logd;
+    DevBuf<double> noise_var, r0, r1, y1, alpha, scal;
+    DevBuf<double> part, trace_out;
+    DevBuf<double> tblk;                       // Npad scratch vector (block right-hand sides of the sharded solves)
+    DevBuf<double> ZdT;                        // gpb200_gpa_grad: Npad x 128 clean upper diagonal tiles of Z' (allocated on first use)
     CUtensorMap mapZdT{};
     // TMA-staged SEIso kernels (gram_fast.cu): inputs stored [Npad x dxp] with an even, zero-padded dxp <= 8
-    double *xp = nullptr, *xpt = nullptr;      // [Npad x dxp] and its transpose [dxp x Npad]
+    DevBuf<double> xp, xpt;                    // [Npad x dxp] and its transpose [dxp x Npad]
     int dxp = 0;
     CUtensorMap mapX{}, mapXT{};
     bool xmap_ok = false;
@@ -51,17 +54,17 @@ struct gpb200_handle {
     // cross-validation (gpb200_cv_*): K_y^-1 mirrored to a full symmetric matrix in G; two N x N temporaries
     bool g_sym = false;
     bool cv_m_ok = false;                                       // cvD holds M_j = Z_j K^-1 of the last cv_param call
-    double *cvD = nullptr, *cvY = nullptr;
+    DevBuf<double> cvD, cvY;
     CUtensorMap mapCvD{}, mapCvY{};
-    double* cvblk = nullptr; long long* cvidx = nullptr; int64_t cvblk_cap = 0, cvidx_cap = 0;   // capacities in elements
+    DevBuf<double> cvblk; DevBuf<long long> cvidx;   // principal sub-blocks of gpb200_cv_block (grown on demand)
     // posterior sampling (gpb200_rand): M x M sub-engine for chol(Sigma* + nugget I), normal draws / samples staging
     gpb200_handle* sub = nullptr;
     bool cov_keep_device = false;              // predict: leave the full covariance in Kss (no D2H)
-    double *rz = nullptr, *rout = nullptr;
+    DevBuf<double> rz, rout;                   // rz_rows x rz_cols each
     int64_t rz_rows = 0, rz_cols = 0;
     CUtensorMap mapRz{};
-    int* info_dev = nullptr;
-    int* flags = nullptr;                      // ready-flags of the single-launch triangular solves (2 x (Npad/128 + 1))
+    DevBuf<int> info_dev;
+    DevBuf<int> flags;                         // ready-flags of the single-launch triangular solves (2 x (Npad/128 + 1))
     int trsv_fused = 1;
     int max_resident_ctas = 0;
     int64_t n_noise = 1;
@@ -69,12 +72,11 @@ struct gpb200_handle {
     CUtensorMap mapF{}, mapG{}, mapDinv{}, mapDinvT{};
     bool tma_ok = false;
     // predict workspace
-    double *xs = nullptr, *Kst = nullptr, *Kss = nullptr, *pmu = nullptr, *pvar = nullptr, *pkdiag = nullptr;
-    int64_t xs_cap = 0, Kst_rows = 0, Kss_rows = 0;
-    double* pdx = nullptr; int64_t pdx_rows = 0;   // gpb200_predict_grad: dmu (Mpad x d), then dvar (Mpad x d)
+    DevBuf<double> xs, Kst, Kss, pmu, pvar, pkdiag;   // grown on demand
+    DevBuf<double> pdx;                        // gpb200_predict_grad: dmu (Mpad x d), then dvar (Mpad x d)
     // gpb200_grad_inputs (first use, freed with the data): a caller's alpha (Npad), the N x d result (Npad x d), and in an
     // in-process group the gathered ranks' results (nranks x Npad x d)
-    double* dxin = nullptr;
+    DevBuf<double> dxin;
     CUtensorMap mapKst{};
     // options
     int nb = 0;                 // outer Cholesky block; 0 = fully recursive (one panel)
@@ -98,21 +100,19 @@ struct gpb200_handle {
     ncclComm_t comm = nullptr;
     cudaStream_t st_comm = nullptr;
     int dist_nb = 0;                           // width of an owned block column; 0 = auto (~Npad/(8*nranks))
-    double* pack[2] = {nullptr, nullptr};      // panel staging (double buffered)
-    size_t pack_elems = 0;
+    DevBuf<double> pack[2];                    // panel staging (double buffered)
     cudaEvent_t ev_packed[2] = {nullptr, nullptr}, ev_bcast[2] = {nullptr, nullptr}, ev_unpacked[2] = {nullptr, nullptr};
     cudaEvent_t ev_x = nullptr, ev_y = nullptr;
-    double *ag_send = nullptr, *ag_recv = nullptr;
-    size_t ag_send_elems = 0, ag_recv_elems = 0;
+    DevBuf<double> ag_send, ag_recv;
     // fused panel broadcast over NVLink peer memory (CUDA IPC): peers' F / Dinv / DinvT / logd / signal words
     bool p2p = false;
     int n_peer = 0;
     int peer_rank[7] = {0, 0, 0, 0, 0, 0, 0};
     double *peer_F[7] = {}, *peer_Dinv[7] = {}, *peer_DinvT[7] = {}, *peer_logd[7] = {};
     int* peer_sig[7] = {};
-    int* sig = nullptr;                        // sig[q] = last panel published by rank q (epoch * 65536 + b + 1); sig[8] = watchdog
+    DevBuf<int> sig;                           // sig[q] = last panel published by rank q (epoch * 65536 + b + 1); sig[8] = watchdog
     int epoch = 0;
-    int** peer_sig_dev = nullptr;              // device array: &peer_sig[q][rank]
+    DevBuf<int*> peer_sig_dev;                 // device array: &peer_sig[q][rank]
     bool push_panel = false;                   // set while the owner factors a panel: leaf + leaf TRSM also store to the peers
     // ---- row-sharded storage (shard_impl.cuh): F / G are virtual address ranges, physical pages exist for owned rows only ----
     int shard_opt = -1;                        // option "shard": -1 auto (when replicated F+G would not fit), 0 never, 1 always
@@ -123,15 +123,15 @@ struct gpb200_handle {
     VmBuf vmF, vmG;
     VmBuf vmCvY, vmCvM;                        // cross-validation work matrices (Y' = K^-1 dK_j, lower triangle of M_j), own rows only
     CUtensorMap mapShCvY{}, mapShCvM{};
-    double* P[4] = {nullptr, nullptr, nullptr, nullptr};   // panel buffers, Npad x NBp (global row order); P[1], P[3] double as NBp x Npad row panels
-    double* Sbuf = nullptr;                    // all-gather staging: nranks regions of S_per_rank doubles; scratch of the inverse sweep
+    DevBuf<double> P[4];                                   // panel buffers, Npad x NBp (global row order); P[1], P[3] double as NBp x Npad row panels
+    DevBuf<double> Sbuf;                       // all-gather staging: nranks regions of S_per_rank doubles; scratch of the inverse sweep
     size_t S_per_rank = 0;
     CUtensorMap mapP[4] = {}, mapXR[2] = {}, mapS{};
-    double* XRbig[2] = {nullptr, nullptr};     // row-panel forms X_J of a BATCH of panels (inverse sweep: batched LAUUM part)
+    DevBuf<double> XRbig[2];                   // row-panel forms X_J of a BATCH of panels (inverse sweep: batched LAUUM part)
     int xr_batch = 1;                          // panels per batch
     CUtensorMap mapXRbig[2] = {};
-    double* red = nullptr;                     // small reduction scratch (local group all-reduce)
-    int* redi = nullptr;
+    DevBuf<double> red;                        // small reduction scratch (local group all-reduce)
+    DevBuf<int> redi;
     struct gpb200_group* grp = nullptr;        // in-process group of virtual ranks on one device (gpb200_group_create)
     std::vector<cudaEvent_t> evring;
     size_t evring_next = 0;
@@ -146,24 +146,50 @@ struct gpb200_group {
 
 
 // ---- FITC (sparse/fully_indep_train_conditional.jl): two dense M x M sub-engines + N-chunk streaming ----
+// The sparse handle's device buffers, grouped by lifetime; assigning {} to a group frees it.
+struct FitcData {                    // the observations: N (+ 128 padding) and Mpad vectors
+    DevBuf<double> x, lam, y, alpha, tmpn;
+    DevBuf<double> bvec, uvec, tmpm, rhsm, scal;
+};
+struct FitcStage {                   // one staging chunk of Nc rows (fitc_stage_alloc)
+    DevBuf<double> xs, w, tmpc, zeroc, tmpc2;
+    DevBuf<double> bufA, bufB;       // Nc x Mpad (K_fu chunk) ; Mpad x Nc (K_uf chunk)
+    CUtensorMap mapA{}, mapB{}, mapB2{};
+};
+struct FitcGradWs {                  // kernel-gradient workspace; sized by N, Nc and Mpad
+    DevBuf<double> bufC, Hbuf, Wbuf, Tbuf, gvec, betav, gpart, gacc, gtmp;
+    CUtensorMap mapAt{}, mapC{}, mapCt{}, mapH{}, mapT{};
+    bool ready = false;
+};
+// cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block), apart from every buffer the likelihood,
+// gradient and prediction schedules keep; sized by N, Nc and Mpad:
+//   G Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  Gt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
+//   Ch Nc x Mpad: Ch = L^-1 K_fu S^-1;  P Nc x Mpad: Ch Q (pass 2) or E (fold blocks)
+//   Mpad x Mpad: Duu = dK_uu, Dp = dK_uu K_uu^-1, R = K_uf L^-1 G, H = K_uf L^-1 Delta L^-1 K_fu, Q = H - R - R'
+struct FitcCvWs {
+    DevBuf<double> G, Gt, Ch, P;
+    DevBuf<double> Duu, Dp, R, H, Q;
+    DevBuf<double> alpha, del, ilam, za, dg;         // N + Nc
+    DevBuf<double> da, q, lamV, delV, xs;            // Nc (xs: Nc x d)
+    DevBuf<double> m;                                // 8 x Mpad: K_uf alpha, G' alpha, K_uf L^-1 Delta alpha, beta, R beta, w, tmp
+    DevBuf<double> out;                              // fold block (padded nV x padded nV), grown on demand
+    DevBuf<long long> idx;
+    CUtensorMap mapG{}, mapGt{}, mapCh{}, mapP{}, mapDuu{}, mapDp{}, mapQ{};
+    bool ready = false;
+    bool m_ok = false;                               // Dp / Q / del hold the state of the last cv_param since factorize
+};
+
 struct gpb200_fitc {
     gpb200_handle* eu = nullptr;     // K_uu  (+1e-10 I)            -> L_uu
     gpb200_handle* es = nullptr;     // Sigma_QR = K_uf L^-1 K_fu + K_uu (+1e-10 I) -> L_s
     int device = 0;
     int64_t N = 0, M = 0, Mpad = 0, Nc = 0;
     int d = 0;
-    double *x = nullptr, *xs = nullptr, *lam = nullptr, *y = nullptr, *alpha = nullptr, *tmpn = nullptr;
-    double *w = nullptr, *tmpc = nullptr, *zeroc = nullptr, *tmpc2 = nullptr;          // Nc
-    double *bvec = nullptr, *uvec = nullptr, *tmpm = nullptr, *rhsm = nullptr, *scal = nullptr;   // Mpad
-    double *bufA = nullptr, *bufB = nullptr;   // Nc x Mpad (K_fu chunk) ; Mpad x Nc (K_uf chunk)
-    CUtensorMap mapA{}, mapB{}, mapB2{};
-    // kernel-gradient workspace (allocated on first use)
-    double *bufC = nullptr, *Hbuf = nullptr, *Wbuf = nullptr, *Tbuf = nullptr, *gvec = nullptr, *betav = nullptr;
-    double *gpart = nullptr, *gacc = nullptr, *gtmp = nullptr;
-    CUtensorMap mapAt{}, mapC{}, mapCt{}, mapH{}, mapT{};
-    bool grad_ws = false;
-    double* Kss = nullptr; int64_t Kss_rows = 0;      // full predictive covariance (gpb200_fitc_predict_cov)
-    double* pdx = nullptr;                            // gpb200_fitc_predict_grad: dmu, dvar of a chunk (2 x Nc x d; first use)
+    FitcData data;                   // per data set
+    FitcStage stage;                 // per staging chunk
+    FitcGradWs grad;                 // kernel-gradient workspace (first use)
+    DevBuf<double> Kss;                               // full predictive covariance (gpb200_fitc_predict_cov)
+    DevBuf<double> pdx;                               // gpb200_fitc_predict_grad: dmu, dvar of a chunk (2 x Nc x d; first use)
     // posterior sampling (gpb200_fitc_rand): the Ms x Ms sub-engine and the staging of the draws are eu's (rand_from_cov)
     bool cov_keep_device = false;                     // predict_fsa: leave Sigma* in caller order on the device (fsa->Sc)
     double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
@@ -172,29 +198,15 @@ struct gpb200_fitc {
     // inducing-point gradient (gpb200_fitc_grad_kernel_inducing; first use): dmll/dXu accumulator (M x d), the events
     // around the call (0, 1) and around each contraction launch (2k, 2k + 1 for k >= 1), and the device times of the last
     // call: the contractions summed, the whole call
-    double* dxu = nullptr;
+    DevBuf<double> dxu;
     std::vector<cudaEvent_t> xu_ev;
     double xu_ms[2] = {0, 0};
     // training-input gradient (gpb200_fitc_grad_kernel_inputs; first use): dmll/dX accumulator (N x d, this rank's rows in
     // the caller's order), the events around the call and its contractions (as xu_ev) and the device times of the last call
-    double* dx = nullptr;
+    DevBuf<double> dx;
     std::vector<cudaEvent_t> x_ev;
     double x_ms[2] = {0, 0};
-    // cross-validation (gpb200_fitc_get_inverse_diag / _cv_param / _cv_block; allocated on first use, apart from every
-    // buffer the likelihood, gradient and prediction schedules keep):
-    //   cvG Nc x Mpad: G = dK_fu - 1/2 K_fu Dp of a chunk;  cvGt Mpad x Nc: G' (pass 1), then the Delta-scaled K_uf L^-1;
-    //   cvCh Nc x Mpad: Ch = L^-1 K_fu S^-1;  cvP Nc x Mpad: Ch Q (pass 2) or E (fold blocks)
-    //   Mpad x Mpad: cvDuu = dK_uu, cvDp = dK_uu K_uu^-1, cvR = K_uf L^-1 G, cvH = K_uf L^-1 Delta L^-1 K_fu, cvQ = H - R - R'
-    double *cvG = nullptr, *cvGt = nullptr, *cvCh = nullptr, *cvP = nullptr;
-    double *cvDuu = nullptr, *cvDp = nullptr, *cvR = nullptr, *cvH = nullptr, *cvQ = nullptr;
-    double *cvalpha = nullptr, *cvdel = nullptr, *cvilam = nullptr, *cvza = nullptr, *cvdg = nullptr;   // N + Nc
-    double *cvda = nullptr, *cvq = nullptr, *cvlamV = nullptr, *cvdelV = nullptr, *cvxs = nullptr;     // Nc (cvxs: Nc x d)
-    double* cvm = nullptr;                            // 8 x Mpad: K_uf alpha, G' alpha, K_uf L^-1 Delta alpha, beta, R beta, w, tmp
-    double* cvout = nullptr; int64_t cvout_rows = 0;  // fold block (padded nV x padded nV)
-    long long* cvidx = nullptr;
-    CUtensorMap mapCvG{}, mapCvGt{}, mapCvCh{}, mapCvP{}, mapCvDuu{}, mapCvDp{}, mapCvQ{};
-    bool cv_ws = false;
-    bool cv_m_ok = false;                             // cvDp / cvQ / cvdel hold the state of the last cv_param since factorize
+    FitcCvWs cv;                     // cross-validation workspace (first use)
     int cv_param = 0;
     // multi-GPU (gpb200_fitc_comm_init): the N observations are sharded over the ranks, every M x M object is replicated;
     // exchanged: one all-reduce of the M x M accumulator Sigma_QR (and of H for the kernel gradient), M-vectors, scalars
@@ -263,6 +275,14 @@ inline int rank_failed(gpb200_handle* q, int rc) {
 #define FCK(call)      TRY(cuda_rc(f->err, (call), #call, __FILE__, __LINE__))
 #define FCKN(call)     TRY(nccl_rc(f->err, (call), #call, __FILE__, __LINE__))
 
+// all-or-nothing workspace: make() allocates the buffers of `group`; if any step fails, the whole group is freed
+template <class Group, class Make>
+int make_group(Group& group, Make make) {
+    const int rc = make();
+    if (rc != GPB200_OK) group = {};
+    return rc;
+}
+
 inline int fail(gpb200_handle* h, int code, const char* msg) {
     if (h) h->err = msg;
     return code;
@@ -277,10 +297,14 @@ inline int fail(gpb200_fitc* f, int code, const std::string& msg) {
         if (rc_ != GPB200_OK) { f->err = std::string(#call) + ": " + (who)->err; return rc_; }     \
     } while (0)
 
-inline GemmBuf bufF(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapF : nullptr, h->F, h->ld}; }
-inline GemmBuf bufG(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapG : nullptr, h->G, h->ld}; }
-inline GemmBuf bufDinv(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapDinv : nullptr, h->Dinv, TILE}; }
-inline GemmBuf bufDinvT(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapDinvT : nullptr, h->DinvT, TILE}; }
+// a GEMM operand: buffer p with leading dimension ld, read through its tensor map when h's GEMM runs on TMA descriptors
+inline GemmBuf gbuf(const gpb200_handle* h, const double* p, const CUtensorMap& map, int64_t ld) {
+    return GemmBuf{h->tma_ok ? &map : nullptr, p, ld};
+}
+inline GemmBuf bufF(gpb200_handle* h) { return gbuf(h, h->F, h->mapF, h->ld); }
+inline GemmBuf bufG(gpb200_handle* h) { return gbuf(h, h->G, h->mapG, h->ld); }
+inline GemmBuf bufDinv(gpb200_handle* h) { return gbuf(h, h->Dinv, h->mapDinv, TILE); }
+inline GemmBuf bufDinvT(gpb200_handle* h) { return gbuf(h, h->DinvT, h->mapDinvT, TILE); }
 inline GemmBuf bufNone() { return GemmBuf{nullptr, nullptr, 0}; }
 
 // ---- dense engine (gpb200.cu) -------------------------------------------------------------------------------------
@@ -310,6 +334,7 @@ size_t fsa_num_chunks(const gpb200_fitc* f);
 const double* fsa_cov(const gpb200_fitc* f);
 
 // ---- FITC (fitc_engine.cu), shared with the FSA schedule --------------------------------------------------------------
+int fitc_stage_alloc(gpb200_fitc* f, int64_t nc, const char* who);
 cudaError_t fitc_kfu(gpb200_fitc* f, const double* xrows, int64_t nc);
 cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc);
 int xu_contract(gpb200_fitc* f, size_t k, const double* z, int64_t n, const double* W, int sym, const double* mask,

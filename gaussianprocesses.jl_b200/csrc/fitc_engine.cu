@@ -23,27 +23,12 @@ static int fitc_allreduce(gpb200_fitc* f, double* v, size_t n) {
     return GPB200_OK;
 }
 
-// cross-validation workspace (gpb200_fitc_cv_*): it depends on N, Nc and Mpad only
-static void fitc_cv_free(gpb200_fitc* f) {
-    double** ptrs[] = {&f->cvG, &f->cvGt, &f->cvCh, &f->cvP, &f->cvDuu, &f->cvDp, &f->cvR, &f->cvH, &f->cvQ, &f->cvalpha,
-                       &f->cvdel, &f->cvilam, &f->cvza, &f->cvdg, &f->cvda, &f->cvq, &f->cvlamV, &f->cvdelV, &f->cvxs,
-                       &f->cvm, &f->cvout};
-    for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
-    if (f->cvidx) cudaFree(f->cvidx);
-    f->cvidx = nullptr; f->cvout_rows = 0;
-    f->cv_ws = f->cv_m_ok = false;
-}
-
 // every buffer that depends on the observations or the inducing points; the FSA blocks refer to the old observations too
 static void fitc_free_data(gpb200_fitc* f) {
-    double** ptrs[] = {&f->x, &f->xs, &f->lam, &f->y, &f->alpha, &f->tmpn, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2,
-                       &f->bvec, &f->uvec, &f->tmpm, &f->rhsm, &f->scal, &f->bufA, &f->bufB,
-                       &f->bufC, &f->Hbuf, &f->Wbuf, &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx,
-                       &f->dxu, &f->dx};
-    for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
-    f->grad_ws = false;
+    f->data = {}; f->stage = {}; f->grad = {};
+    f->pdx.reset(); f->dxu.reset(); f->dx.reset();
     fsa_free(f);
-    fitc_cv_free(f);
+    f->cv = {};
 }
 
 int gpb200_fitc_comm_init(gpb200_fitc* f, int nranks, int rank, const char* id128) {
@@ -64,7 +49,7 @@ void gpb200_fitc_destroy(gpb200_fitc* f) {
     cudaSetDevice(f->device);
     if (f->eu && f->eu->st) cudaStreamSynchronize(f->eu->st);
     fitc_free_data(f);
-    if (f->Kss) cudaFree(f->Kss);
+    f->Kss.reset();
     for (cudaEvent_t e : f->xu_ev) cudaEventDestroy(e);
     for (cudaEvent_t e : f->x_ev) cudaEventDestroy(e);
     if (f->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(f->comm);
@@ -99,6 +84,7 @@ int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, 
     FSUB(gpb200_set_data(f->es, M, d, xu, ldxu), f->es);
     cudaStream_t st = f->eu->st;
     fitc_free_data(f);
+    f->has_data = false;
     f->N = N; f->M = M; f->d = d; f->Mpad = f->eu->Npad;
     // chunk of data rows: two staging buffers of ~2 GB each at most
     int64_t nc = (int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE;
@@ -106,23 +92,16 @@ int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, 
     if (nc > 32768) nc = 32768;                       // grid.y limit of the row-scaling kernel
     if (nc > Nceil) nc = Nceil;
     if (nc < TILE) nc = TILE;
-    f->Nc = nc;
-    FCK(cudaMalloc(&f->x, sizeof(double) * N * d));
-    FCK(cudaMalloc(&f->xs, sizeof(double) * nc * d));
-    for (double** p : {&f->lam, &f->y, &f->alpha, &f->tmpn}) FCK(cudaMalloc(p, sizeof(double) * (N + TILE)));
-    for (double** p : {&f->w, &f->tmpc, &f->zeroc, &f->tmpc2}) FCK(cudaMalloc(p, sizeof(double) * nc));
-    for (double** p : {&f->bvec, &f->uvec, &f->tmpm, &f->rhsm}) FCK(cudaMalloc(p, sizeof(double) * f->Mpad));
-    FCK(cudaMalloc(&f->scal, sizeof(double) * 16));
-    FCK(cudaMalloc(&f->bufA, sizeof(double) * nc * f->Mpad));
-    FCK(cudaMalloc(&f->bufB, sizeof(double) * nc * f->Mpad));
-    FCK(cudaMemsetAsync(f->zeroc, 0, sizeof(double) * nc, st));
-    FCK(cudaMemcpy2DAsync(f->x, sizeof(double) * d, x, sizeof(double) * ldx, sizeof(double) * d, N, cudaMemcpyHostToDevice, st));
-    if (f->eu->tma_ok) {
-        const bool ok = gemm_make_tensor_map(&f->mapA, f->bufA, nc, f->Mpad, f->Mpad) &&
-                        gemm_make_tensor_map(&f->mapB, f->bufB, f->Mpad, nc, nc) &&
-                        gemm_make_tensor_map(&f->mapB2, f->bufB, nc, f->Mpad, f->Mpad);
-        if (!ok) return fail(f, GPB200_ECUDA, "fitc_set_data: cuTensorMapEncodeTiled failed");
-    }
+    TRY(make_group(f->data, [&] {
+        FitcData& g = f->data;
+        FCK(g.x.alloc((size_t)N * d));
+        for (DevBuf<double>* p : {&g.lam, &g.y, &g.alpha, &g.tmpn}) FCK(p->alloc(N + TILE));
+        for (DevBuf<double>* p : {&g.bvec, &g.uvec, &g.tmpm, &g.rhsm}) FCK(p->alloc(f->Mpad));
+        FCK(g.scal.alloc(16));
+        return GPB200_OK;
+    }));
+    TRY(fitc_stage_alloc(f, nc, "fitc_set_data"));
+    FCK(cudaMemcpy2DAsync(f->data.x, sizeof(double) * d, x, sizeof(double) * ldx, sizeof(double) * d, N, cudaMemcpyHostToDevice, st));
     FCK(cudaStreamSynchronize(st));
     f->has_data = true; f->factored = f->alpha_ready = false;
     return GPB200_OK;
@@ -139,13 +118,35 @@ int gpb200_fitc_set_kernel(gpb200_fitc* f, int32_t n_ops, const int32_t* ops, in
 }  // extern "C"
 
 namespace engine __attribute__((visibility("hidden"))) {
+// (re)makes the staging chunk for nc rows, with its tensor maps; the workspaces sized by Nc are freed with the old chunk
+int fitc_stage_alloc(gpb200_fitc* f, int64_t nc, const char* who) {
+    f->grad = {}; f->cv = {}; f->pdx.reset();
+    f->stage = {};
+    f->Nc = nc;
+    return make_group(f->stage, [&] {
+        FitcStage& g = f->stage;
+        FCK(g.xs.alloc((size_t)nc * f->d));
+        for (DevBuf<double>* p : {&g.w, &g.tmpc, &g.zeroc, &g.tmpc2}) FCK(p->alloc(nc));
+        FCK(g.bufA.alloc((size_t)nc * f->Mpad));
+        FCK(g.bufB.alloc((size_t)nc * f->Mpad));
+        FCK(cudaMemsetAsync(g.zeroc, 0, sizeof(double) * nc, f->eu->st));
+        if (f->eu->tma_ok) {
+            const bool ok = gemm_make_tensor_map(&g.mapA, g.bufA, nc, f->Mpad, f->Mpad) &&
+                            gemm_make_tensor_map(&g.mapB, g.bufB, f->Mpad, nc, nc) &&
+                            gemm_make_tensor_map(&g.mapB2, g.bufB, nc, f->Mpad, f->Mpad);
+            if (!ok) return fail(f, GPB200_ECUDA, std::string(who) + ": cuTensorMapEncodeTiled failed");
+        }
+        return GPB200_OK;
+    });
+}
+
 // K_fu chunk (rows r0..r0+nc of x against the inducing points) into bufA [Nc x Mpad]
 cudaError_t fitc_kfu(gpb200_fitc* f, const double* xrows, int64_t nc) {
-    return crossgram_launch(f->eu->prog, xrows, f->d, nc, f->Nc, f->eu->x, f->d, f->M, f->Mpad, f->d, f->bufA, f->Mpad, f->eu->st, &f->eu->launches);
+    return crossgram_launch(f->eu->prog, xrows, f->d, nc, f->Nc, f->eu->x, f->d, f->M, f->Mpad, f->d, f->stage.bufA, f->Mpad, f->eu->st, &f->eu->launches);
 }
 // K_uf chunk into bufB [Mpad x Nc]
 cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc) {
-    return crossgram_launch(f->eu->prog, f->eu->x, f->d, f->M, f->Mpad, xrows, f->d, nc, f->Nc, f->d, f->bufB, f->Nc, f->eu->st, &f->eu->launches);
+    return crossgram_launch(f->eu->prog, f->eu->x, f->d, f->M, f->Mpad, xrows, f->d, nc, f->Nc, f->d, f->stage.bufB, f->Nc, f->eu->st, &f->eu->launches);
 }
 
 // one contraction launch (slot k >= 1 of f->xu_ev) over n rows z against W (ld Mpad) into f->dxu
@@ -202,7 +203,7 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
     if (!isfinite(log_noise)) return fail(f, GPB200_EINVAL, "fitc_factorize: non-finite logNoise");
     if (f->mode == 3) TRY(fsa_check(f, "fitc_factorize"));
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    f->factored = f->alpha_ready = f->cv.m_ok = false;
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     // K_uu + 1e-10 I and its factor (fitc.jl:139-141)
@@ -218,25 +219,25 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
     else FCK(cudaMemsetAsync(es->G, 0, sizeof(double) * (size_t)f->Mpad * (size_t)f->Mpad, st));     // K_uu (+ nuggets, identity padding) enters the sum once
     f->noise_var = exp(2.0 * log_noise);
     if (f->mode == 3) return fsa_factorize(f);
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
-    GemmBuf bB{eu->tma_ok ? &f->mapB : nullptr, f->bufB, f->Nc};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
+    const GemmBuf bB = gbuf(eu, f->stage.bufB, f->stage.mapB, f->Nc);
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
-        const double* xr = f->x + r0 * f->d;
+        const double* xr = f->data.x + r0 * f->d;
         if (f->mode == 0) {
             // Lambda_i = sigma^2 + K_ii - |L_uu^-1 K_ui|^2   (fitc.jl:146-148)
             FCK(fitc_kfu(f, xr, nc));
             FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, nc, f->Mpad, f->tmpc2, st, &eu->launches));
-            FCK(ew_launch(0, nc, f->lam + r0, f->tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
+            FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->stage.tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, nc, f->Mpad, f->stage.tmpc2, st, &eu->launches));
+            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
         } else {
             // SoR / DTC: Lambda = sigma^2 I   (subsetofregressors.jl:100: exp(-2 logNoise) * Kuf * Kfu + Kuu)
-            FCK(ew_launch(0, nc, f->lam + r0, f->zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
+            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
         }
         // Sigma_QR += K_uf Lambda^-1 K_fu   (fitc.jl:150), as (K_uf Lambda^-1/2)(K_uf Lambda^-1/2)'
         FCK(fitc_kuf(f, xr, nc));
-        FCK(scale_launch(0, f->bufB, f->Nc, f->Mpad, nc, f->lam + r0, st, &eu->launches));
+        FCK(scale_launch(0, f->stage.bufB, f->Nc, f->Mpad, nc, f->data.lam + r0, st, &eu->launches));
         FCK(gemm_whole(es, bB, bB, es->G, es->ld, f->Mpad, f->Mpad, f->Nc, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
     }
     // multi-GPU: Sigma_QR = K_uu + sum over ranks of K_uf L^-1 K_fu  -- the one M x M exchange of the FITC likelihood
@@ -255,47 +256,47 @@ int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, d
     FCK(cudaSetDevice(f->device));
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
-    FCK(cudaMemcpyAsync(f->y, y_minus_mean, sizeof(double) * f->N, cudaMemcpyHostToDevice, st));
+    FCK(cudaMemcpyAsync(f->data.y, y_minus_mean, sizeof(double) * f->N, cudaMemcpyHostToDevice, st));
     // b = K_uf Lambda^-1 r
-    FCK(cudaMemsetAsync(f->bvec, 0, sizeof(double) * f->Mpad, st));
+    FCK(cudaMemsetAsync(f->data.bvec, 0, sizeof(double) * f->Mpad, st));
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
-        FCK(fitc_kuf(f, f->x + r0 * f->d, nc));
-        FCK(cudaMemsetAsync(f->w, 0, sizeof(double) * f->Nc, st));
-        FCK(ew_launch(1, nc, f->w, f->y + r0, f->lam + r0, nullptr, 0.0, st, &eu->launches));
-        FCK(rowdot_launch(f->bufB, f->Nc, f->w, f->M, f->Nc, f->tmpm, st, &eu->launches));
-        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(fitc_kuf(f, f->data.x + r0 * f->d, nc));
+        FCK(cudaMemsetAsync(f->stage.w, 0, sizeof(double) * f->Nc, st));
+        FCK(ew_launch(1, nc, f->stage.w, f->data.y + r0, f->data.lam + r0, nullptr, 0.0, st, &eu->launches));
+        FCK(rowdot_launch(f->stage.bufB, f->Nc, f->stage.w, f->M, f->Nc, f->data.tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->data.bvec, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
     }
-    TRY(fitc_allreduce(f, f->bvec, (size_t)f->Mpad));              // b summed over the ranks' rows
+    TRY(fitc_allreduce(f, f->data.bvec, (size_t)f->Mpad));              // b summed over the ranks' rows
     // u = Sigma_QR^-1 b   (== get_alpha_u, fitc.jl:279-286)
-    FCK(cudaMemcpyAsync(f->rhsm, f->bvec, sizeof(double) * f->Mpad, cudaMemcpyDeviceToDevice, st));
-    FCK(solve_device(es, f->rhsm, f->tmpm, f->uvec));
+    FCK(cudaMemcpyAsync(f->data.rhsm, f->data.bvec, sizeof(double) * f->Mpad, cudaMemcpyDeviceToDevice, st));
+    FCK(solve_device(es, f->data.rhsm, f->data.tmpm, f->data.uvec));
     // alpha = Lambda^-1 (r - K_fu u)
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
-        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));
-        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, nc, f->Mpad, f->tmpc, st, &eu->launches));
-        FCK(ew_launch(3, nc, f->alpha + r0, f->y + r0, f->tmpc, f->lam + r0, 0.0, st, &eu->launches));
+        FCK(fitc_kfu(f, f->data.x + r0 * f->d, nc));
+        FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, nc, f->Mpad, f->stage.tmpc, st, &eu->launches));
+        FCK(ew_launch(3, nc, f->data.alpha + r0, f->data.y + r0, f->stage.tmpc, f->data.lam + r0, 0.0, st, &eu->launches));
     }
-    FCK(dot_launch(f->y, f->alpha, f->N, f->scal + 0, st, &eu->launches));
-    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st, &eu->launches));
-    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st, &eu->launches));
-    FCK(ew_launch(4, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));
-    FCK(sum_launch(f->tmpn, f->N, f->scal + 3, st, &eu->launches));
+    FCK(dot_launch(f->data.y, f->data.alpha, f->N, f->data.scal + 0, st, &eu->launches));
+    FCK(sum_launch(es->logd, es->Npad, f->data.scal + 1, st, &eu->launches));
+    FCK(sum_launch(eu->logd, eu->Npad, f->data.scal + 2, st, &eu->launches));
+    FCK(ew_launch(4, f->N, f->data.tmpn, f->data.lam, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(sum_launch(f->data.tmpn, f->N, f->data.scal + 3, st, &eu->launches));
     double s[5];
     if (f->nranks > 1) {
         // r'alpha, sum log Lambda and N are sums over the ranks' rows; the two M x M log-determinants are replicated
         const double nloc = (double)f->N;
-        FCK(cudaMemcpyAsync(f->scal + 8, f->scal + 0, sizeof(double), cudaMemcpyDeviceToDevice, st));
-        FCK(cudaMemcpyAsync(f->scal + 9, f->scal + 3, sizeof(double), cudaMemcpyDeviceToDevice, st));
-        FCK(cudaMemcpyAsync(f->scal + 10, &nloc, sizeof(double), cudaMemcpyHostToDevice, st));
-        TRY(fitc_allreduce(f, f->scal + 8, 3));
-        FCK(cudaMemcpyAsync(f->scal + 0, f->scal + 8, sizeof(double), cudaMemcpyDeviceToDevice, st));
-        FCK(cudaMemcpyAsync(f->scal + 3, f->scal + 9, sizeof(double), cudaMemcpyDeviceToDevice, st));
-        FCK(cudaMemcpyAsync(f->scal + 4, f->scal + 10, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->data.scal + 8, f->data.scal + 0, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->data.scal + 9, f->data.scal + 3, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->data.scal + 10, &nloc, sizeof(double), cudaMemcpyHostToDevice, st));
+        TRY(fitc_allreduce(f, f->data.scal + 8, 3));
+        FCK(cudaMemcpyAsync(f->data.scal + 0, f->data.scal + 8, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->data.scal + 3, f->data.scal + 9, sizeof(double), cudaMemcpyDeviceToDevice, st));
+        FCK(cudaMemcpyAsync(f->data.scal + 4, f->data.scal + 10, sizeof(double), cudaMemcpyDeviceToDevice, st));
     }
-    FCK(cudaMemcpyAsync(s, f->scal, sizeof(double) * 5, cudaMemcpyDeviceToHost, st));
-    if (alpha) FCK(cudaMemcpyAsync(alpha, f->alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(s, f->data.scal, sizeof(double) * 5, cudaMemcpyDeviceToHost, st));
+    if (alpha) FCK(cudaMemcpyAsync(alpha, f->data.alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(es), es);                                   // the solve for u above
     f->Ntotal = f->nranks > 1 ? s[4] : (double)f->N;
@@ -314,21 +315,21 @@ int gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise) {
     FCK(cudaSetDevice(f->device));
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
-        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));
-        FCK(scale_launch(1, f->bufA, f->Mpad, nc, f->Mpad, f->lam + r0, st, &eu->launches));
+        FCK(fitc_kfu(f, f->data.x + r0 * f->d, nc));
+        FCK(scale_launch(1, f->stage.bufA, f->Mpad, nc, f->Mpad, f->data.lam + r0, st, &eu->launches));
         FCK(trsm_rec_buf(es, bA, (int)f->Nc, 0, (int)f->Mpad));
-        FCK(rowvar_launch(f->bufA, f->Mpad, f->zeroc, nc, f->Mpad, f->tmpn + r0, st, &eu->launches));     // = -|row|^2
+        FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.zeroc, nc, f->Mpad, f->data.tmpn + r0, st, &eu->launches));     // = -|row|^2
     }
-    FCK(sum_launch(f->tmpn, f->N, f->scal + 0, st, &eu->launches));
-    FCK(dot_launch(f->alpha, f->alpha, f->N, f->scal + 1, st, &eu->launches));
-    FCK(ew_launch(5, f->N, f->tmpn, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));
-    FCK(sum_launch(f->tmpn, f->N, f->scal + 2, st, &eu->launches));
-    TRY(fitc_allreduce(f, f->scal, 3));                             // sums over the ranks' rows
+    FCK(sum_launch(f->data.tmpn, f->N, f->data.scal + 0, st, &eu->launches));
+    FCK(dot_launch(f->data.alpha, f->data.alpha, f->N, f->data.scal + 1, st, &eu->launches));
+    FCK(ew_launch(5, f->N, f->data.tmpn, f->data.lam, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(sum_launch(f->data.tmpn, f->N, f->data.scal + 2, st, &eu->launches));
+    TRY(fitc_allreduce(f, f->data.scal, 3));                             // sums over the ranks' rows
     double s[3];
-    FCK(cudaMemcpyAsync(s, f->scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(s, f->data.scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     *dmll_noise = f->noise_var * (s[1] - s[2] - s[0]);
     return GPB200_OK;
@@ -343,27 +344,27 @@ int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ld
     FCK(cudaSetDevice(f->device));
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
-    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
+    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, f->Mpad);
     for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
         const int64_t mc = std::min(f->Nc, Ms - m0);
-        FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * f->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * f->d,
+        FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * f->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * f->d,
                               mc, cudaMemcpyHostToDevice, st));
-        FCK(fitc_kfu(f, f->xs, mc));
-        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st, &eu->launches));
-        FCK(cudaMemcpyAsync(mu + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        FCK(fitc_kfu(f, f->stage.xs, mc));
+        FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, mc, f->Mpad, f->stage.tmpc, st, &eu->launches));
+        FCK(cudaMemcpyAsync(mu + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
         if (var) {
-            FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+            FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
             FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
             FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(kdiag_launch(eu->prog, f->xs, f->d, mc, f->tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st, &eu->launches));       // k_xx - q
-            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st, &eu->launches));          // -s
+            FCK(kdiag_launch(eu->prog, f->stage.xs, f->d, mc, f->stage.tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, mc, f->Mpad, f->stage.tmpc2, st, &eu->launches));       // k_xx - q
+            FCK(rowvar_launch(f->stage.bufB, f->Mpad, f->stage.zeroc, mc, f->Mpad, f->stage.w, st, &eu->launches));          // -s
             if (f->mode == 2) {                                                             // SoR: K_xu S^-1 K_ux only (sor.jl:302-321)
-                FCK(cudaMemsetAsync(f->tmpc2, 0, sizeof(double) * mc, st));
+                FCK(cudaMemsetAsync(f->stage.tmpc2, 0, sizeof(double) * mc, st));
             }
-            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st, &eu->launches));               // [k_xx - q] + s
-            FCK(cudaMemcpyAsync(var + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+            FCK(ew_launch(6, mc, f->stage.tmpc, f->stage.tmpc2, f->stage.w, nullptr, 0.0, st, &eu->launches));               // [k_xx - q] + s
+            FCK(cudaMemcpyAsync(var + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
         }
         FCK(cudaStreamSynchronize(st));
     }
@@ -388,37 +389,37 @@ int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int d = f->d;
-    if (!f->pdx) FCK(cudaMalloc(&f->pdx, sizeof(double) * 2 * f->Nc * d));
+    FCK(f->pdx.ensure((size_t)2 * f->Nc * d));
     double* ddmu = f->pdx;
     double* ddvar = f->pdx + f->Nc * d;
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
-    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
+    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, f->Mpad);
     if (var) {
         FCK(mirror_lower_tiles_launch(eu->F, eu->ld, eu->Npad, st, &eu->launches));
         FCK(mirror_lower_tiles_launch(es->F, es->ld, es->Npad, st, &eu->launches));
     }
     for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
         const int64_t mc = std::min(f->Nc, Ms - m0);
-        FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d,
+        FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d,
                               mc, cudaMemcpyHostToDevice, st));
-        FCK(fitc_kfu(f, f->xs, mc));
-        FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, mc, f->Mpad, f->tmpc, st, &eu->launches));
-        FCK(cudaMemcpyAsync(mu + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        FCK(fitc_kfu(f, f->stage.xs, mc));
+        FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, mc, f->Mpad, f->stage.tmpc, st, &eu->launches));
+        FCK(cudaMemcpyAsync(mu + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
         if (var) {                                                          // as gpb200_fitc_predict
-            FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+            FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
             FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
             FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(kdiag_launch(eu->prog, f->xs, d, mc, f->tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->bufA, f->Mpad, f->tmpc, mc, f->Mpad, f->tmpc2, st, &eu->launches));
-            FCK(rowvar_launch(f->bufB, f->Mpad, f->zeroc, mc, f->Mpad, f->w, st, &eu->launches));
-            if (f->mode == 2) FCK(cudaMemsetAsync(f->tmpc2, 0, sizeof(double) * mc, st));
-            FCK(ew_launch(6, mc, f->tmpc, f->tmpc2, f->w, nullptr, 0.0, st, &eu->launches));
-            FCK(cudaMemcpyAsync(var + m0, f->tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+            FCK(kdiag_launch(eu->prog, f->stage.xs, d, mc, f->stage.tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, mc, f->Mpad, f->stage.tmpc2, st, &eu->launches));
+            FCK(rowvar_launch(f->stage.bufB, f->Mpad, f->stage.zeroc, mc, f->Mpad, f->stage.w, st, &eu->launches));
+            if (f->mode == 2) FCK(cudaMemsetAsync(f->stage.tmpc2, 0, sizeof(double) * mc, st));
+            FCK(ew_launch(6, mc, f->stage.tmpc, f->stage.tmpc2, f->stage.w, nullptr, 0.0, st, &eu->launches));
+            FCK(cudaMemcpyAsync(var + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
             if (f->mode != 2) FCK(trsm_right_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));      // A L_uu^-1
             FCK(trsm_right_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));                        // B L_s^-1
         }
-        FCK(crossgram_dx_launch(eu->prog, f->xs, d, mc, eu->x, d, f->M, d, f->uvec, (var && f->mode != 2) ? f->bufA : nullptr,
-                                var ? f->bufB : nullptr, f->Mpad, f->mode == 2 ? 0.0 : 1.0, ddmu, ddvar, st, &eu->launches));
+        FCK(crossgram_dx_launch(eu->prog, f->stage.xs, d, mc, eu->x, d, f->M, d, f->data.uvec, (var && f->mode != 2) ? f->stage.bufA.data() : nullptr,
+                                var ? f->stage.bufB.data() : nullptr, f->Mpad, f->mode == 2 ? 0.0 : 1.0, ddmu, ddvar, st, &eu->launches));
         FCK(cudaMemcpyAsync(dmu + m0 * d, ddmu, sizeof(double) * mc * d, cudaMemcpyDeviceToHost, st));
         if (var) FCK(cudaMemcpyAsync(dvar + m0 * d, ddvar, sizeof(double) * mc * d, cudaMemcpyDeviceToHost, st));
         FCK(cudaStreamSynchronize(st));
@@ -429,28 +430,23 @@ int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64
 // predictMVN with the FULL predictive covariance (fitc.jl:324-332 -> determ_train_conditional.jl:41-59 ->
 // subsetofregressors.jl:302-321):  Sigma* = K** - K*u K_uu^-1 Ku* + K*u S^-1 Ku*   (FITC, DTC);   K*u S^-1 Ku*   (SoR)
 // = K** - A A' + B B' with A = K*u L_uu^-T, B = K*u L_s^-T: two whitening TRSMs and two NT GEMMs.  Ms <= one staging chunk.
-// Sigma* into f->Kss (leading dimension Ms rounded up to 128) and mu into f->tmpc and mu[Ms], on eu's stream; Ms <= Nc
+// Sigma* into f->Kss (leading dimension Ms rounded up to 128) and mu into f->stage.tmpc and mu[Ms], on eu's stream; Ms <= Nc
 static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
-    if (Mspad > f->Kss_rows) {
-        if (f->Kss) cudaFree(f->Kss);
-        f->Kss = nullptr; f->Kss_rows = 0;
-        FCK(cudaMalloc(&f->Kss, sizeof(double) * Mspad * Mspad));
-        f->Kss_rows = Mspad;
-    }
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, f->Mpad};
-    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, f->Mpad};
-    FCK(cudaMemcpy2DAsync(f->xs, sizeof(double) * f->d, xs, sizeof(double) * ldxs, sizeof(double) * f->d, Ms, cudaMemcpyHostToDevice, st));
-    FCK(fitc_kfu(f, f->xs, Ms));                                         // bufA = K*u  (Ms x Mpad, zero padded rows)
-    FCK(rowdot_launch(f->bufA, f->Mpad, f->uvec, Ms, f->Mpad, f->tmpc, st, &eu->launches));
-    FCK(cudaMemcpyAsync(mu, f->tmpc, sizeof(double) * Ms, cudaMemcpyDeviceToHost, st));
-    FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+    FCK(f->Kss.ensure((size_t)Mspad * Mspad));
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
+    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, f->Mpad);
+    FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * f->d, xs, sizeof(double) * ldxs, sizeof(double) * f->d, Ms, cudaMemcpyHostToDevice, st));
+    FCK(fitc_kfu(f, f->stage.xs, Ms));                                         // bufA = K*u  (Ms x Mpad, zero padded rows)
+    FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, Ms, f->Mpad, f->stage.tmpc, st, &eu->launches));
+    FCK(cudaMemcpyAsync(mu, f->stage.tmpc, sizeof(double) * Ms, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
     FCK(trsm_rec_buf(es, bB2, (int)Mspad, 0, (int)f->Mpad));             // B = K*u L_s^-T
     if (f->mode != 2) {
         FCK(trsm_rec_buf(eu, bA, (int)Mspad, 0, (int)f->Mpad));         // A = K*u L_uu^-T
-        FCK(gram_full_launch(eu->prog, f->xs, f->d, Ms, Mspad, f->d, f->Kss, Mspad, st, &eu->launches));
+        FCK(gram_full_launch(eu->prog, f->stage.xs, f->d, Ms, Mspad, f->d, f->Kss, Mspad, st, &eu->launches));
         FCK(gemm_whole(eu, bA, bA, f->Kss, Mspad, Mspad, Mspad, f->Mpad, -1.0, 1.0));
     } else {
         FCK(cudaMemsetAsync(f->Kss, 0, sizeof(double) * Mspad * Mspad, st));
@@ -517,105 +513,106 @@ static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, doubl
     const size_t chunks = f->mode == 3 ? fsa_num_chunks(f) : (size_t)((f->N + f->Nc - 1) / f->Nc);
     if (dmll_xu) {
         TRY(event_pairs(f, f->xu_ev, chunks + 2));
-        if (!f->dxu) FCK(cudaMalloc(&f->dxu, sizeof(double) * f->M * f->d));
+        FCK(f->dxu.ensure((size_t)f->M * f->d));
         FCK(cudaEventRecord(f->xu_ev[0], f->eu->st));
     }
     if (dmll_x) {
         TRY(event_pairs(f, f->x_ev, 2 * chunks + 1));
-        if (!f->dx) FCK(cudaMalloc(&f->dx, sizeof(double) * f->N * f->d));
+        FCK(f->dx.ensure((size_t)f->N * f->d));
         FCK(cudaEventRecord(f->x_ev[0], f->eu->st));
     }
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int np = eu->prog.n_theta;
     const int64_t Mp = f->Mpad, Nc = f->Nc;
-    if (!f->grad_ws) {
-        FCK(cudaMalloc(&f->bufC, sizeof(double) * Nc * Mp));
-        for (double** p : {&f->Hbuf, &f->Wbuf, &f->Tbuf}) FCK(cudaMalloc(p, sizeof(double) * Mp * Mp));
-        FCK(cudaMalloc(&f->gvec, sizeof(double) * (f->N + TILE)));
-        FCK(cudaMalloc(&f->betav, sizeof(double) * Mp));
+    if (!f->grad.ready) TRY(make_group(f->grad, [&] {
+        FitcGradWs& g = f->grad;
+        FCK(g.bufC.alloc((size_t)Nc * Mp));
+        for (DevBuf<double>* p : {&g.Hbuf, &g.Wbuf, &g.Tbuf}) FCK(p->alloc((size_t)Mp * Mp));
+        FCK(g.gvec.alloc(f->N + TILE));
+        FCK(g.betav.alloc(Mp));
         const size_t tiles = (size_t)std::max((Nc / TILE) * (Mp / TILE), (Mp / TILE) * (Mp / TILE));
-        FCK(cudaMalloc(&f->gpart, sizeof(double) * tiles * GPB200_MAX_THETA));
-        FCK(cudaMalloc(&f->gacc, sizeof(double) * GPB200_MAX_THETA));
-        FCK(cudaMalloc(&f->gtmp, sizeof(double) * GPB200_MAX_THETA));
+        FCK(g.gpart.alloc(tiles * GPB200_MAX_THETA));
+        FCK(g.gacc.alloc(GPB200_MAX_THETA));
+        FCK(g.gtmp.alloc(GPB200_MAX_THETA));
         if (eu->tma_ok) {
-            const bool ok = gemm_make_tensor_map(&f->mapAt, f->bufA, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapC, f->bufC, Nc, Mp, Mp) &&
-                            gemm_make_tensor_map(&f->mapCt, f->bufC, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapH, f->Hbuf, Mp, Mp, Mp) &&
-                            gemm_make_tensor_map(&f->mapT, f->Tbuf, Mp, Mp, Mp);
+            const bool ok = gemm_make_tensor_map(&g.mapAt, f->stage.bufA, Mp, Nc, Nc) && gemm_make_tensor_map(&g.mapC, g.bufC, Nc, Mp, Mp) &&
+                            gemm_make_tensor_map(&g.mapCt, g.bufC, Mp, Nc, Nc) && gemm_make_tensor_map(&g.mapH, g.Hbuf, Mp, Mp, Mp) &&
+                            gemm_make_tensor_map(&g.mapT, g.Tbuf, Mp, Mp, Mp);
             if (!ok) return fail(f, GPB200_ECUDA, "fitc_grad_kernel: cuTensorMapEncodeTiled failed");
         }
-        f->grad_ws = true;
-    }
+        g.ready = true;
+        return GPB200_OK;
+    }));
     // explicit K_uu^-1 and Sigma_QR^-1 (full symmetric) in the sub-engines' G buffers
     FSUB(gpb200_grad_prepare(eu), eu);
     FSUB(gpb200_grad_prepare(es), es);
     FCK(symmetrize_launch(eu->G, eu->ld, Mp, st, &eu->launches));
     FCK(symmetrize_launch(es->G, es->ld, Mp, st, &eu->launches));
-    const bool tma = eu->tma_ok;
-    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bAt{tma ? &f->mapAt : nullptr, f->bufA, Nc};
-    GemmBuf bCt{tma ? &f->mapCt : nullptr, f->bufC, Nc};
-    GemmBuf bH{tma ? &f->mapH : nullptr, f->Hbuf, Mp}, bT{tma ? &f->mapT : nullptr, f->Tbuf, Mp};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp), bAt = gbuf(eu, f->stage.bufA, f->grad.mapAt, Nc);
+    const GemmBuf bCt = gbuf(eu, f->grad.bufC, f->grad.mapCt, Nc);
+    const GemmBuf bH = gbuf(eu, f->grad.Hbuf, f->grad.mapH, Mp), bT = gbuf(eu, f->grad.Tbuf, f->grad.mapT, Mp);
     // beta = K_uu^-1 (K_uf alpha)
-    FCK(cudaMemsetAsync(f->rhsm, 0, sizeof(double) * Mp, st));
+    FCK(cudaMemsetAsync(f->data.rhsm, 0, sizeof(double) * Mp, st));
     for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
         const int64_t nc = std::min(Nc, f->N - r0);
-        FCK(fitc_kuf(f, f->x + r0 * f->d, nc));
-        FCK(cudaMemsetAsync(f->w, 0, sizeof(double) * Nc, st));
-        FCK(cudaMemcpyAsync(f->w, f->alpha + r0, sizeof(double) * nc, cudaMemcpyDeviceToDevice, st));
-        FCK(rowdot_launch(f->bufB, Nc, f->w, f->M, Nc, f->tmpm, st, &eu->launches));
-        FCK(ew_launch(2, f->M, f->rhsm, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(fitc_kuf(f, f->data.x + r0 * f->d, nc));
+        FCK(cudaMemsetAsync(f->stage.w, 0, sizeof(double) * Nc, st));
+        FCK(cudaMemcpyAsync(f->stage.w, f->data.alpha + r0, sizeof(double) * nc, cudaMemcpyDeviceToDevice, st));
+        FCK(rowdot_launch(f->stage.bufB, Nc, f->stage.w, f->M, Nc, f->data.tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->data.rhsm, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
     }
-    TRY(fitc_allreduce(f, f->rhsm, (size_t)Mp));                    // K_uf alpha over all rows
-    FCK(solve_device(eu, f->rhsm, f->tmpm, f->betav));
-    FCK(cudaMemsetAsync(f->gacc, 0, sizeof(double) * GPB200_MAX_THETA, st));
-    FCK(cudaMemsetAsync(f->Hbuf, 0, sizeof(double) * Mp * Mp, st));
+    TRY(fitc_allreduce(f, f->data.rhsm, (size_t)Mp));                    // K_uf alpha over all rows
+    FCK(solve_device(eu, f->data.rhsm, f->data.tmpm, f->grad.betav));
+    FCK(cudaMemsetAsync(f->grad.gacc, 0, sizeof(double) * GPB200_MAX_THETA, st));
+    FCK(cudaMemsetAsync(f->grad.Hbuf, 0, sizeof(double) * Mp * Mp, st));
     if (f->mode == 3) return fsa_grad_kernel(f, dmll_kernel, dmll_xu, dmll_x);
     size_t xk = 0, rk = 0;                                                // Xu / X contraction launches so far
     for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
         const int64_t nc = std::min(Nc, f->N - r0);
-        const double* xr = f->x + r0 * f->d;
+        const double* xr = f->data.x + r0 * f->d;
         FCK(fitc_kfu(f, xr, nc));                                         // bufA = K_fu chunk
-        FCK(gemm_whole(es, bA, bufG(es), f->bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));         // P2 = K_fu S^-1 -> bufB (as Nc x Mpad)
-        FCK(rowdot2_launch(f->bufA, f->bufB, Mp, nc, Mp, f->tmpc, st, &eu->launches));
-        if (f->mode == 0) FCK(fitc_g_launch(nc, f->alpha + r0, f->lam + r0, f->tmpc, f->gvec + r0, st, &eu->launches));
-        else FCK(cudaMemsetAsync(f->gvec + r0, 0, sizeof(double) * nc, st));       // SoR part only (sor.jl:219-253)
-        FCK(gemm_whole(eu, bA, bufG(eu), f->bufC, Mp, Nc, Mp, Mp, 1.0, 0.0));         // P1 = K_fu K_uu^-1 -> bufC
-        FCK(fitc_wfu_launch(f->bufB, f->bufC, Mp, nc, f->M, f->alpha + r0, f->lam + r0, f->gvec + r0, f->betav, st, &eu->launches));
-        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufB, Mp, f->gpart, f->gtmp, st, &eu->launches));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
-        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufB, 0, nullptr, xk > 0)); ++xk; }
+        FCK(gemm_whole(es, bA, bufG(es), f->stage.bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));         // P2 = K_fu S^-1 -> bufB (as Nc x Mpad)
+        FCK(rowdot2_launch(f->stage.bufA, f->stage.bufB, Mp, nc, Mp, f->stage.tmpc, st, &eu->launches));
+        if (f->mode == 0) FCK(fitc_g_launch(nc, f->data.alpha + r0, f->data.lam + r0, f->stage.tmpc, f->grad.gvec + r0, st, &eu->launches));
+        else FCK(cudaMemsetAsync(f->grad.gvec + r0, 0, sizeof(double) * nc, st));       // SoR part only (sor.jl:219-253)
+        FCK(gemm_whole(eu, bA, bufG(eu), f->grad.bufC, Mp, Nc, Mp, Mp, 1.0, 0.0));         // P1 = K_fu K_uu^-1 -> bufC
+        FCK(fitc_wfu_launch(f->stage.bufB, f->grad.bufC, Mp, nc, f->M, f->data.alpha + r0, f->data.lam + r0, f->grad.gvec + r0, f->grad.betav, st, &eu->launches));
+        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->stage.bufB, Mp, f->grad.gpart, f->grad.gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->grad.gacc, f->grad.gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->stage.bufB, 0, nullptr, xk > 0)); ++xk; }
         if (dmll_x) {
-            TRY(x_rows(f, rk + 1, xr, nc, f->bufB, f->mode == 0 ? f->gvec + r0 : nullptr, nullptr, nullptr, f->dx + r0 * f->d, 0));
+            TRY(x_rows(f, rk + 1, xr, nc, f->stage.bufB, f->mode == 0 ? f->grad.gvec + r0 : nullptr, nullptr, nullptr, f->dx + r0 * f->d, 0));
             ++rk;
         }
         if (f->mode != 0) continue;                                       // no Lambda-derivative terms for SoR / DTC
         // diagonal term sum_i g_i dK_ii/dθ_p (scratch: bufC as np x nc)
-        FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->gvec + r0, f->bufC, st, &eu->launches));
-        for (int p = 0; p < np; ++p) FCK(sum_launch(f->bufC + (size_t)p * nc, nc, f->gtmp + p, st, &eu->launches));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(kdiag_grad_launch(eu->prog, xr, f->d, nc, f->grad.gvec + r0, f->grad.bufC, st, &eu->launches));
+        for (int p = 0; p < np; ++p) FCK(sum_launch(f->grad.bufC + (size_t)p * nc, nc, f->grad.gtmp + p, st, &eu->launches));
+        FCK(ew_launch(2, np, f->grad.gacc, f->grad.gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         // H += K_uf diag(g) K_fu
-        FCK(crossgram_launch(eu->prog, eu->x, f->d, f->M, Mp, xr, f->d, nc, Nc, f->d, f->bufA, Nc, st, &eu->launches));   // bufA = K_uf chunk (Mpad x Nc)
-        FCK(cudaMemcpyAsync(f->bufC, f->bufA, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
-        FCK(colscale_launch(f->bufC, Nc, Mp, nc, f->gvec + r0, st, &eu->launches));
-        FCK(gemm_whole(eu, bAt, bCt, f->Hbuf, Mp, Mp, Mp, Nc, 1.0, 1.0));
+        FCK(crossgram_launch(eu->prog, eu->x, f->d, f->M, Mp, xr, f->d, nc, Nc, f->d, f->stage.bufA, Nc, st, &eu->launches));   // bufA = K_uf chunk (Mpad x Nc)
+        FCK(cudaMemcpyAsync(f->grad.bufC, f->stage.bufA, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
+        FCK(colscale_launch(f->grad.bufC, Nc, Mp, nc, f->grad.gvec + r0, st, &eu->launches));
+        FCK(gemm_whole(eu, bAt, bCt, f->grad.Hbuf, Mp, Mp, Mp, Nc, 1.0, 1.0));
     }
     // multi-GPU: the per-row traces and H = K_uf diag(g) K_fu are sums over the ranks' rows; the M x M part below is replicated
-    TRY(fitc_allreduce(f, f->gacc, (size_t)np));
-    TRY(fitc_allreduce(f, f->Hbuf, (size_t)Mp * (size_t)Mp));
+    TRY(fitc_allreduce(f, f->grad.gacc, (size_t)np));
+    TRY(fitc_allreduce(f, f->grad.Hbuf, (size_t)Mp * (size_t)Mp));
     if (dmll_xu) TRY(fitc_allreduce(f, f->dxu, (size_t)f->M * f->d));   // W_fu part over all rows
     // T = K_uu^-1 H ; Wbuf = K_uu^-1 T' = K_uu^-1 H K_uu^-1
-    FCK(gemm_whole(eu, bufG(eu), bH, f->Tbuf, Mp, Mp, Mp, Mp, 1.0, 0.0));
-    FCK(gemm_whole(eu, bufG(eu), bT, f->Wbuf, Mp, Mp, Mp, Mp, 1.0, 0.0));
-    FCK(fitc_wuu_launch(f->Wbuf, f->Wbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
-    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
-    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(gemm_whole(eu, bufG(eu), bH, f->grad.Tbuf, Mp, Mp, Mp, Mp, 1.0, 0.0));
+    FCK(gemm_whole(eu, bufG(eu), bT, f->grad.Wbuf, Mp, Mp, Mp, Mp, 1.0, 0.0));
+    FCK(fitc_wuu_launch(f->grad.Wbuf, f->grad.Wbuf, eu->G, es->G, Mp, f->M, f->grad.betav, st, &eu->launches));
+    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->grad.Wbuf, Mp, f->grad.gpart, f->grad.gtmp, st, &eu->launches));
+    FCK(ew_launch(2, np, f->grad.gacc, f->grad.gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
     if (dmll_xu) {
-        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, 1)); ++xk;
+        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->grad.Wbuf, 1, nullptr, 1)); ++xk;
         FCK(cudaEventRecord(f->xu_ev[1], st));
     }
     if (dmll_x) FCK(cudaEventRecord(f->x_ev[1], st));
     std::vector<double> out((size_t)std::max(np, 1));
-    FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(out.data(), f->grad.gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta above
     if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
@@ -651,7 +648,7 @@ int gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_
         return fail(f, GPB200_EINVAL, "fitc_set_inducing: M must be set_data's, xu non-null and ldxu >= d");
     }
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    f->factored = f->alpha_ready = f->cv.m_ok = false;
     FSUB(gpb200_set_data(f->eu, M, f->d, xu, ldxu), f->eu);
     FSUB(gpb200_set_data(f->es, M, f->d, xu, ldxu), f->es);
     return GPB200_OK;
@@ -665,9 +662,9 @@ int gpb200_fitc_set_inputs(gpb200_fitc* f, int64_t N, const double* x, int64_t l
     if (!f->has_data) return fail(f, GPB200_ESTATE, "fitc_set_inputs: set_data first");
     if (N != f->N || !x || ldx < f->d) return fail(f, GPB200_EINVAL, "fitc_set_inputs: N must be set_data's, x non-null and ldx >= d");
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = f->cv_m_ok = false;
+    f->factored = f->alpha_ready = f->cv.m_ok = false;
     cudaStream_t st = f->eu->st;
-    FCK(cudaMemcpy2DAsync(f->x, sizeof(double) * f->d, x, sizeof(double) * ldx, sizeof(double) * f->d, N, cudaMemcpyHostToDevice, st));
+    FCK(cudaMemcpy2DAsync(f->data.x, sizeof(double) * f->d, x, sizeof(double) * ldx, sizeof(double) * f->d, N, cudaMemcpyHostToDevice, st));
     if (f->fsa) TRY(fsa_set_inputs(f, x, ldx));
     FCK(cudaStreamSynchronize(st));
     return GPB200_OK;
@@ -700,23 +697,25 @@ static int fitc_cv_prepare(gpb200_fitc* f) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N;
-    if (!f->cv_ws) {
-        for (double** p : {&f->cvG, &f->cvGt, &f->cvCh, &f->cvP}) FCK(cudaMalloc(p, sizeof(double) * Nc * Mp));
-        for (double** p : {&f->cvDuu, &f->cvDp, &f->cvR, &f->cvH, &f->cvQ}) FCK(cudaMalloc(p, sizeof(double) * Mp * Mp));
-        for (double** p : {&f->cvalpha, &f->cvdel, &f->cvilam, &f->cvza, &f->cvdg}) FCK(cudaMalloc(p, sizeof(double) * (N + Nc)));
-        for (double** p : {&f->cvda, &f->cvq, &f->cvlamV, &f->cvdelV}) FCK(cudaMalloc(p, sizeof(double) * Nc));
-        FCK(cudaMalloc(&f->cvxs, sizeof(double) * Nc * f->d));
-        FCK(cudaMalloc(&f->cvm, sizeof(double) * 8 * Mp));
-        FCK(cudaMalloc(&f->cvidx, sizeof(long long) * Nc));
-        FCK(cudaMemsetAsync(f->cvalpha, 0, sizeof(double) * (N + Nc), st));      // zero tail: chunk vectors are read Nc wide
+    if (!f->cv.ready) TRY(make_group(f->cv, [&] {
+        FitcCvWs& g = f->cv;
+        for (DevBuf<double>* p : {&g.G, &g.Gt, &g.Ch, &g.P}) FCK(p->alloc((size_t)Nc * Mp));
+        for (DevBuf<double>* p : {&g.Duu, &g.Dp, &g.R, &g.H, &g.Q}) FCK(p->alloc((size_t)Mp * Mp));
+        for (DevBuf<double>* p : {&g.alpha, &g.del, &g.ilam, &g.za, &g.dg}) FCK(p->alloc(N + Nc));
+        for (DevBuf<double>* p : {&g.da, &g.q, &g.lamV, &g.delV}) FCK(p->alloc(Nc));
+        FCK(g.xs.alloc((size_t)Nc * f->d));
+        FCK(g.m.alloc(8 * Mp));
+        FCK(g.idx.alloc(Nc));
+        FCK(cudaMemsetAsync(g.alpha, 0, sizeof(double) * (N + Nc), st));      // zero tail: chunk vectors are read Nc wide
         if (eu->tma_ok) {
-            const bool ok = gemm_make_tensor_map(&f->mapCvGt, f->cvGt, Mp, Nc, Nc) && gemm_make_tensor_map(&f->mapCvCh, f->cvCh, Nc, Mp, Mp) &&
-                            gemm_make_tensor_map(&f->mapCvP, f->cvP, Nc, Mp, Mp) && gemm_make_tensor_map(&f->mapCvDuu, f->cvDuu, Mp, Mp, Mp) &&
-                            gemm_make_tensor_map(&f->mapCvDp, f->cvDp, Mp, Mp, Mp) && gemm_make_tensor_map(&f->mapCvQ, f->cvQ, Mp, Mp, Mp);
+            const bool ok = gemm_make_tensor_map(&g.mapGt, g.Gt, Mp, Nc, Nc) && gemm_make_tensor_map(&g.mapCh, g.Ch, Nc, Mp, Mp) &&
+                            gemm_make_tensor_map(&g.mapP, g.P, Nc, Mp, Mp) && gemm_make_tensor_map(&g.mapDuu, g.Duu, Mp, Mp, Mp) &&
+                            gemm_make_tensor_map(&g.mapDp, g.Dp, Mp, Mp, Mp) && gemm_make_tensor_map(&g.mapQ, g.Q, Mp, Mp, Mp);
             if (!ok) return fail(f, GPB200_ECUDA, "fitc_cv: cuTensorMapEncodeTiled failed");
         }
-        f->cv_ws = true;
-    }
+        g.ready = true;
+        return GPB200_OK;
+    }));
     FSUB(gpb200_grad_prepare(eu), eu);
     FSUB(gpb200_grad_prepare(es), es);
     FCK(symmetrize_launch(eu->G, eu->ld, Mp, st, &eu->launches));
@@ -732,16 +731,15 @@ int gpb200_fitc_get_inverse_diag(gpb200_fitc* f, double* diag) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Mp = f->Mpad, Nc = f->Nc;
-    const bool tma = eu->tma_ok;
-    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp);
     for (int64_t r0 = 0; r0 < f->N; r0 += Nc) {
         const int64_t nc = std::min(Nc, f->N - r0);
-        FCK(fitc_kfu(f, f->x + r0 * f->d, nc));                                                   // bufA = K_fu
-        FCK(gemm_whole(f->eu, bA, bufG(es), f->cvCh, Mp, Nc, Mp, Mp, 1.0, 0.0));                      // K_fu S^-1
-        FCK(rowdot2_launch(f->bufA, f->cvCh, Mp, nc, Mp, f->cvq, st, &eu->launches));
-        FCK(fitc_cv_invdiag_launch(nc, f->lam + r0, f->cvq, f->cvdg + r0, st, &eu->launches));
+        FCK(fitc_kfu(f, f->data.x + r0 * f->d, nc));                                                   // bufA = K_fu
+        FCK(gemm_whole(f->eu, bA, bufG(es), f->cv.Ch, Mp, Nc, Mp, Mp, 1.0, 0.0));                      // K_fu S^-1
+        FCK(rowdot2_launch(f->stage.bufA, f->cv.Ch, Mp, nc, Mp, f->cv.q, st, &eu->launches));
+        FCK(fitc_cv_invdiag_launch(nc, f->data.lam + r0, f->cv.q, f->cv.dg + r0, st, &eu->launches));
     }
-    FCK(cudaMemcpyAsync(diag, f->cvdg, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(diag, f->cv.dg, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
@@ -754,82 +752,82 @@ int gpb200_fitc_cv_param(gpb200_fitc* f, int32_t param, const double* alpha, dou
         return fail(f, GPB200_EINVAL, "fitc_cv_param: param must be -1 (noise variance) or a kernel parameter index below " + std::to_string(np));
     FCK(cudaSetDevice(f->device));
     TRY(fitc_cv_prepare(f));
-    f->cv_m_ok = false;
+    f->cv.m_ok = false;
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N, M = f->M;
     const int d = f->d;
-    const bool tma = eu->tma_ok, noise = param < 0;
+    const bool noise = param < 0;
     const int kind = noise ? 2 : (f->mode == 0 ? 0 : 1);
-    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bB{tma ? &f->mapB : nullptr, f->bufB, Nc};
-    GemmBuf bGt{tma ? &f->mapCvGt : nullptr, f->cvGt, Nc}, bCh{tma ? &f->mapCvCh : nullptr, f->cvCh, Mp};
-    GemmBuf bDuu{tma ? &f->mapCvDuu : nullptr, f->cvDuu, Mp}, bDp{tma ? &f->mapCvDp : nullptr, f->cvDp, Mp};
-    GemmBuf bQ{tma ? &f->mapCvQ : nullptr, f->cvQ, Mp};
-    double *kta = f->cvm, *gta = f->cvm + Mp, *uD = f->cvm + 2 * Mp, *beta = f->cvm + 3 * Mp;
-    double *rb = f->cvm + 4 * Mp, *w = f->cvm + 5 * Mp, *tmp = f->cvm + 6 * Mp;
-    if (alpha) FCK(cudaMemcpyAsync(f->cvalpha, alpha, sizeof(double) * N, cudaMemcpyHostToDevice, st));
-    else FCK(cudaMemcpyAsync(f->cvalpha, f->alpha, sizeof(double) * N, cudaMemcpyDeviceToDevice, st));
-    FCK(ew_launch(5, N, f->cvilam, f->lam, nullptr, nullptr, 0.0, st, &eu->launches));              // 1 / Lambda
-    FCK(cudaMemsetAsync(f->cvm, 0, sizeof(double) * 8 * Mp, st));
-    FCK(cudaMemsetAsync(f->cvR, 0, sizeof(double) * Mp * Mp, st));
-    FCK(cudaMemsetAsync(f->cvH, 0, sizeof(double) * Mp * Mp, st));
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp), bB = gbuf(eu, f->stage.bufB, f->stage.mapB, Nc);
+    const GemmBuf bGt = gbuf(eu, f->cv.Gt, f->cv.mapGt, Nc), bCh = gbuf(eu, f->cv.Ch, f->cv.mapCh, Mp);
+    const GemmBuf bDuu = gbuf(eu, f->cv.Duu, f->cv.mapDuu, Mp), bDp = gbuf(eu, f->cv.Dp, f->cv.mapDp, Mp);
+    const GemmBuf bQ = gbuf(eu, f->cv.Q, f->cv.mapQ, Mp);
+    double *kta = f->cv.m, *gta = f->cv.m + Mp, *uD = f->cv.m + 2 * Mp, *beta = f->cv.m + 3 * Mp;
+    double *rb = f->cv.m + 4 * Mp, *w = f->cv.m + 5 * Mp, *tmp = f->cv.m + 6 * Mp;
+    if (alpha) FCK(cudaMemcpyAsync(f->cv.alpha, alpha, sizeof(double) * N, cudaMemcpyHostToDevice, st));
+    else FCK(cudaMemcpyAsync(f->cv.alpha, f->data.alpha, sizeof(double) * N, cudaMemcpyDeviceToDevice, st));
+    FCK(ew_launch(5, N, f->cv.ilam, f->data.lam, nullptr, nullptr, 0.0, st, &eu->launches));              // 1 / Lambda
+    FCK(cudaMemsetAsync(f->cv.m, 0, sizeof(double) * 8 * Mp, st));
+    FCK(cudaMemsetAsync(f->cv.R, 0, sizeof(double) * Mp * Mp, st));
+    FCK(cudaMemsetAsync(f->cv.H, 0, sizeof(double) * Mp * Mp, st));
     if (!noise) {   // Dp = dK_uu K_uu^-1
-        FCK(gram_grad_full_launch(eu->prog, eu->x, d, d, M, Mp, param, f->cvDuu, Mp, st, &eu->launches));
-        FCK(gemm_whole(f->eu, bDuu, bufG(eu), f->cvDp, Mp, Mp, Mp, Mp, 1.0, 0.0));
+        FCK(gram_grad_full_launch(eu->prog, eu->x, d, d, M, Mp, param, f->cv.Duu, Mp, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bDuu, bufG(eu), f->cv.Dp, Mp, Mp, Mp, Mp, 1.0, 0.0));
     }
     // pass 1: Delta, R, H, K_uf alpha, G'alpha, K_uf L^-1 Delta alpha
     for (int64_t r0 = 0; r0 < N; r0 += Nc) {
         const int64_t nc = std::min(Nc, N - r0);
-        const double* xr = f->x + r0 * d;
+        const double* xr = f->data.x + r0 * d;
         FCK(fitc_kfu(f, xr, nc));                                                                     // bufA = K_fu
         if (!noise) {
-            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cvG, Mp, st, &eu->launches));
-            if (kind == 0) FCK(gemm_whole(f->eu, bA, bufG(eu), f->bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));     // bufB = C (Nc x Mpad)
-            FCK(gemm_whole(f->eu, bA, bDp, f->cvG, Mp, Nc, Mp, Mp, -0.5, 1.0, f->cvGt, Nc));              // G and G'
+            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cv.G, Mp, st, &eu->launches));
+            if (kind == 0) FCK(gemm_whole(f->eu, bA, bufG(eu), f->stage.bufB, Mp, Nc, Mp, Mp, 1.0, 0.0));     // bufB = C (Nc x Mpad)
+            FCK(gemm_whole(f->eu, bA, bDp, f->cv.G, Mp, Nc, Mp, Mp, -0.5, 1.0, f->cv.Gt, Nc));              // G and G'
         }
-        FCK(fitc_cv_delta_launch(kind, eu->prog, xr, d, param, f->cvG, f->bufB, Mp, Mp, nc, Nc, f->cvalpha + r0, f->cvdel + r0,
-                                 f->cvda, st, &eu->launches));
+        FCK(fitc_cv_delta_launch(kind, eu->prog, xr, d, param, f->cv.G, f->stage.bufB, Mp, Mp, nc, Nc, f->cv.alpha + r0, f->cv.del + r0,
+                                 f->cv.da, st, &eu->launches));
         FCK(fitc_kuf(f, xr, nc));                                                                     // bufB = K_uf
-        FCK(rowdot_launch(f->bufB, Nc, f->cvalpha + r0, M, Nc, tmp, st, &eu->launches));
+        FCK(rowdot_launch(f->stage.bufB, Nc, f->cv.alpha + r0, M, Nc, tmp, st, &eu->launches));
         FCK(ew_launch(2, M, kta, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
-        FCK(colscale_launch(f->bufB, Nc, Mp, nc, f->cvilam + r0, st, &eu->launches));                // K_uf L^-1
-        FCK(rowdot_launch(f->bufB, Nc, f->cvda, M, Nc, tmp, st, &eu->launches));
+        FCK(colscale_launch(f->stage.bufB, Nc, Mp, nc, f->cv.ilam + r0, st, &eu->launches));                // K_uf L^-1
+        FCK(rowdot_launch(f->stage.bufB, Nc, f->cv.da, M, Nc, tmp, st, &eu->launches));
         FCK(ew_launch(2, M, uD, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
         if (!noise) {
-            FCK(rowdot_launch(f->cvGt, Nc, f->cvalpha + r0, M, Nc, tmp, st, &eu->launches));
+            FCK(rowdot_launch(f->cv.Gt, Nc, f->cv.alpha + r0, M, Nc, tmp, st, &eu->launches));
             FCK(ew_launch(2, M, gta, tmp, nullptr, nullptr, 0.0, st, &eu->launches));
-            FCK(gemm_whole(f->eu, bB, bGt, f->cvR, Mp, Mp, Mp, Nc, 1.0, 1.0));                           // R += K_uf L^-1 G
+            FCK(gemm_whole(f->eu, bB, bGt, f->cv.R, Mp, Mp, Mp, Nc, 1.0, 1.0));                           // R += K_uf L^-1 G
         }
         if (kind != 1) {                                                                              // H += K_uf L^-1 Delta L^-1 K_fu
-            FCK(cudaMemcpyAsync(f->cvGt, f->bufB, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
-            FCK(colscale_launch(f->cvGt, Nc, Mp, nc, f->cvdel + r0, st, &eu->launches));
-            FCK(gemm_whole(f->eu, bB, bGt, f->cvH, Mp, Mp, Mp, Nc, 1.0, 1.0));
+            FCK(cudaMemcpyAsync(f->cv.Gt, f->stage.bufB, sizeof(double) * Mp * Nc, cudaMemcpyDeviceToDevice, st));
+            FCK(colscale_launch(f->cv.Gt, Nc, Mp, nc, f->cv.del + r0, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bB, bGt, f->cv.H, Mp, Mp, Mp, Nc, 1.0, 1.0));
         }
     }
     FCK(rowdot_launch(eu->G, eu->ld, kta, M, Mp, beta, st, &eu->launches));                         // beta = K_uu^-1 K_uf alpha
-    FCK(rowdot_launch(f->cvR, Mp, beta, M, Mp, rb, st, &eu->launches));
+    FCK(rowdot_launch(f->cv.R, Mp, beta, M, Mp, rb, st, &eu->launches));
     FCK(fitc_cv_wvec_launch(M, w, gta, uD, rb, st, &eu->launches));
-    FCK(fitc_cv_qs_launch(f->cvQ, f->cvH, f->cvR, Mp, Mp, st, &eu->launches));
+    FCK(fitc_cv_qs_launch(f->cv.Q, f->cv.H, f->cv.R, Mp, Mp, st, &eu->launches));
     // pass 2: the two N-vectors
     for (int64_t r0 = 0; r0 < N; r0 += Nc) {
         const int64_t nc = std::min(Nc, N - r0);
-        const double* xr = f->x + r0 * d;
+        const double* xr = f->data.x + r0 * d;
         FCK(fitc_kfu(f, xr, nc));
         if (!noise) {
-            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cvG, Mp, st, &eu->launches));
-            FCK(gemm_whole(f->eu, bA, bDp, f->cvG, Mp, Nc, Mp, Mp, -0.5, 1.0));
+            FCK(crossgram_grad_launch(eu->prog, xr, d, nc, Nc, eu->x, d, M, Mp, d, param, f->cv.G, Mp, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bA, bDp, f->cv.G, Mp, Nc, Mp, Mp, -0.5, 1.0));
         }
-        FCK(gemm_whole(f->eu, bA, bufG(es), f->cvCh, Mp, Nc, Mp, Mp, 1.0, 0.0));
-        FCK(scale_launch(1, f->cvCh, Mp, nc, Mp, f->lam + r0, st, &eu->launches));                  // Ch = L^-1 K_fu S^-1
-        FCK(gemm_whole(f->eu, bCh, bQ, f->cvP, Mp, Nc, Mp, Mp, 1.0, 0.0));                                // Ch Q
-        FCK(fitc_cv_rows_launch(noise ? nullptr : f->cvG, f->cvCh, f->bufA, f->cvP, Mp, nc, Mp, f->lam + r0, f->cvdel + r0,
-                                f->cvalpha + r0, beta, w, f->cvza + r0, f->cvdg + r0, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bA, bufG(es), f->cv.Ch, Mp, Nc, Mp, Mp, 1.0, 0.0));
+        FCK(scale_launch(1, f->cv.Ch, Mp, nc, Mp, f->data.lam + r0, st, &eu->launches));                  // Ch = L^-1 K_fu S^-1
+        FCK(gemm_whole(f->eu, bCh, bQ, f->cv.P, Mp, Nc, Mp, Mp, 1.0, 0.0));                                // Ch Q
+        FCK(fitc_cv_rows_launch(noise ? nullptr : f->cv.G.data(), f->cv.Ch, f->stage.bufA, f->cv.P, Mp, nc, Mp, f->data.lam + r0, f->cv.del + r0,
+                                f->cv.alpha + r0, beta, w, f->cv.za + r0, f->cv.dg + r0, st, &eu->launches));
     }
-    FCK(cudaMemcpyAsync(Zj_alpha, f->cvza, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
-    FCK(cudaMemcpyAsync(diag_ZjSinv, f->cvdg, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(Zj_alpha, f->cv.za, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(diag_ZjSinv, f->cv.dg, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     f->cv_param = param;
-    f->cv_m_ok = true;
+    f->cv.m_ok = true;
     return GPB200_OK;
 }
 
@@ -841,7 +839,7 @@ int gpb200_fitc_cv_block(gpb200_fitc* f, int32_t which, int64_t nV, const int64_
         return fail(f, GPB200_EINVAL, "fitc_cv_block: nV must lie in 1.." + std::to_string(f->Nc) + " (one staging chunk)");
     for (int64_t r = 0; r < nV; ++r)
         if (idx[r] < 0 || idx[r] >= f->N) return fail(f, GPB200_EINVAL, "fitc_cv_block: index out of range");
-    if (which == 1 && !f->cv_m_ok) return fail(f, GPB200_ESTATE, "fitc_cv_block: which = 1 needs a fitc_cv_param since the last factorize");
+    if (which == 1 && !f->cv.m_ok) return fail(f, GPB200_ESTATE, "fitc_cv_block: which = 1 needs a fitc_cv_param since the last factorize");
     FCK(cudaSetDevice(f->device));
     TRY(fitc_cv_prepare(f));
     gpb200_handle *eu = f->eu, *es = f->es;
@@ -849,39 +847,33 @@ int gpb200_fitc_cv_block(gpb200_fitc* f, int32_t which, int64_t nV, const int64_
     const int64_t Mp = f->Mpad, M = f->M;
     const int d = f->d;
     const int64_t nVp = (nV + TILE - 1) / TILE * TILE;
-    const bool tma = eu->tma_ok;
-    if (nVp > f->cvout_rows) {
-        if (f->cvout) cudaFree(f->cvout);
-        f->cvout = nullptr; f->cvout_rows = 0;
-        FCK(cudaMalloc(&f->cvout, sizeof(double) * nVp * nVp));
-        f->cvout_rows = nVp;
-    }
-    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp}, bB2{tma ? &f->mapB2 : nullptr, f->bufB, Mp};
-    GemmBuf bCh{tma ? &f->mapCvCh : nullptr, f->cvCh, Mp}, bP{tma ? &f->mapCvP : nullptr, f->cvP, Mp};
-    GemmBuf bDp{tma ? &f->mapCvDp : nullptr, f->cvDp, Mp}, bQ{tma ? &f->mapCvQ : nullptr, f->cvQ, Mp};
-    FCK(cudaMemcpyAsync(f->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, st));
-    FCK(fitc_cv_gather_launch(nV, f->cvidx, f->x, d, d, f->cvxs, f->lam, f->cvlamV, which == 1 ? f->cvdel : nullptr, f->cvdelV,
+    FCK(f->cv.out.ensure((size_t)nVp * nVp));
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp), bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, Mp);
+    const GemmBuf bCh = gbuf(eu, f->cv.Ch, f->cv.mapCh, Mp), bP = gbuf(eu, f->cv.P, f->cv.mapP, Mp);
+    const GemmBuf bDp = gbuf(eu, f->cv.Dp, f->cv.mapDp, Mp), bQ = gbuf(eu, f->cv.Q, f->cv.mapQ, Mp);
+    FCK(cudaMemcpyAsync(f->cv.idx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, st));
+    FCK(fitc_cv_gather_launch(nV, f->cv.idx, f->data.x, d, d, f->cv.xs, f->data.lam, f->cv.lamV, which == 1 ? f->cv.del.data() : nullptr, f->cv.delV,
                               st, &eu->launches));
-    FCK(crossgram_launch(eu->prog, f->cvxs, d, nV, nVp, eu->x, d, M, Mp, d, f->bufA, Mp, st, &eu->launches));   // K_V
-    FCK(gemm_whole(f->eu, bA, bufG(es), f->cvCh, Mp, nVp, Mp, Mp, 1.0, 0.0));
-    FCK(scale_launch(1, f->cvCh, Mp, nV, Mp, f->cvlamV, st, &eu->launches));                       // Ch_V
+    FCK(crossgram_launch(eu->prog, f->cv.xs, d, nV, nVp, eu->x, d, M, Mp, d, f->stage.bufA, Mp, st, &eu->launches));   // K_V
+    FCK(gemm_whole(f->eu, bA, bufG(es), f->cv.Ch, Mp, nVp, Mp, Mp, 1.0, 0.0));
+    FCK(scale_launch(1, f->cv.Ch, Mp, nV, Mp, f->cv.lamV, st, &eu->launches));                       // Ch_V
     if (which == 0) {   // Sigma^-1[V,V] = diag(1/L_V) - Ch_V (L_V^-1 K_V)'
-        FCK(cudaMemcpyAsync(f->bufB, f->bufA, sizeof(double) * nVp * Mp, cudaMemcpyDeviceToDevice, st));
-        FCK(scale_launch(1, f->bufB, Mp, nV, Mp, f->cvlamV, st, &eu->launches));
-        FCK(gemm_whole(f->eu, bCh, bB2, f->cvout, nVp, nVp, nVp, Mp, -1.0, 0.0));
+        FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * nVp * Mp, cudaMemcpyDeviceToDevice, st));
+        FCK(scale_launch(1, f->stage.bufB, Mp, nV, Mp, f->cv.lamV, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bCh, bB2, f->cv.out, nVp, nVp, nVp, Mp, -1.0, 0.0));
     } else {            // (Sigma^-1 dSigma_j Sigma^-1)[V,V] = diag(Delta_V / L_V^2) + E_V Ch_V' + Ch_V E_V'
         const bool noise = f->cv_param < 0;
         if (!noise) {
-            FCK(crossgram_grad_launch(eu->prog, f->cvxs, d, nV, nVp, eu->x, d, M, Mp, d, f->cv_param, f->cvG, Mp, st, &eu->launches));
-            FCK(gemm_whole(f->eu, bA, bDp, f->cvG, Mp, nVp, Mp, Mp, -0.5, 1.0));
+            FCK(crossgram_grad_launch(eu->prog, f->cv.xs, d, nV, nVp, eu->x, d, M, Mp, d, f->cv_param, f->cv.G, Mp, st, &eu->launches));
+            FCK(gemm_whole(f->eu, bA, bDp, f->cv.G, Mp, nVp, Mp, Mp, -0.5, 1.0));
         }
-        FCK(gemm_whole(f->eu, bCh, bQ, f->cvP, Mp, nVp, Mp, Mp, 0.5, 0.0));
-        FCK(fitc_cv_eblock_launch(f->cvP, noise ? nullptr : f->cvG, f->bufA, Mp, nV, Mp, f->cvlamV, f->cvdelV, st, &eu->launches));
-        FCK(gemm_whole(f->eu, bP, bCh, f->cvout, nVp, nVp, nVp, Mp, 1.0, 0.0));
-        FCK(gemm_whole(f->eu, bCh, bP, f->cvout, nVp, nVp, nVp, Mp, 1.0, 1.0));
+        FCK(gemm_whole(f->eu, bCh, bQ, f->cv.P, Mp, nVp, Mp, Mp, 0.5, 0.0));
+        FCK(fitc_cv_eblock_launch(f->cv.P, noise ? nullptr : f->cv.G.data(), f->stage.bufA, Mp, nV, Mp, f->cv.lamV, f->cv.delV, st, &eu->launches));
+        FCK(gemm_whole(f->eu, bP, bCh, f->cv.out, nVp, nVp, nVp, Mp, 1.0, 0.0));
+        FCK(gemm_whole(f->eu, bCh, bP, f->cv.out, nVp, nVp, nVp, Mp, 1.0, 1.0));
     }
-    FCK(fitc_cv_diag_launch(f->cvout, nVp, nV, which, f->cvlamV, f->cvdelV, st, &eu->launches));
-    FCK(cudaMemcpy2DAsync(out, sizeof(double) * nV, f->cvout, sizeof(double) * nVp, sizeof(double) * nV, nV, cudaMemcpyDeviceToHost, st));
+    FCK(fitc_cv_diag_launch(f->cv.out, nVp, nV, which, f->cv.lamV, f->cv.delV, st, &eu->launches));
+    FCK(cudaMemcpy2DAsync(out, sizeof(double) * nV, f->cv.out, sizeof(double) * nVp, sizeof(double) * nV, nV, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
@@ -919,7 +911,7 @@ int gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs,
         TRY(fitc_cov_build(f, Ms, xs, ldxs, mu_minus_mean));
         cov = f->Kss; ldc = (Ms + TILE - 1) / TILE * TILE;
     }
-    FSUB(rand_from_cov(eu, Ms, cov, ldc, f->tmpc, nsamp, z, nugget, samples), eu);
+    FSUB(rand_from_cov(eu, Ms, cov, ldc, f->stage.tmpc, nsamp, z, nugget, samples), eu);
     f->rand_ms[0] = ev_ms(ev_start, eu->ev0);
     f->rand_ms[1] = ev_ms(eu->ev0, eu->ev1);
     f->rand_ms[2] = ev_ms(eu->ev3, eu->ev2);

@@ -3,6 +3,8 @@
 // K_uu, Sigma_QR and N-chunk streaming.
 #include <limits.h>
 
+#include <memory>
+
 #include "engine.cuh"
 #include "fsa.cuh"
 #include "gram.cuh"
@@ -41,39 +43,48 @@ struct FsaChunk {
     FsaLaunch ginv, gyy, gp1t;                          // -X_r' X_c tiles ; += Y_r Y_c' ; (K_uu^-1 K_uf G_bd) (bufA, Mpad x Nc)
     FsaLaunch bdx;                                      // training-input gradient: FsaBlockDxItem list, one per tile row of a block
 };
+// first use of gpb200_fitc_predict_fsa: V* = K_*u L_uu^-T, the C / G tiles of the test rows (Nc x 2048 each) and the
+// per-row vectors
+struct FsaPredWs {
+    DevBuf<double> Vs, Cb, Gb, pvec;
+    CUtensorMap mapVs{};
+    bool ready = false;
+};
+// first use of gpb200_fitc_predict_fsa_grad with variances: the s K_ub' tiles of the test rows (Nc x 2048) and
+// Z = K_*u + E K_fu / 2 (Nc x Mpad)
+struct FsaGradWs {
+    DevBuf<double> Tb, Zb;
+    CUtensorMap mapZb{};
+    bool ready = false;
+};
+// everything gpb200_fitc_set_blocks builds; it lives until the next set_blocks or set_data (fsa_free)
 struct Fsa {
     int64_t nblocks = 0, Np = 0, n_pad = 0, packed = 0;
     int max_tiles = 0;
     std::vector<FsaChunk> chunks;
-    double *xb = nullptr, *mask = nullptr, *X = nullptr, *LT = nullptr, *logd = nullptr;
-    double *r = nullptr, *a = nullptr, *t1 = nullptr, *t2 = nullptr;
-    long long *pos = nullptr, *bstart = nullptr, *boff = nullptr;
-    long long* ipos = nullptr;                          // padded row -> caller index (-1 on padding): inverse of pos
-    FsaBlockDxItem* bdx = nullptr;
+    DevBuf<double> xb, mask, X, LT, logd;
+    DevBuf<double> r, a, t1, t2;
+    DevBuf<long long> pos, bstart, boff;
+    DevBuf<long long> ipos;                             // padded row -> caller index (-1 on padding): inverse of pos
+    DevBuf<FsaBlockDxItem> bdx;
     std::vector<long long> pos_h;                       // pos on the host: gpb200_fitc_set_inputs rebuilds xb through it
-    int *rblk = nullptr, *bsize = nullptr, *info = nullptr;
-    FsaGemmItem* gitems = nullptr;
-    Potrf128Item* litems = nullptr;
-    FsaGramItem* gramitems = nullptr;
+    DevBuf<int> rblk, bsize, info;
+    DevBuf<FsaGemmItem> gitems;
+    DevBuf<Potrf128Item> litems;
+    DevBuf<FsaGramItem> gramitems;
     CUtensorMap mapWt{};                                // bufA as Mpad x Nc (W' = K_uf L_Lambda^-T of a chunk)
-    double *Gpk = nullptr, *gpart = nullptr, *ones = nullptr;   // kernel gradient: one chunk's G_i blocks, trace partials, 1s
+    DevBuf<double> Gpk, gpart, ones;                    // kernel gradient: one chunk's G_i blocks, trace partials, 1s
     std::vector<long long> bstart_h, boff_h;
     std::vector<int> bsize_h, bchunk_h;                 // bchunk_h[b]: staging chunk of block b
-    // predictions (gpb200_fitc_predict_fsa, allocated on first use): V* = K_*u L_uu^-T, the C / G tiles of the test rows
-    // (Nc x 2048 each), the per-row vectors, and the per-call work lists
-    double *Vs = nullptr, *Cb = nullptr, *Gb = nullptr, *pvec = nullptr;
-    CUtensorMap mapVs{};
-    FsaGemmItem* pg = nullptr; FsaGramItem* px = nullptr; FsaRowItem* pr = nullptr;
-    size_t pg_cap = 0, px_cap = 0, pr_cap = 0;
+    FsaPredWs pred;
+    FsaGradWs pgrad;
+    // per-call work lists of the predictions, grown on demand
+    DevBuf<FsaGemmItem> pg; DevBuf<FsaGramItem> px; DevBuf<FsaRowItem> pr;
     // gpb200_fitc_rand: Sigma* gathered into the caller's order (Ms x Ms, dense) through the test-point permutation pp
-    double* Sc = nullptr; long long* pp = nullptr;
-    size_t Sc_cap = 0, pp_cap = 0;
-    // gpb200_fitc_predict_fsa_grad (first use): the s K_ub' tiles of the test rows (Nc x 2048), Z = K_*u + E K_fu / 2
-    // (Nc x Mpad), dmu / dvar in the caller's order (2 x Ms x d) and the contraction's items
-    double *Tb = nullptr, *Zb = nullptr, *pdx = nullptr;
-    CUtensorMap mapZb{};
-    FsaDxItem* pdi = nullptr;
-    size_t pdx_cap = 0, pdi_cap = 0;
+    DevBuf<double> Sc; DevBuf<long long> pp;
+    // gpb200_fitc_predict_fsa_grad: dmu / dvar in the caller's order (2 x Ms x d) and the contraction's items
+    DevBuf<double> pdx;
+    DevBuf<FsaDxItem> pdi;
 };
 
 extern "C" {
@@ -105,32 +116,11 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     FCK(cudaSetDevice(f->device));
     fsa_free(f);
     f->factored = f->alpha_ready = false;
-    {
-        // set_data sizes the staging chunk to N; the padded blocks and the padded test groups of FSA predictions need the
-        // full chunk, so grow it to the cap set_data applies to large N (the buffers are re-made, the gradient workspace freed)
-        const int64_t cap = std::min<int64_t>((int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE, 32768);
-        if (cap > f->Nc) {
-            double** ptrs[] = {&f->xs, &f->w, &f->tmpc, &f->zeroc, &f->tmpc2, &f->bufA, &f->bufB, &f->bufC, &f->Hbuf, &f->Wbuf,
-                               &f->Tbuf, &f->gvec, &f->betav, &f->gpart, &f->gacc, &f->gtmp, &f->pdx};
-            for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
-            f->grad_ws = false;
-            const int64_t nc = cap;
-            f->Nc = nc;
-            FCK(cudaMalloc(&f->xs, sizeof(double) * nc * f->d));
-            for (double** q : {&f->w, &f->tmpc, &f->zeroc, &f->tmpc2}) FCK(cudaMalloc(q, sizeof(double) * nc));
-            FCK(cudaMalloc(&f->bufA, sizeof(double) * nc * f->Mpad));
-            FCK(cudaMalloc(&f->bufB, sizeof(double) * nc * f->Mpad));
-            FCK(cudaMemset(f->zeroc, 0, sizeof(double) * nc));
-            if (f->eu->tma_ok) {
-                const bool ok = gemm_make_tensor_map(&f->mapA, f->bufA, nc, f->Mpad, f->Mpad) &&
-                                gemm_make_tensor_map(&f->mapB, f->bufB, f->Mpad, nc, nc) &&
-                                gemm_make_tensor_map(&f->mapB2, f->bufB, nc, f->Mpad, f->Mpad);
-                if (!ok) return fail(f, GPB200_ECUDA, "fitc_set_blocks: cuTensorMapEncodeTiled failed");
-            }
-        }
-    }
-    Fsa* s = new Fsa();
-    f->fsa = s;
+    // set_data sizes the staging chunk to N; the padded blocks and the padded test groups of FSA predictions need the
+    // full chunk, so grow it to the cap set_data applies to large N (with every workspace sized by the chunk)
+    const int64_t cap = std::min<int64_t>((int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE, 32768);
+    if (cap > f->Nc) TRY(fitc_stage_alloc(f, cap, "fitc_set_blocks"));
+    std::unique_ptr<Fsa> s(new Fsa());            // f->fsa once complete
     s->nblocks = nblocks; s->Np = Np; s->n_pad = Np - N; s->packed = packed; s->max_tiles = max_tiles;
     cudaStream_t st = f->eu->st;
     const int d = f->d;
@@ -139,7 +129,7 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     std::vector<long long> bstart((size_t)nblocks), boff((size_t)nblocks), pos((size_t)N), ipos;
     std::vector<int> bsize((size_t)nblocks), rblk((size_t)Np);
     std::vector<double> mask((size_t)Np, 0.0), xh((size_t)N * d), xb((size_t)Np * d, 0.0);
-    FCK(cudaMemcpy(xh.data(), f->x, sizeof(double) * N * d, cudaMemcpyDeviceToHost));
+    FCK(cudaMemcpy(xh.data(), f->data.x, sizeof(double) * N * d, cudaMemcpyDeviceToHost));
     {
         int64_t P = 0, off = 0;
         for (int64_t b = 0; b < nblocks; ++b) {
@@ -155,26 +145,25 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
             P += B; off += B * B;
         }
     }
-    FCK(cudaMalloc(&s->xb, sizeof(double) * Np * d));
-    for (double** p : {&s->mask, &s->logd, &s->r, &s->a, &s->t1, &s->t2}) FCK(cudaMalloc(p, sizeof(double) * Np));
-    FCK(cudaMalloc(&s->X, sizeof(double) * packed));
-    FCK(cudaMalloc(&s->LT, sizeof(double) * packed));
+    FCK(s->xb.alloc((size_t)Np * d));
+    for (DevBuf<double>* p : {&s->mask, &s->logd, &s->r, &s->a, &s->t1, &s->t2}) FCK(p->alloc(Np));
+    FCK(s->X.alloc(packed));
+    FCK(s->LT.alloc(packed));
     FCK(cudaMemsetAsync(s->X, 0, sizeof(double) * packed, st));
     FCK(cudaMemsetAsync(s->LT, 0, sizeof(double) * packed, st));
-    FCK(cudaMalloc(&s->pos, sizeof(long long) * N));
-    FCK(cudaMalloc(&s->ipos, sizeof(long long) * Np));
-    FCK(cudaMalloc(&s->bstart, sizeof(long long) * nblocks));
-    FCK(cudaMalloc(&s->boff, sizeof(long long) * nblocks));
-    FCK(cudaMalloc(&s->bsize, sizeof(int) * nblocks));
-    FCK(cudaMalloc(&s->rblk, sizeof(int) * Np));
-    FCK(cudaMalloc(&s->info, sizeof(int)));
+    FCK(s->pos.alloc(N));
+    FCK(s->ipos.alloc(Np));
+    FCK(s->bstart.alloc(nblocks));
+    FCK(s->boff.alloc(nblocks));
+    FCK(s->bsize.alloc(nblocks));
+    FCK(s->rblk.alloc(Np));
+    FCK(s->info.alloc(1));
     // a chunk holds sum B_i <= Nc rows of blocks of at most 2048 rows: its blocks' G_i take at most Nc * 2048 doubles
-    const int64_t gpk_elems = std::min<int64_t>(packed, Nc * FSA_MAX_BLOCK);
-    FCK(cudaMalloc(&s->Gpk, sizeof(double) * gpk_elems));
-    FCK(cudaMalloc(&s->gpart, sizeof(double) * (Nc / TILE) * (FSA_MAX_BLOCK / TILE) * GPB200_MAX_THETA));
+    FCK(s->Gpk.alloc(std::min<int64_t>(packed, Nc * FSA_MAX_BLOCK)));
+    FCK(s->gpart.alloc((size_t)(Nc / TILE) * (FSA_MAX_BLOCK / TILE) * GPB200_MAX_THETA));
     {
         std::vector<double> ones((size_t)Nc, 1.0);
-        FCK(cudaMalloc(&s->ones, sizeof(double) * Nc));
+        FCK(s->ones.alloc(Nc));
         FCK(cudaMemcpy(s->ones, ones.data(), sizeof(double) * Nc, cudaMemcpyHostToDevice));
     }
     FCK(cudaMemcpy(s->xb, xb.data(), sizeof(double) * Np * d, cudaMemcpyHostToDevice));
@@ -187,7 +176,7 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     FCK(cudaMemcpy(s->boff, boff.data(), sizeof(long long) * nblocks, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->bsize, bsize.data(), sizeof(int) * nblocks, cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->rblk, rblk.data(), sizeof(int) * Np, cudaMemcpyHostToDevice));
-    if (f->eu->tma_ok && !gemm_make_tensor_map(&s->mapWt, f->bufA, Mp, Nc, Nc)) {
+    if (f->eu->tma_ok && !gemm_make_tensor_map(&s->mapWt, f->stage.bufA, Mp, Nc, Nc)) {
         return fail(f, GPB200_ECUDA, "fitc_set_blocks: cuTensorMapEncodeTiled failed");
     }
     s->bstart_h = bstart; s->boff_h = boff; s->bsize_h = bsize; s->pos_h = pos;
@@ -224,8 +213,8 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
                     FsaGramItem g{};
                     g.dst = Xt(b, i, j); g.ld = bsize[b]; g.row_i = bstart[b] + i * TILE; g.row_j = bstart[b] + j * TILE; g.diag = (i == j);
                     gr.push_back(g);
-                    gemm(Xt(b, i, j), bsize[b], f->bufA + (bstart[b] - ch.r0 + i * TILE) * Mp, Mp,
-                         f->bufA + (bstart[b] - ch.r0 + j * TILE) * Mp, Mp, Mp, -1.0, 1.0, i == j);
+                    gemm(Xt(b, i, j), bsize[b], f->stage.bufA + (bstart[b] - ch.r0 + i * TILE) * Mp, Mp,
+                         f->stage.bufA + (bstart[b] - ch.r0 + j * TILE) * Mp, Mp, Mp, -1.0, 1.0, i == j);
                 }
         }
         ch.gram.n = (int)((int64_t)gr.size() - ch.gram.off);
@@ -273,15 +262,15 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
         for (int64_t b = b0; b < b1; ++b)
             for (int64_t u = 0; u < Mp / TILE; ++u)
                 for (int r = 0; r < bsize[b] / TILE; ++r)
-                    gemm(f->bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, f->bufB + u * TILE * Nc + (bstart[b] - ch.r0), Nc,
+                    gemm(f->stage.bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, f->stage.bufB + u * TILE * Nc + (bstart[b] - ch.r0), Nc,
                          Xt(b, r, 0), bsize[b], (int64_t)(r + 1) * TILE, 1.0, 0.0, false);
         close_g(ch.wt);
         open_g(ch.z);
         for (int64_t b = b0; b < b1; ++b)
             for (int64_t u = 0; u < Mp / TILE; ++u)
                 for (int r = 0; r < bsize[b] / TILE; ++r)
-                    gemm(f->bufB + (bstart[b] - ch.r0 + r * TILE) * Mp + u * TILE, Mp, Lt(b, r, r), bsize[b],
-                         f->bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, bsize[b] - (int64_t)r * TILE, 1.0, 0.0, false);
+                    gemm(f->stage.bufB + (bstart[b] - ch.r0 + r * TILE) * Mp + u * TILE, Mp, Lt(b, r, r), bsize[b],
+                         f->stage.bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, bsize[b] - (int64_t)r * TILE, 1.0, 0.0, false);
         close_g(ch.z);
         // kernel gradient: every tile of G_i (full, G is symmetric), in Gpk at the block's offset within the chunk
         auto Gt = [&](int64_t b, int i, int j) { return s->Gpk + (boff[b] - boff[b0]) + (int64_t)i * TILE * bsize[b] + (int64_t)j * TILE; };
@@ -306,14 +295,14 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
         for (int64_t b = b0; b < b1; ++b)
             for (int i = 0; i < bsize[b] / TILE; ++i)
                 for (int j = 0; j < bsize[b] / TILE; ++j)
-                    gemm(Gt(b, i, j), bsize[b], f->bufB + (bstart[b] - ch.r0 + i * TILE) * Mp, Mp,
-                         f->bufB + (bstart[b] - ch.r0 + j * TILE) * Mp, Mp, Mp, 1.0, 1.0, false);
+                    gemm(Gt(b, i, j), bsize[b], f->stage.bufB + (bstart[b] - ch.r0 + i * TILE) * Mp, Mp,
+                         f->stage.bufB + (bstart[b] - ch.r0 + j * TILE) * Mp, Mp, Mp, 1.0, 1.0, false);
         close_g(ch.gyy);
         open_g(ch.gp1t);                                // (P1' G_bd) with P1' = K_uu^-1 K_uf in bufB (Mpad x Nc) -> bufA (Mpad x Nc)
         for (int64_t b = b0; b < b1; ++b)
             for (int64_t u = 0; u < Mp / TILE; ++u)
                 for (int r = 0; r < bsize[b] / TILE; ++r)
-                    gemm(f->bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, f->bufB + u * TILE * Nc + (bstart[b] - ch.r0), Nc,
+                    gemm(f->stage.bufA + u * TILE * Nc + (bstart[b] - ch.r0) + r * TILE, Nc, f->stage.bufB + u * TILE * Nc + (bstart[b] - ch.r0), Nc,
                          Gt(b, r, 0), bsize[b], bsize[b], 1.0, 0.0, false);
         close_g(ch.gp1t);
         ch.bdx.off = (int64_t)bd.size();                // the real tile rows of every block, G_b in Gpk as above
@@ -326,15 +315,16 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
         s->chunks.push_back(std::move(ch));
         b0 = b1;
     }
-    FCK(cudaMalloc(&s->gitems, sizeof(FsaGemmItem) * std::max<size_t>(gi.size(), 1)));
-    FCK(cudaMalloc(&s->litems, sizeof(Potrf128Item) * std::max<size_t>(li.size(), 1)));
-    FCK(cudaMalloc(&s->gramitems, sizeof(FsaGramItem) * std::max<size_t>(gr.size(), 1)));
+    FCK(s->gitems.alloc(std::max<size_t>(gi.size(), 1)));
+    FCK(s->litems.alloc(std::max<size_t>(li.size(), 1)));
+    FCK(s->gramitems.alloc(std::max<size_t>(gr.size(), 1)));
     FCK(cudaMemcpy(s->gitems, gi.data(), sizeof(FsaGemmItem) * gi.size(), cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->litems, li.data(), sizeof(Potrf128Item) * li.size(), cudaMemcpyHostToDevice));
     FCK(cudaMemcpy(s->gramitems, gr.data(), sizeof(FsaGramItem) * gr.size(), cudaMemcpyHostToDevice));
-    FCK(cudaMalloc(&s->bdx, sizeof(FsaBlockDxItem) * std::max<size_t>(bd.size(), 1)));
+    FCK(s->bdx.alloc(std::max<size_t>(bd.size(), 1)));
     FCK(cudaMemcpy(s->bdx, bd.data(), sizeof(FsaBlockDxItem) * bd.size(), cudaMemcpyHostToDevice));
     FCK(cudaStreamSynchronize(st));
+    f->fsa = s.release();
     return GPB200_OK;
 }
 }  // extern "C"
@@ -345,13 +335,7 @@ size_t fsa_num_chunks(const gpb200_fitc* f) { return f->fsa ? f->fsa->chunks.siz
 const double* fsa_cov(const gpb200_fitc* f) { return f->fsa->Sc; }
 
 void fsa_free(gpb200_fitc* f) {
-    if (!f->fsa) return;
-    Fsa* s = f->fsa;
-    void* ptrs[] = {s->xb, s->mask, s->X, s->LT, s->logd, s->r, s->a, s->t1, s->t2, s->pos, s->bstart, s->boff,
-                    s->rblk, s->bsize, s->info, s->gitems, s->litems, s->gramitems, s->Gpk, s->gpart, s->ones,
-                    s->Vs, s->Cb, s->Gb, s->pvec, s->pg, s->px, s->pr, s->Sc, s->pp, s->Tb, s->Zb, s->pdx, s->pdi, s->ipos, s->bdx};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    delete s;
+    delete f->fsa;
     f->fsa = nullptr;
 }
 
@@ -369,13 +353,13 @@ int fsa_factorize(gpb200_fitc* f) {
     const int64_t Mp = f->Mpad, Nc = f->Nc;
     const int init = INT_MAX;
     FCK(cudaMemcpyAsync(s->info, &init, sizeof(int), cudaMemcpyHostToDevice, st));
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, Mp};
-    GemmBuf bWt{eu->tma_ok ? &s->mapWt : nullptr, f->bufA, Nc};
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp);
+    const GemmBuf bWt = gbuf(eu, f->stage.bufA, s->mapWt, Nc);
     for (const FsaChunk& ch : s->chunks) {
         const double* xr = s->xb + ch.r0 * f->d;
         // V = K_fu L_uu^-T (padding rows zero), then Lambda_i = K_ii + (sigma^2 + 1e-10) I - V_i V_i'
         FCK(fitc_kfu(f, xr, ch.rows));
-        FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
+        FCK(fsa_mask_launch(f->stage.bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
         FCK(trsm_rec_buf(eu, bA, (int)Nc, 0, (int)Mp));
         FCK(fsa_gram_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gram.off, ch.gram.n, s->mask, f->noise_var + 1e-10, st, &eu->launches));
         FCK(fsa_gemm_launch(s->gitems + ch.vv.off, ch.vv.n, st, &eu->launches));
@@ -389,7 +373,7 @@ int fsa_factorize(gpb200_fitc* f) {
         }
         // W' = K_uf L_Lambda^-T, Sigma_QR += W' W
         FCK(fitc_kuf(f, xr, ch.rows));
-        FCK(fsa_mask_launch(f->bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+        FCK(fsa_mask_launch(f->stage.bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
         FCK(fsa_gemm_launch(s->gitems + ch.wt.off, ch.wt.n, st, &eu->launches));
         FCK(gemm_whole(es, bWt, bWt, es->G, es->ld, Mp, Mp, ch.rows, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
     }
@@ -411,34 +395,34 @@ int fsa_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, double* m
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Np = s->Np, Mp = f->Mpad;
-    FCK(cudaMemcpyAsync(f->y, y_minus_mean, sizeof(double) * f->N, cudaMemcpyHostToDevice, st));
+    FCK(cudaMemcpyAsync(f->data.y, y_minus_mean, sizeof(double) * f->N, cudaMemcpyHostToDevice, st));
     FCK(cudaMemsetAsync(s->r, 0, sizeof(double) * Np, st));
-    FCK(fsa_permute_launch(1, f->y, s->pos, f->N, s->r, st, &eu->launches));
+    FCK(fsa_permute_launch(1, f->data.y, s->pos, f->N, s->r, st, &eu->launches));
     FCK(fsa_bdmv_launch(0, s->X, s->rblk, s->bstart, s->bsize, s->boff, s->r, s->t1, Np, st, &eu->launches));
     FCK(fsa_bdmv_launch(1, s->LT, s->rblk, s->bstart, s->bsize, s->boff, s->t1, s->t2, Np, st, &eu->launches));     // t2 = Lambda^-1 r
-    FCK(cudaMemsetAsync(f->bvec, 0, sizeof(double) * Mp, st));
+    FCK(cudaMemsetAsync(f->data.bvec, 0, sizeof(double) * Mp, st));
     for (const FsaChunk& ch : s->chunks) {
         FCK(fitc_kuf(f, s->xb + ch.r0 * f->d, ch.rows));
-        FCK(rowdot_launch(f->bufB, f->Nc, s->t2 + ch.r0, f->M, ch.rows, f->tmpm, st, &eu->launches));
-        FCK(ew_launch(2, f->M, f->bvec, f->tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(rowdot_launch(f->stage.bufB, f->Nc, s->t2 + ch.r0, f->M, ch.rows, f->data.tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->data.bvec, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
     }
-    FCK(cudaMemcpyAsync(f->rhsm, f->bvec, sizeof(double) * Mp, cudaMemcpyDeviceToDevice, st));
-    FCK(solve_device(es, f->rhsm, f->tmpm, f->uvec));
+    FCK(cudaMemcpyAsync(f->data.rhsm, f->data.bvec, sizeof(double) * Mp, cudaMemcpyDeviceToDevice, st));
+    FCK(solve_device(es, f->data.rhsm, f->data.tmpm, f->data.uvec));
     for (const FsaChunk& ch : s->chunks) {
         FCK(fitc_kfu(f, s->xb + ch.r0 * f->d, ch.rows));
-        FCK(rowdot_launch(f->bufA, Mp, f->uvec, ch.rows, Mp, s->t1 + ch.r0, st, &eu->launches));
+        FCK(rowdot_launch(f->stage.bufA, Mp, f->data.uvec, ch.rows, Mp, s->t1 + ch.r0, st, &eu->launches));
     }
     FCK(fsa_resid_launch(s->t1, s->r, s->t1, s->mask, Np, st, &eu->launches));                                      // r - K_fu u, padding 0
     FCK(fsa_bdmv_launch(0, s->X, s->rblk, s->bstart, s->bsize, s->boff, s->t1, s->t2, Np, st, &eu->launches));
     FCK(fsa_bdmv_launch(1, s->LT, s->rblk, s->bstart, s->bsize, s->boff, s->t2, s->a, Np, st, &eu->launches));      // alpha (padded order)
-    FCK(fsa_permute_launch(0, s->a, s->pos, f->N, f->alpha, st, &eu->launches));
-    FCK(dot_launch(s->r, s->a, Np, f->scal + 0, st, &eu->launches));
-    FCK(sum_launch(es->logd, es->Npad, f->scal + 1, st, &eu->launches));
-    FCK(sum_launch(eu->logd, eu->Npad, f->scal + 2, st, &eu->launches));
-    FCK(sum_launch(s->logd, Np, f->scal + 3, st, &eu->launches));
+    FCK(fsa_permute_launch(0, s->a, s->pos, f->N, f->data.alpha, st, &eu->launches));
+    FCK(dot_launch(s->r, s->a, Np, f->data.scal + 0, st, &eu->launches));
+    FCK(sum_launch(es->logd, es->Npad, f->data.scal + 1, st, &eu->launches));
+    FCK(sum_launch(eu->logd, eu->Npad, f->data.scal + 2, st, &eu->launches));
+    FCK(sum_launch(s->logd, Np, f->data.scal + 3, st, &eu->launches));
     double sc[4];
-    FCK(cudaMemcpyAsync(sc, f->scal, sizeof(double) * 4, cudaMemcpyDeviceToHost, st));
-    if (alpha) FCK(cudaMemcpyAsync(alpha, f->alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(sc, f->data.scal, sizeof(double) * 4, cudaMemcpyDeviceToHost, st));
+    if (alpha) FCK(cudaMemcpyAsync(alpha, f->data.alpha, sizeof(double) * f->N, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(es), es);                                   // the solve for u above
     f->Ntotal = (double)f->N;
@@ -456,21 +440,21 @@ int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Np = s->Np, Mp = f->Mpad, Nc = f->Nc;
-    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, Mp};
+    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, Mp);
     for (const FsaChunk& ch : s->chunks) {
         FCK(fitc_kuf(f, s->xb + ch.r0 * f->d, ch.rows));
-        FCK(fsa_mask_launch(f->bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+        FCK(fsa_mask_launch(f->stage.bufB, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
         FCK(fsa_gemm_launch(s->gitems + ch.wt.off, ch.wt.n, st, &eu->launches));  // W' = K_uf X'               (bufA, Mpad x Nc)
         FCK(fsa_gemm_launch(s->gitems + ch.z.off, ch.z.n, st, &eu->launches));    // Z = X' W = Lambda^-1 K_fu  (bufB, Nc x Mpad)
         FCK(trsm_rec_buf(es, bB2, (int)ch.rows, 0, (int)Mp));                 // Y = Z L_s^-T
-        FCK(rowvar_launch(f->bufB, Mp, f->zeroc, ch.rows, Mp, s->t1 + ch.r0, st, &eu->launches));   // -|Y_r|^2
+        FCK(rowvar_launch(f->stage.bufB, Mp, f->stage.zeroc, ch.rows, Mp, s->t1 + ch.r0, st, &eu->launches));   // -|Y_r|^2
     }
-    FCK(sum_launch(s->t1, Np, f->scal + 0, st, &eu->launches));
-    FCK(dot_launch(s->a, s->a, Np, f->scal + 1, st, &eu->launches));
+    FCK(sum_launch(s->t1, Np, f->data.scal + 0, st, &eu->launches));
+    FCK(dot_launch(s->a, s->a, Np, f->data.scal + 1, st, &eu->launches));
     FCK(fsa_bdmv_launch(2, s->X, s->rblk, s->bstart, s->bsize, s->boff, nullptr, s->t2, Np, st, &eu->launches));
-    FCK(sum_launch(s->t2, Np, f->scal + 2, st, &eu->launches));
+    FCK(sum_launch(s->t2, Np, f->data.scal + 2, st, &eu->launches));
     double sc[3];
-    FCK(cudaMemcpyAsync(sc, f->scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(sc, f->data.scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     *dmll_noise = f->noise_var * (sc[1] - (sc[2] - (double)s->n_pad) - sc[0]);
     return GPB200_OK;
@@ -490,27 +474,26 @@ int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double
     cudaStream_t st = eu->st;
     const int np = eu->prog.n_theta;
     const int64_t Mp = f->Mpad, Nc = f->Nc;
-    const bool tma = eu->tma_ok;
-    GemmBuf bA{tma ? &f->mapA : nullptr, f->bufA, Mp};          // bufA as Nc x Mpad
-    GemmBuf bAt{tma ? &s->mapWt : nullptr, f->bufA, Nc};        // bufA as Mpad x Nc
-    GemmBuf bB2{tma ? &f->mapB2 : nullptr, f->bufB, Mp};        // bufB as Nc x Mpad
-    GemmBuf bBt{tma ? &f->mapB : nullptr, f->bufB, Nc};         // bufB as Mpad x Nc
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp);          // bufA as Nc x Mpad
+    const GemmBuf bAt = gbuf(eu, f->stage.bufA, s->mapWt, Nc);        // bufA as Mpad x Nc
+    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, Mp);        // bufB as Nc x Mpad
+    const GemmBuf bBt = gbuf(eu, f->stage.bufB, f->stage.mapB, Nc);         // bufB as Mpad x Nc
     size_t xk = 0, rk = 0;                                        // inducing-point / training-input contractions so far
     for (const FsaChunk& ch : s->chunks) {
         const double* xr = s->xb + ch.r0 * f->d;
         const int64_t nc = ch.rows;
         FCK(fitc_kuf(f, xr, nc));
-        FCK(fsa_mask_launch(f->bufB, Nc, Mp, nc, nullptr, s->mask + ch.r0, st, &eu->launches));
+        FCK(fsa_mask_launch(f->stage.bufB, Nc, Mp, nc, nullptr, s->mask + ch.r0, st, &eu->launches));
         FCK(fsa_gemm_launch(s->gitems + ch.wt.off, ch.wt.n, st, &eu->launches));  // W' = K_uf X'                   (bufA, Mpad x Nc)
         FCK(fsa_gemm_launch(s->gitems + ch.z.off, ch.z.n, st, &eu->launches));    // Z = Lambda^-1 K_fu             (bufB, Nc x Mpad)
-        FCK(gemm_whole(es, bB2, bufG(es), f->bufC, Mp, nc, Mp, Mp, 1.0, 0.0));  // P2 = Z S^-1 -> bufC
+        FCK(gemm_whole(es, bB2, bufG(es), f->grad.bufC, Mp, nc, Mp, Mp, 1.0, 0.0));  // P2 = Z S^-1 -> bufC
         FCK(trsm_rec_buf(es, bB2, (int)nc, 0, (int)Mp));       // Y = Z L_s^-T                   (bufB)
         // G_i = -Lambda_i^-1 + Y_i Y_i' + alpha_i alpha_i'  (Gpk), then sum_i <G_i, dK_ii/dθ_p>
         FCK(fsa_gemm_launch(s->gitems + ch.ginv.off, ch.ginv.n, st, &eu->launches));
         FCK(fsa_gemm_launch(s->gitems + ch.gyy.off, ch.gyy.n, st, &eu->launches));
         FCK(fsa_outer_launch(s->gramitems + ch.gtiles.off, ch.gtiles.n, s->a, st, &eu->launches));
-        FCK(fsa_trace_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gtiles.off, ch.gtiles.n, s->mask, s->gpart, f->gtmp, st, &eu->launches));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(fsa_trace_launch(eu->prog, s->xb, f->d, s->gramitems + ch.gtiles.off, ch.gtiles.n, s->mask, s->gpart, f->grad.gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->grad.gacc, f->grad.gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         if (dmll_x) {                                               // the G_b part of dmll/dX, written in the caller's order
             ++rk;
             FCK(cudaEventRecord(f->x_ev[2 * rk], st));
@@ -519,29 +502,29 @@ int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double
         }
         // P1' = K_uu^-1 K_uf (bufB, Mpad x Nc) from K_fu (bufA)
         FCK(fitc_kfu(f, xr, nc));
-        FCK(fsa_mask_launch(f->bufA, Mp, nc, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
-        FCK(gemm_whole(eu, bufG(eu), bA, f->bufB, Nc, Mp, nc, Mp, 1.0, 0.0));
+        FCK(fsa_mask_launch(f->stage.bufA, Mp, nc, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
+        FCK(gemm_whole(eu, bufG(eu), bA, f->stage.bufB, Nc, Mp, nc, Mp, 1.0, 0.0));
         // W_fu = 2 alpha beta' - 2 P2 - 2 G_bd P1  (bufC); P1' G_bd -> bufA (Mpad x Nc)
-        FCK(fitc_wfu_launch(f->bufC, f->bufA, Mp, nc, f->M, s->a + ch.r0, s->ones, f->zeroc, f->betav, st, &eu->launches));   // g = 0: P1 unused
+        FCK(fitc_wfu_launch(f->grad.bufC, f->stage.bufA, Mp, nc, f->M, s->a + ch.r0, s->ones, f->stage.zeroc, f->grad.betav, st, &eu->launches));   // g = 0: P1 unused
         FCK(fsa_gemm_launch(s->gitems + ch.gp1t.off, ch.gp1t.n, st, &eu->launches));
-        FCK(fsa_axpy_t_launch(f->bufC, Mp, f->bufA, Nc, nc, Mp, -2.0, st, &eu->launches));
-        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->bufC, Mp, f->gpart, f->gtmp, st, &eu->launches));
-        FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(fsa_axpy_t_launch(f->grad.bufC, Mp, f->stage.bufA, Nc, nc, Mp, -2.0, st, &eu->launches));
+        FCK(trace_rect_launch(eu->prog, xr, f->d, nc, eu->x, f->d, f->M, f->d, f->grad.bufC, Mp, f->grad.gpart, f->grad.gtmp, st, &eu->launches));
+        FCK(ew_launch(2, np, f->grad.gacc, f->grad.gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
         // dmll/dXu: the padding rows of the chunk are skipped (mask 0); Xu is in the caller's order (never permuted)
-        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->bufC, 0, s->mask + ch.r0, xk > 0)); ++xk; }
-        if (dmll_x) { TRY(x_rows(f, rk + 1, xr, nc, f->bufC, nullptr, s->mask + ch.r0, s->ipos + ch.r0, f->dx, 1)); ++rk; }
-        FCK(gemm_whole(eu, bBt, bAt, f->Hbuf, Mp, Mp, Mp, nc, 1.0, 1.0));   // H += P1' G_bd P1 = K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
+        if (dmll_xu) { TRY(xu_contract(f, xk + 1, xr, nc, f->grad.bufC, 0, s->mask + ch.r0, xk > 0)); ++xk; }
+        if (dmll_x) { TRY(x_rows(f, rk + 1, xr, nc, f->grad.bufC, nullptr, s->mask + ch.r0, s->ipos + ch.r0, f->dx, 1)); ++rk; }
+        FCK(gemm_whole(eu, bBt, bAt, f->grad.Hbuf, Mp, Mp, Mp, nc, 1.0, 1.0));   // H += P1' G_bd P1 = K_uu^-1 (K_uf G_bd K_fu) K_uu^-1
     }
-    FCK(fitc_wuu_launch(f->Wbuf, f->Hbuf, eu->G, es->G, Mp, f->M, f->betav, st, &eu->launches));
-    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->Wbuf, Mp, f->gpart, f->gtmp, st, &eu->launches));
-    FCK(ew_launch(2, np, f->gacc, f->gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
+    FCK(fitc_wuu_launch(f->grad.Wbuf, f->grad.Hbuf, eu->G, es->G, Mp, f->M, f->grad.betav, st, &eu->launches));
+    FCK(trace_rect_launch(eu->prog, eu->x, f->d, f->M, eu->x, f->d, f->M, f->d, f->grad.Wbuf, Mp, f->grad.gpart, f->grad.gtmp, st, &eu->launches));
+    FCK(ew_launch(2, np, f->grad.gacc, f->grad.gtmp, nullptr, nullptr, 0.0, st, &eu->launches));
     if (dmll_xu) {
-        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->Wbuf, 1, nullptr, xk > 0)); ++xk;
+        TRY(xu_contract(f, xk + 1, eu->x, f->M, f->grad.Wbuf, 1, nullptr, xk > 0)); ++xk;
         FCK(cudaEventRecord(f->xu_ev[1], st));
     }
     if (dmll_x) FCK(cudaEventRecord(f->x_ev[1], st));
     std::vector<double> out((size_t)std::max(np, 1));
-    FCK(cudaMemcpyAsync(out.data(), f->gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
+    FCK(cudaMemcpyAsync(out.data(), f->grad.gacc, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
     FCK(cudaStreamSynchronize(st));
     FSUB(check_trsv_watchdog(eu), eu);                                   // the solve for beta in gpb200_fitc_grad_kernel
     if (dmll_kernel) for (int p = 0; p < np; ++p) dmll_kernel[p] = 0.5 * out[p];
@@ -607,12 +590,7 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
         Msp += tiles * TILE;
     }
     if (cov && Msp > Nc) return fail(f, GPB200_EINVAL, "fitc_predict_fsa: cov needs the padded test blocks in one staging chunk");
-    if (cov && Msp > f->Kss_rows) {
-        if (f->Kss) cudaFree(f->Kss);
-        f->Kss = nullptr; f->Kss_rows = 0;
-        FCK(cudaMalloc(&f->Kss, sizeof(double) * Msp * Msp));
-        f->Kss_rows = Msp;
-    }
+    if (cov) FCK(f->Kss.ensure((size_t)Msp * Msp));
     std::vector<int64_t> ppos((size_t)Ms);
     std::vector<double> xsp((size_t)Msp * d, 0.0);
     for (int64_t i = 0; i < Ms; ++i) {
@@ -620,30 +598,31 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
         ppos[(size_t)i] = r;
         for (int q = 0; q < d; ++q) xsp[(size_t)r * d + q] = xs[i * ldxs + q];
     }
-    if (!s->Vs) {
-        FCK(cudaMalloc(&s->Vs, sizeof(double) * Nc * Mp));
-        FCK(cudaMalloc(&s->Cb, sizeof(double) * Nc * LDC));
-        FCK(cudaMalloc(&s->Gb, sizeof(double) * Nc * LDC));
-        FCK(cudaMalloc(&s->pvec, sizeof(double) * Nc * 6));
-        if (eu->tma_ok && !gemm_make_tensor_map(&s->mapVs, s->Vs, Nc, Mp, Mp)) {
+    if (!s->pred.ready) TRY(make_group(s->pred, [&] {
+        FsaPredWs& g = s->pred;
+        FCK(g.Vs.alloc((size_t)Nc * Mp));
+        FCK(g.Cb.alloc((size_t)Nc * LDC));
+        FCK(g.Gb.alloc((size_t)Nc * LDC));
+        FCK(g.pvec.alloc((size_t)Nc * 6));
+        if (eu->tma_ok && !gemm_make_tensor_map(&g.mapVs, g.Vs, Nc, Mp, Mp)) {
             return fail(f, GPB200_ECUDA, "fitc_predict_fsa: cuTensorMapEncodeTiled failed");
         }
-    }
+        g.ready = true;
+        return GPB200_OK;
+    }));
     const bool grad = dmu != nullptr, gvar = grad && var;
-    if (gvar && !s->Zb) {
-        FCK(cudaMalloc(&s->Tb, sizeof(double) * Nc * LDC));
-        FCK(cudaMalloc(&s->Zb, sizeof(double) * Nc * Mp));
-        if (eu->tma_ok && !gemm_make_tensor_map(&s->mapZb, s->Zb, Nc, Mp, Mp)) {
+    if (gvar && !s->pgrad.ready) TRY(make_group(s->pgrad, [&] {
+        FsaGradWs& g = s->pgrad;
+        FCK(g.Tb.alloc((size_t)Nc * LDC));
+        FCK(g.Zb.alloc((size_t)Nc * Mp));
+        if (eu->tma_ok && !gemm_make_tensor_map(&g.mapZb, g.Zb, Nc, Mp, Mp)) {
             return fail(f, GPB200_ECUDA, "fitc_predict_fsa_grad: cuTensorMapEncodeTiled failed");
         }
-    }
-    if (grad && (size_t)(2 * Ms * d) > s->pdx_cap) {
-        if (s->pdx) cudaFree(s->pdx);
-        s->pdx = nullptr; s->pdx_cap = 0;
-        FCK(cudaMalloc(&s->pdx, sizeof(double) * 2 * Ms * d));
-        s->pdx_cap = (size_t)(2 * Ms * d);
-    }
-    double *mu1 = s->pvec, *mu2 = mu1 + Nc, *q = mu2 + Nc, *g2 = q + Nc, *r2 = g2 + Nc, *vp = r2 + Nc;
+        g.ready = true;
+        return GPB200_OK;
+    }));
+    if (grad) FCK(s->pdx.ensure((size_t)2 * Ms * d));
+    double *mu1 = s->pred.pvec, *mu2 = mu1 + Nc, *q = mu2 + Nc, *g2 = q + Nc, *r2 = g2 + Nc, *vp = r2 + Nc;
     // work lists of every (test chunk, training chunk) pair; t1 .. ak: the gradient's second sweep
     struct Pass { int chunk; FsaLaunch xg, vv, gg, hh, kh; FsaLaunch mu2, g2; FsaLaunch t1, tx, ee, ek, ak; };
     struct Sub { int64_t t0, t1; std::vector<Pass> passes; FsaLaunch ggt, dx; };
@@ -677,7 +656,7 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
             each([&](int64_t b, int64_t tl) {
                 for (int c = 0; c < s->bsize_h[(size_t)b] / TILE; ++c) {
                     FsaGramItem g{};
-                    g.dst = s->Cb + tl * TILE * LDC + c * TILE; g.ld = LDC; g.row_i = tl * TILE; g.row_j = s->bstart_h[(size_t)b] + c * TILE;
+                    g.dst = s->pred.Cb + tl * TILE * LDC + c * TILE; g.ld = LDC; g.row_i = tl * TILE; g.row_j = s->bstart_h[(size_t)b] + c * TILE;
                     xi.push_back(g);
                 }
             });
@@ -685,14 +664,14 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
             ps.vv.off = (int64_t)gi.size();                     // C -= V_* V_b'
             each([&](int64_t b, int64_t tl) {
                 for (int c = 0; c < s->bsize_h[(size_t)b] / TILE; ++c)
-                    gemm(s->Cb + tl * TILE * LDC + c * TILE, LDC, s->Vs + tl * TILE * Mp, Mp,
-                         f->bufA + (s->bstart_h[(size_t)b] - ch.r0 + c * TILE) * Mp, Mp, Mp, -1.0, 1.0);
+                    gemm(s->pred.Cb + tl * TILE * LDC + c * TILE, LDC, s->pred.Vs + tl * TILE * Mp, Mp,
+                         f->stage.bufA + (s->bstart_h[(size_t)b] - ch.r0 + c * TILE) * Mp, Mp, Mp, -1.0, 1.0);
             });
             ps.vv.n = (int)((int64_t)gi.size() - ps.vv.off);
             ps.mu2.off = (int64_t)ri.size();                    // C alpha
             each([&](int64_t b, int64_t tl) {
                 FsaRowItem r{};
-                r.A = s->Cb + tl * TILE * LDC; r.lda = LDC; r.v = s->a + s->bstart_h[(size_t)b]; r.out = mu2 + tl * TILE;
+                r.A = s->pred.Cb + tl * TILE * LDC; r.lda = LDC; r.v = s->a + s->bstart_h[(size_t)b]; r.out = mu2 + tl * TILE;
                 r.K = s->bsize_h[(size_t)b]; r.sq = 0;
                 ri.push_back(r);
             });
@@ -701,14 +680,14 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
             each([&](int64_t b, int64_t tl) {
                 const int B = s->bsize_h[(size_t)b];
                 for (int c = 0; c < B / TILE; ++c)
-                    gemm(s->Gb + tl * TILE * LDC + c * TILE, LDC, s->Cb + tl * TILE * LDC, LDC,
+                    gemm(s->pred.Gb + tl * TILE * LDC + c * TILE, LDC, s->pred.Cb + tl * TILE * LDC, LDC,
                          s->X + s->boff_h[(size_t)b] + (int64_t)c * TILE * B, B, (int64_t)(c + 1) * TILE, 1.0, 0.0);
             });
             ps.gg.n = (int)((int64_t)gi.size() - ps.gg.off);
             ps.g2.off = (int64_t)ri.size();                     // |G|^2
             each([&](int64_t b, int64_t tl) {
                 FsaRowItem r{};
-                r.A = s->Gb + tl * TILE * LDC; r.lda = LDC; r.v = nullptr; r.out = g2 + tl * TILE; r.K = s->bsize_h[(size_t)b]; r.sq = 1;
+                r.A = s->pred.Gb + tl * TILE * LDC; r.lda = LDC; r.v = nullptr; r.out = g2 + tl * TILE; r.K = s->bsize_h[(size_t)b]; r.sq = 1;
                 ri.push_back(r);
             });
             ps.g2.n = (int)((int64_t)ri.size() - ps.g2.off);
@@ -716,30 +695,30 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
             each([&](int64_t b, int64_t tl) {
                 const int B = s->bsize_h[(size_t)b];
                 for (int c = 0; c < B / TILE; ++c)
-                    gemm(s->Cb + tl * TILE * LDC + c * TILE, LDC, s->Gb + tl * TILE * LDC + c * TILE, LDC,
+                    gemm(s->pred.Cb + tl * TILE * LDC + c * TILE, LDC, s->pred.Gb + tl * TILE * LDC + c * TILE, LDC,
                          s->LT + s->boff_h[(size_t)b] + (int64_t)c * TILE * B + c * TILE, B, B - (int64_t)c * TILE, 1.0, 0.0);
             });
             ps.hh.n = (int)((int64_t)gi.size() - ps.hh.off);
             ps.kh.off = (int64_t)gi.size();                     // K_*u -= H K_fu  (= G W)
             each([&](int64_t b, int64_t tl) {
                 for (int64_t u = 0; u < Mp / TILE; ++u)
-                    gemm(f->bufB + tl * TILE * Mp + u * TILE, Mp, s->Cb + tl * TILE * LDC, LDC,
-                         f->bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], -1.0, 1.0);
+                    gemm(f->stage.bufB + tl * TILE * Mp + u * TILE, Mp, s->pred.Cb + tl * TILE * LDC, LDC,
+                         f->stage.bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], -1.0, 1.0);
             });
             ps.kh.n = (int)((int64_t)gi.size() - ps.kh.off);
             if (gvar) {
                 ps.t1.off = (int64_t)gi.size();                 // T = s K_ub'  (bufB = s, bufA = K_fu of the chunk)
                 each([&](int64_t b, int64_t tl) {
                     for (int c = 0; c < s->bsize_h[(size_t)b] / TILE; ++c)
-                        gemm(s->Tb + tl * TILE * LDC + c * TILE, LDC, f->bufB + tl * TILE * Mp, Mp,
-                             f->bufA + (s->bstart_h[(size_t)b] - ch.r0 + c * TILE) * Mp, Mp, Mp, 1.0, 0.0);
+                        gemm(s->pgrad.Tb + tl * TILE * LDC + c * TILE, LDC, f->stage.bufB + tl * TILE * Mp, Mp,
+                             f->stage.bufA + (s->bstart_h[(size_t)b] - ch.r0 + c * TILE) * Mp, Mp, Mp, 1.0, 0.0);
                 });
                 ps.t1.n = (int)((int64_t)gi.size() - ps.t1.off);
                 ps.tx.off = (int64_t)gi.size();                 // T X'  (into the G tiles)
                 each([&](int64_t b, int64_t tl) {
                     const int B = s->bsize_h[(size_t)b];
                     for (int c = 0; c < B / TILE; ++c)
-                        gemm(s->Gb + tl * TILE * LDC + c * TILE, LDC, s->Tb + tl * TILE * LDC, LDC,
+                        gemm(s->pred.Gb + tl * TILE * LDC + c * TILE, LDC, s->pgrad.Tb + tl * TILE * LDC, LDC,
                              s->X + s->boff_h[(size_t)b] + (int64_t)c * TILE * B, B, (int64_t)(c + 1) * TILE, 1.0, 0.0);
                 });
                 ps.tx.n = (int)((int64_t)gi.size() - ps.tx.off);
@@ -747,15 +726,15 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
                 each([&](int64_t b, int64_t tl) {
                     const int B = s->bsize_h[(size_t)b];
                     for (int c = 0; c < B / TILE; ++c)
-                        gemm(s->Cb + tl * TILE * LDC + c * TILE, LDC, s->Gb + tl * TILE * LDC + c * TILE, LDC,
+                        gemm(s->pred.Cb + tl * TILE * LDC + c * TILE, LDC, s->pred.Gb + tl * TILE * LDC + c * TILE, LDC,
                              s->LT + s->boff_h[(size_t)b] + (int64_t)c * TILE * B + c * TILE, B, B - (int64_t)c * TILE, -2.0, -2.0);
                 });
                 ps.ee.n = (int)((int64_t)gi.size() - ps.ee.off);
                 ps.ek.off = (int64_t)gi.size();                 // Z += e K_bu / 2  (bufA = K_uf of the chunk)
                 each([&](int64_t b, int64_t tl) {
                     for (int64_t u = 0; u < Mp / TILE; ++u)
-                        gemm(s->Zb + tl * TILE * Mp + u * TILE, Mp, s->Cb + tl * TILE * LDC, LDC,
-                             f->bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], 0.5, 1.0);
+                        gemm(s->pgrad.Zb + tl * TILE * Mp + u * TILE, Mp, s->pred.Cb + tl * TILE * LDC, LDC,
+                             f->stage.bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], 0.5, 1.0);
                 });
                 ps.ek.n = (int)((int64_t)gi.size() - ps.ek.off);
             }
@@ -763,8 +742,8 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
                 ps.ak.off = (int64_t)gi.size();                 // alpha_b K_bu on every row of the tile (into Vs)
                 each([&](int64_t b, int64_t tl) {
                     for (int64_t u = 0; u < Mp / TILE; ++u)
-                        gemm(s->Vs + tl * TILE * Mp + u * TILE, Mp, s->a + s->bstart_h[(size_t)b], 0,
-                             f->bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], 1.0, 0.0);
+                        gemm(s->pred.Vs + tl * TILE * Mp + u * TILE, Mp, s->a + s->bstart_h[(size_t)b], 0,
+                             f->stage.bufA + u * TILE * Nc + (s->bstart_h[(size_t)b] - ch.r0), Nc, s->bsize_h[(size_t)b], 1.0, 0.0);
                 });
                 ps.ak.n = (int)((int64_t)gi.size() - ps.ak.off);
             }
@@ -778,8 +757,8 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
                 for (int64_t u = sb.t0; u < sb.t1; ++u) {
                     const int64_t b = tile_blk[(size_t)t];
                     if (b < 0 || tile_blk[(size_t)u] != b) continue;
-                    gemm(f->Kss + (t - sb.t0) * TILE * mq + (u - sb.t0) * TILE, mq, s->Gb + (t - sb.t0) * TILE * LDC, LDC,
-                         s->Gb + (u - sb.t0) * TILE * LDC, LDC, s->bsize_h[(size_t)b], -1.0, 1.0);
+                    gemm(f->Kss + (t - sb.t0) * TILE * mq + (u - sb.t0) * TILE, mq, s->pred.Gb + (t - sb.t0) * TILE * LDC, LDC,
+                         s->pred.Gb + (u - sb.t0) * TILE * LDC, LDC, s->bsize_h[(size_t)b], -1.0, 1.0);
                 }
         }
         sb.ggt.n = (int)((int64_t)gi.size() - sb.ggt.off);
@@ -801,28 +780,21 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
             sb.dx.n = (int)((int64_t)di.size() - sb.dx.off);
         }
     }
-    auto upload = [&](auto*& dst, size_t& cap, const auto& v) -> cudaError_t {
-        using T = typename std::decay_t<decltype(v)>::value_type;
-        if (v.size() > cap) {
-            if (dst) cudaFree(dst);
-            dst = nullptr; cap = 0;
-            cudaError_t e = cudaMalloc(&dst, sizeof(T) * v.size());
-            if (e != cudaSuccess) return e;
-            cap = v.size();
-        }
-        return v.empty() ? cudaSuccess : cudaMemcpy(dst, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice);
+    auto upload = [&](auto& dst, const auto& v) -> cudaError_t {
+        const cudaError_t e = dst.ensure(v.size());
+        return e != cudaSuccess || v.empty() ? e : cudaMemcpy(dst, v.data(), sizeof(v[0]) * v.size(), cudaMemcpyHostToDevice);
     };
-    FCK(upload(s->pg, s->pg_cap, gi));
-    FCK(upload(s->px, s->px_cap, xi));
-    FCK(upload(s->pr, s->pr_cap, ri));
-    if (grad) FCK(upload(s->pdi, s->pdi_cap, di));
-    GemmBuf bA{eu->tma_ok ? &f->mapA : nullptr, f->bufA, Mp};
-    GemmBuf bB2{eu->tma_ok ? &f->mapB2 : nullptr, f->bufB, Mp};
-    GemmBuf bVs{eu->tma_ok ? &s->mapVs : nullptr, s->Vs, Mp};
-    GemmBuf bZb{eu->tma_ok ? &s->mapZb : nullptr, s->Zb, Mp};
+    FCK(upload(s->pg, gi));
+    FCK(upload(s->px, xi));
+    FCK(upload(s->pr, ri));
+    if (grad) FCK(upload(s->pdi, di));
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp);
+    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, Mp);
+    const GemmBuf bVs = gbuf(eu, s->pred.Vs, s->pred.mapVs, Mp);
+    const GemmBuf bZb = gbuf(eu, s->pgrad.Zb, s->pgrad.mapZb, Mp);
     const bool cov_host = cov && !f->cov_keep_device;
     std::vector<double> mu_p((size_t)Msp), var_p(var ? (size_t)Msp : 0), cov_p(cov_host ? (size_t)Msp * Msp : 0);
-    double* ddmu = grad ? s->pdx : nullptr;
+    double* ddmu = grad ? s->pdx.data() : nullptr;
     double* ddvar = grad ? s->pdx + Ms * d : nullptr;
     if (grad) {
         for (double& t : f->fsag_ms) t = 0.0;
@@ -832,34 +804,34 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
     for (const Sub& sb : subs) {
         const int64_t row0 = sb.t0 * TILE, mq = (sb.t1 - sb.t0) * TILE;
         if (grad) FCK(cudaEventRecord(eu->ev0, st));
-        FCK(cudaMemcpyAsync(f->xs, xsp.data() + row0 * d, sizeof(double) * mq * d, cudaMemcpyHostToDevice, st));
-        FCK(crossgram_launch(eu->prog, f->xs, d, mq, mq, eu->x, d, f->M, Mp, d, f->bufB, Mp, st, &eu->launches));     // K_*u
-        FCK(rowdot_launch(f->bufB, Mp, f->uvec, mq, Mp, mu1, st, &eu->launches));                                       // K_*u u
-        FCK(cudaMemcpyAsync(s->Vs, f->bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));
-        if (gvar) FCK(cudaMemcpyAsync(s->Zb, f->bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));      // Z = K_*u
+        FCK(cudaMemcpyAsync(f->stage.xs, xsp.data() + row0 * d, sizeof(double) * mq * d, cudaMemcpyHostToDevice, st));
+        FCK(crossgram_launch(eu->prog, f->stage.xs, d, mq, mq, eu->x, d, f->M, Mp, d, f->stage.bufB, Mp, st, &eu->launches));     // K_*u
+        FCK(rowdot_launch(f->stage.bufB, Mp, f->data.uvec, mq, Mp, mu1, st, &eu->launches));                                       // K_*u u
+        FCK(cudaMemcpyAsync(s->pred.Vs, f->stage.bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));
+        if (gvar) FCK(cudaMemcpyAsync(s->pgrad.Zb, f->stage.bufB, sizeof(double) * mq * Mp, cudaMemcpyDeviceToDevice, st));      // Z = K_*u
         FCK(trsm_rec_buf(eu, bVs, (int)mq, 0, (int)Mp));                                                 // V_*'
-        FCK(kdiag_launch(eu->prog, f->xs, d, mq, r2, st, &eu->launches));
-        FCK(rowvar_launch(s->Vs, Mp, r2, mq, Mp, q, st, &eu->launches));                                                 // k** - |V_*|^2
+        FCK(kdiag_launch(eu->prog, f->stage.xs, d, mq, r2, st, &eu->launches));
+        FCK(rowvar_launch(s->pred.Vs, Mp, r2, mq, Mp, q, st, &eu->launches));                                                 // k** - |V_*|^2
         FCK(cudaMemsetAsync(mu2, 0, sizeof(double) * mq, st));
         FCK(cudaMemsetAsync(g2, 0, sizeof(double) * mq, st));
         for (const Pass& ps : sb.passes) {
             const FsaChunk& ch = s->chunks[(size_t)ps.chunk];
             const double* xr = s->xb + ch.r0 * d;
             FCK(fitc_kfu(f, xr, ch.rows));                                                                 // V of the training chunk
-            FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
+            FCK(fsa_mask_launch(f->stage.bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
             FCK(trsm_rec_buf(eu, bA, (int)Nc, 0, (int)Mp));
-            FCK(fsa_crossgram_launch(eu->prog, f->xs, s->xb, d, s->px + ps.xg.off, ps.xg.n, s->mask, st, &eu->launches));
+            FCK(fsa_crossgram_launch(eu->prog, f->stage.xs, s->xb, d, s->px + ps.xg.off, ps.xg.n, s->mask, st, &eu->launches));
             FCK(fsa_gemm_launch(s->pg + ps.vv.off, ps.vv.n, st, &eu->launches));
             FCK(fsa_rowdot_launch(s->pr + ps.mu2.off, ps.mu2.n, st, &eu->launches));
             FCK(fsa_gemm_launch(s->pg + ps.gg.off, ps.gg.n, st, &eu->launches));
             FCK(fsa_rowdot_launch(s->pr + ps.g2.off, ps.g2.n, st, &eu->launches));
             FCK(fsa_gemm_launch(s->pg + ps.hh.off, ps.hh.n, st, &eu->launches));
-            FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->bufA, Nc, st, &eu->launches));   // K_uf of the chunk
-            FCK(fsa_mask_launch(f->bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+            FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->stage.bufA, Nc, st, &eu->launches));   // K_uf of the chunk
+            FCK(fsa_mask_launch(f->stage.bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
             FCK(fsa_gemm_launch(s->pg + ps.kh.off, ps.kh.n, st, &eu->launches));
         }
         FCK(trsm_rec_buf(es, bB2, (int)mq, 0, (int)Mp));                                                  // R = (K_*u - G W) L_s^-T
-        FCK(rowvar_launch(f->bufB, Mp, f->zeroc, mq, Mp, r2, st, &eu->launches));
+        FCK(rowvar_launch(f->stage.bufB, Mp, f->stage.zeroc, mq, Mp, r2, st, &eu->launches));
         FCK(fsa_var_launch(vp, q, g2, r2, mq, st, &eu->launches));
         FCK(ew_launch(2, mq, mu1, mu2, nullptr, nullptr, 0.0, st, &eu->launches));
         FCK(cudaMemcpyAsync(mu_p.data() + row0, mu1, sizeof(double) * mq, cudaMemcpyDeviceToHost, st));
@@ -867,19 +839,19 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
         if (grad) {
             FCK(cudaEventRecord(eu->ev1, st));
             if (var) FCK(trsm_right_rec_buf(es, bB2, (int)mq, 0, (int)Mp));                             // s = R L_s^-1
-            FCK(cudaMemsetAsync(s->Vs, 0, sizeof(double) * mq * Mp, st));
+            FCK(cudaMemsetAsync(s->pred.Vs, 0, sizeof(double) * mq * Mp, st));
             for (const Pass& ps : sb.passes) {                                                           // second sweep
                 const FsaChunk& ch = s->chunks[(size_t)ps.chunk];
                 const double* xr = s->xb + ch.r0 * d;
                 if (var) {
                     FCK(fitc_kfu(f, xr, ch.rows));                                                       // K_fu of the chunk
-                    FCK(fsa_mask_launch(f->bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
+                    FCK(fsa_mask_launch(f->stage.bufA, Mp, ch.rows, Mp, s->mask + ch.r0, nullptr, st, &eu->launches));
                     FCK(fsa_gemm_launch(s->pg + ps.t1.off, ps.t1.n, st, &eu->launches));
                     FCK(fsa_gemm_launch(s->pg + ps.tx.off, ps.tx.n, st, &eu->launches));
                     FCK(fsa_gemm_launch(s->pg + ps.ee.off, ps.ee.n, st, &eu->launches));
                 }
-                FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->bufA, Nc, st, &eu->launches));
-                FCK(fsa_mask_launch(f->bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
+                FCK(crossgram_launch(eu->prog, eu->x, d, f->M, Mp, xr, d, ch.rows, Nc, d, f->stage.bufA, Nc, st, &eu->launches));
+                FCK(fsa_mask_launch(f->stage.bufA, Nc, Mp, ch.rows, nullptr, s->mask + ch.r0, st, &eu->launches));
                 if (var) FCK(fsa_gemm_launch(s->pg + ps.ek.off, ps.ek.n, st, &eu->launches));
                 FCK(fsa_gemm_launch(s->pg + ps.ak.off, ps.ak.n, st, &eu->launches));
             }
@@ -891,13 +863,13 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
                 FCK(trsm_right_rec_buf(eu, bZb, (int)mq, 0, (int)Mp));
             }
             FCK(cudaEventRecord(eu->ev3, st));
-            FCK(fsa_crossgram_dx_launch(eu->prog, f->xs, eu->x, s->xb, d, f->M, f->uvec, s->Vs, f->bufB, s->Zb, Mp, s->mask,
-                                        s->a, s->Cb, LDC, s->pdi + sb.dx.off, sb.dx.n, ddmu, var ? ddvar : nullptr, st,
+            FCK(fsa_crossgram_dx_launch(eu->prog, f->stage.xs, eu->x, s->xb, d, f->M, f->data.uvec, s->pred.Vs, f->stage.bufB, s->pgrad.Zb, Mp, s->mask,
+                                        s->a, s->pred.Cb, LDC, s->pdi + sb.dx.off, sb.dx.n, ddmu, var ? ddvar : nullptr, st,
                                         &eu->launches));
             FCK(cudaEventRecord(eu->ev4, st));
         }
         if (cov) {
-            FCK(gram_full_launch(eu->prog, f->xs, d, mq, mq, d, f->Kss, mq, st, &eu->launches));
+            FCK(gram_full_launch(eu->prog, f->stage.xs, d, mq, mq, d, f->Kss, mq, st, &eu->launches));
             FCK(gemm_whole(eu, bVs, bVs, f->Kss, mq, mq, mq, Mp, -1.0, 1.0));                              // - V_*' V_*
             FCK(gemm_whole(es, bB2, bB2, f->Kss, mq, mq, mq, Mp, 1.0, 1.0));                               // + R R'
             FCK(fsa_gemm_launch(s->pg + sb.ggt.off, sb.ggt.n, st, &eu->launches));  // - G G'
@@ -919,15 +891,10 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
     if (cov && !cov_host) {
         // Sigma* (one sub-chunk: leading dimension Msp) and mu in the caller's order on the device, as the host loop below
         // reorders them
-        if ((size_t)(Ms * Ms) > s->Sc_cap) {
-            if (s->Sc) cudaFree(s->Sc);
-            s->Sc = nullptr; s->Sc_cap = 0;
-            FCK(cudaMalloc(&s->Sc, sizeof(double) * Ms * Ms));
-            s->Sc_cap = (size_t)(Ms * Ms);
-        }
-        FCK(upload(s->pp, s->pp_cap, ppos));
+        FCK(s->Sc.ensure((size_t)Ms * Ms));
+        FCK(upload(s->pp, ppos));
         FCK(gather_block_launch(s->Sc, f->Kss, Msp, s->pp, Ms, st, &eu->launches));
-        FCK(fsa_permute_launch(0, mu1, s->pp, Ms, f->tmpc, st, &eu->launches));
+        FCK(fsa_permute_launch(0, mu1, s->pp, Ms, f->stage.tmpc, st, &eu->launches));
     }
     for (int64_t i = 0; i < Ms; ++i) {
         const size_t r = (size_t)ppos[(size_t)i];

@@ -80,26 +80,18 @@ void free_FG(gpb200_handle* h);               // shard_impl.cuh: F / G are cudaM
 
 void free_data(gpb200_handle* h) {
     free_FG(h);
-    double** ptrs[] = {&h->x, &h->Dinv, &h->DinvT, &h->logd, &h->noise_var, &h->r0, &h->r1,
-                       &h->y1, &h->alpha, &h->scal, &h->part, &h->trace_out, &h->xs, &h->Kst, &h->Kss,
-                       &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp, &h->xpt, &h->ZdT, &h->pdx, &h->dxin};
     h->xmap_ok = false;
-    if (h->cvD) cudaFree(h->cvD);
-    if (h->cvY) cudaFree(h->cvY);
-    if (h->cvblk) cudaFree(h->cvblk);
-    if (h->cvidx) cudaFree(h->cvidx);
-    h->cvD = h->cvY = h->cvblk = nullptr; h->cvidx = nullptr; h->cvblk_cap = h->cvidx_cap = 0; h->g_sym = false; h->cv_m_ok = false;
-    for (auto pp : ptrs) { if (*pp) cudaFree(*pp); *pp = nullptr; }
-    if (h->info_dev) { cudaFree(h->info_dev); h->info_dev = nullptr; }
-    if (h->flags) { cudaFree(h->flags); h->flags = nullptr; }
+    h->cvD.reset(); h->cvY.reset(); h->cvblk.reset(); h->cvidx.reset();
+    h->g_sym = false; h->cv_m_ok = false;
+    for (DevBuf<double>* b : {&h->x, &h->Dinv, &h->DinvT, &h->logd, &h->noise_var, &h->r0, &h->r1, &h->y1, &h->alpha, &h->scal,
+                              &h->part, &h->trace_out, &h->xs, &h->Kst, &h->Kss, &h->pmu, &h->pvar, &h->pkdiag, &h->tblk, &h->xp,
+                              &h->xpt, &h->ZdT, &h->pdx, &h->dxin})
+        b->reset();
+    h->info_dev.reset(); h->flags.reset();
     close_peer_maps(h);                        // peers' mappings refer to the old buffers whether or not p2p is switched on
-    if (h->sig) { cudaFree(h->sig); h->sig = nullptr; }
-    if (h->peer_sig_dev) { cudaFree(h->peer_sig_dev); h->peer_sig_dev = nullptr; }
-    for (int i = 0; i < 2; ++i) { if (h->pack[i]) cudaFree(h->pack[i]); h->pack[i] = nullptr; }
-    if (h->ag_send) cudaFree(h->ag_send);
-    if (h->ag_recv) cudaFree(h->ag_recv);
-    h->ag_send = h->ag_recv = nullptr; h->pack_elems = h->ag_send_elems = h->ag_recv_elems = 0;
-    h->xs_cap = h->Kst_rows = h->Kss_rows = h->pdx_rows = 0;
+    h->sig.reset(); h->peer_sig_dev.reset();
+    h->pack[0].reset(); h->pack[1].reset();
+    h->ag_send.reset(); h->ag_recv.reset();
     h->has_data = h->factored = h->inv_ready = h->s_ready = h->alpha_ready = false;
 }
 
@@ -397,23 +389,14 @@ int dist_alloc(gpb200_handle* h) {
     const size_t Np = (size_t)h->Npad;
     const size_t nbw = (size_t)dist_block(h);
     const size_t need_pack = Np * nbw + 2 * nbw * TILE + nbw + 16;
-    if (need_pack > h->pack_elems) {
-        for (int i = 0; i < 2; ++i) {
-            if (h->pack[i]) cudaFree(h->pack[i]);
-            h->pack[i] = nullptr;
-            CK(cudaMalloc(&h->pack[i], sizeof(double) * need_pack));
-        }
-        h->pack_elems = need_pack;
-    }
+    if (need_pack > h->pack[1].size())
+        for (int i = 0; i < 2; ++i) CK(h->pack[i].alloc(need_pack));
     const size_t need_recv = Np * Np / 4 + Np * TILE;
     const size_t need_send = need_recv / h->nranks + Np * TILE;
-    if (need_recv > h->ag_recv_elems) {
-        if (h->ag_recv) cudaFree(h->ag_recv);
-        if (h->ag_send) cudaFree(h->ag_send);
-        h->ag_recv = h->ag_send = nullptr;
-        CK(cudaMalloc(&h->ag_recv, sizeof(double) * need_recv));
-        CK(cudaMalloc(&h->ag_send, sizeof(double) * need_send));
-        h->ag_recv_elems = need_recv; h->ag_send_elems = need_send;
+    if (need_recv > h->ag_recv.size() || !h->ag_send) {  // ag_send, allocated last, is empty after any failure here
+        h->ag_recv.reset(); h->ag_send.reset();
+        CK(h->ag_recv.alloc(need_recv));
+        CK(h->ag_send.alloc(need_send));
     }
     return GPB200_OK;
 }
@@ -620,7 +603,7 @@ int inverse_dist(gpb200_handle* h) {
         long long rows_total = 0;                                   // sum over problems of n2_z (only the last is short)
         for (int z = 0; z < batch; ++z) rows_total += std::max(0LL, std::min((long long)s, (long long)Np - z * 2 * s - s));
         const long long per_rank = rows_total * wr;
-        if ((size_t)per_rank > h->ag_send_elems || (size_t)per_rank * R > h->ag_recv_elems)
+        if ((size_t)per_rank > h->ag_send.size() || (size_t)per_rank * R > h->ag_recv.size())
             return fail(h, GPB200_ECUDA, "inverse_dist: exchange buffers too small");
         dim3 blk(32, 32), grd((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)batch);
         pack_slices_kernel<<<grd, blk, 0, h->st>>>(h->G, h->ld, h->ag_send, (int)s, wr, R, me, Np);
@@ -685,32 +668,19 @@ int upload_padded(gpb200_handle* h, double* dst, const double* src_host) {
 
 int ensure_predict_ws(gpb200_handle* h, int64_t Mc, bool want_cov) {
     const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
-    if (Mpad > h->xs_cap) {
-        if (h->xs) cudaFree(h->xs);
-        if (h->pmu) cudaFree(h->pmu);
-        if (h->pvar) cudaFree(h->pvar);
-        if (h->pkdiag) cudaFree(h->pkdiag);
-        h->xs = h->pmu = h->pvar = h->pkdiag = nullptr; h->xs_cap = 0;
-        CK(cudaMalloc(&h->xs, sizeof(double) * Mpad * h->d));
-        CK(cudaMalloc(&h->pmu, sizeof(double) * Mpad));
-        CK(cudaMalloc(&h->pvar, sizeof(double) * Mpad));
-        CK(cudaMalloc(&h->pkdiag, sizeof(double) * Mpad));
-        h->xs_cap = Mpad;
+    if ((size_t)Mpad > h->pkdiag.size()) {          // pkdiag, allocated last, is empty after any failure here
+        for (DevBuf<double>* b : {&h->xs, &h->pmu, &h->pvar, &h->pkdiag}) b->reset();
+        CK(h->xs.alloc(Mpad * h->d));
+        for (DevBuf<double>* b : {&h->pmu, &h->pvar, &h->pkdiag}) CK(b->alloc(Mpad));
     }
-    if (Mpad > h->Kst_rows) {
-        if (h->Kst) cudaFree(h->Kst);
-        h->Kst = nullptr; h->Kst_rows = 0;
-        CK(cudaMalloc(&h->Kst, sizeof(double) * Mpad * h->Npad));
-        h->Kst_rows = Mpad;
-        if (h->tma_ok && !gemm_make_tensor_map(&h->mapKst, h->Kst, Mpad, h->Npad, h->Npad))
+    if ((size_t)(Mpad * h->Npad) > h->Kst.size()) {
+        CK(h->Kst.alloc(Mpad * h->Npad));
+        if (h->tma_ok && !gemm_make_tensor_map(&h->mapKst, h->Kst, Mpad, h->Npad, h->Npad)) {
+            h->Kst.reset();
             return fail(h, GPB200_ECUDA, "cuTensorMapEncodeTiled failed for the predict buffer");
+        }
     }
-    if (want_cov && Mpad > h->Kss_rows) {
-        if (h->Kss) cudaFree(h->Kss);
-        h->Kss = nullptr; h->Kss_rows = 0;
-        CK(cudaMalloc(&h->Kss, sizeof(double) * Mpad * Mpad));
-        h->Kss_rows = Mpad;
-    }
+    if (want_cov) CK(h->Kss.ensure(Mpad * Mpad));
     return GPB200_OK;
 }
 
@@ -744,7 +714,7 @@ cudaError_t trsm_rec_buf(gpb200_handle* h, GemmBuf bk, int rows, int c0, int n) 
     return trsm_rec_buf(h, bk, rows, c0 + n1, n2);
 }
 cudaError_t trsm_rec(gpb200_handle* h, int Mpad, int c0, int n) {
-    GemmBuf bk{h->tma_ok ? &h->mapKst : nullptr, h->Kst, h->Npad};
+    const GemmBuf bk = gbuf(h, h->Kst, h->mapKst, h->Npad);
     return trsm_rec_buf(h, bk, Mpad, c0, n);
 }
 
@@ -900,11 +870,10 @@ int rand_from_cov(gpb200_handle* h, int64_t M, const double* cov, int64_t ldc, c
     CK(cudaEventRecord(h->ev1, h->st));
     // draws: Zt (nsamp x M, zero padded) on the device
     if (Spad > h->rz_rows || Mpad > h->rz_cols) {
-        if (h->rz) cudaFree(h->rz);
-        if (h->rout) cudaFree(h->rout);
-        h->rz = h->rout = nullptr; h->rz_rows = h->rz_cols = 0;
-        CK(cudaMalloc(&h->rz, sizeof(double) * Spad * Mpad));
-        CK(cudaMalloc(&h->rout, sizeof(double) * Spad * Mpad));
+        h->rz.reset(); h->rout.reset();
+        h->rz_rows = h->rz_cols = 0;
+        CK(h->rz.alloc(Spad * Mpad));
+        CK(h->rout.alloc(Spad * Mpad));
         h->rz_rows = Spad; h->rz_cols = Mpad;
     }
     const int64_t ldz = h->rz_cols;
@@ -913,7 +882,7 @@ int rand_from_cov(gpb200_handle* h, int64_t M, const double* cov, int64_t ldc, c
     CK(cudaMemcpy2DAsync(h->rz, sizeof(double) * ldz, z, sizeof(double) * M, sizeof(double) * M, nsamp, cudaMemcpyHostToDevice, h->st));
     CK(cudaEventRecord(h->ev3, h->st));
     // out[s, m] = sum_{k <= m} Zt[s, k] L[m, k]       (unwhiten!: L Z)
-    CK(gemm_whole(h, GemmBuf{h->tma_ok ? &h->mapRz : nullptr, h->rz, ldz}, bufF(sb), h->rout, ldz, Spad, Mpad, Mpad, 1.0, 0.0,
+    CK(gemm_whole(h, gbuf(h, h->rz, h->mapRz, ldz), bufF(sb), h->rout, ldz, Spad, Mpad, Mpad, 1.0, 0.0,
                   nullptr, 0, GEMM_KHI_N));
     CK(add_rowvec_launch(h->rout, ldz, mu, nsamp, M, h->st, &h->launches));                              // + mu
     CK(cudaEventRecord(h->ev2, h->st));
@@ -984,8 +953,7 @@ void gpb200_destroy(gpb200_handle* h) {
     }
     if (h->st) cudaStreamSynchronize(h->st);
     if (h->sub) { h->sub->st = nullptr; h->sub->own_stream = false; gpb200_destroy(h->sub); h->sub = nullptr; }
-    if (h->rz) cudaFree(h->rz);
-    if (h->rout) cudaFree(h->rout);
+    h->rz.reset(); h->rout.reset();
     free_data(h);
     for (auto e : h->evring) cudaEventDestroy(e);
     if (h->ev0) cudaEventDestroy(h->ev0);
@@ -1056,6 +1024,7 @@ int gpb200_set_option(gpb200_handle* h, const char* key, int64_t value) {
 }
 
 int64_t gpb200_launch_count(gpb200_handle* h) { return h ? h->launches : 0; }
+int64_t gpb200_device_bytes(void) { return g_device_bytes.load(); }
 
 int gpb200_set_stream(gpb200_handle* h, void* stream) {
     if (!h) return GPB200_EINVAL;
@@ -1088,16 +1057,14 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
     if (realloc) {
         free_data(h);
         h->N = N; h->Npad = Npad; h->ld = Npad; h->d = d;
-        CK(cudaMalloc(&h->x, sizeof(double) * Npad * d));      // Npad rows: N may grow up to Npad without realloc
-        CK(cudaMalloc(&h->Dinv, sizeof(double) * Npad * TILE));
-        CK(cudaMalloc(&h->DinvT, sizeof(double) * Npad * TILE));
-        const size_t nv = sizeof(double) * Npad;
-        CK(cudaMalloc(&h->logd, nv)); CK(cudaMalloc(&h->noise_var, nv)); CK(cudaMalloc(&h->r0, nv));
-        CK(cudaMalloc(&h->r1, nv)); CK(cudaMalloc(&h->y1, nv)); CK(cudaMalloc(&h->alpha, nv)); CK(cudaMalloc(&h->tblk, nv));
-        CK(cudaMalloc(&h->scal, sizeof(double) * 16));
-        CK(cudaMalloc(&h->info_dev, sizeof(int)));
-        CK(cudaMalloc(&h->flags, sizeof(int) * 2 * (Npad / TILE + 1)));
-        CK(cudaMalloc(&h->sig, sizeof(int) * 16));
+        CK(h->x.alloc(Npad * d));                    // Npad rows: N may grow up to Npad without realloc
+        CK(h->Dinv.alloc(Npad * TILE));
+        CK(h->DinvT.alloc(Npad * TILE));
+        for (DevBuf<double>* b : {&h->logd, &h->noise_var, &h->r0, &h->r1, &h->y1, &h->alpha, &h->tblk}) CK(b->alloc(Npad));
+        CK(h->scal.alloc(16));
+        CK(h->info_dev.alloc(1));
+        CK(h->flags.alloc(2 * (Npad / TILE + 1)));
+        CK(h->sig.alloc(16));
         CK(cudaMemsetAsync(h->sig, 0, sizeof(int) * 16, h->st));
         {
             int sms = 0;
@@ -1107,8 +1074,8 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
             h->max_resident_ctas = sms * TRSV_FUSED_CTAS_PER_SM;
         }
         const int64_t T = Npad / TILE;
-        CK(cudaMalloc(&h->part, sizeof(double) * (size_t)(T * (T + 1) / 2) * (GPB200_MAX_THETA + 1)));
-        CK(cudaMalloc(&h->trace_out, sizeof(double) * (GPB200_MAX_THETA + 1)));
+        CK(h->part.alloc((size_t)(T * (T + 1) / 2) * (GPB200_MAX_THETA + 1)));
+        CK(h->trace_out.alloc(GPB200_MAX_THETA + 1));
         // F / G: replicated (cudaMalloc) or row-sharded (virtual range, owned rows mapped) -- decided by the communicator,
         // the problem size and option "shard"; re-checked at every factorize (the communicator may be joined later)
         int rc_fg = ensure_storage(h);
@@ -1122,11 +1089,11 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
     h->xmap_ok = false;
     if (d <= 8) {
         h->dxp = (d + 1) / 2 * 2;
-        if (!h->xp) CK(cudaMalloc(&h->xp, sizeof(double) * Npad * h->dxp));
+        if (!h->xp) CK(h->xp.alloc(Npad * h->dxp));
         CK(cudaMemsetAsync(h->xp, 0, sizeof(double) * Npad * h->dxp, h->st));
         CK(cudaMemcpy2DAsync(h->xp, sizeof(double) * h->dxp, x, sizeof(double) * ldx, sizeof(double) * d, N,
                              cudaMemcpyHostToDevice, h->st));
-        if (!h->xpt) CK(cudaMalloc(&h->xpt, sizeof(double) * Npad * h->dxp));
+        if (!h->xpt) CK(h->xpt.alloc(Npad * h->dxp));
         CK(shard_transpose(h->xpt, Npad, h->xp, h->dxp, Npad, h->dxp, h->st, &h->launches));
         h->xmap_ok = gemm_make_tensor_map_plain(&h->mapX, h->xp, N, h->dxp, h->dxp, TILE, h->dxp) &&
                      gemm_make_tensor_map_plain(&h->mapXT, h->xpt, h->dxp, N, Npad, h->dxp, TILE);
@@ -1354,7 +1321,7 @@ int gpb200_grad_kernel(gpb200_handle* h, const double* alpha, double* dmll_kerne
     if (h->sharded) {
         // fused trace over the own rows of K^-1 (block-cyclic tile rows), P+1 partial sums summed over the ranks
         for (auto* q : Lg) SCK(q, launch_trace(q, q->nranks, q->rank, q->rb));
-        TRY(coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out; }, (size_t)trace_num_acc(h->prog, h->d)));
+        TRY(coll_allreduce_sum(Lg, [&](gpb200_handle* q) { return q->trace_out.data(); }, (size_t)trace_num_acc(h->prog, h->d)));
     } else {
         CK(launch_trace(h, h->nranks, h->rank, 1));
     }
@@ -1417,9 +1384,9 @@ int gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, doub
     h->inv_ready = h->s_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;
     const int Np = (int)h->Npad;
     if (!h->ZdT) {
-        CK(cudaMalloc(&h->ZdT, sizeof(double) * h->Npad * TILE));
+        CK(h->ZdT.alloc(h->Npad * TILE));
         if (h->tma_ok && !gemm_make_tensor_map(&h->mapZdT, h->ZdT, h->Npad, TILE, TILE)) {
-            cudaFree(h->ZdT); h->ZdT = nullptr;
+            h->ZdT.reset();
             return fail(h, GPB200_ECUDA, "gpa_grad: cuTensorMapEncodeTiled failed for the diagonal tiles of Z'");
         }
     }
@@ -1431,7 +1398,7 @@ int gpb200_gpa_grad(gpb200_handle* h, const double* v, const double* dl_df, doub
     {
         GemmDesc g = gemm_desc_default();                       // G[a,b] = -sum_{i >= a} W'[a,i] Z'[b,i]   (a >= b)
         g.A = GemmOperand{bufG(h), bufDinvT(h), 0, 0};
-        g.B = GemmOperand{bufF(h), GemmBuf{h->tma_ok ? &h->mapZdT : nullptr, h->ZdT, TILE}, 0, 0};
+        g.B = GemmOperand{bufF(h), gbuf(h, h->ZdT, h->mapZdT, TILE), 0, 0};
         g.C = h->G; g.ldc = h->ld; g.c_row0 = 0; g.c_col0 = 0;
         g.M = Np; g.N = Np; g.K = Np;
         g.alpha = -1.0;
@@ -1472,14 +1439,14 @@ int gpb200_grad_inputs(gpb200_handle* h, const double* alpha, double* dmll_x) {
     if (h->sharded) TRY(shard_entry(h, L)); else L = Locals{h};
     const int64_t N = h->N, Npad = h->Npad, nd = Npad * h->d;
     for (auto* q : L) {
-        if (!q->dxin) SCK(q, cudaMalloc(&q->dxin, sizeof(double) * (size_t)(Npad + nd * (1 + (q->grp ? q->nranks : 0)))));
+        if (!q->dxin) SCK(q, q->dxin.alloc(Npad + nd * (1 + (q->grp ? q->nranks : 0))));
         if (alpha) TRY(rank_failed(q, upload_padded(q, q->dxin, alpha)));
     }
     auto res = [&](gpb200_handle* q) { return q->dxin + Npad; };
     CK(cudaEventRecord(h->ev0, h->st));
     for (auto* q : L) {
         SeIsoFast sf;
-        const double* a = h->s_ready ? nullptr : alpha ? q->dxin : q->alpha;     // S state: A = -G = S
+        const double* a = h->s_ready ? nullptr : alpha ? q->dxin.data() : q->alpha.data();     // S state: A = -G = S
         SCK(q, inputs_dx_launch(q->prog, use_seiso_fast(q, &sf), q->x, q->d, q->d, N, a, q->G, q->ld, res(q), q->st, &q->launches,
                                 q->nranks, q->rank, q->sharded ? q->rb : 1));
     }
@@ -1572,7 +1539,7 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
             }
             if (cov) {                                                                      // GP.jl:51-54
                 CK(gram_full_launch(h->prog, h->xs, h->d, Mc, Mpad, h->d, h->Kss, Mpad, h->st, &h->launches));
-                GemmBuf bk{h->tma_ok ? &h->mapKst : nullptr, h->Kst, h->Npad};
+                const GemmBuf bk = gbuf(h, h->Kst, h->mapKst, h->Npad);
                 CK(gemm_whole(h, bk, bk, h->Kss, Mpad, Mpad, Mpad, h->Npad, -1.0, 1.0));
                 if (!h->cov_keep_device)
                     CK(cudaMemcpy2DAsync(cov, sizeof(double) * M, h->Kss, sizeof(double) * Mpad, sizeof(double) * M, M,
@@ -1620,14 +1587,9 @@ int gpb200_predict_grad(gpb200_handle* h, int64_t M, const double* xs, int64_t l
         const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
         int rc = ensure_predict_ws(h, Mc, false);
         if (rc) return rc;
-        if (Mpad > h->pdx_rows) {
-            if (h->pdx) cudaFree(h->pdx);
-            h->pdx = nullptr; h->pdx_rows = 0;
-            CK(cudaMalloc(&h->pdx, sizeof(double) * 2 * Mpad * d));
-            h->pdx_rows = Mpad;
-        }
+        CK(h->pdx.ensure(2 * Mpad * d));
         double* ddmu = h->pdx;
-        double* ddvar = h->pdx + h->pdx_rows * d;
+        double* ddvar = h->pdx + h->pdx.size() / 2;             // dmu and dvar take one half each
         CK(cudaEventRecord(h->ev0, h->st));
         CK(cudaMemcpy2DAsync(h->xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d, Mc,
                              cudaMemcpyHostToDevice, h->st));
@@ -1645,11 +1607,11 @@ int gpb200_predict_grad(gpb200_handle* h, int64_t M, const double* xs, int64_t l
         if (var && m0 == 0) CK(mirror_lower_tiles_launch(h->F, h->ld, h->Npad, h->st, &h->launches));   // L' into F's upper tiles
         CK(cudaEventRecord(h->ev5, h->st));
         if (var) {
-            GemmBuf bk{h->tma_ok ? &h->mapKst : nullptr, h->Kst, h->Npad};
+            const GemmBuf bk = gbuf(h, h->Kst, h->mapKst, h->Npad);
             CK(trsm_right_rec_buf(h, bk, (int)Mpad, 0, (int)h->Npad));                     // W' = V' L^-1
         }
         CK(cudaEventRecord(h->ev3, h->st));
-        CK(crossgram_dx_launch(h->prog, h->xs, d, Mc, h->x, d, h->N, d, h->alpha, var ? h->Kst : nullptr, nullptr, h->Npad, 1.0,
+        CK(crossgram_dx_launch(h->prog, h->xs, d, Mc, h->x, d, h->N, d, h->alpha, var ? h->Kst.data() : nullptr, nullptr, h->Npad, 1.0,
                                ddmu, ddvar, h->st, &h->launches));
         CK(cudaEventRecord(h->ev4, h->st));
         CK(cudaMemcpyAsync(dmu + m0 * d, ddmu, sizeof(double) * Mc * d, cudaMemcpyDeviceToHost, h->st));
@@ -1771,15 +1733,13 @@ static int cv_check(gpb200_handle* h) {
 
 static int cv_prepare(gpb200_handle* h) {
     TRY(cv_check(h));
-    const size_t nn = sizeof(double) * (size_t)h->Npad * (size_t)h->Npad;
+    const size_t nn = (size_t)h->Npad * (size_t)h->Npad;
     if (!h->cvD || !h->cvY) {
-        if (h->cvD) { cudaFree(h->cvD); h->cvD = nullptr; }
-        if (h->cvY) { cudaFree(h->cvY); h->cvY = nullptr; }
+        h->cvD.reset(); h->cvY.reset();
         h->cv_m_ok = false;
-        if (cudaMalloc(&h->cvD, nn) != cudaSuccess || cudaMalloc(&h->cvY, nn) != cudaSuccess) {
+        if (h->cvD.alloc(nn) != cudaSuccess || h->cvY.alloc(nn) != cudaSuccess) {
             (void)cudaGetLastError();
-            if (h->cvD) { cudaFree(h->cvD); h->cvD = nullptr; }
-            h->cvY = nullptr;
+            h->cvD.reset();
             return fail(h, GPB200_ECUDA, "cv: out of device memory for the two N x N work matrices");
         }
         if (h->tma_ok && !(gemm_make_tensor_map(&h->mapCvD, h->cvD, h->Npad, h->Npad, h->Npad) &&
@@ -1835,13 +1795,10 @@ static int shard_cv_param(gpb200_handle* h, int32_t param, const double* alpha, 
 
 // principal sub-block workspace: nV indices, `elems` doubles
 static int ensure_cv_block_ws(gpb200_handle* h, int64_t nV, int64_t elems) {
-    if (nV <= h->cvidx_cap && elems <= h->cvblk_cap) return GPB200_OK;
-    if (h->cvblk) cudaFree(h->cvblk);
-    if (h->cvidx) cudaFree(h->cvidx);
-    h->cvblk = nullptr; h->cvidx = nullptr; h->cvblk_cap = h->cvidx_cap = 0;
-    CK(cudaMalloc(&h->cvblk, sizeof(double) * elems));
-    CK(cudaMalloc(&h->cvidx, sizeof(long long) * nV));
-    h->cvblk_cap = elems; h->cvidx_cap = nV;
+    if ((size_t)nV <= h->cvidx.size() && (size_t)elems <= h->cvblk.size()) return GPB200_OK;
+    h->cvblk.reset(); h->cvidx.reset();
+    CK(h->cvblk.alloc(elems));
+    CK(h->cvidx.alloc(nV));
     return GPB200_OK;
 }
 
@@ -1855,7 +1812,7 @@ int gpb200_cv_param(gpb200_handle* h, int32_t param, const double* alpha, double
     if (rc) return rc;
     if (alpha) { rc = upload_padded(h, h->alpha, alpha); if (rc) return rc; h->alpha_ready = true; }
     const int Np = (int)h->Npad;
-    GemmBuf bD{h->tma_ok ? &h->mapCvD : nullptr, h->cvD, h->Npad}, bY{h->tma_ok ? &h->mapCvY : nullptr, h->cvY, h->Npad};
+    const GemmBuf bD = gbuf(h, h->cvD, h->mapCvD, h->Npad), bY = gbuf(h, h->cvY, h->mapCvY, h->Npad);
     const double* Yt = h->cvY;
     if (param >= 0) {
         CK(gram_grad_full_launch(h->prog, h->x, h->d, h->d, h->N, h->Npad, param, h->cvD, h->Npad, h->st, &h->launches));
@@ -1893,7 +1850,7 @@ int gpb200_cv_block(gpb200_handle* h, int32_t which, int64_t nV, const int64_t* 
             SCK(q, cudaMemcpyAsync(q->cvidx, idx, sizeof(long long) * nV, cudaMemcpyHostToDevice, q->st));
             SCK(q, shard_gather_block_own(q->cvblk, which == 0 ? q->G : cv_m(q), q->ld, q->cvidx, nV, own_of(q), q->st, &q->launches));
         }
-        TRY(coll_allreduce_sum(L, [&](gpb200_handle* q) { return q->cvblk; }, nn, [&](gpb200_handle* q) { return q->cvblk + nn; }));
+        TRY(coll_allreduce_sum(L, [&](gpb200_handle* q) { return q->cvblk.data(); }, nn, [&](gpb200_handle* q) { return q->cvblk + nn; }));
         CK(cudaMemcpyAsync(out, h->cvblk, sizeof(double) * nn, cudaMemcpyDeviceToHost, h->st));
         return sync_all(L);
     }
@@ -1914,16 +1871,13 @@ int gpb200_get_gram(gpb200_handle* h, double* K) {
     if (!h || !K) return GPB200_EINVAL;
     if (!h->has_data || !h->has_kernel) return fail(h, GPB200_ESTATE, "get_gram: set_data and set_kernel first");
     CK(cudaSetDevice(h->device));
-    double* tmp = nullptr;
-    const size_t nn = sizeof(double) * (size_t)h->Npad * (size_t)h->Npad;
-    CK(cudaMalloc(&tmp, nn));
-    cudaError_t e = launch_gram(h, tmp, h->Npad, 0, 1, 0, 0);
-    if (e == cudaSuccess)
-        e = cudaMemcpy2DAsync(K, sizeof(double) * h->N, tmp, sizeof(double) * h->Npad, sizeof(double) * h->N, h->N,
-                              cudaMemcpyDeviceToHost, h->st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
-    cudaFree(tmp);
-    CK(e);
+    DevBuf<double> tmp;
+    CK(tmp.alloc((size_t)h->Npad * (size_t)h->Npad));
+    CK(launch_gram(h, tmp, h->Npad, 0, 1, 0, 0));
+    CK(cudaMemcpy2DAsync(K, sizeof(double) * h->N, tmp, sizeof(double) * h->Npad, sizeof(double) * h->N, h->N,
+                         cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
+    tmp.reset();
     const int64_t N = h->N;
     for (int64_t i = 0; i < N; ++i)
         for (int64_t j = i + 1; j < N; ++j) K[i * N + j] = K[j * N + i];
@@ -2036,7 +1990,7 @@ int gpb200_ipc_import(gpb200_handle* h, int nranks, const char* all) {
     h->n_peer = n;
     int* words[7];
     for (int q = 0; q < n; ++q) words[q] = h->peer_sig[q] + h->rank;
-    if (!h->peer_sig_dev) CK(cudaMalloc(&h->peer_sig_dev, sizeof(int*) * 8));
+    if (!h->peer_sig_dev) CK(h->peer_sig_dev.alloc(8));
     CK(cudaMemcpy(h->peer_sig_dev, words, sizeof(int*) * n, cudaMemcpyHostToDevice));
     h->p2p = true;
     return GPB200_OK;

@@ -110,13 +110,11 @@ int gpb200_fsa_gemm_items(gpb200_handle* h, const int64_t* items, const double* 
     }
     if (n == 0) return GPB200_OK;
     CK(cudaSetDevice(h->device));
-    FsaGemmItem* d = nullptr;
-    CK(cudaMalloc(&d, sizeof(FsaGemmItem) * n));
-    cudaError_t e = cudaMemcpyAsync(d, v.data(), sizeof(FsaGemmItem) * n, cudaMemcpyHostToDevice, h->st);
-    if (e == cudaSuccess) e = fsa_gemm_launch(d, n, h->st, &h->launches);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
-    cudaFree(d);
-    CK(e);
+    DevBuf<FsaGemmItem> d;
+    CK(d.alloc(n));
+    CK(cudaMemcpyAsync(d, v.data(), sizeof(FsaGemmItem) * n, cudaMemcpyHostToDevice, h->st));
+    CK(fsa_gemm_launch(d, n, h->st, &h->launches));
+    CK(cudaStreamSynchronize(h->st));
     return GPB200_OK;
 }
 
@@ -125,11 +123,11 @@ int gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t 
     if (mode == 0 && n != 39) return fail(h, GPB200_EINVAL, "potrf_tiles: mode 0 takes 39 arguments");
     if (mode == 1 && (n <= 0 || n % 6)) return fail(h, GPB200_EINVAL, "potrf_tiles: mode 1 takes 6 arguments per tile");
     CK(cudaSetDevice(h->device));
-    int* dinfo = nullptr;
-    Potrf128Item* ditems = nullptr;
+    DevBuf<int> dinfo;
+    DevBuf<Potrf128Item> ditems;
     const int big = INT_MAX;
-    CK(cudaMalloc(&dinfo, sizeof(int)));
-    cudaError_t e = cudaMemcpyAsync(dinfo, &big, sizeof(int), cudaMemcpyHostToDevice, h->st);
+    CK(dinfo.alloc(1));
+    CK(cudaMemcpyAsync(dinfo, &big, sizeof(int), cudaMemcpyHostToDevice, h->st));
     if (mode == 0) {
         // G, ldg, F, ldf, Dinv, DinvT, logd, p0, ntiles, tile_stride, n_peer, then per peer (F, Dinv, DinvT, logd)
         const int64_t* a = args;
@@ -139,10 +137,10 @@ int gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t 
             pp.F[q] = reinterpret_cast<double*>(a[11 + 4 * q]); pp.Dinv[q] = reinterpret_cast<double*>(a[12 + 4 * q]);
             pp.DinvT[q] = reinterpret_cast<double*>(a[13 + 4 * q]); pp.logd[q] = reinterpret_cast<double*>(a[14 + 4 * q]);
         }
-        if (e == cudaSuccess && a[8] > 0)
-            e = potrf128_launch(reinterpret_cast<const double*>(a[0]), a[1], reinterpret_cast<double*>(a[2]), a[3],
+        if (a[8] > 0)
+            CK(potrf128_launch(reinterpret_cast<const double*>(a[0]), a[1], reinterpret_cast<double*>(a[2]), a[3],
                                 reinterpret_cast<double*>(a[4]), reinterpret_cast<double*>(a[5]), reinterpret_cast<double*>(a[6]),
-                                dinfo, (int)a[7], (int)a[8], (int)a[9], h->st, &h->launches, &pp);
+                                dinfo, (int)a[7], (int)a[8], (int)a[9], h->st, &h->launches, &pp));
     } else {
         const int nt = n / 6;
         std::vector<Potrf128Item> v(nt);
@@ -151,16 +149,13 @@ int gpb200_potrf_tiles(gpb200_handle* h, int mode, const int64_t* args, int32_t 
             v[i] = Potrf128Item{reinterpret_cast<const double*>(q[0]), reinterpret_cast<double*>(q[1]),
                                 reinterpret_cast<double*>(q[2]), reinterpret_cast<double*>(q[3]), q[4], (int)q[5], 0};
         }
-        if (e == cudaSuccess) e = cudaMalloc(&ditems, sizeof(Potrf128Item) * nt);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ditems, v.data(), sizeof(Potrf128Item) * nt, cudaMemcpyHostToDevice, h->st);
-        if (e == cudaSuccess) e = potrf128_ptr_launch(ditems, nt, dinfo, h->st, &h->launches);
+        CK(ditems.alloc(nt));
+        CK(cudaMemcpyAsync(ditems, v.data(), sizeof(Potrf128Item) * nt, cudaMemcpyHostToDevice, h->st));
+        CK(potrf128_ptr_launch(ditems, nt, dinfo, h->st, &h->launches));
     }
     int hinfo = big;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&hinfo, dinfo, sizeof(int), cudaMemcpyDeviceToHost, h->st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
-    cudaFree(dinfo);
-    if (ditems) cudaFree(ditems);
-    CK(e);
+    CK(cudaMemcpyAsync(&hinfo, dinfo, sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
     *info = hinfo;
     return GPB200_OK;
 }
@@ -190,15 +185,13 @@ int gpb200_trsv_tiles(gpb200_handle* h, int schedule, int direction, const int64
         CK(cudaStreamSynchronize(h->st));
         return GPB200_OK;
     }
-    int* flags = nullptr;
-    CK(cudaMalloc(&flags, sizeof(int) * (nb + 1)));
-    cudaError_t e = direction == 0 ? trsv_lower_fwd_fused(F, ldf, D, rhs, out, Npad, flags, h->st, &h->launches)
-                                   : trsv_lower_bwd_fused(F, ldf, D, rhs, out, Npad, flags, h->st, &h->launches);
+    DevBuf<int> flags;
+    CK(flags.alloc(nb + 1));
+    CK(direction == 0 ? trsv_lower_fwd_fused(F, ldf, D, rhs, out, Npad, flags, h->st, &h->launches)
+                      : trsv_lower_bwd_fused(F, ldf, D, rhs, out, Npad, flags, h->st, &h->launches));
     int wd = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&wd, flags + nb, sizeof(int), cudaMemcpyDeviceToHost, h->st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->st);
-    cudaFree(flags);
-    CK(e);
+    CK(cudaMemcpyAsync(&wd, flags + nb, sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CK(cudaStreamSynchronize(h->st));
     *watchdog = wd;
     return GPB200_OK;
 }
@@ -266,15 +259,6 @@ static int local_prog(gpb200_handle* h, const char* what, const double* theta, i
                 if (P.dims[P.doff[q] + k] >= d) return fail(h, GPB200_EINVAL, (std::string(what) + ": the program reads a dimension >= d").c_str());
     kprog_set_theta(P, theta);
     return GPB200_OK;
-}
-
-// Copies a host item list to a new device array (the caller frees it after the synchronize); none for an empty list.
-static cudaError_t items_to_device(const void* src, size_t bytes, void** d, cudaStream_t st) {
-    *d = nullptr;
-    if (!bytes) return cudaSuccess;
-    cudaError_t e = cudaMalloc(d, bytes);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(*d, src, bytes, cudaMemcpyHostToDevice, st);
-    return e;
 }
 
 int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
@@ -355,41 +339,39 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
     CK(cudaSetDevice(h->device));
     cudaStream_t st = h->st;
     int64_t* L = &h->launches;
-    FsaGramItem* dg = nullptr;
-    FsaRowItem* dr = nullptr;
-    FsaDxItem* dd = nullptr;
-    FsaBlockDxItem* db = nullptr;
-    cudaError_t e = bdx       ? items_to_device(bitems.data(), sizeof(FsaBlockDxItem) * bitems.size(), reinterpret_cast<void**>(&db), st)
-                    : sd == 6 ? items_to_device(ritems.data(), sizeof(FsaRowItem) * ritems.size(), reinterpret_cast<void**>(&dr), st)
-                    : sd == 4 ? items_to_device(ditems.data(), sizeof(FsaDxItem) * ditems.size(), reinterpret_cast<void**>(&dd), st)
-                              : items_to_device(gitems.data(), sizeof(FsaGramItem) * gitems.size(), reinterpret_cast<void**>(&dg), st);
-    if (e == cudaSuccess) {
-        switch (which) {
-        case 0: e = fsa_gram_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), fargs[nf - 1], st, L); break;
-        case 1: e = fsa_bdmv_launch((int)args[0], ptr(1), reinterpret_cast<const int*>(args[2]), reinterpret_cast<const long long*>(args[3]),
-                                    reinterpret_cast<const int*>(args[4]), reinterpret_cast<const long long*>(args[5]), ptr(6), ptr(7),
-                                    args[8], st, L); break;
-        case 2: e = fsa_mask_launch(ptr(0), args[1], args[2], args[3], ptr(4), ptr(5), st, L); break;
-        case 3: e = fsa_permute_launch((int)args[0], ptr(1), reinterpret_cast<const long long*>(args[2]), args[3], ptr(4), st, L); break;
-        case 4: e = fsa_resid_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
-        case 5: e = fsa_outer_launch(dg, ni, ptr(0), st, L); break;
-        case 6: e = fsa_trace_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), ptr(3), ptr(4), st, L); break;
-        case 7: e = fsa_axpy_t_launch(ptr(0), args[1], ptr(2), args[3], args[4], args[5], fargs[0], st, L); break;
-        case 8: e = fsa_crossgram_launch(P, ptr(0), ptr(1), (int)args[2], dg, ni, ptr(3), st, L); break;
-        case 9: e = fsa_rowdot_launch(dr, ni, st, L); break;
-        case 10: e = fsa_var_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
-        case 11: e = fsa_crossgram_dx_launch(P, ptr(0), ptr(1), ptr(2), (int)args[3], args[4], ptr(5), ptr(6), ptr(7), ptr(8),
-                                             args[9], ptr(10), ptr(11), ptr(12), args[13], dd, ni, ptr(14), ptr(15), st, L); break;
-        case 12: e = fsa_block_dx_launch(P, ptr(0), (int)args[1], db, ni, reinterpret_cast<const long long*>(args[2]), ptr(3),
-                                         (int)args[4], st, L); break;
-        }
+    DevBuf<FsaGramItem> dg;
+    DevBuf<FsaRowItem> dr;
+    DevBuf<FsaDxItem> dd;
+    DevBuf<FsaBlockDxItem> db;
+    auto items_to_device = [&](const auto& v, auto& d) -> cudaError_t {     // none for an empty list
+        if (v.empty()) return cudaSuccess;
+        const cudaError_t e = d.alloc(v.size());
+        return e != cudaSuccess ? e : cudaMemcpyAsync(d, v.data(), sizeof(v[0]) * v.size(), cudaMemcpyHostToDevice, st);
+    };
+    CK(bdx ? items_to_device(bitems, db) : sd == 6 ? items_to_device(ritems, dr)
+                                         : sd == 4 ? items_to_device(ditems, dd) : items_to_device(gitems, dg));
+    cudaError_t e = cudaSuccess;
+    switch (which) {
+    case 0: e = fsa_gram_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), fargs[nf - 1], st, L); break;
+    case 1: e = fsa_bdmv_launch((int)args[0], ptr(1), reinterpret_cast<const int*>(args[2]), reinterpret_cast<const long long*>(args[3]),
+                                reinterpret_cast<const int*>(args[4]), reinterpret_cast<const long long*>(args[5]), ptr(6), ptr(7),
+                                args[8], st, L); break;
+    case 2: e = fsa_mask_launch(ptr(0), args[1], args[2], args[3], ptr(4), ptr(5), st, L); break;
+    case 3: e = fsa_permute_launch((int)args[0], ptr(1), reinterpret_cast<const long long*>(args[2]), args[3], ptr(4), st, L); break;
+    case 4: e = fsa_resid_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
+    case 5: e = fsa_outer_launch(dg, ni, ptr(0), st, L); break;
+    case 6: e = fsa_trace_launch(P, ptr(0), (int)args[1], dg, ni, ptr(2), ptr(3), ptr(4), st, L); break;
+    case 7: e = fsa_axpy_t_launch(ptr(0), args[1], ptr(2), args[3], args[4], args[5], fargs[0], st, L); break;
+    case 8: e = fsa_crossgram_launch(P, ptr(0), ptr(1), (int)args[2], dg, ni, ptr(3), st, L); break;
+    case 9: e = fsa_rowdot_launch(dr, ni, st, L); break;
+    case 10: e = fsa_var_launch(ptr(0), ptr(1), ptr(2), ptr(3), args[4], st, L); break;
+    case 11: e = fsa_crossgram_dx_launch(P, ptr(0), ptr(1), ptr(2), (int)args[3], args[4], ptr(5), ptr(6), ptr(7), ptr(8),
+                                         args[9], ptr(10), ptr(11), ptr(12), args[13], dd, ni, ptr(14), ptr(15), st, L); break;
+    case 12: e = fsa_block_dx_launch(P, ptr(0), (int)args[1], db, ni, reinterpret_cast<const long long*>(args[2]), ptr(3),
+                                     (int)args[4], st, L); break;
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (dg) cudaFree(dg);
-    if (dr) cudaFree(dr);
-    if (dd) cudaFree(dd);
-    if (db) cudaFree(db);
     CK(e);
+    CK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
 

@@ -235,7 +235,7 @@ int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n, ScratchFn scratch) 
 template <class BufFn>
 int coll_allreduce_sum(const Locals& L, BufFn vec, size_t n) {
     if (L[0]->grp && n > 4096) return fail(L[0], GPB200_EINVAL, "coll_allreduce_sum: vector too long for the group scratch");
-    return coll_allreduce_sum(L, vec, n, [](gpb200_handle* q) { return q->red; });
+    return coll_allreduce_sum(L, vec, n, [](gpb200_handle* q) { return q->red.data(); });
 }
 int coll_allreduce_min_info(const Locals& L) {
     gpb200_handle* h0 = L[0];
@@ -277,12 +277,10 @@ int shard_pick_rb(gpb200_handle* h) {
 }
 
 void shard_free_buffers(gpb200_handle* h) {
-    for (int i = 0; i < 4; ++i) { if (h->P[i]) cudaFree(h->P[i]); h->P[i] = nullptr; }
-    for (int i = 0; i < 2; ++i) { if (h->XRbig[i]) cudaFree(h->XRbig[i]); h->XRbig[i] = nullptr; }
-    if (h->Sbuf) cudaFree(h->Sbuf);
-    if (h->red) cudaFree(h->red);
-    if (h->redi) cudaFree(h->redi);
-    h->Sbuf = h->red = nullptr; h->redi = nullptr; h->S_per_rank = 0;
+    for (DevBuf<double>& b : h->P) b.reset();
+    for (DevBuf<double>& b : h->XRbig) b.reset();
+    h->Sbuf.reset(); h->red.reset(); h->redi.reset();
+    h->S_per_rank = 0;
 }
 
 // free F / G whatever their mode (with the row-sharded cross-validation work matrices, which share their layout)
@@ -293,8 +291,7 @@ void free_FG(gpb200_handle* h) {
         h->g_sym = h->cv_m_ok = false;
         shard_free_buffers(h);
     } else {
-        if (h->F) cudaFree(h->F);
-        if (h->G) cudaFree(h->G);
+        h->Frep.reset(); h->Grep.reset();
     }
     h->F = h->G = nullptr;
     h->sharded = false;
@@ -309,11 +306,13 @@ bool make_FG_maps(gpb200_handle* h) {
 }
 
 int alloc_FG_replicated(gpb200_handle* h) {
-    const size_t nn = sizeof(double) * (size_t)h->Npad * (size_t)h->Npad;
-    CK(cudaMalloc(&h->F, nn));
-    CK(cudaMalloc(&h->G, nn));
-    CK(cudaMemsetAsync(h->F, 0, nn, h->st));
-    CK(cudaMemsetAsync(h->G, 0, nn, h->st));
+    const size_t nn = (size_t)h->Npad * (size_t)h->Npad;
+    CK(h->Frep.alloc(nn));
+    h->F = h->Frep;
+    CK(h->Grep.alloc(nn));
+    h->G = h->Grep;
+    CK(cudaMemsetAsync(h->F, 0, sizeof(double) * nn, h->st));
+    CK(cudaMemsetAsync(h->G, 0, sizeof(double) * nn, h->st));
     h->sharded = false;
     h->tma_ok = make_FG_maps(h);
     return GPB200_OK;
@@ -341,17 +340,17 @@ int alloc_FG_sharded(gpb200_handle* h) {
     h->G = (double*)h->vmG.base;
     const size_t nbp = (size_t)shard_panel_width(h);
     const size_t pelems = Np * nbp;
-    for (int i = 0; i < 4; ++i) CK(cudaMalloc(&h->P[i], sizeof(double) * pelems));
+    for (DevBuf<double>& b : h->P) CK(b.alloc(pelems));
     // all-gather staging: every rank's rows below a panel, padded to the largest per-rank count
     const size_t max_own_tiles = (size_t)shard_own_before(tiles, 0, h->rb, h->nranks);      // rank 0 owns the most
     h->S_per_rank = max_own_tiles * TILE * nbp;
     const size_t selems = std::max(h->S_per_rank * (size_t)h->nranks, pelems);
-    CK(cudaMalloc(&h->Sbuf, sizeof(double) * selems));
+    CK(h->Sbuf.alloc(selems));
     // batched LAUUM part of the inverse sweep: up to 4096 columns of row panels at a time (two buffers: look-ahead)
     h->xr_batch = std::max<int>(1, (int)(4096 / nbp));
-    for (int i = 0; i < 2; ++i) CK(cudaMalloc(&h->XRbig[i], sizeof(double) * (size_t)h->xr_batch * nbp * Np));
-    CK(cudaMalloc(&h->red, sizeof(double) * 4096 * 8));
-    CK(cudaMalloc(&h->redi, sizeof(int) * 16));
+    for (DevBuf<double>& b : h->XRbig) CK(b.alloc((size_t)h->xr_batch * nbp * Np));
+    CK(h->red.alloc(4096 * 8));
+    CK(h->redi.alloc(16));
     h->tma_ok = make_FG_maps(h) &&
                 gemm_make_tensor_map(&h->mapP[0], h->P[0], Np, nbp, nbp) &&
                 gemm_make_tensor_map(&h->mapP[1], h->P[1], Np, nbp, nbp) &&
@@ -541,7 +540,7 @@ int shard_cholesky_la(const Locals& L, int kb0 = 0) {
 
 // ---- triangular solves (one right-hand side) ---------------------------------------------------------------------
 // out = K_y^-1 rhs on every rank; rhs (device, Npad, zero padded) identical on every rank; tmp/y scratch vectors
-int shard_solve(const Locals& L, double* gpb200_handle::*rhs, double* gpb200_handle::*ybuf, double* gpb200_handle::*out) {
+int shard_solve(const Locals& L, DevBuf<double> gpb200_handle::*rhs, DevBuf<double> gpb200_handle::*ybuf, DevBuf<double> gpb200_handle::*out) {
     gpb200_handle* h0 = L[0];
     const int Np = (int)h0->Npad, R = h0->nranks, NBp = shard_panel_width(h0);
     const int nblk = (Np + NBp - 1) / NBp;
@@ -768,7 +767,7 @@ int shard_append_solve(const Locals& L, int b0, int Mv) {
         const int c0 = k * NBp, o = k % R, r1 = c0 + NBp;
         for (auto* q : L) {
             if (q->rank != o) continue;
-            GemmBuf bk{q->tma_ok ? &q->mapKst : nullptr, q->Kst, q->Npad};
+            const GemmBuf bk = gbuf(q, q->Kst, q->mapKst, q->Npad);
             SCK(q, trsm_rec_buf(q, bk, Mv, c0, NBp));
             SCK(q, cudaMemcpy2DAsync(q->P[0], sizeof(double) * NBp, q->Kst + c0, sizeof(double) * q->Npad, sizeof(double) * NBp,
                                      (size_t)Mv, cudaMemcpyDeviceToDevice, q->st));
@@ -820,7 +819,7 @@ int shard_append(const Locals& L, int64_t Nold) {
                     SCK(q, cudaMemcpy2DAsync(q->F + (size_t)t * TILE * q->ld, sizeof(double) * q->ld, q->Kst + (size_t)(t * TILE - b0) * q->Npad,
                                              sizeof(double) * q->Npad, sizeof(double) * b0, TILE, cudaMemcpyDeviceToDevice, q->st));
             // Schur complement of the own rows: G[r, c] -= V_r V_c',  r >= c >= b0
-            GemmBuf bv{q->tma_ok ? &q->mapKst : nullptr, q->Kst, q->Npad};
+            const GemmBuf bv = gbuf(q, q->Kst, q->mapKst, q->Npad);
             GemmDesc g = gemm_desc_default();
             g.A = GemmOperand{bv, bufNone(), 0, 0};
             g.B = GemmOperand{bv, bufNone(), 0, 0};
@@ -844,8 +843,8 @@ int shard_append(const Locals& L, int64_t Nold) {
 // Communication: N^2 / 2 doubles once per grad_prepare, N^2 per cv_param, plus the N-vectors.
 double* cv_y(gpb200_handle* h) { return (double*)h->vmCvY.base; }
 double* cv_m(gpb200_handle* h) { return (double*)h->vmCvM.base; }
-GemmBuf bufCvY(gpb200_handle* h) { return GemmBuf{h->tma_ok ? &h->mapShCvY : nullptr, cv_y(h), h->Npad}; }
-GemmBuf bufXRbig(gpb200_handle* h, int set) { return GemmBuf{h->tma_ok ? &h->mapXRbig[set] : nullptr, h->XRbig[set], h->Npad}; }
+GemmBuf bufCvY(gpb200_handle* h) { return gbuf(h, cv_y(h), h->mapShCvY, h->Npad); }
+GemmBuf bufXRbig(gpb200_handle* h, int set) { return gbuf(h, h->XRbig[set], h->mapXRbig[set], h->Npad); }
 
 // Y' and M_j of every rank, backed on the own rows like F and G; all ranks or none
 int shard_cv_alloc(const Locals& L) {

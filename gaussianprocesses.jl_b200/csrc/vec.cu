@@ -9,6 +9,7 @@
 //    CTAs of the same launch still read.
 //  * fixed-order reductions (dot, sum) so that mll / logdet are bitwise reproducible.
 //  * predictive mean / variance epilogues (/root/reference/src/GP.jl:26, 51-54, 75).
+#include "devbuf.cuh"
 #include "vec.cuh"
 #include <math.h>
 
@@ -160,8 +161,8 @@ cudaError_t fp64_peak_measure(cudaStream_t st, int64_t* launches, double* tflops
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int warps = 8, iters = 10000;
-    double* out = nullptr;
-    cudaError_t e = cudaMalloc(&out, sizeof(double) * sms * warps * 32);
+    DevBuf<double> out;
+    const cudaError_t e = out.alloc((size_t)sms * warps * 32);
     if (e != cudaSuccess) return e;
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -181,7 +182,7 @@ cudaError_t fp64_peak_measure(cudaStream_t st, int64_t* launches, double* tflops
     tflops[0] = 2.0 * 2048 * 8.0 * iters * warps * sms / best[0] * 1e-9;    // 8 x (16*8*16 FMA) per warp and iteration
     tflops[1] = 2.0 * 32 * 16.0 * iters * warps * sms / best[1] * 1e-9;
     cudaEventDestroy(e0); cudaEventDestroy(e1);
-    cudaFree(out);
+    out.reset();
     return cudaGetLastError();
 }
 

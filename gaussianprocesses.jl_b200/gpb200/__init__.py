@@ -1,6 +1,6 @@
 """gpb200 -- host-side mirror of the GaussianProcesses.jl GP / GPE / Kernel / predict_f surface
 over libgpb200.so (the H100-native exact-GP hot path).  See DESIGN.md / INTEGRATION.md."""
-from .capi import Engine, FitcEngine, LocalGroupEngine, PosDefException, load_library, declared_symbols, LIB_PATH
+from .capi import Engine, FitcEngine, LocalGroupEngine, PosDefException, load_library, declared_symbols, device_bytes, LIB_PATH
 from .kernels import (Kernel, SEIso, SEArd, SE, Mat12Iso, Mat32Iso, Mat52Iso, Mat12Ard, Mat32Ard, Mat52Ard, Matern,
                       RQIso, RQArd, RQ, Periodic, LinIso, LinArd, Poly, Noise, Const, SumKernel, ProdKernel, Masked,
                       FixedKernel, fix, flatten)

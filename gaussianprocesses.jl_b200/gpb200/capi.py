@@ -52,6 +52,7 @@ _SIGNATURES = {
     "gpb200_get_inverse_diag": (C.c_int, [_H, _dp]),
     "gpb200_get_timings": (C.c_int, [_H, _dp, C.c_int32]),
     "gpb200_launch_count": (C.c_int64, [_H]),
+    "gpb200_device_bytes": (C.c_int64, []),
     "gpb200_set_option": (C.c_int, [_H, C.c_char_p, C.c_int64]),
     "gpb200_set_stream": (C.c_int, [_H, C.c_void_p]),
     "gpb200_fp64_peak": (C.c_int, [_H, _dp, _dp]),
@@ -134,6 +135,11 @@ class PosDefException(np.linalg.LinAlgError):
     def __init__(self, info):
         super().__init__("matrix is not positive definite; Cholesky factorization failed (leading minor %d)" % info)
         self.info = info
+
+
+def device_bytes():
+    """Bytes of device memory the library's buffers hold now, over every engine of the process (diagnostics)."""
+    return int(load_library().gpb200_device_bytes())
 
 
 def _as_dp(a):

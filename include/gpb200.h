@@ -212,6 +212,9 @@ int  gpb200_get_timings(gpb200_handle* h, double* ms, int32_t n);   /* writes mi
 /* number of kernels enqueued by calls on this handle since creation (gpb200_rand includes its M x M sub-engine's
  * Cholesky); cudaMemsetAsync and copies are not counted */
 int64_t gpb200_launch_count(gpb200_handle* h);
+/* bytes of device memory the library's own buffers hold right now, over every handle of the process (diagnostics; the
+ * virtual-memory ranges of row-sharded storage and IPC peer mappings are not counted) */
+int64_t gpb200_device_bytes(void);
 /* tuning knobs (string key):
  *   "nb"         outer Cholesky block: 0 (default) = fully recursive, else 128*2^k <= 4096 (right-looking panels)
  *   "gemm"       0 = TMA/mbarrier DMMA kernel (default), 1 = simple-loader kernel (bring-up / cross-check)
