@@ -1,7 +1,7 @@
 // engine.cuh -- private to the engine's translation units; not installed and not part of the ABI.
 //   gpb200.cu            the dense engine (gpb200_handle) and its C ABI: schedules, IPC / NCCL, in-process groups
 //   kernel_contracts.cu  the raw kernels exposed for the parity tests and the roofline bench (include/gpb200.h)
-//   fitc_engine.cu       the sparse handle (gpb200_fitc): FITC / DTC / SoR, sparse cross-validation, rand
+//   fitc_engine.cu       the sparse handle (gpb200_fitc): FITC / DTC / SoR, sparse cross-validation, rand, append
 //   fsa_engine.cu        the FSA schedule of the sparse handle (mode 3)
 // It holds the handle structs, the error path, and the declarations of what one unit uses from another.
 #pragma once
@@ -178,6 +178,14 @@ struct FitcCvWs {
     bool ready = false;
     bool m_ok = false;                               // Dp / Q / del hold the state of the last cv_param since factorize
 };
+// gpb200_fitc_append: the unfactored Sigma_QR (Mpad x Mpad, lower tiles; allocated on first use, rebuilt once as L_s L_s'
+// after each factorize) and the running sums of the mll over all ranks: r'Lambda^-1 r, sum log Lambda, N
+struct FitcAppend {
+    DevBuf<double> sqr;
+    bool sqr_ok = false;             // sqr is Sigma_QR of the current data
+    bool sums_ok = false;            // s, l, n are those of the current data and residuals
+    double s = 0.0, l = 0.0, n = 0.0;
+};
 
 struct gpb200_fitc {
     gpb200_handle* eu = nullptr;     // K_uu  (+1e-10 I)            -> L_uu
@@ -208,6 +216,11 @@ struct gpb200_fitc {
     double x_ms[2] = {0, 0};
     FitcCvWs cv;                     // cross-validation workspace (first use)
     int cv_param = 0;
+    // rows the N-sized buffers hold (data, grad.gvec, the cross-validation N-vectors): N after set_data, grown
+    // geometrically by gpb200_fitc_append
+    int64_t Ncap = 0;
+    FitcAppend app;
+    bool u_ready = false;            // after gpb200_fitc_append: u, L_uu and L_s match the data, alpha does not (predictions only)
     // multi-GPU (gpb200_fitc_comm_init): the N observations are sharded over the ranks, every M x M object is replicated;
     // exchanged: one all-reduce of the M x M accumulator Sigma_QR (and of H for the kernel gradient), M-vectors, scalars
     ncclComm_t comm = nullptr;
@@ -301,6 +314,12 @@ inline int fail(gpb200_fitc* f, int code, const std::string& msg) {
 inline GemmBuf gbuf(const gpb200_handle* h, const double* p, const CUtensorMap& map, int64_t ld) {
     return GemmBuf{h->tma_ok ? &map : nullptr, p, ld};
 }
+// the factorisation, u and the kept append state no longer match the data, the kernel or the inducing points
+inline void fitc_invalidate(gpb200_fitc* f) {
+    f->factored = f->alpha_ready = f->u_ready = false;
+    f->app.sqr_ok = f->app.sums_ok = false;
+}
+
 inline GemmBuf bufF(gpb200_handle* h) { return gbuf(h, h->F, h->mapF, h->ld); }
 inline GemmBuf bufG(gpb200_handle* h) { return gbuf(h, h->G, h->mapG, h->ld); }
 inline GemmBuf bufDinv(gpb200_handle* h) { return gbuf(h, h->Dinv, h->mapDinv, TILE); }

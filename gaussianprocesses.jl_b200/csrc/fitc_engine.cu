@@ -1,5 +1,5 @@
 // fitc_engine.cu -- the sparse handle gpb200_fitc behind include/gpb200.h: FITC, DTC and SoR (modes 0-2), their
-// cross-validation and posterior draws.  The FSA schedule of the same handle (mode 3) is fsa_engine.cu.
+// cross-validation, posterior draws and append.  The FSA schedule of the same handle (mode 3) is fsa_engine.cu.
 #include "engine.cuh"
 #include "fitc_cv.cuh"
 #include "gram.cuh"
@@ -25,7 +25,7 @@ static int fitc_allreduce(gpb200_fitc* f, double* v, size_t n) {
 
 // every buffer that depends on the observations or the inducing points; the FSA blocks refer to the old observations too
 static void fitc_free_data(gpb200_fitc* f) {
-    f->data = {}; f->stage = {}; f->grad = {};
+    f->data = {}; f->stage = {}; f->grad = {}; f->app = {};
     f->pdx.reset(); f->dxu.reset(); f->dx.reset();
     fsa_free(f);
     f->cv = {};
@@ -40,7 +40,7 @@ int gpb200_fitc_comm_init(gpb200_fitc* f, int nranks, int rank, const char* id12
     memcpy(&id, id128, 128);
     FCKN(g_nccl.CommInitRank(&f->comm, nranks, id, rank));
     f->nranks = nranks; f->rank = rank;
-    f->factored = f->alpha_ready = false;
+    fitc_invalidate(f);
     return GPB200_OK;
 }
 
@@ -103,7 +103,8 @@ int gpb200_fitc_set_data(gpb200_fitc* f, int64_t N, int32_t d, const double* x, 
     TRY(fitc_stage_alloc(f, nc, "fitc_set_data"));
     FCK(cudaMemcpy2DAsync(f->data.x, sizeof(double) * d, x, sizeof(double) * ldx, sizeof(double) * d, N, cudaMemcpyHostToDevice, st));
     FCK(cudaStreamSynchronize(st));
-    f->has_data = true; f->factored = f->alpha_ready = false;
+    f->Ncap = N;
+    f->has_data = true; fitc_invalidate(f);
     return GPB200_OK;
 }
 
@@ -112,7 +113,7 @@ int gpb200_fitc_set_kernel(gpb200_fitc* f, int32_t n_ops, const int32_t* ops, in
     if (!f) return GPB200_EINVAL;
     FSUB(gpb200_set_kernel(f->eu, n_ops, ops, n_dims, dims, n_theta), f->eu);
     FSUB(gpb200_set_kernel(f->es, n_ops, ops, n_dims, dims, n_theta), f->es);
-    f->has_kernel = true; f->factored = f->alpha_ready = false;
+    f->has_kernel = true; fitc_invalidate(f);
     return GPB200_OK;
 }
 }  // extern "C"
@@ -203,7 +204,7 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
     if (!isfinite(log_noise)) return fail(f, GPB200_EINVAL, "fitc_factorize: non-finite logNoise");
     if (f->mode == 3) TRY(fsa_check(f, "fitc_factorize"));
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = f->cv.m_ok = false;
+    fitc_invalidate(f); f->cv.m_ok = false;
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     // K_uu + 1e-10 I and its factor (fitc.jl:139-141)
@@ -304,6 +305,7 @@ int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, d
     if (logdet) *logdet = ld;
     *mll = -(s[0] + ld + LOG2PI * f->Ntotal) / 2.0;
     f->alpha_ready = true;
+    f->app.sums_ok = false;                                              // the residuals may have changed
     return GPB200_OK;
 }
 
@@ -339,7 +341,7 @@ int gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise) {
 //   mu = K_xu u ;  var = k_xx - |L_uu^-1 k_ux|^2 + |L_s^-1 k_ux|^2
 int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* var) {
     if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu) return GPB200_EINVAL;
-    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict: factorize and mll first");
+    if (!f->factored || !(f->alpha_ready || f->u_ready)) return fail(f, GPB200_ESTATE, "fitc_predict: factorize and mll first");
     if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict: FSA predictions need test blocks");
     FCK(cudaSetDevice(f->device));
     gpb200_handle *eu = f->eu, *es = f->es;
@@ -380,7 +382,7 @@ int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ld
 int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* var,
                              double* dmu, double* dvar) {
     if (!f) return GPB200_EINVAL;
-    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict_grad: factorize and mll first");
+    if (!f->factored || !(f->alpha_ready || f->u_ready)) return fail(f, GPB200_ESTATE, "fitc_predict_grad: factorize and mll first");
     if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict_grad: not available for FSA");
     if (f->nranks > 1) return fail(f, GPB200_EINVAL, "fitc_predict_grad: single GPU handles only");
     if (Ms <= 0 || !xs || ldxs < f->d || !mu || !dmu) return fail(f, GPB200_EINVAL, "fitc_predict_grad: bad Ms, xs, ldxs, mu or dmu");
@@ -457,7 +459,7 @@ static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t 
 
 int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* cov) {
     if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu || !cov) return GPB200_EINVAL;
-    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict_cov: factorize and mll first");
+    if (!f->factored || !(f->alpha_ready || f->u_ready)) return fail(f, GPB200_ESTATE, "fitc_predict_cov: factorize and mll first");
     if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict_cov: FSA predictions need test blocks");
     if (Ms > f->Nc) return fail(f, GPB200_EINVAL, "fitc_predict_cov: too many test points for one staging chunk");
     FCK(cudaSetDevice(f->device));
@@ -529,7 +531,7 @@ static int fitc_grad(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, doubl
         FitcGradWs& g = f->grad;
         FCK(g.bufC.alloc((size_t)Nc * Mp));
         for (DevBuf<double>* p : {&g.Hbuf, &g.Wbuf, &g.Tbuf}) FCK(p->alloc((size_t)Mp * Mp));
-        FCK(g.gvec.alloc(f->N + TILE));
+        FCK(g.gvec.alloc(f->Ncap + TILE));
         FCK(g.betav.alloc(Mp));
         const size_t tiles = (size_t)std::max((Nc / TILE) * (Mp / TILE), (Mp / TILE) * (Mp / TILE));
         FCK(g.gpart.alloc(tiles * GPB200_MAX_THETA));
@@ -648,7 +650,7 @@ int gpb200_fitc_set_inducing(gpb200_fitc* f, int64_t M, const double* xu, int64_
         return fail(f, GPB200_EINVAL, "fitc_set_inducing: M must be set_data's, xu non-null and ldxu >= d");
     }
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = f->cv.m_ok = false;
+    fitc_invalidate(f); f->cv.m_ok = false;
     FSUB(gpb200_set_data(f->eu, M, f->d, xu, ldxu), f->eu);
     FSUB(gpb200_set_data(f->es, M, f->d, xu, ldxu), f->es);
     return GPB200_OK;
@@ -662,11 +664,166 @@ int gpb200_fitc_set_inputs(gpb200_fitc* f, int64_t N, const double* x, int64_t l
     if (!f->has_data) return fail(f, GPB200_ESTATE, "fitc_set_inputs: set_data first");
     if (N != f->N || !x || ldx < f->d) return fail(f, GPB200_EINVAL, "fitc_set_inputs: N must be set_data's, x non-null and ldx >= d");
     FCK(cudaSetDevice(f->device));
-    f->factored = f->alpha_ready = f->cv.m_ok = false;
+    fitc_invalidate(f); f->cv.m_ok = false;
     cudaStream_t st = f->eu->st;
     FCK(cudaMemcpy2DAsync(f->data.x, sizeof(double) * f->d, x, sizeof(double) * ldx, sizeof(double) * f->d, N, cudaMemcpyHostToDevice, st));
     if (f->fsa) TRY(fsa_set_inputs(f, x, ldx));
     FCK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+}  // extern "C"
+
+// the N-sized buffers hold at least n rows: capacity doubles (at least to n), x, Lambda and r are copied, and the
+// gradient and cross-validation workspaces, sized by the capacity, are freed to be remade at the next use
+static int fitc_grow(gpb200_fitc* f, int64_t n) {
+    if (n <= f->Ncap) return GPB200_OK;
+    const int64_t cap = std::max(n, 2 * f->Ncap);
+    cudaStream_t st = f->eu->st;
+    FitcData g;
+    FCK(g.x.alloc((size_t)cap * f->d));
+    for (DevBuf<double>* p : {&g.lam, &g.y, &g.alpha, &g.tmpn}) {
+        FCK(p->alloc(cap + TILE));
+        FCK(cudaMemsetAsync(*p, 0, sizeof(double) * (cap + TILE), st));
+    }
+    FCK(cudaMemcpyAsync(g.x, f->data.x, sizeof(double) * f->N * f->d, cudaMemcpyDeviceToDevice, st));
+    FCK(cudaMemcpyAsync(g.lam, f->data.lam, sizeof(double) * f->N, cudaMemcpyDeviceToDevice, st));
+    FCK(cudaMemcpyAsync(g.y, f->data.y, sizeof(double) * f->N, cudaMemcpyDeviceToDevice, st));
+    FCK(cudaStreamSynchronize(st));                                      // before the old buffers are freed
+    f->data.x = std::move(g.x); f->data.lam = std::move(g.lam); f->data.y = std::move(g.y);
+    f->data.alpha = std::move(g.alpha); f->data.tmpn = std::move(g.tmpn);
+    f->grad = {}; f->cv = {};
+    f->Ncap = cap;
+    return GPB200_OK;
+}
+
+extern "C" {
+// ================================================================================================
+// append! for FITC, DTC and SoR: k new observations with the hyper-parameters and Xu fixed.  K_uu, L_uu and the old rows'
+// Lambda_i do not change; Sigma_QR and b change by one rank-k term and one M-vector, so the cost is O(k M^2 + M^3) whatever
+// N is.  With K_nu (k x M) the cross-Gram of the new rows, Lambda_n their diagonal terms (FITC: sigma^2 + k_ii -
+// |L_uu^-1 k_ui|^2, by the launches gpb200_fitc_factorize runs on a chunk; DTC / SoR: sigma^2) and r_n their residuals:
+//   Sigma_QR <- Sigma_QR + K_un Lambda_n^-1 K_nu       (lower-only SYRK on the DMMA GEMM, as in factorize)
+//   b        <- b + K_un Lambda_n^-1 r_n
+//   s        <- s + sum r_n^2 / Lambda_n               (s = r'Lambda^-1 r)
+//   l        <- l + sum log Lambda_n                   (l = sum log Lambda_i)
+//   L_s = chol(Sigma_QR),  u = Sigma_QR^-1 b
+//   mll = -1/2 ( s - b'u + logdet Sigma_QR - logdet K_uu + l + N log 2 pi )
+// using r'alpha = r'Lambda^-1 r - b'Sigma_QR^-1 b: the mll of gpb200_fitc_mll on the concatenated data, without alpha.
+// The unfactored Sigma_QR is kept in f->app.sqr.  factorize leaves only its factor, so the first append after it rebuilds
+// Sigma_QR once as L_s L_s' (one lower-only NT product; GEMM_KHI_N stops each tile's k range at its diagonal tile, so the
+// strict-upper tiles of F, which other schedules use as scratch, are never read, and the diagonal tiles of F are clean above
+// their diagonal: the leaf writes i >= j only).  Later appends add to the kept copy, which is copied into es and factored.
+// s and l are summed over all rows (O(N), no kernel evaluation) on the first append after a mll and carried from then on.
+// On several ranks the call is collective: the M x M increment (accumulated in es->G, which the refactor overwrites
+// anyway), the b increment and the three scalars (s, l, N) are summed with one all-reduce each.
+// ================================================================================================
+int gpb200_fitc_append(gpb200_fitc* f, int64_t k, const double* xnew, int64_t ldx, const double* r_new, double* mll,
+                       double* logdet) {
+    if (!f) return GPB200_EINVAL;
+    if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_append: not available for FSA (mode 3); new rows would need new blocks, refit with set_data");
+    const bool multi = f->nranks > 1;
+    if (k < (multi ? 0 : 1)) return fail(f, GPB200_EINVAL, multi ? "fitc_append: k must be >= 0" : "fitc_append: k must be >= 1");
+    if (ldx < f->d) return fail(f, GPB200_EINVAL, "fitc_append: ldx must be >= d");
+    if (!mll || (k > 0 && (!xnew || !r_new))) return fail(f, GPB200_EINVAL, "fitc_append: xnew, r_new and mll must be non-null");
+    for (int64_t i = 0; i < k; ++i)
+        if (!std::isfinite(r_new[i])) return fail(f, GPB200_EINVAL, "fitc_append: non-finite r_new");
+    if (!f->factored || !(f->alpha_ready || f->u_ready)) return fail(f, GPB200_ESTATE, "fitc_append: factorize and mll first");
+    FCK(cudaSetDevice(f->device));
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    const int64_t Mp = f->Mpad, Nc = f->Nc, N0 = f->N, N1 = N0 + k;
+    const int d = f->d;
+    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp);
+    const GemmBuf bB = gbuf(eu, f->stage.bufB, f->stage.mapB, Nc);
+    if (!f->app.sqr_ok) {                                                // Sigma_QR = L_s L_s', once per factorize
+        FCK(f->app.sqr.ensure((size_t)Mp * Mp));
+        FCK(cudaMemsetAsync(f->app.sqr, 0, sizeof(double) * Mp * Mp, st));           // clean above the diagonal
+        FCK(gemm_whole(es, bufF(es), bufF(es), f->app.sqr, Mp, Mp, Mp, Mp, 1.0, 0.0, nullptr, 0, GEMM_LOWER_ONLY | GEMM_KHI_N));
+        f->app.sqr_ok = true;
+    }
+    TRY(fitc_grow(f, N1));
+    fsa_free(f);                                                         // FSA blocks partition the old rows only
+    // until the refactor below succeeds, the handle holds no factorisation of its data
+    f->factored = f->alpha_ready = f->u_ready = f->cv.m_ok = false;
+    es->inv_ready = false;                                               // es->G is scratch from here on
+    if (k > 0) {
+        FCK(cudaMemcpy2DAsync(f->data.x + N0 * d, sizeof(double) * d, xnew, sizeof(double) * ldx, sizeof(double) * d, k,
+                              cudaMemcpyHostToDevice, st));
+        FCK(cudaMemcpyAsync(f->data.y + N0, r_new, sizeof(double) * k, cudaMemcpyHostToDevice, st));
+    }
+    f->N = N1;
+    // one rank: the increment goes straight into the kept Sigma_QR; several: into es->G (ld Mpad, as in factorize), summed
+    // over the ranks below
+    double* dS = multi ? es->G : f->app.sqr.data();
+    if (multi) FCK(cudaMemsetAsync(es->G, 0, sizeof(double) * Mp * Mp, st));
+    FCK(cudaMemsetAsync(f->data.rhsm, 0, sizeof(double) * Mp, st));     // b increment
+    for (int64_t r0 = N0; r0 < N1; r0 += Nc) {
+        const int64_t nc = std::min(Nc, N1 - r0);
+        const int64_t ncp = (nc + TILE - 1) / TILE * TILE;              // the TRSM and the SYRK stop at the chunk's padded rows
+        const double* xr = f->data.x + r0 * d;
+        if (f->mode == 0) {                                              // as gpb200_fitc_factorize
+            FCK(fitc_kfu(f, xr, nc));
+            FCK(trsm_rec_buf(eu, bA, (int)ncp, 0, (int)Mp));
+            FCK(kdiag_launch(eu->prog, xr, d, nc, f->stage.tmpc, st, &eu->launches));
+            FCK(rowvar_launch(f->stage.bufA, Mp, f->stage.tmpc, nc, Mp, f->stage.tmpc2, st, &eu->launches));
+            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
+        } else {
+            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
+        }
+        FCK(fitc_kuf(f, xr, nc));
+        // b += K_un Lambda_n^-1 r_n   (as gpb200_fitc_mll)
+        FCK(cudaMemsetAsync(f->stage.w, 0, sizeof(double) * Nc, st));
+        FCK(ew_launch(1, nc, f->stage.w, f->data.y + r0, f->data.lam + r0, nullptr, 0.0, st, &eu->launches));
+        FCK(rowdot_launch(f->stage.bufB, Nc, f->stage.w, f->M, Nc, f->data.tmpm, st, &eu->launches));
+        FCK(ew_launch(2, f->M, f->data.rhsm, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+        // Sigma_QR += K_un Lambda_n^-1 K_nu
+        FCK(scale_launch(0, f->stage.bufB, Nc, Mp, nc, f->data.lam + r0, st, &eu->launches));
+        FCK(gemm_whole(es, bB, bB, dS, Mp, Mp, Mp, ncp, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
+    }
+    // s and l over the new rows, or over every row on the first append after a mll; and the row count
+    const int64_t s0 = f->app.sums_ok ? N0 : 0;
+    const double ns = (double)(N1 - s0);
+    FCK(cudaMemsetAsync(f->data.scal + 8, 0, sizeof(double) * 2, st));
+    if (N1 > s0) {
+        FCK(ew_launch(1, N1 - s0, f->data.tmpn + s0, f->data.y + s0, f->data.lam + s0, nullptr, 0.0, st, &eu->launches));
+        FCK(dot_launch(f->data.tmpn + s0, f->data.y + s0, N1 - s0, f->data.scal + 8, st, &eu->launches));
+        FCK(ew_launch(4, N1 - s0, f->data.tmpn + s0, f->data.lam + s0, nullptr, nullptr, 0.0, st, &eu->launches));
+        FCK(sum_launch(f->data.tmpn + s0, N1 - s0, f->data.scal + 9, st, &eu->launches));
+    }
+    FCK(cudaMemcpyAsync(f->data.scal + 10, &ns, sizeof(double), cudaMemcpyHostToDevice, st));
+    if (multi) {
+        TRY(fitc_allreduce(f, es->G, (size_t)Mp * Mp));
+        FCK(ew_launch(2, Mp * Mp, f->app.sqr, es->G, nullptr, nullptr, 0.0, st, &eu->launches));
+        TRY(fitc_allreduce(f, f->data.rhsm, (size_t)Mp));
+        TRY(fitc_allreduce(f, f->data.scal + 8, 3));
+    }
+    FCK(ew_launch(2, f->M, f->data.bvec, f->data.rhsm, nullptr, nullptr, 0.0, st, &eu->launches));
+    double sums[3];
+    FCK(cudaMemcpyAsync(sums, f->data.scal + 8, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    if (f->app.sums_ok) { f->app.s += sums[0]; f->app.l += sums[1]; f->app.n += sums[2]; }
+    else { f->app.s = sums[0]; f->app.l = sums[1]; f->app.n = sums[2]; f->app.sums_ok = true; }
+    // refactor the kept Sigma_QR; u = Sigma_QR^-1 b
+    FCK(cudaMemcpyAsync(es->G, f->app.sqr, sizeof(double) * Mp * Mp, cudaMemcpyDeviceToDevice, st));
+    const int rc = chol_inplace(es);
+    if (rc != GPB200_OK) {
+        fitc_invalidate(f);                                              // the grown data stays; factorize to go on
+        return fail(f, rc, "fitc_append (Sigma_QR): " + es->err);
+    }
+    FCK(cudaMemcpyAsync(f->data.rhsm, f->data.bvec, sizeof(double) * Mp, cudaMemcpyDeviceToDevice, st));
+    FCK(solve_device(es, f->data.rhsm, f->data.tmpm, f->data.uvec));
+    FCK(dot_launch(f->data.bvec, f->data.uvec, f->M, f->data.scal + 0, st, &eu->launches));
+    FCK(sum_launch(es->logd, es->Npad, f->data.scal + 1, st, &eu->launches));
+    FCK(sum_launch(eu->logd, eu->Npad, f->data.scal + 2, st, &eu->launches));
+    double s[3];
+    FCK(cudaMemcpyAsync(s, f->data.scal, sizeof(double) * 3, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+    FSUB(check_trsv_watchdog(es), es);                                   // the solve for u above
+    f->Ntotal = f->app.n;
+    f->factored = f->u_ready = true;
+    const double ld = s[1] - s[2] + f->app.l;
+    if (logdet) *logdet = ld;
+    *mll = -(f->app.s - s[0] + ld + LOG2PI * f->app.n) / 2.0;
     return GPB200_OK;
 }
 
@@ -696,17 +853,17 @@ static int fitc_cv_check(gpb200_fitc* f, const char* who) {
 static int fitc_cv_prepare(gpb200_fitc* f) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
-    const int64_t Mp = f->Mpad, Nc = f->Nc, N = f->N;
+    const int64_t Mp = f->Mpad, Nc = f->Nc, Ncap = f->Ncap;
     if (!f->cv.ready) TRY(make_group(f->cv, [&] {
         FitcCvWs& g = f->cv;
         for (DevBuf<double>* p : {&g.G, &g.Gt, &g.Ch, &g.P}) FCK(p->alloc((size_t)Nc * Mp));
         for (DevBuf<double>* p : {&g.Duu, &g.Dp, &g.R, &g.H, &g.Q}) FCK(p->alloc((size_t)Mp * Mp));
-        for (DevBuf<double>* p : {&g.alpha, &g.del, &g.ilam, &g.za, &g.dg}) FCK(p->alloc(N + Nc));
+        for (DevBuf<double>* p : {&g.alpha, &g.del, &g.ilam, &g.za, &g.dg}) FCK(p->alloc(Ncap + Nc));
         for (DevBuf<double>* p : {&g.da, &g.q, &g.lamV, &g.delV}) FCK(p->alloc(Nc));
         FCK(g.xs.alloc((size_t)Nc * f->d));
         FCK(g.m.alloc(8 * Mp));
         FCK(g.idx.alloc(Nc));
-        FCK(cudaMemsetAsync(g.alpha, 0, sizeof(double) * (N + Nc), st));      // zero tail: chunk vectors are read Nc wide
+        FCK(cudaMemsetAsync(g.alpha, 0, sizeof(double) * (Ncap + Nc), st));      // zero tail: chunk vectors are read Nc wide
         if (eu->tma_ok) {
             const bool ok = gemm_make_tensor_map(&g.mapGt, g.Gt, Mp, Nc, Nc) && gemm_make_tensor_map(&g.mapCh, g.Ch, Nc, Mp, Mp) &&
                             gemm_make_tensor_map(&g.mapP, g.P, Nc, Mp, Mp) && gemm_make_tensor_map(&g.mapDuu, g.Duu, Mp, Mp, Mp) &&
@@ -892,7 +1049,7 @@ int gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs,
     if ((f->mode == 3) != (block_of != nullptr)) {
         return fail(f, GPB200_EINVAL, "fitc_rand: block_of is required in FSA mode (3) and must be NULL otherwise");
     }
-    if (!f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_rand: factorize and mll first");
+    if (!f->factored || !(f->alpha_ready || f->u_ready)) return fail(f, GPB200_ESTATE, "fitc_rand: factorize and mll first");
     if (f->mode != 3 && Ms > f->Nc) return fail(f, GPB200_EINVAL, "fitc_rand: too many test points for one staging chunk");
     FCK(cudaSetDevice(f->device));
     gpb200_handle* eu = f->eu;
@@ -929,7 +1086,7 @@ int gpb200_fitc_get_timings(gpb200_fitc* f, double* ms, int32_t n) {
 
 int gpb200_fitc_set_mode(gpb200_fitc* f, int mode) {
     if (!f || mode < 0 || mode > 3) return GPB200_EINVAL;
-    f->mode = mode; f->factored = f->alpha_ready = false;
+    f->mode = mode; fitc_invalidate(f);
     return GPB200_OK;
 }
 

@@ -115,7 +115,7 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
     }
     FCK(cudaSetDevice(f->device));
     fsa_free(f);
-    f->factored = f->alpha_ready = false;
+    fitc_invalidate(f);
     // set_data sizes the staging chunk to N; the padded blocks and the padded test groups of FSA predictions need the
     // full chunk, so grow it to the cap set_data applies to large N (with every workspace sized by the chunk)
     const int64_t cap = std::min<int64_t>((int64_t)(2.0e9 / (8.0 * (double)f->Mpad)) / TILE * TILE, 32768);

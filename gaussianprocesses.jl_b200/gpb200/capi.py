@@ -84,6 +84,7 @@ _SIGNATURES = {
     "gpb200_fitc_set_inducing": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
     "gpb200_fitc_grad_kernel_inputs": (C.c_int, [_H, _dp, _dp, _dp]),
     "gpb200_fitc_set_inputs": (C.c_int, [_H, C.c_int64, _dp, C.c_int64]),
+    "gpb200_fitc_append": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp]),
     "gpb200_fitc_predict": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp]),
     "gpb200_fitc_predict_grad": (C.c_int, [_H, C.c_int64, _dp, C.c_int64, _dp, _dp, _dp, _dp]),
     "gpb200_fitc_comm_init": (C.c_int, [_H, C.c_int, C.c_int, C.c_char_p]),
@@ -581,6 +582,20 @@ class FitcEngine:
         if x_pm.shape != (self.N, self.d):
             raise ValueError("fitc_set_inputs: the inputs must keep their shape (%d, %d)" % (self.N, self.d))
         self._check(self._lib.gpb200_fitc_set_inputs(self._h, self.N, _as_dp(x_pm), self.d), "fitc_set_inputs")
+
+    def append(self, xnew_pm, r_new):
+        """append the rows xnew_pm (k, d) with residuals r_new = y - m(x) (k,): (mll, logdet) of the grown data.  Predictions
+        work at once; alpha, the gradients and cross-validation need mll(y - m(x)) over all rows first."""
+        xnew_pm = np.ascontiguousarray(xnew_pm, dtype=np.float64).reshape(-1, self.d)
+        r = np.ascontiguousarray(r_new, dtype=np.float64).ravel()
+        if r.size != xnew_pm.shape[0]:
+            raise ValueError("fitc_append: %d rows, but %d residuals" % (xnew_pm.shape[0], r.size))
+        m, ld = C.c_double(), C.c_double()
+        rc = self._lib.gpb200_fitc_append(self._h, r.size, _as_dp(xnew_pm), self.d, _as_dp(r), C.byref(m), C.byref(ld))
+        if rc == OK or rc > 0:                                   # a Sigma_QR that is not positive definite keeps the grown data
+            self.N += r.size
+        self._check(rc, "fitc_append")
+        return m.value, ld.value
 
     def grad_inputs_timings(self):
         """device times (ms) of the last grad_kernel_inputs: the dmll/dX contractions summed, the whole call"""

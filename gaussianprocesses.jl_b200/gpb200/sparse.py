@@ -56,8 +56,43 @@ class FITC:
         self.target = self.mll
         return self
 
+    def append(self, x, y):
+        """append!(gp, x, y) for the sparse strategies (GPEelastic.jl:13-22 has it for the dense model only): add
+        observations keeping the hyper-parameters and the inducing points.  The device adds the new rows' rank-k term to
+        Sigma_QR and refactors it, O(k M^2 + M^3) whatever nobs is, and returns the mll of the grown data; mll and target are
+        set from it.  predict_f, predict_y, predict_f_grad and rand work at once.  alpha is None until the next update_mll,
+        which the gradient and cross-validation methods call first when they need it.  On a distributed model x / y are
+        this rank's new observations; the call is collective and a rank may pass none."""
+        x = _as_dxn(x)
+        if x.shape[0] != self.dim:
+            raise ValueError("Input observations must have the same dimension as the GP")
+        y = np.atleast_1d(np.asarray(y, dtype=np.float64)).ravel()
+        if x.shape[1] != y.size:
+            raise ValueError("%d observations, but %d targets." % (x.shape[1], y.size))        # GPEelastic.jl:15
+        xpm = np.ascontiguousarray(x.T)
+        try:
+            self.mll, self.logdet = self._eng.append(xpm, y - self.mean.mean(xpm))
+        except capi.PosDefException:                              # the device keeps the grown data; update_mll refits it
+            self.mll = self.target = float("nan")
+            raise
+        finally:
+            if self._eng.N == self.nobs + y.size:
+                self.x = np.concatenate([self.x, x], axis=1)
+                self.y = np.concatenate([self.y, y])
+                self.nobs = self.y.size
+                self._xpm = np.ascontiguousarray(self.x.T)
+                self.alpha = None
+        self.target = self.mll
+        return self
+
+    def _need_alpha(self):
+        """alpha of the current data: after append it is refreshed by update_mll (factorize + mll)"""
+        if self.alpha is None:
+            self.update_mll()
+
     def update_dmll_noise_mean(self):
         """[dmll_noise (fitc.jl:243-257); dmll_mean! (GPE.jl:282-288)] -- kernel part not built yet."""
+        self._need_alpha()
         out = [self._eng.grad_noise()]
         if self.mean.num_params() > 0:
             out.extend(self.mean.grad_stack(self._xpm).T @ self.alpha)
@@ -69,6 +104,7 @@ class FITC:
         dmll/dXu as vec(Xu) (one point after another); inputs=True then appends dmll/dX as vec(X) (on a distributed model:
         this rank's points), the device's part plus alpha_i dm(x_i)/dx_i.  The kernel part and the point gradients come from
         one device sweep."""
+        self._need_alpha()
         out = []
         if noise:
             out.append(self._eng.grad_noise())                                   # fitc.jl:243-257
@@ -205,7 +241,8 @@ class FITC:
     # GPE's host assembly, unchanged: the engine's inverse_diag / cv_param / cv_block stream the N rows against the M x M
     # inverses instead of reading a resident N x N inverse.
     def _cv_prepare(self):
-        """the sparse engine's CV entry points prepare their own M x M inverses"""
+        """the sparse engine's CV entry points prepare their own M x M inverses; alpha must be that of the current data"""
+        self._need_alpha()
 
     predict_LOO = GPE.predict_LOO
     logp_LOO = GPE.logp_LOO
@@ -263,6 +300,10 @@ class FSA(FITC):
         self._block_ptr, self._idx = blocks_to_csr(self.blockindices, x.shape[1])
         self._pending_blocks = True
         super().__init__(x, Xu, y, mean=mean, kernel=kernel, logNoise=logNoise, device=device)
+
+    def append(self, x, y):
+        raise ValueError("append is not available for FSA: new observations would need new blocks; build the model again "
+                         "with the grown data and blocks")
 
     def update_mll(self, noise=True, domean=True, kern=True):
         """update_mll! with cK::FullScalePDMat (update_cK! :197-230, `\\` :105-108, logdet :142)."""

@@ -551,6 +551,32 @@ function dmll_inputs(gp::GPE{X,Y,M,K,CS,D,P}) where {X,Y,M,K,CS<:B200SparseStrat
     return g .+ mean_dx(gp.mean, gp.x) .* reshape(gp.alpha, 1, :)
 end
 
+# append! for FITC / DTC / SoR (the reference has it for ElasticGPE only, GPEelastic.jl:13-22): new observations with the
+# hyper-parameters and Xu kept.  gpb200_fitc_append adds the new rows' rank-k term to Sigma_QR and refactors it, O(k M^2 +
+# M^3) whatever nobs is, and returns the mll of the grown data; gp.x, gp.y, gp.nobs, gp.mll and gp.target are updated and
+# predict_f / rand work at once.  gp.alpha still holds the old data's alpha: the next update_mll! (update_target!) refreshes
+# it, and the gradients need it.  B200FSA throws: new observations would need new blocks.
+Base.append!(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractVector, y::Float64) where {X,Y,M,K,CS<:B200Sparse,D,P} =
+    append!(gp, reshape(x, :, 1), [y])
+function Base.append!(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix, y::AbstractVector) where {X,Y,M,K,CS<:B200Sparse,D,P}
+    size(x, 2) == length(y) || error("$(size(x, 2)) observations, but $(length(y)) targets.")       # GPEelastic.jl:14
+    size(x, 1) == gp.dim || throw(ArgumentError("Input observations must have the same dimension as the GP"))
+    Xn = Matrix{Float64}(x); k = length(y)
+    r = Vector{Float64}(y .- mean(gp.mean, Xn))
+    mll = Ref{Float64}(0.0); ld = Ref{Float64}(0.0)
+    checks(gp.cK, ccall((:gpb200_fitc_append, LIB), Cint,
+                        (Ptr{Cvoid}, Int64, Ptr{Float64}, Int64, Ptr{Float64}, Ref{Float64}, Ref{Float64}),
+                        gp.cK.handle, k, Xn, size(Xn, 1), r, mll, ld), "fitc_append")
+    gp.x = convert(X, hcat(gp.x, Xn)); gp.y = convert(Y, vcat(gp.y, y)); gp.nobs += k
+    gp.cK.n += k; gp.cK.logdet = ld[]
+    gp.mll = mll[]
+    gp.target = gp.mll + GaussianProcesses.prior_logpdf(gp.mean) + GaussianProcesses.prior_logpdf(gp.kernel) +
+                GaussianProcesses.prior_logpdf(gp.logNoise)                                          # GPE.jl:348
+    return gp
+end
+Base.append!(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractVecOrMat, y) where {X,Y,M,K,CS<:B200FSA,D,P} =
+    throw(ArgumentError("append!: not available for B200FSA (new observations would need new blocks); build the GP again"))
+
 function predict_f(gp::GPE{X,Y,M,K,CS,D,P}, x::AbstractMatrix; full_cov::Bool=false) where {X,Y,M,K,CS<:B200Sparse,D,P}
     size(x, 1) == gp.dim || throw(ArgumentError("Gaussian Process object and input observations do not have consistent dimensions"))
     Xs = Matrix{Float64}(x); Ms = size(Xs, 2)

@@ -468,6 +468,20 @@ int  gpb200_fitc_grad_kernel_inputs(gpb200_fitc* f, double* dmll_kernel, double*
  * handle given the same x to gpb200_fitc_set_data (and the same gpb200_fitc_set_blocks).  With several ranks every rank
  * passes its own slice.  No kernel is launched.                                                                        */
 int  gpb200_fitc_set_inputs(gpb200_fitc* f, int64_t N, const double* x, int64_t ldx);
+/* append! for FITC, DTC and SoR (modes 0-2; not in the reference for the sparse strategies): k new observations (xnew:
+ * d x k column-major, ld = ldx; r_new[k] = y - m(x) of the new rows) with the hyper-parameters and Xu of the last
+ * factorize.  Sigma_QR, b = K_uf Lambda^-1 r and the mll's scalars are updated by the new rows only and Sigma_QR is
+ * refactored: O(k M^2 + M^3) whatever N is; no pass over the old rows' kernel values.  mll (and logdet, may be NULL) are
+ * those gpb200_fitc_mll gives on the concatenated data.  Needs factorize + mll, or an earlier successful append
+ * (GPB200_ESTATE otherwise).  GPB200_EINVAL, nothing changed: mode 3 (FSA), k < 1 (k < 0 on several ranks), ldx < d, a NULL
+ * xnew, r_new or mll, a non-finite r_new.  Afterwards u, L_uu and L_s match the data: gpb200_fitc_predict, _predict_cov,
+ * _predict_grad and _rand accept the handle; grad_noise, the kernel gradients and cross-validation need alpha and return
+ * GPB200_ESTATE until gpb200_fitc_mll is called with the full residuals (the last cv_param's state is cleared).  The
+ * N-sized buffers grow geometrically; FSA blocks set earlier are dropped.  A Sigma_QR that is not positive definite
+ * returns its leading minor (> 0): the factorisation is cleared, the grown data stays.  On several ranks the call is
+ * collective: each rank passes its own rows (k may be 0 on some ranks).                                               */
+int  gpb200_fitc_append(gpb200_fitc* f, int64_t k, const double* xnew, int64_t ldx, const double* r_new, double* mll,
+                        double* logdet);
 /* mu_minus_mean[Ms], var[Ms] (may be NULL; not clamped) */
 int  gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu_minus_mean, double* var);
 /* Predictive gradients of FITC / DTC / SoR with respect to the test inputs, as gpb200_predict_grad (same layouts, var and
