@@ -1095,8 +1095,7 @@ int gpb200_set_data(gpb200_handle* h, int64_t N, int32_t d, const double* x, int
                              cudaMemcpyHostToDevice, h->st));
         if (!h->xpt) CK(h->xpt.alloc(Npad * h->dxp));
         CK(shard_transpose(h->xpt, Npad, h->xp, h->dxp, Npad, h->dxp, h->st, &h->launches));
-        h->xmap_ok = gemm_make_tensor_map_plain(&h->mapX, h->xp, N, h->dxp, h->dxp, TILE, h->dxp) &&
-                     gemm_make_tensor_map_plain(&h->mapXT, h->xpt, h->dxp, N, Npad, h->dxp, TILE);
+        h->xmap_ok = seiso_make_x_maps(&h->mapX, &h->mapXT, h->xp, h->xpt, h->dxp, N, Npad);
     }
     CK(cudaStreamSynchronize(h->st));
     h->has_data = true;
@@ -1660,8 +1659,7 @@ static int append_inputs(gpb200_handle* h, int64_t k, const double* xnew, int64_
     if (h->xp) {
         CK(cudaMemcpy2DAsync(h->xp + Nold * h->dxp, sizeof(double) * h->dxp, xnew, sizeof(double) * ldx, sizeof(double) * d, k, cudaMemcpyHostToDevice, h->st));
         CK(shard_transpose(h->xpt, Np, h->xp, h->dxp, Np, h->dxp, h->st, &h->launches));
-        h->xmap_ok = gemm_make_tensor_map_plain(&h->mapX, h->xp, Nnew, h->dxp, h->dxp, TILE, h->dxp) &&
-                     gemm_make_tensor_map_plain(&h->mapXT, h->xpt, h->dxp, Nnew, Np, h->dxp, TILE);
+        h->xmap_ok = seiso_make_x_maps(&h->mapX, &h->mapXT, h->xp, h->xpt, h->dxp, Nnew, Np);
     }
     h->N = Nnew;
     h->inv_ready = h->s_ready = h->alpha_ready = false; h->g_sym = false; h->cv_m_ok = false;

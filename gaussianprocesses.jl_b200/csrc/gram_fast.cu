@@ -17,6 +17,7 @@
 // exponential of the rounded argument (the argument's own rounding, |x| eps relative, is what any exp(-r/2l^2) carries).
 // 25 FP64 instructions per output instead of ~46.
 #include "gram_fast.cuh"
+#include "gemm_nt.cuh"
 #include <math.h>
 #include <stdint.h>
 
@@ -322,6 +323,10 @@ bool seiso_fast_prepare(double l2, double s2, SeIsoFast* out) {
     out->s2 = s2;
     for (int j = 0; j < 64; ++j) out->tab[j] = (double)((long double)s2 * exp2l((long double)j / 64.0L));
     return true;
+}
+
+bool seiso_make_x_maps(CUtensorMap* mapX, CUtensorMap* mapXT, const double* xp, const double* xpt, int dx, int64_t N, int64_t Npad) {
+    return gemm_make_tensor_map_plain(mapX, xp, N, dx, dx, TB, dx) && gemm_make_tensor_map_plain(mapXT, xpt, dx, N, Npad, dx, TB);
 }
 
 cudaError_t gram_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* mapXT, int dx, const SeIsoFast& sf, int64_t N, int64_t Npad,

@@ -12,6 +12,10 @@ struct SeIsoFast {
 };
 // false if (l2, s2) lie outside the range in which the exponent arithmetic of the fast exp is safe
 bool seiso_fast_prepare(double l2, double s2, SeIsoFast* out);
+// The two descriptors the kernels below take, as the engine builds them: mapX over xp [N x dx] (row pitch dx), box 128 x dx;
+// mapXT over the transposed copy xpt [dx x N] (row pitch Npad), box dx x 128.  Rows of xp and columns of xpt at or past N
+// lie outside the maps: TMA fills them with zeros and never reads them.  False if a descriptor cannot be encoded.
+bool seiso_make_x_maps(CUtensorMap* mapX, CUtensorMap* mapXT, const double* xp, const double* xpt, int dx, int64_t N, int64_t Npad);
 // mapX: plain TMA descriptor of the inputs stored [N x dx] (dx even, <= 8, zero padded), box 128 x dx;
 // mapXT: descriptor of the transposed copy [dx x N] (row pitch Npad), box dx x 128
 cudaError_t gram_seiso_tma_launch(const CUtensorMap* mapX, const CUtensorMap* mapXT, int dx, const SeIsoFast& sf, int64_t N, int64_t Npad,

@@ -7,6 +7,7 @@
 #include "fsa.cuh"
 #include "gpa.cuh"
 #include "gram.cuh"
+#include "gram_fast.cuh"
 #include "potrf_base.cuh"
 #include "vec.cuh"
 
@@ -376,8 +377,8 @@ int gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t
 }
 
 int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
-    if (!h || (n > 0 && !args) || which < 0 || which > 10 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
-    static const int want[11] = {14, 11, 7, 5, 10, 12, 13, 11, 6, 13, 3};
+    if (!h || (n > 0 && !args) || which < 0 || which > 13 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    static const int want[14] = {14, 11, 7, 5, 10, 12, 13, 11, 6, 13, 3, 12, 14, 14};
     if (n != want[which]) return fail(h, GPB200_EINVAL, "gram_kernels: wrong argument count for this kernel");
     const int64_t* a = args;
     auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
@@ -391,10 +392,10 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
     KProg P{};
     int64_t d = 1;
     if (which != 10) {
-        static const int dpos[10] = {2, 8, 4, 2, 2, 8, 2, 6, 2, 6};
+        static const int dpos[14] = {2, 8, 4, 2, 2, 8, 2, 6, 2, 6, 0, 2, 2, 2};
         d = a[dpos[which]];
         if (d < 1 || d > GPB200_MAX_DIMS) return fail(h, GPB200_EINVAL, "gram_kernels: d outside 1 .. GPB200_MAX_DIMS");
-        const int32_t extra = (which == 0 || which == 9) ? 1 : 0;       // nugget / c after theta
+        const int32_t extra = (which == 0 || which == 9 || which == 12) ? 1 : 0;       // nugget / c after theta
         if (h->has_kernel && nf != h->prog.n_theta + extra)
             return fail(h, GPB200_EINVAL, "gram_kernels: fargs = theta (+ nugget for gram_lower, c for crossgram_dx)");
         TRY(local_prog(h, "gram_kernels", fargs, h->prog.n_theta, d, P));
@@ -403,6 +404,14 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
     }
     const int np = P.n_theta;
     auto jok = [&](int i) { return a[i] >= 0 && a[i] < np; };
+    // the TMA-staged SEIso kernels (12, 13): the single SEIso leaf over d <= 8 dimensions with constants the fast exp accepts,
+    // 16-byte aligned inputs xp [N x dx] and xpt [dx x Npad], dx = d rounded up to even
+    const bool tma = which == 12 || which == 13;
+    SeIsoFast sf{};
+    if (tma && !(kprog_fast(P, (int)d) && d <= 8 && seiso_fast_prepare(P.par[0], P.par[1], &sf) && need({0, 1}) &&
+                 a[0] % 16 == 0 && a[1] % 16 == 0 && a[3] >= 1))
+        return fail(h, GPB200_EINVAL, "gram_kernels: the TMA kernels take a single SEIso leaf over d <= 8 dimensions whose "
+                                      "constants seiso_fast_prepare accepts, N >= 1 and 16-byte aligned xp and xpt");
     bool ok = true;
     switch (which) {
     case 0:     // x, ldx, d, N, Npad, noise_var, n_noise, G, ldg, own_tiles, nranks, rank, own_axis, bm_min
@@ -441,6 +450,18 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
     case 10:    // F, ld, Npad
         ok = need({0}) && a[2] >= 0 && a[2] % TILE == 0 && a[1] >= a[2];
         break;
+    case 11:    // x, ldx, d, N, alpha, G, ldg, out, bm_mod, bm_rem, bm_div, fast
+        ok = need({0, 5, 7}) && a[1] >= d && a[3] >= 0 && a[6] >= a[3] && a[8] >= 1 && a[9] >= 0 && a[9] < a[8] && a[10] >= 1 &&
+             (a[11] == 0 || (a[11] == 1 && kprog_fast(P, (int)d) && d <= 8));
+        break;
+    case 12:    // xp, xpt, d, N, Npad, noise_var, n_noise, G, ldg, own_tiles, nranks, rank, own_axis, sf
+        ok = need({5, 7}) && padded(3, 4) && (a[6] == 1 || a[6] == a[3]) && vec2(7, 8) && a[8] >= a[4] && a[9] >= 0 &&
+             a[10] >= 1 && a[11] >= 0 && a[11] < a[10] && (a[12] == 0 || a[12] == 1);
+        break;
+    case 13:    // xp, xpt, d, N, Npad, alpha, Kinv, ldg, part, out, bm_mod, bm_rem, bm_div, sf
+        ok = need({5, 6, 8, 9}) && padded(3, 4) && vec2(6, 7) && a[7] >= a[4] && a[10] >= 1 && a[11] >= 0 && a[11] < a[10] &&
+             a[12] >= 1;
+        break;
     }
     if (!ok) return fail(h, GPB200_EINVAL, "gram_kernels: a null pointer, a negative size, a bad padding, leading dimension or "
                                            "alignment, j outside [0, n_theta) or a bad ownership argument");
@@ -448,6 +469,17 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
     cudaStream_t st = h->st;
     int64_t* L = &h->launches;
     const int id = (int)d;
+    const int dx = (id + 1) / 2 * 2;
+    CUtensorMap mx, mxt;
+    if (tma) {
+        if (!seiso_make_x_maps(&mx, &mxt, ptr(0), ptr(1), dx, a[3], a[4]))
+            return fail(h, GPB200_ECUDA, "gram_kernels: TMA descriptors of xp / xpt could not be built");
+        if (a[13]) {                                     // the prepared constants: c_hi, il2, s2, tab[64]
+            double* o = reinterpret_cast<double*>(a[13]);
+            o[0] = sf.c_hi; o[1] = sf.il2; o[2] = sf.s2;
+            for (int j = 0; j < 64; ++j) o[3 + j] = sf.tab[j];
+        }
+    }
     cudaError_t e = cudaSuccess;
     switch (which) {
     case 0: e = gram_lower_launch(P, ptr(0), a[1], id, a[3], a[4], ptr(5), a[6], fargs[nf - 1], ptr(7), a[8], st, L, (int)a[9],
@@ -464,9 +496,54 @@ int gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
     case 9: e = crossgram_dx_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], id, ptr(7), ptr(8), ptr(9), a[10], fargs[nf - 1],
                                     ptr(11), ptr(12), st, L); break;
     case 10: e = mirror_lower_tiles_launch(ptr(0), a[1], a[2], st, L); break;
+    case 11: e = inputs_dx_launch(P, a[11] != 0, ptr(0), a[1], id, a[3], ptr(4), ptr(5), a[6], ptr(7), st, L, (int)a[8], (int)a[9],
+                                  (int)a[10]); break;
+    case 12: e = gram_seiso_tma_launch(&mx, &mxt, dx, sf, a[3], a[4], ptr(5), a[6], fargs[nf - 1], ptr(7), a[8], st, L, (int)a[9],
+                                       (int)a[10], (int)a[11], (int)a[12]); break;
+    case 13: e = trace_seiso_tma_launch(&mx, &mxt, dx, sf, a[3], a[4], ptr(5), ptr(6), a[7], ptr(8), ptr(9), st, L, (int)a[10],
+                                        (int)a[11], (int)a[12]); break;
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     CK(e);
+    return GPB200_OK;
+}
+
+int gpb200_vec_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf) {
+    if (!h || !args || which < 0 || which > 3 || nf < 0 || (nf > 0 && !fargs)) return GPB200_EINVAL;
+    static const int want[4] = {6, 6, 5, 5};
+    static const int wantf[4] = {1, 1, 0, 0};
+    if (n != want[which] || nf != wantf[which])
+        return fail(h, GPB200_EINVAL, "vec_kernels: wrong argument count for this kernel (fargs = s for ew, nugget for spd_from_cov)");
+    const int64_t* a = args;
+    auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
+    auto need = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (!a[i]) return false;
+        return true;
+    };
+    bool ok = true;
+    switch (which) {
+    case 0: {   // op, n, out, a, b, c: b for ops 1, 3, 6; c for op 3
+        const int64_t op = a[0];
+        ok = op >= 0 && op <= 6 && a[1] >= 0 && need({2, 3}) && (!(op == 1 || op == 3 || op == 6) || a[4]) && (op != 3 || a[5]);
+        break;
+    }
+    case 1: ok = need({0, 2}) && a[4] >= 0 && a[5] >= a[4] && a[5] >= TILE && a[5] % TILE == 0 && a[1] >= a[5] && a[3] >= a[4]; break;   // dst, ldd, src, lds, n, npad
+    case 2: ok = need({0, 2}) && a[3] >= 0 && a[4] >= 0 && a[1] >= a[4]; break;                  // A, ld, v, nrows, ncols
+    case 3: ok = need({0, 1, 3}) && a[4] >= 0 && a[2] >= 0; break;                               // out, src, ld, idx, nv
+    }
+    if (!ok) return fail(h, GPB200_EINVAL, "vec_kernels: a null pointer, a negative size, a bad op, a bad padding or ld below the row width");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = h->st;
+    int64_t* L = &h->launches;
+    cudaError_t e = cudaSuccess;
+    switch (which) {
+    case 0: e = ew_launch((int)a[0], a[1], ptr(2), ptr(3), ptr(4), ptr(5), fargs[0], st, L); break;
+    case 1: e = spd_from_cov_launch(ptr(0), a[1], ptr(2), a[3], a[4], a[5], fargs[0], st, L); break;
+    case 2: e = add_rowvec_launch(ptr(0), a[1], ptr(2), a[3], a[4], st, L); break;
+    case 3: e = gather_block_launch(ptr(0), ptr(1), a[2], reinterpret_cast<const long long*>(a[3]), a[4], st, L); break;
+    }
+    CK(e);
+    CK(cudaStreamSynchronize(st));
     return GPB200_OK;
 }
 

@@ -13,6 +13,8 @@
 #include "vec.cuh"
 #include <math.h>
 
+#include <algorithm>
+
 namespace {
 constexpr int T = 128;
 
@@ -114,10 +116,6 @@ __global__ void __launch_bounds__(256) rowvar_kernel(const double* __restrict__ 
     __syncthreads();
     for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o]; __syncthreads(); }
     if (threadIdx.x == 0) var[blockIdx.x] = kdiag[blockIdx.x] - s[0];
-}
-__global__ void exp2x_kernel(const double* __restrict__ ln, long long n, double* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = exp(2.0 * ln[i]);
 }
 }  // namespace
 
@@ -514,11 +512,6 @@ cudaError_t rowvar_launch(const double* Vt, int64_t ldk, const double* kdiag, in
     if (launches) ++*launches;
     return cudaGetLastError();
 }
-cudaError_t exp2x_launch(const double* ln, int64_t n, double* out, cudaStream_t st, int64_t* launches) {
-    exp2x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ln, n, out);
-    if (launches) ++*launches;
-    return cudaGetLastError();
-}
 
 // ---- posterior sampling helpers (gpb200_rand) -------------------------------------------------------------------
 namespace {
@@ -532,9 +525,12 @@ __global__ void spd_from_cov_kernel(double* __restrict__ dst, long long ldd, con
     else v = (i == j) ? 1.0 : 0.0;
     dst[i * ldd + j] = v;
 }
+// rows blockIdx.y, blockIdx.y + gridDim.y, ...: gridDim.y is at most 65535, the row count (posterior draws) is not bounded
 __global__ void add_rowvec_kernel(double* __restrict__ A, long long ld, const double* __restrict__ v, long long nrows, long long ncols) {
-    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
-    if (j < ncols && i < nrows) A[i * ld + j] += v[j];
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= ncols) return;
+    const double vj = v[j];
+    for (long long i = blockIdx.y; i < nrows; i += gridDim.y) A[i * ld + j] += vj;
 }
 }  // namespace
 cudaError_t spd_from_cov_launch(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t n, int64_t npad, double nugget, cudaStream_t st, int64_t* launches) {
@@ -544,7 +540,8 @@ cudaError_t spd_from_cov_launch(double* dst, int64_t ldd, const double* src, int
     return cudaGetLastError();
 }
 cudaError_t add_rowvec_launch(double* A, int64_t ld, const double* v, int64_t nrows, int64_t ncols, cudaStream_t st, int64_t* launches) {
-    dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)nrows);
+    if (nrows <= 0 || ncols <= 0) return cudaSuccess;
+    dim3 grid((unsigned)((ncols + 255) / 256), (unsigned)std::min<int64_t>(nrows, 65535));
     add_rowvec_kernel<<<grid, 256, 0, st>>>(A, ld, v, nrows, ncols);
     if (launches) ++*launches;
     return cudaGetLastError();

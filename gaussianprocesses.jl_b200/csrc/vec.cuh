@@ -14,11 +14,9 @@ cudaError_t sum_launch(const double* a, int64_t n, double* out, cudaStream_t st,
 cudaError_t rowdot_launch(const double* Kst, int64_t ldk, const double* alpha, int64_t M, int64_t N, double* mu, cudaStream_t st, int64_t* launches);
 // var[m] = kdiag[m] - sum_n Vt[m,n]^2
 cudaError_t rowvar_launch(const double* Vt, int64_t ldk, const double* kdiag, int64_t M, int64_t N, double* var, cudaStream_t st, int64_t* launches);
-// v[i] = exp(2*ln[i])
-cudaError_t exp2x_launch(const double* ln, int64_t n, double* out, cudaStream_t st, int64_t* launches);
 // FP64 issue-rate microbenchmark: tflops[0] = DMMA.16x8x16, tflops[1] = DFMA (register operands)
 cudaError_t fp64_peak_measure(cudaStream_t st, int64_t* launches, double* tflops);
-// elementwise: op 0 out=a+s | 1 out=a/b | 2 out+=a | 3 out=(a-b)/c | 4 out=log(a) | 5 out=1/a
+// elementwise: op 0 out=a+s | 1 out=a/b | 2 out+=a | 3 out=(a-b)/c | 4 out=log(a) | 5 out=1/a | 6 out=a-b
 cudaError_t ew_launch(int op, int64_t n, double* out, const double* a, const double* b, const double* c, double s, cudaStream_t st, int64_t* launches);
 // mode 0: A[:, j] *= 1/sqrt(v[j]) (j < ncols) ; mode 1: A[r, :] *= 1/v[r] (r < nrows)
 cudaError_t scale_launch(int mode, double* A, int64_t ld, int64_t nrows, int64_t ncols, const double* v, cudaStream_t st, int64_t* launches);
@@ -36,7 +34,7 @@ cudaError_t trsv_lower_fwd_fused(const double* F, int64_t ldf, const double* Din
                                  int* flags, cudaStream_t st, int64_t* launches);
 cudaError_t trsv_lower_bwd_fused(const double* F, int64_t ldf, const double* DinvT, const double* z, double* a, int64_t Npad,
                                  int* flags, cudaStream_t st, int64_t* launches);
-// posterior sampling (gpb200_rand): SPD matrix with nugget + identity padding in the lower tiles; A[i, :] += v
+// posterior sampling (gpb200_rand): SPD matrix with nugget + identity padding in the lower tiles; A[i, :] += v (any nrows)
 cudaError_t spd_from_cov_launch(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t n, int64_t npad, double nugget, cudaStream_t st, int64_t* launches);
 cudaError_t add_rowvec_launch(double* A, int64_t ld, const double* v, int64_t nrows, int64_t ncols, cudaStream_t st, int64_t* launches);
 // out[a * nv + b] = src[idx[a] * ld + idx[b]]   (principal sub-matrix on an index set; cross-validation folds)

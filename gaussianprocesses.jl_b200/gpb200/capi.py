@@ -67,6 +67,7 @@ _SIGNATURES = {
     "gpb200_row_reductions": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
     "gpb200_fsa_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_gram_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
+    "gpb200_vec_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_fitc_cv_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "gpb200_ipc_export": (C.c_int, [_H, C.c_void_p]),
@@ -484,7 +485,8 @@ class Engine:
                                                  _as_dp(f), f.size), "fsa_kernels")
 
     GRAM_KERNELS = ("gram_lower", "crossgram", "gram_full", "kdiag", "gram_grad_full", "crossgram_grad", "trace",
-                    "trace_rect", "kdiag_grad", "crossgram_dx", "mirror_lower_tiles")
+                    "trace_rect", "kdiag_grad", "crossgram_dx", "mirror_lower_tiles", "inputs_dx", "gram_seiso_tma",
+                    "trace_seiso_tma")
 
     def gram_kernels(self, name, args, fargs=()):
         """One dense Gram-family kernel (include/gpb200.h) by name, on device buffers: args = the int64 arguments,
@@ -493,6 +495,16 @@ class Engine:
         f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
         self._check(self._lib.gpb200_gram_kernels(self._h, self.GRAM_KERNELS.index(name), a.ctypes.data_as(_lp), a.size,
                                                   _as_dp(f), f.size), "gram_kernels")
+
+    VEC_KERNELS = ("ew", "spd_from_cov", "add_rowvec", "gather_block")
+
+    def vec_kernels(self, name, args, fargs=()):
+        """One elementwise or sampling helper (include/gpb200.h) by name, on device buffers: fargs = s (ew) or the nugget
+        (spd_from_cov)."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
+        self._check(self._lib.gpb200_vec_kernels(self._h, self.VEC_KERNELS.index(name), a.ctypes.data_as(_lp), a.size,
+                                                 _as_dp(f), f.size), "vec_kernels")
 
     def fitc_cv_kernels(self, name, args, fargs=()):
         """One sparse cross-validation row kernel or FITC element kernel (include/gpb200.h) by name, on device buffers."""

@@ -338,14 +338,40 @@ int  gpb200_fsa_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
  *   which 9  crossgram_dx       : xs, ldxs, M, z, ldz, n, d, a, W1 (0 = none), W2 (0 = none), ldw, dmu, dvar
  *                                 fargs = theta, c
  *   which 10 mirror_lower_tiles : F, ld, Npad                                            (no fargs)
+ *   which 11 inputs_dx          : x, ldx, d, N, alpha (0 = none), G, ldg, out, bm_mod, bm_rem, bm_div, fast
+ *                                 out[i, :] = sum_j A_ij dk(x_i, x_j)/dx_i over the lower triangle of A = alpha alpha' - G
+ *                                 mirrored (A = -G without alpha); N x d point-major (inputs_dx_launch, csrc/gram.cuh).
+ *                                 fast = 1: the SEIso specialisation, only for a single SEIso leaf over all d <= 8 dims
+ *   which 12 gram_seiso_tma     : xp, xpt, d, N, Npad, noise_var, n_noise, G, ldg, own_tiles, nranks, rank, own_axis, sf
+ *                                 fargs = theta, nugget
+ *   which 13 trace_seiso_tma    : xp, xpt, d, N, Npad, alpha, Kinv, ldg, part, out, bm_mod, bm_rem, bm_div, sf
+ *                                 (+ reduce; part: 3 per lower tile, out: 3 entries)      fargs = theta
+ *                                 12 and 13 are the TMA-staged kernels of csrc/gram_fast.cuh on the engine's descriptors
+ *                                 (seiso_make_x_maps): xp is [N x dx] with row pitch dx, xpt is [dx x N] with row pitch
+ *                                 Npad, dx = d rounded up to even (a pad column, if any, must be zero in both).  sf, a HOST
+ *                                 pointer or 0, receives the prepared constants c_hi, il2, s2, tab[64] (67 doubles).
  * GPB200_EINVAL, nothing launched: bad which / n / nf, theta not of n_theta entries, d outside 1 .. GPB200_MAX_DIMS, a
  * program dimension >= d, a null pointer (W1, W2 and, without them, dvar may be null), a negative size, a padded size
  * that is not a multiple of 128 or is below its size, a leading dimension below the row width, an odd leading dimension
  * or a pointer not 16-byte aligned for G, Kst, Kss, Kinv and W, j outside [0, n_theta), bad ownership arguments
  * (nranks >= 1, 0 <= rank < nranks, own_axis 0 or 1; bm_mod, bm_div >= 1, 0 <= bm_rem < bm_mod), row0 or rows not a
- * multiple of 128 or past Npad.
+ * multiple of 128 or past Npad, fast = 1 without the single SEIso leaf over d <= 8 dims; for 12 and 13 also a program that
+ * is not that leaf, d > 8, constants seiso_fast_prepare rejects, N < 1, or xp / xpt not 16-byte aligned.
+ * GPB200_ECUDA: the TMA descriptors of 12 and 13 cannot be built.
  * GPB200_ESTATE: a kernel-program call before gpb200_set_kernel.                                                    */
 int  gpb200_gram_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
+/* The elementwise and sampling helpers (csrc/vec.cuh), synchronous, one launch each through its wrapper (sizes <= 0
+ * launch nothing):
+ *   which 0 ew           : op, n, out, a, b, c                  fargs = s
+ *                          op 0 out = a + s, 1 out = a / b, 2 out += a, 3 out = (a - b) / c, 4 out = log(a), 5 out = 1 / a,
+ *                          6 out = a - b
+ *   which 1 spd_from_cov : dst, ldd, src, lds, n, npad          fargs = nugget
+ *                          lower 128-tiles of dst (npad x npad) = src[:n, :n] + nugget I, identity in the padding
+ *   which 2 add_rowvec   : A, ld, v, nrows, ncols               A[i, j] += v[j] for i < nrows, j < ncols
+ *   which 3 gather_block : out, src, ld, idx, nv                out[a nv + b] = src[idx[a] ld + idx[b]] (idx: int64)
+ * GPB200_EINVAL, nothing launched: bad which / n / nf, a bad op, a null pointer the kernel dereferences, a negative size,
+ * npad not a positive multiple of 128 or below n, a leading dimension below the row width.                          */
+int  gpb200_vec_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
 /* The sparse cross-validation row kernels (csrc/fitc_cv.cuh) and the FITC element kernels that run between the same
  * GEMMs (csrc/vec.cuh), synchronous, one launch each through its wrapper (sizes <= 0 launch nothing):
  *   which 0  delta      : kind, x, ldx, d, j, G, C, ld, ncols, nrows, rows_pad, alpha, delta, da   fargs = theta

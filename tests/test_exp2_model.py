@@ -1,8 +1,10 @@
 """CPU (-m "not gpu"): numpy model of the table-based exp2 the TMA-staged SEIso Gram / trace kernels use
 (csrc/gram_fast.cu: exp2_tab + seiso_fast_prepare).  The model re-executes the kernel's steps -- magic-number rounding, 64-entry
 table, degree-5 polynomial whose coefficients are READ FROM THE SOURCE, exponent added in the integer pipe, integer underflow
-guard -- in IEEE double without fma (numpy has none), so it bounds the algorithm's error rather than reproducing the device bits;
-the device result itself is compared with the oracle in tests/test_gpu_parity.py.  What the reference computes here is
+guard -- in IEEE double without fma, so it bounds the algorithm's error rather than reproducing the device bits.  The model
+that does reproduce them, with an exact fma, is tests/seiso_model.py (tested against this one in tests/test_seiso_model.py);
+the device kernels are compared with it bit for bit in tests/test_gpu_seiso_kernel_contracts.py and with the oracle in
+tests/test_gpu_parity.py.  What the reference computes here is
 exp(-r^2 / (2 l^2)) * sigma^2 (src/kernels/se_iso.jl:27, cov(se, r) = σ² exp(-r/(2ℓ²)) over the squared distance)."""
 import os
 import re

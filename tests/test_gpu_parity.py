@@ -331,7 +331,7 @@ def test_seiso_tma_kernels_match_generic_and_oracle(engine, d, N, ll, ls):
         assert abs(res[1][1] - res[0][1]) <= 1e-7 * abs(res[0][1])
 
 
-@pytest.mark.parametrize("M,n", [(37, 5), (300, 130)])
+@pytest.mark.parametrize("M,n", [(37, 5), (300, 130), (8, 70000)])             # n > 65535: more draws than gridDim.y
 def test_rand_on_device_matches_oracle(engine, M, n):
     """rand(gp, X, n) (src/GP.jl:120-146) on the device: with the SAME standard-normal draws the samples equal
     mu* + chol(Sigma* + nugget I) Z of the oracle's predictMVN (full covariance)."""

@@ -585,7 +585,7 @@ def test_misuse_returns_einval_or_estate_and_launches_nothing(eng):
     for name, args, fa in bad:
         with pytest.raises(ValueError):
             eng.gram_kernels(name, [int(a) for a in args], fa)
-    for which in (-1, 11):
+    for which in (-1, 14):
         a = np.zeros(3, dtype=np.int64)
         rc = eng._lib.gpb200_gram_kernels(eng._h, which, a.ctypes.data_as(gpb200.capi._lp), 3, None, 0)
         assert rc == gpb200.capi.EINVAL
