@@ -59,7 +59,6 @@ struct gpb200_handle {
     DevBuf<double> cvblk; DevBuf<long long> cvidx;   // principal sub-blocks of gpb200_cv_block (grown on demand)
     // posterior sampling (gpb200_rand): M x M sub-engine for chol(Sigma* + nugget I), normal draws / samples staging
     gpb200_handle* sub = nullptr;
-    bool cov_keep_device = false;              // predict: leave the full covariance in Kss (no D2H)
     DevBuf<double> rz, rout;                   // rz_rows x rz_cols each
     int64_t rz_rows = 0, rz_cols = 0;
     CUtensorMap mapRz{};
@@ -199,7 +198,6 @@ struct gpb200_fitc {
     DevBuf<double> Kss;                               // full predictive covariance (gpb200_fitc_predict_cov)
     DevBuf<double> pdx;                               // gpb200_fitc_predict_grad: dmu, dvar of a chunk (2 x Nc x d; first use)
     // posterior sampling (gpb200_fitc_rand): the Ms x Ms sub-engine and the staging of the draws are eu's (rand_from_cov)
-    bool cov_keep_device = false;                     // predict_fsa: leave Sigma* in caller order on the device (fsa->Sc)
     double rand_ms[3] = {0, 0, 0};                    // device times of the last rand: Sigma* build, Cholesky, unwhiten!
     double fsag_ms[4] = {0, 0, 0, 0};                 // last predict_fsa_grad, summed over test chunks: predict_fsa's
                                                       // launches, s + second sweep, K_uu^-1 TRSMs, contraction
@@ -326,6 +324,11 @@ inline GemmBuf bufDinv(gpb200_handle* h) { return gbuf(h, h->Dinv, h->mapDinv, T
 inline GemmBuf bufDinvT(gpb200_handle* h) { return gbuf(h, h->DinvT, h->mapDinvT, TILE); }
 inline GemmBuf bufNone() { return GemmBuf{nullptr, nullptr, 0}; }
 
+// where a prediction puts the full covariance Sigma*: nowhere, the caller's host array, or the device (for rand_from_cov)
+enum class CovDest { none, host, device };
+// mu* (M) and Sigma* (M x M, leading dimension ldc) where a prediction left them on the device
+struct DevPrediction { const double *mu, *cov; int64_t ldc; };
+
 // ---- dense engine (gpb200.cu) -------------------------------------------------------------------------------------
 cudaError_t launch_gemm(gpb200_handle* h, const GemmDesc& d);
 // C[M x N] (+)= alpha A B' on h's DMMA GEMM, A and B whole buffers from (0, 0), C (and the optional transposed copy Ct)
@@ -350,7 +353,8 @@ int fsa_grad_noise(gpb200_fitc* f, double* dmll_noise);
 int fsa_grad_kernel(gpb200_fitc* f, double* dmll_kernel, double* dmll_xu, double* dmll_x);
 int fsa_set_inputs(gpb200_fitc* f, const double* x, int64_t ldx);
 size_t fsa_num_chunks(const gpb200_fitc* f);
-const double* fsa_cov(const gpb200_fitc* f);
+int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of, double* mu, double* var,
+                CovDest cov_to, double* cov, double* dmu, double* dvar, DevPrediction* out);
 
 // ---- FITC (fitc_engine.cu), shared with the FSA schedule --------------------------------------------------------------
 int fitc_stage_alloc(gpb200_fitc* f, int64_t nc, const char* who);

@@ -150,6 +150,46 @@ cudaError_t fitc_kuf(gpb200_fitc* f, const double* xrows, int64_t nc) {
     return crossgram_launch(f->eu->prog, f->eu->x, f->d, f->M, f->Mpad, xrows, f->d, nc, f->Nc, f->d, f->stage.bufB, f->Nc, f->eu->st, &f->eu->launches);
 }
 
+// Lambda of data rows r0 .. r0+nc into data.lam.  FITC: Lambda_i = sigma^2 + K_ii - |L_uu^-1 K_ui|^2 (fitc.jl:146-148), the
+// whitening TRSM over trsm_rows rows of bufA; SoR / DTC: Lambda = sigma^2 I (subsetofregressors.jl:100: exp(-2 logNoise) *
+// Kuf * Kfu + Kuu)
+static int fitc_lambda(gpb200_fitc* f, int64_t r0, int64_t nc, int64_t trsm_rows) {
+    gpb200_handle* eu = f->eu;
+    cudaStream_t st = eu->st;
+    const double* xr = f->data.x + r0 * f->d;
+    if (f->mode == 0) {
+        FCK(fitc_kfu(f, xr, nc));
+        FCK(trsm_rec_buf(eu, gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad), (int)trsm_rows, 0, (int)f->Mpad));
+        FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->stage.tmpc, st, &eu->launches));
+        FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, nc, f->Mpad, f->stage.tmpc2, st, &eu->launches));
+        FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
+    } else {
+        FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
+    }
+    return GPB200_OK;
+}
+
+// b += K_uf Lambda^-1 r over data rows r0 .. r0+nc (r in data.y), with their K_uf in bufB (fitc_kuf)
+static int fitc_b_add(gpb200_fitc* f, int64_t r0, int64_t nc, double* b) {
+    gpb200_handle* eu = f->eu;
+    cudaStream_t st = eu->st;
+    FCK(cudaMemsetAsync(f->stage.w, 0, sizeof(double) * f->Nc, st));
+    FCK(ew_launch(1, nc, f->stage.w, f->data.y + r0, f->data.lam + r0, nullptr, 0.0, st, &eu->launches));
+    FCK(rowdot_launch(f->stage.bufB, f->Nc, f->stage.w, f->M, f->Nc, f->data.tmpm, st, &eu->launches));
+    FCK(ew_launch(2, f->M, b, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+    return GPB200_OK;
+}
+
+// S += K_uf Lambda^-1 K_fu (fitc.jl:150) over data rows r0 .. r0+nc, as (K_uf Lambda^-1/2)(K_uf Lambda^-1/2)': bufB (their
+// K_uf) is scaled in place, then a lower-only SYRK over its first k columns into S (Mpad x Mpad, leading dimension lds)
+static int fitc_syrk_add(gpb200_fitc* f, int64_t r0, int64_t nc, double* S, int64_t lds, int64_t k) {
+    gpb200_handle *eu = f->eu, *es = f->es;
+    const GemmBuf bB = gbuf(eu, f->stage.bufB, f->stage.mapB, f->Nc);
+    FCK(scale_launch(0, f->stage.bufB, f->Nc, f->Mpad, nc, f->data.lam + r0, eu->st, &eu->launches));
+    FCK(gemm_whole(es, bB, bB, S, lds, f->Mpad, f->Mpad, k, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
+    return GPB200_OK;
+}
+
 // one contraction launch (slot k >= 1 of f->xu_ev) over n rows z against W (ld Mpad) into f->dxu
 int xu_contract(gpb200_fitc* f, size_t k, const double* z, int64_t n, const double* W, int sym, const double* mask,
                 int accumulate) {
@@ -220,26 +260,11 @@ int gpb200_fitc_factorize(gpb200_fitc* f, const double* theta, double log_noise)
     else FCK(cudaMemsetAsync(es->G, 0, sizeof(double) * (size_t)f->Mpad * (size_t)f->Mpad, st));     // K_uu (+ nuggets, identity padding) enters the sum once
     f->noise_var = exp(2.0 * log_noise);
     if (f->mode == 3) return fsa_factorize(f);
-    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
-    const GemmBuf bB = gbuf(eu, f->stage.bufB, f->stage.mapB, f->Nc);
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
-        const double* xr = f->data.x + r0 * f->d;
-        if (f->mode == 0) {
-            // Lambda_i = sigma^2 + K_ii - |L_uu^-1 K_ui|^2   (fitc.jl:146-148)
-            FCK(fitc_kfu(f, xr, nc));
-            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(kdiag_launch(eu->prog, xr, f->d, nc, f->stage.tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, nc, f->Mpad, f->stage.tmpc2, st, &eu->launches));
-            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
-        } else {
-            // SoR / DTC: Lambda = sigma^2 I   (subsetofregressors.jl:100: exp(-2 logNoise) * Kuf * Kfu + Kuu)
-            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
-        }
-        // Sigma_QR += K_uf Lambda^-1 K_fu   (fitc.jl:150), as (K_uf Lambda^-1/2)(K_uf Lambda^-1/2)'
-        FCK(fitc_kuf(f, xr, nc));
-        FCK(scale_launch(0, f->stage.bufB, f->Nc, f->Mpad, nc, f->data.lam + r0, st, &eu->launches));
-        FCK(gemm_whole(es, bB, bB, es->G, es->ld, f->Mpad, f->Mpad, f->Nc, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
+        TRY(fitc_lambda(f, r0, nc, f->Nc));
+        FCK(fitc_kuf(f, f->data.x + r0 * f->d, nc));
+        TRY(fitc_syrk_add(f, r0, nc, es->G, es->ld, f->Nc));                 // Sigma_QR += K_uf Lambda^-1 K_fu
     }
     // multi-GPU: Sigma_QR = K_uu + sum over ranks of K_uf L^-1 K_fu  -- the one M x M exchange of the FITC likelihood
     TRY(fitc_allreduce(f, es->G, (size_t)f->Mpad * (size_t)f->Mpad));
@@ -263,10 +288,7 @@ int gpb200_fitc_mll(gpb200_fitc* f, const double* y_minus_mean, double* alpha, d
     for (int64_t r0 = 0; r0 < f->N; r0 += f->Nc) {
         const int64_t nc = std::min(f->Nc, f->N - r0);
         FCK(fitc_kuf(f, f->data.x + r0 * f->d, nc));
-        FCK(cudaMemsetAsync(f->stage.w, 0, sizeof(double) * f->Nc, st));
-        FCK(ew_launch(1, nc, f->stage.w, f->data.y + r0, f->data.lam + r0, nullptr, 0.0, st, &eu->launches));
-        FCK(rowdot_launch(f->stage.bufB, f->Nc, f->stage.w, f->M, f->Nc, f->data.tmpm, st, &eu->launches));
-        FCK(ew_launch(2, f->M, f->data.bvec, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
+        TRY(fitc_b_add(f, r0, nc, f->data.bvec));
     }
     TRY(fitc_allreduce(f, f->data.bvec, (size_t)f->Mpad));              // b summed over the ranks' rows
     // u = Sigma_QR^-1 b   (== get_alpha_u, fitc.jl:279-286)
@@ -337,44 +359,45 @@ int gpb200_fitc_grad_noise(gpb200_fitc* f, double* dmll_noise) {
     return GPB200_OK;
 }
 
-// predictive mean / variance (fitc.jl:324-332 -> dtc.jl:41-59 -> sor.jl:302-321):
-//   mu = K_xu u ;  var = k_xx - |L_uu^-1 k_ux|^2 + |L_s^-1 k_ux|^2
+// predictive mean / variance of mc <= Nc test rows (xs, row stride ldxs; fitc.jl:324-332 -> dtc.jl:41-59 -> sor.jl:302-321):
+//   mu = K_xu u ;  var = k_xx - |L_uu^-1 k_ux|^2 + |L_s^-1 k_ux|^2   (SoR: |L_s^-1 k_ux|^2 only)
+// The rows are left in stage.xs and mu in stage.tmpc; without var, K*u in bufA; with var, A = K*u L_uu^-T in bufA and
+// B = K*u L_s^-T in bufB
+static int fitc_predict_chunk(gpb200_fitc* f, const double* xs, int64_t ldxs, int64_t mc, double* mu, double* var) {
+    gpb200_handle *eu = f->eu, *es = f->es;
+    cudaStream_t st = eu->st;
+    FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * f->d, xs, sizeof(double) * ldxs, sizeof(double) * f->d, mc,
+                          cudaMemcpyHostToDevice, st));
+    FCK(fitc_kfu(f, f->stage.xs, mc));
+    FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, mc, f->Mpad, f->stage.tmpc, st, &eu->launches));
+    FCK(cudaMemcpyAsync(mu, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+    if (!var) return GPB200_OK;
+    FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
+    FCK(trsm_rec_buf(eu, gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad), (int)f->Nc, 0, (int)f->Mpad));
+    FCK(trsm_rec_buf(es, gbuf(eu, f->stage.bufB, f->stage.mapB2, f->Mpad), (int)f->Nc, 0, (int)f->Mpad));
+    FCK(kdiag_launch(eu->prog, f->stage.xs, f->d, mc, f->stage.tmpc, st, &eu->launches));
+    FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, mc, f->Mpad, f->stage.tmpc2, st, &eu->launches));       // k_xx - q
+    FCK(rowvar_launch(f->stage.bufB, f->Mpad, f->stage.zeroc, mc, f->Mpad, f->stage.w, st, &eu->launches));          // -s
+    if (f->mode == 2) FCK(cudaMemsetAsync(f->stage.tmpc2, 0, sizeof(double) * mc, st));
+    FCK(ew_launch(6, mc, f->stage.tmpc, f->stage.tmpc2, f->stage.w, nullptr, 0.0, st, &eu->launches));               // [k_xx - q] + s
+    FCK(cudaMemcpyAsync(var, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+    return GPB200_OK;
+}
+
 int gpb200_fitc_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, double* var) {
     if (!f || Ms <= 0 || !xs || ldxs < f->d || !mu) return GPB200_EINVAL;
     if (!f->factored || !(f->alpha_ready || f->u_ready)) return fail(f, GPB200_ESTATE, "fitc_predict: factorize and mll first");
     if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict: FSA predictions need test blocks");
     FCK(cudaSetDevice(f->device));
-    gpb200_handle *eu = f->eu, *es = f->es;
-    cudaStream_t st = eu->st;
-    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
-    const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, f->Mpad);
     for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
-        const int64_t mc = std::min(f->Nc, Ms - m0);
-        FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * f->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * f->d,
-                              mc, cudaMemcpyHostToDevice, st));
-        FCK(fitc_kfu(f, f->stage.xs, mc));
-        FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, mc, f->Mpad, f->stage.tmpc, st, &eu->launches));
-        FCK(cudaMemcpyAsync(mu + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-        if (var) {
-            FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
-            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(kdiag_launch(eu->prog, f->stage.xs, f->d, mc, f->stage.tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, mc, f->Mpad, f->stage.tmpc2, st, &eu->launches));       // k_xx - q
-            FCK(rowvar_launch(f->stage.bufB, f->Mpad, f->stage.zeroc, mc, f->Mpad, f->stage.w, st, &eu->launches));          // -s
-            if (f->mode == 2) {                                                             // SoR: K_xu S^-1 K_ux only (sor.jl:302-321)
-                FCK(cudaMemsetAsync(f->stage.tmpc2, 0, sizeof(double) * mc, st));
-            }
-            FCK(ew_launch(6, mc, f->stage.tmpc, f->stage.tmpc2, f->stage.w, nullptr, 0.0, st, &eu->launches));               // [k_xx - q] + s
-            FCK(cudaMemcpyAsync(var + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-        }
-        FCK(cudaStreamSynchronize(st));
+        TRY(fitc_predict_chunk(f, xs + m0 * ldxs, ldxs, std::min(f->Nc, Ms - m0), mu + m0, var ? var + m0 : nullptr));
+        FCK(cudaStreamSynchronize(f->eu->st));
     }
     return GPB200_OK;
 }
 
 // Predictive gradients of the sparse models (predict_f with ForwardDiff.Dual inputs): mu and var through
-// gpb200_fitc_predict's launches (A = K*u L_uu^-T in bufA, B = K*u L_s^-T in bufB), then W' = A L_uu^-1 - B L_s^-1
+// gpb200_fitc_predict's chunk step (A = K*u L_uu^-T in bufA, B = K*u L_s^-T in bufB), then W' = A L_uu^-1 - B L_s^-1
 // (= K*u K_uu^-1 - K*u Sigma_QR^-1; SoR: - B L_s^-1) by the right-side TRSM on the two M x M sub-engines, whose F holds L'
 // in its strict-upper tiles for the call, and the contraction over the inducing points with alpha = u:
 //   dmu[m, :] = sum_j dk(x*_m, u_j)/dx*_m u_j,   dvar[m, :] = 2c dk(x*_m, x*_m)/dx*_m - 2 sum_j dk(x*_m, u_j)/dx*_m W'[m, j]
@@ -402,21 +425,8 @@ int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64
     }
     for (int64_t m0 = 0; m0 < Ms; m0 += f->Nc) {
         const int64_t mc = std::min(f->Nc, Ms - m0);
-        FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d,
-                              mc, cudaMemcpyHostToDevice, st));
-        FCK(fitc_kfu(f, f->stage.xs, mc));
-        FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, mc, f->Mpad, f->stage.tmpc, st, &eu->launches));
-        FCK(cudaMemcpyAsync(mu + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
-        if (var) {                                                          // as gpb200_fitc_predict
-            FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
-            FCK(trsm_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(trsm_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));
-            FCK(kdiag_launch(eu->prog, f->stage.xs, d, mc, f->stage.tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->stage.bufA, f->Mpad, f->stage.tmpc, mc, f->Mpad, f->stage.tmpc2, st, &eu->launches));
-            FCK(rowvar_launch(f->stage.bufB, f->Mpad, f->stage.zeroc, mc, f->Mpad, f->stage.w, st, &eu->launches));
-            if (f->mode == 2) FCK(cudaMemsetAsync(f->stage.tmpc2, 0, sizeof(double) * mc, st));
-            FCK(ew_launch(6, mc, f->stage.tmpc, f->stage.tmpc2, f->stage.w, nullptr, 0.0, st, &eu->launches));
-            FCK(cudaMemcpyAsync(var + m0, f->stage.tmpc, sizeof(double) * mc, cudaMemcpyDeviceToHost, st));
+        TRY(fitc_predict_chunk(f, xs + m0 * ldxs, ldxs, mc, mu + m0, var ? var + m0 : nullptr));
+        if (var) {
             if (f->mode != 2) FCK(trsm_right_rec_buf(eu, bA, (int)f->Nc, 0, (int)f->Mpad));      // A L_uu^-1
             FCK(trsm_right_rec_buf(es, bB2, (int)f->Nc, 0, (int)f->Mpad));                        // B L_s^-1
         }
@@ -432,18 +442,15 @@ int gpb200_fitc_predict_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64
 // predictMVN with the FULL predictive covariance (fitc.jl:324-332 -> determ_train_conditional.jl:41-59 ->
 // subsetofregressors.jl:302-321):  Sigma* = K** - K*u K_uu^-1 Ku* + K*u S^-1 Ku*   (FITC, DTC);   K*u S^-1 Ku*   (SoR)
 // = K** - A A' + B B' with A = K*u L_uu^-T, B = K*u L_s^-T: two whitening TRSMs and two NT GEMMs.  Ms <= one staging chunk.
-// Sigma* into f->Kss (leading dimension Ms rounded up to 128) and mu into f->stage.tmpc and mu[Ms], on eu's stream; Ms <= Nc
-static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu) {
+// mu into mu[Ms]; mu* and Sigma* left on the device (stage.tmpc, Kss) as *out says, on eu's stream; Ms <= Nc
+static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, double* mu, DevPrediction* out) {
     gpb200_handle *eu = f->eu, *es = f->es;
     cudaStream_t st = eu->st;
     const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
     FCK(f->Kss.ensure((size_t)Mspad * Mspad));
     const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, f->Mpad);
     const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, f->Mpad);
-    FCK(cudaMemcpy2DAsync(f->stage.xs, sizeof(double) * f->d, xs, sizeof(double) * ldxs, sizeof(double) * f->d, Ms, cudaMemcpyHostToDevice, st));
-    FCK(fitc_kfu(f, f->stage.xs, Ms));                                         // bufA = K*u  (Ms x Mpad, zero padded rows)
-    FCK(rowdot_launch(f->stage.bufA, f->Mpad, f->data.uvec, Ms, f->Mpad, f->stage.tmpc, st, &eu->launches));
-    FCK(cudaMemcpyAsync(mu, f->stage.tmpc, sizeof(double) * Ms, cudaMemcpyDeviceToHost, st));
+    TRY(fitc_predict_chunk(f, xs, ldxs, Ms, mu, nullptr));                    // bufA = K*u  (Ms x Mpad, zero padded rows)
     FCK(cudaMemcpyAsync(f->stage.bufB, f->stage.bufA, sizeof(double) * f->Nc * f->Mpad, cudaMemcpyDeviceToDevice, st));
     FCK(trsm_rec_buf(es, bB2, (int)Mspad, 0, (int)f->Mpad));             // B = K*u L_s^-T
     if (f->mode != 2) {
@@ -454,6 +461,7 @@ static int fitc_cov_build(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t 
         FCK(cudaMemsetAsync(f->Kss, 0, sizeof(double) * Mspad * Mspad, st));
     }
     FCK(gemm_whole(es, bB2, bB2, f->Kss, Mspad, Mspad, Mspad, f->Mpad, 1.0, 1.0));
+    *out = DevPrediction{f->stage.tmpc, f->Kss, Mspad};
     return GPB200_OK;
 }
 
@@ -463,9 +471,9 @@ int gpb200_fitc_predict_cov(gpb200_fitc* f, int64_t Ms, const double* xs, int64_
     if (f->mode == 3) return fail(f, GPB200_EINVAL, "fitc_predict_cov: FSA predictions need test blocks");
     if (Ms > f->Nc) return fail(f, GPB200_EINVAL, "fitc_predict_cov: too many test points for one staging chunk");
     FCK(cudaSetDevice(f->device));
-    TRY(fitc_cov_build(f, Ms, xs, ldxs, mu));
-    const int64_t Mspad = (Ms + TILE - 1) / TILE * TILE;
-    FCK(cudaMemcpy2DAsync(cov, sizeof(double) * Ms, f->Kss, sizeof(double) * Mspad, sizeof(double) * Ms, Ms, cudaMemcpyDeviceToHost, f->eu->st));
+    DevPrediction p;
+    TRY(fitc_cov_build(f, Ms, xs, ldxs, mu, &p));
+    FCK(cudaMemcpy2DAsync(cov, sizeof(double) * Ms, p.cov, sizeof(double) * p.ldc, sizeof(double) * Ms, Ms, cudaMemcpyDeviceToHost, f->eu->st));
     FCK(cudaStreamSynchronize(f->eu->st));
     return GPB200_OK;
 }
@@ -701,8 +709,9 @@ extern "C" {
 // append! for FITC, DTC and SoR: k new observations with the hyper-parameters and Xu fixed.  K_uu, L_uu and the old rows'
 // Lambda_i do not change; Sigma_QR and b change by one rank-k term and one M-vector, so the cost is O(k M^2 + M^3) whatever
 // N is.  With K_nu (k x M) the cross-Gram of the new rows, Lambda_n their diagonal terms (FITC: sigma^2 + k_ii -
-// |L_uu^-1 k_ui|^2, by the launches gpb200_fitc_factorize runs on a chunk; DTC / SoR: sigma^2) and r_n their residuals:
-//   Sigma_QR <- Sigma_QR + K_un Lambda_n^-1 K_nu       (lower-only SYRK on the DMMA GEMM, as in factorize)
+// |L_uu^-1 k_ui|^2; DTC / SoR: sigma^2) and r_n their residuals, with the chunk steps factorize and mll run (fitc_lambda,
+// fitc_syrk_add, fitc_b_add):
+//   Sigma_QR <- Sigma_QR + K_un Lambda_n^-1 K_nu       (lower-only SYRK on the DMMA GEMM)
 //   b        <- b + K_un Lambda_n^-1 r_n
 //   s        <- s + sum r_n^2 / Lambda_n               (s = r'Lambda^-1 r)
 //   l        <- l + sum log Lambda_n                   (l = sum log Lambda_i)
@@ -733,8 +742,6 @@ int gpb200_fitc_append(gpb200_fitc* f, int64_t k, const double* xnew, int64_t ld
     cudaStream_t st = eu->st;
     const int64_t Mp = f->Mpad, Nc = f->Nc, N0 = f->N, N1 = N0 + k;
     const int d = f->d;
-    const GemmBuf bA = gbuf(eu, f->stage.bufA, f->stage.mapA, Mp);
-    const GemmBuf bB = gbuf(eu, f->stage.bufB, f->stage.mapB, Nc);
     if (!f->app.sqr_ok) {                                                // Sigma_QR = L_s L_s', once per factorize
         FCK(f->app.sqr.ensure((size_t)Mp * Mp));
         FCK(cudaMemsetAsync(f->app.sqr, 0, sizeof(double) * Mp * Mp, st));           // clean above the diagonal
@@ -760,25 +767,10 @@ int gpb200_fitc_append(gpb200_fitc* f, int64_t k, const double* xnew, int64_t ld
     for (int64_t r0 = N0; r0 < N1; r0 += Nc) {
         const int64_t nc = std::min(Nc, N1 - r0);
         const int64_t ncp = (nc + TILE - 1) / TILE * TILE;              // the TRSM and the SYRK stop at the chunk's padded rows
-        const double* xr = f->data.x + r0 * d;
-        if (f->mode == 0) {                                              // as gpb200_fitc_factorize
-            FCK(fitc_kfu(f, xr, nc));
-            FCK(trsm_rec_buf(eu, bA, (int)ncp, 0, (int)Mp));
-            FCK(kdiag_launch(eu->prog, xr, d, nc, f->stage.tmpc, st, &eu->launches));
-            FCK(rowvar_launch(f->stage.bufA, Mp, f->stage.tmpc, nc, Mp, f->stage.tmpc2, st, &eu->launches));
-            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.tmpc2, nullptr, nullptr, f->noise_var, st, &eu->launches));
-        } else {
-            FCK(ew_launch(0, nc, f->data.lam + r0, f->stage.zeroc, nullptr, nullptr, f->noise_var, st, &eu->launches));
-        }
-        FCK(fitc_kuf(f, xr, nc));
-        // b += K_un Lambda_n^-1 r_n   (as gpb200_fitc_mll)
-        FCK(cudaMemsetAsync(f->stage.w, 0, sizeof(double) * Nc, st));
-        FCK(ew_launch(1, nc, f->stage.w, f->data.y + r0, f->data.lam + r0, nullptr, 0.0, st, &eu->launches));
-        FCK(rowdot_launch(f->stage.bufB, Nc, f->stage.w, f->M, Nc, f->data.tmpm, st, &eu->launches));
-        FCK(ew_launch(2, f->M, f->data.rhsm, f->data.tmpm, nullptr, nullptr, 0.0, st, &eu->launches));
-        // Sigma_QR += K_un Lambda_n^-1 K_nu
-        FCK(scale_launch(0, f->stage.bufB, Nc, Mp, nc, f->data.lam + r0, st, &eu->launches));
-        FCK(gemm_whole(es, bB, bB, dS, Mp, Mp, Mp, ncp, 1.0, 1.0, nullptr, 0, GEMM_LOWER_ONLY));
+        TRY(fitc_lambda(f, r0, nc, ncp));
+        FCK(fitc_kuf(f, f->data.x + r0 * d, nc));
+        TRY(fitc_b_add(f, r0, nc, f->data.rhsm));                        // b += K_un Lambda_n^-1 r_n
+        TRY(fitc_syrk_add(f, r0, nc, dS, Mp, ncp));                      // Sigma_QR += K_un Lambda_n^-1 K_nu
     }
     // s and l over the new rows, or over every row on the first append after a mll; and the row count
     const int64_t s0 = f->app.sums_ok ? N0 : 0;
@@ -1055,20 +1047,10 @@ int gpb200_fitc_rand(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs,
     gpb200_handle* eu = f->eu;
     cudaEvent_t ev_start = eu->ev4;                      // rand_from_cov records ev0 .. ev3
     FCK(cudaEventRecord(ev_start, eu->st));
-    const double* cov;
-    int64_t ldc;
-    if (f->mode == 3) {
-        static double cov_flag;                          // non-null marker: Sigma* stays on the device
-        f->cov_keep_device = true;
-        const int rc = gpb200_fitc_predict_fsa(f, Ms, xs, ldxs, block_of, mu_minus_mean, nullptr, &cov_flag);
-        f->cov_keep_device = false;
-        if (rc) return rc;
-        cov = fsa_cov(f); ldc = Ms;
-    } else {
-        TRY(fitc_cov_build(f, Ms, xs, ldxs, mu_minus_mean));
-        cov = f->Kss; ldc = (Ms + TILE - 1) / TILE * TILE;
-    }
-    FSUB(rand_from_cov(eu, Ms, cov, ldc, f->stage.tmpc, nsamp, z, nugget, samples), eu);
+    DevPrediction p;
+    if (f->mode == 3) TRY(fsa_predict(f, Ms, xs, ldxs, block_of, mu_minus_mean, nullptr, CovDest::device, nullptr, nullptr, nullptr, &p));
+    else TRY(fitc_cov_build(f, Ms, xs, ldxs, mu_minus_mean, &p));
+    FSUB(rand_from_cov(eu, Ms, p.cov, p.ldc, p.mu, nsamp, z, nugget, samples), eu);
     f->rand_ms[0] = ev_ms(ev_start, eu->ev0);
     f->rand_ms[1] = ev_ms(eu->ev0, eu->ev1);
     f->rand_ms[2] = ev_ms(eu->ev3, eu->ev2);

@@ -80,7 +80,7 @@ struct Fsa {
     FsaGradWs pgrad;
     // per-call work lists of the predictions, grown on demand
     DevBuf<FsaGemmItem> pg; DevBuf<FsaGramItem> px; DevBuf<FsaRowItem> pr;
-    // gpb200_fitc_rand: Sigma* gathered into the caller's order (Ms x Ms, dense) through the test-point permutation pp
+    // CovDest::device: Sigma* gathered into the caller's order (Ms x Ms, dense) through the test-point permutation pp
     DevBuf<double> Sc; DevBuf<long long> pp;
     // gpb200_fitc_predict_fsa_grad: dmu / dvar in the caller's order (2 x Ms x d) and the contraction's items
     DevBuf<double> pdx;
@@ -331,8 +331,6 @@ int gpb200_fitc_set_blocks(gpb200_fitc* f, int64_t nblocks, const int64_t* block
 
 namespace engine __attribute__((visibility("hidden"))) {
 size_t fsa_num_chunks(const gpb200_fitc* f) { return f->fsa ? f->fsa->chunks.size() : 0; }
-// Sigma* of the last gpb200_fitc_predict_fsa run with cov_keep_device
-const double* fsa_cov(const gpb200_fitc* f) { return f->fsa->Sc; }
 
 void fsa_free(gpb200_fitc* f) {
     delete f->fsa;
@@ -550,7 +548,7 @@ int fsa_set_inputs(gpb200_fitc* f, const double* x, int64_t ldx) {
 // G G' is block-diagonal in the test blocks.  Test points are grouped by paired block, each group padded to 128 rows, and
 // streamed in chunks of at most Nc padded rows; per chunk, the training chunks of the paired blocks are revisited (V, K_uf).
 //
-// dmu != null (gpb200_fitc_predict_fsa_grad; cov null): the same launches give mu and var, then per test chunk the
+// dmu != null (gpb200_fitc_predict_fsa_grad; no Sigma*): the same launches give mu and var, then per test chunk the
 // gradients with respect to the test inputs.  With c = C row m, h = H row m, D_u / D_b / D_** the input derivatives of
 // k(x*, u_j), k(x*, x_i) (i in the paired block b) and k(x*, x*), and s = S^-1 r~' (= R L_s^-1, r~ = K_*u - C Lambda_b^-1 K_bu):
 //   dmu  = D_u (u - beta) + D_b alpha_b ,               beta = K_uu^-1 K_ub alpha_b
@@ -561,8 +559,10 @@ int fsa_set_inputs(gpb200_fitc* f, const double* x, int64_t ldx) {
 // with lda = 0, every row of a test tile the same alpha_b) into the Mpad-wide test rows of Zb and Vs; beta is formed per
 // test row rather than once per block, so that it shares the row layout, the GEMM shape and the two K_uu^-1 TRSMs of Z.
 // One fsa_crossgram_dx launch per chunk writes dmu / dvar into the caller's order.
-static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of, double* mu,
-                       double* var, double* cov, double* dmu, double* dvar) {
+// Sigma* (cov_to, into cov with CovDest::host) needs the padded test blocks in one staging chunk; CovDest::device leaves it
+// in Sc and mu* in stage.tmpc, in the caller's order, as *out says.
+int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of, double* mu, double* var,
+                CovDest cov_to, double* cov, double* dmu, double* dvar, DevPrediction* out) {
     if (!f || Ms <= 0 || !xs || !block_of || !mu) return GPB200_EINVAL;
     if (f->mode != 3) return fail(f, GPB200_EINVAL, "fitc_predict_fsa: the handle is not in FSA mode (3)");
     if (!f->fsa || !f->factored || !f->alpha_ready) return fail(f, GPB200_ESTATE, "fitc_predict_fsa: set_blocks, factorize and mll first");
@@ -589,8 +589,9 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
         for (int64_t t = 0; t < tiles; ++t) tile_blk.push_back(b < nb ? b : -1);
         Msp += tiles * TILE;
     }
-    if (cov && Msp > Nc) return fail(f, GPB200_EINVAL, "fitc_predict_fsa: cov needs the padded test blocks in one staging chunk");
-    if (cov) FCK(f->Kss.ensure((size_t)Msp * Msp));
+    const bool want_cov = cov_to != CovDest::none, cov_host = cov_to == CovDest::host;
+    if (want_cov && Msp > Nc) return fail(f, GPB200_EINVAL, "fitc_predict_fsa: cov needs the padded test blocks in one staging chunk");
+    if (want_cov) FCK(f->Kss.ensure((size_t)Msp * Msp));
     std::vector<int64_t> ppos((size_t)Ms);
     std::vector<double> xsp((size_t)Msp * d, 0.0);
     for (int64_t i = 0; i < Ms; ++i) {
@@ -751,7 +752,7 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
             t = te;
         }
         sb.ggt.off = (int64_t)gi.size();                        // cov: -G G' on the tile pairs of the same block
-        if (cov) {
+        if (want_cov) {
             const int64_t mq = (sb.t1 - sb.t0) * TILE;
             for (int64_t t = sb.t0; t < sb.t1; ++t)
                 for (int64_t u = sb.t0; u < sb.t1; ++u) {
@@ -792,7 +793,6 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
     const GemmBuf bB2 = gbuf(eu, f->stage.bufB, f->stage.mapB2, Mp);
     const GemmBuf bVs = gbuf(eu, s->pred.Vs, s->pred.mapVs, Mp);
     const GemmBuf bZb = gbuf(eu, s->pgrad.Zb, s->pgrad.mapZb, Mp);
-    const bool cov_host = cov && !f->cov_keep_device;
     std::vector<double> mu_p((size_t)Msp), var_p(var ? (size_t)Msp : 0), cov_p(cov_host ? (size_t)Msp * Msp : 0);
     double* ddmu = grad ? s->pdx.data() : nullptr;
     double* ddvar = grad ? s->pdx + Ms * d : nullptr;
@@ -868,7 +868,7 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
                                         &eu->launches));
             FCK(cudaEventRecord(eu->ev4, st));
         }
-        if (cov) {
+        if (want_cov) {
             FCK(gram_full_launch(eu->prog, f->stage.xs, d, mq, mq, d, f->Kss, mq, st, &eu->launches));
             FCK(gemm_whole(eu, bVs, bVs, f->Kss, mq, mq, mq, Mp, -1.0, 1.0));                              // - V_*' V_*
             FCK(gemm_whole(es, bB2, bB2, f->Kss, mq, mq, mq, Mp, 1.0, 1.0));                               // + R R'
@@ -888,13 +888,14 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
         if (var) FCK(cudaMemcpyAsync(dvar, ddvar, sizeof(double) * Ms * d, cudaMemcpyDeviceToHost, st));
         FCK(cudaStreamSynchronize(st));
     }
-    if (cov && !cov_host) {
+    if (cov_to == CovDest::device) {
         // Sigma* (one sub-chunk: leading dimension Msp) and mu in the caller's order on the device, as the host loop below
         // reorders them
         FCK(s->Sc.ensure((size_t)Ms * Ms));
         FCK(upload(s->pp, ppos));
         FCK(gather_block_launch(s->Sc, f->Kss, Msp, s->pp, Ms, st, &eu->launches));
         FCK(fsa_permute_launch(0, mu1, s->pp, Ms, f->stage.tmpc, st, &eu->launches));
+        if (out) *out = DevPrediction{f->stage.tmpc, s->Sc, Ms};
     }
     for (int64_t i = 0; i < Ms; ++i) {
         const size_t r = (size_t)ppos[(size_t)i];
@@ -910,7 +911,7 @@ static int fsa_predict(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldx
 extern "C" {
 int gpb200_fitc_predict_fsa(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
                             double* mu, double* var, double* cov) {
-    return fsa_predict(f, Ms, xs, ldxs, block_of, mu, var, cov, nullptr, nullptr);
+    return fsa_predict(f, Ms, xs, ldxs, block_of, mu, var, cov ? CovDest::host : CovDest::none, cov, nullptr, nullptr, nullptr);
 }
 
 int gpb200_fitc_predict_fsa_grad(gpb200_fitc* f, int64_t Ms, const double* xs, int64_t ldxs, const int64_t* block_of,
@@ -923,6 +924,6 @@ int gpb200_fitc_predict_fsa_grad(gpb200_fitc* f, int64_t Ms, const double* xs, i
         return fail(f, GPB200_EINVAL, "fitc_predict_fsa_grad: bad Ms, xs, ldxs, block_of, mu or dmu");
     }
     if (!var != !dvar) return fail(f, GPB200_EINVAL, "fitc_predict_fsa_grad: var and dvar must be given together");
-    return fsa_predict(f, Ms, xs, ldxs, block_of, mu, var, nullptr, dmu, dvar);
+    return fsa_predict(f, Ms, xs, ldxs, block_of, mu, var, CovDest::none, nullptr, dmu, dvar, nullptr);
 }
 }  // extern "C"

@@ -1466,19 +1466,8 @@ int gpb200_grad_inputs(gpb200_handle* h, const double* alpha, double* dmll_x) {
     return GPB200_OK;
 }
 
-int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, const double* alpha,
-                   double* mu, double* var, double* cov) {
-    if (!h) return GPB200_EINVAL;
-    if (!h->factored) return fail(h, GPB200_ESTATE, "predict: factorize first");
-    if (M <= 0 || !xs || ldxs < h->d || !mu) return fail(h, GPB200_EINVAL, "predict: bad M, xs, ldxs or mu");
-    if (!alpha && !h->alpha_ready) return fail(h, GPB200_ESTATE, "predict: no alpha (call mll or pass alpha)");
-    CK(cudaSetDevice(h->device));
-    if (alpha) {
-        int rc = upload_padded(h, h->alpha, alpha);
-        if (rc) return rc;
-        h->alpha_ready = true;
-    }
-    // chunk the test points so that the M_c x Npad workspace stays below ~16 GB
+// test points per chunk, so that the M_c x Npad workspace stays below ~16 GB; a full covariance needs all of V at once
+static int64_t predict_chunk(const gpb200_handle* h, int64_t M, bool want_cov) {
     int64_t cap = (int64_t)(16.0e9 / (8.0 * (double)h->Npad)) / TILE * TILE;
     if (const char* env = getenv("GPB200_PREDICT_CHUNK")) {            // testing hook: force small chunks
         const int64_t v = atoll(env) / TILE * TILE;
@@ -1486,9 +1475,52 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
     }
     if (cap < TILE) cap = TILE;
     if (h->sharded && cap > h->Npad) cap = h->Npad;       // a block of V' travels through the Npad x NBp panel buffer
-    if (cov) cap = (M + TILE - 1) / TILE * TILE;          // full covariance needs all of V at once
-    if (cov && h->sharded && cap > h->Npad) return fail(h, GPB200_EINVAL, "predict: full covariance of more than Npad test points is not supported with sharded storage");
-    const bool need_v = (var != nullptr) || (cov != nullptr);
+    if (want_cov) cap = (M + TILE - 1) / TILE * TILE;
+    return cap;
+}
+
+// K*' of Mc test rows (xs, row stride ldxs) into Kst, on h's stream
+static int predict_cross(gpb200_handle* h, const double* xs, int64_t ldxs, int64_t Mc) {
+    const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
+    CK(cudaMemcpy2DAsync(h->xs, sizeof(double) * h->d, xs, sizeof(double) * ldxs, sizeof(double) * h->d, Mc,
+                         cudaMemcpyHostToDevice, h->st));
+    CK(crossgram_launch(h->prog, h->xs, h->d, Mc, Mpad, h->x, h->d, h->N, h->Npad, h->d, h->Kst, h->Npad, h->st, &h->launches));
+    return GPB200_OK;
+}
+
+// mu = K*' alpha (GP.jl:26) into pmu and mu[0..Mc) on the host
+static int predict_mean(gpb200_handle* h, int64_t Mc, double* mu) {
+    CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));
+    CK(cudaMemcpyAsync(mu, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+    return GPB200_OK;
+}
+
+// V' = K*' L^-T in Kst (whiten!, GP.jl:27); with var, var = k** - |V'|^2 into pvar and var[0..Mc) on the host
+static int predict_var(gpb200_handle* h, int64_t Mc, double* var) {
+    CK(trsm_rec(h, (int)((Mc + TILE - 1) / TILE * TILE), 0, (int)h->Npad));
+    if (!var) return GPB200_OK;
+    CK(kdiag_launch(h->prog, h->xs, h->d, Mc, h->pkdiag, h->st, &h->launches));
+    CK(rowvar_launch(h->Kst, h->Npad, h->pkdiag, Mc, h->Npad, h->pvar, h->st, &h->launches));
+    CK(cudaMemcpyAsync(var, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+    return GPB200_OK;
+}
+
+// gpb200_predict with Sigma* sent to cov_to (CovDest::host: cov, M x M).  *out, if given: pmu holds the last chunk's mu
+// (all of mu* when Sigma* is formed, which takes one chunk) and Kss holds Sigma*.
+static int predict_run(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, const double* alpha, double* mu,
+                       double* var, CovDest cov_to, double* cov, DevPrediction* out) {
+    if (!h->factored) return fail(h, GPB200_ESTATE, "predict: factorize first");
+    if (M <= 0 || !xs || ldxs < h->d || !mu) return fail(h, GPB200_EINVAL, "predict: bad M, xs, ldxs or mu");
+    if (!alpha && !h->alpha_ready) return fail(h, GPB200_ESTATE, "predict: no alpha (call mll or pass alpha)");
+    CK(cudaSetDevice(h->device));
+    if (alpha) {
+        TRY(upload_padded(h, h->alpha, alpha));
+        h->alpha_ready = true;
+    }
+    const bool want_cov = cov_to != CovDest::none;
+    const int64_t cap = predict_chunk(h, M, want_cov);
+    if (want_cov && h->sharded && cap > h->Npad) return fail(h, GPB200_EINVAL, "predict: full covariance of more than Npad test points is not supported with sharded storage");
+    const bool need_v = (var != nullptr) || want_cov;
     Locals Lp;
     if (h->sharded) {
         int rc = shard_entry(h, Lp); if (rc) return rc;
@@ -1500,47 +1532,35 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
         const int64_t Mc = (M - m0 < cap) ? M - m0 : cap;
         const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
         for (auto* q : Lp) {
-            TRY(rank_failed(q, ensure_predict_ws(q, Mc, cov != nullptr)));
-            SCK(q, cudaMemcpy2DAsync(q->xs, sizeof(double) * q->d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * q->d, Mc,
-                                     cudaMemcpyHostToDevice, q->st));
-            SCK(q, crossgram_launch(q->prog, q->xs, q->d, Mc, Mpad, q->x, q->d, q->N, q->Npad, q->d, q->Kst, q->Npad, q->st, &q->launches));
+            TRY(rank_failed(q, ensure_predict_ws(q, Mc, want_cov)));
+            TRY(rank_failed(q, predict_cross(q, xs + m0 * ldxs, ldxs, Mc)));
             if (need_v) {
                 SCK(q, kdiag_launch(q->prog, q->xs, q->d, Mc, q->pvar, q->st, &q->launches));           // running variance starts at k**
-                if (cov) SCK(q, gram_full_launch(q->prog, q->xs, q->d, Mc, Mpad, q->d, q->Kss, Mpad, q->st, &q->launches));
+                if (want_cov) SCK(q, gram_full_launch(q->prog, q->xs, q->d, Mc, Mpad, q->d, q->Kss, Mpad, q->st, &q->launches));
             }
         }
-        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));          // GP.jl:26
-        CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+        TRY(predict_mean(h, Mc, mu + m0));
         if (need_v) {
-            TRY(shard_predict_solve(Lp, (int)Mpad, Mc, var != nullptr, cov != nullptr));
+            TRY(shard_predict_solve(Lp, (int)Mpad, Mc, var != nullptr, want_cov));
             if (var) CK(cudaMemcpyAsync(var + m0, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
-            if (cov && !h->cov_keep_device) CK(cudaMemcpy2DAsync(cov, sizeof(double) * M, h->Kss, sizeof(double) * Mpad, sizeof(double) * M, M,
-                                          cudaMemcpyDeviceToHost, h->st));
+            if (cov_to == CovDest::host) CK(cudaMemcpy2DAsync(cov, sizeof(double) * M, h->Kss, sizeof(double) * Mpad, sizeof(double) * M, M,
+                                                              cudaMemcpyDeviceToHost, h->st));
         }
         TRY(sync_all(Lp));
     }
     for (int64_t m0 = 0; !h->sharded && m0 < M; m0 += cap) {
         const int64_t Mc = (M - m0 < cap) ? M - m0 : cap;
         const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
-        int rc = ensure_predict_ws(h, Mc, cov != nullptr);
-        if (rc) return rc;
-        CK(cudaMemcpy2DAsync(h->xs, sizeof(double) * h->d, xs + m0 * ldxs, sizeof(double) * ldxs,
-                             sizeof(double) * h->d, Mc, cudaMemcpyHostToDevice, h->st));
-        CK(crossgram_launch(h->prog, h->xs, h->d, Mc, Mpad, h->x, h->d, h->N, h->Npad, h->d, h->Kst, h->Npad, h->st, &h->launches));
-        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));          // GP.jl:26
-        CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+        TRY(ensure_predict_ws(h, Mc, want_cov));
+        TRY(predict_cross(h, xs + m0 * ldxs, ldxs, Mc));
+        TRY(predict_mean(h, Mc, mu + m0));
         if (need_v) {
-            CK(trsm_rec(h, (int)Mpad, 0, (int)h->Npad));                                   // whiten!, GP.jl:27
-            if (var) {
-                CK(kdiag_launch(h->prog, h->xs, h->d, Mc, h->pkdiag, h->st, &h->launches));
-                CK(rowvar_launch(h->Kst, h->Npad, h->pkdiag, Mc, h->Npad, h->pvar, h->st, &h->launches));
-                CK(cudaMemcpyAsync(var + m0, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
-            }
-            if (cov) {                                                                      // GP.jl:51-54
+            TRY(predict_var(h, Mc, var ? var + m0 : nullptr));
+            if (want_cov) {                                                                 // GP.jl:51-54
                 CK(gram_full_launch(h->prog, h->xs, h->d, Mc, Mpad, h->d, h->Kss, Mpad, h->st, &h->launches));
                 const GemmBuf bk = gbuf(h, h->Kst, h->mapKst, h->Npad);
                 CK(gemm_whole(h, bk, bk, h->Kss, Mpad, Mpad, Mpad, h->Npad, -1.0, 1.0));
-                if (!h->cov_keep_device)
+                if (cov_to == CovDest::host)
                     CK(cudaMemcpy2DAsync(cov, sizeof(double) * M, h->Kss, sizeof(double) * Mpad, sizeof(double) * M, M,
                                          cudaMemcpyDeviceToHost, h->st));
             }
@@ -1551,10 +1571,17 @@ int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, 
     CK(cudaStreamSynchronize(h->st));
     profile_collect(h);
     h->ms[5] = ev_ms(h->ev2, h->ev3);
+    if (out) *out = DevPrediction{h->pmu, h->Kss, (M + TILE - 1) / TILE * TILE};
     return GPB200_OK;
 }
 
-// Predictive gradients (for ForwardDiff.Dual test inputs of predict_f): mu and var through the same launches as gpb200_predict,
+int gpb200_predict(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, const double* alpha,
+                   double* mu, double* var, double* cov) {
+    if (!h) return GPB200_EINVAL;
+    return predict_run(h, M, xs, ldxs, alpha, mu, var, cov ? CovDest::host : CovDest::none, cov, nullptr);
+}
+
+// Predictive gradients (for ForwardDiff.Dual test inputs of predict_f): mu and var through gpb200_predict's chunk steps,
 // then, with W' = V' L^-1 = K*' K^-1 (rows w_m' = (K^-1 k*_m)'),
 //   dmu[m, :] = sum_i dk(x*_m, x_i)/dx*_m alpha_i,   dvar[m, :] = 2 dk(x*_m, x*_m)/dx*_m - 2 sum_i dk(x*_m, x_i)/dx*_m W'[m, i].
 // F's strict-upper tiles are scratch between calls (inverse merges, GPA's Z'); every call that solves for W' first fills
@@ -1569,39 +1596,24 @@ int gpb200_predict_grad(gpb200_handle* h, int64_t M, const double* xs, int64_t l
     if (!alpha && !h->alpha_ready) return fail(h, GPB200_ESTATE, "predict_grad: no alpha (call mll or pass alpha)");
     CK(cudaSetDevice(h->device));
     if (alpha) {
-        int rc = upload_padded(h, h->alpha, alpha);
-        if (rc) return rc;
+        TRY(upload_padded(h, h->alpha, alpha));
         h->alpha_ready = true;
     }
-    int64_t cap = (int64_t)(16.0e9 / (8.0 * (double)h->Npad)) / TILE * TILE;       // as gpb200_predict
-    if (const char* env = getenv("GPB200_PREDICT_CHUNK")) {
-        const int64_t v = atoll(env) / TILE * TILE;
-        if (v >= TILE && v < cap) cap = v;
-    }
-    if (cap < TILE) cap = TILE;
+    const int64_t cap = predict_chunk(h, M, false);
     const int d = h->d;
     for (int i = 11; i < 16; ++i) h->ms[i] = 0.0;
     for (int64_t m0 = 0; m0 < M; m0 += cap) {
         const int64_t Mc = (M - m0 < cap) ? M - m0 : cap;
         const int64_t Mpad = (Mc + TILE - 1) / TILE * TILE;
-        int rc = ensure_predict_ws(h, Mc, false);
-        if (rc) return rc;
+        TRY(ensure_predict_ws(h, Mc, false));
         CK(h->pdx.ensure(2 * Mpad * d));
         double* ddmu = h->pdx;
         double* ddvar = h->pdx + h->pdx.size() / 2;             // dmu and dvar take one half each
         CK(cudaEventRecord(h->ev0, h->st));
-        CK(cudaMemcpy2DAsync(h->xs, sizeof(double) * d, xs + m0 * ldxs, sizeof(double) * ldxs, sizeof(double) * d, Mc,
-                             cudaMemcpyHostToDevice, h->st));
-        CK(crossgram_launch(h->prog, h->xs, d, Mc, Mpad, h->x, d, h->N, h->Npad, d, h->Kst, h->Npad, h->st, &h->launches));
-        CK(rowdot_launch(h->Kst, h->Npad, h->alpha, Mc, h->Npad, h->pmu, h->st, &h->launches));
-        CK(cudaMemcpyAsync(mu + m0, h->pmu, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
+        TRY(predict_cross(h, xs + m0 * ldxs, ldxs, Mc));
+        TRY(predict_mean(h, Mc, mu + m0));
         CK(cudaEventRecord(h->ev1, h->st));
-        if (var) {
-            CK(trsm_rec(h, (int)Mpad, 0, (int)h->Npad));                                   // V' = K*' L^-T
-            CK(kdiag_launch(h->prog, h->xs, d, Mc, h->pkdiag, h->st, &h->launches));
-            CK(rowvar_launch(h->Kst, h->Npad, h->pkdiag, Mc, h->Npad, h->pvar, h->st, &h->launches));
-            CK(cudaMemcpyAsync(var + m0, h->pvar, sizeof(double) * Mc, cudaMemcpyDeviceToHost, h->st));
-        }
+        if (var) TRY(predict_var(h, Mc, var + m0));                                        // V' = K*' L^-T
         CK(cudaEventRecord(h->ev2, h->st));
         if (var && m0 == 0) CK(mirror_lower_tiles_launch(h->F, h->ld, h->Npad, h->st, &h->launches));   // L' into F's upper tiles
         CK(cudaEventRecord(h->ev5, h->st));
@@ -1634,13 +1646,9 @@ int gpb200_rand(gpb200_handle* h, int64_t M, const double* xs, int64_t ldxs, con
     if (!h) return GPB200_EINVAL;
     if (M <= 0 || nsamp <= 0 || !z || !samples || !mu_minus_mean) return fail(h, GPB200_EINVAL, "rand: bad M, nsamp, z, mu or samples");
     if (!(nugget >= 0.0)) return fail(h, GPB200_EINVAL, "rand: nugget must be >= 0");
-    CK(cudaSetDevice(h->device));
-    static double cov_flag;                                     // non-null marker: the covariance stays in h->Kss
-    h->cov_keep_device = true;
-    int rc = gpb200_predict(h, M, xs, ldxs, alpha, mu_minus_mean, nullptr, &cov_flag);
-    h->cov_keep_device = false;
-    if (rc) return rc;
-    return rand_from_cov(h, M, h->Kss, (M + TILE - 1) / TILE * TILE, h->pmu, nsamp, z, nugget, samples);
+    DevPrediction p;
+    TRY(predict_run(h, M, xs, ldxs, alpha, mu_minus_mean, nullptr, CovDest::device, nullptr, &p));
+    return rand_from_cov(h, M, p.cov, p.ldc, p.mu, nsamp, z, nugget, samples);
 }
 
 // ---- ElasticGPE append! (src/GPEelastic.jl:13-22): extend the factor by k new observations -----------------------------
