@@ -330,52 +330,6 @@ cudaError_t inverse_from_factor(gpb200_handle* h) {
 //   W'W + trace     : tile rows dealt round-robin; only the P+1 partial sums are all-reduced, K^-1
 //                     itself is never exchanged.
 // ================================================================================================
-}  // namespace engine
-namespace {
-// rank q owns the 128-wide tile columns t with t % nranks == q of every W21 block; its "slice" is
-// the concatenation of those tile columns (local column jl <-> global column ((jl/128)*nranks+q)*128 + jl%128)
-__global__ void pack_slices_kernel(const double* __restrict__ G, long long ld, double* __restrict__ out,
-                                   int s, int wr, int nranks, int self, int Np) {
-    const int z = blockIdx.z;
-    const int p = z * 2 * s;
-    const int n2 = min(s, Np - p - s);
-    const int i = blockIdx.y * 32 + threadIdx.y, jl = blockIdx.x * 32 + threadIdx.x;
-    if (n2 <= 0 || i >= n2 || jl >= wr) return;
-    const int gj = ((jl >> 7) * nranks + self) * 128 + (jl & 127);
-    out[(long long)z * s * wr + (long long)i * wr + jl] = G[(long long)(p + s + i) * ld + p + gj];
-}
-// scatter the gathered W21 slices of all other ranks into G (lower block) and, transposed, into
-// G's strict-upper block
-__global__ void unpack_slices_kernel(double* __restrict__ G, long long ld, const double* __restrict__ in,
-                                     long long per_rank, int s, int wr, int Np, int nranks, int self) {
-    __shared__ double tile[32][33];
-    const int batch = (Np + 2 * s - 1) / (2 * s);
-    const int z = blockIdx.z % batch;
-    const int q = blockIdx.z / batch;
-    if (q == self) return;
-    const int p = z * 2 * s;
-    const int n2 = min(s, Np - p - s);
-    if (n2 <= 0) return;
-    const double* src = in + (long long)q * per_rank + (long long)z * s * wr;
-    const int i0 = blockIdx.y * 32, j0 = blockIdx.x * 32;            // 32 | 128: a block never straddles tiles
-    if (i0 >= n2 || j0 >= wr) return;
-    const int i = i0 + threadIdx.y, jl = j0 + threadIdx.x;
-    double v = 0.0;
-    if (i < n2 && jl < wr) {
-        v = src[(long long)i * wr + jl];
-        const int gj = ((jl >> 7) * nranks + q) * 128 + (jl & 127);
-        G[(long long)(p + s + i) * ld + p + gj] = v;
-    }
-    tile[threadIdx.y][threadIdx.x] = v;
-    __syncthreads();
-    const int ti = i0 + threadIdx.x, tjl = j0 + threadIdx.y;
-    if (ti < n2 && tjl < wr) {
-        const int gj = ((tjl >> 7) * nranks + q) * 128 + (tjl & 127);
-        G[(long long)(p + gj) * ld + p + s + ti] = tile[threadIdx.x][threadIdx.y];
-    }
-}
-}  // namespace
-namespace engine __attribute__((visibility("hidden"))) {
 
 int dist_block(gpb200_handle* h) {
     int NB = TILE;
@@ -479,30 +433,6 @@ int cholesky_dist(gpb200_handle* h) {
     return GPB200_OK;
 }
 
-
-}  // namespace engine
-namespace {
-// ---- device-side signalling for the fused (peer-memory) panel broadcast --------------------------
-__global__ void signal_peers_kernel(int* const* peer_sig_words, int n_peer, int value) {
-    // all panel stores of the preceding kernels are complete (stream order); make them visible
-    // system-wide before the flag
-    __threadfence_system();
-    if ((int)threadIdx.x < n_peer)
-        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(peer_sig_words[threadIdx.x]), "r"(value) : "memory");
-}
-__global__ void wait_signal_kernel(const int* word, int target, int* err) {
-    long long spins = 0;
-    int v;
-    do {
-        asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(word) : "memory");
-        if (v >= target) break;
-        if (++spins > (1LL << 27)) { atomicExch(err, 1); break; }
-        __nanosleep(100);
-    } while (true);
-}
-}  // namespace
-namespace engine __attribute__((visibility("hidden"))) {
-
 // Cholesky over block columns with the panel broadcast FUSED into the kernels that produce the panel:
 // the tile leaf and the 128-wide TRSM GEMM store their outputs into every peer's F / Dinv / DinvT / logd
 // through NVLink-mapped pointers (CUDA IPC), then one tiny kernel raises a flag word in each peer; the
@@ -532,17 +462,13 @@ int cholesky_dist_p2p(gpb200_handle* h) {
         cudaError_t e = chol_panel(h, bp(b), bn(b), NB);
         h->push_panel = false;
         CK(e);
-        signal_peers_kernel<<<1, 32, 0, h->st>>>(h->peer_sig_dev, h->n_peer, base + b + 1);
-        ++h->launches;
-        CK(cudaGetLastError());
+        CK(shard_signal_peers(h->peer_sig_dev, h->n_peer, base + b + 1, h->st, &h->launches));
         return GPB200_OK;
     };
     if (owner(0) == me) { int rc = factor_and_publish(0); if (rc) return rc; }
     for (int b = 0; b < nblk; ++b) {
         if (owner(b) != me) {
-            wait_signal_kernel<<<1, 1, 0, h->st>>>(h->sig + owner(b), base + b + 1, h->sig + 8);
-            ++h->launches;
-            CK(cudaGetLastError());
+            CK(shard_wait_signal(h->sig + owner(b), base + b + 1, h->sig + 8, h->st, &h->launches));
         }
         bool did_next = false;
         if (b + 1 < nblk && owner(b + 1) == me) {
@@ -605,19 +531,13 @@ int inverse_dist(gpb200_handle* h) {
         const long long per_rank = rows_total * wr;
         if ((size_t)per_rank > h->ag_send.size() || (size_t)per_rank * R > h->ag_recv.size())
             return fail(h, GPB200_ECUDA, "inverse_dist: exchange buffers too small");
-        dim3 blk(32, 32), grd((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)batch);
-        pack_slices_kernel<<<grd, blk, 0, h->st>>>(h->G, h->ld, h->ag_send, (int)s, wr, R, me, Np);
-        ++h->launches;
-        CK(cudaGetLastError());
+        CK(shard_pack_slices(h->G, h->ld, h->ag_send, (int)s, R, me, Np, h->st, &h->launches));
         CK(cudaEventRecord(h->ev_x, h->st));
         CK(cudaStreamWaitEvent(h->st_comm, h->ev_x, 0));
         CKN(g_nccl.AllGather(h->ag_send, h->ag_recv, (size_t)per_rank, ncclDouble, h->comm, h->st_comm));
         CK(cudaEventRecord(h->ev_y, h->st_comm));
         CK(cudaStreamWaitEvent(h->st, h->ev_y, 0));
-        dim3 grd2((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)(batch * R));
-        unpack_slices_kernel<<<grd2, blk, 0, h->st>>>(h->G, h->ld, h->ag_recv, per_rank, (int)s, wr, Np, R, me);
-        ++h->launches;
-        CK(cudaGetLastError());
+        CK(shard_unpack_slices(h->G, h->ld, h->ag_recv, per_rank, (int)s, R, me, Np, h->st, &h->launches));
     }
     // W'W on this rank's tile rows only (K^-1 stays distributed; the trace needs no more)
     GemmDesc g = gemm_desc_default();

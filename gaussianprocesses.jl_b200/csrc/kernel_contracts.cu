@@ -9,6 +9,7 @@
 #include "gram.cuh"
 #include "gram_fast.cuh"
 #include "potrf_base.cuh"
+#include "shard_kernels.cuh"
 #include "vec.cuh"
 
 using namespace engine;
@@ -624,6 +625,106 @@ int gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int
                                     (int)a[12], st, L); break;
     case 15: e = rows_dx_launch(P, ptr(0), a[1], a[2], ptr(3), a[4], a[5], (int)a[6], ptr(7), a[8], ptr(9), ptr(10),
                                 reinterpret_cast<const long long*>(a[11]), ptr(12), (int)a[13], st, L); break;
+    }
+    CK(e);
+    CK(cudaStreamSynchronize(st));
+    return GPB200_OK;
+}
+
+int gpb200_shard_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n) {
+    if (!h || !args || which < 0 || which > 14) return GPB200_EINVAL;
+    static const int want[15] = {5, 12, 10, 6, 7, 5, 3, 9, 10, 7, 8, 7, 8, 3, 3};
+    if (n != want[which]) return fail(h, GPB200_EINVAL, "shard_kernels: wrong argument count for this kernel");
+    const int64_t* a = args;
+    auto ptr = [&](int i) { return reinterpret_cast<double*>(a[i]); };
+    auto need = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (!a[i]) return false;
+        return true;
+    };
+    auto in_int = [&](std::initializer_list<int> idx) {           // sizes the wrappers take as int: in [0, INT_MAX]
+        for (int i : idx) if (a[i] < 0 || a[i] > INT_MAX) return false;
+        return true;
+    };
+    const int64_t YMAX = 65535;                                    // grid.y / grid.z limit
+    // the ownership {R, me, rb} at a[i], a[i + 1], a[i + 2]
+    auto own_ok = [&](int i) { return a[i] >= 1 && a[i] <= INT_MAX && a[i + 1] >= 0 && a[i + 1] < a[i] && a[i + 2] >= 1 && a[i + 2] <= INT_MAX; };
+    auto own_at = [&](int i) { return ShardOwn{(int)a[i], (int)a[i + 1], (int)a[i + 2]}; };
+    // rows r >= 128 t1 of Npad: Npad a multiple of 128, t1 in [0, Npad / 128], at most 65 535 tiles past t1
+    auto panel_ok = [&](int npad, int t1) {
+        return a[npad] >= 0 && a[npad] % TILE == 0 && a[npad] / TILE <= INT_MAX && a[t1] >= 0 && a[t1] <= a[npad] / TILE &&
+               a[npad] / TILE - a[t1] <= YMAX;
+    };
+    // a level s that inverse_dist splits over R ranks: s a positive multiple of 128 R below Np, grid.y and grid.z in range
+    auto level_ok = [&](int s, int np, int r, int me, int ld) {
+        if (a[r] < 1 || a[r] > INT_MAX || a[me] < 0 || a[me] >= a[r] || a[np] <= 0 || a[np] % TILE || a[np] > INT_MAX) return false;
+        if (a[s] <= 0 || a[s] % (TILE * a[r]) || a[s] >= a[np] || (a[s] + 31) / 32 > YMAX || a[ld] < a[np]) return false;
+        return (a[np] + 2 * a[s] - 1) / (2 * a[s]) * (which == 12 ? a[r] : 1) <= YMAX;
+    };
+    bool ok = true;
+    switch (which) {
+    case 0: ok = need({0, 2}) && in_int({4}) && a[4] <= YMAX && a[1] >= a[4] && a[3] >= a[4]; break;      // dst, ldd, src, lds, n
+    case 1:     // G, F, ld, Npad, c0, nb, t1, S_me, nbp, R, me, rb
+        ok = need({0, 1, 7}) && in_int({4, 5, 8}) && panel_ok(3, 6) && a[5] <= a[8] && a[2] >= a[4] + a[5] && own_ok(9);
+        break;
+    case 2:     // P, nbp, Npad, nb, t1, S, per_rank, R, me, rb; every rank's region holds its rows >= 128 t1
+        ok = need({0, 5}) && in_int({1, 3}) && panel_ok(2, 4) && a[3] <= a[1] && own_ok(7) && a[6] >= 0;
+        if (ok) {
+            const ShardOwn o = own_at(7);
+            for (int q = 0; q < o.R && ok; ++q)
+                ok = a[6] >= (shard_own_before(a[2] / TILE, q, o.rb, o.R) - shard_own_before(a[4], q, o.rb, o.R)) * TILE * a[1];
+        }
+        break;
+    case 3:     // dst, ldd, src, lds, rows, cols
+    case 7:     // dst, ldd, src, lds, rows, cols, R, me, rb
+        ok = need({0, 2}) && a[4] >= 0 && a[5] >= 0 && a[4] <= 32 * YMAX && a[1] >= a[4] && a[3] >= a[5] && (which == 3 || own_ok(6));
+        break;
+    case 4:     // P, nbp, G, ld, Dinv, j0, nb: j0, nb multiples of 128 (the panels of shard_inverse_la)
+        ok = need({0, 2, 4}) && in_int({1, 5, 6}) && a[5] % TILE == 0 && a[6] % TILE == 0 && a[6] <= a[1] && a[6] <= YMAX &&
+             a[3] >= a[5] + a[6];
+        break;
+    case 5: ok = need({0, 1}) && a[3] >= 1 && a[3] <= INT_MAX && a[4] >= 0 && a[2] >= a[4]; break;     // out, in, stride, nranks, n
+    case 6: ok = need({0, 1}) && a[2] >= 1 && a[2] <= INT_MAX; break;                                  // out, in, nranks
+    case 8:     // Y, G, ld, ncols, alpha, N, out, R, me, rb
+        ok = need({0, 1, 4, 6}) && a[3] >= 0 && a[5] >= 0 && a[2] >= a[3] && own_ok(7);
+        break;
+    case 9:     // G, ld, N, out, R, me, rb: the diagonal of every row of the tiles covering 0 .. N
+        ok = need({0, 3}) && a[2] >= 0 && a[1] >= (a[2] + TILE - 1) / TILE * TILE && own_ok(4);
+        break;
+    case 10: ok = need({0, 1, 3}) && a[2] >= 1 && a[4] >= 0 && a[4] <= YMAX && own_ok(5); break;       // out, src, ld, idx, nv, R, me, rb
+    case 11: ok = need({0, 2}) && level_ok(3, 4, 5, 6, 1); break;                                      // G, ld, out, s, Np, R, me
+    case 12:    // G, ld, in, per_rank, s, Np, R, me: per_rank = sum_z n2_z * wr, as inverse_dist computes it
+        ok = need({0, 2}) && level_ok(4, 5, 6, 7, 1);
+        if (ok) {
+            int64_t rows = 0;
+            for (int64_t p = 0; p < a[5]; p += 2 * a[4]) rows += std::max<int64_t>(0, std::min(a[4], a[5] - p - a[4]));
+            ok = a[3] >= rows * (a[4] / a[6]);
+        }
+        break;
+    case 13: ok = need({0}) && a[1] >= 0 && a[1] <= 7 && a[2] >= INT_MIN && a[2] <= INT_MAX; break;   // words, n_peer, value
+    case 14: ok = need({0, 2}) && a[1] >= INT_MIN && a[1] <= INT_MAX; break;                           // word, target, err
+    }
+    if (!ok) return fail(h, GPB200_EINVAL, "shard_kernels: a null pointer, a negative size, a bad ownership, padding or level, a leading "
+                                           "dimension below the row width, a region too small or a grid dimension past 65 535");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = h->st;
+    int64_t* L = &h->launches;
+    cudaError_t e = cudaSuccess;
+    switch (which) {
+    case 0: e = shard_copy_lower(ptr(0), a[1], ptr(2), a[3], (int)a[4], st, L); break;
+    case 1: e = shard_scatter_rows(ptr(0), ptr(1), a[2], a[3], (int)a[4], (int)a[5], (int)a[6], ptr(7), (int)a[8], own_at(9), st, L); break;
+    case 2: e = shard_unpack_panel(ptr(0), (int)a[1], a[2], (int)a[3], (int)a[4], ptr(5), a[6], own_at(7), st, L); break;
+    case 3: e = shard_transpose(ptr(0), a[1], ptr(2), a[3], a[4], a[5], st, L); break;
+    case 4: e = shard_pack_wblock(ptr(0), (int)a[1], ptr(2), a[3], ptr(4), (int)a[5], (int)a[6], st, L); break;
+    case 5: e = shard_sum_ranks(ptr(0), ptr(1), a[2], (int)a[3], a[4], st, L); break;
+    case 6: e = shard_min_ranks(reinterpret_cast<int*>(a[0]), reinterpret_cast<const int*>(a[1]), (int)a[2], st, L); break;
+    case 7: e = shard_transpose_own(ptr(0), a[1], ptr(2), a[3], a[4], a[5], own_at(6), st, L); break;
+    case 8: e = shard_rowdot_own(ptr(0), ptr(1), a[2], a[3], ptr(4), a[5], own_at(7), ptr(6), st, L); break;
+    case 9: e = shard_diag_own(ptr(0), a[1], a[2], own_at(4), ptr(3), st, L); break;
+    case 10: e = shard_gather_block_own(ptr(0), ptr(1), a[2], reinterpret_cast<const long long*>(a[3]), a[4], own_at(5), st, L); break;
+    case 11: e = shard_pack_slices(ptr(0), a[1], ptr(2), (int)a[3], (int)a[5], (int)a[6], (int)a[4], st, L); break;
+    case 12: e = shard_unpack_slices(ptr(0), a[1], ptr(2), a[3], (int)a[4], (int)a[6], (int)a[7], (int)a[5], st, L); break;
+    case 13: e = shard_signal_peers(reinterpret_cast<int* const*>(a[0]), (int)a[1], (int)a[2], st, L); break;
+    case 14: e = shard_wait_signal(reinterpret_cast<const int*>(a[0]), (int)a[1], reinterpret_cast<int*>(a[2]), st, L); break;
     }
     CK(e);
     CK(cudaStreamSynchronize(st));

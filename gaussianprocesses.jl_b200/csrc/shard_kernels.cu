@@ -64,7 +64,7 @@ __global__ void pack_wblock_kernel(double* __restrict__ P, int nbp, const double
     if (i >= nb) return;
     double v = 0.0;
     if ((c >> 7) > (i >> 7)) v = G[(long long)(j0 + c) * ld + j0 + i];        // strictly-lower tile of W_JJ
-    else if ((c >> 7) == (i >> 7)) v = Dinv[(long long)(j0 + c) * T + (i & 127)];   // clean lower diagonal tile (zeros above)
+    else if ((c >> 7) == (i >> 7) && c >= i) v = Dinv[(long long)(j0 + c) * T + (i & 127)];   // lower half of the diagonal tile
     P[(long long)(j0 + c) * nbp + i] = v;
 }
 
@@ -141,6 +141,68 @@ __global__ void gather_block_own_kernel(double* __restrict__ out, const double* 
     const long long r = max(idx[a], idx[b]), c = min(idx[a], idx[b]);
     out[a * nv + b] = ((int)((r / T / own.rb) % own.R) == own.me) ? src[r * ld + c] : 0.0;
 }
+
+// ---- replicated storage (inverse_dist): rank q owns the 128-wide tile columns t with t % nranks == q of every W21 block; its
+// "slice" is the concatenation of those tile columns (local column jl <-> global column ((jl/128)*nranks+q)*128 + jl%128)
+__global__ void pack_slices_kernel(const double* __restrict__ G, long long ld, double* __restrict__ out,
+                                   int s, int wr, int nranks, int self, int Np) {
+    const int z = blockIdx.z;
+    const int p = z * 2 * s;
+    const int n2 = min(s, Np - p - s);
+    const int i = blockIdx.y * 32 + threadIdx.y, jl = blockIdx.x * 32 + threadIdx.x;
+    if (n2 <= 0 || i >= n2 || jl >= wr) return;
+    const int gj = ((jl >> 7) * nranks + self) * 128 + (jl & 127);
+    out[(long long)z * s * wr + (long long)i * wr + jl] = G[(long long)(p + s + i) * ld + p + gj];
+}
+// scatter the gathered W21 slices of all other ranks into G (lower block) and, transposed, into
+// G's strict-upper block
+__global__ void unpack_slices_kernel(double* __restrict__ G, long long ld, const double* __restrict__ in,
+                                     long long per_rank, int s, int wr, int Np, int nranks, int self) {
+    __shared__ double tile[32][33];
+    const int batch = (Np + 2 * s - 1) / (2 * s);
+    const int z = blockIdx.z % batch;
+    const int q = blockIdx.z / batch;
+    if (q == self) return;
+    const int p = z * 2 * s;
+    const int n2 = min(s, Np - p - s);
+    if (n2 <= 0) return;
+    const double* src = in + (long long)q * per_rank + (long long)z * s * wr;
+    const int i0 = blockIdx.y * 32, j0 = blockIdx.x * 32;            // 32 | 128: a block never straddles tiles
+    if (i0 >= n2 || j0 >= wr) return;
+    const int i = i0 + threadIdx.y, jl = j0 + threadIdx.x;
+    double v = 0.0;
+    if (i < n2 && jl < wr) {
+        v = src[(long long)i * wr + jl];
+        const int gj = ((jl >> 7) * nranks + q) * 128 + (jl & 127);
+        G[(long long)(p + s + i) * ld + p + gj] = v;
+    }
+    tile[threadIdx.y][threadIdx.x] = v;
+    __syncthreads();
+    const int ti = i0 + threadIdx.x, tjl = j0 + threadIdx.y;
+    if (ti < n2 && tjl < wr) {
+        const int gj = ((tjl >> 7) * nranks + q) * 128 + (tjl & 127);
+        G[(long long)(p + gj) * ld + p + s + ti] = tile[threadIdx.x][threadIdx.y];
+    }
+}
+
+// ---- device-side signalling for the fused (peer-memory) panel broadcast of cholesky_dist_p2p ----------------------
+__global__ void signal_peers_kernel(int* const* peer_sig_words, int n_peer, int value) {
+    // all panel stores of the preceding kernels are complete (stream order); make them visible
+    // system-wide before the flag
+    __threadfence_system();
+    if ((int)threadIdx.x < n_peer)
+        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(peer_sig_words[threadIdx.x]), "r"(value) : "memory");
+}
+__global__ void wait_signal_kernel(const int* word, int target, int* err) {
+    long long spins = 0;
+    int v;
+    do {
+        asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(word) : "memory");
+        if (v >= target) break;
+        if (++spins > (1LL << 27)) { atomicExch(err, 1); break; }
+        __nanosleep(100);
+    } while (true);
+}
 }  // namespace
 
 cudaError_t shard_copy_lower(double* dst, int64_t ldd, const double* src, int64_t lds, int n, cudaStream_t st, int64_t* launches) {
@@ -174,7 +236,7 @@ cudaError_t shard_unpack_panel(double* P, int nbp, int64_t Npad, int nb, int t1,
 
 cudaError_t shard_transpose(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows, int64_t cols, cudaStream_t st, int64_t* launches) {
     if (rows <= 0 || cols <= 0) return cudaSuccess;
-    // grid.y is limited to 65535 blocks of 32 rows = 2M rows: enough for N <= 2^21
+    // grid.y is limited to 65535 blocks of 32 rows: rows <= 65535 * 32 = 2 097 120 (32 short of 2^21)
     dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32)), block(32, 8);
     transpose_kernel<<<grid, block, 0, st>>>(dst, ldd, src, lds, rows, cols);
     if (launches) ++*launches;
@@ -236,6 +298,36 @@ cudaError_t shard_gather_block_own(double* out, const double* src, int64_t ld, c
     if (nv <= 0) return cudaSuccess;
     dim3 grid((unsigned)((nv + 255) / 256), (unsigned)nv);
     gather_block_own_kernel<<<grid, 256, 0, st>>>(out, src, ld, idx, nv, own);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_pack_slices(const double* G, int64_t ld, double* out, int s, int nranks, int self, int Np, cudaStream_t st,
+                              int64_t* launches) {
+    const int wr = s / nranks, batch = (Np + 2 * s - 1) / (2 * s);
+    dim3 blk(32, 32), grd((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)batch);
+    pack_slices_kernel<<<grd, blk, 0, st>>>(G, ld, out, s, wr, nranks, self, Np);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_unpack_slices(double* G, int64_t ld, const double* in, int64_t per_rank, int s, int nranks, int self, int Np,
+                                cudaStream_t st, int64_t* launches) {
+    const int wr = s / nranks, batch = (Np + 2 * s - 1) / (2 * s);
+    dim3 blk(32, 32), grd((wr + 31) / 32, (unsigned)((s + 31) / 32), (unsigned)(batch * nranks));
+    unpack_slices_kernel<<<grd, blk, 0, st>>>(G, ld, in, per_rank, s, wr, Np, nranks, self);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_signal_peers(int* const* peer_sig_words, int n_peer, int value, cudaStream_t st, int64_t* launches) {
+    signal_peers_kernel<<<1, 32, 0, st>>>(peer_sig_words, n_peer, value);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t shard_wait_signal(const int* word, int target, int* err, cudaStream_t st, int64_t* launches) {
+    wait_signal_kernel<<<1, 1, 0, st>>>(word, target, err);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

@@ -52,3 +52,20 @@ cudaError_t shard_diag_own(const double* G, int64_t ld, int64_t N, ShardOwn own,
 // exactly symmetric principal sub-block of a matrix whose lower triangle is stored
 cudaError_t shard_gather_block_own(double* out, const double* src, int64_t ld, const long long* idx, int64_t nv, ShardOwn own,
                                    cudaStream_t st, int64_t* launches);
+
+// ---- replicated storage (gpb200.cu).  inverse_dist splits a level s of the triangular inverse when (s / 128) % nranks == 0:
+// rank q computes the 128-wide tile columns t % nranks == q of every W21 block, its "slice" (wr = s / nranks columns; local
+// column jl <-> block column ((jl / 128) * nranks + q) * 128 + jl % 128).  Problem z of the level starts at p = 2 s z and has
+// n2_z = min(s, Np - p - s) rows (<= 0: none).
+// out[z s wr + i wr + jl] = G[(p + s + i) ld + p + gj(jl, self)], i < n2_z  (this rank's slice of every W21 block)
+cudaError_t shard_pack_slices(const double* G, int64_t ld, double* out, int s, int nranks, int self, int Np, cudaStream_t st,
+                              int64_t* launches);
+// for every rank q != self: its slice from in + q per_rank (laid out as pack_slices writes it) into W21 (rows p + s + i,
+// columns p + gj(jl, q)) and, transposed, into G's strict-upper block (rows p + gj, columns p + s + i).  The rank's own slice
+// is left alone: its lower half was written by the GEMM, its transpose by the GEMM's Ct epilogue.
+cudaError_t shard_unpack_slices(double* G, int64_t ld, const double* in, int64_t per_rank, int s, int nranks, int self, int Np,
+                                cudaStream_t st, int64_t* launches);
+// cholesky_dist_p2p: after a system-wide fence, *peer_sig_words[q] = value (release, system scope) for q < n_peer (<= 32)
+cudaError_t shard_signal_peers(int* const* peer_sig_words, int n_peer, int value, cudaStream_t st, int64_t* launches);
+// one thread spins (acquire, system scope) until *word >= target; after about 2^27 polls it sets *err = 1 and returns
+cudaError_t shard_wait_signal(const int* word, int target, int* err, cudaStream_t st, int64_t* launches);

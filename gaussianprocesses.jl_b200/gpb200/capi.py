@@ -69,6 +69,7 @@ _SIGNATURES = {
     "gpb200_gram_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_vec_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
     "gpb200_fitc_cv_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32, _dp, C.c_int32]),
+    "gpb200_shard_kernels": (C.c_int, [_H, C.c_int, _lp, C.c_int32]),
     "gpb200_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "gpb200_ipc_export": (C.c_int, [_H, C.c_void_p]),
     "gpb200_ipc_import": (C.c_int, [_H, C.c_int, C.c_void_p]),
@@ -512,6 +513,16 @@ class Engine:
         f = np.ascontiguousarray(fargs, dtype=np.float64).ravel()
         self._check(self._lib.gpb200_fitc_cv_kernels(self._h, self.FITC_CV_KERNELS.index(name), a.ctypes.data_as(_lp),
                                                      a.size, _as_dp(f), f.size), "fitc_cv_kernels")
+
+    SHARD_KERNELS = ("copy_lower", "scatter_rows", "unpack_panel", "transpose", "pack_wblock", "sum_ranks", "min_ranks",
+                     "transpose_own", "rowdot_own", "diag_own", "gather_block_own", "pack_slices", "unpack_slices",
+                     "signal_peers", "wait_signal")
+
+    def shard_kernels(self, name, args):
+        """One data-movement kernel of the multi-rank schedules (include/gpb200.h) by name, on device buffers."""
+        a = np.ascontiguousarray(args, dtype=np.int64).ravel()
+        self._check(self._lib.gpb200_shard_kernels(self._h, self.SHARD_KERNELS.index(name), a.ctypes.data_as(_lp), a.size),
+                    "shard_kernels")
 
 
 class FitcEngine:

@@ -399,6 +399,30 @@ int  gpb200_vec_kernels(gpb200_handle* h, int which, const int64_t* args, int32_
  *                         point-major (rows_dx_launch, csrc/gram.cuh)
  * GPB200_EINVAL, nothing launched: as gpb200_fsa_kernels, plus j outside [0, n_theta) and ldx < d.                   */
 int  gpb200_fitc_cv_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n, const double* fargs, int32_t nf);
+/* The data-movement kernels of the multi-rank schedules (csrc/shard_kernels.cuh) on caller buffers, synchronous, one
+ * launch each through its wrapper (nothing to do: no launch, as the wrappers do).  An ownership (R, me, rb) is the
+ * block-cyclic layout of 128-row tiles, tile t owned by rank (t / rb) % R; one device can act as any rank of any layout.
+ *   which 0  copy_lower      : dst, ldd, src, lds, n                                     (n <= 65 535)
+ *   which 1  scatter_rows    : G, F, ld, Npad, c0, nb, t1, S_me, nbp, R, me, rb
+ *   which 2  unpack_panel    : P, nbp, Npad, nb, t1, S, per_rank, R, me, rb             (per_rank holds every rank's rows)
+ *   which 3  transpose       : dst, ldd, src, lds, rows, cols                            (rows <= 65 535 * 32)
+ *   which 4  pack_wblock     : P, nbp, G, ld, Dinv, j0, nb                               (j0, nb multiples of 128)
+ *   which 5  sum_ranks       : out, in, stride, nranks, n
+ *   which 6  min_ranks       : out, in, nranks                                           (int32 words)
+ *   which 7  transpose_own   : dst, ldd, src, lds, rows, cols, R, me, rb
+ *   which 8  rowdot_own      : Y, G, ld, ncols, alpha, N, out, R, me, rb
+ *   which 9  diag_own        : G, ld, N, out, R, me, rb
+ *   which 10 gather_block_own: out, src, ld, idx, nv, R, me, rb                          (idx int64, nv <= 65 535)
+ *   which 11 pack_slices     : G, ld, out, s, Np, R, me                                  (inverse_dist's slice exchange)
+ *   which 12 unpack_slices   : G, ld, in, per_rank, s, Np, R, me
+ *   which 13 signal_peers    : words (device array of int32 pointers), n_peer, value     (n_peer <= 7)
+ *   which 14 wait_signal     : word, target, err                                         (spins until *word >= target)
+ * The slice kernels take a level inverse_dist splits: s a multiple of 128 R below Np, Np a multiple of 128, ld >= Np, and
+ * for unpack_slices per_rank >= sum_z n2_z s / R.
+ * GPB200_EINVAL, nothing launched: bad which / n, a null pointer, a negative size, R < 1, me outside [0, R), rb < 1, Npad
+ * not a multiple of 128, t1 past the last tile, nb > nbp, a leading dimension below the row width, a region too small
+ * or a grid dimension past 65 535.                                                                                  */
+int  gpb200_shard_kernels(gpb200_handle* h, int which, const int64_t* args, int32_t n);
 
 /* ---- multi-GPU (one process per GPU; NCCL over NVLink) -------------------------------------- */
 /* rank 0 obtains a 128-byte NCCL unique id, the host side broadcasts it (torch.distributed /
